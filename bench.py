@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the nnaudio-b200 hot path (contract: task brief §④ / base contract).
+"""Benchmark of the nnaudio-b200 hot path.
 
-  python bench.py --gpus N --steps K --warmup W [--workload cfg2] [--impl reference]
+  python bench.py --gpus N --steps K --warmup W [--workload cfg2] [--impl reference] [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of synthetic white noise:
 by default ``cfg2`` of BASELINE.json (MelSpectrogram n_fft=2048 hop=512
@@ -12,9 +12,16 @@ HOST buffers (H2D of the input and D2H of the spectrogram inside the timed
 region).  Under torchrun (N > 1) every rank processes its own batch shard
 (weak scaling) and the shards' outputs are all-gathered over NCCL/NVLink.
 
-``--impl reference`` times the CPU arm instead: the NumPy oracle port of the
-reference's conv1d path (oracle/nnaudio_oracle.py) on the host cores — the
-reference itself is Python and cannot travel to the GPU box.
+``--impl reference`` times the CPU arm instead: the unmodified reference when
+oracle/install_ref.sh has installed it into oracle/_ref, else the NumPy oracle
+port of the reference's conv1d path (oracle/nnaudio_oracle.py), on the host cores.
+
+``--steps`` sets the timed steps of the headline workload, of its ``e2e`` leg and of
+its no-gather leg; the secondary workloads in ``workloads`` are timed over
+``--workload-steps``.  ``--dump-outputs DIR`` writes what the headline workload's
+timed path returned in its last timed step as DIR/<workload>.npy (float32; the
+first clips of the batch when the whole output exceeds 64 MB).  The inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -73,8 +80,7 @@ GATHER_DESC = {"peer": "kernels write into symmetric memory, copy-engine pushes 
                "nccl": "ncclAllGather on reserved SMs", "none": "-", "auto": "-"}
 
 # SMs left to the NCCL gather while the persistent kernels run, and the matching NCCL CTA cap
-# (the gather of (N-1) x 14 MB must hide under one ~0.47 ms transform; measured ~14.5 GB/s per
-# NCCL CTA next to the kernels: 8 CTAs suffice at N=4, not at N=8 — profiles/README.md)
+# (the gather of (N-1) shards must hide under one transform; more ranks, more bytes to move)
 DEFAULT_RESERVE = {1: 0, 2: 8, 4: 8, 8: 16}
 
 
@@ -99,7 +105,7 @@ def framed_algorithmic_flops(mod, cls, B, T):
 
 
 # ----------------------------------------------------------------------------
-# clocks sampling (nvidia-smi recipe of B200_PROFILING.md, through NVML)
+# clocks sampling (through NVML)
 # ----------------------------------------------------------------------------
 class ClockSampler:
     BAD = {"hw_slowdown": 0x8, "hw_thermal_slowdown": 0x40, "sw_thermal_slowdown": 0x20}
@@ -224,15 +230,7 @@ def cpu_arm(workload, steps, warmup, budget_s):
     }
 
 
-def static_traffic(workload):
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_summary.json")) as f:
-            return json.load(f).get(workload, {}).get("framed_dram_bytes_per_launch")
-    except Exception:  # noqa: BLE001
-        return None
-
-
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 def reference_available():
@@ -240,8 +238,8 @@ def reference_available():
 
 
 def _reference_module(workload):
-    """The UNMODIFIED reference module of a workload, imported from baseline/_ref
-    (baseline/install_ref.sh; pip --target install of /root/reference/Installation)."""
+    """The UNMODIFIED reference module of a workload, imported from oracle/_ref
+    (oracle/install_ref.sh: a copy of the reference's pure-Python nnAudio package)."""
     if REF_DIR not in sys.path:
         sys.path.insert(0, REF_DIR)
     import importlib
@@ -297,14 +295,14 @@ def reference_cpu_arm(workload, steps, warmup, budget_s):
     return {
         "value": clips * T * steps / dt, "unit": "frames/s", "cores": threads, "kind": "reference",
         "sample": f"{clips} clip(s) x {w['L']} samples of {workload} per step, {steps} steps, unmodified "
-                  f"nnAudio 0.3.3 {w['cls']} (baseline/_ref) on CPU, torch {torch.__version__} conv1d, "
+                  f"nnAudio 0.3.3 {w['cls']} (oracle/_ref) on CPU, torch {torch.__version__} conv1d, "
                   f"{threads} threads (fastest of all / 2 / 4 / 8 of {avail} cores), {dt:.1f}s",
         "ms_per_step": 1e3 * dt / steps,
     }
 
 
 def reference_gpu_leg(workload, dev, budget_s=20.0):
-    """SURVEY.md §2.1 / §8(d): the reference's own modules (cuDNN conv1d) on the SAME B200, inputs
+    """SURVEY.md §2.1 / §8(d): the reference's own modules (cuDNN conv1d) on the same GPU, inputs
     resident, CUDA events.  The batch is halved until the reference fits in memory / its time
     budget; frames/s is reported for the batch that ran."""
     import torch
@@ -351,6 +349,21 @@ def reference_gpu_leg(workload, dev, budget_s=20.0):
     return {"value": None, "unavailable": last_err}
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_output(out_dir, name, y):
+    """DIR/<name>.npy: the output as float32, cut to its first clips when the whole exceeds 64 MB."""
+    import numpy as np
+
+    a = y.detach().float().cpu().numpy()
+    per_clip = max(1, a[:1].nbytes)
+    if a.nbytes > DUMP_LIMIT_BYTES:
+        a = a[:max(1, DUMP_LIMIT_BYTES // per_clip)]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
+
+
 # ----------------------------------------------------------------------------
 def main():
     # stdout carries exactly ONE line (the JSON); libraries that print there (NCCL's version
@@ -369,17 +382,20 @@ def main():
 def _run():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=100,
+                    help="timed steps of the headline workload, of its e2e leg and of its no-gather leg "
+                         "(the secondary workloads use --workload-steps)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--workload", default="cfg2", choices=sorted(WORKLOADS))
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--path", default=None, choices=[None, "auto", "simt", "tcgen05"])
+    ap.add_argument("--path", default=None, choices=[None, "auto", "simt", "tc"])
     ap.add_argument("--batch", type=int, default=None, help="override per-GPU batch (debug)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-chunks", type=int, default=8)
     ap.add_argument("--no-workloads", action="store_true", help="skip the secondary configs (stft2048, cfg3, cfg4, cfg5)")
-    ap.add_argument("--workload-steps", type=int, default=10)
+    ap.add_argument("--workload-steps", type=int, default=10,
+                    help="timed steps of each secondary workload in the same line")
     ap.add_argument("--no-reference-gpu", action="store_true", help="skip the reference's cuDNN leg")
     ap.add_argument("--no-numa-bind", action="store_true")
     ap.add_argument("--watchdog", type=int, default=900, help="seconds after which a stuck run is aborted")
@@ -394,6 +410,9 @@ def _run():
                     help="SMs kept free for the concurrent NCCL gather (default: by world size)")
     ap.add_argument("--nccl-max-ctas", type=int, default=-1,
                     help="-1 = same as the SM reserve (default), 0 = NCCL's own default")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the headline workload's output of its last timed step as DIR/<workload>.npy "
+                         "(float32, <= 64 MB); secondary workloads are not dumped")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -418,10 +437,10 @@ def _run():
             return None
         if reference_available():
             res = reference_cpu_arm(args.workload, args.steps, args.warmup, budget_s=120.0)
-            arm = "the UNMODIFIED reference (baseline/_ref, nnAudio 0.3.3) on the host cores: torch conv1d (oneDNN)"
+            arm = "the UNMODIFIED reference (oracle/_ref, nnAudio 0.3.3) on the host cores: torch conv1d (oneDNN)"
         else:
             res = cpu_arm(args.workload, args.steps, args.warmup, budget_s=120.0)
-            arm = "CPU oracle port of the reference conv1d path (baseline/_ref not installed)"
+            arm = "CPU oracle port of the reference conv1d path (oracle/_ref not installed)"
         line = {
             "impl": "reference", "metric": metric, "value": res["value"], "unit": "frames/s",
             "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
@@ -506,10 +525,10 @@ def _run():
             peaks = json.load(f)
     except Exception:  # noqa: BLE001
         pass
-    tensor_peak = float(peaks.get("bf16_tflops", 1590.0))
-    hbm_peak = float(peaks.get("hbm_gbs", 6500.0))
+    tensor_peak = float(peaks.get("bf16_tflops", 989.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     peak_src = ("measured (MEASURED_PEAKS.json: bf16_tflops burst, hbm_gbs)" if peaks
-                else "fallback (B200_PROFILING.md): 1590 TFLOP/s bf16, 6500 GB/s")
+                else "H100 SXM data sheet (700 W): 989 TFLOP/s dense bf16, 3350 GB/s HBM3")
 
     def sync_all():
         if world > 1:
@@ -537,7 +556,7 @@ def _run():
         mod = getattr(nb.features, w["cls"])(verbose=False, **w["ctor"]).to(dev)
         gen = torch.Generator(device=dev).manual_seed(1234 + rank)
         batch_bytes = B * w["L"] * 4
-        # rotating input batches, > 126 MB of L2 in total: no step re-reads a cached input
+        # rotating input batches, > 160 MB in total (3x the H100's 50 MB L2): no step re-reads a cached input
         n_rot = 1 if batch_bytes > 160e6 else max(3, int(-(-160e6 // batch_bytes)))
         xs = [torch.randn(B, w["L"], generator=gen, device=dev, dtype=torch.float32) for _ in range(n_rot)]
         sharded = BatchShardedTransform(lambda inp: mod(inp, **w["fwd"]), gather=(gather and world > 1),
@@ -589,7 +608,7 @@ def _run():
             sampler.start()
             sync_all()
             e0.record()
-            run_steps(steps)
+            y_last = run_steps(steps)
             e1.record()
             sync_all()
             clocks = sampler.stop()
@@ -616,9 +635,6 @@ def _run():
             "peak": tensor_peak if bound == "tensor" else hbm_peak,
             "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
             "frac": ((tensor_alg / tensor_peak) if tensor_alg else None) if bound == "tensor" else hbm_ach / hbm_peak,
-            "traffic": static_traffic(name),
-            "traffic_note": "dram__bytes_read + write of the dominant kernel per launch from the committed ncu --set "
-                            "full capture (profiles/ncu_summary.json): static, not re-measured in this run",
             "peak_source": peak_src,
             "algorithmic_flops_per_launch": flops_launch, "avg_launch_ms": avg_launch_ms,
             "launches_timed": framed_n, "share_of_step": framed_ms / dev_ms if dev_ms else None,
@@ -637,16 +653,19 @@ def _run():
             "desc": w["desc"], "value": frames_total / (dev_ms * 1e-3), "unit": "frames/s",
             "ms_per_step": dev_ms / steps, "steps": steps, "warmup": warmup, "per_gpu_batch": B,
             "frames_per_clip": T, "gpu_launches": int(launches), "clocks": clocks, "roofline": roof,
-            "l2": f"{n_rot} rotating input batch(es) of {batch_bytes / 1e6:.0f} MB (> 126 MB L2 in total), no flush",
+            "l2": f"{n_rot} rotating input batch(es) of {batch_bytes / 1e6:.0f} MB (> 160 MB in total), no flush",
             "dtype": "bf16x3 split (fp32-equivalent), f32 accumulate" if used_tc else "f32",
         }
-        return res, mod, out_shape, w
+        return res, mod, out_shape, w, y_last
 
-    main, mod, out_shape, w = measure(args.workload, args.steps, args.warmup, gather=True)
+    main, mod, out_shape, w, y_last = measure(args.workload, args.steps, args.warmup, gather=True)
+    if args.dump_outputs and rank == 0:
+        dump_output(args.dump_outputs, args.workload, y_last)
+    del y_last
     B = w["B"]
     no_gather = None
     if world > 1:  # SURVEY.md 8(e): frames/s with and without the gather
-        ng, m_ng, _, _ = measure(args.workload, args.steps, args.warmup, gather=False)
+        ng, m_ng, _, _, _ = measure(args.workload, args.steps, args.warmup, gather=False)
         del m_ng
         no_gather = {"value": ng["value"], "ms_per_step": ng["ms_per_step"],
                      "what": "same run, transform only (shards stay on their GPUs)"}
@@ -714,7 +733,7 @@ def _run():
             for i in range(3):
                 pipe(x_hosts[i & 1], y_host, device=dev)
             sync_all()
-            n_e2e = max(args.steps, 20)
+            n_e2e = args.steps
             a, b_ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             for i in range(n_e2e):
@@ -747,7 +766,7 @@ def _run():
         torch.cuda.empty_cache()
         for name in [n for n in SECONDARY if n != args.workload]:
             try:
-                res, m2, _, _ = measure(name, steps=args.workload_steps, warmup=3, gather=False)
+                res, m2, _, _, _ = measure(name, steps=args.workload_steps, warmup=3, gather=False)
                 del m2
                 others[name] = res
             except Exception as e:  # noqa: BLE001  (never cost the headline line)

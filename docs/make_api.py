@@ -23,7 +23,7 @@ Same class names, constructor arguments (names, order, defaults), `forward` sign
 attributes as `nnAudio.features` v0.3.3 — checked against the unmodified reference by the fixtures in `tests/golden/`
 (signatures, buffers bit-identical for 49 + 7 configurations, attribute surface, exception types, outputs ≤1e-4). What differs:
 
-* inputs must be **CUDA float32** tensors on a B200 (sm_100a); anything else raises — there is no CPU fallback;
+* inputs must be **CUDA float32** tensors on an H100 (sm_90a); anything else raises — there is no CPU fallback;
 * multi-GPU: one process per GPU (`nnaudio_b200.parallel.BatchShardedTransform`, INTEGRATION.md) is the fast path;
   `torch.nn.DataParallel`, the reference's own mode, also works (per-device launch attributes and caches);
 * `Griffin_Lim.forward(S, rand_phase=None)` takes an optional initial phase (reproducible runs); `device` moves the
@@ -32,7 +32,7 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
 * `CFP` / `Combined_Frequency_Periodicity` are forward-only (the reference has no parameters there; a waveform that
   requires grad raises `NotImplementedError`); their FFT stages run as dense contractions (DESIGN.md §3.9).
 
-Environment switches: `NNAUDIO_B200_PATH=auto|simt|tcgen05` (kernel family), `NNAUDIO_B200_DECIM_BWD=fir|simt|tc|ola`
+Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAUDIO_B200_DECIM_BWD=fir|simt|tc|ola`
 (adjoint of the pyramid's FIR stages in training), `NNAB_TALL_BALANCE=0|1` (balanced tile schedule of the CQT1992v2 kernel).
 
 """

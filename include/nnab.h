@@ -21,10 +21,10 @@
  *   - `workspace` is caller-provided scratch of at least the number of bytes
  *     the matching nnab_*_workspace_bytes() query returns (may be NULL iff
  *     that query returns 0);
- *   - `path` selects the kernel family: NNAB_PATH_AUTO picks the tcgen05/TMA
- *     kernel when shape/alignment allow and the packed basis is supplied,
- *     otherwise the generic SIMT kernel.  Both are sm_100a CUDA; there is no
- *     CPU fallback.
+ *   - `path` selects the kernel family: NNAB_PATH_AUTO picks the tensor-core
+ *     (wgmma/TMA) kernels when shape/alignment allow and the packed basis is
+ *     supplied, otherwise the generic SIMT kernel.  Both are sm_90a CUDA; there
+ *     is no CPU fallback.  NNAB_PATH_TCGEN05 forces the tensor-core kernels.
  */
 #ifndef NNAB_H_
 #define NNAB_H_
@@ -46,8 +46,8 @@ extern "C" {
 typedef enum nnab_status {
   NNAB_OK = 0,
   NNAB_EINVAL = -1,     /* bad argument / shape mismatch                      */
-  NNAB_EALIGN = -2,     /* forced tcgen05 path but alignment rules not met    */
-  NNAB_EARCH = -3,      /* device is not sm_100                               */
+  NNAB_EALIGN = -2,     /* forced tensor-core path, alignment rules not met   */
+  NNAB_EARCH = -3,      /* device is not sm_90 (compute capability 9.0)       */
   NNAB_ECUDA = -4,      /* a CUDA runtime / driver call failed                */
   NNAB_EWORKSPACE = -5, /* workspace NULL or too small                        */
   NNAB_EUNSUPPORTED = -6
@@ -74,10 +74,10 @@ const char* nnab_strerror(int status);
 const char* nnab_last_cuda_error(void);
 
 /* ------------------------------------------------------------------------- *
- * Basis packing for the tcgen05 path.
+ * Basis packing for the tensor-core path.
  *
  * Splits the fp32 basis pair (re rows, im rows), each (F, K) row-major, into
- * bf16 hi/lo planes (x = hi + lo to ~2^-17) laid out for TMA/UMMA:
+ * bf16 hi/lo planes (x = hi + lo to ~2^-17) laid out for TMA/wgmma:
  *   packed[plane][tile*BN + part*BN/2 + j][k]   plane 0 = hi, 1 = lo
  *   part 0 = re rows, part 1 = NEGATED im rows, j < BN/2 bins per tile
  * with K padded to a multiple of 64 and bins zero-padded to a multiple of BN/2.
@@ -136,7 +136,7 @@ int nnab_stft_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch,
                       void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
- * Banded filterbank table (tcgen05 path): for every FFT bin the (at most two)
+ * Banded filterbank table (tensor-core path): for every FFT bin the (at most two)
  * non-zero weights of the (n_fb, F) filterbank.  Mel banks are banded like that;
  * for denser banks (gammatone) *h_max_nnz > 2 and the forward calls must be
  * given fb_table = NULL (they then run the un-fused filterbank GEMM).
@@ -151,7 +151,7 @@ int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table,
  * features/gammatone.py:171-189:  out = fb @ (|STFT(x)| ** power).
  *   fb (n_fb, F) = `mel_basis` or `gammatone_basis`;  out (B, n_fb, T)
  *   fb_table: table from nnab_build_filterbank_table (max_nnz <= 2) or NULL.
- *     With a table and the tcgen05 path the filterbank is applied in the
+ *     With a table and the tensor-core path the filterbank is applied in the
  *     contraction kernel's epilogue (no (B,F,T) intermediate in HBM).
  * ------------------------------------------------------------------------- */
 size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, int hop,
@@ -325,8 +325,8 @@ int nnab_profile_read(double* framed_ms, uint64_t* framed_launches);
 /* MMA flops the tensor-core launches EXECUTED since the last read (all bf16 split terms, tile
  * padding and structural zeros included) -> bench.py's roofline.tensor_pipe. */
 int nnab_profile_read_exec_flops(double* exec_flops);
-/* Launches of the tall-A CQT kernel that ran the balanced schedule (tiles shared between two CTA
- * pairs, framed_tc2t_kernel<., true>) since load -- lets a test tell which schedule it exercised. */
+/* Launches of the tall-A CQT kernel that ran the balanced schedule (tiles shared between two
+ * CTAs, framed_tct_kernel<., true>) since load -- lets a test tell which schedule it exercised. */
 uint64_t nnab_balanced_launch_count(void);
 
 #if defined(__GNUC__)

@@ -20,7 +20,8 @@ PAD_REFLECT, PAD_CONSTANT = 0, 1
 FMT_MAGNITUDE, FMT_COMPLEX, FMT_PHASE_ANGLE, FMT_PHASE_UNIT = 0, 1, 2, 3
 PATH_AUTO, PATH_SIMT, PATH_TCGEN05 = 0, 1, 2
 
-_PATH_NAMES = {"auto": PATH_AUTO, "simt": PATH_SIMT, "tcgen05": PATH_TCGEN05}
+# "tc" = the wgmma/TMA tensor-core kernels; "tcgen05" (the C constant's name) means the same
+_PATH_NAMES = {"auto": PATH_AUTO, "simt": PATH_SIMT, "tc": PATH_TCGEN05, "tcgen05": PATH_TCGEN05}
 
 # every symbol include/nnab.h declares: (restype, argtypes)
 _P = c_void_p
@@ -136,7 +137,7 @@ def lib() -> ctypes.CDLL:
 
 
 def default_path() -> int:
-    """Kernel family selector; ``NNAUDIO_B200_PATH=auto|simt|tcgen05``."""
+    """Kernel family selector; ``NNAUDIO_B200_PATH=auto|simt|tc``."""
     return _PATH_NAMES[os.environ.get("NNAUDIO_B200_PATH", "auto").lower()]
 
 
@@ -194,7 +195,7 @@ def _dev_f32(t: torch.Tensor, name: str) -> torch.Tensor:
         raise TypeError(f"{name} must be a torch.Tensor")
     if not t.is_cuda:
         raise RuntimeError(
-            f"{name} is on {t.device}: nnaudio_b200 runs only on CUDA (sm_100a) tensors; "
+            f"{name} is on {t.device}: nnaudio_b200 runs only on CUDA (sm_90a) tensors; "
             "there is no CPU fallback"
         )
     if t.dtype != torch.float32:
@@ -283,14 +284,14 @@ def _rows(x: torch.Tensor):
 
 
 # --------------------------------------------------------------------------- #
-# basis packing (tcgen05 path)
+# basis packing (tensor-core path)
 # --------------------------------------------------------------------------- #
 LAYOUT_DENSE, LAYOUT_GROUPS = 0, 3
 
 
 def pack_basis(w_re: torch.Tensor, w_im: torch.Tensor, layout: int = LAYOUT_DENSE):
-    """bf16 hi/lo split of an (F, K) fp32 basis pair in the TMA/UMMA layout, or
-    ``None`` when the library has no tcgen05 kernel for it.  ``layout``: LAYOUT_GROUPS for long
+    """bf16 hi/lo split of an (F, K) fp32 basis pair in the TMA/wgmma layout, or
+    ``None`` when the library has no tensor-core kernel for it.  ``layout``: LAYOUT_GROUPS for long
     nested CQT banks (per-K-block-width / tall-A kernels)."""
     L = lib()
     F, K = w_re.shape
@@ -350,7 +351,7 @@ def pack_fir(fir: torch.Tensor, dec: int):
 
 def build_filterbank_table(fb: torch.Tensor):
     """Banded (<= 2 non-zeros per FFT bin) table of an (n_fb, F) filterbank for the
-    fused tcgen05 epilogue, or ``None`` when the bank is denser (e.g. gammatone).
+    fused tensor-core epilogue, or ``None`` when the bank is denser (e.g. gammatone).
     Init-time: synchronises the current stream once."""
     L = lib()
     n_fb, F = fb.shape

@@ -1,4 +1,4 @@
-"""nnaudio_b200 — B200-native (sm_100a) audio -> spectrogram engine with the
+"""nnaudio_b200 — H100-native (sm_90a) audio -> spectrogram engine with the
 ``nnAudio.features`` module API.  See DESIGN.md / INTEGRATION.md."""
 __version__ = "0.1.0"
 

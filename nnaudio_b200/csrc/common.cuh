@@ -1,4 +1,4 @@
-// Shared declarations for libnnab.so (sm_100a only).
+// Shared declarations for libnnab.so (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -38,20 +38,20 @@ void add_exec_flops(double flops);
     }                                               \
   } while (0)
 
-// ---- problem description shared by the SIMT and tcgen05 framed kernels ----
+// ---- problem description shared by the SIMT and tensor-core framed kernels ----
 // One "framed complex contraction":
 //   re[b,f,t] = sum_k xpad[b, t*hop + k] * w_re[f,k]
 //   im[b,f,t] = -sum_k xpad[b, t*hop + k] * w_im[f,k]
 // followed by a per-bin scale and one of the output formats of nnab.h (or the
 // internal POWER format used by the filterbank ops).
 constexpr int FMT_POWER = 100;  // internal: (sqrt(re^2+im^2+eps)) ** power -> (B,F,T)
-constexpr int FMT_FBANK = 101;  // internal (tcgen05 only): power -> banded filterbank -> (B,n_fb,T)
-constexpr int FMT_DECIM = 102;  // internal (tcgen05 only): FIR decimator stage of the CQT pyramid
-constexpr int FMT_RAW = 103;    // internal (tcgen05 only): split-K partial sums -> raw (re, im) scratch
-constexpr int FMT_OLA = 104;    // internal (tcgen05 only): inverse STFT frames -> overlap-add buffer
+constexpr int FMT_FBANK = 101;  // internal (tensor-core only): power -> banded filterbank -> (B,n_fb,T)
+constexpr int FMT_DECIM = 102;  // internal (tensor-core only): FIR decimator stage of the CQT pyramid
+constexpr int FMT_RAW = 103;    // internal (tensor-core only): split-K partial sums -> raw (re, im) scratch
+constexpr int FMT_OLA = 104;    // internal (tensor-core only): inverse STFT frames -> overlap-add buffer
 constexpr int FMT_PLANES = 105;   // internal (block-partial kernel only): power spectrum -> bf16 hi/lo operand
                                   //   planes of the dense-filterbank GEMM (`out` = plane base, see planes_*)
-constexpr int FMT_REALPAIR = 106; // internal (dense tcgen05 kernel only): two real outputs per complex column
+constexpr int FMT_REALPAIR = 106; // internal (dense tensor-core kernel only): two real outputs per complex column
                                   //   pair: re -> row f, im -> row f + F of a real (B, out_bins, T) tensor
 
 // FMT_DECIM epilogue target: the NEXT pyramid level, written as bf16 hi/lo planes in
@@ -84,10 +84,10 @@ struct FbStep {
 };
 static_assert(sizeof(FbStep) == 16, "one 128-bit load per bin");
 constexpr int FB_STEP_PAD = 160;  // entries past F (a tile's last chunk may overrun the last bin)
-// epilogue warps per TMEM lane quarter of the fused-filterbank block kernel: each covers a contiguous
+// epilogue warps per 32-row quarter of the fused-filterbank block kernel: each covers a contiguous
 // range of a tile's 8-column chunks, [n_chunks * part / PARTS, n_chunks * (part + 1) / PARTS)
-// (3 measured 7 % faster at cfg2 -- 0.197 vs 0.211 ms -- but then a 53-bin mel filter spans three
-// ranges, its three atomic partial sums no longer commute and results differ run to run: 2 it is.)
+// (with 3, a 53-bin mel filter spans three ranges, its three atomic partial sums no longer commute and
+// results differ run to run: 2 it is.)
 constexpr int FB_EPI_PARTS = 2;
 
 struct FramedProblem {
@@ -113,8 +113,8 @@ struct FramedProblem {
   const FbStep* fb_steps;    // FMT_FBANK, block-partial kernel: [F + FB_STEP_PAD] (nullptr: MelRun path)
   int fb_nb_mask;            // bit i: tile width nb = 32 + 8 i gives <= 2 partial sums per filter
   int n_fb;
-  float* raw;                // tcgen05 split-K scratch: 2 planes (re, im) of B*F*T floats, or nullptr
-  const void* presplit;      // tcgen05: already padded + split signal planes (skip pad_split)
+  float* raw;                // tensor-core split-K scratch: 2 planes (re, im) of B*F*T floats, or nullptr
+  const void* presplit;      // tensor-core path: already padded + split signal planes (skip pad_split)
   int64_t presplit_t_slots;  // > 0: frames per clip slot of the pre-split planes (else derived)
   int64_t presplit_plane_stride;  // elements per plane when presplit_t_slots > 0
   DecimParams dec;           // FMT_DECIM
@@ -127,7 +127,7 @@ struct FramedProblem {
 
 int launch_framed_simt(const FramedProblem& p, cudaStream_t stream);
 
-// tcgen05 path (tc_kernels.cu)
+// tensor-core path (tc_kernels.cu)
 bool tc_supported(const FramedProblem& p);
 size_t tc_workspace_bytes(int64_t B, int64_t L, int K, int hop, int pad);
 int launch_framed_tc(const FramedProblem& p, const void* packed, void* workspace,

@@ -1,4 +1,4 @@
-// Output-format epilogue shared by the SIMT and tcgen05 framed kernels.
+// Output-format epilogue shared by the SIMT and tensor-core framed kernels.
 // Mirrors the element-wise tails of the reference forward() bodies:
 //   STFT   stft.py:299-316     CQT1992v2  cqt.py:752-780
 //   CQT2010v2 cqt.py:1112-1139 Mel/Gammatone power  mel.py:186
@@ -83,8 +83,8 @@ __device__ __forceinline__ void epi_store(const EpiParams& e, int64_t b, int f, 
   }
 }
 
-// Compile-time-format variant for the tcgen05 kernel: keeps the 32x unrolled
-// TMEM read-out loop small enough to stay in the instruction cache.
+// Compile-time-format variant for the tensor-core kernels: keeps the 32x unrolled
+// accumulator read-out loop small enough to stay in the instruction cache.
 //   FMT: 0..3 = NNAB_FMT_*, 4 = FMT_POWER, 9 = FMT_REALPAIR.  `dst` already points at element
 //   (b, bin_offset, t) of the output (float2 elements for the 2-channel formats).
 template <int FMT>

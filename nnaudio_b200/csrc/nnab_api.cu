@@ -50,9 +50,10 @@ static int check_common(const float* x, int64_t B, int64_t L, int64_t x_pitch, i
 static int check_arch() {
   int dev = 0;
   NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  int major = 0;
+  int major = 0, minor = 0;
   NNAB_CUDA_TRY(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  return major == 10 ? NNAB_OK : NNAB_EARCH;
+  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  return (major == 9 && minor == 0) ? NNAB_OK : NNAB_EARCH;  // sm_90a code runs on compute capability 9.0 only
 }
 
 // ---- optional in-stream timing of the framed contraction (bench.py) --------
@@ -142,8 +143,8 @@ const char* nnab_strerror(int status) {
   switch (status) {
     case NNAB_OK: return "ok";
     case NNAB_EINVAL: return "invalid argument or shape mismatch";
-    case NNAB_EALIGN: return "tcgen05 path forced but shape/alignment rules not met";
-    case NNAB_EARCH: return "device is not sm_100 (B200)";
+    case NNAB_EALIGN: return "tensor-core path forced but shape/alignment rules not met";
+    case NNAB_EARCH: return "device is not sm_90 (H100)";
     case NNAB_ECUDA: return "CUDA error";
     case NNAB_EWORKSPACE: return "workspace missing or too small";
     case NNAB_EUNSUPPORTED: return "unsupported size";
@@ -320,13 +321,13 @@ int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table, i
 
 // ---- dense filterbank (Gammatonegram, dense mel banks) on the tensor cores -------------------------
 // The block-partial STFT kernel writes |X| ** power straight into bf16 hi/lo operand planes (FMT_PLANES: one
-// row per frame, 4 B per value, no fp32 (B, F, T) intermediate), a second tcgen05 launch contracts the rows
+// row per frame, 4 B per value, no fp32 (B, F, T) intermediate), a second tensor-core launch contracts the rows
 // with the re-indexed bank (real GEMM on the complex kernel, FMT_REALPAIR) and writes (B, n_fb, T).
 // Workspace: [signal planes of the STFT][operand planes][bank fp32 re | im][packed bank].
 static bool fb_planes_enabled() {
   if (const char* e = getenv("NNAB_FB_PLANES")) return atoi(e) != 0;
-  // on by default: GPU-verified (profiles/r02c_*: oracle <= 8e-6, bit-repeatable; Gammatonegram at the cfg2
-  // shape 0.330 -> 0.249 ms); 0 = fp32 (B, F, T) power spectrogram + CUDA-core filterbank GEMM (round 1)
+  // on by default (tests/test_zz_gpu_fb_planes.py: oracle parity, bit-repeatable); 0 = fp32 (B, F, T) power
+  // spectrogram + CUDA-core filterbank GEMM
   return true;
 }
 
@@ -630,7 +631,7 @@ static size_t plan_pyramid(int64_t B, int64_t L, int n_octaves, int early_factor
 // ---------------------------------------------------------------------------------------------
 // Pyramid, second generation (round 2): ONE plane set per level, shared by the level's octave CQT
 // (reflect margins of `pad` samples, frames every `hop`) and by the FIR stage that produces the next
-// level (256-sample rows, resident taps, clip edges recomputed: launch_fir_stage_tc).  Per level and
+// level (256-sample rows, banded taps, clip edges recomputed: launch_fir_stage_tc).  Per level and
 // sample: one 4-byte write and one read by each consumer, instead of two differently padded copies.
 // ---------------------------------------------------------------------------------------------
 struct Lvl2 {

@@ -1,9 +1,9 @@
-// Generic fp32 CUDA-core kernels of libnnab.so (sm_100a):
+// Generic fp32 CUDA-core kernels of libnnab.so (sm_90a):
 //   * framed complex contraction (any hop / K / F, sparse-support aware)
 //   * filterbank GEMM  out = fb @ P      (mel.py:188, gammatone.py:188)
 //   * MFCC tail        dB -> top_db clamp -> DCT   (mel.py:263-307, 325)
 //   * FIR decimation   conv1d(x, fir, stride=n, padding=127)  (utils.py:73-124)
-// They are the first-correct path and the fallback for shapes the tcgen05/TMA
+// They are the first-correct path and the fallback for shapes the wgmma/TMA
 // kernel does not take (hop % 8 != 0, tiny banks, ...).  No CPU fallback exists.
 #include "common.cuh"
 #include "epilogue.cuh"
@@ -145,7 +145,7 @@ int launch_framed_simt(const FramedProblem& q, cudaStream_t stream) {
   p.epi.raw = nullptr; p.epi.raw_plane = 0;
   p.epi.ola_pitch = 0; p.epi.ola_hop = 0;
   if (q.fmt == FMT_FBANK || q.fmt == FMT_DECIM || q.fmt == FMT_RAW || q.fmt == FMT_OLA)
-    return NNAB_EINVAL;  // fused filterbank exists on the tcgen05 path only
+    return NNAB_EINVAL;  // fused filterbank exists on the tensor-core path only
 
   const int TN = (q.F > 32) ? 4 : 2;
   const int BNB = 16 * TN;
@@ -359,7 +359,7 @@ int launch_filterbank(const float* P, const float* fb, int64_t B, int F, int64_t
   return NNAB_OK;
 }
 
-// Dense filterbank as the B operand of a real GEMM on the complex tcgen05 kernel: the (n_fb, F) weights
+// Dense filterbank as the B operand of a real GEMM on the complex tensor-core kernel: the (n_fb, F) weights
 // re-indexed to the column layout of the block-partial kernel's FMT_PLANES output (tile n, packed column
 // i  <->  FFT bin n (nb - 2) + i - 2; columns 0, 1 of a tile and bins >= F carry zeros), filters
 // [0, fh) in the real bank and filters [fh, 2 fh) NEGATED in the imaginary bank (the contraction returns

@@ -1,5 +1,5 @@
 // FIR-decimator epilogue shared by the tensor-core kernels (tc_kernels.cu FMT_DECIM, tct_kernels.cu
-// fir_tc_kernel): a thread holds 2*half consecutive outputs of one clip in its TMEM lane and writes
+// fir_tc_kernel): a thread holds 2*half consecutive outputs of one clip in its accumulator row and writes
 // them as the NEXT pyramid level -- bf16 hi/lo planes in the layout that level's kernels read
 // (utils.py:73-124 conv1d(stride=2, padding=127); cqt.py:1065-1068 reflect padding per level).
 #pragma once
@@ -16,8 +16,8 @@ __device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bflo
   lo = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
-// trow: TMEM address of this warp's lane quarter / accumulator; tl: frame index inside clip b.
-// [c_lo, c_hi): the TMEM columns (= outputs of the frame) this warp handles (c_hi < 0: all 2*half).
+// trow: accumulator-tile address of this warp's 32 rows (tc_ptx.cuh); tl: frame index inside clip b.
+// [c_lo, c_hi): the accumulator columns (= outputs of the frame) this warp handles (c_hi < 0: all 2*half).
 __device__ __forceinline__ void epilogue_decim(const DecimParams& d, uint32_t trow, int64_t b,
                                                int64_t tl, bool valid, int half, int c_lo = 0,
                                                int c_hi = -1) {
@@ -29,8 +29,7 @@ __device__ __forceinline__ void epilogue_decim(const DecimParams& d, uint32_t tr
 #pragma unroll 1
         for (int c0 = c_lo; c0 < c_hi; c0 += 8) {
           uint32_t v[8];
-          tmem_ld8(trow + (uint32_t)c0, v);  // re half = outputs 0..half-1, im half = the rest
-          tmem_ld_wait();
+          acc_ld8(trow + (uint32_t)c0, v);  // re half = outputs 0..half-1, im half = the rest
           const int64_t n = n0 + c0;
           if (valid && n < d.len_out) {
             __align__(16) __nv_bfloat16 hi[8];

@@ -49,7 +49,7 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
 int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* workspace, size_t ws_bytes,
                           cudaStream_t stream);
 
-// FIR decimator stage with resident taps (tct_kernels.cu); NNAB_EUNSUPPORTED = geometry not eligible
+// FIR decimator stage with banded taps (tct_kernels.cu); NNAB_EUNSUPPORTED = geometry not eligible
 int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int64_t src_pitch,
                         int64_t src_plane_stride, int src_pad, const void* fir_packed,
                         const float* fir, int taps, const DecimParams& dec, cudaStream_t stream);

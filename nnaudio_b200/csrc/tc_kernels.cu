@@ -1,22 +1,22 @@
-// tcgen05 / TMA framed contraction for sm_100a.
+// wgmma / TMA framed contraction for sm_90a.
 //
 //   D[g, n] = sum_k A[g, k] * W[n, k]        g = virtual frame, n = basis row
 //
 // * A is never materialised: the padded waveform is written once as bf16 hi/lo
 //   planes (pad_split_kernel) with a per-clip pitch that is a multiple of hop, so
 //   the frames of the WHOLE batch form one Toeplitz matrix whose row g starts at
-//   element g*hop.  TMA reads 128-frame x BK tiles of it straight into
-//   128B/64B-swizzled shared memory (either as a plain (rows x hop) matrix when
-//   BK | hop, or through an overlapping-stride tensor map otherwise).
+//   element g*hop.  TMA reads 128-frame x 64 tiles of it straight into
+//   128B-swizzled shared memory (either as a plain (rows x hop) matrix when
+//   64 | hop, or through an overlapping-stride tensor map otherwise).
 // * W (basis) is pre-split into bf16 hi/lo planes, re rows and NEGATED im rows
 //   grouped per N tile (pack_basis_kernel).
 // * fp32 parity on bf16 tensor cores: x*w ~= xhi*whi + xlo*whi + xhi*wlo
-//   (3 tcgen05.mma passes into one fp32 TMEM accumulator; error ~2^-16).
-// * Warp roles (256 threads, 1 CTA/SM, persistent over output tiles):
-//     warp 0  TMA producer      warp 1  MMA issuer      warp 2  TMEM alloc
-//     warps 4-7  epilogue: tcgen05.ld -> magnitude/complex/phase/power ->
-//                coalesced stores in the reference's (B, F, T[,2]) layout
-//   smem full/empty mbarrier ring + double-buffered TMEM accumulators.
+//   (3 wgmma passes into one fp32 register accumulator; error ~2^-16).
+// * Warp roles (288 threads, 1 CTA/SM, persistent over output tiles, tc_ptx.cuh):
+//     warps 0-7  two wgmma warpgroups (64 tile rows each), then the epilogue from the shared-memory
+//                accumulator tile -> magnitude/complex/phase/power -> coalesced stores in the
+//                reference's (B, F, T[,2]) layout
+//     warp 8     TMA producer (full/empty mbarrier ring)
 #include <cuda.h>
 #include <atomic>
 #include <mutex>
@@ -35,7 +35,6 @@
 namespace nnab {
 
 constexpr int TC_MAX_N_TILES = 128;
-constexpr int TC_ACC_STRIDE = 256;  // TMEM columns per accumulator buffer
 
 
 // N tile (columns = re + im rows of bn/2 bins): minimise padded columns.
@@ -696,7 +695,6 @@ struct TcParams {
   int hop;          // effective hop (hop * phases)
   int t_mul, t_add;  // output frame index = t * t_mul + t_add (frame phases)
   int k_splits;      // >1: every (m, n) tile is cut into k_splits K-chunks (FMT_RAW epilogue)
-  int split4;        // EXPERIMENTAL (NNAB_SPLIT4=1): add the x_lo * w_lo term (4 MMAs per K16 step)
   int64_t nv, t_slots, T;  // T = valid frames of this phase
   int kb_begin[TC_MAX_N_TILES];
   int kb_end[TC_MAX_N_TILES];
@@ -708,7 +706,7 @@ struct TcParams {
 // no zero-fill of the scratch): all chunks of a tile go to the same worker, consecutively, so chunk c
 // of a tile adds after chunk c-1 has stored, in program order of one thread.  (A balanced round-robin
 // of the units with flag-ordered adds measured 2.04 ms vs 1.27 ms at cfg3: the chunks of a tile
-// finish their MMAs together and their epilogues then serialise while holding TMEM buffers.)
+// finish their MMAs together and their epilogues then serialise.)
 __device__ __forceinline__ int sched_tile(int u, int worker, int n_workers, int num_mn, int ks) {
   const int mn = worker + (u / ks) * n_workers;
   return mn < num_mn ? mn * ks + (u % ks) : -1;
@@ -726,7 +724,7 @@ __device__ __forceinline__ void decode_tile(const TcParams& p, int tile, int& m_
   kb1 = lo + (int)(((int64_t)n * (ks + 1)) / p.k_splits);
 }
 
-// Read one 128-frame x bn accumulator tile out of TMEM (this warp's 32 lanes =
+// Read one 128-frame x bn accumulator tile out of shared memory (this warp's 32 lanes =
 // 32 consecutive frames) and emit it in the requested output format.
 template <int FMT>
 __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, int64_t g,
@@ -743,8 +741,7 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
 #pragma unroll 1
         for (int c0 = 0; c0 < 2 * half; c0 += 8) {
           uint32_t v[8];
-          tmem_ld8(trow + (uint32_t)c0, v);
-          tmem_ld_wait();
+          acc_ld8(trow + (uint32_t)c0, v);
           if (valid) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -763,9 +760,8 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
 #pragma unroll 1
         for (int c0 = 0; c0 < half; c0 += 8) {
           uint32_t re[8], im[8];
-          tmem_ld8(trow + (uint32_t)c0, re);
-          tmem_ld8(trow + (uint32_t)(half + c0), im);
-          tmem_ld_wait();
+          acc_ld8(trow + (uint32_t)c0, re);
+          acc_ld8(trow + (uint32_t)(half + c0), im);
           if (valid) {
             const int jmax = min(8, min(half - c0, p.epi.F - f_base - c0));
 #pragma unroll
@@ -788,14 +784,13 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
         float* mel = p.epi.out + ((int64_t)b * p.epi.n_fb) * p.epi.T + t;
         int cj0 = -1, cj1 = -1;
         float a0 = 0.f, a1 = 0.f;
-        // rolled loop over 8-column TMEM loads: the body must stay I-cache resident
+        // rolled loop over 8-column loads: the body must stay I-cache resident
         // (a 32x unrolled version was ~80 KB of code per tile and fetch-stalled)
 #pragma unroll 1
         for (int c0 = 0; c0 < half; c0 += 8) {
           uint32_t re[8], im[8];
-          tmem_ld8(trow + (uint32_t)c0, re);
-          tmem_ld8(trow + (uint32_t)(half + c0), im);
-          tmem_ld_wait();
+          acc_ld8(trow + (uint32_t)c0, re);
+          acc_ld8(trow + (uint32_t)(half + c0), im);
           const int jmax = min(8, min(half - c0, p.epi.F - f_base - c0));
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -826,12 +821,11 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
       constexpr int CH = (FMT == NNAB_FMT_COMPLEX || FMT == NNAB_FMT_PHASE_UNIT) ? 2 : 1;
       float* dst = p.epi.out + (((int64_t)b * p.epi.out_bins + p.epi.bin_offset) * p.epi.T + t) * CH;
       if constexpr (FMT == NNAB_FMT_MAGNITUDE || FMT == NNAB_FMT_COMPLEX) {
-        // light per-bin code: 32 columns per TMEM load, fully unrolled
+        // light per-bin code: 32 columns per load, fully unrolled
         for (int c0 = 0; c0 < half; c0 += 32) {
           uint32_t re[32], im[32];
-          tmem_ld32(trow + (uint32_t)c0, re);
-          tmem_ld32(trow + (uint32_t)(half + c0), im);
-          tmem_ld_wait();
+          acc_ld32(trow + (uint32_t)c0, re);
+          acc_ld32(trow + (uint32_t)(half + c0), im);
           if (valid) {
             const int jmax = min(32, min(half - c0, p.epi.F - f_base - c0));
             if (jmax == 32) {
@@ -853,9 +847,8 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
 #pragma unroll 1
         for (int c0 = 0; c0 < half; c0 += 8) {
           uint32_t re[8], im[8];
-          tmem_ld8(trow + (uint32_t)c0, re);
-          tmem_ld8(trow + (uint32_t)(half + c0), im);
-          tmem_ld_wait();
+          acc_ld8(trow + (uint32_t)c0, re);
+          acc_ld8(trow + (uint32_t)(half + c0), im);
           if (valid) {
             const int jmax = min(8, min(half - c0, p.epi.F - f_base - c0));
 #pragma unroll
@@ -869,67 +862,56 @@ __device__ __forceinline__ void epilogue_tile(const TcParams& p, uint32_t trow, 
       }
 }
 
-template <int BK, int STAGES>
 struct TcSmem {
-  static constexpr uint32_t A_BYTES = TC_BM * BK * 2;
-  static constexpr uint32_t B_BYTES = 256 * BK * 2;
+  static constexpr int STAGES = 2;
+  static constexpr uint32_t A_BYTES = TC_BM * 64 * 2;   // one plane, 128 rows x 64 bf16
+  static constexpr uint32_t B_BYTES = 256 * 64 * 2;     // one plane, <= 256 basis rows
   static constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr uint32_t BAR_OFFSET = STAGES * STAGE_BYTES;
   static constexpr uint32_t TOTAL = BAR_OFFSET + 256 + 1024;  // + barriers + align slack
+  // the accumulator tile (128 rows x <= 256 fp32) reuses the stages once a unit's K range is drained
+  static_assert(TC_BM * 256 * 4 <= BAR_OFFSET, "accumulator tile does not fit the stage ring");
 };
 
-template <int BK, int STAGES, int FMT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+// Persistent over work units (output tile x K chunk).  Per unit the producer streams the K blocks through
+// a 2-stage ring, both consumer warpgroups accumulate their 64 rows in registers, then store them into the
+// accumulator tile (over the drained ring) and warps 0-3 run the epilogue, one tile row per thread.  The
+// producer starts the next unit's loads once the tile has been read out (drained_bar).
+template <int FMT>
+__global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
 framed_tc_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                  const TcParams p) {
-  using S = TcSmem<BK, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  using S = TcSmem;
+  constexpr int BK = 64, STAGES = S::STAGES;
+  const uint32_t base = acc_tile_base();
   const uint32_t bar_base = base + S::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  const uint32_t drained_bar = bar_base + 8u * (2 * STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a);
-    prefetch_tmap(&tm_b);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 4);  // one arrival per epilogue warp
-    }
+    mbar_init(drained_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   const int num_mn = p.num_m_tiles * p.num_n_tiles;
-  const uint32_t b_tile_bytes = (uint32_t)p.bn * BK * 2;
-
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (elect_one()) {
+      prefetch_tmap(&tm_a);
+      prefetch_tmap(&tm_b);
+      const uint32_t b_tile_bytes = (uint32_t)p.bn * BK * 2;
       int stage = 0;
       uint32_t phase = 0;
       for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, num_mn, p.k_splits)) >= 0; ++u) {
+        if (u > 0) mbar_wait(drained_bar, (uint32_t)(u - 1) & 1u);
         int m_tile, n_tile, kb0, kb1;
         decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
         const int m0 = m_tile * TC_BM;
@@ -952,247 +934,49 @@ framed_tc_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      // instruction descriptor: D=f32 (bit4), A=B=bf16 (bits 7,10), K-major, N>>3 @17, M>>4 @24
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) |
-                             ((uint32_t)(TC_BM >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, num_mn, p.k_splits)) >= 0; ++u) {
-        int m_tile, n_tile, kb0, kb1;
-        decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
-        (void)m_tile;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * TC_ACC_STRIDE;
-        uint32_t accumulate = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
+    return;
+  }
+
+  // ===================== consumers: wgmma (warpgroup wg = rows 64 wg ..) + epilogue =====================
+  const int wg = warp >> 2;
+  const uint32_t a_off = (uint32_t)wg * 64u * (BK * 2);
+  // Row stride of the accumulator tile: the 32-column read-out of epilogue_tile (Magnitude / Complex)
+  // reads im columns half + [0, round_up(half, 32)), past bn when 32 does not divide half; those reads
+  // must stay inside the thread's own row (their values are dropped by the jmax guard).
+  const int half_n = p.bn >> 1;
+  const uint32_t tile_addr = acc_tile(half_n + ((half_n + 31) & ~31));
+  float acc[128];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, num_mn, p.k_splits)) >= 0; ++u) {
+    int m_tile, n_tile, kb0, kb1;
+    decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t koff = (uint32_t)k * 32u;  // 16 bf16 along K inside the swizzle atom
-            const uint64_t a_hi = make_smem_desc<BK>(sb + koff);
-            const uint64_t a_lo = make_smem_desc<BK>(sb + S::A_BYTES + koff);
-            const uint64_t b_hi = make_smem_desc<BK>(sb + 2 * S::A_BYTES + koff);
-            const uint64_t b_lo = make_smem_desc<BK>(sb + 2 * S::A_BYTES + S::B_BYTES + koff);
-            umma_bf16(d_tmem, a_lo, b_hi, idesc, accumulate);
-            umma_bf16(d_tmem, a_hi, b_lo, idesc, 1u);
-            umma_bf16(d_tmem, a_hi, b_hi, idesc, 1u);
-            accumulate = 1u;
-          }
-          umma_commit(empty_bar(stage));  // frees the smem slot when these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(tfull_bar(acc));  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (warps 4..7 <-> TMEM lane quarters) =====================
-    const int quarter = warp & 3;
-    const int half = p.bn >> 1;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, num_mn, p.k_splits)) >= 0; ++u) {
-      int m_tile, n_tile, kb0, kb1;
-      decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
-      (void)kb0; (void)kb1;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const int64_t g = (int64_t)m_tile * TC_BM + quarter * 32 + lane;
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)acc * TC_ACC_STRIDE;
-      epilogue_tile<FMT>(p, trow, g, n_tile, half, tile % p.k_splits, tile / p.k_splits);
-      tcgen05_fence_before();
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;  // (the previous unit's values are dead after acc_store)
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sb = base + stage * S::STAGE_BYTES;
+      wgmma_fence();
+      wg_kblock_split3<256>(p.bn, acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
+                            wg_desc_lo(sb + 2 * S::A_BYTES), wg_desc_lo(sb + 2 * S::A_BYTES + S::B_BYTES),
+                            kb != kb0);
+      wgmma_commit();
+      wgmma_wait_all();
       __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+      if (lane == 0) mbar_arrive(empty_bar(stage));  // this warp is done reading the stage
+      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
     }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-
-// ---------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): a cluster of two CTAs computes a
-// 256-frame x bn tile.  Each CTA stages its own 128 A rows and HALF of the B
-// tile (CTA 0: the re rows, CTA 1: the negated im rows), the leader issues
-// M=256 MMAs that read B from both SMs, and every CTA keeps its 128 x bn
-// accumulators in its own TMEM.  Per SM this halves the B operand reads and TMA
-// fills — the shared-memory bandwidth that bounds the 1-CTA kernel at ~76 %.
-// ---------------------------------------------------------------------------
-template <int BK, int STAGES>
-struct Tc2Smem {
-  static constexpr uint32_t A_BYTES = TC_BM * BK * 2;
-  static constexpr uint32_t B_BYTES = 128 * BK * 2;  // half of a bn <= 256 tile
-  static constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr uint32_t BAR_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr uint32_t TOTAL = BAR_OFFSET + 256 + 1024;
-};
-
-template <int BK, int STAGES, int FMT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-framed_tc2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                  const TcParams p) {
-  using S = Tc2Smem<BK, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = base + S::BAR_OFFSET;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };            // used in the leader
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };  // per CTA
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };       // per CTA
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };  // leader
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta = cluster_ctarank();  // 0 = leader
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a);
-    prefetch_tmap(&tm_b);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 2);   // one arrive.expect_tx per CTA's producer
-      mbar_init(empty_bar(s), 1);  // multicast commit from the leader
+    consumer_sync();  // both warpgroups are done with the ring: the tile may overwrite it
+    acc_store<256>(tile_addr, acc, p.bn, wg * 64);
+    consumer_sync();
+    if (warp < 4) {
+      const int64_t g = (int64_t)m_tile * TC_BM + warp * 32 + lane;
+      epilogue_tile<FMT>(p, tile_addr + acc_row((uint32_t)warp * 32u), g, n_tile, p.bn >> 1,
+                         tile % p.k_splits, tile / p.k_splits);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 8);  // 4 epilogue warps x 2 CTAs
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();  // peer barriers are initialised before any remote arrive / TMA credit
-  if (warp == 2) {
-    tmem_alloc_2sm(tmem_slot, 512);
-    tmem_relinquish_2sm();
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  const int num_mn = p.num_m_tiles * p.num_n_tiles;  // num_m_tiles: 256-frame pairs
-  const int halfn = p.bn >> 1;
-  const uint32_t b_half_bytes = (uint32_t)halfn * BK * 2;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, num_mn, p.k_splits)) >= 0; ++u) {
-        int m_tile, n_tile, kb0, kb1;
-        decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
-        const int m0 = m_tile * (2 * TC_BM) + (int)cta * TC_BM;
-        const int n0 = n_tile * p.bn + (int)cta * halfn;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
-          mbar_expect_tx_remote(full_bar(stage), 0, 2 * S::A_BYTES + 2 * b_half_bytes);
-          const int k0 = kb * BK;
-          int c0 = k0, c1 = m0;
-          if (p.rows_mode) {
-            c1 = m0 + k0 / p.hop;
-            c0 = k0 - (k0 / p.hop) * p.hop;
-          }
-          tma_load_3d_2sm(sb, &tm_a, full_bar(stage), c0, c1, 0);
-          tma_load_3d_2sm(sb + S::A_BYTES, &tm_a, full_bar(stage), c0, c1, 1);
-          tma_load_3d_2sm(sb + 2 * S::A_BYTES, &tm_b, full_bar(stage), k0, n0, 0);
-          tma_load_3d_2sm(sb + 2 * S::A_BYTES + S::B_BYTES, &tm_b, full_bar(stage), k0, n0, 1);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (cta == 0 && elect_one()) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) |
-                             ((uint32_t)((2 * TC_BM) >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, num_mn, p.k_splits)) >= 0; ++u) {
-        int m_tile, n_tile, kb0, kb1;
-        decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
-        (void)m_tile;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * TC_ACC_STRIDE;
-        uint32_t accumulate = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t koff = (uint32_t)k * 32u;
-            const uint64_t a_hi = make_smem_desc<BK>(sb + koff);
-            const uint64_t a_lo = make_smem_desc<BK>(sb + S::A_BYTES + koff);
-            const uint64_t b_hi = make_smem_desc<BK>(sb + 2 * S::A_BYTES + koff);
-            const uint64_t b_lo = make_smem_desc<BK>(sb + 2 * S::A_BYTES + S::B_BYTES + koff);
-            if (p.split4) {  // smallest term first: fp32-like accuracy for the training forward
-              umma_bf16_2sm(d_tmem, a_lo, b_lo, idesc, accumulate);
-              accumulate = 1u;
-            }
-            umma_bf16_2sm(d_tmem, a_lo, b_hi, idesc, accumulate);
-            umma_bf16_2sm(d_tmem, a_hi, b_lo, idesc, 1u);
-            umma_bf16_2sm(d_tmem, a_hi, b_hi, idesc, 1u);
-            accumulate = 1u;
-          }
-          umma_commit_2sm(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_2sm(tfull_bar(acc));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs, own 128 rows) =====================
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, num_mn, p.k_splits)) >= 0; ++u) {
-      int m_tile, n_tile, kb0, kb1;
-      decode_tile(p, tile, m_tile, n_tile, kb0, kb1);
-      (void)kb0; (void)kb1;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const int64_t g = (int64_t)m_tile * (2 * TC_BM) + (int64_t)cta * TC_BM + quarter * 32 + lane;
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)acc * TC_ACC_STRIDE;
-      epilogue_tile<FMT>(p, trow, g, n_tile, halfn, tile % p.k_splits, tile / p.k_splits);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(tempty_bar(acc), 0);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // no CTA leaves (or frees TMEM) while its peer may still touch it
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
+    fence_proxy_async();  // the next TMA writes land on bytes the tile occupied
+    consumer_sync();
+    if (threadIdx.x == 0) mbar_arrive(drained_bar);
   }
 }
 
@@ -1203,8 +987,8 @@ framed_tc2_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 //
 // Packed rows are ordered in 8-bin groups, [re bins 8g..8g+7 | negated im of the same bins], so
 // basis row r is accumulator column r and a K block that only the G longest groups reach needs
-// an MMA of width N = 16 G: TMA fetches 8 G rows per CTA of the pair, the instruction descriptor
-// carries N, the accumulation still lands in TMEM columns [0, N).  K blocks are visited in order
+// an MMA of width N = 16 G: TMA fetches 16 G basis rows, the wgmma instruction is the one of width N,
+// the accumulation still lands in accumulator columns [0, N).  K blocks are visited in order
 // of decreasing width, so the first MMA of a tile (accumulate = 0) initialises every column the
 // tile will touch, and the epilogue of a split-K chunk reads only those.
 // ===========================================================================
@@ -1257,9 +1041,8 @@ __device__ __forceinline__ void epilogue_tile_varn(const TcParams& p, uint32_t t
 #pragma unroll 1
   for (int gi = 0; gi < n_groups; ++gi) {
     uint32_t re[8], im[8];
-    tmem_ld8(trow + (uint32_t)(16 * gi), re);
-    tmem_ld8(trow + (uint32_t)(16 * gi + 8), im);
-    tmem_ld_wait();
+    acc_ld8(trow + (uint32_t)(16 * gi), re);
+    acc_ld8(trow + (uint32_t)(16 * gi + 8), im);
     if (valid) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -1281,156 +1064,108 @@ __device__ __forceinline__ void epilogue_tile_varn(const TcParams& p, uint32_t t
 }
 
 template <int FMT>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-framed_tc2v_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b8,
-                   const __grid_constant__ CUtensorMap tm_b32, const TcParams p,
-                   const __grid_constant__ VarNPlan plan) {
-  constexpr int BK = 64, STAGES = 3;
-  using S = Tc2Smem<BK, STAGES>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+__global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
+framed_tcv_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b8,
+                  const __grid_constant__ CUtensorMap tm_b32, const TcParams p,
+                  const __grid_constant__ VarNPlan plan) {
+  using S = TcSmem;
+  constexpr int BK = 64, STAGES = S::STAGES;
+  const uint32_t base = acc_tile_base();
   const uint32_t bar_base = base + S::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  const uint32_t drained_bar = bar_base + 8u * (2 * STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta = cluster_ctarank();
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a);
-    prefetch_tmap(&tm_b8);
-    prefetch_tmap(&tm_b32);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 2);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 8);
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 8);
-    }
+    mbar_init(drained_bar, 1);
     fence_barrier_init();
   }
-  cluster_sync_all();
-  if (warp == 2) {
-    tmem_alloc_2sm(tmem_slot, 512);
-    tmem_relinquish_2sm();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     if (elect_one()) {
+      prefetch_tmap(&tm_a);
+      prefetch_tmap(&tm_b8);
+      prefetch_tmap(&tm_b32);
       int stage = 0;
       uint32_t phase = 0;
-      for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, p.num_m_tiles, plan.n_chunks)) >= 0; ++u) {
+      for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, p.num_m_tiles, plan.n_chunks)) >= 0; ++u) {
+        if (u > 0) mbar_wait(drained_bar, (uint32_t)(u - 1) & 1u);
         const int chunk = tile % plan.n_chunks;
-        const int m_tile = tile / plan.n_chunks;
-        const int m0 = m_tile * (2 * TC_BM) + (int)cta * TC_BM;
+        const int m0 = (tile / plan.n_chunks) * TC_BM;
         for (int i = plan.chunk_begin[chunk]; i < plan.chunk_begin[chunk + 1]; ++i) {
           const int k0 = (int)plan.order[i] * BK;
-          const int rows = 8 * (int)plan.groups[i];  // basis rows this CTA stages
+          const int rows = 16 * (int)plan.groups[i];  // basis rows of the block's MMA width
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sb = base + stage * S::STAGE_BYTES;
-          mbar_expect_tx_remote(full_bar(stage), 0, 2 * S::A_BYTES + 2 * (uint32_t)rows * BK * 2);
+          mbar_expect_tx(full_bar(stage), 2 * S::A_BYTES + 2 * (uint32_t)rows * BK * 2);
           int c0 = k0, c1 = m0;
           if (p.rows_mode) {
             c1 = m0 + k0 / p.hop;
             c0 = k0 - (k0 / p.hop) * p.hop;
           }
-          tma_load_3d_2sm(sb, &tm_a, full_bar(stage), c0, c1, 0);
-          tma_load_3d_2sm(sb + S::A_BYTES, &tm_a, full_bar(stage), c0, c1, 1);
-          const int row0 = (int)cta * rows;
+          tma_load_3d(sb, &tm_a, full_bar(stage), c0, c1, 0);
+          tma_load_3d(sb + S::A_BYTES, &tm_a, full_bar(stage), c0, c1, 1);
           const uint32_t bh = sb + 2 * S::A_BYTES, bl = bh + S::B_BYTES;
           int r = 0;
           for (; rows - r >= 32; r += 32) {
-            tma_load_3d_2sm(bh + (uint32_t)r * BK * 2, &tm_b32, full_bar(stage), k0, row0 + r, 0);
-            tma_load_3d_2sm(bl + (uint32_t)r * BK * 2, &tm_b32, full_bar(stage), k0, row0 + r, 1);
+            tma_load_3d(bh + (uint32_t)r * BK * 2, &tm_b32, full_bar(stage), k0, r, 0);
+            tma_load_3d(bl + (uint32_t)r * BK * 2, &tm_b32, full_bar(stage), k0, r, 1);
           }
           for (; r < rows; r += 8) {
-            tma_load_3d_2sm(bh + (uint32_t)r * BK * 2, &tm_b8, full_bar(stage), k0, row0 + r, 0);
-            tma_load_3d_2sm(bl + (uint32_t)r * BK * 2, &tm_b8, full_bar(stage), k0, row0 + r, 1);
+            tma_load_3d(bh + (uint32_t)r * BK * 2, &tm_b8, full_bar(stage), k0, r, 0);
+            tma_load_3d(bl + (uint32_t)r * BK * 2, &tm_b8, full_bar(stage), k0, r, 1);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (cta == 0 && elect_one()) {
-      const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * TC_BM) >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, p.num_m_tiles, plan.n_chunks)) >= 0; ++u) {
-        const int chunk = tile % plan.n_chunks;
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * TC_ACC_STRIDE;
-        uint32_t accumulate = 0;
-        for (int i = plan.chunk_begin[chunk]; i < plan.chunk_begin[chunk + 1]; ++i) {
-          const uint32_t idesc = idesc0 | ((uint32_t)(2 * (int)plan.groups[i]) << 17);  // N = 16 G
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t koff = (uint32_t)k * 32u;
-            const uint64_t a_hi = make_smem_desc<BK>(sb + koff);
-            const uint64_t a_lo = make_smem_desc<BK>(sb + S::A_BYTES + koff);
-            const uint64_t b_hi = make_smem_desc<BK>(sb + 2 * S::A_BYTES + koff);
-            const uint64_t b_lo = make_smem_desc<BK>(sb + 2 * S::A_BYTES + S::B_BYTES + koff);
-            umma_bf16_2sm(d_tmem, a_lo, b_hi, idesc, accumulate);
-            umma_bf16_2sm(d_tmem, a_hi, b_lo, idesc, 1u);
-            umma_bf16_2sm(d_tmem, a_hi, b_hi, idesc, 1u);
-            accumulate = 1u;
-          }
-          umma_commit_2sm(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_2sm(tfull_bar(acc));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else if (warp >= 4) {
-    const int quarter = warp & 3;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int u = 0, tile; (tile = sched_tile(u, pair, num_pairs, p.num_m_tiles, plan.n_chunks)) >= 0; ++u) {
-      const int chunk = tile % plan.n_chunks;
-      const int m_tile = tile / plan.n_chunks;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const int64_t g = (int64_t)m_tile * (2 * TC_BM) + (int64_t)cta * TC_BM + quarter * 32 + lane;
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)acc * TC_ACC_STRIDE;
-      // widest block of the chunk = its first: the columns this tile initialised
-      epilogue_tile_varn<FMT>(p, trow, g, (int)plan.groups[plan.chunk_begin[chunk]], chunk, m_tile);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(tempty_bar(acc), 0);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
+  const int wg = warp >> 2;
+  const uint32_t a_off = (uint32_t)wg * 64u * (BK * 2);
+  const uint32_t tile_addr = acc_tile(p.bn);
+  float acc[128];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int u = 0, tile; (tile = sched_tile(u, blockIdx.x, gridDim.x, p.num_m_tiles, plan.n_chunks)) >= 0; ++u) {
+    const int chunk = tile % plan.n_chunks;
+    const int m_tile = tile / plan.n_chunks;
+    const int i0 = plan.chunk_begin[chunk];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int i = i0; i < plan.chunk_begin[chunk + 1]; ++i) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sb = base + stage * S::STAGE_BYTES;
+      wgmma_fence();
+      wg_kblock_split3<256>(16 * (int)plan.groups[i], acc, wg_desc_lo(sb + a_off),
+                            wg_desc_lo(sb + S::A_BYTES + a_off), wg_desc_lo(sb + 2 * S::A_BYTES),
+                            wg_desc_lo(sb + 2 * S::A_BYTES + S::B_BYTES), i != i0);
+      wgmma_commit();
+      wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(stage));
+      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    }
+    // widest block of the chunk = its first: the columns this unit initialised
+    const int n_groups = (int)plan.groups[i0];
+    consumer_sync();
+    acc_store<256>(tile_addr, acc, 16 * n_groups, wg * 64);
+    consumer_sync();
+    if (warp < 4) {
+      const int64_t g = (int64_t)m_tile * TC_BM + warp * 32 + lane;
+      epilogue_tile_varn<FMT>(p, tile_addr + acc_row((uint32_t)warp * 32u), g, n_groups, chunk, m_tile);
+    }
+    fence_proxy_async();
+    consumer_sync();
+    if (threadIdx.x == 0) mbar_arrive(drained_bar);
   }
 }
 
@@ -1530,88 +1265,38 @@ int encode_4d(CUtensorMap* map, void* base, const uint64_t dims[4], const uint64
   return NNAB_OK;
 }
 
-template <int BK, int STAGES, int FMT>
+template <int FMT>
 static int launch_tc_kernel_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
                                 int grid, cudaStream_t stream) {
-  using S = TcSmem<BK, STAGES>;
+  using S = TcSmem;
   // the attribute is per device: one process may drive several GPUs (torch.nn.DataParallel)
   static std::atomic<uint64_t> configured_devs{0};
   int cfg_dev = 0;
   NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
   const bool configured = (configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u;
   if (!configured) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tc_kernel<BK, STAGES, FMT>,
+    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tc_kernel<FMT>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  framed_tc_kernel<BK, STAGES, FMT><<<grid, TC_THREADS, S::TOTAL, stream>>>(ma, mb, prm);
+  framed_tc_kernel<FMT><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb, prm);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
-template <int BK, int STAGES, int FMT>
-static int launch_tc2_kernel_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
-                                 int n_pairs, cudaStream_t stream) {
-  using S = Tc2Smem<BK, STAGES>;
-  // the attribute is per device: one process may drive several GPUs (torch.nn.DataParallel)
-  static std::atomic<uint64_t> configured_devs{0};
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  const bool configured = (configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u;
-  if (!configured) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tc2_kernel<BK, STAGES, FMT>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = S::TOTAL;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NNAB_CUDA_TRY(cudaLaunchKernelEx(&cfg, framed_tc2_kernel<BK, STAGES, FMT>, ma, mb, prm));
-  count_launch();
-  return NNAB_OK;
-}
-
-template <int BK, int STAGES>
-static int launch_tc2_kernel(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
-                             int n_pairs, cudaStream_t stream) {
-  switch (prm.epi.fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tc2_kernel_fmt<BK, STAGES, 0>(ma, mb, prm, n_pairs, stream);
-    case NNAB_FMT_COMPLEX: return launch_tc2_kernel_fmt<BK, STAGES, 1>(ma, mb, prm, n_pairs, stream);
-    case NNAB_FMT_PHASE_ANGLE: return launch_tc2_kernel_fmt<BK, STAGES, 2>(ma, mb, prm, n_pairs, stream);
-    case NNAB_FMT_PHASE_UNIT: return launch_tc2_kernel_fmt<BK, STAGES, 3>(ma, mb, prm, n_pairs, stream);
-    case FMT_POWER: return launch_tc2_kernel_fmt<BK, STAGES, 4>(ma, mb, prm, n_pairs, stream);
-    case FMT_FBANK: return launch_tc2_kernel_fmt<BK, STAGES, 5>(ma, mb, prm, n_pairs, stream);
-    case FMT_DECIM: return launch_tc2_kernel_fmt<BK, STAGES, 6>(ma, mb, prm, n_pairs, stream);
-    case FMT_RAW: return launch_tc2_kernel_fmt<BK, STAGES, 7>(ma, mb, prm, n_pairs, stream);
-    case FMT_OLA: return launch_tc2_kernel_fmt<BK, STAGES, 8>(ma, mb, prm, n_pairs, stream);
-    case FMT_REALPAIR: return launch_tc2_kernel_fmt<BK, STAGES, 9>(ma, mb, prm, n_pairs, stream);
-    default: return NNAB_EINVAL;
-  }
-}
-
-template <int BK, int STAGES>
 static int launch_tc_kernel(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
                             int grid, cudaStream_t stream) {
   switch (prm.epi.fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tc_kernel_fmt<BK, STAGES, 0>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_COMPLEX: return launch_tc_kernel_fmt<BK, STAGES, 1>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_PHASE_ANGLE: return launch_tc_kernel_fmt<BK, STAGES, 2>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_PHASE_UNIT: return launch_tc_kernel_fmt<BK, STAGES, 3>(ma, mb, prm, grid, stream);
-    case FMT_POWER: return launch_tc_kernel_fmt<BK, STAGES, 4>(ma, mb, prm, grid, stream);
-    case FMT_FBANK: return launch_tc_kernel_fmt<BK, STAGES, 5>(ma, mb, prm, grid, stream);
-    case FMT_DECIM: return launch_tc_kernel_fmt<BK, STAGES, 6>(ma, mb, prm, grid, stream);
-    case FMT_RAW: return launch_tc_kernel_fmt<BK, STAGES, 7>(ma, mb, prm, grid, stream);
-    case FMT_OLA: return launch_tc_kernel_fmt<BK, STAGES, 8>(ma, mb, prm, grid, stream);
-    case FMT_REALPAIR: return launch_tc_kernel_fmt<BK, STAGES, 9>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_MAGNITUDE: return launch_tc_kernel_fmt<0>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_COMPLEX: return launch_tc_kernel_fmt<1>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_PHASE_ANGLE: return launch_tc_kernel_fmt<2>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_PHASE_UNIT: return launch_tc_kernel_fmt<3>(ma, mb, prm, grid, stream);
+    case FMT_POWER: return launch_tc_kernel_fmt<4>(ma, mb, prm, grid, stream);
+    case FMT_FBANK: return launch_tc_kernel_fmt<5>(ma, mb, prm, grid, stream);
+    case FMT_DECIM: return launch_tc_kernel_fmt<6>(ma, mb, prm, grid, stream);
+    case FMT_RAW: return launch_tc_kernel_fmt<7>(ma, mb, prm, grid, stream);
+    case FMT_OLA: return launch_tc_kernel_fmt<8>(ma, mb, prm, grid, stream);
+    case FMT_REALPAIR: return launch_tc_kernel_fmt<9>(ma, mb, prm, grid, stream);
     default: return NNAB_EINVAL;
   }
 }
@@ -1728,34 +1413,21 @@ static bool varn_problem_ok(const FramedProblem& q) {
 }
 
 template <int FMT>
-static int launch_tc2v_fmt(const CUtensorMap& ma, const CUtensorMap& mb8, const CUtensorMap& mb32,
-                           const TcParams& prm, const VarNPlan& plan, int n_pairs,
-                           cudaStream_t stream) {
-  using S = Tc2Smem<64, 3>;
+static int launch_tcv_fmt(const CUtensorMap& ma, const CUtensorMap& mb8, const CUtensorMap& mb32,
+                          const TcParams& prm, const VarNPlan& plan, int grid, cudaStream_t stream) {
+  using S = TcSmem;
   // the attribute is per device: one process may drive several GPUs (torch.nn.DataParallel)
   static std::atomic<uint64_t> configured_devs{0};
   int cfg_dev = 0;
   NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
   const bool configured = (configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u;
   if (!configured) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tc2v_kernel<FMT>,
+    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcv_kernel<FMT>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = S::TOTAL;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NNAB_CUDA_TRY(cudaLaunchKernelEx(&cfg, framed_tc2v_kernel<FMT>, ma, mb8, mb32, prm, plan));
-  count_launch();
+  framed_tcv_kernel<FMT><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb8, mb32, prm, plan);
+  NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
@@ -1796,11 +1468,11 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
     if ((rc = tc_varn_plan(q.h_k_begin, q.h_k_end, q.F, q.K, ks, &plan))) return rc;
   }
 
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   NNAB_CUDA_TRY(cudaGetDevice(&dev));
   NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   sms -= sm_reserve();
-  if (sms < 2) sms = 2;
+  if (sms < 1) sms = 1;
 
   CUtensorMap ma, mb8, mb32;
   const int rows_mode = (q.hop % 64 == 0) ? 1 : 0;
@@ -1847,19 +1519,19 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
     final_epi.raw = raw;
     final_epi.raw_plane = plane;
   }
-  prm.num_m_tiles = (int)ceil_div64(g.nv, 2 * TC_BM);
-  const int64_t ptiles = (int64_t)prm.num_m_tiles * plan.n_chunks;
-  const int n_pairs = (int)(ptiles < sms / 2 ? ptiles : sms / 2);
+  prm.num_m_tiles = (int)ceil_div64(g.nv, TC_BM);
+  const int64_t units = (int64_t)prm.num_m_tiles * plan.n_chunks;
+  const int grid = (int)(units < sms ? units : sms);
   {
     double cols = 0.0;
     for (int i = 0; i < plan.n_blocks; ++i) cols += 16.0 * plan.groups[i] * 64.0;
-    add_exec_flops(3.0 * 2.0 * (double)prm.num_m_tiles * (2 * TC_BM) * cols);
+    add_exec_flops(3.0 * 2.0 * (double)prm.num_m_tiles * TC_BM * cols);
   }
   switch (prm.epi.fmt) {
-    case NNAB_FMT_MAGNITUDE: rc = launch_tc2v_fmt<0>(ma, mb8, mb32, prm, plan, n_pairs, stream); break;
-    case NNAB_FMT_COMPLEX: rc = launch_tc2v_fmt<1>(ma, mb8, mb32, prm, plan, n_pairs, stream); break;
-    case NNAB_FMT_PHASE_UNIT: rc = launch_tc2v_fmt<3>(ma, mb8, mb32, prm, plan, n_pairs, stream); break;
-    case FMT_RAW: rc = launch_tc2v_fmt<7>(ma, mb8, mb32, prm, plan, n_pairs, stream); break;
+    case NNAB_FMT_MAGNITUDE: rc = launch_tcv_fmt<0>(ma, mb8, mb32, prm, plan, grid, stream); break;
+    case NNAB_FMT_COMPLEX: rc = launch_tcv_fmt<1>(ma, mb8, mb32, prm, plan, grid, stream); break;
+    case NNAB_FMT_PHASE_UNIT: rc = launch_tcv_fmt<3>(ma, mb8, mb32, prm, plan, grid, stream); break;
+    case FMT_RAW: rc = launch_tcv_fmt<7>(ma, mb8, mb32, prm, plan, grid, stream); break;
     default: rc = NNAB_EINVAL;
   }
   if (rc) return rc;
@@ -1887,8 +1559,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   }
   if (q.B > 65535) return NNAB_EUNSUPPORTED;
 
-  int bk = 64;
-  if (const char* e = getenv("NNAB_TC_BK")) bk = atoi(e) == 32 ? 32 : 64;
+  constexpr int bk = 64;
 
   const int n_ph = num_phases(q.hop);
   const int hop_eff = q.hop * n_ph;
@@ -1920,16 +1591,11 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   }
 
   // ---- tensor maps (shared by all phases) -------------------------------------------
-  // CTA pairs (cta_group::2) by default when there are enough 256-frame tiles to fill the
-  // 74 SM pairs; NNAB_TC_CTA=1|2 overrides (debugging / A-B measurements).
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   NNAB_CUDA_TRY(cudaGetDevice(&dev));
   NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   sms -= sm_reserve();  // SMs left to a concurrent collective (nnab_set_sm_reserve)
-  if (sms < 2) sms = 2;
-  int cta_group = (ceil_div64(g.nv, 2 * TC_BM) * n_tiles >= sms / 2) ? 2 : 1;
-  if (const char* e = getenv("NNAB_TC_CTA")) cta_group = atoi(e) == 2 ? 2 : 1;
-  if (cta_group == 2) bk = 64;
+  if (sms < 1) sms = 1;
   CUtensorMap ma, mb;
   const int rows_mode = (hop_eff % bk == 0) ? 1 : 0;
   int rc;
@@ -1943,8 +1609,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   }
   if (rc) return rc;
   rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, (uint64_t)rows_w, 2,
-                 (uint64_t)kpad * 2, (uint64_t)rows_w * kpad * 2, bk,
-                 cta_group == 2 ? bn / 2 : bn, bk);
+                 (uint64_t)kpad * 2, (uint64_t)rows_w * kpad * 2, bk, bn, bk);
   if (rc) return rc;
 
   // ---- parameters -------------------------------------------------------------------
@@ -1956,10 +1621,6 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   prm.nv = g.nv;
   prm.t_slots = g.t_slots;
   prm.t_mul = n_ph;
-  {
-    const char* e4 = getenv("NNAB_SPLIT4");
-    prm.split4 = (e4 != nullptr && atoi(e4) == 1) ? 1 : 0;  // CTA-pair kernel only
-  }
   const int nkb = kpad / bk;
   const int half = bn / 2;
   for (int tl = 0; tl < n_tiles; ++tl) {
@@ -2044,24 +1705,14 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
       NNAB_LAUNCH_CHECK();
     }
     {
-      const int mrows = (cta_group == 2 ? 2 : 1) * TC_BM;
       double kcols = 0.0;  // sum over N tiles of (k-blocks executed) x bk x bn
       for (int tl = 0; tl < n_tiles; ++tl) kcols += (double)(prm.kb_end[tl] - prm.kb_begin[tl]) * bk * bn;
-      add_exec_flops((prm.split4 && cta_group == 2 ? 4.0 : 3.0) * 2.0 *
-                     (double)ceil_div64(g.nv, mrows) * mrows * kcols);
+      add_exec_flops(3.0 * 2.0 * (double)ceil_div64(g.nv, TC_BM) * TC_BM * kcols);
     }
-    if (cta_group == 2) {
-      prm.num_m_tiles = (int)ceil_div64(g.nv, 2 * TC_BM);  // 256-frame pair tiles
-      const int64_t ptiles = (int64_t)prm.num_m_tiles * prm.num_n_tiles * prm.k_splits;
-      const int n_pairs = (int)(ptiles < sms / 2 ? ptiles : sms / 2);
-      rc = launch_tc2_kernel<64, 3>(ma, mb, prm, n_pairs, stream);
-    } else {
-      prm.num_m_tiles = (int)ceil_div64(g.nv, TC_BM);
-      const int64_t tiles = (int64_t)prm.num_m_tiles * prm.num_n_tiles * prm.k_splits;
-      const int grid = (int)(tiles < sms ? tiles : sms);
-      rc = (bk == 64) ? launch_tc_kernel<64, 2>(ma, mb, prm, grid, stream)
-                      : launch_tc_kernel<32, 4>(ma, mb, prm, grid, stream);
-    }
+    prm.num_m_tiles = (int)ceil_div64(g.nv, TC_BM);
+    const int64_t tiles = (int64_t)prm.num_m_tiles * prm.num_n_tiles * prm.k_splits;
+    const int grid = (int)(tiles < sms ? tiles : sms);
+    rc = launch_tc_kernel(ma, mb, prm, grid, stream);
     if (rc) return rc;
   }
   if (split) {

@@ -1,8 +1,8 @@
-// Hardware probe (test infrastructure, not on any product path): does a K-major SWIZZLE_128B UMMA
+// Hardware probe (test infrastructure, not on any product path): does a K-major SWIZZLE_128B wgmma
 // shared-memory descriptor address an operand that starts at an arbitrary ROW of a TMA-written
 // block (start address = block + r * 128 B), and what must the descriptor's base-offset field
-// (bits 49..51) hold for it?  The answer decides whether overlapping (Toeplitz) A tiles can be
-// read in place from one tall block instead of being re-fetched per K block.
+// (bits 49..51) hold for it?  The tall-A kernels (tct_kernels.cu) read overlapping (Toeplitz) A tiles
+// in place from one tall block and rely on the answer "any row, base offset 0".
 //   out[v][r][128][32] = A[r .. r+128) x B^T  for row offsets r = 0..15 and
 //   v = 0: base_offset = 0        v = 1: base_offset = r & 7
 #include <cuda.h>
@@ -19,63 +19,50 @@ constexpr int PROBE_ROWS = 144, PROBE_N = 32, PROBE_R = 16;
 __global__ void __launch_bounds__(128, 1)
 probe_rowoffset_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                        float* __restrict__ out) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t base = acc_tile_base();
   const uint32_t a_s = base;                           // 144 rows x 128 B = 18 KB
   const uint32_t b_s = base + 20 * 1024;               // 32 rows x 128 B
-  const uint32_t bar_full = base + 28 * 1024, bar_mma = bar_full + 8, tmem_slot = bar_full + 16;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(bar_full, 1);
-    mbar_init(bar_mma, 1);
+  const uint32_t bar = base + 28 * 1024;
+  const int t = threadIdx.x;
+  if (t == 0) {
+    mbar_init(bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 32);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(bar_full, PROBE_ROWS * 128 + PROBE_N * 128);
-    tma_load_3d(a_s, &tm_a, bar_full, 0, 0, 0);
-    tma_load_3d(b_s, &tm_b, bar_full, 0, 0, 0);
+  if (t == 0) {
+    mbar_expect_tx(bar, PROBE_ROWS * 128 + PROBE_N * 128);
+    tma_load_3d(a_s, &tm_a, bar, 0, 0, 0);
+    tma_load_3d(b_s, &tm_b, bar, 0, 0, 0);
   }
-  mbar_wait(bar_full, 0);
-  tcgen05_fence_after();
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(PROBE_N >> 3) << 17) |
-                         ((uint32_t)(128 >> 4) << 24);
-  uint32_t phase = 0;
+  mbar_wait(bar, 0);
+  const uint32_t row_in_half = (t >> 5) * 16 + ((t & 31) >> 2), col = (t & 3) * 2;
   for (int v = 0; v < 2; ++v) {
     for (int r = 0; r < PROBE_R; ++r) {
-      if (threadIdx.x == 0) {
-        for (int k = 0; k < 4; ++k) {
-          uint64_t da = make_smem_desc<64>(a_s + (uint32_t)r * 128u + (uint32_t)k * 32u);
-          if (v == 1) da |= (uint64_t)(r & 7) << 49;
-          const uint64_t db = make_smem_desc<64>(b_s + (uint32_t)k * 32u);
-          umma_bf16(tmem_base, da, db, idesc, k > 0 ? 1u : 0u);
-        }
-        umma_commit(bar_mma);
-      }
-      mbar_wait(bar_mma, phase);
-      phase ^= 1u;
-      tcgen05_fence_after();
-      uint32_t d[32];
-      tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16), d);
-      tmem_ld_wait();
-      float* o = out + (((size_t)v * PROBE_R + r) * 128 + warp * 32 + lane) * PROBE_N;
+      for (int h = 0; h < 2; ++h) {  // the two m64 halves of the 128 rows
+        float d[PROBE_N / 2];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(d[j]);
-      tcgen05_fence_before();
-      __syncthreads();
-      tcgen05_fence_after();
+        for (int i = 0; i < PROBE_N / 2; ++i) d[i] = 0.f;
+        const uint32_t hi = wg_desc_hi() | (v == 1 ? (uint32_t)(r & 7) << 17 : 0u);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = desc64(wg_desc_lo(a_s + (uint32_t)(r + 64 * h) * 128u + (uint32_t)k * 32u), hi);
+          const uint64_t db = desc64(wg_desc_lo(b_s + (uint32_t)k * 32u), wg_desc_hi());
+          Wgmma<PROBE_N>::mma(d, da, db, k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        float* o = out + (((size_t)v * PROBE_R + r) * 128 + 64 * h + row_in_half) * PROBE_N + col;
+#pragma unroll
+        for (int j = 0; j < PROBE_N / 8; ++j) {
+          o[8 * j] = d[4 * j];
+          o[8 * j + 1] = d[4 * j + 1];
+          o[8 * PROBE_N + 8 * j] = d[4 * j + 2];
+          o[8 * PROBE_N + 8 * j + 1] = d[4 * j + 3];
+        }
+      }
     }
   }
-  if (warp == 1) tmem_dealloc(tmem_base, 32);
 }
 
 // a: (144, 64) bf16, b: (32, 64) bf16, out: (2, 16, 128, 32) fp32 -- all device pointers
@@ -92,157 +79,10 @@ int tc_probe_rowoffset(const void* a, const void* b, float* out, cudaStream_t st
   return NNAB_OK;
 }
 
-
-// ---------------------------------------------------------------------------
-// MMA rate probe (measurement only): clock cycles per K block (4 K16 slices) of tcgen05.mma
-// kind::f16 (bf16, operands in shared memory, zeros) as a function of N and of the operand pattern,
-// CTA pair (M = 256) or single CTA (M = 128).  Every SM runs the same loop (a loaded chip).
-// `flags`:
-//   bit 0      the A / B descriptors advance through the 4 K16 slices (else: slice 0 every time)
-//   bit 1      A starts 3 rows into the block (a row offset that is not a multiple of the 8-row swizzle atom)
-//   bit 2      the A row offset changes from K block to K block (it & 31), as in the tall-A kernels
-//   bits 3..4  MMAs per K16 slice: 0 = a_hi*b_hi; 1 = a_lo*b_hi, a_hi*b_hi; 2 = a_lo*b_hi, a_hi*b_lo, a_hi*b_hi
-//   bit 5      B rotates through 2 stage buffers
-//   bit 6      two accumulators, alternating K block by K block
-//   bit 7      TWO issuing threads (warps 0 and 2), each its own accumulator and barrier, `iters` K blocks each
-//   bit 10     a tcgen05.commit (to a barrier nobody waits on) after every K block, as a ring-stage release does
-//   bits 8..9  order of the MMAs of a K block: 0 = as bits 3..4 say; 1 = the same count per slice, all with
-//              a_hi (b alternating); 2 = term-major (4 slices of a_hi*b_hi, then of a_lo*b_hi, then a_hi*b_lo)
-// out[pair or CTA] = cycles from the first issue to the completion of the last MMA.
-// ---------------------------------------------------------------------------
-template <int CG>
-__global__ void __launch_bounds__(128, 1) probe_mma_rate_kernel(int n, int flags, int iters,
-                                                                 unsigned long long* __restrict__ out) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  constexpr uint32_t A_PLANE = 24 * 1024, B_PLANE = 32 * 1024, B_STAGE = 2 * B_PLANE;
-  const uint32_t a_s = base;                    // 2 planes x 192 rows x 128 B = 48 KB
-  const uint32_t b_s = base + 2 * A_PLANE;      // 2 stages x 2 planes x 256 rows x 128 B = 128 KB
-  constexpr uint32_t DATA = 2 * A_PLANE + 2 * B_STAGE;
-  const uint32_t bar = base + DATA, tmem_slot = bar + 48;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-  const int warp = threadIdx.x >> 5;
-  for (uint32_t i = threadIdx.x; i < DATA / 16; i += blockDim.x)
-    reinterpret_cast<uint4*>(smem_raw + (base - smem_u32(smem_raw)))[i] = make_uint4(0, 0, 0, 0);
-  fence_proxy_async();
-  if (threadIdx.x == 0) {
-    mbar_init(bar, 1);
-    mbar_init(bar + 8, 1);
-    mbar_init(bar + 24, 0xFFFFF);  // absorbs the per-block commits of flag bit 10
-    mbar_init(bar + 32, 0xFFFFF);
-    fence_barrier_init();
-  }
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) {
-    if (CG == 2) { tmem_alloc_2sm(tmem_slot, 512); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  const bool leader = CG == 1 || cluster_ctarank() == 0;
-  long long t0 = 0, t1 = 0;
-  const bool two = (flags & 128) != 0;
-  const int issuer = threadIdx.x == 0 ? 0 : (threadIdx.x == 64 && two ? 1 : -1);
-  __syncthreads();
-  if (issuer >= 0 && leader) {
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) |
-                           ((uint32_t)((CG == 2 ? 256 : 128) >> 4) << 24);
-    const uint32_t dhi = smem_desc_hi<64>();
-    const int terms = (flags >> 3) & 3, order = (flags >> 8) & 3;
-    const uint32_t kstep = (flags & 1) ? 2u : 0u;
-    auto mma = [&](uint32_t d, uint64_t a, uint64_t b) {
-      if (CG == 2) umma_bf16_2sm_i<true>(d, a, b, idesc);
-      else umma_bf16(d, a, b, idesc, 1u);
-    };
-    t0 = clock64();
-    for (int it = 0; it < iters; ++it) {
-      uint32_t a_row = (flags & 2) ? 3u * 128u : 0u;
-      if (flags & 4) a_row = (uint32_t)(it & 31) * 128u;
-      const uint32_t bst = (flags & 32) ? (uint32_t)(it & 1) * B_STAGE : 0u;
-      const uint32_t d = tmem_base + (two ? (uint32_t)issuer * 256u : ((flags & 64) ? (uint32_t)(it & 1) * 256u : 0u));
-      const uint32_t ah = smem_desc_lo<64>(a_s + a_row), al = smem_desc_lo<64>(a_s + A_PLANE + a_row);
-      const uint32_t bh = smem_desc_lo<64>(b_s + bst), bl = smem_desc_lo<64>(b_s + bst + B_PLANE);
-      if (order == 2) {
-        for (int t = 0; t <= terms; ++t) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            mma(d, desc64((t == 1 ? al : ah) + kstep * k, dhi), desc64((t == 2 ? bl : bh) + kstep * k, dhi));
-        }
-      } else {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint64_t a_hi = desc64(ah + kstep * k, dhi), a_lo = order == 1 ? a_hi : desc64(al + kstep * k, dhi);
-          const uint64_t b_hi = desc64(bh + kstep * k, dhi), b_lo = desc64(bl + kstep * k, dhi);
-          if (terms >= 1) mma(d, a_lo, b_hi);
-          if (terms >= 2) mma(d, a_hi, b_lo);
-          mma(d, a_hi, b_hi);
-        }
-      }
-      if (flags & 1024) {
-        if (CG == 2) umma_commit_2sm(bar + 24u + 8u * issuer); else umma_commit(bar + 24u + 8u * issuer);
-      }
-    }
-    if (CG == 2) umma_commit_2sm(bar + 8u * issuer); else umma_commit(bar + 8u * issuer);
-  }
-  if (issuer >= 0) {
-    mbar_wait(bar + 8u * issuer, 0);
-    t1 = clock64();
-    if (leader) out[(CG == 2 ? blockIdx.x / 2 : blockIdx.x) + issuer * (int)(gridDim.x / CG)] = (unsigned long long)(t1 - t0);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (CG == 2) cluster_sync_all();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if (CG == 2) tmem_dealloc_2sm(tmem_base, 512); else tmem_dealloc(tmem_base, 512);
-  }
-}
-
-template <int CG>
-static int launch_probe_mma_rate(int n, int flags, int iters, unsigned long long* out, int ctas,
-                                 cudaStream_t stream) {
-  const int smem = (48 + 128 + 2) * 1024;
-  NNAB_CUDA_TRY(cudaFuncSetAttribute(probe_mma_rate_kernel<CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)ctas);
-  cfg.blockDim = dim3(128);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NNAB_CUDA_TRY(cudaLaunchKernelEx(&cfg, probe_mma_rate_kernel<CG>, n, flags, iters, out));
-  return NNAB_OK;
-}
-
-int tc_probe_mma_rate(int cta_group, int n, int flags, int iters, unsigned long long* out, int ctas,
-                      cudaStream_t stream) {
-  if (n < 16 || n > 256 || n % 16 != 0 || flags < 0 || flags > 2047 || ((flags >> 8) & 3) == 3 || ((flags >> 3) & 3) == 3 || iters < 1 ||
-      ctas < cta_group || ctas % cta_group != 0)
-    return NNAB_EINVAL;
-  if (cta_group == 2) return launch_probe_mma_rate<2>(n, flags, iters, out, ctas, stream);
-  if (cta_group == 1) return launch_probe_mma_rate<1>(n, flags, iters, out, ctas, stream);
-  return NNAB_EINVAL;
-}
-
 }  // namespace nnab
 
 extern "C" __attribute__((visibility("default"))) int nnab_probe_rowoffset(const void* a, const void* b,
                                                                          float* out, void* stream) {
   if (a == nullptr || b == nullptr || out == nullptr) return NNAB_EINVAL;
   return nnab::tc_probe_rowoffset(a, b, out, (cudaStream_t)stream);
-}
-
-extern "C" __attribute__((visibility("default"))) int nnab_probe_mma_rate(int cta_group, int n, int flags,
-                                                                        int iters, unsigned long long* out,
-                                                                        int ctas, void* stream) {
-  if (out == nullptr) return NNAB_EINVAL;
-  return nnab::tc_probe_mma_rate(cta_group, n, flags, iters, out, ctas, (cudaStream_t)stream);
 }

@@ -1,4 +1,4 @@
-// Block-partial ("sliding") STFT on tcgen05 for sm_100a — the default kernel of the STFT family
+// Block-partial ("sliding") STFT on wgmma for sm_90a — the default kernel of the STFT family
 // (STFT / MelSpectrogram / MFCC / Gammatonegram with a periodic Hann window and hop = n_fft / R,
 // R = 2 or 4: the reference's defaults, stft.py:177-178).
 //
@@ -19,13 +19,13 @@
 // as a (rows x hop) matrix), K = hop, N = 2 * (F + 2) columns (re | im of bins -1 .. F: the two
 // extra bins are the k-1 / k+1 neighbours of the edge bins).
 //
-// Tiling (CTA pairs, cta_group::2, same pipeline roles as framed_tc2_kernel):
-//   * N tile = nb packed bins (re half staged by CTA 0, im half by CTA 1); consecutive tiles
-//     overlap by 2 bins, a tile emits nb - 2 output bins.
-//   * M: each epilogue warp owns one 32-lane TMEM quarter = 32 consecutive block rows and emits
-//     33 - R frames; the 4 quarters of a CTA are loaded as four 32-row TMA boxes whose row origins
-//     are 33 - R apart, so no frame needs a row of another warp (no smem exchange, no barrier).
-//     4 * (33 - R) frames per CTA tile (116 of 128 rows for R = 4).
+// Tiling (same pipeline roles as framed_tc_kernel, tc_ptx.cuh):
+//   * N tile = nb packed bins, re rows then im rows (MMA N = 2 nb); consecutive tiles overlap by
+//     2 bins, a tile emits nb - 2 output bins.
+//   * M: each epilogue warp owns one 32-row quarter of the accumulator tile = 32 consecutive block
+//     rows and emits 33 - R frames; the 4 quarters of a tile are loaded as four 32-row TMA boxes whose
+//     row origins are 33 - R apart, so no frame needs a row of another warp (no exchange, no barrier).
+//     4 * (33 - R) frames per tile (116 of 128 rows for R = 4).
 //   * fp32 parity: x*w = xhi*whi + xlo*whi + xhi*wlo on bf16 tensor cores, fp32 accumulation.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -42,11 +42,10 @@
 namespace nnab {
 
 constexpr int TCB_BK = 64;
-constexpr int TCB_STAGES = 3;
-constexpr int TCB_ACC_STRIDE = 256;
+constexpr int TCB_STAGES = 2;
 
 struct TcbParams {
-  int num_m_pairs;   // pair tiles along M
+  int num_m_tiles;   // 128-row tiles along M (4 * (33 - R) frames each)
   int num_n_tiles;
   int nb;            // packed bins per N tile (MMA N = 2 nb)
   int kb_n;          // hop / 64
@@ -56,10 +55,12 @@ struct TcbParams {
 
 struct TcbSmem {
   static constexpr uint32_t A_BYTES = TC_BM * TCB_BK * 2;   // one plane, 128 rows
-  static constexpr uint32_t B_BYTES = 128 * TCB_BK * 2;     // one plane, <= 128 rows (this CTA's half)
+  static constexpr uint32_t B_BYTES = 256 * TCB_BK * 2;     // one plane, re + im rows (2 nb <= 256)
   static constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr uint32_t BAR_OFFSET = TCB_STAGES * STAGE_BYTES;
   static constexpr uint32_t TOTAL = BAR_OFFSET + 256 + 1024;
+  // the accumulator tile (128 rows x 2 nb fp32) reuses the stages once a tile's K range is drained
+  static_assert(TC_BM * 256 * 4 <= BAR_OFFSET, "accumulator tile does not fit the stage ring");
 };
 
 // rows of one (plane, part) slab of the packed block basis
@@ -149,10 +150,10 @@ int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
 }
 
 // ---------------------------------------------------------------------------
-// epilogue: one warp = one TMEM lane quarter (32 consecutive block rows) x a range of 8-column chunks.
-// The body of a chunk is straight-line code (no branches between the TMEM load and the stores), so
-// the 8 bins' dependency chains (3-tap filter -> shuffles -> twiddles -> magnitude) interleave: with
-// one or two warps per scheduler the epilogue is latency-bound, not issue-bound.
+// epilogue: one warp = one 32-row quarter of the accumulator tile (32 consecutive block rows) x a range
+// of 8-column chunks.  The body of a chunk is straight-line code (no branches between the load and the
+// stores), so the 8 bins' dependency chains (3-tap filter -> shuffles -> twiddles -> magnitude)
+// interleave: with one or two warps per scheduler the epilogue is latency-bound, not issue-bound.
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ float sqrt_approx(float x) {
   float r;
@@ -209,16 +210,15 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
   wr[8] = wr[9] = wi[8] = wi[9] = 0.f;
   if (c_begin > 0) {  // a column range that starts inside the tile: seed the two carried columns
     uint32_t re[8], im[8];
-    tmem_ld8(trow + (uint32_t)(8 * (c_begin - 1)), re);
-    tmem_ld8(trow + (uint32_t)(nb + 8 * (c_begin - 1)), im);
-    tmem_ld_wait();
+    acc_ld8(trow + (uint32_t)(8 * (c_begin - 1)), re);
+    acc_ld8(trow + (uint32_t)(nb + 8 * (c_begin - 1)), im);
     wr[8] = __uint_as_float(re[6]); wr[9] = __uint_as_float(re[7]);
     wi[8] = __uint_as_float(im[6]); wi[9] = __uint_as_float(im[7]);
   }
 #pragma unroll 1
   for (int c = c_begin; c < c_end; ++c) {
     wr[0] = wr[8]; wr[1] = wr[9]; wi[0] = wi[8]; wi[1] = wi[9];
-    int4 st[8];  // FMT 5: this chunk's filterbank actions, requested before the TMEM round trip
+    int4 st[8];  // FMT 5: this chunk's filterbank actions, requested before the accumulator loads
     if constexpr (FMT == 5) {
       if (fast_fb) {
         const int kq = k_tile0 + 8 * c - 2;
@@ -229,9 +229,8 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
     }
     {
       uint32_t re[8], im[8];
-      tmem_ld8(trow + (uint32_t)(8 * c), re);
-      tmem_ld8(trow + (uint32_t)(nb + 8 * c), im);
-      tmem_ld_wait();
+      acc_ld8(trow + (uint32_t)(8 * c), re);
+      acc_ld8(trow + (uint32_t)(nb + 8 * c), im);
 #pragma unroll
       for (int e = 0; e < 8; ++e) { wr[e + 2] = __uint_as_float(re[e]); wi[e + 2] = __uint_as_float(im[e]); }
     }
@@ -367,164 +366,116 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
   if constexpr (FMT == 5) run.flush(p.epi, mel, valid);
 }
 
-// epilogue warps: 2 per TMEM lane quarter (column halves); 3 for the fused filterbank, whose longer
-// per-bin chain needs the extra warp per scheduler to stay under the MMA time of a tile
-template <int FMT> struct TcbCfg {
-  static constexpr int PARTS = (FMT == 5) ? FB_EPI_PARTS : 2;
-  static constexpr int EPI_WARPS = 4 * PARTS;
-  static constexpr int THREADS = 128 + 32 * EPI_WARPS;  // warps 0-3: TMA, MMA, TMEM alloc, idle
-};
+// Epilogue warps: all 8 consumer warps, 2 per 32-row quarter of the tile (column halves).  For the fused
+// filterbank the two halves are also FB_EPI_PARTS, the range cuts fb_steps was built for.
+constexpr int TCB_PARTS = 2;
+static_assert(FB_EPI_PARTS == TCB_PARTS, "fused-filterbank column ranges follow the epilogue warps");
 
 template <int FMT, int R>
-__global__ void __launch_bounds__(TcbCfg<FMT>::THREADS, 1)
+__global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
 framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const TcbParams p) {
   constexpr int BK = TCB_BK, STAGES = TCB_STAGES;
   constexpr int FW = 33 - R;  // frames per warp quarter
   using S = TcbSmem;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t base = acc_tile_base();
   const uint32_t bar_base = base + S::BAR_OFFSET;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };            // used in the leader
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };  // per CTA
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };       // per CTA
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };  // leader
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const uint32_t drained_bar = bar_base + 8u * (2 * STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t cta = cluster_ctarank();  // 0 = leader
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a);
-    prefetch_tmap(&tm_b);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 2);   // one arrive.expect_tx per CTA's producer
-      mbar_init(empty_bar(s), 1);  // multicast commit from the leader
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 2 * TcbCfg<FMT>::EPI_WARPS);  // epilogue warps x 2 CTAs
-    }
+    mbar_init(drained_bar, 1);
     fence_barrier_init();
   }
-  cluster_sync_all();
-  if (warp == 2) {
-    tmem_alloc_2sm(tmem_slot, 512);
-    tmem_relinquish_2sm();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  const int num_tiles = p.num_m_pairs * p.num_n_tiles;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
   const int nb = p.nb;
-  const uint32_t b_bytes = (uint32_t)nb * BK * 2;
 
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
+  if (warp == TC_PRODUCER_WARP) {
+    // ===================== TMA producer =====================
     if (elect_one()) {
+      prefetch_tmap(&tm_a);
+      prefetch_tmap(&tm_b);
+      const uint32_t part_bytes = (uint32_t)nb * BK * 2;  // nb basis rows of one (plane, part)
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int m_pair = tile / p.num_n_tiles;
-        const int n_tile = tile - m_pair * p.num_n_tiles;
-        const int m0 = (2 * m_pair + (int)cta) * (4 * FW);
+      int u = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++u) {
+        if (u > 0) mbar_wait(drained_bar, (uint32_t)(u - 1) & 1u);
+        const int m_tile = tile / p.num_n_tiles;
+        const int n_tile = tile - m_tile * p.num_n_tiles;
+        const int m0 = m_tile * (4 * FW);
         const int n0 = n_tile * (nb - 2);
         for (int kb = 0; kb < p.kb_n; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sb = base + stage * S::STAGE_BYTES;
-          mbar_expect_tx_remote(full_bar(stage), 0, 2 * S::A_BYTES + 2 * b_bytes);
+          mbar_expect_tx(full_bar(stage), 2 * S::A_BYTES + 4 * part_bytes);
           const int k0 = kb * BK;
 #pragma unroll
           for (int q = 0; q < 4; ++q) {  // 32-row boxes, row origins FW apart
-            tma_load_3d_2sm(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0,
-                            m0 + q * FW, 0);
-            tma_load_3d_2sm(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0,
-                            m0 + q * FW, 1);
+            tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0, m0 + q * FW, 0);
+            tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0,
+                        m0 + q * FW, 1);
           }
-          tma_load_3d_2sm(sb + 2 * S::A_BYTES, &tm_b, full_bar(stage), k0, n0, (int)cta);
-          tma_load_3d_2sm(sb + 2 * S::A_BYTES + S::B_BYTES, &tm_b, full_bar(stage), k0, n0,
-                          2 + (int)cta);
+          // B rows [0, nb) = re part, [nb, 2 nb) = im part: accumulator columns of the N = 2 nb MMA
+          const uint32_t bh = sb + 2 * S::A_BYTES, bl = bh + S::B_BYTES;
+          tma_load_3d(bh, &tm_b, full_bar(stage), k0, n0, 0);
+          tma_load_3d(bh + part_bytes, &tm_b, full_bar(stage), k0, n0, 1);
+          tma_load_3d(bl, &tm_b, full_bar(stage), k0, n0, 2);
+          tma_load_3d(bl + part_bytes, &tm_b, full_bar(stage), k0, n0, 3);
           if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (cta == 0 && elect_one()) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * nb) >> 3) << 17) |
-                             ((uint32_t)((2 * TC_BM) >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * TCB_ACC_STRIDE;
-        uint32_t accumulate = 0;
-        for (int kb = 0; kb < p.kb_n; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tcgen05_fence_after();
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t koff = (uint32_t)k * 32u;
-            const uint64_t a_hi = make_smem_desc<BK>(sb + koff);
-            const uint64_t a_lo = make_smem_desc<BK>(sb + S::A_BYTES + koff);
-            const uint64_t b_hi = make_smem_desc<BK>(sb + 2 * S::A_BYTES + koff);
-            const uint64_t b_lo = make_smem_desc<BK>(sb + 2 * S::A_BYTES + S::B_BYTES + koff);
-            umma_bf16_2sm(d_tmem, a_lo, b_hi, idesc, accumulate);
-            umma_bf16_2sm(d_tmem, a_hi, b_lo, idesc, 1u);
-            umma_bf16_2sm(d_tmem, a_hi, b_hi, idesc, 1u);
-            accumulate = 1u;
-          }
-          umma_commit_2sm(empty_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_2sm(tfull_bar(acc));
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue (both CTAs, own rows) =====================
-    const int quarter = warp & 3;             // TMEM lanes 32 * (warp % 4) .. + 31
-    constexpr int PARTS = TcbCfg<FMT>::PARTS;  // warps per quarter, each a contiguous chunk range
-    const int part = (warp - 4) >> 2;
-    const int n_chunks = nb / 8;
-    const int c_begin = (n_chunks * part) / PARTS, c_end = (n_chunks * (part + 1)) / PARTS;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int m_pair = tile / p.num_n_tiles;
-      const int n_tile = tile - m_pair * p.num_n_tiles;
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tcgen05_fence_after();
-      const int64_t g = (int64_t)(2 * m_pair + (int)cta) * (4 * FW) + quarter * FW + lane;
-      const uint32_t trow = tmem_base + ((uint32_t)(quarter * 32) << 16) +
-                            (uint32_t)acc * TCB_ACC_STRIDE;
-      epilogue_tile_block<FMT, R>(p, trow, g, lane, n_tile, c_begin, c_end);
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(tempty_bar(acc), 0);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512);
+  // ===================== consumers: wgmma, then the epilogue =====================
+  const int wg = warp >> 2;
+  const uint32_t a_off = (uint32_t)wg * 64u * (BK * 2);
+  const uint32_t tile_addr = acc_tile(2 * nb);
+  const int quarter = warp & 3;  // tile rows 32 quarter .. + 31
+  const int part = warp >> 2;    // column half of the tile
+  const int n_chunks = nb / 8;
+  const int c_begin = (n_chunks * part) / TCB_PARTS, c_end = (n_chunks * (part + 1)) / TCB_PARTS;
+  float acc[128];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m_tile = tile / p.num_n_tiles;
+    const int n_tile = tile - m_tile * p.num_n_tiles;
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < p.kb_n; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sb = base + stage * S::STAGE_BYTES;
+      wgmma_fence();
+      wg_kblock_split3<256>(2 * nb, acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
+                            wg_desc_lo(sb + 2 * S::A_BYTES), wg_desc_lo(sb + 2 * S::A_BYTES + S::B_BYTES),
+                            kb != 0);
+      wgmma_commit();
+      wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(stage));
+      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    }
+    consumer_sync();
+    acc_store<256>(tile_addr, acc, 2 * nb, wg * 64);
+    consumer_sync();
+    const int64_t g = (int64_t)m_tile * (4 * FW) + quarter * FW + lane;
+    epilogue_tile_block<FMT, R>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, n_tile, c_begin,
+                                c_end);
+    fence_proxy_async();
+    consumer_sync();
+    if (threadIdx.x == 0) mbar_arrive(drained_bar);
   }
 }
 
@@ -532,8 +483,8 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 // host side
 // ---------------------------------------------------------------------------
 template <int FMT, int R>
-static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm,
-                          int n_pairs, cudaStream_t stream) {
+static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
+                          cudaStream_t stream) {
   using S = TcbSmem;
   static std::atomic<uint64_t> configured_devs{0};  // the attribute is per device
   int cfg_dev = 0;
@@ -543,33 +494,21 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(2 * n_pairs));
-  cfg.blockDim = dim3(TcbCfg<FMT>::THREADS);
-  cfg.dynamicSmemBytes = S::TOTAL;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  NNAB_CUDA_TRY(cudaLaunchKernelEx(&cfg, framed_tcb_kernel<FMT, R>, ma, mb, prm));
-  count_launch();
+  framed_tcb_kernel<FMT, R><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb, prm);
+  NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
 template <int R>
-static int launch_tcb(int fmt, const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm,
-                      int n_pairs, cudaStream_t stream) {
+static int launch_tcb(int fmt, const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
+                      cudaStream_t stream) {
   switch (fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R>(ma, mb, prm, n_pairs, stream);
-    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R>(ma, mb, prm, n_pairs, stream);
-    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R>(ma, mb, prm, n_pairs, stream);
-    case FMT_POWER: return launch_tcb_fmt<4, R>(ma, mb, prm, n_pairs, stream);
-    case FMT_FBANK: return launch_tcb_fmt<5, R>(ma, mb, prm, n_pairs, stream);
-    case FMT_PLANES: return launch_tcb_fmt<9, R>(ma, mb, prm, n_pairs, stream);
+    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R>(ma, mb, prm, grid, stream);
+    case FMT_POWER: return launch_tcb_fmt<4, R>(ma, mb, prm, grid, stream);
+    case FMT_FBANK: return launch_tcb_fmt<5, R>(ma, mb, prm, grid, stream);
+    case FMT_PLANES: return launch_tcb_fmt<9, R>(ma, mb, prm, grid, stream);
     default: return NNAB_EINVAL;
   }
 }
@@ -612,11 +551,11 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   int rc = tc_pad_split(q.x, q.B, q.L, q.x_pitch, q.K, q.hop, q.pad, q.pad_mode, planes, stream);
   if (rc) return rc;
 
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   NNAB_CUDA_TRY(cudaGetDevice(&dev));
   NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   sms -= sm_reserve();
-  if (sms < 2) sms = 2;
+  if (sms < 1) sms = 1;
 
   int nb = block_choose_nb(q.F);
   if (q.fmt == FMT_FBANK && q.fb_steps != nullptr && q.fb_nb_mask != 0) {
@@ -643,9 +582,8 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   if (rc) return rc;
 
   TcbParams prm{};
-  const int frames_per_cta = 4 * (33 - R);
-  const int64_t cta_tiles = ceil_div64(g.nv, frames_per_cta);
-  prm.num_m_pairs = (int)((cta_tiles + 1) / 2);
+  const int frames_per_tile = 4 * (33 - R);
+  prm.num_m_tiles = (int)ceil_div64(g.nv, frames_per_tile);
   prm.num_n_tiles = n_tiles;
   prm.nb = nb;
   prm.kb_n = q.hop / 64;
@@ -660,11 +598,11 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.epi.ola_pitch = 0; prm.epi.ola_hop = 0;
   prm.epi.planes_stride = q.planes_stride; prm.epi.planes_pitch = q.planes_pitch;
   if (q.fmt == FMT_PLANES && (int64_t)n_tiles * nb > q.planes_pitch) return NNAB_EINVAL;
-  const int64_t ptiles = (int64_t)prm.num_m_pairs * n_tiles;
-  const int n_pairs = (int)(ptiles < sms / 2 ? ptiles : sms / 2);
-  add_exec_flops(3.0 * 2.0 * (double)ptiles * (2 * TC_BM) * (2 * nb) * q.hop);
-  return R == 4 ? launch_tcb<4>(q.fmt, ma, mb, prm, n_pairs, stream)
-                : launch_tcb<2>(q.fmt, ma, mb, prm, n_pairs, stream);
+  const int64_t tiles = (int64_t)prm.num_m_tiles * n_tiles;
+  const int grid = (int)(tiles < sms ? tiles : sms);
+  add_exec_flops(3.0 * 2.0 * (double)tiles * TC_BM * (2 * nb) * q.hop);
+  return R == 4 ? launch_tcb<4>(q.fmt, ma, mb, prm, grid, stream)
+                : launch_tcb<2>(q.fmt, ma, mb, prm, grid, stream);
 }
 
 }  // namespace nnab

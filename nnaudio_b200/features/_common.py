@@ -198,7 +198,7 @@ def tap_support(bank_2d: np.ndarray):
 
 
 class FilterbankTable:
-    """Cache of the banded-filterbank table used by the fused tcgen05 epilogue
+    """Cache of the banded-filterbank table used by the fused tensor-core epilogue
     (rebuilt when the filterbank tensor changes; ``None`` for dense banks)."""
 
     def __init__(self):

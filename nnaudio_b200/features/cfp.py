@@ -6,7 +6,7 @@ Blackman-Harris window of ``window_size`` samples (``torch.stft``), magnitude / 
 non-linearity, then alternately ``Re FFT_N(.) / sqrt(N)`` + cut-off + power (generalised cepstrum ->
 generalised spectrum -> ...), and finally two triangular log-frequency maps whose product is ``Z``.
 
-B200 formulation — no FFT, three dense contractions on the tcgen05 framed kernel:
+Formulation here — no FFT, three dense contractions on the tensor-core framed kernel:
 
 * **STFT stage.**  Only ``window_size`` of the ``N`` window samples are non-zero, so the frame is a
   framed contraction with ``K ~ window_size`` taps (not ``N``) against the one-sided windowed DFT rows

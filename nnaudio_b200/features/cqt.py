@@ -469,7 +469,7 @@ class _DecimateFn(torch.autograd.Function):
         use_tc = packed is not None and os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "tc"
         c = _C.cqt1992v2_forward(gp.contiguous(), poly, poly_zero, packed if use_tc else None, None,
                                  None, 1, False, _C.PAD_CONSTANT, None, 1.0, _C.FMT_COMPLEX, 0.0,
-                                 path="tcgen05" if use_tc else "simt")
+                                 path="tc" if use_tc else "simt")
         d_padded = c[..., 0].permute(0, 2, 1).reshape(g.shape[0], M * n)   # [n*m + p] = phase p, m
         return d_padded[:, half:half + L].contiguous(), None, None, None, None
 
@@ -490,14 +490,13 @@ class _FirDecimateFn(torch.autograd.Function):
 def _decimate_autograd(mod, tag, sig, fir, n):
     """Differentiable ``downsampling_by_n`` / ``_by_2`` stage of the training path.
 
-    ``NNAUDIO_B200_DECIM_BWD`` picks the adjoint (CQT2010v2 32 x 30 s forward + backward, worst dX error
-    of the pyramid cases vs the reference's autograd):
-    ``fir`` (default since round 2) the dedicated CUDA-core FIR stage + adjoint kernel
+    ``NNAUDIO_B200_DECIM_BWD`` picks the adjoint:
+    ``fir`` (default) the dedicated CUDA-core FIR stage + adjoint kernel
     (``nnab_fir_decimate`` / ``nnab_fir_decimate_adjoint``: every input sample written once, no
-    atomics) -- 2.96 ms, within the 1e-4 bar on every pyramid gradient case;
-    ``simt`` polyphase FIRs on the framed CUDA-core kernel -- 42.0 ms, 6.1e-5; ``tc`` the same on the
-    tensor-core kernel (8 frame phases) -- 30.1 ms, 6.1e-5; ``ola`` a K=1 adjoint GEMM + overlap-add
-    atomics (256 atomics per input sample) -- 24.4 ms but 1.04e-4 on the Magnitude case, over the bar."""
+    atomics), within the 1e-4 bar on every pyramid gradient case;
+    ``simt`` polyphase FIRs on the framed CUDA-core kernel; ``tc`` the same on the tensor-core kernel
+    (8 frame phases); ``ola`` a K=1 adjoint GEMM + overlap-add atomics (256 atomics per input sample),
+    whose worst dX error on the Magnitude case is just over the bar."""
     if os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "fir":
         return _FirDecimateFn.apply(sig, fir.detach().reshape(-1).contiguous(), int(n))
     if os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "ola":

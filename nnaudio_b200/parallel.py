@@ -41,7 +41,7 @@ class BatchShardedTransform:
                  group: Optional[dist.ProcessGroup] = None, gather: bool = True,
                  reserve_sms: int = 8):
         """``reserve_sms``: SMs kept out of the persistent tensor-core grids while a
-        gather may be in flight — the kernels otherwise occupy all 148 SMs and NCCL's
+        gather may be in flight — the kernels otherwise occupy every SM and NCCL's
         CTAs could only start at their tail (no overlap)."""
         self.transform = transform
         self.group = group
@@ -102,7 +102,7 @@ class BatchShardedTransform:
     # after its transform a rank pushes its shard into the same slice of every peer's buffer
     # (``gather_to='all'``) or of the root's only (``gather_to='root'``: what the north star names;
     # 1/world of the fabric bytes) with plain device-to-device copies over NVLink -- copy engines,
-    # so the persistent kernels keep all 148 SMs and nothing is reserved for a collective.  Two
+    # so the persistent kernels keep every SM and nothing is reserved for a collective.  Two
     # device-side barriers per step order the slot reuse (every rank has consumed the slot) and the
     # arrival of the pushes.
     def _symm_setup(self, y: torch.Tensor):
@@ -186,9 +186,8 @@ class BatchShardedTransform:
     # its slice of a symmetric-memory buffer (``_C.output_into``), copy engines push the slice over
     # NVLink into the same slice of every destination's buffer, and the slot handshakes are stream
     # memory operations (cuStreamWriteValue32 / cuStreamWaitValue32 on flag words in symmetric
-    # memory) -- measured on 2 x B200 next to the persistent kernels: a peer copy of a 14 MB shard
-    # 32 us (442 GB/s), while torch's barrier KERNEL took 59 us and a local staging copy 64 us because
-    # both must squeeze onto SMs the transform occupies (tools/symm_diag.py).
+    # memory): a torch barrier KERNEL or a local staging copy would have to squeeze onto SMs the
+    # transform occupies (tools/symm_diag.py measures both next to the persistent kernels).
     #   flags[slot][0][r] on rank d: "rank r's shard of use #c has landed in d's slot"   (r writes it)
     #   flags[slot][1][d] on rank r: "rank d has consumed use #c of the slot"             (d writes it)
     def _peer_setup(self, shard_shape, dtype, device):

@@ -1,7 +1,7 @@
 """Generate the golden fixtures by running the UNMODIFIED reference (nnAudio
-v0.3.3, imported read-only from ``$NNAUDIO_REF`` = /root/reference/Installation)
-on CPU in the build container.  The GPU box has no /root/reference, so the
-outputs are committed:
+v0.3.3, imported read-only from ``$NNAUDIO_REF``, the reference repository's
+``Installation`` directory) on CPU.  The tests must not depend on the reference
+being present, so the outputs are committed:
 
   ref_outputs.npz        reference forward() outputs for tests/golden/cases.py
   ref_buffers.json       sha256 of every state_dict buffer of the case modules
@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get("NNAUDIO_REF", "/root/reference/Installation")
+REF = os.environ["NNAUDIO_REF"]  # the reference repository's Installation/ directory
 sys.dont_write_bytecode = True
 sys.path.insert(0, REF)
 sys.path.insert(0, HERE)

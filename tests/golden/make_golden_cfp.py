@@ -27,7 +27,7 @@ import scipy.signal.windows
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = os.environ.get("NNAUDIO_REF", "/root/reference/Installation")
+REF = os.environ["NNAUDIO_REF"]  # the reference repository's Installation/ directory
 sys.dont_write_bytecode = True
 sys.path.insert(0, REF)
 sys.path.insert(0, HERE)

@@ -31,7 +31,7 @@ def test_abi_version_and_strerror():
     lib = _C.lib()
     assert lib.nnab_abi_version() == 1
     assert lib.nnab_strerror(0) == b"ok"
-    assert b"tcgen05" in lib.nnab_strerror(-2)
+    assert b"tensor-core" in lib.nnab_strerror(-2)
     assert lib.nnab_pack_tile_n(1025) == 208 and lib.nnab_pack_tile_n(84) == 176
 
 

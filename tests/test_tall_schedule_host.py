@@ -1,8 +1,8 @@
 """Host-side replay of the balanced schedule of the tall-A CQT kernel (csrc/tct_kernels.cu: TallSched<true>):
 the same integer arithmetic in Python, checked for the properties the kernel relies on — every (tile, chunk)
-unit is visited exactly once, a tile is shared by at most two CTA pairs, the pair holding a tile's LAST
-chunks is `reader + 1` and meets the tile as its FIRST piece (so its parked sums exist long before the
-reader, which meets the tile as its LAST piece, asks for them: no cyclic wait)."""
+unit is visited exactly once, a tile is shared by at most two CTAs (`pairs` below counts CTAs), the one
+holding a tile's LAST chunks is `reader + 1` and meets the tile as its FIRST piece (so its parked sums exist
+long before the reader, which meets the tile as its LAST piece, asks for them: no cyclic wait)."""
 import pytest
 
 
@@ -21,7 +21,8 @@ def pieces(pair, num_pairs, total_tiles, n_cols):
 
 
 @pytest.mark.parametrize("tiles,pairs,n_cols", [(463, 74, 8), (170, 74, 8), (8, 3, 8), (8, 5, 8), (75, 74, 8),
-                                                (147, 74, 1), (149, 66, 4), (1000, 74, 16), (5, 5, 8), (7, 2, 3)])
+                                                (147, 74, 1), (149, 66, 4), (1000, 74, 16), (5, 5, 8), (7, 2, 3),
+                                                (926, 132, 8), (29, 7, 8), (133, 132, 8)])
 def test_balanced_ranges_cover_once_and_share_tiles_pairwise(tiles, pairs, n_cols):
     assert pairs <= tiles  # the launcher's condition: a range is at least one tile long
     seen = {}

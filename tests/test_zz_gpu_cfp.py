@@ -1,5 +1,5 @@
 """GPU parity of Combined_Frequency_Periodicity / CFP (-m gpu; collected last): the three contraction
-stages run on the tcgen05 framed kernel (and, as the cross-check, on the fp32 CUDA-core kernel) through
+stages run on the tensor-core framed kernel (and, as the cross-check, on the fp32 CUDA-core kernel) through
 the C ABI, against the unmodified reference's outputs (tests/golden/ref_cfp.npz) and the CPU oracle.
 
 Tolerances.  CFP raises magnitudes to small powers (|X|^0.24, ceps^0.6) and, with a zero exponent, takes

@@ -1,5 +1,5 @@
 """Dense filterbanks on the tensor cores (-m gpu): Gammatonegram (and any mel bank that is not banded) as
-block-partial STFT -> bf16 hi/lo operand planes (FMT_PLANES epilogue) -> second tcgen05 contraction with the
+block-partial STFT -> bf16 hi/lo operand planes (FMT_PLANES epilogue) -> second tensor-core contraction with the
 re-indexed bank (FMT_REALPAIR), csrc/nnab_api.cu.  NNAB_FB_PLANES=1 selects it, 0 the round-1 path (fp32
 (B, F, T) power spectrogram + CUDA-core filterbank GEMM).  Checked against the CPU oracle / the reference
 fixtures at the 1e-4 bar, against the old path, and for bit-repeatability."""

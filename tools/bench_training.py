@@ -48,9 +48,7 @@ def main():
         _mel_and_inverse(args, dev, report)
     if args.only in ("all", "cqt"):
         _pyramid(args, dev, report)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/bench_training.json", "w") as f:
-        json.dump(out, f, indent=1)
+    print(json.dumps(out, indent=1))
 
 
 def _mel_and_inverse(args, dev, report):

@@ -48,7 +48,7 @@ def emulate(x, n_fft, hop, B=1):
             for quarter in range(4):
                 m0 = ct * 4 * FW + quarter * FW
                 A = rows[m0: m0 + 32]                       # one 32-row TMA box
-                acc = A @ basis[n0: n0 + nb].T                # (32 lanes, nb) TMEM columns (re + i im)
+                acc = A @ basis[n0: n0 + nb].T                # (32 rows, nb) accumulator columns (re + i im)
                 tw = [np.exp(-2j * np.pi * ((k_tile0 + 2 + i) % R) / R) for i in range(4)]
                 w = np.zeros((32, 10), dtype=complex)
                 for c in range(nb // 8):

@@ -1,7 +1,9 @@
 #!/usr/bin/env python
-"""GPU probe: UMMA smem descriptors that start at an arbitrary row of a SWIZZLE_128B block
+"""GPU probe: wgmma smem descriptors that start at an arbitrary row of a SWIZZLE_128B block
 (nnab_probe_rowoffset, csrc/tc_probe.cu).  Prints, per row offset r, whether
-base_offset = 0 and / or base_offset = r & 7 reproduce A[r:r+128] @ B^T."""
+base_offset = 0 and / or base_offset = r & 7 reproduce A[r:r+128] @ B^T.
+
+    python tools/probe_rowoffset.py [result.json]"""
 import ctypes, json, os, sys
 
 import numpy as np
@@ -33,6 +35,6 @@ ok0 = [r for r in range(16) if res[f"v0_r{r}"] < 1e-3]
 ok1 = [r for r in range(16) if res[f"v1_r{r}"] < 1e-3]
 print("base_offset = 0      correct for r in", ok0)
 print("base_offset = r & 7  correct for r in", ok1)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump({"errors": res, "ok_base0": ok0, "ok_base_r": ok1},
-          open(os.path.join(ROOT, "gpurun_out", "probe_rowoffset.json"), "w"), indent=1)
+if len(sys.argv) > 1:
+    with open(sys.argv[1], "w") as f:
+        json.dump({"errors": res, "ok_base0": ok0, "ok_base_r": ok1}, f, indent=1)

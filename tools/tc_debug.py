@@ -1,5 +1,5 @@
 """GPU debugging aid: run one module on both kernel families and print where
-(which bins / frames / clips) the tcgen05 path deviates from the SIMT path."""
+(which bins / frames / clips) the tensor-core path deviates from the SIMT path."""
 import os
 import sys
 
@@ -53,16 +53,16 @@ def main():
         x = torch.randn(*shape, device="cuda")
         ref = run(mod, x, "simt", **kw)
         try:
-            got = run(mod, x, "tcgen05", **kw)
+            got = run(mod, x, "tc", **kw)
         except Exception as e:  # noqa: BLE001
-            print(f"{name}: tcgen05 path raised {type(e).__name__}: {e}")
+            print(f"{name}: tensor-core path raised {type(e).__name__}: {e}")
             continue
         report(name, got, ref)
         if "--oracle" in sys.argv:
             sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
             from helpers import run_oracle
             orc = run_oracle(type(mod).__name__, mod, x.cpu().numpy(), kw)
-            report(name + " [tcgen05 vs fp64 oracle]", got, orc)
+            report(name + " [tensor-core vs fp64 oracle]", got, orc)
             report(name + " [simt    vs fp64 oracle]", ref, orc)
 
 

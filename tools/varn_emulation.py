@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """CPU emulation of the per-K-block-width kernel's data flow (branch radix2-wip): the packed row
 order of pack_basis_varn_kernel, the REAL host plan (nnab_debug_varn_plan through ctypes), the
-mixed-width accumulation into one TMEM tile (garbage = NaN until the first MMA of a tile writes a
-column) and the epilogue's column -> bin mapping, against the oracle's CQT1992v2.  Also runs the
-split-K variant (chunks accumulate into a zeroed raw buffer).  No tcgen05 mechanics, only logic."""
+mixed-width accumulation into one accumulator tile (garbage = NaN until the first MMA of a tile writes
+a column) and the epilogue's column -> bin mapping, against the oracle's CQT1992v2.  Also runs the
+split-K variant (chunks accumulate into a zeroed raw buffer).  No wgmma mechanics, only logic."""
 import os
 import sys
 
