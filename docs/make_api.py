@@ -32,8 +32,8 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
 * `CFP` / `Combined_Frequency_Periodicity` are forward-only (the reference has no parameters there; a waveform that
   requires grad raises `NotImplementedError`); their FFT stages run as dense contractions (DESIGN.md §3.9).
 
-Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAUDIO_B200_DECIM_BWD=fir|simt|tc|ola`
-(adjoint of the pyramid's FIR stages in training), `NNAB_TALL_BALANCE=0|1` (balanced tile schedule of the CQT1992v2 kernel).
+Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
+schedule of the CQT1992v2 kernel).
 
 """
 

@@ -422,17 +422,34 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
   }
   const size_t need = nnab_filterbank_workspace_bytes(B, L, n_fft, F, hop, center, n_fb, path, 0);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
-  {
-    FbPlanes fp;
-    if (fb_planes_enabled() && path != NNAB_PATH_SIMT && packed != nullptr && packed_kind(packed) == PACK_BLOCK &&
-        wants_tc(path, n_fft, hop) && B <= 65535 &&
-        fb_planes_layout(B, L, n_fft, F, hop, pad, T, n_fb, &fp) && ws_bytes >= fp.total) {
-      char* ws = reinterpret_cast<char*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-      __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(ws + fp.off_planes);
-      float* w_re = reinterpret_cast<float*>(ws + fp.off_w);
-      float* w_im = reinterpret_cast<float*>(ws + fp.off_w + align_up((size_t)fp.fh * fp.kp * sizeof(float), 256));
-      void* bank = ws + fp.off_packed;
-      const int64_t plane_stride = fp.rows * fp.kp;
+  FbPlanes fp;
+  if (fb_planes_enabled() && path != NNAB_PATH_SIMT && packed != nullptr && packed_kind(packed) == PACK_BLOCK &&
+      wants_tc(path, n_fft, hop) && B <= 65535 &&
+      fb_planes_layout(B, L, n_fft, F, hop, pad, T, n_fb, &fp) && ws_bytes >= fp.total) {
+    char* ws = reinterpret_cast<char*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(ws + fp.off_planes);
+    float* w_re = reinterpret_cast<float*>(ws + fp.off_w);
+    float* w_im = reinterpret_cast<float*>(ws + fp.off_w + align_up((size_t)fp.fh * fp.kp * sizeof(float), 256));
+    void* bank = ws + fp.off_packed;
+    const int64_t plane_stride = fp.rows * fp.kp;
+    // 1. STFT -> |X| ** power as operand planes (block-partial kernel, FMT_PLANES)
+    FramedProblem p{};
+    p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+    p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
+    p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
+    p.fmt = FMT_PLANES; p.eps = sqrt_eps; p.power = power; p.out = reinterpret_cast<float*>(planes); p.T = T;
+    p.out_bins = F; p.bin_offset = 0;
+    p.planes_stride = plane_stride; p.planes_pitch = fp.kp;
+    // 2. rows x bank on the dense kernel: every frame is one "hop" of kp samples
+    FramedProblem g{};
+    g.x = nullptr; g.B = B; g.L = T * fp.kp; g.x_pitch = T * fp.kp;
+    g.w_re = w_re; g.w_im = w_im; g.F = fp.fh; g.K = fp.kp; g.hop = fp.kp;
+    g.pad = 0; g.pad_mode = NNAB_PAD_CONSTANT; g.scale = nullptr; g.scale_all = 1.f;
+    g.fmt = FMT_REALPAIR; g.eps = 0.f; g.power = 1.f; g.out = out; g.T = T;
+    g.out_bins = n_fb; g.bin_offset = 0;
+    g.presplit = planes; g.presplit_t_slots = T; g.presplit_plane_stride = plane_stride;
+    // a shape either contraction rejects takes the fp32 path below, before anything is enqueued
+    if (tc_supported(p) && tc_supported(g)) {
       // the re-indexed bank (tiny: fh x kp) and its bf16 hi/lo packing
       if ((rc = launch_fb_tile_bank(fb, n_fb, F, fp.nb, fp.n_tiles, fp.kp, fp.fh, w_re, w_im, s))) return rc;
       if ((rc = tc_pack_basis(w_re, w_im, fp.fh, fp.kp, bank, s))) return rc;
@@ -440,23 +457,7 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
       if (fp.kp > fp.nb * fp.n_tiles)
         NNAB_CUDA_TRY(cudaMemset2DAsync(planes + fp.nb * fp.n_tiles, (size_t)fp.kp * 2, 0,
                                         (size_t)(fp.kp - fp.nb * fp.n_tiles) * 2, (size_t)(2 * fp.rows), s));
-      // 1. STFT -> |X| ** power as operand planes (block-partial kernel, FMT_PLANES)
-      FramedProblem p{};
-      p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
-      p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
-      p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
-      p.fmt = FMT_PLANES; p.eps = sqrt_eps; p.power = power; p.out = reinterpret_cast<float*>(planes); p.T = T;
-      p.out_bins = F; p.bin_offset = 0;
-      p.planes_stride = plane_stride; p.planes_pitch = fp.kp;
       if ((rc = run_framed(p, packed, ws, fp.off_planes, NNAB_PATH_TCGEN05, s))) return rc;
-      // 2. rows x bank on the dense kernel: every frame is one "hop" of kp samples
-      FramedProblem g{};
-      g.x = nullptr; g.B = B; g.L = T * fp.kp; g.x_pitch = T * fp.kp;
-      g.w_re = w_re; g.w_im = w_im; g.F = fp.fh; g.K = fp.kp; g.hop = fp.kp;
-      g.pad = 0; g.pad_mode = NNAB_PAD_CONSTANT; g.scale = nullptr; g.scale_all = 1.f;
-      g.fmt = FMT_REALPAIR; g.eps = 0.f; g.power = 1.f; g.out = out; g.T = T;
-      g.out_bins = n_fb; g.bin_offset = 0;
-      g.presplit = planes; g.presplit_t_slots = T; g.presplit_plane_stride = plane_stride;
       return run_framed(g, bank, nullptr, 0, NNAB_PATH_TCGEN05, s);
     }
   }
@@ -583,17 +584,17 @@ static size_t planes_bytes(int64_t B, int64_t L, int K, int hop, int pad, int64_
 }
 
 // Fills lv[0..n_octaves) and returns the workspace size; `pf_early` receives the offset of
-// the raw-signal FIR input when early downsampling is active.
+// the raw-signal FIR input when early downsampling is active, `scratch` the offset of the
+// split-signal scratch of the octaves that run from fp32.
 static size_t plan_pyramid(int64_t B, int64_t L, int n_octaves, int early_factor, int hop,
                            const int32_t* widths, int fixed_width, int pad_mode, PyrLevel* lv,
-                           size_t* pf_early) {
+                           size_t* pf_early, size_t* scratch) {
   size_t off = 0;
   auto take = [&](size_t n) { size_t o = off; off += n; return o; };
   int64_t len = L;
   if (early_factor > 1) {
-    const size_t o = take(planes_bytes(B, L, tc_fir_k(FIR_TAPS, early_factor), 128 * early_factor,
-                                       FIR_OFF, nullptr, nullptr));
-    if (pf_early) *pf_early = o;
+    *pf_early = take(planes_bytes(B, L, tc_fir_k(FIR_TAPS, early_factor), 128 * early_factor,
+                                  FIR_OFF, nullptr, nullptr));
     len = decimated_len(L, early_factor);
   }
   int cur_hop = hop;
@@ -620,6 +621,7 @@ static size_t plan_pyramid(int64_t B, int64_t L, int n_octaves, int early_factor
                                &l.pf_plane));
   }
   // scratch for octaves that run from fp32 (several frame phases): sized for the first such level
+  *scratch = off;
   for (int i = 0; i < n_octaves; ++i)
     if (!lv[i].presplit && lv[i].len > 0 && lv[i].hop > 0) {
       off += tc_workspace_bytes(B, lv[i].len, lv[i].width, lv[i].hop, lv[i].pad);
@@ -645,9 +647,10 @@ struct Lvl2 {
 
 static int64_t gcd64(int64_t a, int64_t b) { return b == 0 ? a : gcd64(b, a % b); }
 
-// false: the shape does not fit this plan (caller uses the first-generation pyramid)
+// false: the shape does not fit this plan.  `scratch` receives the offset of the split-signal
+// scratch of the octaves that run from fp32, `total` the workspace size.
 static bool plan_pyramid2(int64_t B, int64_t L, int n_octaves, int hop, const int32_t* widths,
-                          int fixed_width, int pad_mode, Lvl2* lv, size_t* total) {
+                          int fixed_width, int pad_mode, Lvl2* lv, size_t* scratch, size_t* total) {
   size_t off = 0;
   auto take = [&](size_t n) { size_t o = off; off += align_up(n, 256); return o; };
   int64_t len = L;
@@ -688,6 +691,7 @@ static bool plan_pyramid2(int64_t B, int64_t L, int n_octaves, int hop, const in
     }
   }
   // scratch for octaves that run from fp32 (several frame phases): sized for the first such level
+  *scratch = off;
   for (int i = 0; i < n_octaves; ++i)
     if (!lv[i].presplit) {
       off += tc_workspace_bytes(B, lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) + 256;
@@ -751,13 +755,14 @@ size_t nnab_cqt_pyramid_workspace_bytes(int64_t B, int64_t L, int n_octaves, int
     // (b) all-tensor-core pyramid: every level's planes (upper bound with max_width)
     if (n_octaves <= 32) {
       PyrLevel lv[32];
+      size_t pf_early = 0, scratch = 0;
       const size_t full = plan_pyramid(B, L, n_octaves, early_factor, hop, nullptr, max_width,
-                                       NNAB_PAD_REFLECT, lv, nullptr) + 1024;
+                                       NNAB_PAD_REFLECT, lv, &pf_early, &scratch) + 1024;
       if (full > n) n = full;
       Lvl2 lv2[32];
       size_t full2 = 0;
-      if (early_factor <= 1 &&
-          plan_pyramid2(B, L, n_octaves, hop, nullptr, max_width, NNAB_PAD_REFLECT, lv2, &full2)) {
+      if (early_factor <= 1 && plan_pyramid2(B, L, n_octaves, hop, nullptr, max_width, NNAB_PAD_REFLECT,
+                                             lv2, &scratch, &full2)) {
         full2 += 2048;
         if (full2 > n) n = full2;
       }
@@ -766,70 +771,96 @@ size_t nnab_cqt_pyramid_workspace_bytes(int64_t B, int64_t L, int n_octaves, int
   return n;
 }
 
-static int pyramid_fused2(const float* x, int64_t B, int64_t L, int64_t x_pitch, int n_octaves,
-                          const float* const* h_k_real, const float* const* h_k_imag,
-                          const void* const* h_packed, const int32_t* h_widths, int n_filters,
-                          const float* lowpass, const void* lowpass_packed, int hop, int pad_mode,
-                          int n_bins, const float* scale, float scale_all, int out_format,
-                          float sqrt_eps, float* out, int64_t T, void* workspace, size_t ws_bytes,
-                          cudaStream_t s) {
-  if (n_octaves > 32 || B > 65535) return NNAB_EUNSUPPORTED;
-  Lvl2 lv[32];
+// Arguments of one nnab_cqt_pyramid_forward call, shared by its three plans (same order as the call's).
+struct PyramidCall {
+  const float* x; int64_t B, L, x_pitch; int n_octaves;
+  const float* const* k_real; const float* const* k_imag; const void* const* packed; const int32_t* widths;
+  int n_filters; const float* lowpass; const void* lowpass_packed; const void* early_packed;
+  int early_factor, hop, pad_mode, n_bins; const float* scale; float scale_all; int out_format; float sqrt_eps;
+  float* out; int64_t T;
+  char* ws;  // the workspace aligned up to 256 bytes (the plans' size checks leave room for it)
+  size_t ws_bytes; cudaStream_t s;
+};
+
+// Octave i (0 = top) on a level of `len` samples framed every `hop`: its n_filters bins land
+// n_filters * (i + 1) rows below the top of the output, and the per-bin scale, indexed by output
+// row, is shifted by the same offset.
+static FramedProblem octave_problem(const PyramidCall& c, int i, int64_t len, int hop, int pad_mode) {
+  FramedProblem p{};
+  p.B = c.B; p.L = len;
+  p.w_re = c.k_real[i]; p.w_im = c.k_imag[i]; p.F = c.n_filters; p.K = c.widths[i]; p.hop = hop;
+  p.pad = p.K / 2; p.pad_mode = pad_mode; p.scale_all = c.scale_all;
+  p.fmt = c.out_format; p.eps = c.sqrt_eps; p.power = 1.f; p.out = c.out; p.T = c.T;
+  p.out_bins = c.n_bins;
+  p.bin_offset = c.n_bins - c.n_filters * (i + 1);
+  p.scale = c.scale ? c.scale + p.bin_offset : nullptr;
+  return p;
+}
+
+// Octave i of the gen-2 plan: on the level planes (one frame phase) or on the fp32 level.
+static FramedProblem octave2_problem(const PyramidCall& c, const Lvl2& l, int i) {
+  FramedProblem p = octave_problem(c, i, l.len, l.hop, l.mode);
+  if (l.presplit) {
+    p.presplit = c.ws + l.pc;
+    p.presplit_t_slots = l.t_slots;
+    p.presplit_plane_stride = l.plane;
+  } else {
+    p.x = (i == 0) ? c.x : (const float*)(c.ws + l.y32);
+    p.x_pitch = (i == 0) ? c.x_pitch : l.y32_pitch;
+  }
+  return p;
+}
+
+// Gen-2 plan of a call: NNAB_OK with lv and the scratch offset filled, NNAB_EUNSUPPORTED when the
+// call needs another plan, NNAB_EINVAL when an octave's frame count is not T.
+static int select_fused2(const PyramidCall& c, Lvl2* lv, size_t* scratch) {
+  if (c.n_octaves > 32 || c.B > 65535) return NNAB_EUNSUPPORTED;
   size_t need = 0;
-  if (!plan_pyramid2(B, L, n_octaves, hop, h_widths, 0, pad_mode, lv, &need)) return NNAB_EUNSUPPORTED;
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  if (need + 512 > ws_bytes) return NNAB_EUNSUPPORTED;
-  for (int i = 0; i < n_octaves; ++i)
-    if (frames_of(lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) != T) return NNAB_EINVAL;
-  size_t scratch_off = need;
-  for (int i = 0; i < n_octaves; ++i)
-    if (!lv[i].presplit) {
-      scratch_off -= tc_workspace_bytes(B, lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) + 256;
-      break;
-    }
+  if (!plan_pyramid2(c.B, c.L, c.n_octaves, c.hop, c.widths, 0, c.pad_mode, lv, scratch, &need))
+    return NNAB_EUNSUPPORTED;
+  if (need + 512 > c.ws_bytes) return NNAB_EUNSUPPORTED;
+  for (int i = 0; i < c.n_octaves; ++i)
+    if (frames_of(lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) != c.T) return NNAB_EINVAL;
+  // an octave the octave kernel does not take runs on the dense kernel (the FIR stages fit by construction)
+  for (int i = 0; i < c.n_octaves; ++i) {
+    const FramedProblem p = octave2_problem(c, lv[i], i);
+    if (!octave_tc_ok(p) && !tc_supported(p)) return NNAB_EUNSUPPORTED;
+  }
+  return NNAB_OK;
+}
+
+static int pyramid_fused2(const PyramidCall& c, const Lvl2* lv, size_t scratch_off) {
+  const int64_t B = c.B;
+  char* const ws = c.ws;
+  cudaStream_t s = c.s;
   char* scratch = ws + scratch_off;
+  const size_t scratch_bytes = c.ws_bytes - 256 - scratch_off;
   int rc;
-  const size_t scratch_bytes = ws_bytes - 256 - scratch_off;
 
   // level 0: the caller's fp32 waveform -> planes (one pass; writes the whole clip slot)
   if (lv[0].planes) {
-    rc = tc_pad_split_ex(x, B, L, x_pitch, lv[0].pad, lv[0].mode, lv[0].pitch, lv[0].plane,
+    rc = tc_pad_split_ex(c.x, B, c.L, c.x_pitch, lv[0].pad, lv[0].mode, lv[0].pitch, lv[0].plane,
                          ws + lv[0].pc, s);
     if (rc) return rc;
   }
-  for (int i = 0; i < n_octaves; ++i) {
-    Lvl2& l = lv[i];
-    FramedProblem p{};
-    p.B = B; p.L = l.len;
-    p.w_re = h_k_real[i]; p.w_im = h_k_imag[i]; p.F = n_filters; p.K = l.width; p.hop = l.hop;
-    p.pad = l.pad; p.pad_mode = l.mode; p.scale_all = scale_all;
-    p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
-    p.out_bins = n_bins;
-    p.bin_offset = n_bins - n_filters * (i + 1);
-    p.scale = scale ? scale + p.bin_offset : nullptr;
-    if (l.presplit) {
-      p.presplit = ws + l.pc;
-      p.presplit_t_slots = l.t_slots;
-      p.presplit_plane_stride = l.plane;
-      bool done = false;
-      if (!done) {
-        // resident bank + tall A blocks + frame phases: one fetch per sample and tile
-        std::pair<cudaEvent_t, cudaEvent_t> pr;
-        const bool timed = prof_begin(s, &pr);
-        rc = launch_octave_tc(p, h_packed[i], s);
-        if (timed) prof_end(s, pr);
-        if (rc == NNAB_OK) done = true;
-        else if (rc != NNAB_EUNSUPPORTED) return rc;
-      }
-      if (!done && (rc = run_framed(p, h_packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
+  for (int i = 0; i < c.n_octaves; ++i) {
+    const Lvl2& l = lv[i];
+    const FramedProblem p = octave2_problem(c, l, i);
+    if (octave_tc_ok(p)) {
+      // resident bank + tall A blocks + frame phases: one fetch per sample and tile
+      std::pair<cudaEvent_t, cudaEvent_t> pr;
+      const bool timed = prof_begin(s, &pr);
+      rc = launch_octave_tc(p, c.packed[i], s);
+      if (timed) prof_end(s, pr);
+    } else if (l.presplit) {
+      rc = run_framed(p, c.packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s);
     } else {
-      const float* src = (i == 0) ? x : (const float*)(ws + l.y32);
-      p.x = src; p.x_pitch = (i == 0) ? x_pitch : l.y32_pitch;
-      if ((rc = run_framed(p, h_packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s))) return rc;
+      rc = run_framed(p, c.packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s);
     }
-    if (i == n_octaves - 1) break;
+    if (rc) return rc;
+    if (i == c.n_octaves - 1) break;
     // ---- FIR stage: level i -> level i + 1
-    Lvl2& d = lv[i + 1];
+    const Lvl2& d = lv[i + 1];
     DecimParams dec{};
     dec.len_out = d.len;
     if (d.planes) {
@@ -842,52 +873,79 @@ static int pyramid_fused2(const float* x, int64_t B, int64_t L, int64_t x_pitch,
       dec.pc_reflect = refl ? 1 : 0;
     }
     if (d.y32 != SIZE_MAX) { dec.y32 = (float*)(ws + d.y32); dec.y32_pitch = d.y32_pitch; }
-    rc = launch_fir_stage_tc(ws + l.pc, B, l.len, l.pitch, l.plane, l.pad, lowpass_packed, lowpass,
+    rc = launch_fir_stage_tc(ws + l.pc, B, l.len, l.pitch, l.plane, l.pad, c.lowpass_packed, c.lowpass,
                              FIR_TAPS, dec, s);
-    if (rc) return rc;  // (EUNSUPPORTED cannot happen after plan_pyramid2 accepted the shape)
+    if (rc) return rc;
   }
   return NNAB_OK;
 }
 
-// All-tensor-core pyramid; returns NNAB_EUNSUPPORTED when the plan cannot be used (the caller
-// then takes the per-octave path).
-static int pyramid_fused(const float* x, int64_t B, int64_t L, int64_t x_pitch, int n_octaves,
-                         const float* const* h_k_real, const float* const* h_k_imag,
-                         const void* const* h_packed, const int32_t* h_widths, int n_filters,
-                         const void* lowpass_packed, const void* early_packed, int early_factor,
-                         int hop, int pad_mode, int n_bins, const float* scale, float scale_all,
-                         int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
-                         size_t ws_bytes, cudaStream_t s) {
-  if (n_octaves > 32 || B > 65535) return NNAB_EUNSUPPORTED;
-  PyrLevel lv[32];
-  size_t pf_early = SIZE_MAX;
-  const size_t need = plan_pyramid(B, L, n_octaves, early_factor, hop, h_widths, 0, pad_mode, lv,
-                                   &pf_early);
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  if (need + 256 > ws_bytes) return NNAB_EUNSUPPORTED;
-  for (int i = 0; i < n_octaves; ++i) {
+// Octave i of the gen-1 plan: on the level's reflect-padded planes (one frame phase) or on the fp32 level.
+static FramedProblem octave1_problem(const PyramidCall& c, const PyrLevel& l, int i) {
+  FramedProblem p = octave_problem(c, i, l.len, l.hop, l.mode);
+  if (l.presplit) {
+    p.presplit = c.ws + l.pc;
+  } else if (i == 0 && c.early_factor <= 1) {  // level 0 is the caller's waveform
+    p.x = c.x; p.x_pitch = c.x_pitch;
+  } else {
+    p.x = (const float*)(c.ws + l.y32); p.x_pitch = l.y32_pitch;
+  }
+  return p;
+}
+
+// FIR stage of the gen-1 plan: planes `src` (level signal at FIR_OFF, zero margins) -> level `dst`.
+static FramedProblem fir1_problem(const PyramidCall& c, const void* src, int64_t src_len, int dec,
+                                  const PyrLevel& dst) {
+  FramedProblem p{};
+  p.x = nullptr; p.B = c.B; p.L = src_len; p.x_pitch = 0;
+  p.w_re = nullptr; p.w_im = nullptr; p.F = 64; p.K = tc_fir_k(FIR_TAPS, dec); p.hop = 128 * dec;
+  p.pad = FIR_OFF; p.pad_mode = NNAB_PAD_CONSTANT; p.scale = nullptr; p.scale_all = 1.f;
+  p.fmt = FMT_DECIM; p.eps = 0.f; p.power = 1.f; p.out = nullptr;
+  p.T = (dst.len + 127) / 128;
+  p.out_bins = 64; p.bin_offset = 0;
+  p.presplit = src;
+  p.dec.pc = dst.pc != SIZE_MAX ? c.ws + dst.pc : nullptr;
+  p.dec.pc_plane = dst.pc_plane; p.dec.pc_pitch = dst.pc_pitch; p.dec.pc_off = dst.pad;
+  p.dec.pc_reflect = dst.mode == NNAB_PAD_REFLECT ? 1 : 0;
+  p.dec.pf = dst.pf != SIZE_MAX ? c.ws + dst.pf : nullptr;
+  p.dec.pf_plane = dst.pf_plane; p.dec.pf_pitch = dst.pf_pitch;
+  p.dec.y32 = dst.y32 != SIZE_MAX ? (float*)(c.ws + dst.y32) : nullptr;
+  p.dec.y32_pitch = dst.y32_pitch;
+  p.dec.len_out = dst.len;
+  return p;
+}
+
+// Gen-1 plan of a call: as select_fused2, plus the offset of the early FIR stage's input.
+static int select_fused(const PyramidCall& c, PyrLevel* lv, size_t* pf_early, size_t* scratch) {
+  if (c.n_octaves > 32 || c.B > 65535) return NNAB_EUNSUPPORTED;
+  const size_t need = plan_pyramid(c.B, c.L, c.n_octaves, c.early_factor, c.hop, c.widths, 0, c.pad_mode,
+                                   lv, pf_early, scratch);
+  if (need + 256 > c.ws_bytes) return NNAB_EUNSUPPORTED;
+  for (int i = 0; i < c.n_octaves; ++i) {
     if (lv[i].len <= 0 || lv[i].hop <= 0) return NNAB_EINVAL;
-    if (frames_of(lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) != T) return NNAB_EINVAL;
+    if (frames_of(lv[i].len, lv[i].width, lv[i].hop, lv[i].pad) != c.T) return NNAB_EINVAL;
   }
-  // scratch region for fp32-driven octaves lives after the planned buffers
-  size_t planned = 0;
-  {
-    PyrLevel tmp[32];
-    planned = plan_pyramid(B, L, n_octaves, early_factor, hop, h_widths, 0, pad_mode, tmp, nullptr);
-    for (int i = 0; i < n_octaves; ++i)
-      if (!tmp[i].presplit) {
-        planned -= tc_workspace_bytes(B, tmp[i].len, tmp[i].width, tmp[i].hop, tmp[i].pad);
-        break;
-      }
+  if (c.early_factor > 1 && !tc_supported(fir1_problem(c, c.ws + *pf_early, c.L, c.early_factor, lv[0])))
+    return NNAB_EUNSUPPORTED;
+  for (int i = 0; i < c.n_octaves; ++i) {
+    if (!tc_supported(octave1_problem(c, lv[i], i))) return NNAB_EUNSUPPORTED;
+    if (i < c.n_octaves - 1 && !tc_supported(fir1_problem(c, c.ws + lv[i].pf, lv[i].len, 2, lv[i + 1])))
+      return NNAB_EUNSUPPORTED;
   }
-  char* scratch = ws + planned;
-  const size_t scratch_bytes = ws_bytes - 256 - planned;
+  return NNAB_OK;
+}
+
+static int pyramid_fused(const PyramidCall& c, const PyrLevel* lv, size_t pf_early, size_t scratch_off) {
+  const int64_t B = c.B;
+  char* const ws = c.ws;
+  cudaStream_t s = c.s;
+  char* scratch = ws + scratch_off;
+  const size_t scratch_bytes = c.ws_bytes - 256 - scratch_off;
   int rc;
 
   // One FIR stage: planes `src` (level signal, zero margins) -> level `dst`
   auto fir_stage = [&](const void* src, int64_t src_len, int dec, const void* fir_packed,
-                       PyrLevel& dst) -> int {
-    const int kf = tc_fir_k(FIR_TAPS, dec);
+                       const PyrLevel& dst) -> int {
     // parts of the destination buffers the epilogue never writes
     if (dst.pc != SIZE_MAX) {
       const bool refl = dst.mode == NNAB_PAD_REFLECT;
@@ -900,76 +958,42 @@ static int pyramid_fused(const float* x, int64_t B, int64_t L, int64_t x_pitch, 
                            FIR_OFF + dst.len, s);
       if (rc) return rc;
     }
-    FramedProblem p{};
-    p.x = nullptr; p.B = B; p.L = src_len; p.x_pitch = 0;
-    p.w_re = nullptr; p.w_im = nullptr; p.F = 64; p.K = kf; p.hop = 128 * dec;
-    p.pad = FIR_OFF; p.pad_mode = NNAB_PAD_CONSTANT; p.scale = nullptr; p.scale_all = 1.f;
-    p.fmt = FMT_DECIM; p.eps = 0.f; p.power = 1.f; p.out = nullptr;
-    p.T = (dst.len + 127) / 128;
-    p.out_bins = 64; p.bin_offset = 0;
-    p.presplit = src;
-    p.dec.pc = dst.pc != SIZE_MAX ? ws + dst.pc : nullptr;
-    p.dec.pc_plane = dst.pc_plane; p.dec.pc_pitch = dst.pc_pitch; p.dec.pc_off = dst.pad;
-    p.dec.pc_reflect = dst.mode == NNAB_PAD_REFLECT ? 1 : 0;
-    p.dec.pf = dst.pf != SIZE_MAX ? ws + dst.pf : nullptr;
-    p.dec.pf_plane = dst.pf_plane; p.dec.pf_pitch = dst.pf_pitch;
-    p.dec.y32 = dst.y32 != SIZE_MAX ? (float*)(ws + dst.y32) : nullptr;
-    p.dec.y32_pitch = dst.y32_pitch;
-    p.dec.len_out = dst.len;
-    return run_framed(p, fir_packed, nullptr, 0, NNAB_PATH_TCGEN05, s);
+    return run_framed(fir1_problem(c, src, src_len, dec, dst), fir_packed, nullptr, 0, NNAB_PATH_TCGEN05, s);
   };
 
   // ---- level 0 ------------------------------------------------------------------------
-  const float* x0 = x;         // fp32 level-0 signal when available
-  int64_t x0_pitch = x_pitch;
-  if (early_factor > 1) {
-    rc = tc_pad_split(x, B, L, x_pitch, tc_fir_k(FIR_TAPS, early_factor), 128 * early_factor,
+  if (c.early_factor > 1) {
+    rc = tc_pad_split(c.x, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, c.early_factor), 128 * c.early_factor,
                       FIR_OFF, NNAB_PAD_CONSTANT, ws + pf_early, s);
     if (rc) return rc;
-    if ((rc = fir_stage(ws + pf_early, L, early_factor, early_packed, lv[0]))) return rc;
-    x0 = lv[0].y32 != SIZE_MAX ? (const float*)(ws + lv[0].y32) : nullptr;
-    x0_pitch = lv[0].y32_pitch;
+    if ((rc = fir_stage(ws + pf_early, c.L, c.early_factor, c.early_packed, lv[0]))) return rc;
   } else {
     if (lv[0].pc != SIZE_MAX && lv[0].pf != SIZE_MAX) {
       // one pass over x: reflect-padded copy for the octave CQT + zero-margin copy for the FIR
-      rc = tc_pad_split2(x, B, L, x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
+      rc = tc_pad_split2(c.x, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
                          ws + lv[0].pc, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, NNAB_PAD_CONSTANT,
                          ws + lv[0].pf, s);
       if (rc) return rc;
     } else if (lv[0].pc != SIZE_MAX) {
-      rc = tc_pad_split(x, B, L, x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
+      rc = tc_pad_split(c.x, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
                         ws + lv[0].pc, s);
       if (rc) return rc;
     } else if (lv[0].pf != SIZE_MAX) {
-      rc = tc_pad_split(x, B, L, x_pitch, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, NNAB_PAD_CONSTANT,
+      rc = tc_pad_split(c.x, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, NNAB_PAD_CONSTANT,
                         ws + lv[0].pf, s);
       if (rc) return rc;
     }
   }
 
   // ---- octaves --------------------------------------------------------------------------
-  for (int i = 0; i < n_octaves; ++i) {
-    PyrLevel& l = lv[i];
-    FramedProblem p{};
-    p.B = B; p.L = l.len;
-    p.w_re = h_k_real[i]; p.w_im = h_k_imag[i]; p.F = n_filters; p.K = l.width; p.hop = l.hop;
-    p.pad = l.pad; p.pad_mode = l.mode; p.scale_all = scale_all;
-    p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
-    p.out_bins = n_bins;
-    p.bin_offset = n_bins - n_filters * (i + 1);
-    p.scale = scale ? scale + p.bin_offset : nullptr;
-    if (l.presplit) {
-      p.x = nullptr; p.x_pitch = 0; p.presplit = ws + l.pc;
-      if ((rc = run_framed(p, h_packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
-    } else {
-      const float* src = (i == 0) ? x0 : (const float*)(ws + l.y32);
-      const int64_t pitch = (i == 0) ? x0_pitch : l.y32_pitch;
-      if (src == nullptr) return NNAB_EINVAL;
-      p.x = src; p.x_pitch = pitch; p.presplit = nullptr;
-      if ((rc = run_framed(p, h_packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s))) return rc;
-    }
-    if (i < n_octaves - 1)
-      if ((rc = fir_stage(ws + l.pf, l.len, 2, lowpass_packed, lv[i + 1]))) return rc;
+  for (int i = 0; i < c.n_octaves; ++i) {
+    const PyrLevel& l = lv[i];
+    const FramedProblem p = octave1_problem(c, l, i);
+    if (l.presplit) rc = run_framed(p, c.packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s);
+    else rc = run_framed(p, c.packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s);
+    if (rc) return rc;
+    if (i < c.n_octaves - 1)
+      if ((rc = fir_stage(ws + l.pf, l.len, 2, c.lowpass_packed, lv[i + 1]))) return rc;
   }
   return NNAB_OK;
 }
@@ -1000,22 +1024,30 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
       nnab_cqt_pyramid_workspace_bytes(B, L, n_octaves, early_factor, max_width, hop, path);
   if (need > 0 && (workspace == nullptr || ws_bytes < need)) return NNAB_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
+  const PyramidCall c{x, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed, h_widths, n_filters,
+                      lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
+                      scale_all, out_format, sqrt_eps, out, T,
+                      (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), ws_bytes, s};
 
-  // ---- all-tensor-core pyramid when every packed operand is available -------------------
+  // One plan per call, fixed before anything is enqueued: gen-2 (all-tensor-core, one plane set per
+  // level), else gen-1 (all-tensor-core, early downsampling and any bank width), else per-octave --
+  // the first whose conditions hold, tc_supported of every stage it runs on the dense tensor-core
+  // kernel included.  Once chosen, a plan's every error (NNAB_EUNSUPPORTED too) goes to the caller.
   bool all_packed = (path != NNAB_PATH_SIMT) && h_packed != nullptr && lowpass_packed != nullptr &&
                     (early_factor <= 1 || early_packed != nullptr);
   for (int i = 0; all_packed && i < n_octaves; ++i) all_packed = h_packed[i] != nullptr;
-  if (all_packed && getenv("NNAB_PYRAMID_UNFUSED") == nullptr && early_factor <= 1 &&
-      !(getenv("NNAB_PYRAMID2") != nullptr && atoi(getenv("NNAB_PYRAMID2")) == 0)) {
-    rc = pyramid_fused2(x, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed, h_widths, n_filters,
-                        lowpass, lowpass_packed, hop, pad_mode, n_bins, scale, scale_all, out_format,
-                        sqrt_eps, out, T, workspace, ws_bytes, s);
+  if (all_packed && early_factor <= 1) {
+    Lvl2 lv[32];
+    size_t scratch = 0;
+    rc = select_fused2(c, lv, &scratch);
+    if (rc == NNAB_OK) return pyramid_fused2(c, lv, scratch);
     if (rc != NNAB_EUNSUPPORTED) return rc;
   }
-  if (all_packed && getenv("NNAB_PYRAMID_UNFUSED") == nullptr) {
-    rc = pyramid_fused(x, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
-                       n_filters, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins,
-                       scale, scale_all, out_format, sqrt_eps, out, T, workspace, ws_bytes, s);
+  if (all_packed) {
+    PyrLevel lv[32];
+    size_t pf_early = 0, scratch = 0;
+    rc = select_fused(c, lv, &pf_early, &scratch);
+    if (rc == NNAB_OK) return pyramid_fused(c, lv, pf_early, scratch);
     if (rc != NNAB_EUNSUPPORTED) return rc;
   }
 
@@ -1059,16 +1091,8 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
     int mode = pad_mode;
     if (mode == NNAB_PAD_REFLECT && pad >= cur_len) mode = NNAB_PAD_CONSTANT;
     if (frames_of(cur_len, width, cur_hop, pad) != T) return NNAB_EINVAL;
-    FramedProblem p{};
-    p.x = cur; p.B = B; p.L = cur_len; p.x_pitch = cur_pitch;
-    p.w_re = h_k_real[i]; p.w_im = h_k_imag[i]; p.F = n_filters; p.K = width; p.hop = cur_hop;
-    p.pad = pad; p.pad_mode = mode; p.scale = nullptr; p.scale_all = scale_all;
-    p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
-    p.out_bins = n_bins;
-    // octave i (0 = top) lands n_filters*(i+1) rows below the top of the output
-    p.bin_offset = n_bins - n_filters * (i + 1);
-    // per-bin scale is indexed by OUTPUT row: shift the pointer by the same offset
-    p.scale = scale ? scale + p.bin_offset : nullptr;
+    FramedProblem p = octave_problem(c, i, cur_len, cur_hop, mode);
+    p.x = cur; p.x_pitch = cur_pitch;
     const void* pk = (h_packed != nullptr) ? h_packed[i] : nullptr;
     if (pk != nullptr && path != NNAB_PATH_SIMT && tc_supported(p) &&
         tc_ws_bytes >= tc_workspace_bytes(B, cur_len, width, cur_hop, pad)) {

@@ -55,6 +55,7 @@ int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int6
                         const float* fir, int taps, const DecimParams& dec, cudaStream_t stream);
 
 // octave CQT on shared level planes: resident bank, tall A blocks, frame phases (tct_kernels.cu)
+bool octave_tc_ok(const FramedProblem& q);
 int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t stream);
 int tc_tile_n(int F);
 

@@ -196,27 +196,21 @@ __global__ void __launch_bounds__(256) pack_basis_kernel(
 }
 
 void tc_forget_packed(const void* packed);
-bool tc_varn_enabled();
 bool tc_varn_basis_ok(int F, int K);
 int tc_pack_basis_varn(const float* w_re, const float* w_im, int F, int K, void* packed,
                        cudaStream_t stream);
 
 // layout: 0 = dense (always valid); 3 = 8-bin-group layout for the per-K-block-width / tall-A kernels
-// (any basis with F <= 128).  NNAB_VARN=0 forces dense.
+// (any basis with F <= 128; dense otherwise).
 int tc_pack_basis_layout(const float* w_re, const float* w_im, int F, int K, int layout, void* packed,
                          cudaStream_t stream) {
-  const char* ev = getenv("NNAB_VARN");
-  if (layout == 3 && !(ev != nullptr && atoi(ev) == 0) && tc_varn_basis_ok(F, K))
-    return tc_pack_basis_varn(w_re, w_im, F, K, packed, stream);
+  if (layout == 3 && tc_varn_basis_ok(F, K)) return tc_pack_basis_varn(w_re, w_im, F, K, packed, stream);
   if (layout != 0 && layout != 3) return NNAB_EINVAL;
   return tc_pack_basis(w_re, w_im, F, K, packed, stream);
 }
 
 int tc_pack_basis(const float* w_re, const float* w_im, int F, int K, void* packed,
                   cudaStream_t stream) {
-  // (NNAB_VARN=1: debugging switch -- the 8-bin-group layout for every long bank)
-  if (tc_varn_enabled() && tc_varn_basis_ok(F, K) && K >= 4096)
-    return tc_pack_basis_varn(w_re, w_im, F, K, packed, stream);
   tc_forget_packed(packed);
   const int bn = choose_bn(F);
   const int n_tiles = (2 * F + bn - 1) / bn;
@@ -1326,13 +1320,8 @@ void tc_forget_packed(const void* packed) { mark_packed(packed, PACK_DENSE); }
 
 
 // ---------------------------------------------------------------------------
-// per-K-block MMA width, host side (layout NNAB_LAYOUT_GROUPS; NNAB_VARN=0 forces dense)
+// per-K-block MMA width, host side (layout NNAB_LAYOUT_GROUPS)
 // ---------------------------------------------------------------------------
-bool tc_varn_enabled() {
-  const char* e = getenv("NNAB_VARN");
-  return e != nullptr && atoi(e) == 1;
-}
-
 bool tc_varn_basis_ok(int F, int K) { return F >= 1 && F <= 128 && K >= 64 && K <= 64 * VN_MAX_BLOCKS; }
 
 int tc_pack_basis_varn(const float* w_re, const float* w_im, int F, int K, void* packed,

@@ -452,9 +452,6 @@ static int launch_tct_fmt(const CUtensorMap& ma, const CUtensorMap& mb8, const C
 int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* workspace, size_t ws_bytes,
                           cudaStream_t stream) {
   if (!tc_tall_problem_ok(q)) return NNAB_EUNSUPPORTED;
-  if (const char* e = getenv("NNAB_TALL")) {
-    if (atoi(e) == 0) return NNAB_EUNSUPPORTED;  // A/B switch: per-K-block-width kernel without A reuse
-  }
   TallPlan plan;
   int rc = build_tall_plan(q, &plan);
   if (rc) return rc;
@@ -984,32 +981,31 @@ static int launch_octave_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const
   return NNAB_OK;
 }
 
-// q: an octave problem on caller-managed planes (presplit + presplit_t_slots); packed: the DENSE
-// packed bank (tc_pack_basis) with bn = 32.  NNAB_EUNSUPPORTED = not applicable, nothing enqueued.
+// Whether octave_tc_kernel takes the octave problem q: caller-managed planes (presplit + presplit_t_slots),
+// a dense bank of <= 16 bins, whole K blocks whose row shifts fit the A block, and a hop that is a multiple of
+// 64 with a power-of-two number of column blocks, or a divisor of 64 (frame phases) of at least 8.
+bool octave_tc_ok(const FramedProblem& q) {
+  if (q.presplit == nullptr || q.presplit_t_slots <= 0) return false;
+  if (q.F > 16 || tc_tile_n(q.F) != 32 || q.K % 64 != 0 || q.K / 64 > OCT_MAX_KB || q.B > 65535) return false;
+  if (q.h_k_begin != nullptr) return false;
+  if (q.fmt != NNAB_FMT_MAGNITUDE && q.fmt != NNAB_FMT_COMPLEX && q.fmt != NNAB_FMT_PHASE_UNIT) return false;
+  if (q.hop >= 64 ? (q.hop % 64 != 0) : (q.hop < 8 || 64 % q.hop != 0)) return false;
+  const int hop_eff = q.hop >= 64 ? q.hop : 64;
+  const int hb = hop_eff / 64;
+  if ((hb & (hb - 1)) != 0) return false;           // the kernel shifts by log2(hb)
+  if ((q.K / 64 - 1) / hb > 8) return false;          // row shifts must fit the 136-row block
+  return (q.presplit_t_slots * q.hop) % hop_eff == 0;
+}
+
+// q: an octave problem octave_tc_ok accepts; packed: the DENSE packed bank (tc_pack_basis) with bn = 32.
+// NNAB_EUNSUPPORTED = not applicable, nothing enqueued.
 int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t stream) {
-  if (const char* e = getenv("NNAB_OCTAVE_TC")) {
-    if (atoi(e) == 0) return NNAB_EUNSUPPORTED;
-  }
-  if (q.presplit == nullptr || q.presplit_t_slots <= 0 || packed == nullptr) return NNAB_EUNSUPPORTED;
-  if (q.F > 16 || tc_tile_n(q.F) != 32 || q.K % 64 != 0 || q.K / 64 > OCT_MAX_KB || q.B > 65535)
-    return NNAB_EUNSUPPORTED;
-  if (q.h_k_begin != nullptr) return NNAB_EUNSUPPORTED;
-  if (q.fmt != NNAB_FMT_MAGNITUDE && q.fmt != NNAB_FMT_COMPLEX && q.fmt != NNAB_FMT_PHASE_UNIT)
-    return NNAB_EUNSUPPORTED;
-  int P = 1, hop_eff = q.hop;
-  if (q.hop >= 64) {
-    if (q.hop % 64 != 0) return NNAB_EUNSUPPORTED;
-  } else {
-    if (q.hop < 8 || 64 % q.hop != 0) return NNAB_EUNSUPPORTED;
-    P = 64 / q.hop;
-    hop_eff = 64;
-  }
+  if (!octave_tc_ok(q) || packed == nullptr) return NNAB_EUNSUPPORTED;
+  const int P = tall_phases(q.hop);
+  const int hop_eff = q.hop >= 64 ? q.hop : 64;
   const int hb = hop_eff / 64;
   const int n_kb = q.K / 64;
-  if ((n_kb - 1) / hb > 8) return NNAB_EUNSUPPORTED;  // row shifts must fit the 136-row block
-  const int64_t pitch = q.presplit_t_slots * q.hop;
-  if (pitch % hop_eff != 0) return NNAB_EUNSUPPORTED;
-  const int64_t t_slots = pitch / hop_eff;
+  const int64_t t_slots = q.presplit_t_slots * q.hop / hop_eff;
   const int64_t plane_stride = q.presplit_plane_stride;
   __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(q.presplit));
 
@@ -1025,7 +1021,8 @@ int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t st
     const uint64_t strides[3] = {(uint64_t)(P > 1 ? q.hop : hop_eff) * 2, (uint64_t)hop_eff * 2,
                                  (uint64_t)plane_stride * 2};
     const uint32_t box[3] = {64, 1, OCT_A_ROWS};
-    if (encode_4d(&ma, planes, dims, strides, box)) return NNAB_EUNSUPPORTED;
+    const int rc = encode_4d(&ma, planes, dims, strides, box);
+    if (rc) return rc;
   }
   const int kpad = round_up_i(q.K, 64);
   int rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, 32, 2, (uint64_t)kpad * 2,
@@ -1036,7 +1033,6 @@ int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t st
   prm.hb = hb;
   prm.hb_log2 = 0;
   while ((1 << prm.hb_log2) < hb) ++prm.hb_log2;
-  if ((1 << prm.hb_log2) != hb) return NNAB_EUNSUPPORTED;
   prm.n_kb = n_kb;
   prm.nv = q.B * t_slots;
   prm.t_slots = t_slots;

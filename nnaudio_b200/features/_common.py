@@ -156,20 +156,17 @@ class PackedBasis:
         """``groups``: long nested CQT bank -> 8-bin-group layout (per-K-block-width / tall-A kernels);
         ``block_hop``: STFT-family module -> block-partial layout when the buffers ARE the periodic-Hann
         DFT (checked here on the tensors)."""
-        import os
 
         def build():
-            # block-partial layout (default for the STFT family): the module computes a plain
-            # one-sided STFT with hop ``block_hop`` and an output format the block kernel has an
-            # epilogue for; the buffers must BE the periodic-Hann DFT (NNAUDIO_B200_BLOCK=0: off)
-            if block_hop and os.environ.get("NNAUDIO_B200_BLOCK", "1") != "0" \
-                    and _C.block_layout_ok(int(w_re.shape[1]), int(block_hop)) \
+            # block-partial layout (the STFT family): the module computes a plain one-sided STFT
+            # with hop ``block_hop`` and an output format the block kernel has an epilogue for;
+            # the buffers must BE the periodic-Hann DFT
+            if block_hop and _C.block_layout_ok(int(w_re.shape[1]), int(block_hop)) \
                     and is_hann_dft(w_re, w_im):
                 return _C.pack_basis_block(w_re, int(block_hop))
-            # long CQT banks (CQT1992v2): per-K-block MMA width, the default since round 2
-            # (GPU-verified: reference chirp goldens + cfg3 full size; NNAUDIO_B200_VARN=0: dense)
-            if groups and w_re.shape[0] <= 128 and w_re.shape[1] >= 4096 \
-                    and os.environ.get("NNAUDIO_B200_VARN", "1") != "0":
+            # long CQT banks (CQT1992v2): per-K-block MMA width
+            # (GPU-verified: reference chirp goldens + cfg3 full size)
+            if groups and w_re.shape[0] <= 128 and w_re.shape[1] >= 4096:
                 return _C.pack_basis(w_re, w_im, _C.LAYOUT_GROUPS)
             return _C.pack_basis(w_re, w_im)
 

@@ -5,7 +5,6 @@ Buffer names follow the reference, including its spelling ``lenghts``.
 """
 from __future__ import annotations
 
-import os
 import warnings
 from time import time
 
@@ -437,43 +436,6 @@ def _framed_complex_autograd(mod, tag, sig, w_re, w_im, hop, center, pad_mode):
     return FramedComplexFn.apply(sig, w_re, w_im, fwd, bwd, bwd_w)
 
 
-class _DecimateFn(torch.autograd.Function):
-    """``conv1d(sig, fir, stride=n, padding=(taps-1)//2)`` (utils.py:73-100) with a gradient for
-    ``sig``.  Forward: a one-row framed contraction on the zero-padded signal.  Backward: the
-    adjoint of an n-fold decimating FIR is n interleaved stride-1 FIRs of ``dL/dy`` with the
-    polyphase components ``h_p[q] = fir[n*q + p]`` — again a framed contraction (n rows,
-    ceil(taps/n) taps, hop 1), so every input sample is written once instead of receiving
-    ``taps`` atomics from an overlap-add."""
-
-    @staticmethod
-    def forward(ctx, sig, fir_row, zero_row, poly, n):
-        taps = fir_row.shape[1]
-        half = (taps - 1) // 2
-        ctx.n, ctx.half, ctx.L, ctx.poly = n, half, sig.shape[-1], poly
-        padded = torch.nn.functional.pad(sig, (half, half))
-        c = _C.cqt1992v2_forward(padded, fir_row, zero_row, None, None, None, n, False,
-                                 _C.PAD_CONSTANT, None, 1.0, _C.FMT_COMPLEX, 0.0)
-        return c[:, 0, :, 0].contiguous()
-
-    @staticmethod
-    def backward(ctx, g):
-        n, half, L = ctx.n, ctx.half, ctx.L
-        poly, poly_zero, packed = ctx.poly          # (n, Q) time-reversed polyphase rows, zeros
-        Q = poly.shape[1]
-        Lp = L + 2 * half
-        M = (Lp + n - 1) // n                       # outputs per phase
-        T = g.shape[-1]
-        gp = torch.nn.functional.pad(g.contiguous(), (Q - 1, max(M - T, 0)))[:, : M + Q - 1]
-        # hop 1: CUDA-core kernel by default; NNAUDIO_B200_DECIM_BWD=tc runs the 8 frame phases
-        # of the tensor-core kernel instead
-        use_tc = packed is not None and os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "tc"
-        c = _C.cqt1992v2_forward(gp.contiguous(), poly, poly_zero, packed if use_tc else None, None,
-                                 None, 1, False, _C.PAD_CONSTANT, None, 1.0, _C.FMT_COMPLEX, 0.0,
-                                 path="tc" if use_tc else "simt")
-        d_padded = c[..., 0].permute(0, 2, 1).reshape(g.shape[0], M * n)   # [n*m + p] = phase p, m
-        return d_padded[:, half:half + L].contiguous(), None, None, None, None
-
-
 class _FirDecimateFn(torch.autograd.Function):
     """``nnab_fir_decimate`` / ``nnab_fir_decimate_adjoint``: one launch each way (GPU-verified round 2)."""
 
@@ -488,41 +450,11 @@ class _FirDecimateFn(torch.autograd.Function):
 
 
 def _decimate_autograd(mod, tag, sig, fir, n):
-    """Differentiable ``downsampling_by_n`` / ``_by_2`` stage of the training path.
-
-    ``NNAUDIO_B200_DECIM_BWD`` picks the adjoint:
-    ``fir`` (default) the dedicated CUDA-core FIR stage + adjoint kernel
-    (``nnab_fir_decimate`` / ``nnab_fir_decimate_adjoint``: every input sample written once, no
-    atomics), within the 1e-4 bar on every pyramid gradient case;
-    ``simt`` polyphase FIRs on the framed CUDA-core kernel; ``tc`` the same on the tensor-core kernel
-    (8 frame phases); ``ola`` a K=1 adjoint GEMM + overlap-add atomics (256 atomics per input sample),
-    whose worst dX error on the Magnitude case is just over the bar."""
-    if os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "fir":
-        return _FirDecimateFn.apply(sig, fir.detach().reshape(-1).contiguous(), int(n))
-    if os.environ.get("NNAUDIO_B200_DECIM_BWD", "fir") == "ola":
-        taps = fir.numel()
-        w_re = fir.detach().reshape(1, taps)
-        zeros = mod.__dict__.setdefault("_fir_zeros", {})
-        if tag not in zeros or zeros[tag].shape != w_re.shape or zeros[tag].device != w_re.device:
-            zeros[tag] = torch.zeros_like(w_re)
-        half = (taps - 1) // 2
-        padded = torch.nn.functional.pad(sig, (half, half))
-        c = _framed_complex_autograd(mod, tag, padded, w_re, zeros[tag], n, False, _C.PAD_CONSTANT)
-        return c[:, 0, :, 0].contiguous()
-    cache = mod.__dict__.setdefault("_decim_cache", {})
-
-    def build():
-        taps = fir.numel()
-        row = fir.detach().reshape(1, taps).contiguous()
-        Q = (taps + n - 1) // n
-        padded = torch.nn.functional.pad(row[0], (0, Q * n - taps))
-        poly = padded.reshape(Q, n).t().flip(1).contiguous()      # poly[p, k] = fir[n*(Q-1-k) + p]
-        poly_zero = torch.zeros_like(poly)
-        return row, torch.zeros_like(row), (poly, poly_zero, _C.pack_basis(poly, poly_zero))
-
-    key = (fir.data_ptr(), fir._version, int(n))
-    row, zero_row, poly = cache.setdefault(tag, PerDeviceCache()).lookup(fir.device, key, build)
-    return _DecimateFn.apply(sig, row, zero_row, poly, int(n))
+    """Differentiable ``downsampling_by_n`` / ``_by_2`` stage ``tag`` of ``mod``'s training path: the
+    dedicated CUDA-core FIR stage and its adjoint kernel (``nnab_fir_decimate`` /
+    ``nnab_fir_decimate_adjoint``: every input sample written once, no atomics), within the 1e-4 bar on
+    every pyramid gradient case.  The stage keeps no per-module state, so ``mod`` and ``tag`` only name it."""
+    return _FirDecimateFn.apply(sig, fir.detach().reshape(-1).contiguous(), int(n))
 
 
 def _pyramid_forward_autograd(mod, x, output_format, fallbacks, factor, scale, scale_all, eps):

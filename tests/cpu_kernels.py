@@ -29,13 +29,6 @@ def _framed(x, w_re, w_im, hop, center, pad_mode):
     return torch.stack((re, im), -1)
 
 
-def fir_decimate(x, fir, factor):
-    """conv1d(x, fir, stride=factor, padding=(taps-1)//2) (utils.py:73-100), float64."""
-    taps = fir.numel()
-    return torch.nn.functional.conv1d(x[:, None, :].double(), fir.reshape(1, 1, -1).double(), stride=factor,
-                                      padding=(taps - 1) // 2)[:, 0, :]
-
-
 def _scaled(c, scale, scale_all):
     if scale is not None:
         c = c * scale.double().view(1, -1, 1, 1)
@@ -145,6 +138,7 @@ def istft_forward(X, packed, window, n_fft, hop, center, length):
 
 
 def fir_decimate(x, fir, factor):
+    """conv1d(x, fir, stride=factor, padding=(taps-1)//2) (utils.py:73-100), computed in float64."""
     taps = fir.numel()
     return torch.nn.functional.conv1d(x[:, None, :].double(), fir.reshape(1, 1, -1).double(), stride=factor,
                                       padding=(taps - 1) // 2)[:, 0, :].float()

@@ -99,9 +99,10 @@ def test_folded_bank_reproduces_two_stage_reference(case, monkeypatch):
 @pytest.mark.parametrize("taps,n,L", [(256, 2, 1000), (256, 2, 1001), (256, 4, 4099), (255, 3, 777),
                                       (16, 5, 64), (9, 2, 9)])
 def test_polyphase_decimation_adjoint_equals_conv1d_autograd(taps, n, L, monkeypatch):
-    """The backward of a decimating FIR stage is computed as n interleaved stride-1 FIRs with the
-    polyphase components (no overlap-add): identical to autograd through
-    conv1d(stride=n, padding=(taps-1)//2) (utils.py:73-100), for even/odd taps and lengths."""
+    """A decimating FIR stage of the training path runs the dedicated FIR decimation forward and
+    the dedicated FIR adjoint backward, with the filter flattened and the stride and input length
+    passed through: identical to autograd through conv1d(stride=n, padding=(taps-1)//2)
+    (utils.py:73-100), for even/odd taps and lengths."""
     from nnaudio_b200.features.cqt import _decimate_autograd
 
     cpu_kernels.install(monkeypatch)

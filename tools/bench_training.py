@@ -101,7 +101,7 @@ def _pyramid(args, dev, report):
 
     report("cqt2010v2_forward_backward_dX", timed(cqt_bwd, xc, args.iters), Bc * Tc,
            note="octave-by-octave training path (7 octaves, 6 FIR stages); decimation adjoint via "
-                + os.environ.get("NNAUDIO_B200_DECIM_BWD", "simt"))
+                "the dedicated FIR-adjoint kernel")
 
 
 if __name__ == "__main__":
