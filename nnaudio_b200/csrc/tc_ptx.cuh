@@ -110,6 +110,11 @@ __device__ __forceinline__ void wgmma_commit() {
 __device__ __forceinline__ void wgmma_wait_all() {
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
+// at most `PENDING` committed groups of this warpgroup still in flight
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
+}
 
 // K-major SWIZZLE_128B shared-memory matrix descriptor (64 bf16 = 128 B per row, 8-row atoms):
 //   [0,14) start >> 4 | [16,30) LBO >> 4 (unused when swizzled) | [32,46) SBO >> 4 = 1024 B | [62,64) 1
@@ -118,21 +123,25 @@ __device__ __forceinline__ void wgmma_wait_all() {
 // start at any 128-byte row of a TMA-written block (tc_probe.cu checks this on the device).
 __device__ __forceinline__ uint32_t wg_desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint32_t wg_desc_hi() { return (1024u >> 4) | (1u << 30); }
+// K-major SWIZZLE_64B (32 bf16 = 64 B per row): SBO = 8 rows = 512 B, layout type [62,64) 2.  The low word
+// is the same; a K16 slice is still +32 B.  An operand starts at a 512-byte boundary (one swizzle atom).
+__device__ __forceinline__ uint32_t wg_desc_hi_sw64() { return (512u >> 4) | (2u << 30); }
 __device__ __forceinline__ uint64_t desc64(uint32_t lo, uint32_t hi) {
   uint64_t d;
   asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
   return d;
 }
 
-// One K block (64 = four K16 slices) of the 3-term bf16 split, x*w ~= xlo*whi + xhi*wlo + xhi*whi, for this
-// warpgroup's 64 rows: A (hi, lo planes) x B (hi, lo planes) -> d (N / 2 registers).  Arguments are the low
-// descriptor words of the four operand blocks.
-template <int N>
+// One K block (BK = 64: four K16 slices, SWIZZLE_128B; BK = 32: two, SWIZZLE_64B) of the 3-term bf16
+// split, x*w ~= xlo*whi + xhi*wlo + xhi*whi, for this warpgroup's 64 rows: A (hi, lo planes) x B (hi, lo
+// planes) -> d (N / 2 registers).  Arguments are the low descriptor words of the four operand blocks.
+template <int N, int BK = 64>
 __device__ __forceinline__ void wg_kblock_split3_n(float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                                    uint32_t b_lo, bool first_accumulates) {
-  const uint32_t hi = wg_desc_hi();
+  static_assert(BK == 64 || BK == 32, "K block is one 128-byte or 64-byte swizzled row");
+  const uint32_t hi = (BK == 64) ? wg_desc_hi() : wg_desc_hi_sw64();
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
+  for (int k = 0; k < BK / 16; ++k) {
     const uint32_t o = 2u * k;
     Wgmma<N>::mma(d, desc64(a_lo + o, hi), desc64(b_hi + o, hi), (k == 0 && !first_accumulates) ? 0u : 1u);
     Wgmma<N>::mma(d, desc64(a_hi + o, hi), desc64(b_lo + o, hi), 1u);

@@ -41,26 +41,35 @@
 
 namespace nnab {
 
-constexpr int TCB_BK = 64;
-constexpr int TCB_STAGES = 2;
+constexpr int TCB_BK = 32;          // K block: one 64-byte swizzled row per operand row
+constexpr int TCB_MAX_STAGES = 4;
 
 struct TcbParams {
   int num_m_tiles;   // 128-row tiles along M (4 * (33 - R) frames each)
   int num_n_tiles;
   int nb;            // packed bins per N tile (MMA N = 2 nb)
-  int kb_n;          // hop / 64
+  int kb_n;          // hop / TCB_BK
+  int stages;        // ring depth, TcbSmem::stages(nb)
   int64_t nv, t_slots, T;
   EpiParams epi;
 };
 
+// Dynamic shared memory: [1024-byte alignment slack][accumulator tile][stage ring][barriers].  The
+// accumulator tile has its own space, so the producer refills the ring while the epilogue reads the tile.
 struct TcbSmem {
-  static constexpr uint32_t A_BYTES = TC_BM * TCB_BK * 2;   // one plane, 128 rows
-  static constexpr uint32_t B_BYTES = 256 * TCB_BK * 2;     // one plane, re + im rows (2 nb <= 256)
-  static constexpr uint32_t STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr uint32_t BAR_OFFSET = TCB_STAGES * STAGE_BYTES;
-  static constexpr uint32_t TOTAL = BAR_OFFSET + 256 + 1024;
-  // the accumulator tile (128 rows x 2 nb fp32) reuses the stages once a tile's K range is drained
-  static_assert(TC_BM * 256 * 4 <= BAR_OFFSET, "accumulator tile does not fit the stage ring");
+  static constexpr uint32_t A_BYTES = TC_BM * TCB_BK * 2;  // one plane, 128 rows
+  static constexpr uint32_t LIMIT = 227 * 1024;            // opt-in dynamic shared memory per block
+  static constexpr uint32_t BAR_BYTES = 16 * TCB_MAX_STAGES;
+  // 128 fp32 rows of 2 nb columns, rounded up to 32 columns (acc_tile)
+  __host__ __device__ static uint32_t acc_bytes(int nb) { return TC_BM * (uint32_t)((2 * nb + 31) / 32) * 128u; }
+  // one (plane, part) box of the basis: nb rows; a multiple of 512 B, so every operand starts on an atom
+  __host__ __device__ static uint32_t part_bytes(int nb) { return (uint32_t)nb * TCB_BK * 2; }
+  __host__ __device__ static uint32_t stage_bytes(int nb) { return 2 * A_BYTES + 4 * part_bytes(nb); }
+  static int stages(int nb) {
+    const int s = (int)((LIMIT - 1024 - BAR_BYTES - acc_bytes(nb)) / stage_bytes(nb));
+    return s < TCB_MAX_STAGES ? s : TCB_MAX_STAGES;
+  }
+  static uint32_t total(int nb) { return 1024 + acc_bytes(nb) + stages(nb) * stage_bytes(nb) + BAR_BYTES; }
 };
 
 // rows of one (plane, part) slab of the packed block basis
@@ -371,67 +380,100 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
 constexpr int TCB_PARTS = 2;
 static_assert(FB_EPI_PARTS == TCB_PARTS, "fused-filterbank column ranges follow the epilogue warps");
 
+// The stage ring.  A stage holds A (hi, lo planes: four 32-row boxes each) and B (four nb-row boxes: hi re,
+// hi im, lo re, lo im); its empty barrier counts the 8 consumer warps.
+struct TcbRing {
+  uint32_t base, stage_bytes, bars;
+  int stages;
+  __device__ uint32_t stage(int s) const { return base + (uint32_t)s * stage_bytes; }
+  __device__ uint32_t full(int s) const { return bars + 8u * s; }
+  __device__ uint32_t empty(int s) const { return bars + 8u * (TCB_MAX_STAGES + s); }
+};
+
+// One tile's K loop at MMA width N = 2 nb.  Each K block is committed as one wgmma group; the stage of the
+// PREVIOUS block is released once that group has retired, so one group is always in flight.  A width fixed
+// at compile time keeps every in-flight wgmma off divergent paths (ptxas would serialise them).
+template <int N>
+__device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, int kb_n, uint32_t a_off,
+                                             uint32_t part_bytes, int lane, int& stage, uint32_t& phase) {
+  using S = TcbSmem;
+  int prev = 0;
+  for (int kb = 0; kb < kb_n; ++kb) {
+    mbar_wait(ring.full(stage), phase);
+    const uint32_t sb = ring.stage(stage);
+    const uint32_t b = sb + 2 * S::A_BYTES;
+    wgmma_fence();
+    wg_kblock_split3_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
+                                  wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes), kb != 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+    __syncwarp();
+    if (kb > 0 && lane == 0) mbar_arrive(ring.empty(prev));
+    prev = stage;
+    if (++stage == ring.stages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  __syncwarp();
+  if (lane == 0) mbar_arrive(ring.empty(prev));
+}
+
 template <int FMT, int R>
 __global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
 framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const TcbParams p) {
-  constexpr int BK = TCB_BK, STAGES = TCB_STAGES;
+  constexpr int BK = TCB_BK;
   constexpr int FW = 33 - R;  // frames per warp quarter
   using S = TcbSmem;
-  const uint32_t base = acc_tile_base();
-  const uint32_t bar_base = base + S::BAR_OFFSET;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t drained_bar = bar_base + 8u * (2 * STAGES);
+  const int nb = p.nb;
+  TcbRing ring;
+  ring.base = acc_tile_base() + S::acc_bytes(nb);
+  ring.stage_bytes = S::stage_bytes(nb);
+  ring.stages = p.stages;
+  ring.bars = ring.base + (uint32_t)p.stages * ring.stage_bytes;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
+    for (int s = 0; s < p.stages; ++s) {
+      mbar_init(ring.full(s), 1);
+      mbar_init(ring.empty(s), 8);  // one arrival per consumer warp
     }
-    mbar_init(drained_bar, 1);
     fence_barrier_init();
   }
   __syncthreads();
 
   const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int nb = p.nb;
+  const uint32_t part_bytes = S::part_bytes(nb);
 
   if (warp == TC_PRODUCER_WARP) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       prefetch_tmap(&tm_a);
       prefetch_tmap(&tm_b);
-      const uint32_t part_bytes = (uint32_t)nb * BK * 2;  // nb basis rows of one (plane, part)
       int stage = 0;
       uint32_t phase = 0;
-      int u = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++u) {
-        if (u > 0) mbar_wait(drained_bar, (uint32_t)(u - 1) & 1u);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_tile = tile / p.num_n_tiles;
         const int n_tile = tile - m_tile * p.num_n_tiles;
         const int m0 = m_tile * (4 * FW);
         const int n0 = n_tile * (nb - 2);
         for (int kb = 0; kb < p.kb_n; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sb = base + stage * S::STAGE_BYTES;
-          mbar_expect_tx(full_bar(stage), 2 * S::A_BYTES + 4 * part_bytes);
+          mbar_wait(ring.empty(stage), phase ^ 1u);
+          const uint32_t sb = ring.stage(stage);
+          const uint32_t full = ring.full(stage);
+          mbar_expect_tx(full, ring.stage_bytes);
           const int k0 = kb * BK;
 #pragma unroll
           for (int q = 0; q < 4; ++q) {  // 32-row boxes, row origins FW apart
-            tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0, m0 + q * FW, 0);
-            tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full_bar(stage), k0,
-                        m0 + q * FW, 1);
+            tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 0);
+            tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 1);
           }
-          // B rows [0, nb) = re part, [nb, 2 nb) = im part: accumulator columns of the N = 2 nb MMA
-          const uint32_t bh = sb + 2 * S::A_BYTES, bl = bh + S::B_BYTES;
-          tma_load_3d(bh, &tm_b, full_bar(stage), k0, n0, 0);
-          tma_load_3d(bh + part_bytes, &tm_b, full_bar(stage), k0, n0, 1);
-          tma_load_3d(bl, &tm_b, full_bar(stage), k0, n0, 2);
-          tma_load_3d(bl + part_bytes, &tm_b, full_bar(stage), k0, n0, 3);
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+          // B rows [0, nb) = re part, [nb, 2 nb) = im part of each plane: accumulator columns of the
+          // N = 2 nb MMA
+          const uint32_t b = sb + 2 * S::A_BYTES;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) tma_load_3d(b + (uint32_t)j * part_bytes, &tm_b, full, k0, n0, j);
+          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
         }
       }
     }
@@ -454,28 +496,21 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     const int n_tile = tile - m_tile * p.num_n_tiles;
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < p.kb_n; ++kb) {
-      mbar_wait(full_bar(stage), phase);
-      const uint32_t sb = base + stage * S::STAGE_BYTES;
-      wgmma_fence();
-      wg_kblock_split3<256>(2 * nb, acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
-                            wg_desc_lo(sb + 2 * S::A_BYTES), wg_desc_lo(sb + 2 * S::A_BYTES + S::B_BYTES),
-                            kb != 0);
-      wgmma_commit();
-      wgmma_wait_all();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(stage));
-      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    switch (2 * nb) {  // nb = 32 .. 128 in steps of 8
+#define NNAB_TCB_CASE(N) \
+  case N: tcb_mainloop<N>(acc, ring, p.kb_n, a_off, part_bytes, lane, stage, phase); break;
+      NNAB_TCB_CASE(64) NNAB_TCB_CASE(80) NNAB_TCB_CASE(96) NNAB_TCB_CASE(112) NNAB_TCB_CASE(128)
+      NNAB_TCB_CASE(144) NNAB_TCB_CASE(160) NNAB_TCB_CASE(176) NNAB_TCB_CASE(192) NNAB_TCB_CASE(208)
+      NNAB_TCB_CASE(224) NNAB_TCB_CASE(240) NNAB_TCB_CASE(256)
+#undef NNAB_TCB_CASE
+      default: break;
     }
-    consumer_sync();
+    consumer_sync();  // every warp is done reading the previous tile
     acc_store<256>(tile_addr, acc, 2 * nb, wg * 64);
     consumer_sync();
     const int64_t g = (int64_t)m_tile * (4 * FW) + quarter * FW + lane;
     epilogue_tile_block<FMT, R>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, n_tile, c_begin,
                                 c_end);
-    fence_proxy_async();
-    consumer_sync();
-    if (threadIdx.x == 0) mbar_arrive(drained_bar);
   }
 }
 
@@ -491,10 +526,10 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
   if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
     NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::LIMIT));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  framed_tcb_kernel<FMT, R><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb, prm);
+  framed_tcb_kernel<FMT, R><<<grid, TC_KERNEL_THREADS, S::total(prm.nb), stream>>>(ma, mb, prm);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -575,10 +610,10 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   const int p_rows = block_p_rows(q.F);
   CUtensorMap ma, mb;
   rc = encode_3d(&ma, planes, (uint64_t)q.hop, (uint64_t)g.rows, 2, (uint64_t)q.hop * 2,
-                 (uint64_t)g.plane_stride * 2, 64, 32, 64);
+                 (uint64_t)g.plane_stride * 2, TCB_BK, 32, TCB_BK);
   if (rc) return rc;
   rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)q.hop, (uint64_t)p_rows, 4,
-                 (uint64_t)q.hop * 2, (uint64_t)p_rows * q.hop * 2, 64, (uint32_t)nb, 64);
+                 (uint64_t)q.hop * 2, (uint64_t)p_rows * q.hop * 2, TCB_BK, (uint32_t)nb, TCB_BK);
   if (rc) return rc;
 
   TcbParams prm{};
@@ -586,7 +621,8 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.num_m_tiles = (int)ceil_div64(g.nv, frames_per_tile);
   prm.num_n_tiles = n_tiles;
   prm.nb = nb;
-  prm.kb_n = q.hop / 64;
+  prm.kb_n = q.hop / TCB_BK;
+  prm.stages = TcbSmem::stages(nb);
   prm.nv = g.nv;
   prm.t_slots = g.t_slots;
   prm.T = q.T;
