@@ -24,6 +24,11 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
 (signatures, buffers bit-identical for 49 + 7 configurations, attribute surface, exception types, outputs ≤1e-4). What differs:
 
 * inputs must be **CUDA float32** tensors on an H100 (sm_90a); anything else raises — there is no CPU fallback;
+* exception: a waveform passed to `forward` (every module but `iSTFT` / `Griffin_Lim`, whose inputs are spectrograms)
+  may also be **bfloat16 or float16**.  The output is float32 whatever the input dtype, with fp32-grade accuracy on
+  the given samples: the result equals that of `x.float()` (on the tensor-core routes bit for bit).  The reference
+  raises for a half waveform outside `torch.autocast` and returns half inside it.  Inference reads the 16-bit tensor
+  as is; the autograd path upcasts once and returns `x.grad` in the input's dtype;
 * multi-GPU: one process per GPU (`nnaudio_b200.parallel.BatchShardedTransform`, INTEGRATION.md) is the fast path;
   `torch.nn.DataParallel`, the reference's own mode, also works (per-device launch attributes and caches);
 * `Griffin_Lim.forward(S, rand_phase=None)` takes an optional initial phase (reproducible runs); `device` moves the

@@ -68,6 +68,15 @@ typedef enum nnab_status {
 #define NNAB_PATH_SIMT 1
 #define NNAB_PATH_TCGEN05 2
 
+/* Sample type of the waveform `x` of the *_forward_ex entry points.  Everything else (bases, filterbanks,
+ * outputs) stays fp32, and the result is the fp32 transform of the given samples: the tensor-core
+ * pre-pass converts each sample to fp32 exactly before splitting it.  Plans that would read `x` as
+ * fp32 directly (the SIMT kernels, the per-octave CQT pyramid) return NNAB_EUNSUPPORTED for a 16-bit
+ * `x` before anything is enqueued; the caller may then upcast and call again. */
+#define NNAB_DTYPE_F32 0
+#define NNAB_DTYPE_BF16 1
+#define NNAB_DTYPE_F16 2
+
 int nnab_abi_version(void);
 const char* nnab_strerror(int status);
 /* Last CUDA error string recorded by a call that returned NNAB_ECUDA (thread local). */
@@ -134,6 +143,13 @@ int nnab_stft_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch,
                       int n_fft, int F, int hop, int center, int pad_mode,
                       int out_format, float sqrt_eps, float* out, int64_t T,
                       void* workspace, size_t ws_bytes, int path, void* stream);
+/* The same for a waveform of sample type x_dtype (NNAB_DTYPE_*); x_pitch stays in samples.
+ * nnab_stft_forward is this call with NNAB_DTYPE_F32; so are the other *_forward / *_forward_ex pairs. */
+int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                         const float* wcos, const float* wsin, const void* packed,
+                         int n_fft, int F, int hop, int center, int pad_mode,
+                         int out_format, float sqrt_eps, float* out, int64_t T,
+                         void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
  * Banded filterbank table (tensor-core path): for every FFT bin the (at most two)
@@ -162,6 +178,12 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
                                  float sqrt_eps, float power, const float* fb, int n_fb,
                                  const void* fb_table, float* out, int64_t T,
                                  void* workspace, size_t ws_bytes, int path, void* stream);
+int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                                    const float* wcos, const float* wsin, const void* packed,
+                                    int n_fft, int F, int hop, int center, int pad_mode,
+                                    float sqrt_eps, float power, const float* fb, int n_fb,
+                                    const void* fb_table, float* out, int64_t T,
+                                    void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
  * MFCC.forward — features/mel.py:309-326 (= mel -> _power_to_db :263-279 ->
@@ -178,6 +200,13 @@ int nnab_mfcc_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch,
                       const void* fb_table, float amin, float ref, float top_db,
                       const float* dct, int n_mfcc, float* out, int64_t T,
                       void* workspace, size_t ws_bytes, int path, void* stream);
+int nnab_mfcc_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                         const float* wcos, const float* wsin, const void* packed,
+                         int n_fft, int F, int hop, int center, int pad_mode,
+                         float sqrt_eps, float power, const float* mel_basis, int n_mels,
+                         const void* fb_table, float amin, float ref, float top_db,
+                         const float* dct, int n_mfcc, float* out, int64_t T,
+                         void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
  * CQT1992v2.forward — features/cqt.py:712-780.
@@ -197,6 +226,13 @@ int nnab_cqt1992v2_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch
                            const float* scale, float scale_all, int out_format,
                            float sqrt_eps, float* out, int64_t T,
                            void* workspace, size_t ws_bytes, int path, void* stream);
+int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                              const float* k_real, const float* k_imag, const void* packed,
+                              const int32_t* h_k_begin, const int32_t* h_k_end,
+                              int n_bins, int width, int hop, int center, int pad_mode,
+                              const float* scale, float scale_all, int out_format,
+                              float sqrt_eps, float* out, int64_t T,
+                              void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
  * CQT2010v2.forward / VQT.forward — features/cqt.py:1070-1139,
@@ -256,6 +292,18 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
                              const float* scale, float scale_all, int out_format,
                              float sqrt_eps, float* out, int64_t T,
                              void* workspace, size_t ws_bytes, int path, void* stream);
+/* 16-bit x: the all-tensor-core plans only (every packed input present, path != SIMT); the
+ * per-octave plan decimates x on the CUDA cores and returns NNAB_EUNSUPPORTED. */
+int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                                int n_octaves, const float* const* h_k_real,
+                                const float* const* h_k_imag, const void* const* h_packed,
+                                const int32_t* h_widths,
+                                int n_filters, const float* lowpass, const void* lowpass_packed,
+                                const float* early_filter, const void* early_packed,
+                                int early_factor, int hop, int pad_mode, int n_bins,
+                                const float* scale, float scale_all, int out_format,
+                                float sqrt_eps, float* out, int64_t T,
+                                void* workspace, size_t ws_bytes, int path, void* stream);
 
 /* ------------------------------------------------------------------------- *
  * STFT.inverse / iSTFT.forward — features/stft.py:15-63 (inverse_stft), :318-356,

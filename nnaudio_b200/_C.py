@@ -3,7 +3,7 @@
 PyTorch is used only for device memory and the current CUDA stream; every
 compute call goes through the C ABI with raw device pointers.  There is no
 CPU / eager fallback: if the library is missing, or a tensor is not a CUDA
-fp32 tensor, the call fails loudly.
+fp32 tensor (a waveform may also be bfloat16 or float16), the call fails loudly.
 """
 from __future__ import annotations
 
@@ -19,6 +19,11 @@ LIB_PATH = os.path.join(_HERE, "libnnab.so")
 PAD_REFLECT, PAD_CONSTANT = 0, 1
 FMT_MAGNITUDE, FMT_COMPLEX, FMT_PHASE_ANGLE, FMT_PHASE_UNIT = 0, 1, 2, 3
 PATH_AUTO, PATH_SIMT, PATH_TCGEN05 = 0, 1, 2
+DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2
+EUNSUPPORTED = -6
+
+# sample types of the waveform the forward entry points read (NNAB_DTYPE_*)
+_WAVE_DTYPES = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16, torch.float16: DTYPE_F16}
 
 # "tc" = the wgmma/TMA tensor-core kernels; "tcgen05" (the C constant's name) means the same
 _PATH_NAMES = {"auto": PATH_AUTO, "simt": PATH_SIMT, "tc": PATH_TCGEN05, "tcgen05": PATH_TCGEN05}
@@ -111,6 +116,11 @@ SIGNATURES = {
          c_int, c_int, _P, c_float, c_int, c_float, _P, c_int64, _P, c_size_t, c_int, _P],
     ),
 }
+# the *_ex forward entry points: the same arguments, (x, x_dtype) in place of x
+for _name in ("nnab_stft_forward", "nnab_stft_filterbank_forward", "nnab_mfcc_forward",
+              "nnab_cqt1992v2_forward", "nnab_cqt_pyramid_forward"):
+    _res, _args = SIGNATURES[_name]
+    SIGNATURES[_name + "_ex"] = (_res, [_P, c_int] + _args[1:])
 
 _lib = None
 
@@ -203,6 +213,20 @@ def _dev_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     return t
 
 
+def _dev_wave(t: torch.Tensor, name: str) -> torch.Tensor:
+    """``_dev_f32`` for a waveform: float32, bfloat16 or float16."""
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor")
+    if not t.is_cuda:
+        raise RuntimeError(
+            f"{name} is on {t.device}: nnaudio_b200 runs only on CUDA (sm_90a) tensors; "
+            "there is no CPU fallback"
+        )
+    if t.dtype not in _WAVE_DTYPES:
+        raise RuntimeError(f"{name} must be float32, bfloat16 or float16, got {t.dtype}")
+    return t
+
+
 def _ptr(t):
     return c_void_p(t.data_ptr()) if t is not None else None
 
@@ -272,15 +296,37 @@ def _batch_chunked(fn):
     return wrapper
 
 
-def _rows(x: torch.Tensor):
-    """(B, L) view with unit inner stride -> (tensor, B, L, pitch)."""
-    x = _dev_f32(x, "x")
+def _as_rows(x: torch.Tensor):
     if x.dim() != 2:
         raise ValueError("internal: expected (B, L)")
     if x.stride(-1) != 1 or (x.shape[0] > 1 and x.stride(0) < x.shape[1]):
         x = x.contiguous()
     pitch = x.stride(0) if x.shape[0] > 1 else x.shape[1]
     return x, x.shape[0], x.shape[1], pitch
+
+
+def _rows(x: torch.Tensor):
+    """(B, L) fp32 view with unit inner stride -> (tensor, B, L, pitch)."""
+    return _as_rows(_dev_f32(x, "x"))
+
+
+def _wave_rows(x: torch.Tensor):
+    """``_rows`` of a waveform in any sample type the forward entry points take
+    -> (tensor, B, L, pitch, NNAB dtype).  A 16-bit waveform is passed on as is (no fp32 copy)."""
+    x, B, L, pitch = _as_rows(_dev_wave(x, "x"))
+    return x, B, L, pitch, _WAVE_DTYPES[x.dtype]
+
+
+def _call_wave(call, x, pitch, dtype, strict_dtype):
+    """``call(x, pitch, dtype)`` -> status of a forward entry point.  When the plan the library chose
+    cannot read a 16-bit waveform (NNAB_EUNSUPPORTED, returned before anything is enqueued: the SIMT
+    kernels, the per-octave CQT pyramid), run it once more on the float32 upcast; ``strict_dtype``
+    (tests) turns that into an error instead, so a 16-bit route that is missing cannot hide."""
+    rc = call(x, pitch, dtype)
+    if rc == EUNSUPPORTED and dtype != DTYPE_F32 and not strict_dtype:
+        x, _, _, pitch = _as_rows(x.float())
+        rc = call(x, pitch, DTYPE_F32)
+    return rc
 
 
 # --------------------------------------------------------------------------- #
@@ -366,11 +412,12 @@ def build_filterbank_table(fb: torch.Tensor):
 # --------------------------------------------------------------------------- #
 # forward calls
 # --------------------------------------------------------------------------- #
+# x of the forward calls: a float32, bfloat16 or float16 (B, L) CUDA tensor; the output is float32.
 @_batch_chunked
 def stft_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format, sqrt_eps,
-                 path=None):
+                 path=None, strict_dtype=False):
     L = lib()
-    x, B, Ln, pitch = _rows(x)
+    x, B, Ln, pitch, dt = _wave_rows(x)
     F = wcos.shape[0]
     pad = n_fft // 2 if center else 0
     T = (Ln + 2 * pad - n_fft) // hop + 1
@@ -380,18 +427,19 @@ def stft_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format
     with torch.cuda.device(x.device):
         ws, wsb = _workspace(L.nnab_stft_workspace_bytes(B, Ln, n_fft, F, hop, int(center), path),
                              x.device)
-        rc = L.nnab_stft_forward(_ptr(x), B, Ln, pitch, _ptr(wcos), _ptr(wsin), _ptr(packed),
-                                 n_fft, F, hop, int(center), pad_mode, out_format, sqrt_eps,
-                                 _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device))
-    _check(rc, "nnab_stft_forward")
+        rc = _call_wave(lambda xs, p, d: L.nnab_stft_forward_ex(
+            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center),
+            pad_mode, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)),
+            x, pitch, dt, strict_dtype)
+    _check(rc, "nnab_stft_forward_ex")
     return out
 
 
 @_batch_chunked
 def stft_filterbank_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
-                            fb, fb_table=None, path=None):
+                            fb, fb_table=None, path=None, strict_dtype=False):
     L = lib()
-    x, B, Ln, pitch = _rows(x)
+    x, B, Ln, pitch, dt = _wave_rows(x)
     F = wcos.shape[0]
     n_fb = fb.shape[0]
     pad = n_fft // 2 if center else 0
@@ -403,19 +451,19 @@ def stft_filterbank_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode,
             L.nnab_filterbank_workspace_bytes(B, Ln, n_fft, F, hop, int(center), n_fb, path,
                                               int(fb_table is not None)),
             x.device)
-        rc = L.nnab_stft_filterbank_forward(
-            _ptr(x), B, Ln, pitch, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
+        rc = _call_wave(lambda xs, p, d: L.nnab_stft_filterbank_forward_ex(
+            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
             int(center), pad_mode, sqrt_eps, power, _ptr(fb), n_fb, _ptr(fb_table), _ptr(out), T,
-            _ptr(ws), wsb, path, _stream(x.device))
-    _check(rc, "nnab_stft_filterbank_forward")
+            _ptr(ws), wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
+    _check(rc, "nnab_stft_filterbank_forward_ex")
     return out
 
 
 @_batch_chunked
 def mfcc_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power, mel_basis,
-                 amin, ref, top_db, dct, fb_table=None, path=None):
+                 amin, ref, top_db, dct, fb_table=None, path=None, strict_dtype=False):
     L = lib()
-    x, B, Ln, pitch = _rows(x)
+    x, B, Ln, pitch, dt = _wave_rows(x)
     F = wcos.shape[0]
     n_mels = mel_basis.shape[0]
     n_mfcc = dct.shape[0]
@@ -427,21 +475,21 @@ def mfcc_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, 
         ws, wsb = _workspace(
             L.nnab_mfcc_workspace_bytes(B, Ln, n_fft, F, hop, int(center), n_mels, path,
                                         int(fb_table is not None)), x.device)
-        rc = L.nnab_mfcc_forward(
-            _ptr(x), B, Ln, pitch, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
+        rc = _call_wave(lambda xs, p, d: L.nnab_mfcc_forward_ex(
+            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
             int(center), pad_mode, sqrt_eps, power, _ptr(mel_basis), n_mels, _ptr(fb_table), amin, ref,
             -1.0 if top_db is None else float(top_db), _ptr(dct), n_mfcc, _ptr(out), T, _ptr(ws),
-            wsb, path, _stream(x.device))
-    _check(rc, "nnab_mfcc_forward")
+            wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
+    _check(rc, "nnab_mfcc_forward_ex")
     return out
 
 
 @_batch_chunked
 def cqt1992v2_forward(x, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode, scale,
-                      scale_all, out_format, sqrt_eps, path=None):
+                      scale_all, out_format, sqrt_eps, path=None, strict_dtype=False):
     """k_begin / k_end: host int32 numpy arrays (per-bin support) or None."""
     L = lib()
-    x, B, Ln, pitch = _rows(x)
+    x, B, Ln, pitch, dt = _wave_rows(x)
     n_bins, width = k_real.shape
     pad = width // 2 if center else 0
     T = (Ln + 2 * pad - width) // hop + 1
@@ -454,22 +502,22 @@ def cqt1992v2_forward(x, k_real, k_imag, packed, k_begin, k_end, hop, center, pa
         ws, wsb = _workspace(
             L.nnab_cqt1992v2_workspace_bytes(B, Ln, width, n_bins, hop, int(center), path),
             x.device)
-        rc = L.nnab_cqt1992v2_forward(
-            _ptr(x), B, Ln, pitch, _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins,
+        rc = _call_wave(lambda xs, p, d: L.nnab_cqt1992v2_forward_ex(
+            _ptr(xs), d, B, Ln, p, _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins,
             width, hop, int(center), pad_mode, _ptr(scale), scale_all, out_format, sqrt_eps,
-            _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device))
-    _check(rc, "nnab_cqt1992v2_forward")
+            _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
+    _check(rc, "nnab_cqt1992v2_forward_ex")
     return out
 
 
 @_batch_chunked
 def cqt_pyramid_forward(x, banks_real, banks_imag, packed, lowpass, lowpass_packed, early_filter,
                         early_packed, early_factor, hop, pad_mode, n_bins, scale, scale_all,
-                        out_format, sqrt_eps, T, path=None):
+                        out_format, sqrt_eps, T, path=None, strict_dtype=False):
     """banks_*: lists (octave 0 = top) of (n_filters, width_i) fp32 CUDA tensors;
     packed: list of packed-basis tensors (or None entries) per octave."""
     L = lib()
-    x, B, Ln, pitch = _rows(x)
+    x, B, Ln, pitch, dt = _wave_rows(x)
     n_oct = len(banks_real)
     n_filters = banks_real[0].shape[0]
     re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
@@ -484,12 +532,13 @@ def cqt_pyramid_forward(x, banks_real, banks_imag, packed, lowpass, lowpass_pack
         ws, wsb = _workspace(
             L.nnab_cqt_pyramid_workspace_bytes(B, Ln, n_oct, early_factor, max_width, hop, path),
             x.device)
-        rc = L.nnab_cqt_pyramid_forward(
-            _ptr(x), B, Ln, pitch, n_oct, re_arr, im_arr, pk_arr, widths, n_filters,
+        rc = _call_wave(lambda xs, p, d: L.nnab_cqt_pyramid_forward_ex(
+            _ptr(xs), d, B, Ln, p, n_oct, re_arr, im_arr, pk_arr, widths, n_filters,
             _ptr(lowpass), _ptr(lowpass_packed), _ptr(early_filter), _ptr(early_packed),
             early_factor, hop, pad_mode, n_bins, _ptr(scale),
-            scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device))
-    _check(rc, "nnab_cqt_pyramid_forward")
+            scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)),
+            x, pitch, dt, strict_dtype)
+    _check(rc, "nnab_cqt_pyramid_forward_ex")
     return out
 
 

@@ -91,7 +91,8 @@ constexpr int FB_STEP_PAD = 160;  // entries past F (a tile's last chunk may ove
 constexpr int FB_EPI_PARTS = 2;
 
 struct FramedProblem {
-  const float* x;      // (B, L) rows, pitch x_pitch
+  const void* x;       // (B, L) rows, pitch x_pitch samples of type x_dtype
+  int x_dtype;         // NNAB_DTYPE_*: only the pad / split pre-pass reads 16-bit samples, the SIMT kernel fp32
   int64_t B, L, x_pitch;
   const float* w_re;   // (F, K)
   const float* w_im;   // (F, K)
@@ -141,13 +142,14 @@ int tc_pack_basis_layout(const float* w_re, const float* w_im, int F, int K, int
 // split-signal geometry / helpers for callers that manage the planes themselves (pyramid)
 void tc_split_geometry(int64_t B, int64_t L, int K, int hop, int pad, int64_t* t_slots,
                        int64_t* plane_stride, int* hop_eff);
-int tc_pad_split(const float* x, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
+// (x: samples of type x_dtype, NNAB_DTYPE_*; the planes equal those of the samples converted to fp32)
+int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
                  int pad_mode, void* planes, cudaStream_t stream);
-int tc_pad_split_ex(const float* x, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
+int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
                     int64_t clip_pitch, int64_t plane_stride, void* planes, cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
                   int64_t keep_hi, cudaStream_t stream);
-int tc_pad_split2(const float* x, int64_t B, int64_t L, int64_t x_pitch,
+int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
                   int K_a, int hop_a, int pad_a, int mode_a, void* planes_a,
                   int K_b, int hop_b, int pad_b, int mode_b, void* planes_b, cudaStream_t stream);
 int tc_zero_margins(void* planes, int64_t B, int64_t L, int K, int hop, int pad, int64_t keep_lo,

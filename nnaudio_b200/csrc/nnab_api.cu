@@ -36,9 +36,13 @@ static inline int64_t frames_of(int64_t L, int K, int hop, int pad) {
   return span < 0 ? 0 : span / hop + 1;
 }
 
-static int check_common(const float* x, int64_t B, int64_t L, int64_t x_pitch, int K, int F,
+static bool dtype_ok(int x_dtype) {
+  return x_dtype == NNAB_DTYPE_F32 || x_dtype == NNAB_DTYPE_BF16 || x_dtype == NNAB_DTYPE_F16;
+}
+
+static int check_common(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int F,
                         int hop, int pad, int pad_mode, int64_t T) {
-  if (x == nullptr || B < 0 || L <= 0 || x_pitch < L || K <= 0 || F <= 0 || hop <= 0)
+  if (x == nullptr || !dtype_ok(x_dtype) || B < 0 || L <= 0 || x_pitch < L || K <= 0 || F <= 0 || hop <= 0)
     return NNAB_EINVAL;
   if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
   // nn.ReflectionPad1d needs pad < L; callers raise the reference's exception first.
@@ -255,8 +259,16 @@ int nnab_stft_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
                       const float* wsin, const void* packed, int n_fft, int F, int hop,
                       int center, int pad_mode, int out_format, float sqrt_eps, float* out,
                       int64_t T, void* workspace, size_t ws_bytes, int path, void* stream) {
+  return nnab_stft_forward_ex(x, NNAB_DTYPE_F32, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, center,
+                              pad_mode, out_format, sqrt_eps, out, T, workspace, ws_bytes, path, stream);
+}
+
+int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, const float* wcos,
+                         const float* wsin, const void* packed, int n_fft, int F, int hop,
+                         int center, int pad_mode, int out_format, float sqrt_eps, float* out,
+                         int64_t T, void* workspace, size_t ws_bytes, int path, void* stream) {
   const int pad = center ? n_fft / 2 : 0;
-  int rc = check_common(x, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
+  int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
   if (rc) return rc;
   if (wcos == nullptr || wsin == nullptr || out == nullptr) return NNAB_EINVAL;
   if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
@@ -264,7 +276,7 @@ int nnab_stft_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
     return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
   FramedProblem p{};
-  p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
   p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
   p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
   p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
@@ -373,13 +385,13 @@ size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, i
   return n;
 }
 
-static int power_spectrogram(const float* x, int64_t B, int64_t L, int64_t x_pitch,
+static int power_spectrogram(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
                              const float* wcos, const float* wsin, const void* packed,
                              int n_fft, int F, int hop, int pad, int pad_mode, float sqrt_eps,
                              float power, float* P, int64_t T, void* tc_ws, size_t tc_ws_bytes,
                              int path, cudaStream_t stream) {
   FramedProblem p{};
-  p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
   p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
   p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
   p.fmt = FMT_POWER; p.eps = sqrt_eps; p.power = power; p.out = P; p.T = T;
@@ -393,8 +405,19 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
                                  float sqrt_eps, float power, const float* fb, int n_fb,
                                  const void* fb_table, float* out, int64_t T, void* workspace,
                                  size_t ws_bytes, int path, void* stream) {
+  return nnab_stft_filterbank_forward_ex(x, NNAB_DTYPE_F32, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop,
+                                         center, pad_mode, sqrt_eps, power, fb, n_fb, fb_table, out, T,
+                                         workspace, ws_bytes, path, stream);
+}
+
+int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                                    const float* wcos, const float* wsin, const void* packed,
+                                    int n_fft, int F, int hop, int center, int pad_mode,
+                                    float sqrt_eps, float power, const float* fb, int n_fb,
+                                    const void* fb_table, float* out, int64_t T, void* workspace,
+                                    size_t ws_bytes, int path, void* stream) {
   const int pad = center ? n_fft / 2 : 0;
-  int rc = check_common(x, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
+  int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
   if (rc) return rc;
   if (wcos == nullptr || wsin == nullptr || fb == nullptr || out == nullptr || n_fb <= 0)
     return NNAB_EINVAL;
@@ -403,7 +426,7 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
   bool fused = fused_fbank(path, packed, fb_table, n_fft, hop);
   if (fused) {
     FramedProblem p{};
-    p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+    p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
     p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
     p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
     p.fmt = FMT_FBANK; p.eps = sqrt_eps; p.power = power; p.out = out; p.T = T;
@@ -434,7 +457,7 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
     const int64_t plane_stride = fp.rows * fp.kp;
     // 1. STFT -> |X| ** power as operand planes (block-partial kernel, FMT_PLANES)
     FramedProblem p{};
-    p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+    p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
     p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
     p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
     p.fmt = FMT_PLANES; p.eps = sqrt_eps; p.power = power; p.out = reinterpret_cast<float*>(planes); p.T = T;
@@ -463,7 +486,7 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
   }
   float* P = (float*)workspace;
   const size_t pb = power_bytes(B, F, T);
-  rc = power_spectrogram(x, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, pad, pad_mode,
+  rc = power_spectrogram(x, x_dtype, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, pad, pad_mode,
                          sqrt_eps, power, P, T, (char*)workspace + pb, ws_bytes - pb, path, s);
   if (rc) return rc;
   return launch_filterbank(P, fb, B, F, T, n_fb, out, s);
@@ -489,8 +512,19 @@ int nnab_mfcc_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
                       const float* mel_basis, int n_mels, const void* fb_table, float amin,
                       float ref, float top_db, const float* dct, int n_mfcc, float* out,
                       int64_t T, void* workspace, size_t ws_bytes, int path, void* stream) {
+  return nnab_mfcc_forward_ex(x, NNAB_DTYPE_F32, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, center,
+                              pad_mode, sqrt_eps, power, mel_basis, n_mels, fb_table, amin, ref, top_db, dct,
+                              n_mfcc, out, T, workspace, ws_bytes, path, stream);
+}
+
+int nnab_mfcc_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, const float* wcos,
+                         const float* wsin, const void* packed, int n_fft, int F, int hop,
+                         int center, int pad_mode, float sqrt_eps, float power,
+                         const float* mel_basis, int n_mels, const void* fb_table, float amin,
+                         float ref, float top_db, const float* dct, int n_mfcc, float* out,
+                         int64_t T, void* workspace, size_t ws_bytes, int path, void* stream) {
   const int pad = center ? n_fft / 2 : 0;
-  int rc = check_common(x, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
+  int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
   if (rc) return rc;
   if (wcos == nullptr || wsin == nullptr || mel_basis == nullptr || dct == nullptr ||
       out == nullptr || n_mels <= 0 || n_mfcc <= 0 || !(amin > 0.f))
@@ -502,9 +536,9 @@ int nnab_mfcc_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
       align_up(nnab_filterbank_workspace_bytes(B, L, n_fft, F, hop, center, n_mels, path, 0), 256);
   float* mel = (float*)((char*)workspace + fbw);
   unsigned int* scratch = (unsigned int*)((char*)workspace + fbw + mel_bytes(B, n_mels, T));
-  rc = nnab_stft_filterbank_forward(x, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, center,
-                                    pad_mode, sqrt_eps, power, mel_basis, n_mels, fb_table, mel,
-                                    T, workspace, fbw, path, stream);
+  rc = nnab_stft_filterbank_forward_ex(x, x_dtype, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, center,
+                                       pad_mode, sqrt_eps, power, mel_basis, n_mels, fb_table, mel,
+                                       T, workspace, fbw, path, stream);
   if (rc) return rc;
   return launch_mfcc_tail(mel, B, n_mels, T, amin, ref, top_db, dct, n_mfcc, out, scratch,
                           (cudaStream_t)stream);
@@ -526,8 +560,20 @@ int nnab_cqt1992v2_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch
                            float scale_all, int out_format, float sqrt_eps, float* out,
                            int64_t T, void* workspace, size_t ws_bytes, int path,
                            void* stream) {
+  return nnab_cqt1992v2_forward_ex(x, NNAB_DTYPE_F32, B, L, x_pitch, k_real, k_imag, packed, h_k_begin,
+                                   h_k_end, n_bins, width, hop, center, pad_mode, scale, scale_all, out_format,
+                                   sqrt_eps, out, T, workspace, ws_bytes, path, stream);
+}
+
+int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                              const float* k_real, const float* k_imag, const void* packed,
+                              const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins,
+                              int width, int hop, int center, int pad_mode, const float* scale,
+                              float scale_all, int out_format, float sqrt_eps, float* out,
+                              int64_t T, void* workspace, size_t ws_bytes, int path,
+                              void* stream) {
   const int pad = center ? width / 2 : 0;
-  int rc = check_common(x, B, L, x_pitch, width, n_bins, hop, pad, pad_mode, T);
+  int rc = check_common(x, x_dtype, B, L, x_pitch, width, n_bins, hop, pad, pad_mode, T);
   if (rc) return rc;
   if (k_real == nullptr || k_imag == nullptr || out == nullptr) return NNAB_EINVAL;
   if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
@@ -535,7 +581,7 @@ int nnab_cqt1992v2_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch
     return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
   FramedProblem p{};
-  p.x = x; p.B = B; p.L = L; p.x_pitch = x_pitch;
+  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
   p.w_re = k_real; p.w_im = k_imag; p.F = n_bins; p.K = width; p.hop = hop;
   p.pad = pad; p.pad_mode = pad_mode; p.scale = scale; p.scale_all = scale_all;
   p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
@@ -773,7 +819,7 @@ size_t nnab_cqt_pyramid_workspace_bytes(int64_t B, int64_t L, int n_octaves, int
 
 // Arguments of one nnab_cqt_pyramid_forward call, shared by its three plans (same order as the call's).
 struct PyramidCall {
-  const float* x; int64_t B, L, x_pitch; int n_octaves;
+  const void* x; int x_dtype; int64_t B, L, x_pitch; int n_octaves;
   const float* const* k_real; const float* const* k_imag; const void* const* packed; const int32_t* widths;
   int n_filters; const float* lowpass; const void* lowpass_packed; const void* early_packed;
   int early_factor, hop, pad_mode, n_bins; const float* scale; float scale_all; int out_format; float sqrt_eps;
@@ -804,9 +850,10 @@ static FramedProblem octave2_problem(const PyramidCall& c, const Lvl2& l, int i)
     p.presplit = c.ws + l.pc;
     p.presplit_t_slots = l.t_slots;
     p.presplit_plane_stride = l.plane;
+  } else if (i == 0) {  // the caller's waveform
+    p.x = c.x; p.x_dtype = c.x_dtype; p.x_pitch = c.x_pitch;
   } else {
-    p.x = (i == 0) ? c.x : (const float*)(c.ws + l.y32);
-    p.x_pitch = (i == 0) ? c.x_pitch : l.y32_pitch;
+    p.x = c.ws + l.y32; p.x_pitch = l.y32_pitch;
   }
   return p;
 }
@@ -837,9 +884,9 @@ static int pyramid_fused2(const PyramidCall& c, const Lvl2* lv, size_t scratch_o
   const size_t scratch_bytes = c.ws_bytes - 256 - scratch_off;
   int rc;
 
-  // level 0: the caller's fp32 waveform -> planes (one pass; writes the whole clip slot)
+  // level 0: the caller's waveform -> planes (one pass; writes the whole clip slot)
   if (lv[0].planes) {
-    rc = tc_pad_split_ex(c.x, B, c.L, c.x_pitch, lv[0].pad, lv[0].mode, lv[0].pitch, lv[0].plane,
+    rc = tc_pad_split_ex(c.x, c.x_dtype, B, c.L, c.x_pitch, lv[0].pad, lv[0].mode, lv[0].pitch, lv[0].plane,
                          ws + lv[0].pc, s);
     if (rc) return rc;
   }
@@ -886,9 +933,9 @@ static FramedProblem octave1_problem(const PyramidCall& c, const PyrLevel& l, in
   if (l.presplit) {
     p.presplit = c.ws + l.pc;
   } else if (i == 0 && c.early_factor <= 1) {  // level 0 is the caller's waveform
-    p.x = c.x; p.x_pitch = c.x_pitch;
+    p.x = c.x; p.x_dtype = c.x_dtype; p.x_pitch = c.x_pitch;
   } else {
-    p.x = (const float*)(c.ws + l.y32); p.x_pitch = l.y32_pitch;
+    p.x = c.ws + l.y32; p.x_pitch = l.y32_pitch;
   }
   return p;
 }
@@ -963,24 +1010,24 @@ static int pyramid_fused(const PyramidCall& c, const PyrLevel* lv, size_t pf_ear
 
   // ---- level 0 ------------------------------------------------------------------------
   if (c.early_factor > 1) {
-    rc = tc_pad_split(c.x, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, c.early_factor), 128 * c.early_factor,
-                      FIR_OFF, NNAB_PAD_CONSTANT, ws + pf_early, s);
+    rc = tc_pad_split(c.x, c.x_dtype, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, c.early_factor),
+                      128 * c.early_factor, FIR_OFF, NNAB_PAD_CONSTANT, ws + pf_early, s);
     if (rc) return rc;
     if ((rc = fir_stage(ws + pf_early, c.L, c.early_factor, c.early_packed, lv[0]))) return rc;
   } else {
     if (lv[0].pc != SIZE_MAX && lv[0].pf != SIZE_MAX) {
       // one pass over x: reflect-padded copy for the octave CQT + zero-margin copy for the FIR
-      rc = tc_pad_split2(c.x, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
+      rc = tc_pad_split2(c.x, c.x_dtype, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
                          ws + lv[0].pc, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, NNAB_PAD_CONSTANT,
                          ws + lv[0].pf, s);
       if (rc) return rc;
     } else if (lv[0].pc != SIZE_MAX) {
-      rc = tc_pad_split(c.x, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
+      rc = tc_pad_split(c.x, c.x_dtype, B, c.L, c.x_pitch, lv[0].width, lv[0].hop, lv[0].pad, lv[0].mode,
                         ws + lv[0].pc, s);
       if (rc) return rc;
     } else if (lv[0].pf != SIZE_MAX) {
-      rc = tc_pad_split(c.x, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, NNAB_PAD_CONSTANT,
-                        ws + lv[0].pf, s);
+      rc = tc_pad_split(c.x, c.x_dtype, B, c.L, c.x_pitch, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF,
+                        NNAB_PAD_CONSTANT, ws + lv[0].pf, s);
       if (rc) return rc;
     }
   }
@@ -1007,7 +1054,22 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
                              const float* scale, float scale_all, int out_format, float sqrt_eps,
                              float* out, int64_t T, void* workspace, size_t ws_bytes, int path,
                              void* stream) {
-  if (x == nullptr || out == nullptr || h_k_real == nullptr || h_k_imag == nullptr ||
+  return nnab_cqt_pyramid_forward_ex(x, NNAB_DTYPE_F32, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed,
+                                     h_widths, n_filters, lowpass, lowpass_packed, early_filter, early_packed,
+                                     early_factor, hop, pad_mode, n_bins, scale, scale_all, out_format,
+                                     sqrt_eps, out, T, workspace, ws_bytes, path, stream);
+}
+
+int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                                int n_octaves, const float* const* h_k_real, const float* const* h_k_imag,
+                                const void* const* h_packed, const int32_t* h_widths, int n_filters,
+                                const float* lowpass, const void* lowpass_packed,
+                                const float* early_filter, const void* early_packed,
+                                int early_factor, int hop, int pad_mode, int n_bins,
+                                const float* scale, float scale_all, int out_format, float sqrt_eps,
+                                float* out, int64_t T, void* workspace, size_t ws_bytes, int path,
+                                void* stream) {
+  if (x == nullptr || !dtype_ok(x_dtype) || out == nullptr || h_k_real == nullptr || h_k_imag == nullptr ||
       h_widths == nullptr || lowpass == nullptr || B < 0 || L <= 0 || x_pitch < L ||
       n_octaves <= 0 || n_filters <= 0 || hop <= 0 || n_bins <= 0 || early_factor < 1)
     return NNAB_EINVAL;
@@ -1024,7 +1086,7 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
       nnab_cqt_pyramid_workspace_bytes(B, L, n_octaves, early_factor, max_width, hop, path);
   if (need > 0 && (workspace == nullptr || ws_bytes < need)) return NNAB_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
-  const PyramidCall c{x, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed, h_widths, n_filters,
+  const PyramidCall c{x, x_dtype, B, L, x_pitch, n_octaves, h_k_real, h_k_imag, h_packed, h_widths, n_filters,
                       lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
                       scale_all, out_format, sqrt_eps, out, T,
                       (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255), ws_bytes, s};
@@ -1052,18 +1114,20 @@ int nnab_cqt_pyramid_forward(const float* x, int64_t B, int64_t L, int64_t x_pit
   }
 
   // ---- per-octave path: CUDA-core FIR stages, octaves on either kernel family -----------
+  // (its FIR stages read the caller's waveform as fp32)
+  if (x_dtype != NNAB_DTYPE_F32) return NNAB_EUNSUPPORTED;
   const size_t level_bytes = pyramid_level_bytes(B, L, early_factor);
   char* tc_ws = (char*)workspace + level_bytes;
   const size_t tc_ws_bytes = ws_bytes - level_bytes;
   char* wsp = (char*)workspace;
-  const float* cur = x;
+  const float* cur = static_cast<const float*>(x);
   int64_t cur_len = L, cur_pitch = x_pitch;
   if (early_factor > 1) {
     const int64_t L0 = decimated_len(L, early_factor);
     const int64_t pitch0 = (int64_t)align_up((size_t)L0, 4);
     float* e = (float*)wsp;
     wsp += align_up((size_t)B * pitch0 * sizeof(float), 256);
-    if ((rc = launch_fir_decimate(x, B, L, x_pitch, early_filter, 256, early_factor, e, L0,
+    if ((rc = launch_fir_decimate(cur, B, L, x_pitch, early_filter, 256, early_factor, e, L0,
                                   pitch0, s)))
       return rc;
     cur = e; cur_len = L0; cur_pitch = pitch0;

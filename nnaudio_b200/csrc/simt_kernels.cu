@@ -133,8 +133,9 @@ __global__ void __launch_bounds__(256) framed_cplx_simt_kernel(const SimtParams 
 int launch_framed_simt(const FramedProblem& q, cudaStream_t stream) {
   if (q.B <= 0 || q.T <= 0 || q.F <= 0) return NNAB_OK;
   if (q.B > 65535) return NNAB_EUNSUPPORTED;
+  if (q.x_dtype != NNAB_DTYPE_F32) return NNAB_EUNSUPPORTED;  // this kernel reads fp32 samples only
   SimtParams p;
-  p.x = q.x; p.L = q.L; p.x_pitch = q.x_pitch;
+  p.x = static_cast<const float*>(q.x); p.L = q.L; p.x_pitch = q.x_pitch;
   p.w_re = q.w_re; p.w_im = q.w_im;
   p.F = q.F; p.K = q.K; p.hop = q.hop; p.pad = q.pad; p.pad_mode = q.pad_mode;
   p.epi.scale = q.scale; p.epi.scale_all = q.scale_all; p.epi.fmt = q.fmt;

@@ -24,6 +24,7 @@
 #include <algorithm>
 #include <vector>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -101,43 +102,89 @@ bool tc_supported(const FramedProblem& p) {
 // pre-pass kernels
 // ---------------------------------------------------------------------------
 
-// One thread = 8 consecutive samples of one clip's slot region (16-byte stores).
-__global__ void __launch_bounds__(256) pad_split_kernel(
-    const float* __restrict__ x, int64_t L, int64_t x_pitch, int pad, int pad_mode, int shift,
-    int64_t clip_pitch, int64_t plane_stride, __nv_bfloat16* __restrict__ planes) {
-  const int64_t b = blockIdx.y;
-  const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
-  if (i0 >= clip_pitch) return;
-  const float* __restrict__ xb = x + b * x_pitch;
+// Waveform samples as fp32: exact for all three sample types.  The planes are then a function of the fp32
+// value only, so a 16-bit waveform gives the bytes its fp32 upcast gives (bf16: lo = 0; fp16: 11 significant
+// bits, exactly hi + lo).
+__device__ __forceinline__ float sample_f32(float v) { return v; }
+__device__ __forceinline__ float sample_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float sample_f32(__half v) { return __half2float(v); }
+
+// Samples i0 .. i0 + 7 of the centre-padded clip xb (L samples, `pad` on each side) as fp32.  Runs of 8 inside
+// the clip whose address is 16-byte aligned are read with 16-byte loads.
+template <typename Tx>
+__device__ __forceinline__ void padded_samples8(const Tx* __restrict__ xb, int64_t L, int pad, int pad_mode,
+                                                int64_t i0, float (&v)[8]) {
+  const int64_t j0 = i0 - pad;
+  if (j0 >= 0 && j0 + 8 <= L && (reinterpret_cast<uintptr_t>(xb + j0) & 15u) == 0) {
+    constexpr int PER = 16 / (int)sizeof(Tx);  // samples per 16-byte load
+#pragma unroll
+    for (int c = 0; c < 8 / PER; ++c) {
+      const uint4 u = __ldg(reinterpret_cast<const uint4*>(xb + j0) + c);
+      const Tx* s = reinterpret_cast<const Tx*>(&u);
+#pragma unroll
+      for (int e = 0; e < PER; ++e) v[c * PER + e] = sample_f32(s[e]);
+    }
+    return;
+  }
   const int64_t padded_len = L + 2 * (int64_t)pad;
-  __align__(16) __nv_bfloat16 hi[8];
-  __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    const int64_t i = i0 + e + shift;  // index into the centre-padded clip
-    float v = 0.f;
+    const int64_t i = i0 + e;
+    v[e] = 0.f;
     if (i < padded_len) {
       int64_t j = i - pad;
       if (j < 0) j = (pad_mode == NNAB_PAD_REFLECT) ? -j : -1;
       else if (j >= L) j = (pad_mode == NNAB_PAD_REFLECT) ? 2 * (L - 1) - j : -1;
-      if (j >= 0 && j < L) v = __ldg(xb + j);
+      if (j >= 0 && j < L) v[e] = sample_f32(__ldg(xb + j));
     }
-    split_bf16(v, hi[e], lo[e]);
   }
+}
+
+// One thread = 8 consecutive samples of one clip's slot region (16-byte stores).
+template <typename Tx>
+__global__ void __launch_bounds__(256) pad_split_kernel(
+    const Tx* __restrict__ x, int64_t L, int64_t x_pitch, int pad, int pad_mode, int shift,
+    int64_t clip_pitch, int64_t plane_stride, __nv_bfloat16* __restrict__ planes) {
+  const int64_t b = blockIdx.y;
+  const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if (i0 >= clip_pitch) return;
+  float v[8];
+  padded_samples8(x + b * x_pitch, L, pad, pad_mode, i0 + shift, v);  // i0 + shift: index into the padded clip
+  __align__(16) __nv_bfloat16 hi[8];
+  __align__(16) __nv_bfloat16 lo[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) split_bf16(v[e], hi[e], lo[e]);
   const int64_t o = b * clip_pitch + i0;
   *reinterpret_cast<uint4*>(planes + o) = *reinterpret_cast<const uint4*>(hi);
   *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
+// pad_split_kernel on the waveform's sample type (NNAB_DTYPE_*)
+static int launch_pad_split(dim3 grid, cudaStream_t stream, const void* x, int x_dtype, int64_t L,
+                            int64_t x_pitch, int pad, int pad_mode, int shift, int64_t clip_pitch,
+                            int64_t plane_stride, __nv_bfloat16* planes) {
+  auto launch = [&](auto* xs) {
+    pad_split_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad, pad_mode, shift, clip_pitch, plane_stride,
+                                               planes);
+  };
+  if (x_dtype == NNAB_DTYPE_F32) launch(static_cast<const float*>(x));
+  else if (x_dtype == NNAB_DTYPE_BF16) launch(static_cast<const __nv_bfloat16*>(x));
+  else if (x_dtype == NNAB_DTYPE_F16) launch(static_cast<const __half*>(x));
+  else return NNAB_EINVAL;
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
 // Two differently padded split copies of the same batch in one pass over x (level 0 of
 // the CQT pyramid: reflect-padded copy for the octave CQT + zero-margin copy for the FIR).
+template <typename Tx>
 __global__ void __launch_bounds__(256) pad_split2_kernel(
-    const float* __restrict__ x, int64_t L, int64_t x_pitch,
+    const Tx* __restrict__ x, int64_t L, int64_t x_pitch,
     int pad_a, int mode_a, int64_t pitch_a, int64_t plane_a, __nv_bfloat16* __restrict__ pa,
     int pad_b, int mode_b, int64_t pitch_b, int64_t plane_b, __nv_bfloat16* __restrict__ pb) {
   const int64_t b = blockIdx.y;
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
-  const float* __restrict__ xb = x + b * x_pitch;
+  const Tx* __restrict__ xb = x + b * x_pitch;
 #pragma unroll
   for (int which = 0; which < 2; ++which) {
     const int pad = which ? pad_b : pad_a;
@@ -146,21 +193,12 @@ __global__ void __launch_bounds__(256) pad_split2_kernel(
     const int64_t plane = which ? plane_b : plane_a;
     __nv_bfloat16* __restrict__ dst = which ? pb : pa;
     if (i0 >= pitch) continue;
-    const int64_t padded_len = L + 2 * (int64_t)pad;
+    float v[8];
+    padded_samples8(xb, L, pad, mode, i0, v);
     __align__(16) __nv_bfloat16 hi[8];
     __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int64_t i = i0 + e;
-      float v = 0.f;
-      if (i < padded_len) {
-        int64_t j = i - pad;
-        if (j < 0) j = (mode == NNAB_PAD_REFLECT) ? -j : -1;
-        else if (j >= L) j = (mode == NNAB_PAD_REFLECT) ? 2 * (L - 1) - j : -1;
-        if (j >= 0 && j < L) v = __ldg(xb + j);
-      }
-      split_bf16(v, hi[e], lo[e]);
-    }
+    for (int e = 0; e < 8; ++e) split_bf16(v[e], hi[e], lo[e]);
     const int64_t o = b * pitch + i0;
     *reinterpret_cast<uint4*>(dst + o) = *reinterpret_cast<const uint4*>(hi);
     *reinterpret_cast<uint4*>(dst + plane + o) = *reinterpret_cast<const uint4*>(lo);
@@ -273,8 +311,8 @@ static int zero_tail(__nv_bfloat16* planes, const SplitGeom& g, int hop_eff, cud
   return NNAB_OK;
 }
 
-// phase-0 pad + split of an fp32 batch into caller-managed planes
-int tc_pad_split(const float* x, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
+// phase-0 pad + split of a batch into caller-managed planes
+int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
                  int pad_mode, void* planes_v, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
   const SplitGeom g = split_geom(B, L, K, hop, pad);
@@ -284,10 +322,8 @@ int tc_pad_split(const float* x, int64_t B, int64_t L, int64_t x_pitch, int K, i
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * hop_eff;
   dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
-  pad_split_kernel<<<grid, 256, 0, stream>>>(x, L, x_pitch, pad, pad_mode, 0, clip_pitch,
-                                             g.plane_stride, planes);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  return launch_pad_split(grid, stream, x, x_dtype, L, x_pitch, pad, pad_mode, 0, clip_pitch, g.plane_stride,
+                          planes);
 }
 
 __global__ void zero_margins_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride,
@@ -296,7 +332,7 @@ __global__ void zero_margins_kernel(__nv_bfloat16* __restrict__ planes, int64_t 
 // pad + split into caller-defined geometry (clip pitch / plane stride in elements).  pad_split_kernel
 // writes the whole [0, clip_pitch) slot of every clip (zeros past the padded signal); the tail
 // [B * clip_pitch, plane_stride) is zeroed here.
-int tc_pad_split_ex(const float* x, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
+int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
                     int64_t clip_pitch, int64_t plane_stride, void* planes_v, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
   if (clip_pitch % 8 != 0 || plane_stride < B * clip_pitch) return NNAB_EINVAL;
@@ -306,10 +342,8 @@ int tc_pad_split_ex(const float* x, int64_t B, int64_t L, int64_t x_pitch, int p
     NNAB_CUDA_TRY(cudaMemsetAsync(planes + pl * plane_stride + B * clip_pitch, 0,
                                   (size_t)tail * sizeof(__nv_bfloat16), stream));
   dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
-  pad_split_kernel<<<grid, 256, 0, stream>>>(x, L, x_pitch, pad, pad_mode, 0, clip_pitch, plane_stride,
-                                             planes);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  return launch_pad_split(grid, stream, x, x_dtype, L, x_pitch, pad, pad_mode, 0, clip_pitch, plane_stride,
+                          planes);
 }
 
 // zero [keep_hi, clip_pitch) and [0, keep_lo) of every clip slot (both planes) + the tail of the planes
@@ -333,10 +367,11 @@ int tc_zero_slots(void* planes_v, int64_t B, int64_t clip_pitch, int64_t plane_s
   return NNAB_OK;
 }
 
-int tc_pad_split2(const float* x, int64_t B, int64_t L, int64_t x_pitch,
+int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
                   int K_a, int hop_a, int pad_a, int mode_a, void* planes_a,
                   int K_b, int hop_b, int pad_b, int mode_b, void* planes_b, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
+  if (x_dtype != NNAB_DTYPE_F32 && x_dtype != NNAB_DTYPE_BF16 && x_dtype != NNAB_DTYPE_F16) return NNAB_EINVAL;
   const SplitGeom ga = split_geom(B, L, K_a, hop_a, pad_a);
   const SplitGeom gb = split_geom(B, L, K_b, hop_b, pad_b);
   const int he_a = hop_a * num_phases(hop_a), he_b = hop_b * num_phases(hop_b);
@@ -346,10 +381,14 @@ int tc_pad_split2(const float* x, int64_t B, int64_t L, int64_t x_pitch,
   const int64_t pitch_a = ga.t_slots * he_a, pitch_b = gb.t_slots * he_b;
   const int64_t pmax = pitch_a > pitch_b ? pitch_a : pitch_b;
   dim3 grid((unsigned)ceil_div64(pmax, 256 * 8), (unsigned)B);
-  pad_split2_kernel<<<grid, 256, 0, stream>>>(x, L, x_pitch, pad_a, mode_a, pitch_a,
-                                              ga.plane_stride, (__nv_bfloat16*)planes_a, pad_b,
-                                              mode_b, pitch_b, gb.plane_stride,
-                                              (__nv_bfloat16*)planes_b);
+  auto launch = [&](auto* xs) {
+    pad_split2_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad_a, mode_a, pitch_a, ga.plane_stride,
+                                                (__nv_bfloat16*)planes_a, pad_b, mode_b, pitch_b,
+                                                gb.plane_stride, (__nv_bfloat16*)planes_b);
+  };
+  if (x_dtype == NNAB_DTYPE_F32) launch(static_cast<const float*>(x));
+  else if (x_dtype == NNAB_DTYPE_BF16) launch(static_cast<const __nv_bfloat16*>(x));
+  else launch(static_cast<const __half*>(x));
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -1440,9 +1479,9 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * q.hop;
   dim3 pgrid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-  pad_split_kernel<<<pgrid, 256, 0, stream>>>(q.x, q.L, q.x_pitch, q.pad, q.pad_mode, 0, clip_pitch,
-                                              g.plane_stride, planes);
-  NNAB_LAUNCH_CHECK();
+  if ((rc = launch_pad_split(pgrid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, 0, clip_pitch,
+                             g.plane_stride, planes)))
+    return rc;
 
   // split-K only with the caller's raw scratch (long kernels): <= 64 K blocks per accumulator
   VarNPlan plan;
@@ -1689,9 +1728,9 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     prm.T = (q.T - ph + n_ph - 1) / n_ph;  // frames t = ph, ph + n_ph, ... < T
     if (q.presplit == nullptr) {
       dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-      pad_split_kernel<<<grid, 256, 0, stream>>>(q.x, q.L, q.x_pitch, q.pad, q.pad_mode,
-                                                 ph * q.hop, clip_pitch, g.plane_stride, planes);
-      NNAB_LAUNCH_CHECK();
+      if ((rc = launch_pad_split(grid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, ph * q.hop,
+                                 clip_pitch, g.plane_stride, planes)))
+        return rc;
     }
     {
       double kcols = 0.0;  // sum over N tiles of (k-blocks executed) x bk x bn

@@ -149,6 +149,22 @@ __device__ __forceinline__ void wg_kblock_split3_n(float* d, uint32_t a_hi, uint
   }
 }
 
+// The 2-term form for an A operand that is exactly bf16 (a bf16 waveform: xlo == 0), xhi*wlo + xhi*whi.
+// It issues the last two wgmmas of wg_kblock_split3_n in the same order, so every accumulator gets what
+// the 3-term form gives on a zero lo plane (there, d + 0 = d), up to the sign of a zero.
+template <int N, int BK = 64>
+__device__ __forceinline__ void wg_kblock_split2_n(float* d, uint32_t a_hi, uint32_t b_hi, uint32_t b_lo,
+                                                   bool first_accumulates) {
+  static_assert(BK == 64 || BK == 32, "K block is one 128-byte or 64-byte swizzled row");
+  const uint32_t hi = (BK == 64) ? wg_desc_hi() : wg_desc_hi_sw64();
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint32_t o = 2u * k;
+    Wgmma<N>::mma(d, desc64(a_hi + o, hi), desc64(b_lo + o, hi), (k == 0 && !first_accumulates) ? 0u : 1u);
+    Wgmma<N>::mma(d, desc64(a_hi + o, hi), desc64(b_hi + o, hi), 1u);
+  }
+}
+
 // the same with N chosen at run time (a multiple of 16, <= NMAX); d holds NMAX / 2 registers
 template <int NMAX>
 __device__ __forceinline__ void wg_kblock_split3(int n, float* d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,

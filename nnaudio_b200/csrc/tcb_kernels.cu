@@ -26,7 +26,8 @@
 //     rows and emits 33 - R frames; the 4 quarters of a tile are loaded as four 32-row TMA boxes whose
 //     row origins are 33 - R apart, so no frame needs a row of another warp (no exchange, no barrier).
 //     4 * (33 - R) frames per tile (116 of 128 rows for R = 4).
-//   * fp32 parity: x*w = xhi*whi + xlo*whi + xhi*wlo on bf16 tensor cores, fp32 accumulation.
+//   * fp32 parity: x*w = xhi*whi + xlo*whi + xhi*wlo on bf16 tensor cores, fp32 accumulation.  A bf16
+//     waveform has xlo = 0: that kernel instance (PASSES = 2) skips the xlo*whi pass and the A lo plane.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <atomic>
@@ -56,6 +57,8 @@ struct TcbParams {
 
 // Dynamic shared memory: [1024-byte alignment slack][accumulator tile][stage ring][barriers].  The
 // accumulator tile has its own space, so the producer refills the ring while the epilogue reads the tile.
+// PASSES = 3: the split product xlo*whi + xhi*wlo + xhi*whi, a stage holds both A planes.  PASSES = 2 (a
+// bf16 waveform, xlo == 0): xhi*wlo + xhi*whi, a stage holds the A hi plane only, so the ring may be deeper.
 struct TcbSmem {
   static constexpr uint32_t A_BYTES = TC_BM * TCB_BK * 2;  // one plane, 128 rows
   static constexpr uint32_t LIMIT = 227 * 1024;            // opt-in dynamic shared memory per block
@@ -64,12 +67,18 @@ struct TcbSmem {
   __host__ __device__ static uint32_t acc_bytes(int nb) { return TC_BM * (uint32_t)((2 * nb + 31) / 32) * 128u; }
   // one (plane, part) box of the basis: nb rows; a multiple of 512 B, so every operand starts on an atom
   __host__ __device__ static uint32_t part_bytes(int nb) { return (uint32_t)nb * TCB_BK * 2; }
-  __host__ __device__ static uint32_t stage_bytes(int nb) { return 2 * A_BYTES + 4 * part_bytes(nb); }
-  static int stages(int nb) {
-    const int s = (int)((LIMIT - 1024 - BAR_BYTES - acc_bytes(nb)) / stage_bytes(nb));
+  // A planes per stage: 2 (hi, lo) with three passes, 1 (hi) with two
+  __host__ __device__ static constexpr uint32_t a_planes(int passes) { return passes == 3 ? 2u : 1u; }
+  __host__ __device__ static uint32_t stage_bytes(int nb, int passes) {
+    return a_planes(passes) * A_BYTES + 4 * part_bytes(nb);
+  }
+  static int stages(int nb, int passes) {
+    const int s = (int)((LIMIT - 1024 - BAR_BYTES - acc_bytes(nb)) / stage_bytes(nb, passes));
     return s < TCB_MAX_STAGES ? s : TCB_MAX_STAGES;
   }
-  static uint32_t total(int nb) { return 1024 + acc_bytes(nb) + stages(nb) * stage_bytes(nb) + BAR_BYTES; }
+  static uint32_t total(int nb, int passes) {
+    return 1024 + acc_bytes(nb) + stages(nb, passes) * stage_bytes(nb, passes) + BAR_BYTES;
+  }
 };
 
 // rows of one (plane, part) slab of the packed block basis
@@ -380,8 +389,8 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
 constexpr int TCB_PARTS = 2;
 static_assert(FB_EPI_PARTS == TCB_PARTS, "fused-filterbank column ranges follow the epilogue warps");
 
-// The stage ring.  A stage holds A (hi, lo planes: four 32-row boxes each) and B (four nb-row boxes: hi re,
-// hi im, lo re, lo im); its empty barrier counts the 8 consumer warps.
+// The stage ring.  A stage holds A (hi, lo planes, or hi only with two passes: four 32-row boxes each) and B
+// (four nb-row boxes: hi re, hi im, lo re, lo im); its empty barrier counts the 8 consumer warps.
 struct TcbRing {
   uint32_t base, stage_bytes, bars;
   int stages;
@@ -393,7 +402,7 @@ struct TcbRing {
 // One tile's K loop at MMA width N = 2 nb.  Each K block is committed as one wgmma group; the stage of the
 // PREVIOUS block is released once that group has retired, so one group is always in flight.  A width fixed
 // at compile time keeps every in-flight wgmma off divergent paths (ptxas would serialise them).
-template <int N>
+template <int N, int PASSES>
 __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, int kb_n, uint32_t a_off,
                                              uint32_t part_bytes, int lane, int& stage, uint32_t& phase) {
   using S = TcbSmem;
@@ -401,10 +410,14 @@ __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, in
   for (int kb = 0; kb < kb_n; ++kb) {
     mbar_wait(ring.full(stage), phase);
     const uint32_t sb = ring.stage(stage);
-    const uint32_t b = sb + 2 * S::A_BYTES;
+    const uint32_t b = sb + S::a_planes(PASSES) * S::A_BYTES;
     wgmma_fence();
-    wg_kblock_split3_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
-                                  wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes), kb != 0);
+    if constexpr (PASSES == 3)
+      wg_kblock_split3_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
+                                    wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes), kb != 0);
+    else
+      wg_kblock_split2_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes),
+                                    kb != 0);
     wgmma_commit();
     wgmma_wait<1>();
     __syncwarp();
@@ -417,7 +430,7 @@ __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, in
   if (lane == 0) mbar_arrive(ring.empty(prev));
 }
 
-template <int FMT, int R>
+template <int FMT, int R, int PASSES>
 __global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
 framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const TcbParams p) {
@@ -427,7 +440,7 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   const int nb = p.nb;
   TcbRing ring;
   ring.base = acc_tile_base() + S::acc_bytes(nb);
-  ring.stage_bytes = S::stage_bytes(nb);
+  ring.stage_bytes = S::stage_bytes(nb, PASSES);
   ring.stages = p.stages;
   ring.bars = ring.base + (uint32_t)p.stages * ring.stage_bytes;
 
@@ -466,11 +479,12 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 #pragma unroll
           for (int q = 0; q < 4; ++q) {  // 32-row boxes, row origins FW apart
             tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 0);
-            tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 1);
+            if constexpr (PASSES == 3)
+              tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 1);
           }
           // B rows [0, nb) = re part, [nb, 2 nb) = im part of each plane: accumulator columns of the
           // N = 2 nb MMA
-          const uint32_t b = sb + 2 * S::A_BYTES;
+          const uint32_t b = sb + S::a_planes(PASSES) * S::A_BYTES;
 #pragma unroll
           for (int j = 0; j < 4; ++j) tma_load_3d(b + (uint32_t)j * part_bytes, &tm_b, full, k0, n0, j);
           if (++stage == p.stages) { stage = 0; phase ^= 1u; }
@@ -498,7 +512,7 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     switch (2 * nb) {  // nb = 32 .. 128 in steps of 8
 #define NNAB_TCB_CASE(N) \
-  case N: tcb_mainloop<N>(acc, ring, p.kb_n, a_off, part_bytes, lane, stage, phase); break;
+  case N: tcb_mainloop<N, PASSES>(acc, ring, p.kb_n, a_off, part_bytes, lane, stage, phase); break;
       NNAB_TCB_CASE(64) NNAB_TCB_CASE(80) NNAB_TCB_CASE(96) NNAB_TCB_CASE(112) NNAB_TCB_CASE(128)
       NNAB_TCB_CASE(144) NNAB_TCB_CASE(160) NNAB_TCB_CASE(176) NNAB_TCB_CASE(192) NNAB_TCB_CASE(208)
       NNAB_TCB_CASE(224) NNAB_TCB_CASE(240) NNAB_TCB_CASE(256)
@@ -517,7 +531,7 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-template <int FMT, int R>
+template <int FMT, int R, int PASSES>
 static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
                           cudaStream_t stream) {
   using S = TcbSmem;
@@ -525,25 +539,25 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   int cfg_dev = 0;
   NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
   if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R>,
+    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R, PASSES>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::LIMIT));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  framed_tcb_kernel<FMT, R><<<grid, TC_KERNEL_THREADS, S::total(prm.nb), stream>>>(ma, mb, prm);
+  framed_tcb_kernel<FMT, R, PASSES><<<grid, TC_KERNEL_THREADS, S::total(prm.nb, PASSES), stream>>>(ma, mb, prm);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
-template <int R>
+template <int R, int PASSES>
 static int launch_tcb(int fmt, const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
                       cudaStream_t stream) {
   switch (fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R>(ma, mb, prm, grid, stream);
-    case FMT_POWER: return launch_tcb_fmt<4, R>(ma, mb, prm, grid, stream);
-    case FMT_FBANK: return launch_tcb_fmt<5, R>(ma, mb, prm, grid, stream);
-    case FMT_PLANES: return launch_tcb_fmt<9, R>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R, PASSES>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R, PASSES>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R, PASSES>(ma, mb, prm, grid, stream);
+    case FMT_POWER: return launch_tcb_fmt<4, R, PASSES>(ma, mb, prm, grid, stream);
+    case FMT_FBANK: return launch_tcb_fmt<5, R, PASSES>(ma, mb, prm, grid, stream);
+    case FMT_PLANES: return launch_tcb_fmt<9, R, PASSES>(ma, mb, prm, grid, stream);
     default: return NNAB_EINVAL;
   }
 }
@@ -583,8 +597,10 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
   __nv_bfloat16* planes =
       reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  int rc = tc_pad_split(q.x, q.B, q.L, q.x_pitch, q.K, q.hop, q.pad, q.pad_mode, planes, stream);
+  int rc = tc_pad_split(q.x, q.x_dtype, q.B, q.L, q.x_pitch, q.K, q.hop, q.pad, q.pad_mode, planes, stream);
   if (rc) return rc;
+  // a bf16 waveform has an all-zero lo plane: the xlo * whi pass would add exact zeros
+  const int passes = (q.x_dtype == NNAB_DTYPE_BF16) ? 2 : 3;
 
   int dev = 0, sms = 132;
   NNAB_CUDA_TRY(cudaGetDevice(&dev));
@@ -622,7 +638,7 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.num_n_tiles = n_tiles;
   prm.nb = nb;
   prm.kb_n = q.hop / TCB_BK;
-  prm.stages = TcbSmem::stages(nb);
+  prm.stages = TcbSmem::stages(nb, passes);
   prm.nv = g.nv;
   prm.t_slots = g.t_slots;
   prm.T = q.T;
@@ -636,9 +652,12 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   if (q.fmt == FMT_PLANES && (int64_t)n_tiles * nb > q.planes_pitch) return NNAB_EINVAL;
   const int64_t tiles = (int64_t)prm.num_m_tiles * n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);
-  add_exec_flops(3.0 * 2.0 * (double)tiles * TC_BM * (2 * nb) * q.hop);
-  return R == 4 ? launch_tcb<4>(q.fmt, ma, mb, prm, grid, stream)
-                : launch_tcb<2>(q.fmt, ma, mb, prm, grid, stream);
+  add_exec_flops(passes * 2.0 * (double)tiles * TC_BM * (2 * nb) * q.hop);
+  if (passes == 2)
+    return R == 4 ? launch_tcb<4, 2>(q.fmt, ma, mb, prm, grid, stream)
+                  : launch_tcb<2, 2>(q.fmt, ma, mb, prm, grid, stream);
+  return R == 4 ? launch_tcb<4, 3>(q.fmt, ma, mb, prm, grid, stream)
+                : launch_tcb<2, 3>(q.fmt, ma, mb, prm, grid, stream);
 }
 
 }  // namespace nnab

@@ -55,6 +55,13 @@ def wants_grad(module: torch.nn.Module, x: torch.Tensor) -> bool:
     return x.requires_grad or any(p.requires_grad for p in module.parameters())
 
 
+def upcast_16bit(x: torch.Tensor) -> torch.Tensor:
+    """A bfloat16 / float16 waveform as float32, anything else unchanged (so other dtypes still fail
+    in the C wrappers).  The differentiable branches call it once at their top: they run the fp32
+    training kernels, and autograd returns ``x.grad`` in the input's dtype."""
+    return x.float() if x.dtype in (torch.bfloat16, torch.float16) else x
+
+
 class FramedComplexFn(torch.autograd.Function):
     """Differentiable complex framed contraction ``(x, w_re, w_im) -> (B, F, T, 2)``:
     forward = the fused kernel; backward = ``nnab_framed_backward_input`` (GEMM with the

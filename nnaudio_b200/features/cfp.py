@@ -35,7 +35,7 @@ import torch
 import torch.nn as nn
 
 from .. import _C, design
-from ._common import PerDeviceCache
+from ._common import PerDeviceCache, upcast_16bit
 
 EPSILON = 1e-8  # utils.py:20
 
@@ -234,7 +234,8 @@ class _CFPBase(nn.Module):
             raise RuntimeError(f"stft: expected a 1D or 2D tensor, but got {x.dim()}D tensor")
         if torch.is_grad_enabled() and x.requires_grad:
             raise NotImplementedError("nnaudio_b200: CFP is forward-only; run under torch.no_grad()")
-        x = _C._dev_f32(x, "x")
+        # a 16-bit waveform is upcast here: the cost of this transform is in its dense contractions
+        x = _C._dev_f32(upcast_16bit(x), "x")
         tfr0 = self._stft_magnitude(x)                       # (B, H, T)
         if drop_edge_frames:
             tfr0 = tfr0[:, :, 1:-1].contiguous()             # cfp.py:151-153

@@ -14,7 +14,7 @@ import torch.nn as nn
 
 from .. import _C, design
 from ._common import (AdjointBasis, FramedComplexFn, PackedBasis, PackedFir, PerDeviceCache, as_matrix,
-                      broadcast_dim, pad_mode_id, tap_support, wants_grad)
+                      broadcast_dim, pad_mode_id, tap_support, upcast_16bit, wants_grad)
 
 _FORMATS = {
     "Magnitude": _C.FMT_MAGNITUDE,
@@ -163,8 +163,8 @@ class CQT1992v2(nn.Module):
                 return _C.framed_backward_weight(g, xin, self.kernel_width, self.hop_length,
                                                  self.center, pad_mode_id(self.pad_mode))
 
-            c = FramedComplexFn.apply(x, self.cqt_kernels_real, self.cqt_kernels_imag, fwd, bwd,
-                                      bwd_w)
+            c = FramedComplexFn.apply(upcast_16bit(x), self.cqt_kernels_real, self.cqt_kernels_imag, fwd,
+                                      bwd, bwd_w)
             if scale is not None:
                 c = c * scale.view(1, -1, 1, 1)
             elif scale_all != 1.0:
@@ -385,8 +385,8 @@ def _pyramid_forward(mod, x, output_format, normalization):
                 UserWarning,
             )
     if wants_grad(mod, x):
-        return _pyramid_forward_autograd(mod, x, output_format, fallbacks, factor, scale, scale_all,
-                                         eps)
+        return _pyramid_forward_autograd(mod, upcast_16bit(x), output_format, fallbacks, factor, scale,
+                                         scale_all, eps)
     lowpass = mod.lowpass_filter.detach().reshape(-1)
     early_flat = early.detach().reshape(-1) if early is not None else None
     for t in (lowpass, early_flat):

@@ -25,7 +25,7 @@ import torch.nn as nn
 from scipy.fftpack import fft as _fft
 
 from .. import _C, design
-from ._common import PackedBasis, PerDeviceCache, broadcast_dim, pad_mode_id, wants_grad
+from ._common import PackedBasis, PerDeviceCache, broadcast_dim, pad_mode_id, upcast_16bit, wants_grad
 from .cqt import (_ScaleCache, _check_format_and_norm, _framed_complex_autograd,
                   _pyramid_forward)
 
@@ -160,7 +160,7 @@ class CQT1992(nn.Module):
                 w_re, w_im = self._folded.differentiable(self, negate)
             else:
                 w_re, w_im, _ = self._folded.get(self, negate)
-            c = _framed_complex_autograd(self, f"folded{int(negate)}", x, w_re, w_im,
+            c = _framed_complex_autograd(self, f"folded{int(negate)}", upcast_16bit(x), w_re, w_im,
                                          self.hop_length, self.center, mode)
             if scale is not None:
                 c = c * scale.view(1, -1, 1, 1)

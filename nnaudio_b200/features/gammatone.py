@@ -9,7 +9,7 @@ import torch
 import torch.nn as nn
 
 from .. import _C, design
-from ._common import FilterbankTable, pad_mode_id, wants_grad
+from ._common import FilterbankTable, pad_mode_id, upcast_16bit, wants_grad
 from .stft import STFT
 
 
@@ -76,7 +76,7 @@ class Gammatonegram(nn.Module):
     def forward(self, x):
         x = self.stft._checked_input(x)
         if wants_grad(self, x):
-            return torch.matmul(self.gammatone_basis, self.stft._magnitude_diff(x) ** self.power)
+            return torch.matmul(self.gammatone_basis, self.stft._magnitude_diff(upcast_16bit(x)) ** self.power)
         wcos, wsin, packed = self.stft._bases(block_ok=True)
         fb = self.gammatone_basis.detach()
         _C._dev_f32(fb, "gammatone_basis")

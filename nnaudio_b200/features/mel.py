@@ -11,7 +11,7 @@ import torch
 import torch.nn as nn
 
 from .. import _C, design
-from ._common import FilterbankTable, pad_mode_id, wants_grad
+from ._common import FilterbankTable, pad_mode_id, upcast_16bit, wants_grad
 from .stft import STFT
 
 
@@ -81,7 +81,7 @@ class MelSpectrogram(nn.Module):
     def forward(self, x):
         x = self.stft._checked_input(x)
         if wants_grad(self, x):  # mel.py:186-188 on top of the differentiable STFT magnitude
-            return torch.matmul(self._filterbank(), self.stft._magnitude_diff(x) ** self.power)
+            return torch.matmul(self._filterbank(), self.stft._magnitude_diff(upcast_16bit(x)) ** self.power)
         wcos, wsin, packed = self.stft._bases(block_ok=True)
         fb = self._filterbank().detach()
         _C._dev_f32(fb, "filterbank")
@@ -134,7 +134,7 @@ class MFCC(nn.Module):
         mel = self.melspec_layer
         x = mel.stft._checked_input(x)
         if wants_grad(self, x):  # mel.py:263-279, :281-307 composed in torch for autograd
-            S = mel(x)
+            S = mel(upcast_16bit(x))
             amin = torch.tensor(self._amin_host, device=S.device)
             log_spec = 10.0 * torch.log10(torch.clamp(S, min=self._amin_host))
             log_spec = log_spec - 10.0 * torch.log10(torch.clamp(amin, min=self._ref_host))

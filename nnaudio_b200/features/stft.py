@@ -15,7 +15,7 @@ import torch.nn as nn
 from .. import _C, design
 from ._common import (AdjointBasis, FramedComplexFn, PackedBasis, PerDeviceCache, as_matrix,
                       broadcast_dim,
-                      forward_only_guard, pad_mode_id, wants_grad)
+                      forward_only_guard, pad_mode_id, upcast_16bit, wants_grad)
 
 _FORMATS = {
     "Magnitude": _C.FMT_MAGNITUDE,
@@ -284,6 +284,7 @@ class STFT(nn.Module):
         if wants_grad(self, x):
             # training through the layer: fused complex contraction + dX kernel, the light
             # element-wise tail (stft.py:299-316) composed in torch for autograd
+            x = upcast_16bit(x)
             if output_format == "Complex":
                 return self._complex_diff(x)
             if output_format == "Magnitude":
