@@ -35,7 +35,12 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   module's buffers at construction, as the reference creates its window there;
 * trainable inverse kernels / window of `iSTFT` raise `NotImplementedError` under autograd (no dW path yet);
 * `CFP` / `Combined_Frequency_Periodicity` are forward-only (the reference has no parameters there; a waveform that
-  requires grad raises `NotImplementedError`); their FFT stages run as dense contractions (DESIGN.md §3.9).
+  requires grad raises `NotImplementedError`); their FFT stages run as dense contractions (DESIGN.md §3.9);
+* beyond the reference: `nnaudio_b200.streaming.StreamingTransform(module, batch)` streams live audio chunk by chunk
+  through STFT, MelSpectrogram, Gammatonegram, MFCC (`top_db=None`), CQT1992v2 / CQT and CQT1992 (`push(chunk)`,
+  `flush()`, `reset()`).  The concatenated outputs equal `module(x)` on the whole stream, bit for bit on the
+  tensor-core routes except across the CQT1992v2 kernel's two tile schedules (2e-6; DESIGN.md §3.10).
+  `StreamingInverse(istft_module, batch)` does the same for the inverse STFT, to fp32 rounding.
 
 Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
 schedule of the CQT1992v2 kernel).

@@ -354,6 +354,81 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
                                 int pad_mode, float* dw, void* workspace, size_t ws_bytes,
                                 void* stream);
 
+/* ------------------------------------------------------------------------- *
+ * Chunked streams: B streams that advance together, one push per chunk (DESIGN.md §3.10).
+ * Each *_chunk_forward takes the arguments of the matching *_forward_ex with (x, L, x_pitch) replaced by
+ *   state     DEVICE fp32 carry ring of nnab_chunk_state_bytes(B, K) bytes (K = n_fft or width), owned by
+ *             the caller for the stream's lifetime (its contents need no initialisation)
+ *   received, n_carry, frames   host counters: raw samples pushed before this chunk, how many of the last
+ *             of them the ring carries, frames returned so far (0, 0, 0 for a new stream; the library
+ *             returns NNAB_EINVAL for counters no stream can have)
+ *   chunk, chunk_dtype, n, chunk_pitch   the new (B, n) samples (NNAB_DTYPE_*; chunk may be NULL iff n == 0)
+ *   flush     1 on the last push: the remaining frames, with the right centre padding
+ * T is the number of frames THIS push returns: every frame whose samples have all arrived (frame t needs
+ * t*hop + K - pad of them, reflect padding also pad + 1), all remaining frames on flush.  The library
+ * returns NNAB_EINVAL when T disagrees.  out holds those T frames in the offline layout.  The frames are
+ * those the offline call gives for the whole stream, bit for bit on the tensor-core plans.  After the call
+ * the caller advances its counters: received += n, frames += T,
+ * n_carry = received - max(0, min(frames*hop - pad, pad > 0 ? received - pad - 1 : received)).
+ * Plans that read x as fp32 directly (SIMT) return NNAB_EUNSUPPORTED before anything is enqueued.
+ * The MFCC call takes top_db < 0 (None) only: the floor is a maximum over the whole clip.
+ * ------------------------------------------------------------------------- */
+size_t nnab_chunk_state_bytes(int64_t B, int K);
+size_t nnab_stft_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                       int n_fft, int F, int hop, int center, int pad_mode, int path);
+int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                            int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush,
+                            const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                            int center, int pad_mode, int out_format, float sqrt_eps, float* out, int64_t T,
+                            void* workspace, size_t ws_bytes, int path, void* stream);
+size_t nnab_filterbank_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                             int n_fft, int F, int hop, int center, int pad_mode, int n_fb,
+                                             int path, int has_table);
+int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                       const void* chunk, int chunk_dtype, int64_t B, int64_t n,
+                                       int64_t chunk_pitch, int flush, const float* wcos, const float* wsin,
+                                       const void* packed, int n_fft, int F, int hop, int center, int pad_mode,
+                                       float sqrt_eps, float power, const float* fb, int n_fb,
+                                       const void* fb_table, float* out, int64_t T, void* workspace,
+                                       size_t ws_bytes, int path, void* stream);
+size_t nnab_mfcc_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                       int n_fft, int F, int hop, int center, int pad_mode, int n_mels, int path,
+                                       int has_table);
+int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                            int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush,
+                            const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                            int center, int pad_mode, float sqrt_eps, float power, const float* mel_basis,
+                            int n_mels, const void* fb_table, float amin, float ref, float top_db,
+                            const float* dct, int n_mfcc, float* out, int64_t T, void* workspace,
+                            size_t ws_bytes, int path, void* stream);
+size_t nnab_cqt1992v2_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                            int width, int n_bins, int hop, int center, int pad_mode, int path);
+int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                 const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
+                                 int flush, const float* k_real, const float* k_imag, const void* packed,
+                                 const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins, int width,
+                                 int hop, int center, int pad_mode, const float* scale, float scale_all,
+                                 int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
+                                 size_t ws_bytes, int path, void* stream);
+
+/* Streamed inverse STFT: nnab_istft_forward's arguments, with the frames of ONE push as X (B, f_in, T, 2)
+ * (T may be 0) and in front of them
+ *   state     DEVICE fp32, nnab_chunk_state_bytes(B, n_fft) bytes: the overlap-add partial sums later frames
+ *             still reach (no initialisation needed)
+ *   frames, emitted   host counters: frames pushed before X, output samples returned so far
+ * and behind `center`: flush (1 on the last push) and length (< 0: None; read on flush only).
+ * out receives the samples no later frame can change: overlap-add positions below (frames + T) * hop (and
+ * below the earliest end the output can still have), the centre crop applied at the start; on flush the rest,
+ * with the offline length / centre rules.  out_len must be that count; NNAB_EINVAL for counters no stream has
+ * or a length shorter than the samples already returned.  Each sample is divided by the window sum-square of
+ * its global position.  The concatenation equals nnab_istft_forward on all frames to fp32 rounding (both
+ * overlap-add with fp32 atomics). */
+size_t nnab_istft_chunk_workspace_bytes(int64_t B, int f_in, int64_t T, int n_fft, int hop);
+int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const float* X, int64_t B, int f_in,
+                             int64_t T, const void* packed, const float* window, int n_fft, int hop, int center,
+                             int flush, int64_t length, float* out, int64_t out_len, void* workspace,
+                             size_t ws_bytes, void* stream);
+
 /* Kernel launches issued by this library since load (process wide; used by
  * bench.py for its `gpu_launches` claim). */
 uint64_t nnab_launch_count(void);

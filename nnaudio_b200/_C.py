@@ -121,6 +121,22 @@ for _name in ("nnab_stft_forward", "nnab_stft_filterbank_forward", "nnab_mfcc_fo
               "nnab_cqt1992v2_forward", "nnab_cqt_pyramid_forward"):
     _res, _args = SIGNATURES[_name]
     SIGNATURES[_name + "_ex"] = (_res, [_P, c_int] + _args[1:])
+# the *_chunk_forward entry points: (state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch,
+# flush) in place of (x, B, L, x_pitch); their workspace queries take (B, received, frames, n, flush) in place
+# of (B, L) and the pad mode after `center`
+_CHUNK_HEAD = [_P, c_int64, c_int64, c_int64, _P, c_int, c_int64, c_int64, c_int64, c_int]
+_CHUNK_WS_HEAD = [c_int64, c_int64, c_int64, c_int64, c_int]
+SIGNATURES["nnab_chunk_state_bytes"] = (c_size_t, [c_int64, c_int])
+for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_forward", "nnab_filterbank"),
+                   ("nnab_mfcc_forward", "nnab_mfcc"), ("nnab_cqt1992v2_forward", "nnab_cqt1992v2")):
+    _res, _args = SIGNATURES[_name]
+    SIGNATURES[_name.replace("_forward", "_chunk_forward")] = (_res, _CHUNK_HEAD + _args[4:])
+    _wres, _wargs = SIGNATURES[_ws + "_workspace_bytes"]
+    SIGNATURES[_ws + "_chunk_workspace_bytes"] = (_wres, _CHUNK_WS_HEAD + _wargs[2:6] + [c_int] + _wargs[6:])
+SIGNATURES["nnab_istft_chunk_workspace_bytes"] = SIGNATURES["nnab_istft_workspace_bytes"]
+SIGNATURES["nnab_istft_chunk_forward"] = (
+    c_int, [_P, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, c_int, c_int64, _P,
+            c_int64, _P, c_size_t, _P])
 
 _lib = None
 
@@ -539,6 +555,124 @@ def cqt_pyramid_forward(x, banks_real, banks_imag, packed, lowpass, lowpass_pack
             scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)),
             x, pitch, dt, strict_dtype)
     _check(rc, "nnab_cqt_pyramid_forward_ex")
+    return out
+
+
+# --------------------------------------------------------------------------- #
+# chunk calls (nnaudio_b200.streaming): one push of B streams.  `st` carries the device carry ring
+# (st.ring, nnab_chunk_state_bytes) and the host counters (st.received, st.n_carry, st.frames); `x` is the
+# (B, n) chunk or None; T the frames this push returns.  The remaining arguments are those of the offline
+# call above.  Returns the frames, or None when the plan cannot read a chunk (NNAB_EUNSUPPORTED, nothing
+# enqueued): the caller then takes the concat route.
+# --------------------------------------------------------------------------- #
+def chunk_state_bytes(B: int, K: int) -> int:
+    return int(lib().nnab_chunk_state_bytes(int(B), int(K)))
+
+
+def _chunk_args(st, x):
+    if x is None or x.shape[-1] == 0:
+        return None, 0, 0, _WAVE_DTYPES[st.dtype]
+    x, _, n, pitch, dt = _wave_rows(x)
+    return x, n, pitch, dt
+
+
+def _chunk_result(rc, out, what):
+    if rc == EUNSUPPORTED:
+        return None
+    _check(rc, what)
+    return out
+
+
+def stft_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format, sqrt_eps,
+                       path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    B, F, dev = st.batch, wcos.shape[0], st.ring.device
+    out = torch.empty((B, F, T, 2) if out_format == FMT_COMPLEX else (B, F, T), dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_stft_chunk_workspace_bytes(B, st.received, st.frames, n, int(flush), n_fft, F,
+                                                               hop, int(center), pad_mode, path), dev)
+        rc = L.nnab_stft_chunk_forward(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
+            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, out_format, sqrt_eps,
+            _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_stft_chunk_forward")
+
+
+def stft_filterbank_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps,
+                                  power, fb, fb_table=None, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    B, F, n_fb, dev = st.batch, wcos.shape[0], fb.shape[0], st.ring.device
+    out = torch.empty((B, n_fb, T), dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_filterbank_chunk_workspace_bytes(
+            B, st.received, st.frames, n, int(flush), n_fft, F, hop, int(center), pad_mode, n_fb, path,
+            int(fb_table is not None)), dev)
+        rc = L.nnab_stft_filterbank_chunk_forward(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
+            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(fb),
+            n_fb, _ptr(fb_table), _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_stft_filterbank_chunk_forward")
+
+
+def mfcc_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
+                       mel_basis, amin, ref, top_db, dct, fb_table=None, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    B, F, n_mels, n_mfcc, dev = st.batch, wcos.shape[0], mel_basis.shape[0], dct.shape[0], st.ring.device
+    out = torch.empty((B, n_mfcc, T), dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_mfcc_chunk_workspace_bytes(
+            B, st.received, st.frames, n, int(flush), n_fft, F, hop, int(center), pad_mode, n_mels, path,
+            int(fb_table is not None)), dev)
+        rc = L.nnab_mfcc_chunk_forward(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
+            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power,
+            _ptr(mel_basis), n_mels, _ptr(fb_table), amin, ref, -1.0 if top_db is None else float(top_db),
+            _ptr(dct), n_mfcc, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_mfcc_chunk_forward")
+
+
+def cqt1992v2_chunk_forward(st, x, flush, T, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode, scale,
+                            scale_all, out_format, sqrt_eps, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    (n_bins, width), B, dev = k_real.shape, st.batch, st.ring.device
+    out = torch.empty((B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2), dtype=torch.float32,
+                      device=dev)
+    path = resolve_path(path)
+    kb = k_begin.ctypes.data_as(c_void_p) if k_begin is not None else None
+    ke = k_end.ctypes.data_as(c_void_p) if k_end is not None else None
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_cqt1992v2_chunk_workspace_bytes(
+            B, st.received, st.frames, n, int(flush), width, n_bins, hop, int(center), pad_mode, path), dev)
+        rc = L.nnab_cqt1992v2_chunk_forward(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
+            _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode,
+            _ptr(scale), scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_cqt1992v2_chunk_forward")
+
+
+def istft_chunk_forward(st, X, flush, length, n_out, packed, window, n_fft, hop, center):
+    """One push of a streamed inverse STFT: X (B, f_in, T, 2) fp32 CUDA (T may be 0) -> the n_out samples it
+    completes.  ``st``: device state ``st.state`` and host counters ``st.frames`` / ``st.emitted``."""
+    L = lib()
+    X = _dev_f32(X, "X")
+    X = X if X.is_contiguous() else X.contiguous()
+    B, f_in, T, _ = X.shape
+    dev = st.state.device
+    out = torch.empty((B, n_out), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_istft_chunk_workspace_bytes(B, f_in, T, n_fft, hop), dev)
+        rc = L.nnab_istft_chunk_forward(_ptr(st.state), st.frames, st.emitted, _ptr(X) if T > 0 else None, B,
+                                        f_in, T, _ptr(packed), _ptr(window), n_fft, hop, int(center), int(flush),
+                                        -1 if length is None else int(length), _ptr(out), n_out, _ptr(ws), wsb,
+                                        _stream(dev))
+    _check(rc, "nnab_istft_chunk_forward")
     return out
 
 

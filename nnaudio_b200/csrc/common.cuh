@@ -90,6 +90,22 @@ constexpr int FB_STEP_PAD = 160;  // entries past F (a tile's last chunk may ove
 // results differ run to run: 2 it is.)
 constexpr int FB_EPI_PARTS = 2;
 
+// The signal of one push of a chunked stream (DESIGN §3.10): the "virtual clip" of `length` samples whose
+// sample i is raw stream sample r = origin + i.  Raw samples [.., received) come from the fp32 carry ring
+// (raw r of stream b at ring[b * ring_pitch + r % ring_len]), [received, total) from the chunk (samples of
+// type FramedProblem::x_dtype, rows of chunk_pitch).  r < 0 is the left centre padding; on the last push
+// (at_end) r >= total is the right one.
+struct ChunkSource {
+  const float* ring;
+  int64_t ring_pitch;
+  int64_t ring_len;
+  const void* chunk;
+  int64_t chunk_pitch;
+  int64_t received, total, origin, length;
+  int pad_mode;
+  int at_end;
+};
+
 struct FramedProblem {
   const void* x;       // (B, L) rows, pitch x_pitch samples of type x_dtype
   int x_dtype;         // NNAB_DTYPE_*: only the pad / split pre-pass reads 16-bit samples, the SIMT kernel fp32
@@ -124,6 +140,9 @@ struct FramedProblem {
   int k_splits_hint;         // FMT_OLA only (its atomics already accumulate): cut K into chunks
   int64_t planes_stride;     // FMT_PLANES: elements between the hi and the lo plane
   int planes_pitch;          // FMT_PLANES: elements per frame row (multiple of 64)
+  // non-null: the tensor-core pre-pass builds the planes from this push's virtual clip instead of x
+  // (then L = chunk->length, pad = 0); the SIMT kernel returns NNAB_EUNSUPPORTED
+  const ChunkSource* chunk;
 };
 
 int launch_framed_simt(const FramedProblem& p, cudaStream_t stream);
@@ -147,6 +166,10 @@ int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pit
                  int pad_mode, void* planes, cudaStream_t stream);
 int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
                     int64_t clip_pitch, int64_t plane_stride, void* planes, cudaStream_t stream);
+// tc_pad_split on the problem's own signal: the waveform x with its centre padding, or a push's virtual clip
+int tc_problem_split(const FramedProblem& q, void* planes, cudaStream_t stream);
+// store raw samples [from, total) of the chunk into the carry ring (cs.received = raw index of chunk[0])
+int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
                   int64_t keep_hi, cudaStream_t stream);
 int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
@@ -174,6 +197,9 @@ int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes, 
 int tc_istft_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window,
                       int n_fft, int hop, int64_t T, int64_t offset, float* out, int64_t out_len,
                       cudaStream_t stream);
+int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window, int n_fft,
+                            int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
+                            int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream);
 size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K);
 // block-partial kernel (tcb_kernels.cu): default N-tile geometry for F bins (nb packed columns per tile,
 // nb - 2 new bins each) -- the column layout of the FMT_PLANES operand planes

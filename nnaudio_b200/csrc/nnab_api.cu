@@ -135,6 +135,161 @@ static bool wants_tc(int path, int K, int hop) {
   return tc_supported(q);
 }
 
+// The signal a forward call's framed problems read: the caller's waveform with its centre padding, or one
+// push's virtual clip (chunk != nullptr; then L is the clip's length and pad 0).
+struct Wave {
+  const void* x;
+  int x_dtype;
+  int64_t B, L, x_pitch;
+  int pad, pad_mode;
+  const ChunkSource* chunk;
+};
+
+static void set_wave(FramedProblem& p, const Wave& w) {
+  p.x = w.x; p.x_dtype = w.x_dtype; p.B = w.B; p.L = w.L; p.x_pitch = w.x_pitch;
+  p.pad = w.pad; p.pad_mode = w.pad_mode; p.chunk = w.chunk;
+}
+
+// ---- chunked streams (DESIGN §3.10) ------------------------------------------------------------
+// Host counters of a stream: `received` raw samples so far, the last `n_carry` of them in the carry ring,
+// `frames` frames returned.  Frame t is returned by the first push after which every raw sample it reads
+// has arrived: t * hop + K - pad samples (reflect padding: and at least pad + 1, the left mirror of frame
+// 0), or all remaining frames on the last push.
+static int64_t chunk_ready_frames(int64_t total, int K, int hop, int pad, int pad_mode) {
+  if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && total < pad + 1) return 0;
+  const int64_t need = (int64_t)K - pad;
+  return total < need ? 0 : (total - need) / hop + 1;
+}
+
+// First raw sample the push after `frames` frames still reads: the first frame's start, and with centre
+// padding no later than total - (pad + 1) (the right mirror of the last push reads that far back).
+static int64_t chunk_carry_start(int64_t total, int64_t frames, int hop, int pad) {
+  int64_t s = frames * hop - pad;
+  if (pad > 0 && s > total - (pad + 1)) s = total - (pad + 1);
+  if (s < 0) s = 0;
+  return s < total ? s : total;
+}
+
+struct ChunkPlan {
+  ChunkSource cs;
+  int64_t T;          // frames this push returns
+  int64_t from;       // raw samples [from, total) go into the ring after the push
+};
+
+static int chunk_plan(const void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                      int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush, int K, int hop,
+                      int pad, int pad_mode, ChunkPlan* o) {
+  if (state == nullptr || !dtype_ok(chunk_dtype) || B < 0 || B > 65535 || n < 0 || (n > 0 && chunk == nullptr) ||
+      chunk_pitch < n || K < 2 || hop <= 0 || received < 0 || frames < 0)
+    return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  // the counters must be those of a stream that returned every ready frame
+  if (frames != chunk_ready_frames(received, K, hop, pad, pad_mode) ||
+      n_carry != received - chunk_carry_start(received, frames, hop, pad))
+    return NNAB_EINVAL;
+  const int64_t total = received + n;
+  int64_t t_end;
+  if (flush) {
+    if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad >= total) return NNAB_EINVAL;
+    t_end = frames_of(total, K, hop, pad);
+    if (t_end <= 0) return NNAB_EINVAL;
+  } else {
+    t_end = chunk_ready_frames(total, K, hop, pad, pad_mode);
+  }
+  ChunkSource& c = o->cs;
+  c.ring = static_cast<const float*>(state);
+  c.ring_pitch = K;
+  c.ring_len = K;
+  c.chunk = chunk;
+  c.chunk_pitch = chunk_pitch;
+  c.received = received;
+  c.total = total;
+  c.origin = frames * hop - pad;
+  c.length = t_end > frames ? (t_end - frames - 1) * hop + K : 0;
+  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
+  c.at_end = flush ? 1 : 0;
+  o->T = t_end - frames;
+  const int64_t keep = chunk_carry_start(total, t_end, hop, pad);
+  o->from = keep > received ? keep : received;
+  return NNAB_OK;
+}
+
+static Wave chunk_wave(const ChunkPlan& cp, int chunk_dtype, int64_t B) {
+  return Wave{nullptr, chunk_dtype, B, cp.cs.length, cp.cs.length, 0, cp.cs.pad_mode, &cp.cs};
+}
+
+// Length of a push's virtual clip (0: the push returns no frame); host only, no validation.
+static int64_t chunk_clip_length(int64_t received, int64_t frames, int64_t n, int flush, int K, int hop,
+                                 int pad, int pad_mode) {
+  const int64_t total = received + n;
+  const int64_t t_end = flush ? frames_of(total, K, hop, pad) : chunk_ready_frames(total, K, hop, pad, pad_mode);
+  return t_end > frames ? (t_end - frames - 1) * (int64_t)hop + K : 0;
+}
+
+// The frames of a push on the offline plan (stft_run & co. with the virtual clip as their signal), then the
+// samples the next push needs into the carry ring.  A plan that cannot read the clip (the SIMT kernels)
+// returns NNAB_EUNSUPPORTED before anything is enqueued, the ring included.
+template <typename Run>
+static int chunk_forward(const ChunkPlan& cp, int chunk_dtype, int64_t B, Run&& run, void* stream) {
+  int rc = check_arch();
+  if (rc) return rc;
+  if (cp.T > 0 && B > 0 && (rc = run(chunk_wave(cp, chunk_dtype, B), (cudaStream_t)stream))) return rc;
+  return tc_chunk_carry(cp.cs, chunk_dtype, B, cp.from, (cudaStream_t)stream);
+}
+
+// ---- streamed inverse STFT -----------------------------------------------------------------------
+// Overlap-add positions s (pad-cropped output sample s - offset).  After n frames, positions below n * hop are
+// final; the output can still end as early as istft_end_min(n) (length None).
+static int64_t istft_end_min(int64_t n, int n_fft, int hop, int center) {
+  const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
+  return center ? ola_len - n_fft / 2 : ola_len;
+}
+
+struct IstftChunkPlan {
+  int64_t origin;      // first position the push's overlap-add buffer holds (= first carried position)
+  int64_t carried;     // positions carried in: [origin, origin + carried)
+  int64_t buf_len;     // positions the push's buffer holds
+  int64_t emit_begin, emit_end;
+  int64_t carry_begin, carry_len;  // carried out
+};
+
+// Host counters: `frames` frames pushed so far, `emitted` output samples returned.  EINVAL for counters no
+// stream has, or a `length` shorter than what was returned.
+static int istft_chunk_plan(int64_t frames, int64_t emitted, int64_t T, int n_fft, int hop, int center, int flush,
+                            int64_t length, IstftChunkPlan* o) {
+  if (frames < 0 || emitted < 0 || T < 0 || n_fft <= 0 || hop <= 0 || hop > n_fft) return NNAB_EINVAL;
+  const int64_t offset = center ? n_fft / 2 : 0;
+  auto emitted_end = [&](int64_t n) {  // end of the positions returned by the pushes of n frames
+    if (n <= 0) return offset;
+    const int64_t e = n * hop < istft_end_min(n, n_fft, hop, center) ? n * hop : istft_end_min(n, n_fft, hop, center);
+    return e > offset ? e : offset;
+  };
+  const int64_t E = emitted_end(frames);
+  if (offset + emitted != E) return NNAB_EINVAL;
+  const int64_t n = frames + T;
+  if (flush && n <= 0) return NNAB_EINVAL;
+  o->origin = frames > 0 ? (E < frames * hop ? E : frames * hop) : 0;
+  o->carried = frames > 0 ? (frames - 1) * (int64_t)hop + n_fft - o->origin : 0;
+  o->buf_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - o->origin : 0;
+  o->emit_begin = E;
+  if (flush) {
+    const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
+    int64_t want = length >= 0 ? length : (center ? ola_len - 2 * offset : ola_len);
+    if (offset + want > ola_len) want = ola_len - offset;  // slicing past the end just truncates
+    if (want < 0) want = 0;
+    if (offset + want < E) return NNAB_EINVAL;  // shorter than the samples already returned
+    o->emit_end = offset + want;
+    o->carry_begin = o->carry_len = 0;
+  } else {
+    o->emit_end = emitted_end(n);
+    const int64_t c = n > 0 ? (o->emit_end < n * hop ? o->emit_end : n * hop) : 0;
+    o->carry_begin = c;
+    o->carry_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - c : 0;
+  }
+  if (o->carried > n_fft || o->carry_len > n_fft) return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
 }  // namespace nnab
 
 using namespace nnab;
@@ -263,6 +418,27 @@ int nnab_stft_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
                               pad_mode, out_format, sqrt_eps, out, T, workspace, ws_bytes, path, stream);
 }
 
+static int stft_args_ok(const float* wcos, const float* wsin, int out_format) {
+  if (wcos == nullptr || wsin == nullptr) return NNAB_EINVAL;
+  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
+      out_format != NNAB_FMT_PHASE_ANGLE)
+    return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+static int stft_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft, int F,
+                    int hop, int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
+                    size_t ws_bytes, int path, cudaStream_t stream) {
+  FramedProblem p{};
+  set_wave(p, w);
+  p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
+  p.scale = nullptr; p.scale_all = 1.f;
+  p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
+  p.out_bins = F; p.bin_offset = 0;
+  attach_splitk_scratch(p, workspace, ws_bytes);
+  return run_framed(p, packed, workspace, ws_bytes, path, stream);
+}
+
 int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, const float* wcos,
                          const float* wsin, const void* packed, int n_fft, int F, int hop,
                          int center, int pad_mode, int out_format, float sqrt_eps, float* out,
@@ -270,19 +446,10 @@ int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64
   const int pad = center ? n_fft / 2 : 0;
   int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
   if (rc) return rc;
-  if (wcos == nullptr || wsin == nullptr || out == nullptr) return NNAB_EINVAL;
-  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
-      out_format != NNAB_FMT_PHASE_ANGLE)
-    return NNAB_EINVAL;
+  if (out == nullptr || (rc = stft_args_ok(wcos, wsin, out_format))) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  FramedProblem p{};
-  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
-  p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
-  p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
-  p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
-  p.out_bins = F; p.bin_offset = 0;
-  attach_splitk_scratch(p, workspace, ws_bytes);
-  return run_framed(p, packed, workspace, ws_bytes, path, (cudaStream_t)stream);
+  return stft_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
+                  out_format, sqrt_eps, out, T, workspace, ws_bytes, path, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------- Mel / Gammatone / MFCC ----
@@ -370,9 +537,8 @@ static bool fused_fbank(int path, const void* packed, const void* fb_table, int 
          wants_tc(path, n_fft, hop);
 }
 
-size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, int hop,
-                                       int center, int n_fb, int path, int has_table) {
-  const int pad = center ? n_fft / 2 : 0;
+static size_t filterbank_ws_bytes(int64_t B, int64_t L, int n_fft, int F, int hop, int pad, int n_fb, int path,
+                                  int has_table) {
   const int64_t T = frames_of(L, n_fft, hop, pad);
   const bool tc = wants_tc(path, n_fft, hop);
   size_t n = 0;
@@ -385,15 +551,19 @@ size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, i
   return n;
 }
 
-static int power_spectrogram(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
-                             const float* wcos, const float* wsin, const void* packed,
-                             int n_fft, int F, int hop, int pad, int pad_mode, float sqrt_eps,
+size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, int hop,
+                                       int center, int n_fb, int path, int has_table) {
+  return filterbank_ws_bytes(B, L, n_fft, F, hop, center ? n_fft / 2 : 0, n_fb, path, has_table);
+}
+
+static int power_spectrogram(const Wave& w, const float* wcos, const float* wsin, const void* packed,
+                             int n_fft, int F, int hop, float sqrt_eps,
                              float power, float* P, int64_t T, void* tc_ws, size_t tc_ws_bytes,
                              int path, cudaStream_t stream) {
   FramedProblem p{};
-  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
+  set_wave(p, w);
   p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
-  p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
+  p.scale = nullptr; p.scale_all = 1.f;
   p.fmt = FMT_POWER; p.eps = sqrt_eps; p.power = power; p.out = P; p.T = T;
   p.out_bins = F; p.bin_offset = 0;
   return run_framed(p, packed, tc_ws, tc_ws_bytes, path, stream);
@@ -410,25 +580,23 @@ int nnab_stft_filterbank_forward(const float* x, int64_t B, int64_t L, int64_t x
                                          workspace, ws_bytes, path, stream);
 }
 
-int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
-                                    const float* wcos, const float* wsin, const void* packed,
-                                    int n_fft, int F, int hop, int center, int pad_mode,
-                                    float sqrt_eps, float power, const float* fb, int n_fb,
-                                    const void* fb_table, float* out, int64_t T, void* workspace,
-                                    size_t ws_bytes, int path, void* stream) {
-  const int pad = center ? n_fft / 2 : 0;
-  int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
-  if (rc) return rc;
-  if (wcos == nullptr || wsin == nullptr || fb == nullptr || out == nullptr || n_fb <= 0)
-    return NNAB_EINVAL;
-  if ((rc = check_arch())) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
+static int filterbank_args_ok(const float* wcos, const float* wsin, const float* fb, int n_fb) {
+  return (wcos == nullptr || wsin == nullptr || fb == nullptr || n_fb <= 0) ? NNAB_EINVAL : NNAB_OK;
+}
+
+static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft,
+                          int F, int hop, float sqrt_eps, float power, const float* fb, int n_fb,
+                          const void* fb_table, float* out, int64_t T, void* workspace, size_t ws_bytes, int path,
+                          cudaStream_t s) {
+  const int64_t B = w.B, L = w.L;
+  const int pad = w.pad;
+  int rc;
   bool fused = fused_fbank(path, packed, fb_table, n_fft, hop);
   if (fused) {
     FramedProblem p{};
-    p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
+    set_wave(p, w);
     p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
-    p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
+    p.scale = nullptr; p.scale_all = 1.f;
     p.fmt = FMT_FBANK; p.eps = sqrt_eps; p.power = power; p.out = out; p.T = T;
     p.out_bins = n_fb; p.bin_offset = 0;
     p.fb_table = reinterpret_cast<const FbEntry*>(fb_table); p.n_fb = n_fb;
@@ -443,7 +611,7 @@ int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64
     }
     fused = false;
   }
-  const size_t need = nnab_filterbank_workspace_bytes(B, L, n_fft, F, hop, center, n_fb, path, 0);
+  const size_t need = filterbank_ws_bytes(B, L, n_fft, F, hop, pad, n_fb, path, 0);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
   FbPlanes fp;
   if (fb_planes_enabled() && path != NNAB_PATH_SIMT && packed != nullptr && packed_kind(packed) == PACK_BLOCK &&
@@ -457,9 +625,9 @@ int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64
     const int64_t plane_stride = fp.rows * fp.kp;
     // 1. STFT -> |X| ** power as operand planes (block-partial kernel, FMT_PLANES)
     FramedProblem p{};
-    p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
+    set_wave(p, w);
     p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
-    p.pad = pad; p.pad_mode = pad_mode; p.scale = nullptr; p.scale_all = 1.f;
+    p.scale = nullptr; p.scale_all = 1.f;
     p.fmt = FMT_PLANES; p.eps = sqrt_eps; p.power = power; p.out = reinterpret_cast<float*>(planes); p.T = T;
     p.out_bins = F; p.bin_offset = 0;
     p.planes_stride = plane_stride; p.planes_pitch = fp.kp;
@@ -486,24 +654,43 @@ int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64
   }
   float* P = (float*)workspace;
   const size_t pb = power_bytes(B, F, T);
-  rc = power_spectrogram(x, x_dtype, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, pad, pad_mode,
-                         sqrt_eps, power, P, T, (char*)workspace + pb, ws_bytes - pb, path, s);
+  rc = power_spectrogram(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, P, T, (char*)workspace + pb,
+                         ws_bytes - pb, path, s);
   if (rc) return rc;
   return launch_filterbank(P, fb, B, F, T, n_fb, out, s);
+}
+
+int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
+                                    const float* wcos, const float* wsin, const void* packed,
+                                    int n_fft, int F, int hop, int center, int pad_mode,
+                                    float sqrt_eps, float power, const float* fb, int n_fb,
+                                    const void* fb_table, float* out, int64_t T, void* workspace,
+                                    size_t ws_bytes, int path, void* stream) {
+  const int pad = center ? n_fft / 2 : 0;
+  int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
+  if (rc) return rc;
+  if (out == nullptr || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
+  if ((rc = check_arch())) return rc;
+  return filterbank_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F,
+                        hop, sqrt_eps, power, fb, n_fb, fb_table, out, T, workspace, ws_bytes, path,
+                        (cudaStream_t)stream);
 }
 
 static size_t mel_bytes(int64_t B, int n_mels, int64_t T) {
   return align_up((size_t)B * n_mels * T * sizeof(float), 256);
 }
 
-size_t nnab_mfcc_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, int hop, int center,
-                                 int n_mels, int path, int has_table) {
-  const int pad = center ? n_fft / 2 : 0;
+static size_t mfcc_ws_bytes(int64_t B, int64_t L, int n_fft, int F, int hop, int pad, int n_mels, int path) {
   const int64_t T = frames_of(L, n_fft, hop, pad);
   // the un-fused size is the upper bound (a huge batch can still fall back to it)
-  const size_t fbw = nnab_filterbank_workspace_bytes(B, L, n_fft, F, hop, center, n_mels, path, 0);
-  (void)has_table;
+  const size_t fbw = filterbank_ws_bytes(B, L, n_fft, F, hop, pad, n_mels, path, 0);
   return align_up(fbw, 256) + mel_bytes(B, n_mels, T) + align_up((size_t)B * sizeof(unsigned int), 256);
+}
+
+size_t nnab_mfcc_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, int hop, int center,
+                                 int n_mels, int path, int has_table) {
+  (void)has_table;
+  return mfcc_ws_bytes(B, L, n_fft, F, hop, center ? n_fft / 2 : 0, n_mels, path);
 }
 
 int nnab_mfcc_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, const float* wcos,
@@ -517,6 +704,29 @@ int nnab_mfcc_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch, con
                               n_mfcc, out, T, workspace, ws_bytes, path, stream);
 }
 
+static int mfcc_args_ok(const float* wcos, const float* wsin, const float* mel_basis, int n_mels,
+                        const float* dct, int n_mfcc, float amin) {
+  if (wcos == nullptr || wsin == nullptr || mel_basis == nullptr || dct == nullptr || n_mels <= 0 ||
+      n_mfcc <= 0 || !(amin > 0.f))
+    return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+static int mfcc_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft, int F,
+                    int hop, float sqrt_eps, float power, const float* mel_basis, int n_mels,
+                    const void* fb_table, float amin, float ref, float top_db, const float* dct, int n_mfcc,
+                    float* out, int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream) {
+  const size_t need = mfcc_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path);
+  if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
+  const size_t fbw = align_up(filterbank_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path, 0), 256);
+  float* mel = (float*)((char*)workspace + fbw);
+  unsigned int* scratch = (unsigned int*)((char*)workspace + fbw + mel_bytes(w.B, n_mels, T));
+  int rc = filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table,
+                          mel, T, workspace, fbw, path, stream);
+  if (rc) return rc;
+  return launch_mfcc_tail(mel, w.B, n_mels, T, amin, ref, top_db, dct, n_mfcc, out, scratch, stream);
+}
+
 int nnab_mfcc_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, const float* wcos,
                          const float* wsin, const void* packed, int n_fft, int F, int hop,
                          int center, int pad_mode, float sqrt_eps, float power,
@@ -526,22 +736,11 @@ int nnab_mfcc_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64
   const int pad = center ? n_fft / 2 : 0;
   int rc = check_common(x, x_dtype, B, L, x_pitch, n_fft, F, hop, pad, pad_mode, T);
   if (rc) return rc;
-  if (wcos == nullptr || wsin == nullptr || mel_basis == nullptr || dct == nullptr ||
-      out == nullptr || n_mels <= 0 || n_mfcc <= 0 || !(amin > 0.f))
-    return NNAB_EINVAL;
+  if (out == nullptr || mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin)) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  const size_t need = nnab_mfcc_workspace_bytes(B, L, n_fft, F, hop, center, n_mels, path, 0);
-  if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
-  const size_t fbw =
-      align_up(nnab_filterbank_workspace_bytes(B, L, n_fft, F, hop, center, n_mels, path, 0), 256);
-  float* mel = (float*)((char*)workspace + fbw);
-  unsigned int* scratch = (unsigned int*)((char*)workspace + fbw + mel_bytes(B, n_mels, T));
-  rc = nnab_stft_filterbank_forward_ex(x, x_dtype, B, L, x_pitch, wcos, wsin, packed, n_fft, F, hop, center,
-                                       pad_mode, sqrt_eps, power, mel_basis, n_mels, fb_table, mel,
-                                       T, workspace, fbw, path, stream);
-  if (rc) return rc;
-  return launch_mfcc_tail(mel, B, n_mels, T, amin, ref, top_db, dct, n_mfcc, out, scratch,
-                          (cudaStream_t)stream);
+  return mfcc_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
+                  sqrt_eps, power, mel_basis, n_mels, fb_table, amin, ref, top_db, dct, n_mfcc, out, T, workspace,
+                  ws_bytes, path, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------- CQT1992v2 ----
@@ -551,6 +750,29 @@ size_t nnab_cqt1992v2_workspace_bytes(int64_t B, int64_t L, int width, int n_bin
   const int pad = center ? width / 2 : 0;
   return align_up(tc_workspace_bytes(B, L, width, hop, pad), 256) +
          tc_splitk_scratch_bytes(B, n_bins, frames_of(L, width, hop, pad), width);
+}
+
+static int cqt1992v2_args_ok(const float* k_real, const float* k_imag, int out_format) {
+  if (k_real == nullptr || k_imag == nullptr) return NNAB_EINVAL;
+  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
+      out_format != NNAB_FMT_PHASE_UNIT)
+    return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+static int cqt1992v2_run(const Wave& w, const float* k_real, const float* k_imag, const void* packed,
+                         const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins, int width, int hop,
+                         const float* scale, float scale_all, int out_format, float sqrt_eps, float* out,
+                         int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream) {
+  FramedProblem p{};
+  set_wave(p, w);
+  p.w_re = k_real; p.w_im = k_imag; p.F = n_bins; p.K = width; p.hop = hop;
+  p.scale = scale; p.scale_all = scale_all;
+  p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
+  p.out_bins = n_bins; p.bin_offset = 0;
+  p.h_k_begin = h_k_begin; p.h_k_end = h_k_end;
+  attach_splitk_scratch(p, workspace, ws_bytes);
+  return run_framed(p, packed, workspace, ws_bytes, path, stream);
 }
 
 int nnab_cqt1992v2_forward(const float* x, int64_t B, int64_t L, int64_t x_pitch,
@@ -575,20 +797,11 @@ int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, 
   const int pad = center ? width / 2 : 0;
   int rc = check_common(x, x_dtype, B, L, x_pitch, width, n_bins, hop, pad, pad_mode, T);
   if (rc) return rc;
-  if (k_real == nullptr || k_imag == nullptr || out == nullptr) return NNAB_EINVAL;
-  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX &&
-      out_format != NNAB_FMT_PHASE_UNIT)
-    return NNAB_EINVAL;
+  if (out == nullptr || cqt1992v2_args_ok(k_real, k_imag, out_format)) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  FramedProblem p{};
-  p.x = x; p.x_dtype = x_dtype; p.B = B; p.L = L; p.x_pitch = x_pitch;
-  p.w_re = k_real; p.w_im = k_imag; p.F = n_bins; p.K = width; p.hop = hop;
-  p.pad = pad; p.pad_mode = pad_mode; p.scale = scale; p.scale_all = scale_all;
-  p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
-  p.out_bins = n_bins; p.bin_offset = 0;
-  p.h_k_begin = h_k_begin; p.h_k_end = h_k_end;
-  attach_splitk_scratch(p, workspace, ws_bytes);
-  return run_framed(p, packed, workspace, ws_bytes, path, (cudaStream_t)stream);
+  return cqt1992v2_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, k_real, k_imag, packed, h_k_begin,
+                       h_k_end, n_bins, width, hop, scale, scale_all, out_format, sqrt_eps, out, T, workspace,
+                       ws_bytes, path, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------ CQT2010v2 / VQT pyramid ----
@@ -1244,6 +1457,64 @@ int nnab_istft_forward(const float* X, int64_t B, int f_in, int64_t T, const voi
   return tc_istft_finalize(ola, ola_pitch, B, window, n_fft, hop, T, offset, out, want, s);
 }
 
+size_t nnab_istft_chunk_workspace_bytes(int64_t B, int f_in, int64_t T, int n_fft, int hop) {
+  // the push's buffer holds at most T * hop + n_fft positions: that of T + 1 frames
+  return nnab_istft_workspace_bytes(B, f_in, (T > 0 ? T : 1) + 1, n_fft, hop);
+}
+
+int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const float* X, int64_t B, int f_in,
+                             int64_t T, const void* packed, const float* window, int n_fft, int hop, int center,
+                             int flush, int64_t length, float* out, int64_t out_len, void* workspace,
+                             size_t ws_bytes, void* stream) {
+  if (state == nullptr || (T > 0 && X == nullptr) || packed == nullptr || window == nullptr || B < 0 ||
+      B > 65535 || f_in <= 0)
+    return NNAB_EINVAL;
+  IstftChunkPlan pl;
+  int rc = istft_chunk_plan(frames, emitted, T, n_fft, hop, center, flush, length, &pl);
+  if (rc) return rc;
+  const int64_t n_out = pl.emit_end - pl.emit_begin;
+  if (out_len != n_out || (n_out > 0 && out == nullptr)) return NNAB_EINVAL;
+  if ((rc = check_arch())) return rc;
+  const size_t need = nnab_istft_chunk_workspace_bytes(B, f_in, T, n_fft, hop);
+  if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
+  if (B == 0 || (T == 0 && n_out == 0)) return NNAB_OK;  // nothing new: the carry stays as it is
+  cudaStream_t s = (cudaStream_t)stream;
+  float* carry = static_cast<float*>(state);
+
+  // same layout as nnab_istft_forward, with room for T + 1 frames of overlap-add positions
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  void* planes = ws;
+  int64_t ola_pitch = 0;
+  const size_t planes_b = align_up(tc_istft_planes_bytes(B, T > 0 ? T : 1, f_in), 256);
+  const size_t ola_b = istft_ola_bytes(B, (T > 0 ? T : 1) + 1, n_fft, hop, &ola_pitch);
+  float* ola = (float*)(ws + planes_b);
+  float* scale = (float*)(ws + planes_b + ola_b);
+
+  // 1. the buffer: carried partial sums, then zeros
+  NNAB_CUDA_TRY(cudaMemsetAsync(ola, 0, (size_t)B * ola_pitch * sizeof(float), s));
+  if (pl.carried > 0)
+    NNAB_CUDA_TRY(cudaMemcpy2DAsync(ola, (size_t)ola_pitch * sizeof(float), carry, (size_t)n_fft * sizeof(float),
+                                    (size_t)pl.carried * sizeof(float), (size_t)B, cudaMemcpyDeviceToDevice, s));
+  // 2. the new frames, overlap-added at their global positions (the FMT_OLA GEMM of nnab_istft_forward)
+  if (T > 0) {
+    if ((rc = tc_istft_prep(X, B, f_in, T, planes, s))) return rc;
+    istft_scale_kernel<<<(n_fft + 255) / 256, 256, 0, s>>>(window, 1.0f / (float)n_fft, n_fft, scale);
+    NNAB_LAUNCH_CHECK();
+    const int kpad = tc_istft_k(f_in);
+    FramedProblem p{};
+    p.x = nullptr; p.B = B; p.L = T * (int64_t)kpad; p.x_pitch = 0;
+    p.F = n_fft; p.K = kpad; p.hop = kpad; p.pad = 0; p.pad_mode = NNAB_PAD_CONSTANT;
+    p.scale = scale; p.scale_all = 1.f; p.fmt = FMT_OLA; p.eps = 0.f; p.power = 1.f;
+    p.out = ola + (frames * (int64_t)hop - pl.origin); p.T = T; p.out_bins = n_fft; p.bin_offset = 0;
+    p.presplit = planes;
+    p.ola_pitch = ola_pitch; p.ola_hop = hop;
+    if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
+  }
+  // 3. final samples / window sum-square at their global positions, the open tail into the carry
+  return tc_istft_chunk_finalize(ola, ola_pitch, B, window, n_fft, hop, frames + T, pl.origin, pl.emit_begin, out,
+                                 n_out, pl.carry_begin, pl.carry_len, carry, s);
+}
+
 // ------------------------------------------------------------- input gradient ----
 size_t nnab_packed_adjoint_bytes(int K, int F) { return tc_packed_istft_bytes(K, F); }
 
@@ -1339,6 +1610,112 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
   p.k_splits_hint = (int)((gpad / 64 + 63) / 64);  // <= 64 k-blocks per accumulator chunk
   if (p.k_splits_hint > 64) p.k_splits_hint = 64;
   return run_framed(p, frames, nullptr, 0, NNAB_PATH_TCGEN05, s);
+}
+
+// ------------------------------------------------------------ chunked streams ----
+size_t nnab_chunk_state_bytes(int64_t B, int K) {
+  return (B <= 0 || K <= 0) ? 0 : (size_t)B * K * sizeof(float);
+}
+
+size_t nnab_stft_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                       int n_fft, int F, int hop, int center, int pad_mode, int path) {
+  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return Lv > 0 ? nnab_stft_workspace_bytes(B, Lv, n_fft, F, hop, 0, path) : 0;
+}
+
+int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                            int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush,
+                            const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                            int center, int pad_mode, int out_format, float sqrt_eps, float* out, int64_t T,
+                            void* workspace, size_t ws_bytes, int path, void* stream) {
+  ChunkPlan cp;
+  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  if (rc) return rc;
+  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
+  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+    return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+size_t nnab_filterbank_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                             int n_fft, int F, int hop, int center, int pad_mode, int n_fb,
+                                             int path, int has_table) {
+  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return Lv > 0 ? filterbank_ws_bytes(B, Lv, n_fft, F, hop, 0, n_fb, path, has_table) : 0;
+}
+
+int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                       const void* chunk, int chunk_dtype, int64_t B, int64_t n,
+                                       int64_t chunk_pitch, int flush, const float* wcos, const float* wsin,
+                                       const void* packed, int n_fft, int F, int hop, int center, int pad_mode,
+                                       float sqrt_eps, float power, const float* fb, int n_fb,
+                                       const void* fb_table, float* out, int64_t T, void* workspace,
+                                       size_t ws_bytes, int path, void* stream) {
+  ChunkPlan cp;
+  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  if (rc) return rc;
+  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb))
+    return NNAB_EINVAL;
+  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+    return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T,
+                          workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+size_t nnab_mfcc_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                       int n_fft, int F, int hop, int center, int pad_mode, int n_mels, int path,
+                                       int has_table) {
+  (void)has_table;
+  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return Lv > 0 ? mfcc_ws_bytes(B, Lv, n_fft, F, hop, 0, n_mels, path) : 0;
+}
+
+int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                            int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush,
+                            const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                            int center, int pad_mode, float sqrt_eps, float power, const float* mel_basis,
+                            int n_mels, const void* fb_table, float amin, float ref, float top_db,
+                            const float* dct, int n_mfcc, float* out, int64_t T, void* workspace,
+                            size_t ws_bytes, int path, void* stream) {
+  ChunkPlan cp;
+  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  if (rc) return rc;
+  // the top_db floor is a maximum over the whole clip: a stream cannot apply it frame by frame
+  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || top_db >= 0.f ||
+      mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin))
+    return NNAB_EINVAL;
+  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+    return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
+                    ref, top_db, dct, n_mfcc, out, T, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+size_t nnab_cqt1992v2_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
+                                            int width, int n_bins, int hop, int center, int pad_mode, int path) {
+  const int64_t Lv = chunk_clip_length(received, frames, n, flush, width, hop, center ? width / 2 : 0, pad_mode);
+  return Lv > 0 ? nnab_cqt1992v2_workspace_bytes(B, Lv, width, n_bins, hop, 0, path) : 0;
+}
+
+int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                 const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
+                                 int flush, const float* k_real, const float* k_imag, const void* packed,
+                                 const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins, int width,
+                                 int hop, int center, int pad_mode, const float* scale, float scale_all,
+                                 int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
+                                 size_t ws_bytes, int path, void* stream) {
+  ChunkPlan cp;
+  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, width, hop,
+                      center ? width / 2 : 0, pad_mode, &cp);
+  if (rc) return rc;
+  if (T != cp.T || n_bins <= 0 || (T > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
+    return NNAB_EINVAL;
+  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+    return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
+                         out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
+  }, stream);
 }
 
 }  // extern "C"

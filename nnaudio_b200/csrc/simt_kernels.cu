@@ -134,6 +134,7 @@ int launch_framed_simt(const FramedProblem& q, cudaStream_t stream) {
   if (q.B <= 0 || q.T <= 0 || q.F <= 0) return NNAB_OK;
   if (q.B > 65535) return NNAB_EUNSUPPORTED;
   if (q.x_dtype != NNAB_DTYPE_F32) return NNAB_EUNSUPPORTED;  // this kernel reads fp32 samples only
+  if (q.chunk != nullptr) return NNAB_EUNSUPPORTED;           // ... of a plain waveform
   SimtParams p;
   p.x = static_cast<const float*>(q.x); p.L = q.L; p.x_pitch = q.x_pitch;
   p.w_re = q.w_re; p.w_im = q.w_im;

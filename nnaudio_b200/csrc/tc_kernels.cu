@@ -175,6 +175,90 @@ static int launch_pad_split(dim3 grid, cudaStream_t stream, const void* x, int x
   return NNAB_OK;
 }
 
+// pad_split_kernel on a push's virtual clip (ChunkSource): each sample is taken from the fp32 carry ring or
+// the chunk, with the reflect / constant centre padding of the whole stream at its two ends.  The planes of
+// frame t0 + j are then those the whole-clip pre-pass writes for frame t0 + j.
+template <typename Tx>
+__global__ void __launch_bounds__(256) chunk_split_kernel(
+    ChunkSource c, const Tx* __restrict__ chunk, int shift, int64_t clip_pitch, int64_t plane_stride,
+    __nv_bfloat16* __restrict__ planes) {
+  const int64_t b = blockIdx.y;
+  const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if (i0 >= clip_pitch) return;
+  const float* __restrict__ ring = c.ring + b * c.ring_pitch;
+  const Tx* __restrict__ xb = chunk + b * c.chunk_pitch;
+  const bool reflect = c.pad_mode == NNAB_PAD_REFLECT;
+  __align__(16) __nv_bfloat16 hi[8];
+  __align__(16) __nv_bfloat16 lo[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int64_t i = i0 + shift + e;
+    float v = 0.f;
+    if (i < c.length) {
+      int64_t r = c.origin + i;
+      bool live = true;
+      if (r < 0) {
+        if (reflect) r = -r; else live = false;
+      } else if (r >= c.total) {
+        if (c.at_end && reflect) r = 2 * (c.total - 1) - r; else live = false;
+      }
+      if (live) v = r < c.received ? __ldg(ring + r % c.ring_len) : sample_f32(__ldg(xb + (r - c.received)));
+    }
+    split_bf16(v, hi[e], lo[e]);
+  }
+  const int64_t o = b * clip_pitch + i0;
+  *reinterpret_cast<uint4*>(planes + o) = *reinterpret_cast<const uint4*>(hi);
+  *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
+}
+
+// Raw samples [from, total) of the chunk into the carry ring.  Runs after every kernel of the push that reads
+// the ring (same stream), and never overwrites a sample the next push reads: the ring holds ring_len >= the
+// longest carry.
+template <typename Tx>
+__global__ void __launch_bounds__(256) chunk_carry_kernel(ChunkSource c, const Tx* __restrict__ chunk,
+                                                          int64_t from) {
+  const int64_t b = blockIdx.y;
+  const int64_t r = from + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= c.total) return;
+  const_cast<float*>(c.ring)[b * c.ring_pitch + r % c.ring_len] =
+      sample_f32(__ldg(chunk + b * c.chunk_pitch + (r - c.received)));
+}
+
+template <typename F>
+static int with_sample_type(int x_dtype, const void* x, F&& f) {
+  if (x_dtype == NNAB_DTYPE_F32) f(static_cast<const float*>(x));
+  else if (x_dtype == NNAB_DTYPE_BF16) f(static_cast<const __nv_bfloat16*>(x));
+  else if (x_dtype == NNAB_DTYPE_F16) f(static_cast<const __half*>(x));
+  else return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+// The pre-pass of every tensor-core launcher: the planes of q's signal, shifted by `shift` samples.
+static int launch_problem_split(const FramedProblem& q, dim3 grid, int shift, int64_t clip_pitch,
+                                int64_t plane_stride, __nv_bfloat16* planes, cudaStream_t stream) {
+  if (q.chunk == nullptr)
+    return launch_pad_split(grid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, shift, clip_pitch,
+                            plane_stride, planes);
+  const int rc = with_sample_type(q.x_dtype, q.chunk->chunk, [&](auto* xs) {
+    chunk_split_kernel<<<grid, 256, 0, stream>>>(*q.chunk, xs, shift, clip_pitch, plane_stride, planes);
+  });
+  if (rc) return rc;
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream) {
+  if (from >= cs.total || B <= 0) return NNAB_OK;
+  if (B > 65535) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(cs.total - from, 256), (unsigned)B);
+  const int rc = with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    chunk_carry_kernel<<<grid, 256, 0, stream>>>(cs, xs, from);
+  });
+  if (rc) return rc;
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
 // Two differently padded split copies of the same batch in one pass over x (level 0 of
 // the CQT pyramid: reflect-padded copy for the octave CQT + zero-margin copy for the FIR).
 template <typename Tx>
@@ -312,18 +396,24 @@ static int zero_tail(__nv_bfloat16* planes, const SplitGeom& g, int hop_eff, cud
 }
 
 // phase-0 pad + split of a batch into caller-managed planes
-int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
-                 int pad_mode, void* planes_v, cudaStream_t stream) {
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  const SplitGeom g = split_geom(B, L, K, hop, pad);
-  const int hop_eff = hop * num_phases(hop);
+int tc_problem_split(const FramedProblem& q, void* planes_v, cudaStream_t stream) {
+  if (q.B > 65535) return NNAB_EUNSUPPORTED;
+  const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
+  const int hop_eff = q.hop * num_phases(q.hop);
   __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
   int rc = zero_tail(planes, g, hop_eff, stream);
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * hop_eff;
-  dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
-  return launch_pad_split(grid, stream, x, x_dtype, L, x_pitch, pad, pad_mode, 0, clip_pitch, g.plane_stride,
-                          planes);
+  dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
+  return launch_problem_split(q, grid, 0, clip_pitch, g.plane_stride, planes, stream);
+}
+
+int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
+                 int pad_mode, void* planes_v, cudaStream_t stream) {
+  FramedProblem q{};
+  q.x = x; q.x_dtype = x_dtype; q.B = B; q.L = L; q.x_pitch = x_pitch;
+  q.K = K; q.hop = hop; q.pad = pad; q.pad_mode = pad_mode;
+  return tc_problem_split(q, planes_v, stream);
 }
 
 __global__ void zero_margins_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride,
@@ -713,6 +803,49 @@ int tc_istft_finalize(const float* ola, int64_t ola_pitch, int64_t B, const floa
   dim3 grid((unsigned)ceil_div64(out_len, 256), (unsigned)B);
   istft_finalize_kernel<<<grid, 256, 0, stream>>>(ola, ola_pitch, window, n_fft, hop, T, offset,
                                                   out, out_len);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+// One push of a streamed inverse STFT.  `ola` holds overlap-add positions [origin, ...) of the stream (the
+// carried partial sums, then this push's frames).  Samples [emit_begin, emit_begin + out_len) are final: divided
+// by the window sum-square of their GLOBAL position over the T frames received so far (the same sum, in the same
+// order, as istft_finalize_kernel) and written to out.  Positions [carry_begin, carry_begin + carry_len), still
+// open to later frames, go un-normalised into the carry state (rows of n_fft floats).
+__global__ void __launch_bounds__(256) istft_chunk_finalize_kernel(
+    const float* __restrict__ ola, int64_t ola_pitch, const float* __restrict__ window, int n_fft, int hop,
+    int64_t T, int64_t origin, int64_t emit_begin, float* __restrict__ out, int64_t out_len, int64_t carry_begin,
+    int64_t carry_len, float* __restrict__ carry) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t b = blockIdx.y;
+  const float* __restrict__ row = ola + b * ola_pitch;
+  if (i < out_len) {
+    const int64_t s = emit_begin + i;
+    int64_t t_hi = s / hop;
+    if (t_hi > T - 1) t_hi = T - 1;
+    float wss = 0.f;
+    for (int64_t t = t_hi; t >= 0; --t) {
+      const int64_t n = s - t * hop;
+      if (n >= n_fft) break;
+      const float w = __ldg(window + n);
+      wss = fmaf(w, w, wss);
+    }
+    float v = row[s - origin];
+    if (wss > 1e-10f) v = v / wss;
+    out[b * out_len + i] = v;
+  }
+  if (i < carry_len) carry[b * n_fft + i] = row[carry_begin - origin + i];
+}
+
+int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window, int n_fft,
+                            int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
+                            int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream) {
+  if (B > 65535) return NNAB_EUNSUPPORTED;
+  const int64_t n = out_len > carry_len ? out_len : carry_len;
+  if (n <= 0 || B <= 0) return NNAB_OK;
+  dim3 grid((unsigned)ceil_div64(n, 256), (unsigned)B);
+  istft_chunk_finalize_kernel<<<grid, 256, 0, stream>>>(ola, ola_pitch, window, n_fft, hop, T, origin, emit_begin,
+                                                        out, out_len, carry_begin, carry_len, carry);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -1479,9 +1612,7 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * q.hop;
   dim3 pgrid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-  if ((rc = launch_pad_split(pgrid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, 0, clip_pitch,
-                             g.plane_stride, planes)))
-    return rc;
+  if ((rc = launch_problem_split(q, pgrid, 0, clip_pitch, g.plane_stride, planes, stream))) return rc;
 
   // split-K only with the caller's raw scratch (long kernels): <= 64 K blocks per accumulator
   VarNPlan plan;
@@ -1728,9 +1859,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     prm.T = (q.T - ph + n_ph - 1) / n_ph;  // frames t = ph, ph + n_ph, ... < T
     if (q.presplit == nullptr) {
       dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-      if ((rc = launch_pad_split(grid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, ph * q.hop,
-                                 clip_pitch, g.plane_stride, planes)))
-        return rc;
+      if ((rc = launch_problem_split(q, grid, ph * q.hop, clip_pitch, g.plane_stride, planes, stream))) return rc;
     }
     {
       double kcols = 0.0;  // sum over N tiles of (k-blocks executed) x bk x bn

@@ -597,7 +597,7 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
   __nv_bfloat16* planes =
       reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  int rc = tc_pad_split(q.x, q.x_dtype, q.B, q.L, q.x_pitch, q.K, q.hop, q.pad, q.pad_mode, planes, stream);
+  int rc = tc_problem_split(q, planes, stream);
   if (rc) return rc;
   // a bf16 waveform has an all-zero lo plane: the xlo * whi pass would add exact zeros
   const int passes = (q.x_dtype == NNAB_DTYPE_BF16) ? 2 : 3;

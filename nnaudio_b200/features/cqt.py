@@ -35,6 +35,18 @@ def _check_format_and_norm(output_format, normalization_type):
         )
 
 
+def _check_cqt_length(mod, B, n):
+    """The reference's exceptions for ``B`` clips of ``n`` samples through a framed CQT (cqt.py:740-750)."""
+    pad = mod.kernel_width // 2 if mod.center else 0
+    if mod.center and mod.pad_mode == "reflect" and n <= pad:
+        raise RuntimeError(
+            "Padding size should be less than the corresponding input dimension, but got: "
+            f"padding ({pad}, {pad}) at dimension 2 of input {(B, 1, n)}"
+        )
+    if n + 2 * pad < mod.kernel_width:
+        raise RuntimeError("Kernel size can't be greater than actual input size")
+
+
 class _ScaleCache:
     """sqrt(lenghts) * factor on the device, recomputed when ``lenghts`` changes."""
 
@@ -119,19 +131,12 @@ class CQT1992v2(nn.Module):
         key = (kr.data_ptr(), kr._version, ki.data_ptr(), ki._version)
         return self._support.lookup(kr.device, key, build)
 
-    def forward(self, x, output_format=None, normalization_type="librosa"):
-        output_format = output_format or self.output_format
-        _check_format_and_norm(output_format, normalization_type)
-        x = broadcast_dim(x)
-        pad = self.kernel_width // 2 if self.center else 0
-        if self.center and self.pad_mode == "reflect" and x.shape[-1] <= pad:
-            raise RuntimeError(
-                "Padding size should be less than the corresponding input dimension, but got: "
-                f"padding ({pad}, {pad}) at dimension 2 of input {tuple(x[:, None, :].shape)}"
-            )
-        if x.shape[-1] + 2 * pad < self.kernel_width:
-            raise RuntimeError("Kernel size can't be greater than actual input size")
+    def _check_length(self, B, n):
+        """Raise what the reference raises for ``B`` clips of ``n`` samples (also the end of a stream)."""
+        _check_cqt_length(self, B, n)
 
+    def _infer_args(self, output_format, normalization_type):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path."""
         k_real, k_imag = as_matrix(self.cqt_kernels_real), as_matrix(self.cqt_kernels_imag)
         packed = self._packed.get(k_real, k_imag,
                                   groups=(not self.trainable) and self.hop_length % 8 == 0)
@@ -142,6 +147,22 @@ class CQT1992v2(nn.Module):
         elif normalization_type == "wrap":
             scale_all = 2.0
         eps = 1e-8 if (self.trainable and output_format == "Magnitude") else 0.0
+        return "cqt1992v2_forward", dict(
+            k_real=k_real, k_imag=k_imag, packed=packed, k_begin=k_begin, k_end=k_end, hop=self.hop_length,
+            center=self.center, pad_mode=pad_mode_id(self.pad_mode), scale=scale, scale_all=scale_all,
+            out_format=_FORMATS[output_format], sqrt_eps=eps,
+        )
+
+    def forward(self, x, output_format=None, normalization_type="librosa"):
+        output_format = output_format or self.output_format
+        _check_format_and_norm(output_format, normalization_type)
+        x = broadcast_dim(x)
+        self._check_length(x.shape[0], x.shape[-1])
+
+        args = self._infer_args(output_format, normalization_type)[1]
+        k_real, k_imag, packed = args["k_real"], args["k_imag"], args["packed"]
+        k_begin, k_end = args["k_begin"], args["k_end"]
+        scale, scale_all, eps = args["scale"], args["scale_all"], args["sqrt_eps"]
         if wants_grad(self, x):
             # un-normalised complex CQT through the fused kernel + dX / dW kernels; normalisation and
             # output format (cqt.py:752-780) composed in torch for autograd
@@ -175,10 +196,7 @@ class CQT1992v2(nn.Module):
                 return torch.sqrt(c[..., 0].pow(2) + c[..., 1].pow(2) + eps)
             ang = torch.atan2(c[..., 1], c[..., 0])
             return torch.stack((torch.cos(ang), torch.sin(ang)), -1)
-        return _C.cqt1992v2_forward(
-            x, k_real, k_imag, packed, k_begin, k_end, self.hop_length, self.center,
-            pad_mode_id(self.pad_mode), scale, scale_all, _FORMATS[output_format], eps,
-        )
+        return _C.cqt1992v2_forward(x, **args)
 
 
 class CQT(CQT1992v2):

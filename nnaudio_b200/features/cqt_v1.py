@@ -26,7 +26,7 @@ from scipy.fftpack import fft as _fft
 
 from .. import _C, design
 from ._common import PackedBasis, PerDeviceCache, broadcast_dim, pad_mode_id, upcast_16bit, wants_grad
-from .cqt import (_ScaleCache, _check_format_and_norm, _framed_complex_autograd,
+from .cqt import (_ScaleCache, _check_cqt_length, _check_format_and_norm, _framed_complex_autograd,
                   _pyramid_forward)
 
 
@@ -136,25 +136,8 @@ class CQT1992(nn.Module):
         output_format = output_format or self.output_format
         _check_format_and_norm(output_format, normalization_type)
         x = broadcast_dim(x)
-        width = self.kernel_width
-        pad = width // 2 if self.center else 0
-        if self.center and self.pad_mode == "reflect" and x.shape[-1] <= pad:
-            raise RuntimeError(
-                "Padding size should be less than the corresponding input dimension, but got: "
-                f"padding ({pad}, {pad}) at dimension 2 of input {tuple(x[:, None, :].shape)}"
-            )
-        if x.shape[-1] + 2 * pad < width:
-            raise RuntimeError("Kernel size can't be greater than actual input size")
-        mode = pad_mode_id(self.pad_mode) if self.center else _C.PAD_CONSTANT
-
-        scale, scale_all = None, 1.0
-        if normalization_type == "librosa":  # sqrt(lenghts) / kernel_width, cqt.py:224-225
-            scale = self._scale.get(self.lenghts, 1.0 / width)
-        elif normalization_type == "wrap":
-            scale_all = 2.0 / width
-        # 'Phase' takes atan2 of the *un-negated* imaginary part (cqt.py:246-249), the other
-        # formats stack (real, -imag) (cqt.py:222): choose the sign of the imaginary rows to match
-        negate = output_format == "Phase"
+        self._check_length(x.shape[0], x.shape[-1])
+        mode, scale, scale_all, negate = self._plan(output_format, normalization_type)
         if wants_grad(self, x):
             if _has_trainable(self):
                 w_re, w_im = self._folded.differentiable(self, negate)
@@ -172,11 +155,35 @@ class CQT1992(nn.Module):
                 return torch.sqrt(c[..., 0].pow(2) + c[..., 1].pow(2))
             ang = torch.atan2(c[..., 1], c[..., 0])
             return torch.stack((torch.cos(ang), torch.sin(ang)), -1)
+        return _C.cqt1992v2_forward(x, **self._infer_args(output_format, normalization_type)[1])
+
+    def _check_length(self, B, n):
+        """Raise what the reference raises for ``B`` clips of ``n`` samples (also the end of a stream)."""
+        _check_cqt_length(self, B, n)
+
+    def _plan(self, output_format, normalization_type):
+        width = self.kernel_width
+        mode = pad_mode_id(self.pad_mode) if self.center else _C.PAD_CONSTANT
+        scale, scale_all = None, 1.0
+        if normalization_type == "librosa":  # sqrt(lenghts) / kernel_width, cqt.py:224-225
+            scale = self._scale.get(self.lenghts, 1.0 / width)
+        elif normalization_type == "wrap":
+            scale_all = 2.0 / width
+        # 'Phase' takes atan2 of the *un-negated* imaginary part (cqt.py:246-249), the other
+        # formats stack (real, -imag) (cqt.py:222): choose the sign of the imaginary rows to match
+        negate = output_format == "Phase"
+        return mode, scale, scale_all, negate
+
+    def _infer_args(self, output_format, normalization_type):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path."""
+        mode, scale, scale_all, negate = self._plan(output_format, normalization_type)
         w_re, w_im, packed = self._folded.get(self, negate)
         fmt = {"Magnitude": _C.FMT_MAGNITUDE, "Complex": _C.FMT_COMPLEX,
                "Phase": _C.FMT_PHASE_UNIT}[output_format]
-        return _C.cqt1992v2_forward(x, w_re, w_im, packed, None, None, self.hop_length,
-                                    self.center, mode, scale, scale_all, fmt, 0.0)
+        return "cqt1992v2_forward", dict(
+            k_real=w_re, k_imag=w_im, packed=packed, k_begin=None, k_end=None, hop=self.hop_length,
+            center=self.center, pad_mode=mode, scale=scale, scale_all=scale_all, out_format=fmt, sqrt_eps=0.0,
+        )
 
     def extra_repr(self) -> str:
         return "STFT kernel size = {}, CQT kernel size = {}".format(

@@ -77,14 +77,19 @@ class Gammatonegram(nn.Module):
         x = self.stft._checked_input(x)
         if wants_grad(self, x):
             return torch.matmul(self.gammatone_basis, self.stft._magnitude_diff(upcast_16bit(x)) ** self.power)
+        return _C.stft_filterbank_forward(x, **self._infer_args()[1])
+
+    def _infer_args(self):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path."""
         wcos, wsin, packed = self.stft._bases(block_ok=True)
         fb = self.gammatone_basis.detach()
         _C._dev_f32(fb, "gammatone_basis")
         fb = fb if fb.is_contiguous() else fb.contiguous()
         eps = 1e-8 if self.stft.trainable else 0.0
-        return _C.stft_filterbank_forward(
-            x, wcos, wsin, packed, self.n_fft, self.stride, self.center,
-            pad_mode_id(self.pad_mode), eps, float(self.power), fb, self._fb_table.get(fb),
+        return "stft_filterbank_forward", dict(
+            wcos=wcos, wsin=wsin, packed=packed, n_fft=self.n_fft, hop=self.stride, center=self.center,
+            pad_mode=pad_mode_id(self.pad_mode), sqrt_eps=eps, power=float(self.power), fb=fb,
+            fb_table=self._fb_table.get(fb),
         )
 
     def extra_repr(self) -> str:

@@ -82,14 +82,19 @@ class MelSpectrogram(nn.Module):
         x = self.stft._checked_input(x)
         if wants_grad(self, x):  # mel.py:186-188 on top of the differentiable STFT magnitude
             return torch.matmul(self._filterbank(), self.stft._magnitude_diff(upcast_16bit(x)) ** self.power)
+        return _C.stft_filterbank_forward(x, **self._infer_args()[1])
+
+    def _infer_args(self):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path."""
         wcos, wsin, packed = self.stft._bases(block_ok=True)
         fb = self._filterbank().detach()
         _C._dev_f32(fb, "filterbank")
         fb = fb if fb.is_contiguous() else fb.contiguous()
         eps = 1e-8 if self.stft.trainable else 0.0
-        return _C.stft_filterbank_forward(
-            x, wcos, wsin, packed, self.n_fft, self.stride, self.center,
-            pad_mode_id(self.pad_mode), eps, float(self.power), fb, self._fb_table.get(fb),
+        return "stft_filterbank_forward", dict(
+            wcos=wcos, wsin=wsin, packed=packed, n_fft=self.n_fft, hop=self.stride, center=self.center,
+            pad_mode=pad_mode_id(self.pad_mode), sqrt_eps=eps, power=float(self.power), fb=fb,
+            fb_table=self._fb_table.get(fb),
         )
 
     def extra_repr(self) -> str:
@@ -142,15 +147,21 @@ class MFCC(nn.Module):
                 peak = log_spec.flatten(1).max(1)[0][:, None, None]
                 log_spec = torch.max(log_spec, peak - self.top_db)
             return torch.matmul(self._dct_rows, log_spec)
+        return _C.mfcc_forward(x, **self._infer_args()[1])
+
+    def _infer_args(self):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path."""
+        mel = self.melspec_layer
         wcos, wsin, packed = mel.stft._bases(block_ok=True)
         fb = mel.mel_basis.detach()
         _C._dev_f32(fb, "mel_basis")
         fb = fb if fb.is_contiguous() else fb.contiguous()
         eps = 1e-8 if mel.stft.trainable else 0.0
-        return _C.mfcc_forward(
-            x, wcos, wsin, packed, mel.n_fft, mel.stride, mel.center, pad_mode_id(mel.pad_mode),
-            eps, float(mel.power), fb, self._amin_host, self._ref_host, self.top_db,
-            self._dct_rows, mel._fb_table.get(fb),
+        return "mfcc_forward", dict(
+            wcos=wcos, wsin=wsin, packed=packed, n_fft=mel.n_fft, hop=mel.stride, center=mel.center,
+            pad_mode=pad_mode_id(mel.pad_mode), sqrt_eps=eps, power=float(mel.power), mel_basis=fb,
+            amin=self._amin_host, ref=self._ref_host, top_db=self.top_db, dct=self._dct_rows,
+            fb_table=mel._fb_table.get(fb),
         )
 
     def extra_repr(self) -> str:

@@ -79,15 +79,15 @@ class _InverseSTFTFn(torch.autograd.Function):
         return ctx.grad_spec(gy.contiguous().float(), ctx.T), None, None
 
 
-def _inverse_stft(mod, X, kernel_cos, kernel_sin, window_mask, onesided, length):
-    """Shared by ``STFT.inverse`` and ``iSTFT.forward`` (STFTBase.inverse_stft, stft.py:15-63)."""
+def _inverse_args(mod, f_in, kernel_cos, kernel_sin, window_mask, onesided):
+    """(kc, ks, packed, win) of an inverse STFT of ``f_in``-bin spectra, with the reference's exceptions;
+    shared by the offline inverse and ``nnaudio_b200.streaming.StreamingInverse``."""
     n_fft = mod.n_fft
     kc = kernel_cos.detach().reshape(kernel_cos.shape[0], -1)
     ks = kernel_sin.detach().reshape(kernel_sin.shape[0], -1)
     _C._dev_f32(kc, "kernel_cos")
     if kc.shape != (n_fft, n_fft) or ks.shape != (n_fft, n_fft):
         raise RuntimeError("inverse kernels must be (n_fft, n_fft)")
-    f_in = X.shape[1]
     expect = n_fft // 2 + 1 if onesided else n_fft
     if f_in != expect:
         raise RuntimeError(
@@ -102,7 +102,13 @@ def _inverse_stft(mod, X, kernel_cos, kernel_sin, window_mask, onesided, length)
     if not hasattr(mod, "_inv_basis"):
         mod._inv_basis = _InverseBasis()
     packed = mod._inv_basis.get(kc.contiguous(), ks.contiguous(), f_in, onesided)
-    win = win.contiguous()
+    return kc, ks, packed, win.contiguous()
+
+
+def _inverse_stft(mod, X, kernel_cos, kernel_sin, window_mask, onesided, length):
+    """Shared by ``STFT.inverse`` and ``iSTFT.forward`` (STFTBase.inverse_stft, stft.py:15-63)."""
+    n_fft = mod.n_fft
+    kc, ks, packed, win = _inverse_args(mod, X.shape[1], kernel_cos, kernel_sin, window_mask, onesided)
 
     def run(spec):
         return _C.istft_forward(spec, packed, win, n_fft, mod.stride, mod.center, length)
@@ -220,19 +226,23 @@ class STFT(nn.Module):
         (utils.py:219-221, stft.py:283-286)."""
         self.num_samples = x.shape[-1]
         x = broadcast_dim(x)
+        self._check_length(self.num_samples)
+        return x
+
+    def _check_length(self, n):
+        """Raise what the reference raises for a clip of ``n`` samples (also the end of a stream)."""
         if self.center and self.pad_mode == "reflect":
-            if self.num_samples < self.pad_amount:
+            if n < self.pad_amount:
                 raise AssertionError(
                     "Signal length shorter than reflect padding length (n_fft // 2)."
                 )
-            if self.num_samples == self.pad_amount:
+            if n == self.pad_amount:
                 raise RuntimeError(
                     "Padding size should be less than the corresponding input dimension"
                 )
         pad = self.pad_amount if self.center else 0
-        if self.num_samples + 2 * pad < self.n_fft:
+        if n + 2 * pad < self.n_fft:
             raise RuntimeError("Kernel size can't be greater than actual input size")
-        return x
 
     def _bases(self, block_ok=False):
         """``block_ok``: the caller's output format has a block-partial epilogue (all STFT formats,
@@ -245,13 +255,18 @@ class STFT(nn.Module):
         block_hop = self.stride if (block_ok and not self.trainable) else 0
         return wcos, wsin, self._packed.get(wcos, wsin, block_hop=block_hop)
 
-    def _run(self, x, output_format):
+    def _infer_args(self, output_format):
+        """(name, keyword arguments after ``x``) of the ``_C`` call of the inference path; the streaming
+        API (nnaudio_b200.streaming) makes the same call per chunk."""
         wcos, wsin, packed = self._bases(block_ok=True)
         eps = 1e-8 if (self.trainable and output_format == "Magnitude") else 0.0
-        return _C.stft_forward(
-            x, wcos, wsin, packed, self.n_fft, self.stride, self.center,
-            pad_mode_id(self.pad_mode), _FORMATS[output_format], eps,
+        return "stft_forward", dict(
+            wcos=wcos, wsin=wsin, packed=packed, n_fft=self.n_fft, hop=self.stride, center=self.center,
+            pad_mode=pad_mode_id(self.pad_mode), out_format=_FORMATS[output_format], sqrt_eps=eps,
         )
+
+    def _run(self, x, output_format):
+        return _C.stft_forward(x, **self._infer_args(output_format)[1])
 
     def _backward_input(self, g, L):
         wcos, wsin, _ = self._bases()

@@ -1,0 +1,274 @@
+"""Chunk-by-chunk streaming through the forward transforms and the inverse STFT (DESIGN.md §3.10).
+
+``StreamingTransform(module, batch)`` runs ``batch`` streams that advance together.  Each ``push(chunk)``
+returns every frame whose samples have all arrived; ``flush()`` returns the rest, with the module's right
+padding.  Concatenated along time, the outputs equal ``module(x)`` on the whole stream: same frame count,
+same reflect / constant padding at both ends, bit for bit on the tensor-core routes (for a 16-bit stream:
+bit for bit ``module(x.float())``).  One exception: the CQT1992v2 tall kernel picks its balanced tile schedule
+from a launch's tile count, so a whole-clip call on that schedule and pushes on the static one agree to 2e-6.
+
+Each push is one C call on the offline kernels (``_C.*_chunk_forward``): the tensor-core pre-pass builds its
+bf16 planes from the carried fp32 samples and the new chunk.  Plans that read the waveform as fp32 directly
+(the SIMT kernels, ``NNAUDIO_B200_PATH=simt``) take the concat route instead: the carried samples and the
+upcast chunk, padded and concatenated with torch, through the module's offline call with ``center=False``.
+A push never reads the device back or synchronises.
+
+``StreamingInverse(module, batch)`` streams complex frames through the inverse STFT: each push returns the
+output samples no later frame can change, ``flush(length=None)`` the rest.
+"""
+from __future__ import annotations
+
+import torch
+
+from . import _C
+from .features.cqt import CQT1992v2
+from .features.cqt_v1 import CQT1992
+from .features.gammatone import Gammatonegram
+from .features.mel import MFCC, MelSpectrogram
+from .features.stft import STFT, _inverse_args, iSTFT
+
+__all__ = ["StreamingTransform", "StreamingInverse"]
+
+_SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
+
+
+def _ready_frames(total, K, hop, pad, reflect):
+    """Frames whose raw samples have all arrived after ``total`` samples: frame t reads up to raw sample
+    t * hop + K - pad - 1, and with reflect padding frame 0 also mirrors raw sample ``pad``."""
+    if reflect and total < pad + 1:
+        return 0
+    need = K - pad
+    return 0 if total < need else (total - need) // hop + 1
+
+
+def _carry_start(total, frames, hop, pad):
+    """First raw sample the next push reads (the carry ring holds [start, total))."""
+    s = frames * hop - pad
+    if pad > 0:
+        s = min(s, total - (pad + 1))  # the right mirror of the last push reads pad + 1 samples back
+    return min(max(s, 0), total)
+
+
+class StreamingTransform:
+    """Stream ``batch`` signals chunk by chunk through ``module``.
+
+    ``module``: ``STFT``, ``MelSpectrogram``, ``Gammatonegram``, ``MFCC`` (``top_db=None`` only),
+    ``CQT1992v2`` / ``CQT`` or ``CQT1992``.  ``forward_kwargs`` are passed on as the module's ``forward``
+    keywords (``output_format``, ``normalization_type``).
+    """
+
+    def __init__(self, module, batch, _strict=False, **forward_kwargs):
+        if not isinstance(module, _SUPPORTED):
+            raise TypeError(
+                f"StreamingTransform supports STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2 / CQT and "
+                f"CQT1992, not {type(module).__name__} (the CQT2010 pyramids carry per-octave filter state)"
+            )
+        if isinstance(module, MFCC) and module.top_db is not None:
+            raise ValueError(
+                "MFCC with top_db set cannot be streamed: its floor is a maximum over the whole clip. "
+                "Build the module with top_db=None."
+            )
+        batch = int(batch)
+        if batch < 1 or batch > _C.MAX_BATCH:
+            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        self.module, self.batch, self._strict = module, batch, bool(_strict)
+        if isinstance(module, (CQT1992v2, CQT1992)):
+            fmt = forward_kwargs.get("output_format") or module.output_format
+            norm = forward_kwargs.get("normalization_type", "librosa")
+            self._args = lambda: module._infer_args(fmt, norm)
+            self._check_length = lambda n: module._check_length(self.batch, n)
+            self.K = module.kernel_width
+        else:
+            stft = module.melspec_layer.stft if isinstance(module, MFCC) else (
+                module if isinstance(module, STFT) else module.stft)
+            if isinstance(module, STFT):
+                fmt = forward_kwargs.get("output_format") or module.output_format
+                self._args = lambda: module._infer_args(fmt)
+            else:
+                self._args = module._infer_args
+            self._check_length = stft._check_length
+            self.K = stft.n_fft
+        name, kw = self._args()
+        self.hop = kw["hop"]
+        self.pad = self.K // 2 if kw["center"] else 0
+        self._reflect = self.pad > 0 and kw["pad_mode"] == _C.PAD_REFLECT
+        device = next(iter(module.buffers())).device
+        self.ring = torch.empty((batch, self.K), dtype=torch.float32, device=device)  # carried raw samples
+        self.reset()
+
+    def reset(self):
+        """Start new streams (same module, same batch)."""
+        self.received = self.n_carry = self.frames = 0
+        self.dtype = None
+        self._flushed = False
+
+    # ------------------------------------------------------------------------------------------------ #
+    def push(self, chunk: torch.Tensor) -> torch.Tensor:
+        """Feed ``chunk`` (batch, n), any n >= 0; returns the frames completed by it."""
+        if self._flushed:
+            raise RuntimeError("push() after flush(): call reset() to start new streams")
+        if not isinstance(chunk, torch.Tensor):
+            raise TypeError("chunk must be a torch.Tensor")
+        if chunk.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+        if chunk.dim() != 2 or chunk.shape[0] != self.batch:
+            raise ValueError(f"chunk must be ({self.batch}, n), got {tuple(chunk.shape)}")
+        if chunk.dtype not in _C._WAVE_DTYPES:
+            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
+        if self.dtype is None:
+            self.dtype = chunk.dtype
+        elif chunk.dtype != self.dtype:
+            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within a stream")
+        n = chunk.shape[1]
+        T = _ready_frames(self.received + n, self.K, self.hop, self.pad, self._reflect) - self.frames
+        return self._advance(chunk, n, False, T)
+
+    def flush(self) -> torch.Tensor:
+        """End of stream: the remaining frames, with the module's right padding."""
+        if self._flushed:
+            raise RuntimeError("flush() after flush(): call reset() to start new streams")
+        self._check_length(self.received)  # the exception module(x) raises for a stream this short
+        if self.dtype is None:
+            self.dtype = torch.float32
+        T = (self.received + 2 * self.pad - self.K) // self.hop + 1 - self.frames
+        out = self._advance(None, 0, True, T)
+        self._flushed = True
+        return out
+
+    # ------------------------------------------------------------------------------------------------ #
+    def _advance(self, chunk, n, flush, T):
+        name, kw = self._args()
+        out = getattr(_C, name.replace("_forward", "_chunk_forward"))(self, chunk, flush, T, **kw)
+        if out is None:
+            if self._strict:
+                raise RuntimeError(f"{name}: no fused chunk route for this configuration (NNAB_EUNSUPPORTED)")
+            out = self._concat_route(chunk, n, flush, T, name, kw)
+        total = self.received + n
+        self.received, self.frames = total, self.frames + T
+        self.n_carry = total - _carry_start(total, self.frames, self.hop, self.pad)
+        return out
+
+    def _concat_route(self, chunk, n, flush, T, name, kw):
+        """The push on the module's offline call: the virtual clip (carried samples, chunk, the stream's
+        padding at its ends) built with torch, framed with center=False; then the carry ring update."""
+        R, K, dev = self.received, self.K, self.ring.device
+        total = R + n
+        x = chunk.float() if n > 0 else self.ring[:, :0]
+        out = None
+        if T > 0:
+            origin = self.frames * self.hop - self.pad
+            r = torch.arange(origin, origin + (T - 1) * self.hop + K, device=dev)
+            if self._reflect:
+                r = torch.where(r < 0, -r, r)
+                if flush:
+                    r = torch.where(r >= total, 2 * (total - 1) - r, r)
+            live = (r >= 0) & (r < total)
+            rc = r.clamp(0, max(total - 1, 0))
+            v = self.ring[:, rc % K]
+            if n > 0:
+                v = torch.where(rc < R, v, x[:, (rc - R).clamp(0, n - 1)])
+            v = torch.where(live, v, torch.zeros((), device=dev))
+            out = getattr(_C, name)(v, **dict(kw, center=False))
+        keep = max(_carry_start(total, self.frames + T, self.hop, self.pad), R)
+        if keep < total:
+            idx = torch.arange(keep, total, device=dev)
+            self.ring[:, idx % K] = x[:, idx - R]
+        return out if out is not None else self._empty(name, kw)
+
+    def _empty(self, name, kw):
+        """The offline call's output layout with no frame."""
+        dev = self.ring.device
+        if name == "stft_forward":
+            F = kw["wcos"].shape[0]
+            return torch.empty((self.batch, F, 0, 2) if kw["out_format"] == _C.FMT_COMPLEX else (self.batch, F, 0),
+                               device=dev)
+        if name == "stft_filterbank_forward":
+            return torch.empty((self.batch, kw["fb"].shape[0], 0), device=dev)
+        if name == "mfcc_forward":
+            return torch.empty((self.batch, kw["dct"].shape[0], 0), device=dev)
+        n_bins = kw["k_real"].shape[0]
+        return torch.empty((self.batch, n_bins, 0) if kw["out_format"] == _C.FMT_MAGNITUDE
+                           else (self.batch, n_bins, 0, 2), device=dev)
+
+
+class StreamingInverse:
+    """Stream ``batch`` complex spectrograms frame block by frame block through an inverse STFT.
+
+    ``module``: an ``iSTFT``, or an ``STFT`` built with ``iSTFT=True`` (its ``inverse``).  ``onesided``
+    defaults to the module's own default (``iSTFT``: False, ``STFT.inverse``: True).  ``push(X)`` takes
+    ``(batch, bins, t, 2)`` float32 frames, any t >= 0, and returns the output samples no later frame can change;
+    ``flush(length=None)`` returns the rest with the module's ``length`` / ``center`` rules.  The concatenation
+    equals ``module(X)`` / ``module.inverse(X)`` on all frames to fp32 rounding (both overlap-add with fp32
+    atomics, so neither is bit-repeatable).
+    """
+
+    def __init__(self, module, batch, onesided=None):
+        if isinstance(module, iSTFT):
+            bufs = (module.kernel_cos, module.kernel_sin, module.window_mask)
+            onesided = False if onesided is None else bool(onesided)
+        elif isinstance(module, STFT) and hasattr(module, "kernel_cos_inv"):
+            bufs = (module.kernel_cos_inv, module.kernel_sin_inv, module.window_mask)
+            onesided = True if onesided is None else bool(onesided)
+        else:
+            raise TypeError(f"StreamingInverse takes an iSTFT or an STFT built with iSTFT=True, not "
+                            f"{type(module).__name__}{'' if not isinstance(module, STFT) else ' without iSTFT=True'}")
+        batch = int(batch)
+        if batch < 1 or batch > _C.MAX_BATCH:
+            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        self.module, self.batch, self.onesided = module, batch, onesided
+        self.n_fft, self.hop, self.center = module.n_fft, module.stride, bool(module.center)
+        if self.hop > self.n_fft:
+            raise ValueError(f"hop_length {self.hop} > n_fft {self.n_fft}: the frames do not overlap")
+        self.f_in = self.n_fft // 2 + 1 if onesided else self.n_fft
+        self._args = lambda: _inverse_args(module, self.f_in, *bufs, onesided)
+        self.offset = self.n_fft // 2 if self.center else 0
+        device = next(iter(module.buffers())).device
+        self.state = torch.empty((batch, self.n_fft), dtype=torch.float32, device=device)  # open partial sums
+        self.reset()
+
+    def reset(self):
+        self.frames = self.emitted = 0
+        self._flushed = False
+
+    def _emit_end(self, n):
+        """End (overlap-add position) of the samples returned after n frames: below n * hop, and below the
+        earliest end the output can still have."""
+        if n <= 0:
+            return self.offset
+        end_min = self.n_fft + self.hop * (n - 1) - (self.offset if self.center else 0)
+        return max(self.offset, min(n * self.hop, end_min))
+
+    def push(self, X: torch.Tensor) -> torch.Tensor:
+        if self._flushed:
+            raise RuntimeError("push() after flush(): call reset() to start new streams")
+        if not isinstance(X, torch.Tensor):
+            raise TypeError("X must be a torch.Tensor")
+        if X.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the frames require grad")
+        if X.dim() != 4 or X.shape[0] != self.batch or X.shape[1] != self.f_in or X.shape[3] != 2:
+            raise ValueError(f"frames must be ({self.batch}, {self.f_in}, t, 2), got {tuple(X.shape)}")
+        T = X.shape[2]
+        n_out = self._emit_end(self.frames + T) - (self.offset + self.emitted)
+        return self._advance(X, False, None, n_out)
+
+    def flush(self, length=None) -> torch.Tensor:
+        if self._flushed:
+            raise RuntimeError("flush() after flush(): call reset() to start new streams")
+        if self.frames == 0:
+            raise RuntimeError("flush() of a stream without frames: the inverse STFT needs at least one")
+        ola_len = self.n_fft + self.hop * (self.frames - 1)
+        want = length if length is not None else (ola_len - 2 * self.offset if self.center else ola_len)
+        want = max(0, min(want, ola_len - self.offset))
+        if want < self.emitted:
+            raise ValueError(f"length {length} is shorter than the {self.emitted} samples already returned")
+        X = self.state.new_empty((self.batch, self.f_in, 0, 2))
+        out = self._advance(X, True, length, want - self.emitted)
+        self._flushed = True
+        return out
+
+    def _advance(self, X, flush, length, n_out):
+        _, _, packed, win = self._args()
+        out = _C.istft_chunk_forward(self, X, flush, length, n_out, packed, win, self.n_fft, self.hop, self.center)
+        self.frames += X.shape[2]
+        self.emitted += n_out
+        return out
