@@ -90,6 +90,37 @@ constexpr int FB_STEP_PAD = 160;  // entries past F (a tile's last chunk may ove
 // results differ run to run: 2 it is.)
 constexpr int FB_EPI_PARTS = 2;
 
+// The four-phase block kernel (tcb_kernels.cu) emits bin k of an n_fft = 4 M transform (F = 2 M + 1) from one
+// of four "families" of the M-point phase DFTs, each over k' = 0 .. M/2:
+//   f0 [0, M/2): k' = k    f1 [M/2, M): k' = M - k    f2 [M, 3M/2): k' = k - M    f3 [3M/2, 2M]: k' = 2M - k
+// Tile t of width nb holds k' in [t (nb - 2), (t + 1)(nb - 2)); f1 and f3 run reversed inside it, so that every
+// family emits ascending bins: output position o = k' - t (nb - 2) for f0 / f2, nb - 3 - that for f1 / f3.
+// The two warps of a family quarter (column parts) hand the sums of the filters open at their cut over inside
+// the CTA, so the range that adds one partial sum to each filter it meets (fused filterbank) is (family, tile).
+__host__ __device__ inline int poly4_family(int k, int M, int* kq) {
+  const int f = k < M / 2 ? 0 : (k < M ? 1 : (k < 3 * M / 2 ? 2 : 3));
+  *kq = (f == 0) ? k : (f == 1 ? M - k : (f == 2 ? k - M : 2 * M - k));
+  return f;
+}
+// Bins of family f in tile n: output o (0 <= o < nb - 2) is bin *k0 + o, and the family emits it iff it lies in
+// [*lo, *hi).  M = 0 is the one-phase kernel: one family, bins n (nb - 2) + o below F.
+__host__ __device__ inline void block_family_span(int n, int f, int nb, int M, int F, int* k0, int* lo, int* hi) {
+  const int kq0 = n * (nb - 2);
+  if (M == 0) {
+    *k0 = kq0; *lo = 0; *hi = F;
+    return;
+  }
+  *k0 = (f == 0) ? kq0 : (f == 1 ? M - kq0 - (nb - 3) : (f == 2 ? M + kq0 : 2 * M - kq0 - (nb - 3)));
+  *lo = f * (M / 2);
+  const int h = (f == 3) ? 2 * M + 1 : (f + 1) * (M / 2);
+  *hi = h < F ? h : F;
+}
+__host__ __device__ inline int poly4_range(int k, int M, int nb) {
+  int kq;
+  const int f = poly4_family(k, M, &kq);
+  return f * 4096 + kq / (nb - 2);
+}
+
 // The signal of one push of a chunked stream (DESIGN §3.10): the "virtual clip" of `length` samples whose
 // sample i is raw stream sample r = origin + i.  Raw samples [.., received) come from the fp32 carry ring
 // (raw r of stream b at ring[b * ring_pitch + r % ring_len]), [received, total) from the chunk (samples of
@@ -129,6 +160,7 @@ struct FramedProblem {
   const FbEntry* fb_table;   // FMT_FBANK: device table [F]; out is (B, n_fb, T), pre-zeroed
   const FbStep* fb_steps;    // FMT_FBANK, block-partial kernel: [F + FB_STEP_PAD] (nullptr: MelRun path)
   int fb_nb_mask;            // bit i: tile width nb = 32 + 8 i gives <= 2 partial sums per filter
+  int fb_poly_tile;          // four-phase block kernel: the cheapest nb giving <= 2 partial sums, or 0
   int n_fb;
   float* raw;                // tensor-core split-K scratch: 2 planes (re, im) of B*F*T floats, or nullptr
   const void* presplit;      // tensor-core path: already padded + split signal planes (skip pad_split)
@@ -166,8 +198,12 @@ int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pit
                  int pad_mode, void* planes, cudaStream_t stream);
 int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int pad, int pad_mode,
                     int64_t clip_pitch, int64_t plane_stride, void* planes, cudaStream_t stream);
-// tc_pad_split on the problem's own signal: the waveform x with its centre padding, or a push's virtual clip
-int tc_problem_split(const FramedProblem& q, void* planes, cudaStream_t stream);
+// tc_pad_split on the problem's own signal: the waveform x with its centre padding, or a push's virtual clip.
+// TC_SPLIT_POLY4 (hop % 128 == 0) stores every hop-sized block in polyphase order: position q * hop / 4 + m
+// holds sample 4 m + q (the four-phase block-partial kernel reads the four phases as four K ranges).
+constexpr int TC_SPLIT_PLAIN = 0;
+constexpr int TC_SPLIT_POLY4 = 1;
+int tc_problem_split(const FramedProblem& q, void* planes, cudaStream_t stream, int layout);
 // store raw samples [from, total) of the chunk into the carry ring (cs.received = raw index of chunk[0])
 int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
@@ -201,9 +237,10 @@ int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, cons
                             int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
                             int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream);
 size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K);
-// block-partial kernel (tcb_kernels.cu): default N-tile geometry for F bins (nb packed columns per tile,
-// nb - 2 new bins each) -- the column layout of the FMT_PLANES operand planes
-void tc_block_tile_geometry(int F, int* nb, int* n_tiles);
+// block-partial kernel (tcb_kernels.cu): default N-tile geometry of an (n_fft, hop) transform (nb packed
+// columns per tile, nb - 2 new bins each, `phases` families per tile: 1, or 4 when hop % 128 == 0) -- the column
+// layout of the FMT_PLANES operand planes: tile n, family f at columns nb (phases n + f) ..
+void tc_block_tile_geometry(int n_fft, int hop, int* nb, int* n_tiles, int* phases);
 bool tc_block_shape_ok(int n_fft, int hop);
 size_t tc_packed_fir_bytes(int taps, int dec);
 int tc_fir_k(int taps, int dec);
@@ -211,14 +248,15 @@ int tc_pack_fir(const float* fir, int taps, int dec, void* packed, cudaStream_t 
 int launch_fb_table(const float* fb, int n_fb, int F, FbEntry* table, int* d_max_nnz,
                     cudaStream_t stream);
 // FbEntry[F] -> FbStep[F + FB_STEP_PAD]; d_meta[0] = widest filter support (bins), d_meta[1] = bit mask
-// of the tile widths nb = 32 + 8 i under which every filter gets <= 2 partial sums
+// of the tile widths nb = 32 + 8 i under which every filter gets <= 2 partial sums in the one-phase block
+// kernel, d_meta[2] = the cheapest nb that does so in the four-phase kernel, or 0
 int launch_fb_steps(const FbEntry* table, int n_fb, int F, FbStep* steps, int* d_meta,
                     cudaStream_t stream);
 
 // filterbank / MFCC tail / FIR decimation (simt_kernels.cu)
 int launch_filterbank(const float* P, const float* fb, int64_t B, int F, int64_t T, int n_fb,
                       float* out, cudaStream_t stream);
-int launch_fb_tile_bank(const float* fb, int n_fb, int F, int nb, int n_tiles, int kp, int fh, float* w_re,
+int launch_fb_tile_bank(const float* fb, int n_fb, int F, int nb, int n_tiles, int phases, int kp, int fh, float* w_re,
                         float* w_im, cudaStream_t stream);
 int launch_mfcc_tail(const float* mel, int64_t B, int n_mels, int64_t T, float amin, float ref,
                      float top_db, const float* dct, int n_mfcc, float* out,

@@ -465,13 +465,15 @@ size_t nnab_filterbank_table_bytes(int F) {
   return fb_steps_offset(F) + (size_t)(F + FB_STEP_PAD) * sizeof(FbStep);
 }
 
-// deterministic-tile-width mask per table buffer (host copy of the device meta word; read at launch time)
+// deterministic tile widths per table buffer (host copy of the device meta words; read at launch time):
+// the one-phase kernel's nb mask and the four-phase kernel's (nb | split << 8)
+struct FbWidth { int nb_mask, poly_tile; };
 static std::mutex g_fbw_mu;
-static std::unordered_map<const void*, int> g_fb_width;
-static int fb_width_of(const void* table) {
+static std::unordered_map<const void*, FbWidth> g_fb_width;
+static FbWidth fb_width_of(const void* table) {
   std::lock_guard<std::mutex> lk(g_fbw_mu);
   auto it = g_fb_width.find(table);
-  return it == g_fb_width.end() ? 0 : it->second;
+  return it == g_fb_width.end() ? FbWidth{0, 0} : it->second;
 }
 
 int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table, int* h_max_nnz,
@@ -487,13 +489,13 @@ int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table, i
       (rc = launch_fb_steps(reinterpret_cast<const FbEntry*>(table), n_fb, F,
                             reinterpret_cast<FbStep*>(base + fb_steps_offset(F)), d_meta + 1, s)))
     return rc;
-  int h_meta[3] = {0, 0, 0};
+  int h_meta[4] = {0, 0, 0, 0};
   NNAB_CUDA_TRY(cudaMemcpyAsync(h_meta, d_meta, sizeof(h_meta), cudaMemcpyDeviceToHost, s));
   NNAB_CUDA_TRY(cudaStreamSynchronize(s));
   *h_max_nnz = h_meta[0];
   {
     std::lock_guard<std::mutex> lk(g_fbw_mu);
-    g_fb_width[table] = (n_fb < 32768) ? h_meta[2] : 0;
+    g_fb_width[table] = (n_fb < 32768) ? FbWidth{h_meta[2], h_meta[3]} : FbWidth{0, 0};
   }
   return NNAB_OK;
 }
@@ -511,7 +513,7 @@ static bool fb_planes_enabled() {
 }
 
 struct FbPlanes {
-  int nb, n_tiles, kp, fh;
+  int nb, n_tiles, phases, kp, fh;
   int64_t rows;  // B * T frame rows
   size_t off_planes, off_w, off_packed, total;
 };
@@ -519,8 +521,8 @@ struct FbPlanes {
 static bool fb_planes_layout(int64_t B, int64_t L, int n_fft, int F, int hop, int pad, int64_t T, int n_fb,
                              FbPlanes* o) {
   if (!tc_block_shape_ok(n_fft, hop) || F != n_fft / 2 + 1 || n_fb < 1 || T <= 0 || B <= 0) return false;
-  tc_block_tile_geometry(F, &o->nb, &o->n_tiles);
-  o->kp = (o->nb * o->n_tiles + 63) / 64 * 64;
+  tc_block_tile_geometry(n_fft, hop, &o->nb, &o->n_tiles, &o->phases);
+  o->kp = (o->nb * o->n_tiles * o->phases + 63) / 64 * 64;
   o->fh = (n_fb + 1) / 2;
   o->rows = B * T;
   if (o->rows >= (1ll << 31) || o->kp > 32768) return false;
@@ -601,7 +603,9 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     p.out_bins = n_fb; p.bin_offset = 0;
     p.fb_table = reinterpret_cast<const FbEntry*>(fb_table); p.n_fb = n_fb;
     p.fb_steps = reinterpret_cast<const FbStep*>(reinterpret_cast<const char*>(fb_table) + fb_steps_offset(F));
-    p.fb_nb_mask = fb_width_of(fb_table);
+    const FbWidth fw = fb_width_of(fb_table);
+    p.fb_nb_mask = fw.nb_mask;
+    p.fb_poly_tile = fw.poly_tile;
     if (tc_supported(p)) {
       const size_t need = tc_workspace_bytes(B, L, n_fft, hop, pad);
       if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
@@ -642,12 +646,14 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     // a shape either contraction rejects takes the fp32 path below, before anything is enqueued
     if (tc_supported(p) && tc_supported(g)) {
       // the re-indexed bank (tiny: fh x kp) and its bf16 hi/lo packing
-      if ((rc = launch_fb_tile_bank(fb, n_fb, F, fp.nb, fp.n_tiles, fp.kp, fp.fh, w_re, w_im, s))) return rc;
+      if ((rc = launch_fb_tile_bank(fb, n_fb, F, fp.nb, fp.n_tiles, fp.phases, fp.kp, fp.fh, w_re, w_im, s)))
+        return rc;
       if ((rc = tc_pack_basis(w_re, w_im, fp.fh, fp.kp, bank, s))) return rc;
-      // columns no tile writes (kp is the 64-multiple above n_tiles * nb): finite zeros in both planes
-      if (fp.kp > fp.nb * fp.n_tiles)
-        NNAB_CUDA_TRY(cudaMemset2DAsync(planes + fp.nb * fp.n_tiles, (size_t)fp.kp * 2, 0,
-                                        (size_t)(fp.kp - fp.nb * fp.n_tiles) * 2, (size_t)(2 * fp.rows), s));
+      // columns no tile writes (kp is the 64-multiple above n_tiles * phases * nb): finite zeros in both planes
+      const int written = fp.nb * fp.n_tiles * fp.phases;
+      if (fp.kp > written)
+        NNAB_CUDA_TRY(cudaMemset2DAsync(planes + written, (size_t)fp.kp * 2, 0, (size_t)(fp.kp - written) * 2,
+                                        (size_t)(2 * fp.rows), s));
       if ((rc = run_framed(p, packed, ws, fp.off_planes, NNAB_PATH_TCGEN05, s))) return rc;
       return run_framed(g, bank, nullptr, 0, NNAB_PATH_TCGEN05, s);
     }

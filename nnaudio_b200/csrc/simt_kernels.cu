@@ -282,52 +282,67 @@ int launch_fb_table(const float* fb, int n_fb, int F, FbEntry* table, int* d_max
 }
 
 // Sequential (one thread; F ~ 1e3, init time) replay of the two-slot running-sum logic over the bin
-// axis, recording the actions per bin (see FbStep).
-__global__ void fb_steps_kernel(const FbEntry* __restrict__ table, int n_fb, int F,
-                                FbStep* __restrict__ steps, int* __restrict__ meta) {
-  if (blockIdx.x != 0 || threadIdx.x != 0) return;
-  int cur_a = -1, cur_b = -1;
-  for (int k = 0; k < F + FB_STEP_PAD; ++k) {
-    FbStep st{0.f, 0.f, (short)-1, (short)-1, (short)cur_a, (short)cur_b};
-    if (k < F) {
-      const FbEntry e = table[k];
-      const int js[2] = {e.j0, e.j1};
-      const float ws[2] = {e.w0, e.w1};
-      bool used_a = false;
-      for (int i = 0; i < 2; ++i) {  // filters already held keep their slot
-        if (js[i] < 0) continue;
-        if (js[i] == cur_a) { st.wa = ws[i]; used_a = true; }
-        else if (js[i] == cur_b) { st.wb = ws[i]; }
-      }
-      for (int i = 0; i < 2; ++i) {  // new filters take a free slot (its old sum is flushed first)
-        if (js[i] < 0 || js[i] == cur_a || js[i] == cur_b) continue;
-        if (!used_a) {
-          if (cur_a >= 0) st.flush_a = (short)cur_a;
-          cur_a = js[i]; st.wa = ws[i]; used_a = true;
-        } else {
-          if (cur_b >= 0) st.flush_b = (short)cur_b;
-          cur_b = js[i]; st.wb = ws[i];
+// axis, recording the actions per bin (see FbStep).  Then, one filter per thread, the tile widths (and for
+// the four-phase kernel the warp split) under which the fused filterbank stays run-to-run identical.
+constexpr int FB_STEPS_THREADS = 256;
+__global__ void __launch_bounds__(FB_STEPS_THREADS) fb_steps_kernel(const FbEntry* __restrict__ table, int n_fb,
+                                                                    int F, FbStep* __restrict__ steps,
+                                                                    int* __restrict__ meta) {
+  __shared__ unsigned s_mask, s_poly;  // bit i: nb = 32 + 8 i qualifies (one phase / four phases)
+  __shared__ int s_widest;
+  if (threadIdx.x == 0) {
+    s_mask = 0x1FFFu;
+    s_poly = 0x1FFFu;
+    s_widest = 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int cur_a = -1, cur_b = -1;
+    for (int k = 0; k < F + FB_STEP_PAD; ++k) {
+      FbStep st{0.f, 0.f, (short)-1, (short)-1, (short)cur_a, (short)cur_b};
+      if (k < F) {
+        const FbEntry e = table[k];
+        const int js[2] = {e.j0, e.j1};
+        const float ws[2] = {e.w0, e.w1};
+        bool used_a = false;
+        for (int i = 0; i < 2; ++i) {  // filters already held keep their slot
+          if (js[i] < 0) continue;
+          if (js[i] == cur_a) { st.wa = ws[i]; used_a = true; }
+          else if (js[i] == cur_b) { st.wb = ws[i]; }
+        }
+        for (int i = 0; i < 2; ++i) {  // new filters take a free slot (its old sum is flushed first)
+          if (js[i] < 0 || js[i] == cur_a || js[i] == cur_b) continue;
+          if (!used_a) {
+            if (cur_a >= 0) st.flush_a = (short)cur_a;
+            cur_a = js[i]; st.wa = ws[i]; used_a = true;
+          } else {
+            if (cur_b >= 0) st.flush_b = (short)cur_b;
+            cur_b = js[i]; st.wb = ws[i];
+          }
         }
       }
+      st.cur_a = (short)cur_a;
+      st.cur_b = (short)cur_b;
+      steps[k] = st;
     }
-    st.cur_a = (short)cur_a;
-    st.cur_b = (short)cur_b;
-    steps[k] = st;
   }
   // For which tile widths nb = 32 + 8 i (i = 0..12) does every filter receive at most two partial
-  // sums?  A partial sum comes from each bin range (tile x warp part, cut exactly as
-  // framed_tcb_kernel cuts them) that intersects the filter's support; with <= 2 of them the
-  // atomic adds commute and the fused filterbank is run-to-run identical.
-  int widest = 0;
-  unsigned mask = 0x1FFFu;
-  for (int j = 0; j < n_fb; ++j) {
+  // sums?  A partial sum comes from each bin range (one phase: tile x warp part; four phases: family x
+  // tile, common.cuh poly4_range; cut exactly as framed_tcb_kernel cuts them) that intersects the
+  // filter's support; with <= 2 of them the atomic adds commute and the fused filterbank is run-to-run
+  // identical.  Every range is a run of consecutive bins, so the count is 1 + the number of range
+  // changes across the support.
+  const int M = (F - 1) / 2;
+  const bool poly = (F % 2 == 1) && M % 2 == 0 && M >= 64;  // F = n_fft / 2 + 1 of a four-phase shape
+  for (int j = threadIdx.x; j < n_fb; j += blockDim.x) {
     int lo = -1, hi = -1;
     for (int k = 0; k < F; ++k) {
       const FbEntry e = table[k];
       if (e.j0 == j || e.j1 == j) { if (lo < 0) lo = k; hi = k; }
     }
     if (lo < 0) continue;
-    if (hi - lo + 1 > widest) widest = hi - lo + 1;
+    atomicMax(&s_widest, hi - lo + 1);
+    unsigned mask = 0x1FFFu, pmask = poly ? 0x1FFFu : 0u;
     for (int i = 0; i < 13; ++i) {
       const int nb = 32 + 8 * i, outs = nb - 2, n_chunks = nb / 8;
       // range index of bin k: tile k / outs, then the warp part that owns chunk (o + 2) / 8 of output o
@@ -338,15 +353,36 @@ __global__ void fb_steps_kernel(const FbEntry* __restrict__ table, int n_fb, int
         return FB_EPI_PARTS * (k / outs) + part;
       };
       if (range_of(hi) - range_of(lo) + 1 > 2) mask &= ~(1u << i);
+      if (!poly) continue;
+      int n = 1, prev = poly4_range(lo, M, nb);
+      for (int k = lo + 1; k <= hi && n <= 2; ++k) {
+        const int r = poly4_range(k, M, nb);
+        n += (r != prev);
+        prev = r;
+      }
+      if (n > 2) pmask &= ~(1u << i);
     }
+    if (mask != 0x1FFFu) atomicAnd(&s_mask, mask);
+    if (pmask != 0x1FFFu) atomicAnd(&s_poly, pmask);
   }
-  meta[0] = widest;
-  meta[1] = (int)mask;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  // the four-phase tile width: fewest packed columns (block_choose_nb's cost)
+  int best = 0, best_cost = 1 << 30;
+  for (int i = 0; poly && i < 13; ++i) {
+    if (!((s_poly >> i) & 1u)) continue;
+    const int nb = 32 + 8 * i;
+    const int cost = (M / 2 + 1 + nb - 3) / (nb - 2) * (nb + 6);
+    if (cost < best_cost) { best_cost = cost; best = nb; }
+  }
+  meta[0] = s_widest;
+  meta[1] = (int)s_mask;
+  meta[2] = best;
 }
 
 int launch_fb_steps(const FbEntry* table, int n_fb, int F, FbStep* steps, int* d_meta,
                     cudaStream_t stream) {
-  fb_steps_kernel<<<1, 32, 0, stream>>>(table, n_fb, F, steps, d_meta);
+  fb_steps_kernel<<<1, FB_STEPS_THREADS, 0, stream>>>(table, n_fb, F, steps, d_meta);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -362,21 +398,24 @@ int launch_filterbank(const float* P, const float* fb, int64_t B, int F, int64_t
 }
 
 // Dense filterbank as the B operand of a real GEMM on the complex tensor-core kernel: the (n_fb, F) weights
-// re-indexed to the column layout of the block-partial kernel's FMT_PLANES output (tile n, packed column
-// i  <->  FFT bin n (nb - 2) + i - 2; columns 0, 1 of a tile and bins >= F carry zeros), filters
-// [0, fh) in the real bank and filters [fh, 2 fh) NEGATED in the imaginary bank (the contraction returns
-// -sum x w_im, FMT_REALPAIR then writes re -> row f, im -> row f + fh).
+// re-indexed to the column layout of the block-partial kernel's FMT_PLANES output (tile n, family f, packed
+// column i at nb (phases n + f) + i  <->  output i - 2 of that family, bin k0 + i - 2 of block_family_span;
+// columns 0, 1 of a tile, bins another family emits and bins >= F carry zeros), filters [0, fh) in the real
+// bank and filters [fh, 2 fh) NEGATED in the imaginary bank (the contraction returns -sum x w_im, FMT_REALPAIR
+// then writes re -> row f, im -> row f + fh).
 __global__ void __launch_bounds__(256) fb_tile_bank_kernel(const float* __restrict__ fb, int n_fb, int F,
-                                                           int nb, int n_tiles, int kp, int fh,
+                                                           int nb, int n_tiles, int phases, int kp, int fh,
                                                            float* __restrict__ w_re, float* __restrict__ w_im) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (int64_t)fh * kp) return;
   const int j = (int)(idx / kp), col = (int)(idx % kp);
-  const int n = col / nb, i = col - n * nb;
+  const int n = col / (phases * nb), f = (col / nb) % phases, i = col % nb;
   float a = 0.f, b = 0.f;
+  int k0 = 0, lo = 0, hi = 0;
+  block_family_span(n, f, nb, phases == 4 ? (F - 1) / 2 : 0, F, &k0, &lo, &hi);
   if (n < n_tiles && i >= 2) {
-    const int k = n * (nb - 2) + i - 2;
-    if (k < F) {
+    const int k = k0 + i - 2;
+    if (k >= lo && k < hi) {
       a = __ldg(fb + (int64_t)j * F + k);
       if (j + fh < n_fb) b = -__ldg(fb + (int64_t)(j + fh) * F + k);
     }
@@ -385,10 +424,10 @@ __global__ void __launch_bounds__(256) fb_tile_bank_kernel(const float* __restri
   w_im[idx] = b;
 }
 
-int launch_fb_tile_bank(const float* fb, int n_fb, int F, int nb, int n_tiles, int kp, int fh, float* w_re,
-                        float* w_im, cudaStream_t stream) {
+int launch_fb_tile_bank(const float* fb, int n_fb, int F, int nb, int n_tiles, int phases, int kp, int fh,
+                        float* w_re, float* w_im, cudaStream_t stream) {
   const int64_t n = (int64_t)fh * kp;
-  fb_tile_bank_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, stream>>>(fb, n_fb, F, nb, n_tiles, kp, fh,
+  fb_tile_bank_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, stream>>>(fb, n_fb, F, nb, n_tiles, phases, kp, fh,
                                                                         w_re, w_im);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;

@@ -140,16 +140,45 @@ __device__ __forceinline__ void padded_samples8(const Tx* __restrict__ xb, int64
   }
 }
 
-// One thread = 8 consecutive samples of one clip's slot region (16-byte stores).
+// Slot position -> sample of the clip slot.  poly_hop = 0: the identity.  poly_hop = hop (a multiple of 128):
+// every hop-sized block is stored in polyphase order, position q * hop / 4 + m holding sample 4 m + q
+// (TC_SPLIT_POLY4, the block-partial kernel's four-phase layout).  8 consecutive positions stay in one phase.
+__device__ __forceinline__ int64_t split_src(int64_t i, int poly_hop) {
+  if (poly_hop == 0) return i;
+  const int64_t g = i / poly_hop;
+  const int r = (int)(i - g * poly_hop), kq = poly_hop >> 2;
+  const int q = r / kq;
+  return g * poly_hop + 4 * (r - q * kq) + q;
+}
+
+// One thread = 8 consecutive positions of one clip's slot region (16-byte stores).
 template <typename Tx>
 __global__ void __launch_bounds__(256) pad_split_kernel(
     const Tx* __restrict__ x, int64_t L, int64_t x_pitch, int pad, int pad_mode, int shift,
-    int64_t clip_pitch, int64_t plane_stride, __nv_bfloat16* __restrict__ planes) {
+    int64_t clip_pitch, int64_t plane_stride, int poly_hop, __nv_bfloat16* __restrict__ planes) {
   const int64_t b = blockIdx.y;
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i0 >= clip_pitch) return;
   float v[8];
-  padded_samples8(x + b * x_pitch, L, pad, pad_mode, i0 + shift, v);  // i0 + shift: index into the padded clip
+  if (poly_hop == 0) {
+    padded_samples8(x + b * x_pitch, L, pad, pad_mode, i0 + shift, v);  // i0 + shift: index into the padded clip
+  } else {
+    // samples 4 m + q .. 4 (m + 7) + q of one block: a stride-4 gather (the warp's other phases hit in L1)
+    const Tx* __restrict__ xb = x + b * x_pitch;
+    const int64_t s0 = split_src(i0, poly_hop) + shift;
+    const int64_t padded_len = L + 2 * (int64_t)pad;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int64_t i = s0 + 4 * e;
+      v[e] = 0.f;
+      if (i < padded_len) {
+        int64_t j = i - pad;
+        if (j < 0) j = (pad_mode == NNAB_PAD_REFLECT) ? -j : -1;
+        else if (j >= L) j = (pad_mode == NNAB_PAD_REFLECT) ? 2 * (L - 1) - j : -1;
+        if (j >= 0 && j < L) v[e] = sample_f32(__ldg(xb + j));
+      }
+    }
+  }
   __align__(16) __nv_bfloat16 hi[8];
   __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
@@ -162,10 +191,10 @@ __global__ void __launch_bounds__(256) pad_split_kernel(
 // pad_split_kernel on the waveform's sample type (NNAB_DTYPE_*)
 static int launch_pad_split(dim3 grid, cudaStream_t stream, const void* x, int x_dtype, int64_t L,
                             int64_t x_pitch, int pad, int pad_mode, int shift, int64_t clip_pitch,
-                            int64_t plane_stride, __nv_bfloat16* planes) {
+                            int64_t plane_stride, __nv_bfloat16* planes, int poly_hop = 0) {
   auto launch = [&](auto* xs) {
     pad_split_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad, pad_mode, shift, clip_pitch, plane_stride,
-                                               planes);
+                                               poly_hop, planes);
   };
   if (x_dtype == NNAB_DTYPE_F32) launch(static_cast<const float*>(x));
   else if (x_dtype == NNAB_DTYPE_BF16) launch(static_cast<const __nv_bfloat16*>(x));
@@ -181,18 +210,20 @@ static int launch_pad_split(dim3 grid, cudaStream_t stream, const void* x, int x
 template <typename Tx>
 __global__ void __launch_bounds__(256) chunk_split_kernel(
     ChunkSource c, const Tx* __restrict__ chunk, int shift, int64_t clip_pitch, int64_t plane_stride,
-    __nv_bfloat16* __restrict__ planes) {
+    int poly_hop, __nv_bfloat16* __restrict__ planes) {
   const int64_t b = blockIdx.y;
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i0 >= clip_pitch) return;
   const float* __restrict__ ring = c.ring + b * c.ring_pitch;
   const Tx* __restrict__ xb = chunk + b * c.chunk_pitch;
   const bool reflect = c.pad_mode == NNAB_PAD_REFLECT;
+  const int64_t s0 = split_src(i0, poly_hop) + shift;
+  const int step = poly_hop ? 4 : 1;  // the 8 positions of a thread: consecutive samples, or one phase
   __align__(16) __nv_bfloat16 hi[8];
   __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    const int64_t i = i0 + shift + e;
+    const int64_t i = s0 + step * e;
     float v = 0.f;
     if (i < c.length) {
       int64_t r = c.origin + i;
@@ -235,12 +266,12 @@ static int with_sample_type(int x_dtype, const void* x, F&& f) {
 
 // The pre-pass of every tensor-core launcher: the planes of q's signal, shifted by `shift` samples.
 static int launch_problem_split(const FramedProblem& q, dim3 grid, int shift, int64_t clip_pitch,
-                                int64_t plane_stride, __nv_bfloat16* planes, cudaStream_t stream) {
+                                int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream) {
   if (q.chunk == nullptr)
     return launch_pad_split(grid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, shift, clip_pitch,
-                            plane_stride, planes);
+                            plane_stride, planes, poly_hop);
   const int rc = with_sample_type(q.x_dtype, q.chunk->chunk, [&](auto* xs) {
-    chunk_split_kernel<<<grid, 256, 0, stream>>>(*q.chunk, xs, shift, clip_pitch, plane_stride, planes);
+    chunk_split_kernel<<<grid, 256, 0, stream>>>(*q.chunk, xs, shift, clip_pitch, plane_stride, poly_hop, planes);
   });
   if (rc) return rc;
   NNAB_LAUNCH_CHECK();
@@ -395,9 +426,10 @@ static int zero_tail(__nv_bfloat16* planes, const SplitGeom& g, int hop_eff, cud
   return NNAB_OK;
 }
 
-// phase-0 pad + split of a batch into caller-managed planes
-int tc_problem_split(const FramedProblem& q, void* planes_v, cudaStream_t stream) {
+// phase-0 pad + split of a batch into caller-managed planes, in the given layout (TC_SPLIT_*)
+int tc_problem_split(const FramedProblem& q, void* planes_v, cudaStream_t stream, int layout) {
   if (q.B > 65535) return NNAB_EUNSUPPORTED;
+  if (layout != TC_SPLIT_PLAIN && (layout != TC_SPLIT_POLY4 || q.hop % 128 != 0)) return NNAB_EINVAL;
   const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
   const int hop_eff = q.hop * num_phases(q.hop);
   __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
@@ -405,7 +437,8 @@ int tc_problem_split(const FramedProblem& q, void* planes_v, cudaStream_t stream
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * hop_eff;
   dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-  return launch_problem_split(q, grid, 0, clip_pitch, g.plane_stride, planes, stream);
+  return launch_problem_split(q, grid, 0, clip_pitch, g.plane_stride, layout == TC_SPLIT_POLY4 ? q.hop : 0,
+                              planes, stream);
 }
 
 int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch, int K, int hop, int pad,
@@ -413,7 +446,7 @@ int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pit
   FramedProblem q{};
   q.x = x; q.x_dtype = x_dtype; q.B = B; q.L = L; q.x_pitch = x_pitch;
   q.K = K; q.hop = hop; q.pad = pad; q.pad_mode = pad_mode;
-  return tc_problem_split(q, planes_v, stream);
+  return tc_problem_split(q, planes_v, stream, TC_SPLIT_PLAIN);
 }
 
 __global__ void zero_margins_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride,
@@ -1612,7 +1645,7 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
   if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * q.hop;
   dim3 pgrid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-  if ((rc = launch_problem_split(q, pgrid, 0, clip_pitch, g.plane_stride, planes, stream))) return rc;
+  if ((rc = launch_problem_split(q, pgrid, 0, clip_pitch, g.plane_stride, 0, planes, stream))) return rc;
 
   // split-K only with the caller's raw scratch (long kernels): <= 64 K blocks per accumulator
   VarNPlan plan;
@@ -1859,7 +1892,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     prm.T = (q.T - ph + n_ph - 1) / n_ph;  // frames t = ph, ph + n_ph, ... < T
     if (q.presplit == nullptr) {
       dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-      if ((rc = launch_problem_split(q, grid, ph * q.hop, clip_pitch, g.plane_stride, planes, stream))) return rc;
+      if ((rc = launch_problem_split(q, grid, ph * q.hop, clip_pitch, g.plane_stride, 0, planes, stream))) return rc;
     }
     {
       double kcols = 0.0;  // sum over N tiles of (k-blocks executed) x bk x bn

@@ -211,6 +211,11 @@ __device__ __forceinline__ void acc_ld4(uint32_t taddr, uint32_t row, uint32_t* 
                : "r"(acc_chunk_smem(taddr, row))
                : "memory");
 }
+__device__ __forceinline__ void acc_st4(uint32_t taddr, uint32_t row, float a, float b, float c, float d) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(acc_chunk_smem(taddr, row)), "f"(a), "f"(b),
+               "f"(c), "f"(d)
+               : "memory");
+}
 __device__ __forceinline__ void acc_ld8(uint32_t taddr, uint32_t (&v)[8]) {
   const uint32_t row = ((taddr >> 16) & 0xFFu) + (threadIdx.x & 31u);
   acc_ld4(taddr, row, v);

@@ -28,6 +28,20 @@
 //     4 * (33 - R) frames per tile (116 of 128 rows for R = 4).
 //   * fp32 parity: x*w = xhi*whi + xlo*whi + xhi*wlo on bf16 tensor cores, fp32 accumulation.  A bf16
 //     waveform has xlo = 0: that kernel instance (PASSES = 2) skips the xlo*whi pass and the A lo plane.
+//
+// Four phases (PH = 4, whenever hop % 128 == 0): only hop of the N samples of Z_g are non-zero, so the N-point
+// block DFT is split by decimation in time.  With M = N / 4 and the polyphase rows x_q[m] = x[g hop + 4 m + q]
+// (m < hop / 4, stored in that order by the pre-pass, TC_SPLIT_POLY4):
+//
+//   Y_q(k') = sum_m x_q[m] e^{-2 pi i k' m / M},   k' = -1 .. M/2 + 1      K = hop / 4, ONE basis for all q
+//   T_q = e^{-2 pi i k' q / N} Y_q,   A0 = T0 + T2, A1 = T0 - T2, B0 = T1 + T3, B1 = T1 - T3
+//   Z[k'] = A0 + B0   Z[M + k'] = A1 - i B1   Z[M - k'] = conj(A1 + i B1)   Z[2M - k'] = conj(A0 - B0)
+//
+// (tools/block_poly_emulation.py is the executable spec.)  A quarter of the MMA work and of the operand bytes.
+// The 4 TMA boxes of an M tile are the 4 phases of the same 32 block rows (column origins q hop / 4); after
+// the MMAs a butterfly pass in the accumulator tile turns quarter q = phase q into quarter f = family f
+// (f1, f3 column-reversed so that every family runs over ascending bins, common.cuh block_family_span), and
+// the epilogue above runs on each quarter with its family's bin origin and bin range.  33 - R frames per tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <atomic>
@@ -46,11 +60,15 @@ constexpr int TCB_BK = 32;          // K block: one 64-byte swizzled row per ope
 constexpr int TCB_MAX_STAGES = 4;
 
 struct TcbParams {
-  int num_m_tiles;   // 128-row tiles along M (4 * (33 - R) frames each)
+  int num_m_tiles;   // 128-row tiles along M (4 * (33 - R) frames each; 33 - R with four phases)
   int num_n_tiles;
   int nb;            // packed bins per N tile (MMA N = 2 nb)
-  int kb_n;          // hop / TCB_BK
+  int kb_n;          // K / TCB_BK (K = hop, or hop / 4 with four phases)
   int stages;        // ring depth, TcbSmem::stages(nb)
+  int c_split;       // warp part 0 of a quarter owns the 8-column chunks [0, c_split), part 1 the rest
+  int fam_M;         // four phases: M = n_fft / 4 (family bins, block_family_span); 0 with one phase
+  const float2* twiddle;  // four phases: [q - 1][p] = e^{-2 pi i (p - 1) q / N}, q = 1 .. 3
+  int tw_rows;
   int64_t nv, t_slots, T;
   EpiParams epi;
 };
@@ -62,7 +80,8 @@ struct TcbParams {
 struct TcbSmem {
   static constexpr uint32_t A_BYTES = TC_BM * TCB_BK * 2;  // one plane, 128 rows
   static constexpr uint32_t LIMIT = 227 * 1024;            // opt-in dynamic shared memory per block
-  static constexpr uint32_t BAR_BYTES = 16 * TCB_MAX_STAGES;
+  // the ring's full / empty barriers, then the fused filterbank's hand-over sums (4 quarters x 32 rows x 2)
+  static constexpr uint32_t BAR_BYTES = 16 * TCB_MAX_STAGES + 4 * 32 * 8;
   // 128 fp32 rows of 2 nb columns, rounded up to 32 columns (acc_tile)
   __host__ __device__ static uint32_t acc_bytes(int nb) { return TC_BM * (uint32_t)((2 * nb + 31) / 32) * 128u; }
   // one (plane, part) box of the basis: nb rows; a multiple of 512 B, so every operand starts on an atom
@@ -92,17 +111,33 @@ static int block_choose_nb(int F) {
   return best;
 }
 static int block_n_tiles(int F, int nb) { return (F + nb - 3) / (nb - 2); }
-void tc_block_tile_geometry(int F, int* nb, int* n_tiles) {
-  *nb = block_choose_nb(F);
-  *n_tiles = block_n_tiles(F, *nb);
-}
 // rows of one (plane, part) slab: bins -1 .. F plus zero rows so that the last tile of ANY nb <= 128
 // stays inside the slab (the launch picks nb, e.g. wider tiles for the fused filterbank)
 static int block_p_rows(int F) { return round_up_i(F + 2 + 128, 8); }
 
+// The four-phase form: K = hop / 4 in K blocks of 32, and the packed "bins" are k' = 0 .. M/2 (F' = M/2 + 1).
+static bool block_poly4(int hop) { return hop % 128 == 0; }
+// packed bins of the basis (F of the one-phase form, F' with four phases) and its K
+static int block_basis_F(int n_fft, int hop) { return block_poly4(hop) ? n_fft / 8 + 1 : n_fft / 2 + 1; }
+static int block_basis_K(int hop) { return block_poly4(hop) ? hop / 4 : hop; }
+// byte offset of the four-phase twiddle table behind the basis slabs
+static size_t block_twiddle_offset(int n_fft, int hop) {
+  const size_t slabs = (size_t)4 * block_p_rows(block_basis_F(n_fft, hop)) * block_basis_K(hop) * sizeof(__nv_bfloat16);
+  return (slabs + 255) / 256 * 256;
+}
+
 size_t tc_packed_block_bytes(int n_fft, int hop) {
   if (!tc_block_shape_ok(n_fft, hop)) return 0;
-  return (size_t)4 * block_p_rows(n_fft / 2 + 1) * hop * sizeof(__nv_bfloat16) + 256;
+  size_t n = block_twiddle_offset(n_fft, hop);
+  if (block_poly4(hop)) n += (size_t)3 * block_p_rows(block_basis_F(n_fft, hop)) * sizeof(float2);
+  return n + 256;
+}
+
+void tc_block_tile_geometry(int n_fft, int hop, int* nb, int* n_tiles, int* phases) {
+  const int F = block_basis_F(n_fft, hop);
+  *nb = block_choose_nb(F);
+  *n_tiles = block_n_tiles(F, *nb);
+  *phases = block_poly4(hop) ? 4 : 1;
 }
 
 bool tc_block_shape_ok(int n_fft, int hop) {
@@ -113,6 +148,7 @@ bool tc_block_shape_ok(int n_fft, int hop) {
 
 // packed[plane hi|lo][part re|im][p][n]: bin k = p - 1, sample n < hop:
 //   re row:  cos(2 pi k n / N)      im row: -sin(2 pi k n / N)     (so re + i im = e^{-i theta k n})
+// Four phases: the same rows of the M-point DFT over hop / 4 samples (n_fft = M, hop = hop / 4, F = F').
 __global__ void __launch_bounds__(256) pack_block_basis_kernel(int n_fft, int hop, int F, int p_rows,
                                                                __nv_bfloat16* __restrict__ packed) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -147,18 +183,36 @@ __global__ void __launch_bounds__(256) pack_block_basis_kernel(int n_fft, int ho
   *reinterpret_cast<uint4*>(packed + 3 * slab + o) = *reinterpret_cast<const uint4*>(il);
 }
 
+// four phases: tw[q - 1][p] = e^{-2 pi i k q / N}, k = p - 1, q = 1 .. 3 (fp32, from float64)
+__global__ void __launch_bounds__(256) pack_block_twiddle_kernel(int n_fft, int p_rows, float2* __restrict__ tw) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= 3 * p_rows) return;
+  const int q = idx / p_rows + 1, p = idx - (q - 1) * p_rows;
+  long long m = ((long long)(p - 1) * q) % n_fft;
+  if (m < 0) m += n_fft;
+  double sd, cd;
+  sincospi(2.0 * (double)m / (double)n_fft, &sd, &cd);
+  tw[idx] = make_float2((float)cd, (float)(-sd));
+}
+
 struct BlockPack { int n_fft, hop; };
 static std::mutex g_blk_mu;
 static std::unordered_map<const void*, BlockPack> g_blk;
 
 int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
   if (!tc_block_shape_ok(n_fft, hop) || packed == nullptr) return NNAB_EINVAL;
-  const int F = n_fft / 2 + 1;
+  const bool poly = block_poly4(hop);
+  const int F = block_basis_F(n_fft, hop), K = block_basis_K(hop);
   const int p_rows = block_p_rows(F);
-  const int64_t threads = (int64_t)p_rows * (hop / 8);
+  const int64_t threads = (int64_t)p_rows * (K / 8);
   pack_block_basis_kernel<<<(unsigned)ceil_div64(threads, 256), 256, 0, stream>>>(
-      n_fft, hop, F, p_rows, (__nv_bfloat16*)packed);
+      poly ? n_fft / 4 : n_fft, K, F, p_rows, (__nv_bfloat16*)packed);
   NNAB_LAUNCH_CHECK();
+  if (poly) {
+    pack_block_twiddle_kernel<<<(unsigned)ceil_div64(3 * p_rows, 256), 256, 0, stream>>>(
+        n_fft, p_rows, reinterpret_cast<float2*>((char*)packed + block_twiddle_offset(n_fft, hop)));
+    NNAB_LAUNCH_CHECK();
+  }
   {
     std::lock_guard<std::mutex> lk(g_blk_mu);
     g_blk[packed] = BlockPack{n_fft, hop};
@@ -189,14 +243,22 @@ __device__ __forceinline__ void red_add_if(float* addr, float v, bool on) {
       : "memory");
 }
 
-template <int FMT, int R>
-__device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t trow, int64_t g,
-                                                    int lane, int n_tile, int c_begin, int c_end) {
+// One quarter of the tile holds a run of packed columns over ascending bins: output o (column o + 1) is bin
+// k_tile0 + o, and the outputs with bins in [klo, khi) are this quarter's to emit.  FMT_PLANES writes chunk c
+// at plane column col0 + 8 c.
+//
+// Four phases, fused filterbank: the two warps of a quarter (parts 0, 1, cut at chunk c_split) hand over the
+// sums of the filters open at the cut.  Part 1 keeps the first flush of each slot, which belongs to the filter
+// part 0 ends with, and passes it through shared memory (`handover`, named barrier 2 + quarter); part 0 adds it
+// to its own final sum before its one atomic add.  So a filter gets one partial sum per (family, tile).
+template <int FMT, int R, int PH>
+__device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t trow, int64_t g, int lane,
+                                                    int k_tile0, int klo, int khi, int64_t col0, int c_begin,
+                                                    int c_end, int part, int quarter, uint32_t handover) {
   const int nb = p.nb;
   const int64_t b = g / p.t_slots;
   const int64_t t = g - b * p.t_slots;  // frame index inside the clip = index of its first block
   const bool valid = (lane < 33 - R) && (g < p.nv) && (t < p.T);
-  const int k_tile0 = n_tile * (nb - 2);  // first output bin of this tile
   constexpr int CH = (FMT == NNAB_FMT_COMPLEX) ? 2 : 1;
   float* dst = nullptr;
   float* mel = nullptr;
@@ -208,6 +270,17 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
   const bool fast_fb = (FMT == 5) && p.epi.fb_steps != nullptr && p.epi.power == 2.0f && p.epi.eps == 0.f;
   float ma = 0.f, mb = 0.f;  // FMT 5, static action list: the two running filter sums
   int mca = -1, mcb = -1;    //   and the filters they currently belong to
+  constexpr bool HANDOVER = FMT == 5 && PH == 4;
+  bool first_a = false, first_b = false;  // part 1: the next flush of the slot is the filter open at the cut
+  float head_a = 0.f, head_b = 0.f;
+  if constexpr (HANDOVER) {
+    const int kq = k_tile0 + 8 * c_begin - 3;  // the bin before this part's first
+    if (fast_fb && part == 1 && kq >= 0) {
+      const int w = __ldg(reinterpret_cast<const int4*>(p.epi.fb_steps) + kq).w;
+      first_a = (short)(w & 0xffff) >= 0;
+      first_b = (short)((unsigned)w >> 16) >= 0;
+    }
+  }
 
   // twiddles c_k^j of the 4 residues the unrolled loop meets: output o = 8c - 2 + e is bin
   // k = k_tile0 + o, so k mod 4 = (k_tile0 + 2 + e) mod 4 (8c drops out).
@@ -283,12 +356,13 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
     }
     const int k0 = k_tile0 + 8 * c - 2;          // bin of e = 0 (outputs -2, -1 of chunk 0 do not exist)
     const int e_lo = (c == 0) ? 2 : 0;
+    auto own = [&](int e) { return e >= e_lo && k0 + e >= klo && k0 + e < khi; };
     if constexpr (FMT == NNAB_FMT_MAGNITUDE || FMT == NNAB_FMT_COMPLEX || FMT == 4) {
       float* q = dst + (int64_t)k0 * p.epi.T * CH;
       const int64_t step = p.epi.T * CH;
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        const bool ok = valid && e >= e_lo && (k0 + e) < p.epi.F;
+        const bool ok = valid && own(e);
         if constexpr (FMT == NNAB_FMT_COMPLEX) {
           if (ok) *reinterpret_cast<float2*>(q) = make_float2(xr[e], xi[e]);
         } else {
@@ -307,9 +381,10 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
       }
     } else if constexpr (FMT == 9) {
       // operand planes of the dense-filterbank GEMM (FMT_PLANES): frame (b, t) is row b * T + t, the 8
-      // packed columns of chunk c of tile n sit at nb * n + 8 c (16-byte aligned: nb is a multiple of 8),
-      // |X| ** power as bf16 hi / lo.  The two columns a tile repeats from its left neighbour and the bins
-      // past F are written as zeros (the re-indexed bank has zero rows there).
+      // packed columns of chunk c of tile n (family f) sit at nb * (PH n + f) + 8 c (16-byte aligned: nb is a
+      // multiple of 8), |X| ** power as bf16 hi / lo.  The two columns a tile repeats from its left neighbour,
+      // the bins another family emits and the bins past F are written as zeros (the re-indexed bank has zero
+      // rows there).
       __align__(16) __nv_bfloat16 hi[8];
       __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
@@ -318,32 +393,40 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
         if (p.epi.eps != 0.f) pw = __fadd_rn(pw, p.epi.eps);
         float v = (p.epi.power == 2.0f) ? pw
                   : ((p.epi.power == 1.0f) ? sqrt_approx(pw) : powf(sqrt_approx(pw), p.epi.power));
-        if (e < e_lo || (k0 + e) >= p.epi.F) v = 0.f;
+        if (!own(e)) v = 0.f;
         split_bf16(v, hi[e], lo[e]);
       }
       if (valid) {
         __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(p.epi.out) +
-                           (b * p.epi.T + t) * (int64_t)p.epi.planes_pitch + (int64_t)nb * n_tile + 8 * c;
+                           (b * p.epi.T + t) * (int64_t)p.epi.planes_pitch + col0 + 8 * c;
         *reinterpret_cast<uint4*>(q) = *reinterpret_cast<const uint4*>(hi);
         *reinterpret_cast<uint4*>(q + p.epi.planes_stride) = *reinterpret_cast<const uint4*>(lo);
       }
     } else if constexpr (FMT == 5) {
       if (fast_fb) {
         // banded filterbank, static action list: branch-free, two running sums per row.
-        // Bins past F have neutral table entries (and zero basis rows); the two columns of chunk 0
-        // that belong to the previous tile contribute with power 0.
-        if (c == 0) { xr[0] = xi[0] = xr[1] = xi[1] = 0.f; }
+        // Bins this quarter does not own (the two columns of chunk 0 that belong to the previous tile,
+        // another family's bins, bins past F) contribute with power 0.
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           const int4 raw = st[e];
           // power == 2 (the default, mel.py:186: |X| ** 2): the power spectrum itself, to 1 ulp
-          const float pw = __fadd_rn(__fmul_rn(xr[e], xr[e]), __fmul_rn(xi[e], xi[e]));
+          const float pw = own(e) ? __fadd_rn(__fmul_rn(xr[e], xr[e]), __fmul_rn(xi[e], xi[e])) : 0.f;
           // a filter ends at ~1 bin in 6 (and at the same bins for every row): one warp-uniform test
           // on the packed flush word keeps the address / predicate / RED code off the common path
           if (__any_sync(0xffffffffu, raw.z != -1)) {
             const int fa = (int)(short)(raw.z & 0xffff), fb = (int)(short)((unsigned)raw.z >> 16);
-            red_add_if(mel + (int64_t)fa * p.epi.T, ma, fa >= 0 && valid);
-            red_add_if(mel + (int64_t)fb * p.epi.T, mb, fb >= 0 && valid);
+            bool keep_a = false, keep_b = false;
+            if constexpr (HANDOVER) {
+              keep_a = first_a && fa >= 0;
+              keep_b = first_b && fb >= 0;
+              head_a = keep_a ? ma : head_a;
+              head_b = keep_b ? mb : head_b;
+              first_a = first_a && !keep_a;
+              first_b = first_b && !keep_b;
+            }
+            red_add_if(mel + (int64_t)fa * p.epi.T, ma, fa >= 0 && valid && !keep_a);
+            red_add_if(mel + (int64_t)fb * p.epi.T, mb, fb >= 0 && valid && !keep_b);
             ma = fa >= 0 ? 0.f : ma;
             mb = fb >= 0 ? 0.f : mb;
           }
@@ -356,7 +439,8 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
 #pragma unroll 1
         for (int e = e_lo; e < 8; ++e) {
           const int k = k0 + e;
-          if (k >= p.epi.F) break;  // warp-uniform
+          if (k >= khi) break;  // warp-uniform
+          if (k < klo) continue;
           float re = xr[0], im = xi[0];
 #pragma unroll
           for (int j = 1; j < 8; ++j) { re = (e == j) ? xr[j] : re; im = (e == j) ? xi[j] : im; }
@@ -368,12 +452,30 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
 #pragma unroll 1
       for (int e = e_lo; e < 8; ++e) {
         const int k = k0 + e;
-        if (k >= p.epi.F) break;  // warp-uniform
+        if (k >= khi) break;  // warp-uniform
+        if (k < klo) continue;
         // dynamic index into xr/xi would spill: select with a short unrolled scan
         float re = xr[0], im = xi[0];
 #pragma unroll
         for (int j = 1; j < 8; ++j) { re = (e == j) ? xr[j] : re; im = (e == j) ? xi[j] : im; }
         if (valid) epi_store_fmt<FMT>(p.epi, dst, k, re, im);
+      }
+    }
+  }
+  if constexpr (HANDOVER) {
+    if (fast_fb) {
+      const uint32_t slot = handover + (uint32_t)(quarter * 32 + lane) * 8u;
+      if (part == 1) {
+        if (first_a) { head_a = ma; mca = -1; }  // no flush in this part: its whole sum is the open filter's
+        if (first_b) { head_b = mb; mcb = -1; }
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(slot), "f"(head_a), "f"(head_b) : "memory");
+        asm volatile("bar.arrive %0, 64;" ::"r"(2 + quarter) : "memory");
+      } else {
+        asm volatile("bar.sync %0, 64;" ::"r"(2 + quarter) : "memory");
+        float ha, hb;
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ha), "=f"(hb) : "r"(slot) : "memory");
+        ma += ha;
+        mb += hb;
       }
     }
   }
@@ -430,12 +532,76 @@ __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, in
   if (lane == 0) mbar_arrive(ring.empty(prev));
 }
 
-template <int FMT, int R, int PASSES>
+// Four phases: the radix-4 butterfly, in place in the accumulator tile.  Quarter q holds Y_q of the tile's
+// packed columns (column i <-> k' = n_tile (nb - 2) + i - 1) for 32 block rows; afterwards quarter f holds
+// family f, f1 and f3 at the mirrored column nb - 1 - i.  A thread owns row `lane` of all four quarters and a
+// 4-column group together with its mirror group, so every location it writes is one it alone reads.
+__device__ __forceinline__ void tcb_butterfly(const TcbParams& p, uint32_t tile, int n_tile, int warp, int lane) {
+  const int nb = p.nb;
+  const float2* __restrict__ tw = p.twiddle + n_tile * (nb - 2);
+#pragma unroll 1
+  for (int gi = warp; gi < nb / 8; gi += 8) {
+    int col[2];
+    col[0] = 4 * gi;
+    col[1] = nb - 4 - 4 * gi;  // the mirror group (never the same: nb is a multiple of 8)
+    float yr[4][8], yi[4][8];   // [phase][column: group 0, then group 1]
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t re[4], im[4];
+        acc_ld4(tile + (uint32_t)col[h], (uint32_t)(32 * q + lane), re);
+        acc_ld4(tile + (uint32_t)(nb + col[h]), (uint32_t)(32 * q + lane), im);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) { yr[q][4 * h + e] = __uint_as_float(re[e]); yi[q][4 * h + e] = __uint_as_float(im[e]); }
+      }
+    }
+    float fr[4][8], fi[4][8];  // [family][column]
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = col[j >> 2] + (j & 3);
+      float tr[4], ti[4];
+      tr[0] = yr[0][j]; ti[0] = yi[0][j];
+#pragma unroll
+      for (int q = 1; q < 4; ++q) {
+        const float2 w = __ldg(tw + (q - 1) * p.tw_rows + c);
+        tr[q] = w.x * yr[q][j] - w.y * yi[q][j];
+        ti[q] = w.x * yi[q][j] + w.y * yr[q][j];
+      }
+      const float a0r = tr[0] + tr[2], a0i = ti[0] + ti[2], a1r = tr[0] - tr[2], a1i = ti[0] - ti[2];
+      const float b0r = tr[1] + tr[3], b0i = ti[1] + ti[3], b1r = tr[1] - tr[3], b1i = ti[1] - ti[3];
+      fr[0][j] = a0r + b0r;  fi[0][j] = a0i + b0i;     // Z[k']
+      fr[1][j] = a1r - b1i;  fi[1][j] = -(a1i + b1r);  // Z[M - k'] = conj(A1 + i B1)
+      fr[2][j] = a1r + b1i;  fi[2][j] = a1i - b1r;     // Z[M + k'] = A1 - i B1
+      fr[3][j] = a0r - b0r;  fi[3][j] = b0i - a0i;     // Z[2M - k'] = conj(A0 - B0)
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int j = 4 * h, m = 4 * (1 - h) + 3;  // group h in place; the other group's columns reversed
+#pragma unroll
+      for (int f = 0; f < 4; f += 2) {
+        const uint32_t r = (uint32_t)(32 * f + lane);
+        acc_st4(tile + (uint32_t)col[h], r, fr[f][j], fr[f][j + 1], fr[f][j + 2], fr[f][j + 3]);
+        acc_st4(tile + (uint32_t)(nb + col[h]), r, fi[f][j], fi[f][j + 1], fi[f][j + 2], fi[f][j + 3]);
+      }
+#pragma unroll
+      for (int f = 1; f < 4; f += 2) {
+        const uint32_t r = (uint32_t)(32 * f + lane);
+        acc_st4(tile + (uint32_t)col[h], r, fr[f][m], fr[f][m - 1], fr[f][m - 2], fr[f][m - 3]);
+        acc_st4(tile + (uint32_t)(nb + col[h]), r, fi[f][m], fi[f][m - 1], fi[f][m - 2], fi[f][m - 3]);
+      }
+    }
+  }
+}
+
+template <int FMT, int R, int PASSES, int PH>
 __global__ void __launch_bounds__(TC_KERNEL_THREADS, 1)
 framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                   const TcbParams p) {
   constexpr int BK = TCB_BK;
   constexpr int FW = 33 - R;  // frames per warp quarter
+  constexpr int TILE_ROWS = PH == 4 ? FW : 4 * FW;  // block rows an M tile advances
+  static_assert(PH == 1 || PH == 4, "one or four phases");
   using S = TcbSmem;
   const int nb = p.nb;
   TcbRing ring;
@@ -468,7 +634,7 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_tile = tile / p.num_n_tiles;
         const int n_tile = tile - m_tile * p.num_n_tiles;
-        const int m0 = m_tile * (4 * FW);
+        const int m0 = m_tile * TILE_ROWS;
         const int n0 = n_tile * (nb - 2);
         for (int kb = 0; kb < p.kb_n; ++kb) {
           mbar_wait(ring.empty(stage), phase ^ 1u);
@@ -477,10 +643,13 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
           mbar_expect_tx(full, ring.stage_bytes);
           const int k0 = kb * BK;
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {  // 32-row boxes, row origins FW apart
-            tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 0);
+          for (int q = 0; q < 4; ++q) {
+            // one phase: 32-row boxes, row origins FW apart; four phases: phase q of the same 32 block rows
+            const int kc = PH == 4 ? q * p.kb_n * BK + k0 : k0;
+            const int row = PH == 4 ? m0 : m0 + q * FW;
+            tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, &tm_a, full, kc, row, 0);
             if constexpr (PASSES == 3)
-              tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full, k0, m0 + q * FW, 1);
+              tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, &tm_a, full, kc, row, 1);
           }
           // B rows [0, nb) = re part, [nb, 2 nb) = im part of each plane: accumulator columns of the
           // N = 2 nb MMA
@@ -498,10 +667,9 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
   const int wg = warp >> 2;
   const uint32_t a_off = (uint32_t)wg * 64u * (BK * 2);
   const uint32_t tile_addr = acc_tile(2 * nb);
-  const int quarter = warp & 3;  // tile rows 32 quarter .. + 31
-  const int part = warp >> 2;    // column half of the tile
-  const int n_chunks = nb / 8;
-  const int c_begin = (n_chunks * part) / TCB_PARTS, c_end = (n_chunks * (part + 1)) / TCB_PARTS;
+  const int quarter = warp & 3;  // tile rows 32 quarter .. + 31 (four phases: family `quarter`)
+  const int part = warp >> 2;    // column part of the tile
+  const int c_begin = part == 0 ? 0 : p.c_split, c_end = part == 0 ? p.c_split : nb / 8;
   float acc[128];
   int stage = 0;
   uint32_t phase = 0;
@@ -522,16 +690,24 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     consumer_sync();  // every warp is done reading the previous tile
     acc_store<256>(tile_addr, acc, 2 * nb, wg * 64);
     consumer_sync();
-    const int64_t g = (int64_t)m_tile * (4 * FW) + quarter * FW + lane;
-    epilogue_tile_block<FMT, R>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, n_tile, c_begin,
-                                c_end);
+    if constexpr (PH == 4) {
+      tcb_butterfly(p, tile_addr, n_tile, warp, lane);
+      consumer_sync();
+    }
+    const int64_t g = (int64_t)m_tile * TILE_ROWS + (PH == 4 ? 0 : quarter * FW) + lane;
+    int k_tile0, klo, khi;
+    block_family_span(n_tile, PH == 4 ? quarter : 0, nb, PH == 4 ? p.fam_M : 0, p.epi.F, &k_tile0, &klo, &khi);
+    if (klo < k_tile0) klo = k_tile0;
+    const int64_t col0 = (int64_t)nb * (PH * n_tile + (PH == 4 ? quarter : 0));
+    epilogue_tile_block<FMT, R, PH>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, k_tile0, klo, khi,
+                                    col0, c_begin, c_end, part, quarter, ring.bars + 16u * TCB_MAX_STAGES);
   }
 }
 
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-template <int FMT, int R, int PASSES>
+template <int FMT, int R, int PASSES, int PH>
 static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
                           cudaStream_t stream) {
   using S = TcbSmem;
@@ -539,27 +715,37 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   int cfg_dev = 0;
   NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
   if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R, PASSES>,
+    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R, PASSES, PH>,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::LIMIT));
     configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
   }
-  framed_tcb_kernel<FMT, R, PASSES><<<grid, TC_KERNEL_THREADS, S::total(prm.nb, PASSES), stream>>>(ma, mb, prm);
+  framed_tcb_kernel<FMT, R, PASSES, PH><<<grid, TC_KERNEL_THREADS, S::total(prm.nb, PASSES), stream>>>(ma, mb, prm);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
-template <int R, int PASSES>
+template <int R, int PASSES, int PH>
 static int launch_tcb(int fmt, const CUtensorMap& ma, const CUtensorMap& mb, const TcbParams& prm, int grid,
                       cudaStream_t stream) {
   switch (fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R, PASSES>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R, PASSES>(ma, mb, prm, grid, stream);
-    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R, PASSES>(ma, mb, prm, grid, stream);
-    case FMT_POWER: return launch_tcb_fmt<4, R, PASSES>(ma, mb, prm, grid, stream);
-    case FMT_FBANK: return launch_tcb_fmt<5, R, PASSES>(ma, mb, prm, grid, stream);
-    case FMT_PLANES: return launch_tcb_fmt<9, R, PASSES>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_MAGNITUDE: return launch_tcb_fmt<0, R, PASSES, PH>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_COMPLEX: return launch_tcb_fmt<1, R, PASSES, PH>(ma, mb, prm, grid, stream);
+    case NNAB_FMT_PHASE_ANGLE: return launch_tcb_fmt<2, R, PASSES, PH>(ma, mb, prm, grid, stream);
+    case FMT_POWER: return launch_tcb_fmt<4, R, PASSES, PH>(ma, mb, prm, grid, stream);
+    case FMT_FBANK: return launch_tcb_fmt<5, R, PASSES, PH>(ma, mb, prm, grid, stream);
+    case FMT_PLANES: return launch_tcb_fmt<9, R, PASSES, PH>(ma, mb, prm, grid, stream);
     default: return NNAB_EINVAL;
   }
+}
+
+template <int PH>
+static int launch_tcb_ph(int R, int passes, int fmt, const CUtensorMap& ma, const CUtensorMap& mb,
+                         const TcbParams& prm, int grid, cudaStream_t stream) {
+  if (passes == 2)
+    return R == 4 ? launch_tcb<4, 2, PH>(fmt, ma, mb, prm, grid, stream)
+                  : launch_tcb<2, 2, PH>(fmt, ma, mb, prm, grid, stream);
+  return R == 4 ? launch_tcb<4, 3, PH>(fmt, ma, mb, prm, grid, stream)
+                : launch_tcb<2, 3, PH>(fmt, ma, mb, prm, grid, stream);
 }
 
 int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* workspace,
@@ -594,10 +780,13 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   if (q.B > 65535) return NNAB_EUNSUPPORTED;
 
   const int R = q.K / q.hop;
+  const bool poly = block_poly4(q.hop);
+  const int PH = poly ? 4 : 1;
+  const int Fb = block_basis_F(q.K, q.hop), Kb = block_basis_K(q.hop);  // the GEMM's packed bins and K
   const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
   __nv_bfloat16* planes =
       reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  int rc = tc_problem_split(q, planes, stream);
+  int rc = tc_problem_split(q, planes, stream, poly ? TC_SPLIT_POLY4 : TC_SPLIT_PLAIN);
   if (rc) return rc;
   // a bf16 waveform has an all-zero lo plane: the xlo * whi pass would add exact zeros
   const int passes = (q.x_dtype == NNAB_DTYPE_BF16) ? 2 : 3;
@@ -608,8 +797,13 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   sms -= sm_reserve();
   if (sms < 1) sms = 1;
 
-  int nb = block_choose_nb(q.F);
-  if (q.fmt == FMT_FBANK && q.fb_steps != nullptr && q.fb_nb_mask != 0) {
+  int nb = block_choose_nb(Fb);
+  if (q.fmt == FMT_FBANK && q.fb_steps != nullptr && poly && q.fb_poly_tile != 0) {
+    // run-to-run identical filterbank sums: the table builder replayed the four-phase range cuts (family
+    // seams and tiles; the warp parts hand over inside the CTA) and chose the cheapest width that gives
+    // every filter <= 2 partial sums
+    nb = q.fb_poly_tile;
+  } else if (q.fmt == FMT_FBANK && q.fb_steps != nullptr && !poly && q.fb_nb_mask != 0) {
     // run-to-run identical filterbank sums: with at most two partial sums per filter the atomic
     // adds commute.  The table builder replayed the range cuts for every tile width; take the
     // cheapest width that qualifies (fewest padded columns), else keep the default.
@@ -622,23 +816,30 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
     }
     if (best > 0) nb = best;
   }
-  const int n_tiles = block_n_tiles(q.F, nb);
-  const int p_rows = block_p_rows(q.F);
+  if (nb < 32 || nb > 128 || nb % 8 != 0) return NNAB_EINVAL;
+  const int c_split = (nb / 8) / TCB_PARTS;  // the two warp parts split the chunks evenly (>= 2: both own some)
+  const int n_tiles = block_n_tiles(Fb, nb);
+  const int p_rows = block_p_rows(Fb);
   CUtensorMap ma, mb;
   rc = encode_3d(&ma, planes, (uint64_t)q.hop, (uint64_t)g.rows, 2, (uint64_t)q.hop * 2,
                  (uint64_t)g.plane_stride * 2, TCB_BK, 32, TCB_BK);
   if (rc) return rc;
-  rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)q.hop, (uint64_t)p_rows, 4,
-                 (uint64_t)q.hop * 2, (uint64_t)p_rows * q.hop * 2, TCB_BK, (uint32_t)nb, TCB_BK);
+  rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)Kb, (uint64_t)p_rows, 4,
+                 (uint64_t)Kb * 2, (uint64_t)p_rows * Kb * 2, TCB_BK, (uint32_t)nb, TCB_BK);
   if (rc) return rc;
 
   TcbParams prm{};
-  const int frames_per_tile = 4 * (33 - R);
-  prm.num_m_tiles = (int)ceil_div64(g.nv, frames_per_tile);
+  const int rows_per_tile = poly ? 33 - R : 4 * (33 - R);  // block rows (= frames) an M tile advances
+  prm.num_m_tiles = (int)ceil_div64(g.nv, rows_per_tile);
   prm.num_n_tiles = n_tiles;
   prm.nb = nb;
-  prm.kb_n = q.hop / TCB_BK;
+  prm.kb_n = Kb / TCB_BK;
   prm.stages = TcbSmem::stages(nb, passes);
+  prm.c_split = c_split;
+  prm.fam_M = poly ? q.K / 4 : 0;
+  prm.twiddle = poly ? reinterpret_cast<const float2*>((const char*)packed + block_twiddle_offset(q.K, q.hop))
+                     : nullptr;
+  prm.tw_rows = p_rows;
   prm.nv = g.nv;
   prm.t_slots = g.t_slots;
   prm.T = q.T;
@@ -649,15 +850,12 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.epi.raw = nullptr; prm.epi.raw_plane = 0;
   prm.epi.ola_pitch = 0; prm.epi.ola_hop = 0;
   prm.epi.planes_stride = q.planes_stride; prm.epi.planes_pitch = q.planes_pitch;
-  if (q.fmt == FMT_PLANES && (int64_t)n_tiles * nb > q.planes_pitch) return NNAB_EINVAL;
+  if (q.fmt == FMT_PLANES && (int64_t)n_tiles * PH * nb > q.planes_pitch) return NNAB_EINVAL;
   const int64_t tiles = (int64_t)prm.num_m_tiles * n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);
-  add_exec_flops(passes * 2.0 * (double)tiles * TC_BM * (2 * nb) * q.hop);
-  if (passes == 2)
-    return R == 4 ? launch_tcb<4, 2>(q.fmt, ma, mb, prm, grid, stream)
-                  : launch_tcb<2, 2>(q.fmt, ma, mb, prm, grid, stream);
-  return R == 4 ? launch_tcb<4, 3>(q.fmt, ma, mb, prm, grid, stream)
-                : launch_tcb<2, 3>(q.fmt, ma, mb, prm, grid, stream);
+  add_exec_flops(passes * 2.0 * (double)tiles * TC_BM * (2 * nb) * Kb);
+  return poly ? launch_tcb_ph<4>(R, passes, q.fmt, ma, mb, prm, grid, stream)
+              : launch_tcb_ph<1>(R, passes, q.fmt, ma, mb, prm, grid, stream);
 }
 
 }  // namespace nnab

@@ -474,7 +474,7 @@ int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* work
     if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
     const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
     planes = reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-    rc = tc_problem_split(q, planes, stream);
+    rc = tc_problem_split(q, planes, stream, TC_SPLIT_PLAIN);
     if (rc) return rc;
     t_slots = g.t_slots;
     plane_stride = g.plane_stride;
