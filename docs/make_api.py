@@ -41,6 +41,8 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   `flush()`, `reset()`).  The concatenated outputs equal `module(x)` on the whole stream, bit for bit on the
   tensor-core routes except across the CQT1992v2 kernel's two tile schedules (2e-6; DESIGN.md §3.10).
   `StreamingInverse(istft_module, batch)` does the same for the inverse STFT, to fp32 rounding.
+  `StreamingPyramid(module, batch)` streams the CQT pyramid of `CQT2010v2` / `VQT` / `CQT2010` bit for bit on the
+  whole-clip call's tensor-core plan (DESIGN.md §3.10).
 
 Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
 schedule of the CQT1992v2 kernel).

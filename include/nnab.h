@@ -411,6 +411,43 @@ int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry,
                                  int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
                                  size_t ws_bytes, int path, void* stream);
 
+/* Streamed CQT pyramid: nnab_cqt_pyramid_forward_ex's arguments with (x, L, x_pitch) replaced by state, the
+ * three host counters, the chunk and flush as above.
+ *   state     DEVICE fp32, nnab_cqt_pyramid_chunk_state_bytes(B, n_octaves, widths, hop, early_factor) bytes:
+ *             one ring per signal (the raw samples, then every decimated level); no initialisation needed
+ *   n_carry   raw samples the raw ring carries: received - max(0, min(frames*hop - pad_0 [no early stage],
+ *             received - pad_0 - 1 [no early stage], 128 d floor(R_1 / 128) - 128)), R_1 the final samples of
+ *             the next signal and d its factor (DESIGN.md §3.10)
+ * Before the end, sample n of a decimated signal is final once d n + c samples of its source have arrived
+ * (d = 2, or early_factor for the early stage; c = 130 on the plan without early downsampling whose FIR-source
+ * banks are 256 wide ("generation 2"), else 129), and T counts the frames final in every octave; on flush
+ * every level gets its full length and T is the rest (octave frame counts that differ: NNAB_EINVAL).  The
+ * pushes run the whole-clip call's tensor-core plan and kernels, so their frames equal it bit for bit.  hop
+ * must be a multiple of 2^(n_octaves - 1).  The SIMT path, a missing packed operand, or a launch outside the
+ * kernels' limits returns NNAB_EUNSUPPORTED before anything is enqueued.  Both size queries are host-only. */
+size_t nnab_cqt_pyramid_chunk_state_bytes(int64_t B, int n_octaves, const int32_t* widths, int hop,
+                                          int early_factor);
+size_t nnab_cqt_pyramid_chunk_workspace_bytes(int64_t B, int64_t received, int64_t n_carry, int64_t frames,
+                                              int64_t n, int flush, int n_octaves, const int32_t* widths,
+                                              int hop, int early_factor, int pad_mode);
+int nnab_cqt_pyramid_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                   const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
+                                   int flush, int n_octaves, const float* const* h_k_real,
+                                   const float* const* h_k_imag, const void* const* h_packed,
+                                   const int32_t* h_widths, int n_filters, const float* lowpass,
+                                   const void* lowpass_packed, const float* early_filter, const void* early_packed,
+                                   int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
+                                   float scale_all, int out_format, float sqrt_eps, float* out, int64_t T,
+                                   void* workspace, size_t ws_bytes, int path, void* stream);
+/* Host-only plan of one push (B = 1) for tests: per signal s (the raw samples first when early_factor > 1),
+ * out[8 s ..] = final samples before and after the push, ring length, first sample kept after it, source origin
+ * of its FIR stage and that stage's first output row (-1: the stage computes nothing), and the stage's CUDA-core
+ * edge-fix windows of next-level outputs: head [R0 of s + 1, out[8 s + 6]) and tail [out[8 s + 7], R1 of s + 1)
+ * (none: 0 / -1); then out[8 n_signals] = the frame bound after the push. */
+int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int flush,
+                                  int n_octaves, const int32_t* widths, int hop, int early_factor, int pad_mode,
+                                  int64_t* out);
+
 /* Streamed inverse STFT: nnab_istft_forward's arguments, with the frames of ONE push as X (B, f_in, T, 2)
  * (T may be 0) and in front of them
  *   state     DEVICE fp32, nnab_chunk_state_bytes(B, n_fft) bytes: the overlap-add partial sums later frames

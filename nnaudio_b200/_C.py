@@ -133,6 +133,13 @@ for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_fo
     SIGNATURES[_name.replace("_forward", "_chunk_forward")] = (_res, _CHUNK_HEAD + _args[4:])
     _wres, _wargs = SIGNATURES[_ws + "_workspace_bytes"]
     SIGNATURES[_ws + "_chunk_workspace_bytes"] = (_wres, _CHUNK_WS_HEAD + _wargs[2:6] + [c_int] + _wargs[6:])
+SIGNATURES["nnab_cqt_pyramid_chunk_state_bytes"] = (c_size_t, [c_int64, c_int, _P, c_int, c_int])
+SIGNATURES["nnab_cqt_pyramid_chunk_workspace_bytes"] = (
+    c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int, _P, c_int, c_int, c_int])
+SIGNATURES["nnab_cqt_pyramid_chunk_forward"] = (
+    c_int, _CHUNK_HEAD + SIGNATURES["nnab_cqt_pyramid_forward"][1][4:])
+SIGNATURES["nnab_debug_pyramid_chunk_plan"] = (
+    c_int, [c_int64, c_int64, c_int64, c_int64, c_int, c_int, _P, c_int, c_int, c_int, _P])
 SIGNATURES["nnab_istft_chunk_workspace_bytes"] = SIGNATURES["nnab_istft_workspace_bytes"]
 SIGNATURES["nnab_istft_chunk_forward"] = (
     c_int, [_P, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, c_int, c_int64, _P,
@@ -655,6 +662,52 @@ def cqt1992v2_chunk_forward(st, x, flush, T, k_real, k_imag, packed, k_begin, k_
             _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode,
             _ptr(scale), scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
     return _chunk_result(rc, out, "nnab_cqt1992v2_chunk_forward")
+
+
+def cqt_pyramid_chunk_state_bytes(B: int, widths, hop: int, early_factor: int) -> int:
+    w = (c_int32 * len(widths))(*[int(v) for v in widths])
+    return int(lib().nnab_cqt_pyramid_chunk_state_bytes(int(B), len(widths), w, int(hop), int(early_factor)))
+
+
+def cqt_pyramid_chunk_plan(received, n_carry, frames, n, flush, widths, hop, pad_mode, early_factor=1):
+    """Host-only plan of one push (``nnab_debug_pyramid_chunk_plan``): per signal (R before, R after, ring
+    length, first sample kept, FIR source origin, first FIR row or -1, head edge-fix end, tail edge-fix start),
+    and the frame bound after the push.  Raises on counters no stream can have."""
+    n_sig = len(widths) + (1 if early_factor > 1 else 0)
+    w = (c_int32 * len(widths))(*[int(v) for v in widths])
+    buf = (c_int64 * (8 * n_sig + 1))()
+    _check(lib().nnab_debug_pyramid_chunk_plan(int(received), int(n_carry), int(frames), int(n), int(flush),
+                                               len(widths), w, int(hop), int(early_factor), int(pad_mode), buf),
+          "nnab_debug_pyramid_chunk_plan")
+    return [tuple(buf[8 * s:8 * s + 8]) for s in range(n_sig)], int(buf[8 * n_sig])
+
+
+def cqt_pyramid_chunk_forward(st, x, flush, T, banks_real, banks_imag, packed, lowpass, lowpass_packed,
+                              early_filter, early_packed, early_factor, hop, pad_mode, n_bins, scale, scale_all,
+                              out_format, sqrt_eps, path=None):
+    """One push of ``nnaudio_b200.streaming.StreamingPyramid`` (``st``: its rings and counters); the remaining
+    arguments are ``cqt_pyramid_forward``'s.  None when the configuration has no streamed plan
+    (NNAB_EUNSUPPORTED, nothing enqueued)."""
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    B, dev = st.batch, st.ring.device
+    n_oct = len(banks_real)
+    re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
+    im_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_imag])
+    pk_arr = (c_void_p * n_oct)(*[(t.data_ptr() if t is not None else None) for t in packed])
+    widths = (c_int32 * n_oct)(*[int(t.shape[1]) for t in banks_real])
+    out = torch.empty((B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2), dtype=torch.float32,
+                      device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(L.nnab_cqt_pyramid_chunk_workspace_bytes(
+            B, st.received, st.n_carry, st.frames, n, int(flush), n_oct, widths, hop, early_factor, pad_mode), dev)
+        rc = L.nnab_cqt_pyramid_chunk_forward(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush), n_oct,
+            re_arr, im_arr, pk_arr, widths, banks_real[0].shape[0], _ptr(lowpass), _ptr(lowpass_packed),
+            _ptr(early_filter), _ptr(early_packed), early_factor, hop, pad_mode, n_bins, _ptr(scale), scale_all,
+            out_format, sqrt_eps, _ptr(out) if T > 0 else None, T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_cqt_pyramid_chunk_forward")
 
 
 def istft_chunk_forward(st, X, flush, length, n_out, packed, window, n_fft, hop, center):

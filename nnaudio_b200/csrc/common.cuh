@@ -64,6 +64,11 @@ struct DecimParams {
   void* pf; int64_t pf_plane, pf_pitch;
   float* y32; int64_t y32_pitch;
   int64_t len_out;  // valid samples per clip of the next level
+  // streamed pushes (DESIGN §3.10): outputs below `lo` are not stored and y32 holds output n at n - lo;
+  // skip_edges bit 0 / 1: fir_edge_fix_kernel leaves the head / tail alone (the launch does not start at the
+  // stream's first output / the stream has not ended).  Zero for the whole-clip call.
+  int64_t lo;
+  int skip_edges;
 };
 
 // Banded filterbank table: the (at most two) non-zero weights of every FFT bin.
@@ -204,6 +209,9 @@ int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_
 constexpr int TC_SPLIT_PLAIN = 0;
 constexpr int TC_SPLIT_POLY4 = 1;
 int tc_problem_split(const FramedProblem& q, void* planes, cudaStream_t stream, int layout);
+// planes of the virtual clip cs (clip_pitch samples per clip from its first sample) in a caller geometry
+int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_pitch, int64_t plane_stride,
+                   void* planes, cudaStream_t stream);
 // store raw samples [from, total) of the chunk into the carry ring (cs.received = raw index of chunk[0])
 int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,

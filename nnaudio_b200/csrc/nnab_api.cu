@@ -1388,6 +1388,377 @@ int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L
   return NNAB_OK;
 }
 
+// ------------------------------------------------------------ streamed pyramid ----
+// Signals of a stream: the raw samples when an early stage feeds level 0, then one per octave (octave i on
+// signal i + e).  Stage s turns signal s into s + 1 (factor d[s]): y[n] = sum_m fir[m] x[d n + m - 127].
+// Every per-signal number is a function of the raw count alone: before the end, sample n of signal s + 1 is
+// final once d n + c of signal s have arrived -- c = 129 (its last tap reads d n + 128), 130 on the gen-2 plan,
+// whose edge fix recomputes the last 64 outputs of the whole clip on the CUDA cores: with one sample more, n is
+// never one of them.  Signal s keeps an fp32 ring (stream b at ring[b * len + r % len]) of what later pushes read.
+struct PyrStream {
+  int n_sig, e, n_oct, c;
+  bool gen2;
+  int d[33];
+  int width[32], hop[32], pad[32];
+  int64_t ring_len[33];
+  size_t ring_off[33];  // floats
+  size_t state_floats;  // per stream
+};
+
+static bool pyr_stream_init(int n_octaves, const int32_t* widths, int hop, int early_factor, bool gen2,
+                            PyrStream* ps) {
+  if (n_octaves <= 0 || n_octaves > 32 || widths == nullptr || hop <= 0 || early_factor < 1) return false;
+  if (hop % (1 << (n_octaves - 1)) != 0) return false;  // every octave frames at hop / 2^i
+  PyrStream& p = *ps;
+  p.n_oct = n_octaves;
+  p.e = early_factor > 1 ? 1 : 0;
+  p.n_sig = n_octaves + p.e;
+  p.gen2 = gen2;
+  p.c = gen2 ? 130 : 129;
+  for (int s = 0; s + 1 < p.n_sig; ++s) p.d[s] = (p.e && s == 0) ? early_factor : 2;
+  for (int i = 0; i < n_octaves; ++i) {
+    if (widths[i] < 2) return false;
+    p.width[i] = widths[i]; p.hop[i] = hop >> i; p.pad[i] = widths[i] / 2;
+  }
+  // ring bounds (with the 130 of either plan, so the state size does not depend on the plan): a FIR source reads
+  // back from row origin 128 d floor(R'/128) - 128, at most 130 + 127 d + 128 samples; an octave from its first
+  // unreturned frame, which the slowest octave holds back by at most (130 + need_i) 2^(i - l) samples of level l
+  // (need_i = width_i - pad_i)
+  size_t off = 0;
+  for (int s = 0; s < p.n_sig; ++s) {
+    int64_t span = 0;
+    if (s + 1 < p.n_sig) span = 130 + 127 * (int64_t)p.d[s] + 128;
+    const int l = s - p.e;
+    if (l >= 0) {
+      int64_t lag = 0;
+      for (int i = 0; i < n_octaves; ++i) {
+        const int64_t need = p.width[i] - p.pad[i];
+        const int64_t a = i >= l ? (130 + need) << (i - l) : need;
+        lag = a > lag ? a : lag;
+      }
+      const int64_t o = p.pad[l] + 1 + lag;
+      span = o > span ? o : span;
+    }
+    p.ring_len[s] = (span + 64 + 63) / 64 * 64;
+    p.ring_off[s] = off;
+    off += (size_t)p.ring_len[s];
+  }
+  p.state_floats = off;
+  return true;
+}
+
+// Samples of every signal after `raw` raw samples: final ones before the end, all of them on flush.
+static void pyr_counts(const PyrStream& p, int64_t raw, int flush, int64_t* R) {
+  R[0] = raw;
+  for (int s = 0; s + 1 < p.n_sig; ++s) {
+    if (flush) R[s + 1] = decimated_len(R[s], p.d[s]);
+    else R[s + 1] = R[s] >= p.c ? (R[s] - p.c) / p.d[s] + 1 : 0;
+  }
+}
+
+// Frames final in every octave (before the end).
+static int64_t pyr_ready_frames(const PyrStream& p, const int64_t* R, int pad_mode) {
+  int64_t t = INT64_MAX;
+  for (int i = 0; i < p.n_oct; ++i) {
+    const int64_t f = chunk_ready_frames(R[i + p.e], p.width[i], p.hop[i], p.pad[i], pad_mode);
+    t = f < t ? f : t;
+  }
+  return t;
+}
+
+// First sample of signal s a later push reads, after `frames` frames with the counts R.
+static int64_t pyr_keep(const PyrStream& p, int s, const int64_t* R, int64_t frames) {
+  int64_t k = R[s];
+  const int l = s - p.e;
+  if (l >= 0) k = chunk_carry_start(R[s], frames, p.hop[l], p.pad[l]);
+  if (s + 1 < p.n_sig) {
+    int64_t f = 128 * (int64_t)p.d[s] * (R[s + 1] / 128) - 128;
+    f = f < 0 ? 0 : f;
+    k = f < k ? f : k;
+  }
+  return k;
+}
+
+// One push: the counts before (R0) and after (R1) it, the frames it returns and the workspace layout.
+struct PyrPush {
+  int64_t R0[33], R1[33];
+  int64_t t_end;
+  int mode[32];               // each octave's padding (reflect falls back to constant on short levels at flush)
+  int64_t np[33];             // new-sample buffer pitch of signal s >= 1 (floats)
+  size_t nbuf[33], scratch, scratch_bytes, total;
+};
+
+// Plane geometry of octave l's push clip of `len` samples for the octave kernel (gen-2 single-phase levels):
+// (clip pitch, plane stride); the pitch is a multiple of lcm(hop, 64), as the kernel's row blocks need.
+static void pyr_oct_geom(const PyrStream& p, int l, int64_t B, int64_t len, int64_t* pitch, int64_t* plane) {
+  const int h = p.hop[l];
+  const int64_t gran = (int64_t)h / gcd64(h, 64) * 64;
+  *pitch = (len + gran - 1) / gran * gran;
+  const int64_t kpad = (p.width[l] + 63) / 64 * 64;
+  const int64_t rows = B * (*pitch / h) + (kpad + h - 1) / h + 1;
+  *plane = (rows * h + 255) / 256 * 256;
+}
+
+static int pyr_push_plan(const PyrStream& p, int64_t B, int64_t received, int64_t n_carry, int64_t frames,
+                         int64_t n, int flush, int pad_mode, PyrPush* o) {
+  if (B < 0 || B > 65535 || received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  pyr_counts(p, received, 0, o->R0);
+  if (frames != pyr_ready_frames(p, o->R0, pad_mode) || n_carry != received - pyr_keep(p, 0, o->R0, frames))
+    return NNAB_EINVAL;
+  const int64_t total = received + n;
+  pyr_counts(p, total, flush, o->R1);
+  for (int i = 0; i < p.n_oct; ++i) {
+    const int64_t len = o->R1[i + p.e];
+    o->mode[i] = (flush && pad_mode == NNAB_PAD_REFLECT && p.pad[i] >= len) ? NNAB_PAD_CONSTANT : pad_mode;
+  }
+  if (flush) {
+    o->t_end = -1;
+    for (int i = 0; i < p.n_oct; ++i) {
+      const int64_t len = o->R1[i + p.e];
+      if (len <= 0) return NNAB_EINVAL;
+      const int64_t f = frames_of(len, p.width[i], p.hop[i], p.pad[i]);
+      if (f <= 0 || (o->t_end >= 0 && f != o->t_end)) return NNAB_EINVAL;
+      o->t_end = f;
+    }
+    if (o->t_end < frames) return NNAB_EINVAL;
+  } else {
+    o->t_end = pyr_ready_frames(p, o->R1, pad_mode);
+    for (int s = 0; s < p.n_sig; ++s)
+      if (o->R1[s] - pyr_keep(p, s, o->R1, o->t_end) > p.ring_len[s]) return NNAB_EINVAL;
+  }
+  // workspace: the new samples of every computed signal, then one scratch reused by the launches in order
+  size_t off = 0;
+  for (int s = 1; s < p.n_sig; ++s) {
+    o->np[s] = (int64_t)align_up((size_t)(o->R1[s] - o->R0[s] > 0 ? o->R1[s] - o->R0[s] : 1), 8);
+    o->nbuf[s] = off;
+    off += align_up((size_t)B * o->np[s] * sizeof(float), 256);
+  }
+  size_t sc = 0;
+  const int64_t T = o->t_end - frames;
+  for (int s = 0; s < p.n_sig; ++s) {
+    const int l = s - p.e;
+    if (l >= 0 && T > 0) {
+      const int64_t len = (T - 1) * p.hop[l] + p.width[l];
+      size_t need = tc_workspace_bytes(B, len, p.width[l], p.hop[l], 0);
+      if (p.gen2 && p.hop[l] % 8 == 0) {
+        int64_t pitch, plane;
+        pyr_oct_geom(p, l, B, len, &pitch, &plane);
+        need = (size_t)plane * 4 + 256;
+      }
+      sc = need > sc ? need : sc;
+    }
+    if (s + 1 < p.n_sig && o->R1[s + 1] > o->R0[s + 1]) {
+      const int64_t FT = (o->R1[s + 1] + 127) / 128 - o->R0[s + 1] / 128;
+      const int kf = tc_fir_k(FIR_TAPS, p.d[s]);
+      const size_t need = p.gen2 ? (size_t)((B * (FT + 1) + 2) * 256) * 4 + 256
+                                 : tc_workspace_bytes(B, (FT - 1) * 128 * (int64_t)p.d[s] + kf, kf, 128 * p.d[s], 0);
+      sc = need > sc ? need : sc;
+    }
+  }
+  o->scratch = off;
+  o->scratch_bytes = sc;
+  o->total = off + sc + 512;
+  return NNAB_OK;
+}
+
+// The whole-clip call's plan for these shapes: gen-2 without early downsampling when every FIR-source bank is
+// 256 wide (plan_pyramid2), else gen-1.
+static bool pyr_gen2(int n_octaves, const int32_t* widths, int early_factor) {
+  if (early_factor > 1) return false;
+  for (int i = 0; i + 1 < n_octaves; ++i)
+    if (widths[i] / 2 != 128) return false;
+  return true;
+}
+
+size_t nnab_cqt_pyramid_chunk_state_bytes(int64_t B, int n_octaves, const int32_t* widths, int hop,
+                                          int early_factor) {
+  PyrStream p;
+  if (B < 0 || widths == nullptr || !pyr_stream_init(n_octaves, widths, hop, early_factor, false, &p)) return 0;
+  return (size_t)B * p.state_floats * sizeof(float);
+}
+
+size_t nnab_cqt_pyramid_chunk_workspace_bytes(int64_t B, int64_t received, int64_t n_carry, int64_t frames,
+                                              int64_t n, int flush, int n_octaves, const int32_t* widths,
+                                              int hop, int early_factor, int pad_mode) {
+  PyrStream p;
+  PyrPush pp;
+  if (widths == nullptr ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return 0;
+  if (pyr_push_plan(p, B, received, n_carry, frames, n, flush, pad_mode, &pp)) return 0;
+  return pp.total;
+}
+
+int nnab_cqt_pyramid_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                   const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
+                                   int flush, int n_octaves, const float* const* h_k_real,
+                                   const float* const* h_k_imag, const void* const* h_packed,
+                                   const int32_t* h_widths, int n_filters, const float* lowpass,
+                                   const void* lowpass_packed, const float* early_filter, const void* early_packed,
+                                   int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
+                                   float scale_all, int out_format, float sqrt_eps, float* out, int64_t T,
+                                   void* workspace, size_t ws_bytes, int path, void* stream) {
+  if (state == nullptr || !dtype_ok(chunk_dtype) || (n > 0 && chunk == nullptr) || chunk_pitch < n ||
+      (T > 0 && out == nullptr) || h_k_real == nullptr || h_k_imag == nullptr || h_widths == nullptr ||
+      lowpass == nullptr || n_octaves <= 0 || n_octaves > 32 || n_filters <= 0 || hop <= 0 || n_bins <= 0 ||
+      early_factor < 1 || (early_factor > 1 && early_filter == nullptr) || T < 0)
+    return NNAB_EINVAL;
+  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX && out_format != NNAB_FMT_PHASE_UNIT)
+    return NNAB_EINVAL;
+  const bool gen2 = pyr_gen2(n_octaves, h_widths, early_factor);
+  PyrStream p;
+  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, gen2, &p)) return NNAB_EUNSUPPORTED;
+  PyrPush pp;
+  int rc = pyr_push_plan(p, B, received, n_carry, frames, n, flush, pad_mode, &pp);
+  if (rc) return rc;
+  if (T != pp.t_end - frames) return NNAB_EINVAL;
+  // the whole-clip call's all-tensor-core plans need every packed operand and the tensor-core path
+  bool packed_ok = path != NNAB_PATH_SIMT && h_packed != nullptr && lowpass_packed != nullptr &&
+                   (early_factor <= 1 || early_packed != nullptr);
+  for (int i = 0; packed_ok && i < n_octaves; ++i) packed_ok = h_packed[i] != nullptr;
+  if (!packed_ok) return NNAB_EUNSUPPORTED;
+  if ((rc = check_arch())) return rc;
+  if (workspace == nullptr || ws_bytes < pp.total) return NNAB_EWORKSPACE;
+  if (B == 0) return NNAB_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* scratch = ws + pp.scratch;
+  const PyramidCall c{nullptr, NNAB_DTYPE_F32, B, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
+                      n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
+                      scale_all, out_format, sqrt_eps, out, T, ws, ws_bytes, s};
+  float* ring = static_cast<float*>(state);
+
+  // pass 0 checks every launch against the kernels' limits (as the whole-clip plan selection does) so that a
+  // push that cannot run returns before anything is enqueued; pass 1 runs them
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int sg = 0; sg < p.n_sig; ++sg) {
+      // signal sg of this push: ring [keep, R0) then the new samples [R0, R1) (the chunk for the raw signal)
+      ChunkSource cs{};
+      cs.ring = ring + (size_t)B * p.ring_off[sg];
+      cs.ring_pitch = cs.ring_len = p.ring_len[sg];
+      cs.chunk = sg == 0 ? chunk : (const void*)(ws + pp.nbuf[sg]);
+      cs.chunk_pitch = sg == 0 ? chunk_pitch : pp.np[sg];
+      cs.received = pp.R0[sg];
+      cs.total = pp.R1[sg];
+      const int dt = sg == 0 ? chunk_dtype : NNAB_DTYPE_F32;
+      const int l = sg - p.e;
+      if (l >= 0 && T > 0) {
+        // octave l: frames [frames, t_end) from its first unreturned frame, on the whole-clip plan's kernel
+        ChunkSource co = cs;
+        co.origin = frames * p.hop[l] - p.pad[l];
+        co.length = (T - 1) * p.hop[l] + p.width[l];
+        co.pad_mode = pp.mode[l];
+        co.at_end = flush ? 1 : 0;
+        FramedProblem q = octave_problem(c, l, co.length, p.hop[l], pp.mode[l]);
+        q.pad = 0; q.x_dtype = dt; q.chunk = &co;
+        if (gen2 && p.hop[l] % 8 == 0) {
+          // gen-2 single-phase level: caller planes, the octave kernel when it takes the problem
+          int64_t pitch, plane;
+          pyr_oct_geom(p, l, B, co.length, &pitch, &plane);
+          FramedProblem qp = q;
+          qp.chunk = nullptr;
+          qp.presplit = scratch; qp.presplit_t_slots = pitch / p.hop[l]; qp.presplit_plane_stride = plane;
+          const bool oct = octave_tc_ok(qp);
+          if (pass == 0) {
+            if (!oct && !tc_supported(qp)) return NNAB_EUNSUPPORTED;
+          } else {
+            if ((rc = tc_chunk_split(co, dt, B, pitch, plane, scratch, s))) return rc;
+            if (oct) {
+              std::pair<cudaEvent_t, cudaEvent_t> pr;
+              const bool timed = prof_begin(s, &pr);
+              rc = launch_octave_tc(qp, c.packed[l], s);
+              if (timed) prof_end(s, pr);
+            } else {
+              rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
+            }
+            if (rc) return rc;
+          }
+        } else if (pass == 0) {
+          if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+        } else if ((rc = run_framed(q, c.packed[l], scratch, pp.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+          return rc;
+        }
+      }
+      if (sg + 1 < p.n_sig && pp.R1[sg + 1] > pp.R0[sg + 1]) {
+        // stage sg -> sg + 1 from the row holding its first new output: the rows' accumulation order is the
+        // whole clip's; only the new outputs are stored, and the edge fix runs only at the stream's true ends
+        const int d = p.d[sg];
+        const int64_t t0 = pp.R0[sg + 1] / 128;
+        const int64_t FT = (pp.R1[sg + 1] + 127) / 128 - t0;
+        ChunkSource cf = cs;
+        cf.origin = 128 * d * t0 - 128;
+        cf.pad_mode = NNAB_PAD_CONSTANT;
+        cf.at_end = 1;
+        DecimParams dec{};
+        dec.len_out = pp.R1[sg + 1] - 128 * t0;
+        dec.lo = pp.R0[sg + 1] - 128 * t0;
+        dec.y32 = (float*)(ws + pp.nbuf[sg + 1]);
+        dec.y32_pitch = pp.np[sg + 1];
+        dec.skip_edges = (t0 > 0 ? 1 : 0) | (flush ? 0 : 2);
+        const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
+        if (gen2) {
+          if (pass == 1) {
+            const int64_t pitch = 256 * (FT + 1), plane = (B * (FT + 1) + 2) * 256;
+            cf.length = pitch;
+            if ((rc = tc_chunk_split(cf, dt, B, pitch, plane, scratch, s))) return rc;
+            if ((rc = launch_fir_stage_tc(scratch, B, pp.R1[sg] - 256 * t0, pitch, plane, FIR_OFF, fir_packed,
+                                          c.lowpass, FIR_TAPS, dec, s)))
+              return rc;
+          }
+        } else {
+          FramedProblem q{};
+          q.B = B; q.x_dtype = dt; q.F = 64; q.K = tc_fir_k(FIR_TAPS, d); q.hop = 128 * d;
+          q.L = (FT - 1) * q.hop + q.K; q.pad = 0; q.pad_mode = NNAB_PAD_CONSTANT; q.scale_all = 1.f;
+          q.fmt = FMT_DECIM; q.power = 1.f; q.T = FT; q.out_bins = 64;
+          q.dec = dec;
+          cf.length = q.L;
+          q.chunk = &cf;
+          if (pass == 0) {
+            if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+          } else if ((rc = run_framed(q, fir_packed, scratch, pp.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+            return rc;
+          }
+        }
+      }
+      if (pass == 1 && !flush) {  // after this signal's readers: what later pushes read of it into its ring
+        const int64_t keep = pyr_keep(p, sg, pp.R1, pp.t_end);
+        if ((rc = tc_chunk_carry(cs, dt, B, keep > pp.R0[sg] ? keep : pp.R0[sg], s))) return rc;
+      }
+    }
+  }
+  return NNAB_OK;
+}
+
+int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int flush,
+                                  int n_octaves, const int32_t* widths, int hop, int early_factor, int pad_mode,
+                                  int64_t* out) {
+  if (out == nullptr) return NNAB_EINVAL;
+  PyrStream p;
+  PyrPush pp;
+  if (widths == nullptr ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  const int rc = pyr_push_plan(p, 1, received, n_carry, frames, n, flush, pad_mode, &pp);
+  if (rc) return rc;
+  // per signal: R before, R after, ring length, keep after (flush: R after), FIR source origin, first row
+  // (-1: no stage), then the stage's edge-fix windows of next-level outputs: head [R0', head_end) and tail
+  // [tail_begin, R1') (empty: head_end = 0, tail_begin = -1); then the frame bound
+  for (int s = 0; s < p.n_sig; ++s) {
+    int64_t* r = out + 8 * s;
+    r[0] = pp.R0[s]; r[1] = pp.R1[s]; r[2] = p.ring_len[s];
+    r[3] = flush ? pp.R1[s] : pyr_keep(p, s, pp.R1, pp.t_end);
+    const bool stage = s + 1 < p.n_sig && pp.R1[s + 1] > pp.R0[s + 1];
+    const int64_t t0 = stage ? pp.R0[s + 1] / 128 : 0;
+    r[4] = stage ? 128 * (int64_t)p.d[s] * t0 - 128 : 0;
+    r[5] = stage ? t0 : -1;
+    r[6] = (stage && p.gen2 && t0 == 0) ? (pp.R1[s + 1] < 64 ? pp.R1[s + 1] : 64) : 0;
+    r[7] = (stage && p.gen2 && flush) ? (pp.R1[s + 1] - 64 > pp.R0[s + 1] ? pp.R1[s + 1] - 64 : pp.R0[s + 1]) : -1;
+  }
+  out[8 * p.n_sig] = pp.t_end;
+  return NNAB_OK;
+}
+
 // ----------------------------------------------------------------- inverse STFT ----
 static __global__ void istft_scale_kernel(const float* __restrict__ window, float inv_n, int n,
                                           float* __restrict__ scale) {

@@ -278,6 +278,20 @@ static int launch_problem_split(const FramedProblem& q, dim3 grid, int shift, in
   return NNAB_OK;
 }
 
+int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_pitch, int64_t plane_stride,
+                   void* planes, cudaStream_t stream) {
+  if (B <= 0 || clip_pitch <= 0) return NNAB_OK;
+  if (B > 65535 || clip_pitch % 8 != 0) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
+  const int rc = with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    chunk_split_kernel<<<grid, 256, 0, stream>>>(cs, xs, 0, clip_pitch, plane_stride, 0,
+                                                 static_cast<__nv_bfloat16*>(planes));
+  });
+  if (rc) return rc;
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
 int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream) {
   if (from >= cs.total || B <= 0) return NNAB_OK;
   if (B > 65535) return NNAB_EUNSUPPORTED;

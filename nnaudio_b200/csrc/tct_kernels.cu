@@ -735,15 +735,20 @@ __global__ void __launch_bounds__(128) fir_edge_fix_kernel(
   const int64_t b = blockIdx.y;
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * 4 + (threadIdx.x >> 5);  // 0..63: head outputs, 64..127: tail outputs
+  const bool head = !(d.skip_edges & 1);
+  if (i < 64 ? !head : (d.skip_edges & 2) != 0) return;
   const int64_t n = (i < 64) ? i : d.len_out - 128 + i;
-  if (i >= 64 && n < 64) return;  // short clip: the head half already covers it
-  if (n < 0 || n >= d.len_out) return;
+  if (i >= 64 && head && n < 64) return;  // short clip: the head half already covers it
+  if (n < d.lo || n >= d.len_out) return;
   const __nv_bfloat16* sb = src + b * src_pitch + src_off;
+  // below the launch's first sample lies the stream's zero padding, or (a push past the stream's first row)
+  // the src_off carried samples in front of it
+  const int64_t j_lo = head ? 0 : -(int64_t)src_off;
   float acc = 0.f;
 #pragma unroll 8
   for (int m = lane; m < taps; m += 32) {  // taps / 32 independent loads in flight per lane
     const int64_t j = 2 * n + m - (taps - 1) / 2;
-    const bool in = j >= 0 && j < len_src;
+    const bool in = j >= j_lo && j < len_src;
     const float hi = in ? __bfloat162float(sb[j]) : 0.f;
     const float lo = in ? __bfloat162float(sb[src_plane + j]) : 0.f;
     acc = fmaf(__ldg(fir + m), hi + lo, acc);
@@ -764,7 +769,7 @@ __global__ void __launch_bounds__(128) fir_edge_fix_kernel(
       }
     }
   }
-  if (d.y32 != nullptr) d.y32[b * d.y32_pitch + n] = acc;
+  if (d.y32 != nullptr) d.y32[b * d.y32_pitch + (n - d.lo)] = acc;
 }
 
 // One FIR stage: source level planes (single set, samples at offset src_pad, clip pitch a multiple of

@@ -382,29 +382,32 @@ def _v2_normalization(mod, normalization_type, output_format):
     return scale, scale_all, eps
 
 
-def _pyramid_forward(mod, x, output_format, normalization):
-    """Shared by CQT2010v2, VQT and CQT2010: plan the octave lengths on the host (for the
-    reference's warnings / errors), then one C call.  ``normalization`` = (scale, scale_all, eps)."""
-    scale, scale_all, eps = normalization
-    banks_real, banks_imag, packed = mod._banks()
-    early = mod.early_downsample_filter if mod.earlydownsample else None
+def _pyramid_length_plan(mod, B, L):
+    """(T, per-octave reflect fallbacks) of ``B`` clips of ``L`` samples through ``mod``'s pyramid, with the
+    reference's errors and warnings (also the end of a stream)."""
     factor = int(mod.downsample_factor) if mod.earlydownsample else 1
-    L = x.shape[-1]
     L0 = (L - 2) // factor + 1 if factor > 1 else L
     if factor > 1 and L < 2:
         raise RuntimeError("Kernel size can't be greater than actual input size")
-    widths = [int(b.shape[1]) for b in banks_real]
+    widths = [int(b.shape[1]) for b in mod._banks()[0]]
     T, fallbacks = _octave_plan(L0, mod.hop_length, widths, mod.pad_mode)
     for i, fb in enumerate(fallbacks):
         if fb:
             warnings.warn(
-                f"\ninput size = {(x.shape[0], 1, L0)}\tkernel size = {widths[i]}\n"
+                f"\ninput size = {(B, 1, L0)}\tkernel size = {widths[i]}\n"
                 "padding with reflection mode might not be the best choice, try using constant padding",
                 UserWarning,
             )
-    if wants_grad(mod, x):
-        return _pyramid_forward_autograd(mod, upcast_16bit(x), output_format, fallbacks, factor, scale,
-                                         scale_all, eps)
+    return T, fallbacks
+
+
+def _pyramid_args(mod, output_format, normalization):
+    """Keyword arguments after ``x`` (``T`` aside) of the ``_C.cqt_pyramid_forward`` call of the inference
+    path; shared with ``nnaudio_b200.streaming.StreamingPyramid``."""
+    scale, scale_all, eps = normalization
+    banks_real, banks_imag, packed = mod._banks()
+    early = mod.early_downsample_filter if mod.earlydownsample else None
+    factor = int(mod.downsample_factor) if mod.earlydownsample else 1
     lowpass = mod.lowpass_filter.detach().reshape(-1)
     early_flat = early.detach().reshape(-1) if early is not None else None
     for t in (lowpass, early_flat):
@@ -414,11 +417,22 @@ def _pyramid_forward(mod, x, output_format, normalization):
         mod._fir_packed = (PackedFir(), PackedFir())
     lowpass_packed = mod._fir_packed[0].get(lowpass, 2)
     early_packed = mod._fir_packed[1].get(early_flat, factor) if early_flat is not None else None
-    return _C.cqt_pyramid_forward(
-        x, banks_real, banks_imag, packed, lowpass, lowpass_packed, early_flat, early_packed,
-        factor, mod.hop_length,
-        pad_mode_id(mod.pad_mode), mod.n_bins, scale, scale_all, _FORMATS[output_format], eps, T,
-    )
+    return dict(banks_real=banks_real, banks_imag=banks_imag, packed=packed, lowpass=lowpass,
+                lowpass_packed=lowpass_packed, early_filter=early_flat, early_packed=early_packed,
+                early_factor=factor, hop=mod.hop_length, pad_mode=pad_mode_id(mod.pad_mode), n_bins=mod.n_bins,
+                scale=scale, scale_all=scale_all, out_format=_FORMATS[output_format], sqrt_eps=eps)
+
+
+def _pyramid_forward(mod, x, output_format, normalization):
+    """Shared by CQT2010v2, VQT and CQT2010: plan the octave lengths on the host (for the
+    reference's warnings / errors), then one C call.  ``normalization`` = (scale, scale_all, eps)."""
+    scale, scale_all, eps = normalization
+    T, fallbacks = _pyramid_length_plan(mod, x.shape[0], x.shape[-1])
+    if wants_grad(mod, x):
+        factor = int(mod.downsample_factor) if mod.earlydownsample else 1
+        return _pyramid_forward_autograd(mod, upcast_16bit(x), output_format, fallbacks, factor, scale,
+                                         scale_all, eps)
+    return _C.cqt_pyramid_forward(x, T=T, **_pyramid_args(mod, output_format, normalization))
 
 
 def _framed_complex_autograd(mod, tag, sig, w_re, w_im, hop, center, pad_mode):

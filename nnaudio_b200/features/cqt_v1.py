@@ -322,12 +322,16 @@ class CQT2010(nn.Module):
         output_format = output_format or self.output_format
         _check_format_and_norm(output_format, normalization_type)
         x = broadcast_dim(x)
+        return _pyramid_forward(self, x, output_format, self._normalization(normalization_type))
+
+    def _normalization(self, normalization_type):
+        """(per-bin scale or None, global factor, sqrt eps) of the pyramid call (cqt.py:531-532)."""
         scale, scale_all = None, 1.0
-        if normalization_type == "librosa":  # cqt.py:531-532
+        if normalization_type == "librosa":
             scale = self._scale.get(self.lenghts, 1.0 / self.n_fft)
         elif normalization_type == "wrap":
             scale_all = 2.0 / self.n_fft
-        return _pyramid_forward(self, x, output_format, (scale, scale_all, 0.0))
+        return scale, scale_all, 0.0
 
     def extra_repr(self) -> str:
         return "STFT kernel size = {}, CQT kernel size = {}".format(

@@ -13,6 +13,9 @@ bf16 planes from the carried fp32 samples and the new chunk.  Plans that read th
 upcast chunk, padded and concatenated with torch, through the module's offline call with ``center=False``.
 A push never reads the device back or synchronises.
 
+``StreamingPyramid(module, batch)`` streams through the ÷2 resampling pyramid of ``CQT2010v2``, ``VQT`` and
+``CQT2010`` on the whole-clip call's tensor-core plan: each push returns the frames final in every octave.
+
 ``StreamingInverse(module, batch)`` streams complex frames through the inverse STFT: each push returns the
 output samples no later frame can change, ``flush(length=None)`` the rest.
 """
@@ -21,15 +24,18 @@ from __future__ import annotations
 import torch
 
 from . import _C
-from .features.cqt import CQT1992v2
-from .features.cqt_v1 import CQT1992
+from .features.cqt import (CQT1992v2, CQT2010v2, _check_format_and_norm, _pyramid_args, _pyramid_length_plan,
+                           _v2_normalization)
+from .features.cqt_v1 import CQT1992, CQT2010
 from .features.gammatone import Gammatonegram
 from .features.mel import MFCC, MelSpectrogram
 from .features.stft import STFT, _inverse_args, iSTFT
+from .features.vqt import VQT
 
-__all__ = ["StreamingTransform", "StreamingInverse"]
+__all__ = ["StreamingTransform", "StreamingPyramid", "StreamingInverse"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
+_PYRAMIDS = (CQT2010v2, VQT, CQT2010)
 
 
 def _ready_frames(total, K, hop, pad, reflect):
@@ -61,7 +67,8 @@ class StreamingTransform:
         if not isinstance(module, _SUPPORTED):
             raise TypeError(
                 f"StreamingTransform supports STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2 / CQT and "
-                f"CQT1992, not {type(module).__name__} (the CQT2010 pyramids carry per-octave filter state)"
+                f"CQT1992, not {type(module).__name__}"
+                + (": stream the CQT2010 pyramids with StreamingPyramid" if isinstance(module, _PYRAMIDS) else "")
             )
         if isinstance(module, MFCC) and module.top_db is not None:
             raise ValueError(
@@ -189,6 +196,145 @@ class StreamingTransform:
         n_bins = kw["k_real"].shape[0]
         return torch.empty((self.batch, n_bins, 0) if kw["out_format"] == _C.FMT_MAGNITUDE
                            else (self.batch, n_bins, 0, 2), device=dev)
+
+
+def _check_chunk(st, chunk):
+    """The checks every push makes (shape, dtype, grad, one dtype per stream), as StreamingTransform.push."""
+    if st._flushed:
+        raise RuntimeError("push() after flush(): call reset() to start new streams")
+    if not isinstance(chunk, torch.Tensor):
+        raise TypeError("chunk must be a torch.Tensor")
+    if chunk.requires_grad:
+        raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+    if chunk.dim() != 2 or chunk.shape[0] != st.batch:
+        raise ValueError(f"chunk must be ({st.batch}, n), got {tuple(chunk.shape)}")
+    if chunk.dtype not in _C._WAVE_DTYPES:
+        raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
+    if st.dtype is not None and chunk.dtype != st.dtype:
+        raise ValueError(f"chunk dtype changed from {st.dtype} to {chunk.dtype} within a stream")
+
+
+class StreamingPyramid:
+    """Stream ``batch`` signals chunk by chunk through the CQT pyramid of ``CQT2010v2``, ``VQT`` or ``CQT2010``.
+
+    ``push(chunk)`` returns every frame final in all octaves; ``flush()`` the rest, raising (and warning) as
+    ``module(x)`` does for the stream's total length.  Concatenated along time the outputs are bitwise
+    ``module(x)`` (a 16-bit stream: ``module(x.float())``): each push runs the whole-clip call's tensor-core plan
+    (generation 2, or generation 1 with or without early downsampling) on the new samples, with the levels
+    carried in fp32 rings (DESIGN.md §3.10).  Before the end, sample n of a decimated level is final once
+    ``d n + c`` samples of its source have arrived (``c`` = 130 on generation 2, 129 otherwise), and an octave
+    frame under the ``_ready_frames`` rule of its own level, so the lowest octave sets the latency.
+    ``hop_length`` must be a multiple of ``2 ** (n_octaves - 1)``.  ``forward_kwargs``: ``output_format``,
+    ``normalization_type``.
+    """
+
+    def __init__(self, module, batch, **forward_kwargs):
+        if not isinstance(module, _PYRAMIDS):
+            raise TypeError(f"StreamingPyramid supports CQT2010v2, VQT and CQT2010, not {type(module).__name__}")
+        batch = int(batch)
+        if batch < 1 or batch > _C.MAX_BATCH:
+            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        fmt = forward_kwargs.get("output_format") or module.output_format
+        norm = forward_kwargs.get("normalization_type", "librosa")
+        _check_format_and_norm(fmt, norm)
+        if isinstance(module, CQT2010):
+            self._args = lambda: _pyramid_args(module, fmt, module._normalization(norm))
+        else:
+            self._args = lambda: _pyramid_args(module, fmt, _v2_normalization(module, norm, fmt))
+        self.module, self.batch = module, batch
+        kw = self._args()
+        self.widths = [int(b.shape[1]) for b in kw["banks_real"]]
+        self.hop, self.early = kw["hop"], kw["early_factor"]
+        n_oct = len(self.widths)
+        if self.hop % (1 << (n_oct - 1)):
+            # hop_i = hop >> i then drifts from hop / 2^i: the octaves' frame counts agree (and module(x) runs)
+            # only for clips below a length bound, so no stream of unbounded length can match it
+            raise ValueError(f"hop_length {self.hop} is not a multiple of 2^{n_oct - 1}: the octaves frame at "
+                             "different rates")
+        self._reflect = kw["pad_mode"] == _C.PAD_REFLECT
+        # the whole-clip plan: generation 2 without early downsampling when every FIR-source bank is 256 wide
+        self.generation = 2 if self.early == 1 and all(w // 2 == 128 for w in self.widths[:-1]) else 1
+        n_bytes = _C.cqt_pyramid_chunk_state_bytes(batch, self.widths, self.hop, self.early)
+        device = next(iter(module.buffers())).device
+        self.ring = torch.empty(n_bytes // 4, dtype=torch.float32, device=device)  # one fp32 ring per level
+        self.reset()
+
+    def reset(self):
+        """Start new streams (same module, same batch)."""
+        self.received = self.n_carry = self.frames = 0
+        self.dtype = None
+        self._flushed = False
+
+    # ------------------------------------------------------------------------------------------------ #
+    def _counts(self, raw):
+        """Final samples of every signal after ``raw`` raw samples (the raw samples first when an early stage
+        feeds level 0): sample n of the next signal is final once d n + c of this one have arrived."""
+        c = 130 if self.generation == 2 else 129
+        R = [raw]
+        for s in range(len(self.widths) + (self.early > 1) - 1):
+            d = self.early if (self.early > 1 and s == 0) else 2
+            R.append((R[-1] - c) // d + 1 if R[-1] >= c else 0)
+        return R
+
+    def _ready(self, raw):
+        """Frames final in every octave after ``raw`` samples."""
+        R = self._counts(raw)[1 if self.early > 1 else 0:]
+        return min(_ready_frames(R[i], w, self.hop >> i, w // 2, self._reflect) for i, w in enumerate(self.widths))
+
+    def _n_carry(self, raw, frames):
+        """Raw samples the raw ring carries (nnab.h): the top octave's (no early stage) and the first FIR stage's
+        read-back."""
+        keep = raw
+        if self.early == 1:
+            keep = _carry_start(raw, frames, self.hop, self.widths[0] // 2)
+        R = self._counts(raw)
+        if len(R) > 1:
+            d = self.early if self.early > 1 else 2
+            keep = min(keep, max(0, 128 * d * (R[1] // 128) - 128))
+        return raw - keep
+
+    def latency(self):
+        """Raw samples a push holds back behind frame t's centre t * hop in the steady state: frame t is
+        returned once t * hop + latency() samples have arrived."""
+        t = 1000 + max(self.widths)  # past every start-up effect
+        lo, hi = 0, (t + 8) * self.hop * 4 + (1 << 22)
+        while lo < hi:
+            mid = (lo + hi) // 2
+            if self._ready(mid) > t:
+                hi = mid
+            else:
+                lo = mid + 1
+        return lo - t * self.hop
+
+    def push(self, chunk: torch.Tensor) -> torch.Tensor:
+        """Feed ``chunk`` (batch, n), any n >= 0; returns the frames final in every octave."""
+        _check_chunk(self, chunk)
+        if self.dtype is None:
+            self.dtype = chunk.dtype
+        n = chunk.shape[1]
+        T = self._ready(self.received + n) - self.frames
+        return self._advance(chunk, n, False, T)
+
+    def flush(self) -> torch.Tensor:
+        """End of stream: the remaining frames (raises and warns as ``module(x)`` for this length)."""
+        if self._flushed:
+            raise RuntimeError("flush() after flush(): call reset() to start new streams")
+        T_total, _ = _pyramid_length_plan(self.module, self.batch, self.received)
+        if self.dtype is None:
+            self.dtype = torch.float32
+        out = self._advance(None, 0, True, T_total - self.frames)
+        self._flushed = True
+        return out
+
+    def _advance(self, chunk, n, flush, T):
+        out = _C.cqt_pyramid_chunk_forward(self, chunk, flush, T, **self._args())
+        if out is None:
+            raise RuntimeError(f"{type(self.module).__name__}: no streamed tensor-core pyramid plan for this "
+                               "call (NNAB_EUNSUPPORTED, e.g. NNAUDIO_B200_PATH=simt); the stream is unchanged")
+        total = self.received + n
+        self.received, self.frames = total, self.frames + T
+        self.n_carry = self._n_carry(total, self.frames)
+        return out
 
 
 class StreamingInverse:

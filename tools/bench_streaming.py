@@ -6,7 +6,9 @@ latency (push + synchronise), device time per push over many pushes (CUDA events
            center=False), i.e. the launches a push cannot avoid
   concat   the concat route (carried samples + chunk with torch, then the offline call)
 The STFT -> iSTFT case pushes each chunk through the streamed STFT and its frames through the streamed inverse
-(the offline baseline: STFT of one push's clip, then the offline inverse of its frames).
+(the offline baseline: STFT of one push's clip, then the offline inverse of its frames).  The pyramid case
+(cfg4-like: CQT2010v2, 88 bins, 64 streams, 100 ms pushes) streams through StreamingPyramid; its offline baseline
+is the whole-clip call on a clip giving one push's frames (the pyramid has no concat route).
 
     python tools/bench_streaming.py [--pushes 400] [--out results.json]
 """
@@ -24,7 +26,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from nnaudio_b200 import _C, features  # noqa: E402
-from nnaudio_b200.streaming import StreamingInverse, StreamingTransform  # noqa: E402
+from nnaudio_b200.streaming import StreamingInverse, StreamingPyramid, StreamingTransform  # noqa: E402
 
 CASES = {
     "stft1024_1x256": (lambda: features.STFT(n_fft=1024, hop_length=256, verbose=False), 1, 256),
@@ -68,6 +70,24 @@ def _measure(fn, x, chunk, pushes):
     e1.record()
     torch.cuda.synchronize()
     return statistics.median(issue), statistics.median(lat), e0.elapsed_time(e1) / pushes
+
+
+def _pyramid_row(pushes):
+    """cfg4-like pyramid: 64 streams, 100 ms pushes at 22.05 kHz."""
+    m = features.CQT2010v2(sr=22050, hop_length=512, n_bins=88, verbose=False).cuda()
+    B, chunk = 64, 2205
+    x = torch.randn(B, 200 * chunk + 8192, device="cuda")
+    with torch.no_grad():
+        st = StreamingPyramid(m, B)
+        row = {"batch": B, "chunk": chunk, "fused": _measure(st.push, x, chunk, pushes)}
+        T = max(1, round(chunk / st.hop))
+        clip = x[:, :T * st.hop - 1].contiguous()  # T frames in every octave
+        row["offline"] = _measure(lambda c: m(clip), x, chunk, pushes)
+    for k in ("fused", "offline"):
+        issue, lat, dev = row[k]
+        row[k] = {"issue_ms": round(issue, 4), "latency_ms": round(lat, 4), "device_ms": round(dev, 4),
+                  "frames_per_s": round(B * chunk / st.hop / (dev * 1e-3))}
+    return row
 
 
 def main():
@@ -120,6 +140,9 @@ def main():
                           "frames_per_s": round(B * frames_per_push / (dev * 1e-3))}
         res["cases"][name] = row
         print(name, json.dumps(row), flush=True)
+    row = _pyramid_row(args.pushes)
+    res["cases"]["pyramid_cfg4_64x100ms"] = row
+    print("pyramid_cfg4_64x100ms", json.dumps(row), flush=True)
     print(json.dumps({"card": res["card"]}))
     if args.out:
         with open(args.out, "w") as f:
