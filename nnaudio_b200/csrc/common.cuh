@@ -185,7 +185,8 @@ struct FramedProblem {
 int launch_framed_simt(const FramedProblem& p, cudaStream_t stream);
 
 // tensor-core path (tc_kernels.cu)
-bool tc_supported(const FramedProblem& p);
+// packed: the basis the launch will use, when known (a block-partial basis has its own shape limits)
+bool tc_supported(const FramedProblem& p, const void* packed = nullptr);
 size_t tc_workspace_bytes(int64_t B, int64_t L, int K, int hop, int pad);
 int launch_framed_tc(const FramedProblem& p, const void* packed, void* workspace,
                      size_t ws_bytes, cudaStream_t stream);

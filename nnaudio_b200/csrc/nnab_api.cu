@@ -109,10 +109,10 @@ static int run_framed_inner(const FramedProblem& p, const void* packed, void* ws
                       int path, cudaStream_t stream) {
   bool use_tc = false;
   if (path == NNAB_PATH_TCGEN05) {
-    if (packed == nullptr || !tc_supported(p)) return NNAB_EALIGN;
+    if (packed == nullptr || !tc_supported(p, packed)) return NNAB_EALIGN;
     use_tc = true;
   } else if (path == NNAB_PATH_AUTO) {
-    use_tc = (packed != nullptr) && tc_supported(p);
+    use_tc = (packed != nullptr) && tc_supported(p, packed);
   } else if (path != NNAB_PATH_SIMT) {
     return NNAB_EINVAL;
   }
@@ -606,7 +606,7 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     const FbWidth fw = fb_width_of(fb_table);
     p.fb_nb_mask = fw.nb_mask;
     p.fb_poly_tile = fw.poly_tile;
-    if (tc_supported(p)) {
+    if (tc_supported(p, packed)) {
       const size_t need = tc_workspace_bytes(B, L, n_fft, hop, pad);
       if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
       // the epilogue accumulates filter sums with fp32 atomics: start from zero
@@ -644,7 +644,7 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     g.out_bins = n_fb; g.bin_offset = 0;
     g.presplit = planes; g.presplit_t_slots = T; g.presplit_plane_stride = plane_stride;
     // a shape either contraction rejects takes the fp32 path below, before anything is enqueued
-    if (tc_supported(p) && tc_supported(g)) {
+    if (tc_supported(p, packed) && tc_supported(g)) {
       // the re-indexed bank (tiny: fh x kp) and its bf16 hi/lo packing
       if ((rc = launch_fb_tile_bank(fb, n_fb, F, fp.nb, fp.n_tiles, fp.phases, fp.kp, fp.fh, w_re, w_im, s)))
         return rc;

@@ -87,12 +87,15 @@ size_t tc_workspace_bytes(int64_t B, int64_t L, int K, int hop, int pad) {
   return (size_t)(2 * g.plane_stride) * sizeof(__nv_bfloat16) + 256;
 }
 
-bool tc_supported(const FramedProblem& p) {
+bool tc_supported(const FramedProblem& p, const void* packed) {
   if (p.hop <= 0 || p.K < 16) return false;
   // (pre-split planes are laid out by the caller, which guarantees >= 1 valid frame)
   if (p.presplit == nullptr && p.L + 2 * (int64_t)p.pad < p.K) return false;
   const SplitGeom g = split_geom(p.B > 0 ? p.B : 1, p.L, p.K, p.hop, p.pad);
   if (g.rows >= (1ll << 31) || g.plane_stride >= (1ll << 38)) return false;
+  // a block-partial basis runs on framed_tcb_kernel, whose nb-wide N tiles tc_block_shape_ok bounds (35 at
+  // n_fft = 32768); the dense kernel's N-tile limit below would send n_fft = 24576 and 32768 to the SIMT kernel
+  if (packed != nullptr && packed_kind(packed) == PACK_BLOCK) return tc_block_shape_ok(p.K, p.hop);
   const int bn = choose_bn(p.F);
   if ((2 * p.F + bn - 1) / bn > TC_MAX_N_TILES) return false;
   return true;
