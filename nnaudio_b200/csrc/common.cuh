@@ -220,8 +220,6 @@ int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_str
 int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
                   int K_a, int hop_a, int pad_a, int mode_a, void* planes_a,
                   int K_b, int hop_b, int pad_b, int mode_b, void* planes_b, cudaStream_t stream);
-int tc_zero_margins(void* planes, int64_t B, int64_t L, int K, int hop, int pad, int64_t keep_lo,
-                    int64_t keep_hi, cudaStream_t stream);
 // inverse STFT pieces (tc_kernels.cu)
 int tc_istft_k(int f_in);
 int tc_istft_bn(int n_fft);

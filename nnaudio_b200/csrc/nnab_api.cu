@@ -1215,13 +1215,12 @@ static int pyramid_fused(const PyramidCall& c, const PyrLevel* lv, size_t pf_ear
     // parts of the destination buffers the epilogue never writes
     if (dst.pc != SIZE_MAX) {
       const bool refl = dst.mode == NNAB_PAD_REFLECT;
-      rc = tc_zero_margins(ws + dst.pc, B, dst.len, dst.width, dst.hop, dst.pad,
-                           refl ? 0 : dst.pad, refl ? dst.len + 2 * dst.pad : dst.pad + dst.len, s);
+      rc = tc_zero_slots(ws + dst.pc, B, dst.pc_pitch, dst.pc_plane, refl ? 0 : dst.pad,
+                         refl ? dst.len + 2 * dst.pad : dst.pad + dst.len, s);
       if (rc) return rc;
     }
     if (dst.pf != SIZE_MAX) {
-      rc = tc_zero_margins(ws + dst.pf, B, dst.len, tc_fir_k(FIR_TAPS, 2), 256, FIR_OFF, FIR_OFF,
-                           FIR_OFF + dst.len, s);
+      rc = tc_zero_slots(ws + dst.pf, B, dst.pf_pitch, dst.pf_plane, FIR_OFF, FIR_OFF + dst.len, s);
       if (rc) return rc;
     }
     return run_framed(fir1_problem(c, src, src_len, dec, dst), fir_packed, nullptr, 0, NNAB_PATH_TCGEN05, s);

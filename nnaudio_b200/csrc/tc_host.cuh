@@ -1,8 +1,9 @@
-// Host-side pieces shared by the tensor-core translation units (tc_kernels.cu, tcb_kernels.cu).
+// Host-side pieces shared by the tensor-core translation units (tc_kernels.cu, tcb_kernels.cu, tct_kernels.cu).
 #pragma once
 
 #include <cuda.h>
 #include <stdint.h>
+#include <atomic>
 
 #include "common.cuh"
 
@@ -12,6 +13,32 @@ constexpr int TC_BM = 128;
 constexpr int TC_THREADS = 256;
 
 static inline int round_up_i(int v, int a) { return (v + a - 1) / a * a; }
+
+// Launches the persistent tensor-core kernel K.  Its dynamic shared-memory limit (smem_limit bytes) is set
+// first, once per device: the attribute is per device, and one process may drive several GPUs
+// (torch.nn.DataParallel).  Devices are tracked in a 64-bit mask indexed by device & 63.
+template <auto K, typename... Args>
+int launch_persistent(int grid, int threads, size_t smem, size_t smem_limit, cudaStream_t stream,
+                      const Args&... args) {
+  static std::atomic<uint64_t> configured_devs{0};
+  int dev = 0;
+  NNAB_CUDA_TRY(cudaGetDevice(&dev));
+  if (!((configured_devs.load(std::memory_order_relaxed) >> (dev & 63)) & 1u)) {
+    NNAB_CUDA_TRY(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit));
+    configured_devs.fetch_or(1ull << (dev & 63), std::memory_order_relaxed);
+  }
+  K<<<grid, threads, smem, stream>>>(args...);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+// SMs a persistent launch may use: the device's, less those kept for a concurrent collective
+// (nnab_set_sm_reserve), at least 1
+int usable_sms(int* sms);
+
+// the epilogue parameters of problem q (no split-K scratch: raw = nullptr)
+struct EpiParams;
+EpiParams epilogue_of(const FramedProblem& q);
 
 // geometry of the split / padded signal workspace (tc_kernels.cu)
 struct SplitGeom {
@@ -33,10 +60,11 @@ size_t tc_packed_bytes(int F, int K);
 int tc_pack_basis_varn(const float* w_re, const float* w_im, int F, int K, void* packed,
                        cudaStream_t stream);
 
-// layout of a packed basis, keyed by its device pointer
+// layout of a packed basis, keyed by its device pointer: the kind, and for PACK_BLOCK the (n_fft, hop) of the
+// transform it was packed for.  Marking an address PACK_DENSE drops its entry.
 enum { PACK_DENSE = 0, PACK_VARN = 2, PACK_BLOCK = 4 };
-int packed_kind(const void* packed);
-void mark_packed(const void* packed, int kind);
+int packed_kind(const void* packed, int* n_fft = nullptr, int* hop = nullptr);
+void mark_packed(const void* packed, int kind, int n_fft = 0, int hop = 0);
 
 // block-partial ("sliding") STFT kernel (tcb_kernels.cu)
 int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream);

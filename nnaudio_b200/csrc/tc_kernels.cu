@@ -18,7 +18,6 @@
 //                reference's (B, F, T[,2]) layout
 //     warp 8     TMA producer (full/empty mbarrier ring)
 #include <cuda.h>
-#include <atomic>
 #include <mutex>
 #include <unordered_map>
 #include <algorithm>
@@ -191,22 +190,6 @@ __global__ void __launch_bounds__(256) pad_split_kernel(
   *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
-// pad_split_kernel on the waveform's sample type (NNAB_DTYPE_*)
-static int launch_pad_split(dim3 grid, cudaStream_t stream, const void* x, int x_dtype, int64_t L,
-                            int64_t x_pitch, int pad, int pad_mode, int shift, int64_t clip_pitch,
-                            int64_t plane_stride, __nv_bfloat16* planes, int poly_hop = 0) {
-  auto launch = [&](auto* xs) {
-    pad_split_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad, pad_mode, shift, clip_pitch, plane_stride,
-                                               poly_hop, planes);
-  };
-  if (x_dtype == NNAB_DTYPE_F32) launch(static_cast<const float*>(x));
-  else if (x_dtype == NNAB_DTYPE_BF16) launch(static_cast<const __nv_bfloat16*>(x));
-  else if (x_dtype == NNAB_DTYPE_F16) launch(static_cast<const __half*>(x));
-  else return NNAB_EINVAL;
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
-}
-
 // pad_split_kernel on a push's virtual clip (ChunkSource): each sample is taken from the fp32 carry ring or
 // the chunk, with the reflect / constant centre padding of the whole stream at its two ends.  The planes of
 // frame t0 + j are then those the whole-clip pre-pass writes for frame t0 + j.
@@ -258,53 +241,31 @@ __global__ void __launch_bounds__(256) chunk_carry_kernel(ChunkSource c, const T
       sample_f32(__ldg(chunk + b * c.chunk_pitch + (r - c.received)));
 }
 
+// The one sample-type dispatch (NNAB_DTYPE_*): f(samples) launches one kernel on x as fp32, bf16 or fp16
+// samples, and the launch is checked.  (The deduced return type instantiates each call's kernels where the call
+// stands, which keeps the module's kernel order.)
 template <typename F>
-static int with_sample_type(int x_dtype, const void* x, F&& f) {
+static auto with_sample_type(int x_dtype, const void* x, F&& f) {
   if (x_dtype == NNAB_DTYPE_F32) f(static_cast<const float*>(x));
   else if (x_dtype == NNAB_DTYPE_BF16) f(static_cast<const __nv_bfloat16*>(x));
   else if (x_dtype == NNAB_DTYPE_F16) f(static_cast<const __half*>(x));
   else return NNAB_EINVAL;
+  NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
+
+static int launch_chunk_split(const ChunkSource& cs, int x_dtype, dim3 grid, int shift, int64_t clip_pitch,
+                              int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream);
 
 // The pre-pass of every tensor-core launcher: the planes of q's signal, shifted by `shift` samples.
 static int launch_problem_split(const FramedProblem& q, dim3 grid, int shift, int64_t clip_pitch,
                                 int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream) {
   if (q.chunk == nullptr)
-    return launch_pad_split(grid, stream, q.x, q.x_dtype, q.L, q.x_pitch, q.pad, q.pad_mode, shift, clip_pitch,
-                            plane_stride, planes, poly_hop);
-  const int rc = with_sample_type(q.x_dtype, q.chunk->chunk, [&](auto* xs) {
-    chunk_split_kernel<<<grid, 256, 0, stream>>>(*q.chunk, xs, shift, clip_pitch, plane_stride, poly_hop, planes);
-  });
-  if (rc) return rc;
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
-}
-
-int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_pitch, int64_t plane_stride,
-                   void* planes, cudaStream_t stream) {
-  if (B <= 0 || clip_pitch <= 0) return NNAB_OK;
-  if (B > 65535 || clip_pitch % 8 != 0) return NNAB_EUNSUPPORTED;
-  const dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
-  const int rc = with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
-    chunk_split_kernel<<<grid, 256, 0, stream>>>(cs, xs, 0, clip_pitch, plane_stride, 0,
-                                                 static_cast<__nv_bfloat16*>(planes));
-  });
-  if (rc) return rc;
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
-}
-
-int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream) {
-  if (from >= cs.total || B <= 0) return NNAB_OK;
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  const dim3 grid((unsigned)ceil_div64(cs.total - from, 256), (unsigned)B);
-  const int rc = with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
-    chunk_carry_kernel<<<grid, 256, 0, stream>>>(cs, xs, from);
-  });
-  if (rc) return rc;
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+    return with_sample_type(q.x_dtype, q.x, [&](auto* xs) {
+      pad_split_kernel<<<grid, 256, 0, stream>>>(xs, q.L, q.x_pitch, q.pad, q.pad_mode, shift, clip_pitch,
+                                                 plane_stride, poly_hop, planes);
+    });
+  return launch_chunk_split(*q.chunk, q.x_dtype, grid, shift, clip_pitch, plane_stride, poly_hop, planes, stream);
 }
 
 // Two differently padded split copies of the same batch in one pass over x (level 0 of
@@ -365,7 +326,7 @@ __global__ void __launch_bounds__(256) pack_basis_kernel(
   *reinterpret_cast<uint4*>(packed + (int64_t)rows * kpad + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
-void tc_forget_packed(const void* packed);
+static void tc_forget_packed(const void* packed) { mark_packed(packed, PACK_DENSE); }
 bool tc_varn_basis_ok(int F, int K);
 int tc_pack_basis_varn(const float* w_re, const float* w_im, int F, int K, void* packed,
                        cudaStream_t stream);
@@ -419,7 +380,7 @@ __global__ void __launch_bounds__(256) pack_fir_kernel(const float* __restrict__
 }
 
 int tc_pack_fir(const float* fir, int taps, int dec, void* packed, cudaStream_t stream) {
-  tc_forget_packed(packed);  // dense rows: drop any stale layout tag of a recycled address
+  tc_forget_packed(packed);  // dense rows: drop any stale layout entry of a recycled address
   const int kpad = tc_fir_k(taps, dec);
   pack_fir_kernel<<<(128 * kpad + 255) / 256, 256, 0, stream>>>(fir, taps, dec, kpad,
                                                                (__nv_bfloat16*)packed);
@@ -435,11 +396,13 @@ void tc_split_geometry(int64_t B, int64_t L, int K, int hop, int pad, int64_t* t
   if (hop_eff) *hop_eff = hop * num_phases(hop);
 }
 
-static int zero_tail(__nv_bfloat16* planes, const SplitGeom& g, int hop_eff, cudaStream_t stream) {
-  const int64_t tail = g.plane_stride - g.nv * hop_eff;
-  for (int pl = 0; pl < 2; ++pl)
-    NNAB_CUDA_TRY(cudaMemsetAsync(planes + pl * g.plane_stride + g.nv * hop_eff, 0,
-                                  (size_t)tail * sizeof(__nv_bfloat16), stream));
+// Zero [used, plane_stride) of both planes: the K-overhang rows past the last clip slot, which TMA reads and the
+// basis multiplies by its zero padding (they must hold finite values).
+static int zero_tail(__nv_bfloat16* planes, int64_t used, int64_t plane_stride, cudaStream_t stream) {
+  const int64_t tail = plane_stride - used;
+  for (int pl = 0; pl < 2 && tail > 0; ++pl)
+    NNAB_CUDA_TRY(cudaMemsetAsync(planes + pl * plane_stride + used, 0, (size_t)tail * sizeof(__nv_bfloat16),
+                                  stream));
   return NNAB_OK;
 }
 
@@ -450,9 +413,9 @@ int tc_problem_split(const FramedProblem& q, void* planes_v, cudaStream_t stream
   const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
   const int hop_eff = q.hop * num_phases(q.hop);
   __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
-  int rc = zero_tail(planes, g, hop_eff, stream);
-  if (rc) return rc;
   const int64_t clip_pitch = g.t_slots * hop_eff;
+  int rc = zero_tail(planes, q.B * clip_pitch, g.plane_stride, stream);
+  if (rc) return rc;
   dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
   return launch_problem_split(q, grid, 0, clip_pitch, g.plane_stride, layout == TC_SPLIT_POLY4 ? q.hop : 0,
                               planes, stream);
@@ -466,9 +429,6 @@ int tc_pad_split(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pit
   return tc_problem_split(q, planes_v, stream, TC_SPLIT_PLAIN);
 }
 
-__global__ void zero_margins_kernel(__nv_bfloat16* __restrict__ planes, int64_t plane_stride,
-                                    int64_t pitch, int64_t keep_lo, int64_t keep_hi);
-
 // pad + split into caller-defined geometry (clip pitch / plane stride in elements).  pad_split_kernel
 // writes the whole [0, clip_pitch) slot of every clip (zeros past the padded signal); the tail
 // [B * clip_pitch, plane_stride) is zeroed here.
@@ -477,60 +437,33 @@ int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_
   if (B > 65535) return NNAB_EUNSUPPORTED;
   if (clip_pitch % 8 != 0 || plane_stride < B * clip_pitch) return NNAB_EINVAL;
   __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
-  const int64_t tail = plane_stride - B * clip_pitch;
-  for (int pl = 0; pl < 2 && tail > 0; ++pl)
-    NNAB_CUDA_TRY(cudaMemsetAsync(planes + pl * plane_stride + B * clip_pitch, 0,
-                                  (size_t)tail * sizeof(__nv_bfloat16), stream));
+  const int rc = zero_tail(planes, B * clip_pitch, plane_stride, stream);
+  if (rc) return rc;
   dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
-  return launch_pad_split(grid, stream, x, x_dtype, L, x_pitch, pad, pad_mode, 0, clip_pitch, plane_stride,
-                          planes);
-}
-
-// zero [keep_hi, clip_pitch) and [0, keep_lo) of every clip slot (both planes) + the tail of the planes
-int tc_zero_slots(void* planes_v, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
-                  int64_t keep_hi, cudaStream_t stream) {
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
-  const int64_t tail = plane_stride - B * clip_pitch;
-  for (int pl = 0; pl < 2 && tail > 0; ++pl)
-    NNAB_CUDA_TRY(cudaMemsetAsync(planes + pl * plane_stride + B * clip_pitch, 0,
-                                  (size_t)tail * sizeof(__nv_bfloat16), stream));
-  if (keep_hi > clip_pitch) keep_hi = clip_pitch;
-  if (keep_lo < 0) keep_lo = 0;
-  const int64_t n = keep_lo + (clip_pitch - keep_hi);
-  if (n <= 0) return NNAB_OK;
-  int gx = (int)ceil_div64(n, 256);
-  if (gx > 64) gx = 64;
-  zero_margins_kernel<<<dim3(gx, (unsigned)B), 256, 0, stream>>>(planes, plane_stride, clip_pitch,
-                                                                keep_lo, keep_hi);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  return with_sample_type(x_dtype, x, [&](auto* xs) {
+    pad_split_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad, pad_mode, 0, clip_pitch, plane_stride, 0,
+                                               planes);
+  });
 }
 
 int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
                   int K_a, int hop_a, int pad_a, int mode_a, void* planes_a,
                   int K_b, int hop_b, int pad_b, int mode_b, void* planes_b, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
-  if (x_dtype != NNAB_DTYPE_F32 && x_dtype != NNAB_DTYPE_BF16 && x_dtype != NNAB_DTYPE_F16) return NNAB_EINVAL;
   const SplitGeom ga = split_geom(B, L, K_a, hop_a, pad_a);
   const SplitGeom gb = split_geom(B, L, K_b, hop_b, pad_b);
-  const int he_a = hop_a * num_phases(hop_a), he_b = hop_b * num_phases(hop_b);
-  int rc = zero_tail((__nv_bfloat16*)planes_a, ga, he_a, stream);
-  if (rc) return rc;
-  if ((rc = zero_tail((__nv_bfloat16*)planes_b, gb, he_b, stream))) return rc;
-  const int64_t pitch_a = ga.t_slots * he_a, pitch_b = gb.t_slots * he_b;
+  const int64_t pitch_a = ga.t_slots * hop_a * num_phases(hop_a), pitch_b = gb.t_slots * hop_b * num_phases(hop_b);
   const int64_t pmax = pitch_a > pitch_b ? pitch_a : pitch_b;
   dim3 grid((unsigned)ceil_div64(pmax, 256 * 8), (unsigned)B);
-  auto launch = [&](auto* xs) {
+  // the kernel writes the clip slots, [0, B * pitch) of each plane set; the tails past them are zeroed after
+  int rc = with_sample_type(x_dtype, x, [&](auto* xs) {
     pad_split2_kernel<<<grid, 256, 0, stream>>>(xs, L, x_pitch, pad_a, mode_a, pitch_a, ga.plane_stride,
                                                 (__nv_bfloat16*)planes_a, pad_b, mode_b, pitch_b,
                                                 gb.plane_stride, (__nv_bfloat16*)planes_b);
-  };
-  if (x_dtype == NNAB_DTYPE_F32) launch(static_cast<const float*>(x));
-  else if (x_dtype == NNAB_DTYPE_BF16) launch(static_cast<const __nv_bfloat16*>(x));
-  else launch(static_cast<const __half*>(x));
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  });
+  if (rc) return rc;
+  if ((rc = zero_tail((__nv_bfloat16*)planes_a, B * pitch_a, ga.plane_stride, stream))) return rc;
+  return zero_tail((__nv_bfloat16*)planes_b, B * pitch_b, gb.plane_stride, stream);
 }
 
 // Zero every element of each clip's slot region outside [keep_lo, keep_hi) (both planes)
@@ -550,22 +483,20 @@ __global__ void __launch_bounds__(256) zero_margins_kernel(__nv_bfloat16* __rest
   }
 }
 
-int tc_zero_margins(void* planes_v, int64_t B, int64_t L, int K, int hop, int pad, int64_t keep_lo,
-                    int64_t keep_hi, cudaStream_t stream) {
+// zero [keep_hi, clip_pitch) and [0, keep_lo) of every clip slot (both planes) + the tail of the planes
+int tc_zero_slots(void* planes_v, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
+                  int64_t keep_hi, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
-  const SplitGeom g = split_geom(B, L, K, hop, pad);
-  const int hop_eff = hop * num_phases(hop);
   __nv_bfloat16* planes = (__nv_bfloat16*)planes_v;
-  int rc = zero_tail(planes, g, hop_eff, stream);
+  const int rc = zero_tail(planes, B * clip_pitch, plane_stride, stream);
   if (rc) return rc;
-  const int64_t pitch = g.t_slots * hop_eff;
-  if (keep_hi > pitch) keep_hi = pitch;
+  if (keep_hi > clip_pitch) keep_hi = clip_pitch;
   if (keep_lo < 0) keep_lo = 0;
-  const int64_t n = keep_lo + (pitch - keep_hi);
+  const int64_t n = keep_lo + (clip_pitch - keep_hi);
   if (n <= 0) return NNAB_OK;
   int gx = (int)ceil_div64(n, 256);
   if (gx > 64) gx = 64;
-  zero_margins_kernel<<<dim3(gx, (unsigned)B), 256, 0, stream>>>(planes, g.plane_stride, pitch,
+  zero_margins_kernel<<<dim3(gx, (unsigned)B), 256, 0, stream>>>(planes, plane_stride, clip_pitch,
                                                                 keep_lo, keep_hi);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
@@ -682,7 +613,7 @@ int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes_v
   if (kpad != 2 * f_in) {
     NNAB_CUDA_TRY(cudaMemsetAsync(planes, 0, (size_t)2 * g.plane_stride * sizeof(__nv_bfloat16), stream));
   } else {
-    const int rc = zero_tail(planes, g, kpad, stream);
+    const int rc = zero_tail(planes, g.nv * kpad, g.plane_stride, stream);
     if (rc) return rc;
   }
   dim3 grid((unsigned)ceil_div64(T, 32), (unsigned)((f_in + 31) / 32), (unsigned)B);
@@ -1404,6 +1335,34 @@ size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K) {
 }
 
 // ---------------------------------------------------------------------------
+// pre-pass of a streamed push (chunk_split_kernel, chunk_carry_kernel)
+// ---------------------------------------------------------------------------
+static int launch_chunk_split(const ChunkSource& cs, int x_dtype, dim3 grid, int shift, int64_t clip_pitch,
+                              int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream) {
+  return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    chunk_split_kernel<<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop, planes);
+  });
+}
+
+int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_pitch, int64_t plane_stride,
+                   void* planes, cudaStream_t stream) {
+  if (B <= 0 || clip_pitch <= 0) return NNAB_OK;
+  if (B > 65535 || clip_pitch % 8 != 0) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)B);
+  return launch_chunk_split(cs, x_dtype, grid, 0, clip_pitch, plane_stride, 0, static_cast<__nv_bfloat16*>(planes),
+                            stream);
+}
+
+int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream) {
+  if (from >= cs.total || B <= 0) return NNAB_OK;
+  if (B > 65535) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(cs.total - from, 256), (unsigned)B);
+  return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    chunk_carry_kernel<<<grid, 256, 0, stream>>>(cs, xs, from);
+  });
+}
+
+// ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -1481,23 +1440,32 @@ int encode_4d(CUtensorMap* map, void* base, const uint64_t dims[4], const uint64
   return NNAB_OK;
 }
 
+int usable_sms(int* sms) {
+  int dev = 0;
+  NNAB_CUDA_TRY(cudaGetDevice(&dev));
+  NNAB_CUDA_TRY(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  *sms -= sm_reserve();
+  if (*sms < 1) *sms = 1;
+  return NNAB_OK;
+}
+
+EpiParams epilogue_of(const FramedProblem& q) {
+  EpiParams e{};
+  e.scale = q.scale; e.scale_all = q.scale_all; e.fmt = q.fmt;
+  e.eps = q.eps; e.power = q.power; e.out = q.out; e.T = q.T;
+  e.out_bins = q.out_bins; e.bin_offset = q.bin_offset; e.F = q.F;
+  e.fb_table = q.fb_table; e.fb_steps = q.fb_steps; e.n_fb = q.n_fb;
+  e.dec = q.dec;
+  e.ola_pitch = q.ola_pitch; e.ola_hop = q.ola_hop;
+  e.planes_stride = q.planes_stride; e.planes_pitch = q.planes_pitch;
+  return e;
+}
+
 template <int FMT>
 static int launch_tc_kernel_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
                                 int grid, cudaStream_t stream) {
-  using S = TcSmem;
-  // the attribute is per device: one process may drive several GPUs (torch.nn.DataParallel)
-  static std::atomic<uint64_t> configured_devs{0};
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  const bool configured = (configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u;
-  if (!configured) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tc_kernel<FMT>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
-  }
-  framed_tc_kernel<FMT><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb, prm);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  return launch_persistent<framed_tc_kernel<FMT>>(grid, TC_KERNEL_THREADS, TcSmem::TOTAL, TcSmem::TOTAL, stream,
+                                                  ma, mb, prm);
 }
 
 static int launch_tc_kernel(const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& prm,
@@ -1520,25 +1488,27 @@ static int launch_tc_kernel(const CUtensorMap& ma, const CUtensorMap& mb, const 
 
 // ---------------------------------------------------------------------------
 // layout of a packed basis, keyed by its device pointer.  Every function that produces a buffer for the
-// `packed` argument of launch_framed_tc sets (or clears) the tag, so a recycled address cannot carry a
+// `packed` argument of launch_framed_tc sets (or clears) the entry, so a recycled address cannot carry a
 // stale layout.
 // ---------------------------------------------------------------------------
+struct PackedLayout { int kind, n_fft, hop; };
 static std::mutex g_pack_mu;
-static std::unordered_map<const void*, int> g_pack_kind;
+static std::unordered_map<const void*, PackedLayout> g_packed;
 
-int packed_kind(const void* packed) {
+int packed_kind(const void* packed, int* n_fft, int* hop) {
   std::lock_guard<std::mutex> lk(g_pack_mu);
-  auto it = g_pack_kind.find(packed);
-  return it == g_pack_kind.end() ? PACK_DENSE : it->second;
+  auto it = g_packed.find(packed);
+  const PackedLayout l = it == g_packed.end() ? PackedLayout{PACK_DENSE, 0, 0} : it->second;
+  if (n_fft) *n_fft = l.n_fft;
+  if (hop) *hop = l.hop;
+  return l.kind;
 }
 
-void mark_packed(const void* packed, int kind) {
+void mark_packed(const void* packed, int kind, int n_fft, int hop) {
   std::lock_guard<std::mutex> lk(g_pack_mu);
-  if (kind == PACK_DENSE) g_pack_kind.erase(packed);
-  else g_pack_kind[packed] = kind;
+  if (kind == PACK_DENSE) g_packed.erase(packed);
+  else g_packed[packed] = PackedLayout{kind, n_fft, hop};
 }
-
-void tc_forget_packed(const void* packed) { mark_packed(packed, PACK_DENSE); }
 
 
 // ---------------------------------------------------------------------------
@@ -1626,18 +1596,82 @@ static bool varn_problem_ok(const FramedProblem& q) {
 template <int FMT>
 static int launch_tcv_fmt(const CUtensorMap& ma, const CUtensorMap& mb8, const CUtensorMap& mb32,
                           const TcParams& prm, const VarNPlan& plan, int grid, cudaStream_t stream) {
-  using S = TcSmem;
-  // the attribute is per device: one process may drive several GPUs (torch.nn.DataParallel)
-  static std::atomic<uint64_t> configured_devs{0};
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  const bool configured = (configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u;
-  if (!configured) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcv_kernel<FMT>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
+  return launch_persistent<framed_tcv_kernel<FMT>>(grid, TC_KERNEL_THREADS, TcSmem::TOTAL, TcSmem::TOTAL, stream,
+                                                   ma, mb8, mb32, prm, plan);
+}
+
+// The front half of the dense and VarN launchers: q's split-signal planes (the caller's pre-split planes, or the
+// workspace with its K-overhang tail zeroed), their A-operand map and the SMs of the launch.  split_phase then
+// writes the planes of each frame phase.
+struct FramedSignal {
+  SplitGeom g;
+  int n_ph, hop_eff;
+  int rows_mode;  // 1: A viewed as a (rows x hop_eff) matrix (64 | hop_eff); 0: overlapping-stride map
+  __nv_bfloat16* planes;
+  int sms;
+  CUtensorMap ma;
+};
+
+static int framed_signal(const FramedProblem& q, void* workspace, size_t ws_bytes, cudaStream_t stream,
+                         FramedSignal* s) {
+  if (q.presplit == nullptr) {
+    const size_t need = tc_workspace_bytes(q.B, q.L, q.K, q.hop, q.pad);
+    if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
+  } else if (num_phases(q.hop) != 1) {
+    return NNAB_EALIGN;  // pre-split planes exist for one frame phase only
   }
-  framed_tcv_kernel<FMT><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb8, mb32, prm, plan);
+  if (q.B > 65535) return NNAB_EUNSUPPORTED;
+  s->n_ph = num_phases(q.hop);
+  s->hop_eff = q.hop * s->n_ph;
+  SplitGeom& g = s->g;
+  g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
+  if (q.presplit != nullptr && q.presplit_t_slots > 0) {
+    // caller-defined plane geometry (pyramid levels shared with the FIR stage): frame g of the batch
+    // still starts at element g * hop, with presplit_t_slots frames per clip slot
+    g.t_slots = q.presplit_t_slots;
+    g.nv = q.B * g.t_slots;
+    g.plane_stride = q.presplit_plane_stride;
+    g.rows = g.plane_stride / s->hop_eff;
+    if (g.rows < g.nv) return NNAB_EINVAL;
+  }
+  int rc;
+  if (q.presplit != nullptr) {
+    s->planes = reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(q.presplit));
+  } else {
+    s->planes = reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+    if ((rc = zero_tail(s->planes, g.nv * s->hop_eff, g.plane_stride, stream))) return rc;
+  }
+  if ((rc = usable_sms(&s->sms))) return rc;
+  s->rows_mode = (s->hop_eff % 64 == 0) ? 1 : 0;
+  if (s->rows_mode)
+    return encode_3d(&s->ma, s->planes, (uint64_t)s->hop_eff, (uint64_t)g.rows, 2, (uint64_t)s->hop_eff * 2,
+                     (uint64_t)g.plane_stride * 2, 64, TC_BM, 64);
+  // overlapping rows: row g starts at element g * hop_eff and is kpad long
+  return encode_3d(&s->ma, s->planes, (uint64_t)round_up_i(q.K, 64), (uint64_t)g.nv, 2, (uint64_t)s->hop_eff * 2,
+                   (uint64_t)g.plane_stride * 2, 64, TC_BM, 64);
+}
+
+// the planes of frame phase ph: the signal shifted by ph * hop samples (pre-split planes are the caller's)
+static int split_phase(const FramedProblem& q, const FramedSignal& s, int ph, cudaStream_t stream) {
+  if (q.presplit != nullptr) return NNAB_OK;
+  const int64_t clip_pitch = s.g.t_slots * s.hop_eff;
+  dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
+  return launch_problem_split(q, grid, ph * q.hop, clip_pitch, s.g.plane_stride, 0, s.planes, stream);
+}
+
+// Split-K (long kernels, with the caller's raw scratch): the kernel writes raw (re, im) partial sums to the
+// scratch, and splitk_finalize_kernel then applies the returned epilogue to them.
+static EpiParams use_splitk_scratch(const FramedProblem& q, EpiParams* e) {
+  e->raw = reinterpret_cast<float*>(((uintptr_t)q.raw + 255) & ~(uintptr_t)255);
+  e->raw_plane = (int64_t)q.B * q.F * q.T;
+  const EpiParams final_epi = *e;
+  e->fmt = FMT_RAW;
+  return final_epi;
+}
+
+static int launch_splitk_finalize(const EpiParams& e, int64_t B, cudaStream_t stream) {
+  dim3 grid((unsigned)ceil_div64(e.T, 256), (unsigned)e.F, (unsigned)(B < 64 ? B : 64));
+  splitk_finalize_kernel<<<grid, 256, 0, stream>>>(e, B);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -1650,19 +1684,12 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
     const int trc = launch_framed_tc_tall(q, packed, workspace, ws_bytes, stream);
     if (trc != NNAB_EUNSUPPORTED) return trc;
   }
-  const size_t need = tc_workspace_bytes(q.B, q.L, q.K, q.hop, q.pad);
-  if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
-  if (q.B > 65535) return NNAB_EUNSUPPORTED;
-  const SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
+  FramedSignal s;
+  int rc = framed_signal(q, workspace, ws_bytes, stream, &s);
+  if (rc) return rc;
+  if ((rc = split_phase(q, s, 0, stream))) return rc;  // one frame phase (varn_problem_ok)
   const int kpad = round_up_i(q.K, 64);
   const int rows_w = 16 * ((q.F + 7) / 8);
-  __nv_bfloat16* planes =
-      reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  int rc = zero_tail(planes, g, q.hop, stream);
-  if (rc) return rc;
-  const int64_t clip_pitch = g.t_slots * q.hop;
-  dim3 pgrid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-  if ((rc = launch_problem_split(q, pgrid, 0, clip_pitch, g.plane_stride, 0, planes, stream))) return rc;
 
   // split-K only with the caller's raw scratch (long kernels): <= 64 K blocks per accumulator
   VarNPlan plan;
@@ -1677,21 +1704,7 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
     if ((rc = tc_varn_plan(q.h_k_begin, q.h_k_end, q.F, q.K, ks, &plan))) return rc;
   }
 
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();
-  if (sms < 1) sms = 1;
-
-  CUtensorMap ma, mb8, mb32;
-  const int rows_mode = (q.hop % 64 == 0) ? 1 : 0;
-  if (rows_mode)
-    rc = encode_3d(&ma, planes, (uint64_t)q.hop, (uint64_t)g.rows, 2, (uint64_t)q.hop * 2,
-                   (uint64_t)g.plane_stride * 2, 64, TC_BM, 64);
-  else
-    rc = encode_3d(&ma, planes, (uint64_t)kpad, (uint64_t)g.nv, 2, (uint64_t)q.hop * 2,
-                   (uint64_t)g.plane_stride * 2, 64, TC_BM, 64);
-  if (rc) return rc;
+  CUtensorMap mb8, mb32;
   if ((rc = encode_3d(&mb8, const_cast<void*>(packed), (uint64_t)kpad, (uint64_t)rows_w, 2,
                       (uint64_t)kpad * 2, (uint64_t)rows_w * kpad * 2, 64, 8, 64)))
     return rc;
@@ -1702,133 +1715,68 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
   TcParams prm{};
   prm.num_n_tiles = 1;
   prm.bn = rows_w;
-  prm.rows_mode = rows_mode;
-  prm.hop = q.hop;
-  prm.nv = g.nv;
-  prm.t_slots = g.t_slots;
+  prm.rows_mode = s.rows_mode;
+  prm.hop = s.hop_eff;
+  prm.nv = s.g.nv;
+  prm.t_slots = s.g.t_slots;
   prm.t_mul = 1;
   prm.t_add = 0;
   prm.T = q.T;
   prm.k_splits = plan.n_chunks;
-  prm.epi.scale = q.scale; prm.epi.scale_all = q.scale_all; prm.epi.fmt = q.fmt;
-  prm.epi.eps = q.eps; prm.epi.power = q.power; prm.epi.out = q.out; prm.epi.T = q.T;
-  prm.epi.out_bins = q.out_bins; prm.epi.bin_offset = q.bin_offset; prm.epi.F = q.F;
-  prm.epi.fb_table = nullptr; prm.epi.n_fb = 0;
-  prm.epi.dec = q.dec;
-  prm.epi.raw = nullptr; prm.epi.raw_plane = 0;
-  prm.epi.ola_pitch = 0; prm.epi.ola_hop = 0;
-  EpiParams final_epi = prm.epi;
+  prm.epi = epilogue_of(q);
+  prm.epi.fb_table = nullptr;
   const bool split = plan.n_chunks > 1;
-  if (split) {
-    float* raw = reinterpret_cast<float*>(((uintptr_t)q.raw + 255) & ~(uintptr_t)255);
-    const int64_t plane = (int64_t)q.B * q.F * q.T;
-    prm.epi.fmt = FMT_RAW;
-    prm.epi.raw = raw;
-    prm.epi.raw_plane = plane;
-    final_epi.raw = raw;
-    final_epi.raw_plane = plane;
-  }
-  prm.num_m_tiles = (int)ceil_div64(g.nv, TC_BM);
+  const EpiParams final_epi = split ? use_splitk_scratch(q, &prm.epi) : prm.epi;
+  prm.num_m_tiles = (int)ceil_div64(s.g.nv, TC_BM);
   const int64_t units = (int64_t)prm.num_m_tiles * plan.n_chunks;
-  const int grid = (int)(units < sms ? units : sms);
+  const int grid = (int)(units < s.sms ? units : s.sms);
   {
     double cols = 0.0;
     for (int i = 0; i < plan.n_blocks; ++i) cols += 16.0 * plan.groups[i] * 64.0;
     add_exec_flops(3.0 * 2.0 * (double)prm.num_m_tiles * TC_BM * cols);
   }
   switch (prm.epi.fmt) {
-    case NNAB_FMT_MAGNITUDE: rc = launch_tcv_fmt<0>(ma, mb8, mb32, prm, plan, grid, stream); break;
-    case NNAB_FMT_COMPLEX: rc = launch_tcv_fmt<1>(ma, mb8, mb32, prm, plan, grid, stream); break;
-    case NNAB_FMT_PHASE_UNIT: rc = launch_tcv_fmt<3>(ma, mb8, mb32, prm, plan, grid, stream); break;
-    case FMT_RAW: rc = launch_tcv_fmt<7>(ma, mb8, mb32, prm, plan, grid, stream); break;
+    case NNAB_FMT_MAGNITUDE: rc = launch_tcv_fmt<0>(s.ma, mb8, mb32, prm, plan, grid, stream); break;
+    case NNAB_FMT_COMPLEX: rc = launch_tcv_fmt<1>(s.ma, mb8, mb32, prm, plan, grid, stream); break;
+    case NNAB_FMT_PHASE_UNIT: rc = launch_tcv_fmt<3>(s.ma, mb8, mb32, prm, plan, grid, stream); break;
+    case FMT_RAW: rc = launch_tcv_fmt<7>(s.ma, mb8, mb32, prm, plan, grid, stream); break;
     default: rc = NNAB_EINVAL;
   }
   if (rc) return rc;
-  if (split) {
-    dim3 grid((unsigned)ceil_div64(q.T, 256), (unsigned)q.F, (unsigned)(q.B < 64 ? q.B : 64));
-    splitk_finalize_kernel<<<grid, 256, 0, stream>>>(final_epi, q.B);
-    NNAB_LAUNCH_CHECK();
-  }
-  return NNAB_OK;
+  return split ? launch_splitk_finalize(final_epi, q.B, stream) : NNAB_OK;
 }
 
 int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace, size_t ws_bytes,
                      cudaStream_t stream) {
   if (q.B <= 0 || q.T <= 0 || q.F <= 0) return NNAB_OK;
   if (packed == nullptr) return NNAB_EINVAL;
-  if (packed_kind(packed) == PACK_BLOCK)
-    return launch_framed_tc_block(q, packed, workspace, ws_bytes, stream);
-  if (packed_kind(packed) == PACK_VARN)
-    return launch_framed_tc_varn(q, packed, workspace, ws_bytes, stream);
-  if (q.presplit == nullptr) {
-    const size_t need = tc_workspace_bytes(q.B, q.L, q.K, q.hop, q.pad);
-    if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
-  } else if (num_phases(q.hop) != 1) {
-    return NNAB_EALIGN;  // pre-split planes exist for one frame phase only
-  }
-  if (q.B > 65535) return NNAB_EUNSUPPORTED;
+  const int kind = packed_kind(packed);
+  if (kind == PACK_BLOCK) return launch_framed_tc_block(q, packed, workspace, ws_bytes, stream);
+  if (kind == PACK_VARN) return launch_framed_tc_varn(q, packed, workspace, ws_bytes, stream);
+  FramedSignal s;
+  int rc = framed_signal(q, workspace, ws_bytes, stream, &s);
+  if (rc) return rc;
 
   constexpr int bk = 64;
-
-  const int n_ph = num_phases(q.hop);
-  const int hop_eff = q.hop * n_ph;
-  SplitGeom g = split_geom(q.B, q.L, q.K, q.hop, q.pad);
-  if (q.presplit != nullptr && q.presplit_t_slots > 0) {
-    // caller-defined plane geometry (pyramid levels shared with the FIR stage): frame g of the batch
-    // still starts at element g * hop, with presplit_t_slots frames per clip slot
-    g.t_slots = q.presplit_t_slots;
-    g.nv = q.B * g.t_slots;
-    g.plane_stride = q.presplit_plane_stride;
-    g.rows = g.plane_stride / hop_eff;
-    if (g.rows < g.nv) return NNAB_EINVAL;
-  }
+  const int n_ph = s.n_ph;
   const int kpad = round_up_i(q.K, 64);
   // FMT_OLA: the N axis is the frame's n_fft output samples (q.F), not (re | im) bin pairs
   const int bn = (q.fmt == FMT_OLA) ? tc_istft_bn(q.F) : choose_bn(q.F);
   const int n_tiles = (q.fmt == FMT_OLA) ? (q.F + bn - 1) / bn : (2 * q.F + bn - 1) / bn;
   const int rows_w = n_tiles * bn;
-  __nv_bfloat16* planes =
-      q.presplit != nullptr
-          ? reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(q.presplit))
-          : reinterpret_cast<__nv_bfloat16*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-
-  // K overhang rows past the last clip must be finite zeros (the basis is zero-padded there)
-  const int64_t clip_pitch = g.t_slots * hop_eff;
-  if (q.presplit == nullptr) {
-    const int zrc = zero_tail(planes, g, hop_eff, stream);
-    if (zrc) return zrc;
-  }
-
-  // ---- tensor maps (shared by all phases) -------------------------------------------
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();  // SMs left to a concurrent collective (nnab_set_sm_reserve)
-  if (sms < 1) sms = 1;
-  CUtensorMap ma, mb;
-  const int rows_mode = (hop_eff % bk == 0) ? 1 : 0;
-  int rc;
-  if (rows_mode) {
-    rc = encode_3d(&ma, planes, (uint64_t)hop_eff, (uint64_t)g.rows, 2, (uint64_t)hop_eff * 2,
-                   (uint64_t)g.plane_stride * 2, bk, TC_BM, bk);
-  } else {
-    // overlapping rows: row g starts at element g*hop_eff and is kpad long
-    rc = encode_3d(&ma, planes, (uint64_t)kpad, (uint64_t)g.nv, 2, (uint64_t)hop_eff * 2,
-                   (uint64_t)g.plane_stride * 2, bk, TC_BM, bk);
-  }
-  if (rc) return rc;
+  CUtensorMap mb;
   rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, (uint64_t)rows_w, 2,
                  (uint64_t)kpad * 2, (uint64_t)rows_w * kpad * 2, bk, bn, bk);
   if (rc) return rc;
 
   // ---- parameters -------------------------------------------------------------------
-  TcParams prm;
+  TcParams prm{};
   prm.num_n_tiles = n_tiles;
   prm.bn = bn;
-  prm.rows_mode = rows_mode;
-  prm.hop = hop_eff;
-  prm.nv = g.nv;
-  prm.t_slots = g.t_slots;
+  prm.rows_mode = s.rows_mode;
+  prm.hop = s.hop_eff;
+  prm.nv = s.g.nv;
+  prm.t_slots = s.g.t_slots;
   prm.t_mul = n_ph;
   const int nkb = kpad / bk;
   const int half = bn / 2;
@@ -1854,13 +1802,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     prm.kb_begin[tl] = lo;
     prm.kb_end[tl] = hi;
   }
-  prm.epi.scale = q.scale; prm.epi.scale_all = q.scale_all; prm.epi.fmt = q.fmt;
-  prm.epi.eps = q.eps; prm.epi.power = q.power; prm.epi.out = q.out; prm.epi.T = q.T;
-  prm.epi.out_bins = q.out_bins; prm.epi.bin_offset = q.bin_offset; prm.epi.F = q.F;
-  prm.epi.fb_table = q.fb_table; prm.epi.n_fb = q.n_fb;
-  prm.epi.dec = q.dec;
-  prm.epi.raw = nullptr; prm.epi.raw_plane = 0;
-  prm.epi.ola_pitch = q.ola_pitch; prm.epi.ola_hop = q.ola_hop;
+  prm.epi = epilogue_of(q);
   prm.k_splits = 1;
   if (q.fmt == FMT_FBANK && (q.fb_table == nullptr || q.n_fb <= 0)) return NNAB_EINVAL;
   if (q.fmt == FMT_DECIM && (bn != 128 || n_tiles != 1)) return NNAB_EINVAL;
@@ -1892,13 +1834,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     if (ks > 1) {
       split = true;
       prm.k_splits = ks;
-      float* raw = reinterpret_cast<float*>(((uintptr_t)q.raw + 255) & ~(uintptr_t)255);
-      const int64_t plane = (int64_t)q.B * q.F * q.T;
-        prm.epi.fmt = FMT_RAW;
-      prm.epi.raw = raw;
-      prm.epi.raw_plane = plane;
-      final_epi.raw = raw;
-      final_epi.raw_plane = plane;
+      final_epi = use_splitk_scratch(q, &prm.epi);
     }
   }
 
@@ -1907,27 +1843,19 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     if (ph >= q.T) break;
     prm.t_add = ph;
     prm.T = (q.T - ph + n_ph - 1) / n_ph;  // frames t = ph, ph + n_ph, ... < T
-    if (q.presplit == nullptr) {
-      dim3 grid((unsigned)ceil_div64(clip_pitch, 256 * 8), (unsigned)q.B);
-      if ((rc = launch_problem_split(q, grid, ph * q.hop, clip_pitch, g.plane_stride, 0, planes, stream))) return rc;
-    }
+    if ((rc = split_phase(q, s, ph, stream))) return rc;
     {
       double kcols = 0.0;  // sum over N tiles of (k-blocks executed) x bk x bn
       for (int tl = 0; tl < n_tiles; ++tl) kcols += (double)(prm.kb_end[tl] - prm.kb_begin[tl]) * bk * bn;
-      add_exec_flops(3.0 * 2.0 * (double)ceil_div64(g.nv, TC_BM) * TC_BM * kcols);
+      add_exec_flops(3.0 * 2.0 * (double)ceil_div64(s.g.nv, TC_BM) * TC_BM * kcols);
     }
-    prm.num_m_tiles = (int)ceil_div64(g.nv, TC_BM);
+    prm.num_m_tiles = (int)ceil_div64(s.g.nv, TC_BM);
     const int64_t tiles = (int64_t)prm.num_m_tiles * prm.num_n_tiles * prm.k_splits;
-    const int grid = (int)(tiles < sms ? tiles : sms);
-    rc = launch_tc_kernel(ma, mb, prm, grid, stream);
+    const int grid = (int)(tiles < s.sms ? tiles : s.sms);
+    rc = launch_tc_kernel(s.ma, mb, prm, grid, stream);
     if (rc) return rc;
   }
-  if (split) {
-    dim3 grid((unsigned)ceil_div64(q.T, 256), (unsigned)q.F, (unsigned)(q.B < 64 ? q.B : 64));
-    splitk_finalize_kernel<<<grid, 256, 0, stream>>>(final_epi, q.B);
-    NNAB_LAUNCH_CHECK();
-  }
-  return NNAB_OK;
+  return split ? launch_splitk_finalize(final_epi, q.B, stream) : NNAB_OK;
 }
 
 }  // namespace nnab

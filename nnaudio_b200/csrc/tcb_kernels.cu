@@ -44,9 +44,6 @@
 // the epilogue above runs on each quarter with its family's bin origin and bin range.  33 - R frames per tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <atomic>
-#include <mutex>
-#include <unordered_map>
 
 #include "common.cuh"
 #include "epilogue.cuh"
@@ -198,10 +195,6 @@ __global__ void __launch_bounds__(256) pack_block_twiddle_kernel(int n_fft, int 
   tw[idx] = make_float2((float)cd, (float)(-sd));
 }
 
-struct BlockPack { int n_fft, hop; };
-static std::mutex g_blk_mu;
-static std::unordered_map<const void*, BlockPack> g_blk;
-
 int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
   if (!tc_block_shape_ok(n_fft, hop) || packed == nullptr) return NNAB_EINVAL;
   const bool poly = block_poly4(hop);
@@ -216,11 +209,7 @@ int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
         n_fft, p_rows, reinterpret_cast<float2*>((char*)packed + block_twiddle_offset(n_fft, hop)));
     NNAB_LAUNCH_CHECK();
   }
-  {
-    std::lock_guard<std::mutex> lk(g_blk_mu);
-    g_blk[packed] = BlockPack{n_fft, hop};
-  }
-  mark_packed(packed, PACK_BLOCK);
+  mark_packed(packed, PACK_BLOCK, n_fft, hop);
   return NNAB_OK;
 }
 
@@ -863,27 +852,14 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   // keep framed_tcb_kernel: their epilogue is shorter than the MMA warps' share of a tile, and with separate roles
   // Magnitude STFT-2048 measured 7 % slower, where the Mel, MFCC and Gammatone workloads run 3-5 % faster.
   constexpr bool WS = PH == 4 && (FMT == 5 || FMT == 9);
-  static std::atomic<uint64_t> configured_devs{0};  // the attributes are per device
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_kernel<FMT, R, PASSES, PH>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::LIMIT));
-    if constexpr (WS)
-      NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tcb_ws_kernel<FMT, R, PASSES>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::LIMIT));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
-  }
-  if constexpr (WS) {
-    if (prm.nb <= TCB_WS_NB_MAX) {
-      framed_tcb_ws_kernel<FMT, R, PASSES><<<grid, TCB_WS_THREADS, S::total(prm.nb, PASSES), stream>>>(ma, mb, prm);
-      NNAB_LAUNCH_CHECK();
-      return NNAB_OK;
-    }
-  }
-  framed_tcb_kernel<FMT, R, PASSES, PH><<<grid, TC_KERNEL_THREADS, S::total(prm.nb, PASSES), stream>>>(ma, mb, prm);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  const size_t smem = S::total(prm.nb, PASSES);
+  if (!WS || prm.nb > TCB_WS_NB_MAX)
+    return launch_persistent<framed_tcb_kernel<FMT, R, PASSES, PH>>(grid, TC_KERNEL_THREADS, smem, S::LIMIT, stream,
+                                                                    ma, mb, prm);
+  if constexpr (WS)
+    return launch_persistent<framed_tcb_ws_kernel<FMT, R, PASSES>>(grid, TCB_WS_THREADS, smem, S::LIMIT, stream,
+                                                                   ma, mb, prm);
+  return NNAB_EINVAL;  // (not reached)
 }
 
 template <int R, int PASSES, int PH>
@@ -912,15 +888,10 @@ static int launch_tcb_ph(int R, int passes, int fmt, const CUtensorMap& ma, cons
 
 int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* workspace,
                            size_t ws_bytes, cudaStream_t stream) {
-  BlockPack bp{};
-  {
-    std::lock_guard<std::mutex> lk(g_blk_mu);
-    auto it = g_blk.find(packed);
-    if (it == g_blk.end()) return NNAB_EINVAL;
-    bp = it->second;
-  }
+  int n_fft = 0, hop = 0;
+  if (packed_kind(packed, &n_fft, &hop) != PACK_BLOCK) return NNAB_EINVAL;
   // the basis was packed for exactly this transform: anything else is a caller bug
-  if (bp.n_fft != q.K || bp.hop != q.hop || q.F != q.K / 2 + 1) return NNAB_EINVAL;
+  if (n_fft != q.K || hop != q.hop || q.F != q.K / 2 + 1) return NNAB_EINVAL;
   if (q.presplit != nullptr || q.h_k_begin != nullptr || q.scale != nullptr || q.scale_all != 1.f)
     return NNAB_EINVAL;
   switch (q.fmt) {
@@ -953,11 +924,8 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   // a bf16 waveform has an all-zero lo plane: the xlo * whi pass would add exact zeros
   const int passes = (q.x_dtype == NNAB_DTYPE_BF16) ? 2 : 3;
 
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();
-  if (sms < 1) sms = 1;
+  int sms;
+  if ((rc = usable_sms(&sms))) return rc;
 
   int nb = block_choose_nb(Fb);
   if (q.fmt == FMT_FBANK && q.fb_steps != nullptr && poly && q.fb_poly_tile != 0) {
@@ -1005,13 +973,7 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.nv = g.nv;
   prm.t_slots = g.t_slots;
   prm.T = q.T;
-  prm.epi.scale = nullptr; prm.epi.scale_all = 1.f; prm.epi.fmt = q.fmt;
-  prm.epi.eps = q.eps; prm.epi.power = q.power; prm.epi.out = q.out; prm.epi.T = q.T;
-  prm.epi.out_bins = q.out_bins; prm.epi.bin_offset = q.bin_offset; prm.epi.F = q.F;
-  prm.epi.fb_table = q.fb_table; prm.epi.n_fb = q.n_fb; prm.epi.fb_steps = q.fb_steps;
-  prm.epi.raw = nullptr; prm.epi.raw_plane = 0;
-  prm.epi.ola_pitch = 0; prm.epi.ola_hop = 0;
-  prm.epi.planes_stride = q.planes_stride; prm.epi.planes_pitch = q.planes_pitch;
+  prm.epi = epilogue_of(q);
   if (q.fmt == FMT_PLANES && (int64_t)n_tiles * PH * nb > q.planes_pitch) return NNAB_EINVAL;
   const int64_t tiles = (int64_t)prm.num_m_tiles * n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);

@@ -19,7 +19,6 @@
 // and the epilogue writes the final format once.  No scratch, no atomics, no finalize kernel.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <atomic>
 #include <stdlib.h>
 #include <string.h>
 
@@ -430,21 +429,36 @@ static int build_tall_plan(const FramedProblem& q, TallPlan* plan) {
   return n > 0 ? NNAB_OK : NNAB_EUNSUPPORTED;
 }
 
-template <int FMT, bool SK>
-static int launch_tct_fmt(const CUtensorMap& ma, const CUtensorMap& mb8, const CUtensorMap& mb32,
-                          const TctParams& prm, const TallPlan& plan, int grid, cudaStream_t stream) {
+// SK: the balanced (shared-tile) schedule
+template <bool SK>
+static int launch_tct(int fmt, const CUtensorMap& ma, const CUtensorMap& mb8, const CUtensorMap& mb32,
+                      const TctParams& prm, const TallPlan& plan, int grid, cudaStream_t stream) {
   using S = TctSmem;
-  static std::atomic<uint64_t> configured_devs{0};  // the attribute is per device
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(framed_tct_kernel<FMT, SK>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
+  switch (fmt) {
+    case NNAB_FMT_MAGNITUDE:
+      return launch_persistent<framed_tct_kernel<0, SK>>(grid, TC_KERNEL_THREADS, S::TOTAL, S::TOTAL, stream, ma,
+                                                         mb8, mb32, prm, plan);
+    case NNAB_FMT_COMPLEX:
+      return launch_persistent<framed_tct_kernel<1, SK>>(grid, TC_KERNEL_THREADS, S::TOTAL, S::TOTAL, stream, ma,
+                                                         mb8, mb32, prm, plan);
+    case NNAB_FMT_PHASE_UNIT:
+      return launch_persistent<framed_tct_kernel<3, SK>>(grid, TC_KERNEL_THREADS, S::TOTAL, S::TOTAL, stream, ma,
+                                                         mb8, mb32, prm, plan);
+    default: return NNAB_EINVAL;
   }
-  framed_tct_kernel<FMT, SK><<<grid, TC_KERNEL_THREADS, S::TOTAL, stream>>>(ma, mb8, mb32, prm, plan);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+}
+
+// A operand of the tall-A kernels: the planes as {column within a row of hop_eff samples, frame phase, row,
+// plane}, phase p starting p * hop samples on (P = hop_eff / hop phases when hop < 64; rows past the end: zero
+// fill), box {64, 1, a_rows}
+static int encode_phase_rows(CUtensorMap* map, void* planes, int hop, int hop_eff, int P, int64_t plane_stride,
+                             uint32_t a_rows) {
+  const int64_t rows = (plane_stride - (int64_t)(P - 1) * hop) / hop_eff;
+  const uint64_t dims[4] = {(uint64_t)hop_eff, (uint64_t)P, (uint64_t)rows, 2};
+  const uint64_t strides[3] = {(uint64_t)(P > 1 ? hop : hop_eff) * 2, (uint64_t)hop_eff * 2,
+                               (uint64_t)plane_stride * 2};
+  const uint32_t box[3] = {64, 1, a_rows};
+  return encode_4d(map, planes, dims, strides, box);
 }
 
 // `packed`: the 8-bin-group layout of tc_pack_basis_varn.  Returns NNAB_EUNSUPPORTED (nothing
@@ -481,23 +495,12 @@ int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* work
   }
   nv = q.B * t_slots;
   // frames of a phase that exist: ceil((T - p) / P) <= t_slots by construction of the planes
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();
-  if (sms < 1) sms = 1;
+  int sms;
+  if ((rc = usable_sms(&sms))) return rc;
 
   CUtensorMap ma, mb8, mb32;
-  {
-    // A: {column within a row, frame phase, row, plane}; rows past the end: zero fill
-    const int64_t rows = (plane_stride - (int64_t)(P - 1) * q.hop) / hop_eff;
-    const uint64_t dims[4] = {(uint64_t)hop_eff, (uint64_t)P, (uint64_t)rows, 2};
-    const uint64_t strides[3] = {(uint64_t)(P > 1 ? q.hop : hop_eff) * 2, (uint64_t)hop_eff * 2,
-                                 (uint64_t)plane_stride * 2};
-    const uint32_t box[3] = {64, 1, (uint32_t)plan.a_rows};
-    rc = encode_4d(&ma, planes, dims, strides, box);
-    if (rc) return NNAB_EUNSUPPORTED;  // (e.g. a driver that rejects the overlapping phase stride)
-  }
+  if (encode_phase_rows(&ma, planes, q.hop, hop_eff, P, plane_stride, (uint32_t)plan.a_rows))
+    return NNAB_EUNSUPPORTED;  // (e.g. a driver that rejects the overlapping phase stride)
   if ((rc = encode_3d(&mb8, const_cast<void*>(packed), (uint64_t)kpad, (uint64_t)rows_w, 2,
                       (uint64_t)kpad * 2, (uint64_t)rows_w * kpad * 2, 64, 8, 64)))
     return rc;
@@ -513,9 +516,7 @@ int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* work
   prm.nv = nv;
   prm.t_slots = t_slots;
   prm.T = q.T;
-  prm.epi.scale = q.scale; prm.epi.scale_all = q.scale_all; prm.epi.fmt = q.fmt;
-  prm.epi.eps = q.eps; prm.epi.power = q.power; prm.epi.out = q.out; prm.epi.T = q.T;
-  prm.epi.out_bins = q.out_bins; prm.epi.bin_offset = q.bin_offset; prm.epi.F = q.F;
+  prm.epi = epilogue_of(q);
   const int64_t tiles = (int64_t)prm.num_m_tiles * P;
   int grid = (int)(tiles < sms ? tiles : sms);
   if (const char* e = getenv("NNAB_TALL_CTAS")) {  // tests: force shared tiles on small problems
@@ -544,19 +545,9 @@ int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* work
   }
   if (balanced) {
     count_balanced_launch();
-    switch (q.fmt) {
-      case NNAB_FMT_MAGNITUDE: return launch_tct_fmt<0, true>(ma, mb8, mb32, prm, plan, grid, stream);
-      case NNAB_FMT_COMPLEX: return launch_tct_fmt<1, true>(ma, mb8, mb32, prm, plan, grid, stream);
-      case NNAB_FMT_PHASE_UNIT: return launch_tct_fmt<3, true>(ma, mb8, mb32, prm, plan, grid, stream);
-      default: return NNAB_EINVAL;
-    }
+    return launch_tct<true>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
   }
-  switch (q.fmt) {
-    case NNAB_FMT_MAGNITUDE: return launch_tct_fmt<0, false>(ma, mb8, mb32, prm, plan, grid, stream);
-    case NNAB_FMT_COMPLEX: return launch_tct_fmt<1, false>(ma, mb8, mb32, prm, plan, grid, stream);
-    case NNAB_FMT_PHASE_UNIT: return launch_tct_fmt<3, false>(ma, mb8, mb32, prm, plan, grid, stream);
-    default: return NNAB_EINVAL;
-  }
+  return launch_tct<false>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
 }
 
 // ===========================================================================
@@ -782,15 +773,13 @@ int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int6
   const int64_t FT = (dec.len_out + 127) / 128;
   const int64_t t_slots = src_pitch / 256;
   if (256 * (FT + 2) > src_pitch + 256) return NNAB_EUNSUPPORTED;  // last frame's rows
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();
-  if (sms < 1) sms = 1;
+  int sms;
+  int rc = usable_sms(&sms);
+  if (rc) return rc;
   CUtensorMap ma, mb;
   const int64_t rows = src_plane_stride / 256;
-  int rc = encode_3d(&ma, const_cast<void*>(src_planes), 256, (uint64_t)rows, 2, 512,
-                     (uint64_t)src_plane_stride * 2, 64, FIR_A_ROWS, 64);
+  rc = encode_3d(&ma, const_cast<void*>(src_planes), 256, (uint64_t)rows, 2, 512,
+                 (uint64_t)src_plane_stride * 2, 64, FIR_A_ROWS, 64);
   if (rc) return rc;
   const int kf = tc_fir_k(taps, 2);  // 512
   if (kf != 64 * FIR_KBLOCKS) return NNAB_EUNSUPPORTED;
@@ -804,16 +793,9 @@ int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int6
   prm.num_m_tiles = (int)ceil_div64(prm.nv, TC_BM);
   prm.dec = dec;
   const int grid = prm.num_m_tiles < sms ? prm.num_m_tiles : sms;
-  static std::atomic<uint64_t> configured_devs{0};
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(fir_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)FirSmem::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
-  }
-  fir_tc_kernel<<<grid, TC_KERNEL_THREADS, FirSmem::TOTAL, stream>>>(ma, mb, prm);
-  NNAB_LAUNCH_CHECK();
+  if ((rc = launch_persistent<fir_tc_kernel>(grid, TC_KERNEL_THREADS, FirSmem::TOTAL, FirSmem::TOTAL, stream, ma,
+                                             mb, prm)))
+    return rc;
   add_exec_flops(3.0 * 2.0 * (double)prm.num_m_tiles * TC_BM * 640.0 * 64.0);  // banded: 640 columns x 64
   // clip edges
   fir_edge_fix_kernel<<<dim3(32, (unsigned)B), 128, 0, stream>>>(
@@ -973,17 +955,8 @@ octave_tc_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
 template <int FMT>
 static int launch_octave_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const OctParams& prm, int grid,
                              cudaStream_t stream) {
-  static std::atomic<uint64_t> configured_devs{0};
-  int cfg_dev = 0;
-  NNAB_CUDA_TRY(cudaGetDevice(&cfg_dev));
-  if (!((configured_devs.load(std::memory_order_relaxed) >> (cfg_dev & 63)) & 1u)) {
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(octave_tc_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)OctSmem::TOTAL));
-    configured_devs.fetch_or(1ull << (cfg_dev & 63), std::memory_order_relaxed);
-  }
-  octave_tc_kernel<FMT><<<grid, TC_KERNEL_THREADS, OctSmem::TOTAL, stream>>>(ma, mb, prm);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
+  return launch_persistent<octave_tc_kernel<FMT>>(grid, TC_KERNEL_THREADS, OctSmem::TOTAL, OctSmem::TOTAL, stream,
+                                                  ma, mb, prm);
 }
 
 // Whether octave_tc_kernel takes the octave problem q: caller-managed planes (presplit + presplit_t_slots),
@@ -1014,24 +987,14 @@ int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t st
   const int64_t plane_stride = q.presplit_plane_stride;
   __nv_bfloat16* planes = reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(q.presplit));
 
-  int dev = 0, sms = 132;
-  NNAB_CUDA_TRY(cudaGetDevice(&dev));
-  NNAB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  sms -= sm_reserve();
-  if (sms < 1) sms = 1;
+  int sms;
+  int rc = usable_sms(&sms);
+  if (rc) return rc;
   CUtensorMap ma, mb;
-  {
-    const int64_t rows = (plane_stride - (int64_t)(P - 1) * q.hop) / hop_eff;
-    const uint64_t dims[4] = {(uint64_t)hop_eff, (uint64_t)P, (uint64_t)rows, 2};
-    const uint64_t strides[3] = {(uint64_t)(P > 1 ? q.hop : hop_eff) * 2, (uint64_t)hop_eff * 2,
-                                 (uint64_t)plane_stride * 2};
-    const uint32_t box[3] = {64, 1, OCT_A_ROWS};
-    const int rc = encode_4d(&ma, planes, dims, strides, box);
-    if (rc) return rc;
-  }
+  if ((rc = encode_phase_rows(&ma, planes, q.hop, hop_eff, P, plane_stride, OCT_A_ROWS))) return rc;
   const int kpad = round_up_i(q.K, 64);
-  int rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, 32, 2, (uint64_t)kpad * 2,
-                     (uint64_t)32 * kpad * 2, 64, 32, 64);
+  rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, 32, 2, (uint64_t)kpad * 2,
+                 (uint64_t)32 * kpad * 2, 64, 32, 64);
   if (rc) return rc;
   OctParams prm{};
   prm.n_phases = P;
@@ -1043,9 +1006,7 @@ int launch_octave_tc(const FramedProblem& q, const void* packed, cudaStream_t st
   prm.t_slots = t_slots;
   prm.T = q.T;
   prm.num_m_tiles = (int)ceil_div64(prm.nv, TC_BM);
-  prm.epi.scale = q.scale; prm.epi.scale_all = q.scale_all; prm.epi.fmt = q.fmt;
-  prm.epi.eps = q.eps; prm.epi.power = q.power; prm.epi.out = q.out; prm.epi.T = q.T;
-  prm.epi.out_bins = q.out_bins; prm.epi.bin_offset = q.bin_offset; prm.epi.F = q.F;
+  prm.epi = epilogue_of(q);
   const int64_t tiles = (int64_t)prm.num_m_tiles * P;
   const int grid = (int)(tiles < sms ? tiles : sms);
   add_exec_flops(3.0 * 2.0 * (double)tiles * TC_BM * 32.0 * q.K);
