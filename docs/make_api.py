@@ -41,6 +41,11 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   `flush()`, `reset()`).  The concatenated outputs equal `module(x)` on the whole stream, bit for bit on the
   tensor-core routes except across the CQT1992v2 kernel's two tile schedules (2e-6; DESIGN.md §3.10).
   `StreamingInverse(istft_module, batch)` does the same for the inverse STFT, to fp32 rounding.
+  `StreamPool(module, slots)` serves independent streams of the same modules that advance by their own amounts:
+  `push(chunk, lengths, end=None)` gives slot s `chunk[s, :lengths[s]]`, ends the slots flagged in `end` and returns
+  a `PoolOutput(frames, slots, counts)` with a row for each slot that has new frames; `reset(slots)` starts new
+  streams in some slots while the others carry on.  Each slot's rows equal `module(x)` on its own stream, with the
+  rules of `StreamingTransform`.
   `StreamingPyramid(module, batch)` streams the CQT pyramid of `CQT2010v2` / `VQT` / `CQT2010` bit for bit on the
   whole-clip call's tensor-core plan (DESIGN.md §3.10).
 

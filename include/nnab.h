@@ -411,6 +411,63 @@ int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry,
                                  int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
                                  size_t ws_bytes, int path, void* stream);
 
+/* Stream pools: `slots` independent streams that advance by their own amounts (DESIGN.md §3.10).  Each
+ * *_pool_forward takes the arguments of the matching *_chunk_forward with (received, n_carry, frames) and
+ * flush replaced by a lane table, B by `slots` and T by T_max:
+ *   state     DEVICE fp32 carry ring of nnab_chunk_state_bytes(slots, K) bytes; row s belongs to slot s
+ *   lanes, d_lanes   the same n_lanes lanes, a HOST copy the library checks and a DEVICE copy the kernels
+ *             read (the caller keeps both alive until the call's work has run).  One lane per slot that
+ *             receives samples, ends, or returns frames in this push: its counters before the push (as for
+ *             *_chunk_forward), n new samples chunk[slot, :n] and end = 1 on the stream's last push (its
+ *             remaining frames, with the right padding, as flush).  The A lanes that return frames come
+ *             first, then the others; slots ascend within each group and appear once.
+ *   chunk, chunk_dtype, slots, n, chunk_pitch   the (slots, n) samples; every lane's n <= this n
+ *   A, T_max  lanes that return frames and the most frames one of them returns
+ * out is (A, ..., T_max) in the offline layout: row i holds lane i's new frames, bit for bit those of the
+ * offline call on its whole stream (tensor-core plans), and exact zeros at t >= its count.  NNAB_EINVAL for
+ * counters no stream can have, a slot out of range / repeated / out of order, a lane n above the chunk width,
+ * an A or T_max that disagrees with the lanes, a lane with nothing to do, or an end on a stream too short for
+ * its padding; all checks run before anything is enqueued.  The launches are those of the offline call on
+ * (A, (T_max - 1) * hop + K samples), one carry launch and one mask launch; idle slots cost nothing.  After the
+ * call the caller advances each lane's counters as for *_chunk_forward.  The SIMT plans return
+ * NNAB_EUNSUPPORTED before anything is enqueued.  The workspace queries equal the offline queries for A clips
+ * of (T_max - 1) * hop + K samples, uncentred (0 when A or T_max is 0). */
+typedef struct nnab_stream_lane {
+  int64_t slot, received, n_carry, frames, n, end;
+} nnab_stream_lane;
+size_t nnab_stft_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int path);
+int nnab_stft_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                           int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots, int64_t n,
+                           int64_t chunk_pitch, const float* wcos, const float* wsin, const void* packed, int n_fft,
+                           int F, int hop, int center, int pad_mode, int out_format, float sqrt_eps, float* out,
+                           int64_t T_max, void* workspace, size_t ws_bytes, int path, void* stream);
+size_t nnab_filterbank_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_fb,
+                                            int path, int has_table);
+int nnab_stft_filterbank_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                      int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                      int64_t n, int64_t chunk_pitch, const float* wcos, const float* wsin,
+                                      const void* packed, int n_fft, int F, int hop, int center, int pad_mode,
+                                      float sqrt_eps, float power, const float* fb, int n_fb, const void* fb_table,
+                                      float* out, int64_t T_max, void* workspace, size_t ws_bytes, int path,
+                                      void* stream);
+size_t nnab_mfcc_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_mels, int path,
+                                      int has_table);
+int nnab_mfcc_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                           int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots, int64_t n,
+                           int64_t chunk_pitch, const float* wcos, const float* wsin, const void* packed, int n_fft,
+                           int F, int hop, int center, int pad_mode, float sqrt_eps, float power,
+                           const float* mel_basis, int n_mels, const void* fb_table, float amin, float ref,
+                           float top_db, const float* dct, int n_mfcc, float* out, int64_t T_max, void* workspace,
+                           size_t ws_bytes, int path, void* stream);
+size_t nnab_cqt1992v2_pool_workspace_bytes(int64_t A, int64_t T_max, int width, int n_bins, int hop, int path);
+int nnab_cqt1992v2_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                int64_t n, int64_t chunk_pitch, const float* k_real, const float* k_imag,
+                                const void* packed, const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins,
+                                int width, int hop, int center, int pad_mode, const float* scale, float scale_all,
+                                int out_format, float sqrt_eps, float* out, int64_t T_max, void* workspace,
+                                size_t ws_bytes, int path, void* stream);
+
 /* Streamed CQT pyramid: nnab_cqt_pyramid_forward_ex's arguments with (x, L, x_pitch) replaced by state, the
  * three host counters, the chunk and flush as above.
  *   state     DEVICE fp32, nnab_cqt_pyramid_chunk_state_bytes(B, n_octaves, widths, hop, early_factor) bytes:

@@ -126,6 +126,7 @@ for _name in ("nnab_stft_forward", "nnab_stft_filterbank_forward", "nnab_mfcc_fo
 # of (B, L) and the pad mode after `center`
 _CHUNK_HEAD = [_P, c_int64, c_int64, c_int64, _P, c_int, c_int64, c_int64, c_int64, c_int]
 _CHUNK_WS_HEAD = [c_int64, c_int64, c_int64, c_int64, c_int]
+_POOL_HEAD = [_P, _P, _P, c_int64, c_int64, _P, c_int, c_int64, c_int64, c_int64]
 SIGNATURES["nnab_chunk_state_bytes"] = (c_size_t, [c_int64, c_int])
 for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_forward", "nnab_filterbank"),
                    ("nnab_mfcc_forward", "nnab_mfcc"), ("nnab_cqt1992v2_forward", "nnab_cqt1992v2")):
@@ -133,6 +134,11 @@ for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_fo
     SIGNATURES[_name.replace("_forward", "_chunk_forward")] = (_res, _CHUNK_HEAD + _args[4:])
     _wres, _wargs = SIGNATURES[_ws + "_workspace_bytes"]
     SIGNATURES[_ws + "_chunk_workspace_bytes"] = (_wres, _CHUNK_WS_HEAD + _wargs[2:6] + [c_int] + _wargs[6:])
+    # the *_pool_forward entry points: (state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots, n,
+    # chunk_pitch) in place of (x, B, L, x_pitch); their workspace queries take (A, T_max) in place of (B, L)
+    # and no `center`
+    SIGNATURES[_name.replace("_forward", "_pool_forward")] = (_res, _POOL_HEAD + _args[4:])
+    SIGNATURES[_ws + "_pool_workspace_bytes"] = (_wres, [c_int64, c_int64] + _wargs[2:5] + _wargs[6:])
 SIGNATURES["nnab_cqt_pyramid_chunk_state_bytes"] = (c_size_t, [c_int64, c_int, _P, c_int, c_int])
 SIGNATURES["nnab_cqt_pyramid_chunk_workspace_bytes"] = (
     c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int, _P, c_int, c_int, c_int])
@@ -662,6 +668,100 @@ def cqt1992v2_chunk_forward(st, x, flush, T, k_real, k_imag, packed, k_begin, k_
             _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode,
             _ptr(scale), scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
     return _chunk_result(rc, out, "nnab_cqt1992v2_chunk_forward")
+
+
+# --------------------------------------------------------------------------- #
+# pool calls (nnaudio_b200.streaming.StreamPool): one push of a stream pool.  `pool` carries the device carry
+# ring (pool.ring, one row per slot), pool.slots and pool.dtype; `lanes` is the push's (n_lanes, 6) int64 lane
+# table (nnab_stream_lane rows, the A lanes with frames first); `x` the (slots, n) chunk or None.  The remaining
+# arguments are those of the offline call.  Returns the (A, ..., T_max) frames, or None when the plan cannot
+# read a chunk (NNAB_EUNSUPPORTED, nothing enqueued).
+# --------------------------------------------------------------------------- #
+LANE_FIELDS = ("slot", "received", "n_carry", "frames", "n", "end")
+
+
+def _pool_lanes(pool, lanes):
+    """Host and device copies of a lane table: the host copy in pinned memory, the device copy made from it
+    without blocking (torch's host allocator keeps the pinned block until the copy has run)."""
+    if len(lanes) == 0:
+        return None, None
+    host = torch.as_tensor(lanes, dtype=torch.int64).contiguous().pin_memory()
+    return host, host.to(pool.ring.device, non_blocking=True)
+
+
+def stft_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format,
+                      sqrt_eps, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    F, dev = wcos.shape[0], pool.ring.device
+    out = torch.empty((A, F, T_max, 2) if out_format == FMT_COMPLEX else (A, F, T_max), dtype=torch.float32,
+                      device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        hl, dl = _pool_lanes(pool, lanes)
+        ws, wsb = _workspace(L.nnab_stft_pool_workspace_bytes(A, T_max, n_fft, F, hop, path), dev)
+        rc = L.nnab_stft_pool_forward(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
+            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, out_format, sqrt_eps, _ptr(out), T_max,
+            _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_stft_pool_forward")
+
+
+def stft_filterbank_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode,
+                                 sqrt_eps, power, fb, fb_table=None, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    F, n_fb, dev = wcos.shape[0], fb.shape[0], pool.ring.device
+    out = torch.empty((A, n_fb, T_max), dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        hl, dl = _pool_lanes(pool, lanes)
+        ws, wsb = _workspace(L.nnab_filterbank_pool_workspace_bytes(A, T_max, n_fft, F, hop, n_fb, path,
+                                                                    int(fb_table is not None)), dev)
+        rc = L.nnab_stft_filterbank_pool_forward(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
+            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(fb), n_fb,
+            _ptr(fb_table), _ptr(out), T_max, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_stft_filterbank_pool_forward")
+
+
+def mfcc_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
+                      mel_basis, amin, ref, top_db, dct, fb_table=None, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    F, n_mels, n_mfcc, dev = wcos.shape[0], mel_basis.shape[0], dct.shape[0], pool.ring.device
+    out = torch.empty((A, n_mfcc, T_max), dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        hl, dl = _pool_lanes(pool, lanes)
+        ws, wsb = _workspace(L.nnab_mfcc_pool_workspace_bytes(A, T_max, n_fft, F, hop, n_mels, path,
+                                                              int(fb_table is not None)), dev)
+        rc = L.nnab_mfcc_pool_forward(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
+            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(mel_basis), n_mels,
+            _ptr(fb_table), amin, ref, -1.0 if top_db is None else float(top_db), _ptr(dct), n_mfcc, _ptr(out),
+            T_max, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_mfcc_pool_forward")
+
+
+def cqt1992v2_pool_forward(pool, lanes, x, A, T_max, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode,
+                           scale, scale_all, out_format, sqrt_eps, path=None):
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    (n_bins, width), dev = k_real.shape, pool.ring.device
+    out = torch.empty((A, n_bins, T_max) if out_format == FMT_MAGNITUDE else (A, n_bins, T_max, 2),
+                      dtype=torch.float32, device=dev)
+    path = resolve_path(path)
+    kb = k_begin.ctypes.data_as(c_void_p) if k_begin is not None else None
+    ke = k_end.ctypes.data_as(c_void_p) if k_end is not None else None
+    with torch.cuda.device(dev):
+        hl, dl = _pool_lanes(pool, lanes)
+        ws, wsb = _workspace(L.nnab_cqt1992v2_pool_workspace_bytes(A, T_max, width, n_bins, hop, path), dev)
+        rc = L.nnab_cqt1992v2_pool_forward(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(k_real),
+            _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode, _ptr(scale), scale_all,
+            out_format, sqrt_eps, _ptr(out), T_max, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_cqt1992v2_pool_forward")
 
 
 def cqt_pyramid_chunk_state_bytes(B: int, widths, hop: int, early_factor: int) -> int:

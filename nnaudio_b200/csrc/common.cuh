@@ -131,6 +131,10 @@ __host__ __device__ inline int poly4_range(int k, int M, int nb) {
 // (raw r of stream b at ring[b * ring_pitch + r % ring_len]), [received, total) from the chunk (samples of
 // type FramedProblem::x_dtype, rows of chunk_pitch).  r < 0 is the left centre padding; on the last push
 // (at_end) r >= total is the right one.
+// A stream pool's push (lanes != nullptr) gives every batch row b its own stream: lane b of the DEVICE lane
+// table names its ring row and chunk row (`slot`), its counters and its end; origin = frames * hop - pad and
+// received / total / at_end come from the lane, and the fields of the same name above are unused.  The clip
+// length is the batch's longest; a row's samples past its own stream read as zeros.
 struct ChunkSource {
   const float* ring;
   int64_t ring_pitch;
@@ -140,7 +144,41 @@ struct ChunkSource {
   int64_t received, total, origin, length;
   int pad_mode;
   int at_end;
+  const nnab_stream_lane* lanes;  // pools only, else nullptr
+  int K, hop, pad;                // pools only: the framing that places each lane's clip
 };
+
+// ---- the counters of one stream (DESIGN §3.10), shared by the host checks and the pool kernels ----------
+// Frame t is returned by the first push after which every raw sample it reads has arrived: t * hop + K - pad
+// samples (reflect padding: and at least pad + 1, the left mirror of frame 0), or all remaining frames on
+// the last push.
+__host__ __device__ inline int64_t chunk_ready_frames(int64_t total, int K, int hop, int pad, int pad_mode) {
+  if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && total < pad + 1) return 0;
+  const int64_t need = (int64_t)K - pad;
+  return total < need ? 0 : (total - need) / hop + 1;
+}
+
+// Frames of the whole stream of `total` samples, once it has ended (the offline call's T).
+__host__ __device__ inline int64_t chunk_end_frames(int64_t total, int K, int hop, int pad) {
+  const int64_t span = total + 2 * (int64_t)pad - K;
+  return span < 0 ? 0 : span / hop + 1;
+}
+
+// First raw sample the push after `frames` frames still reads: the first frame's start, and with centre
+// padding no later than total - (pad + 1) (the right mirror of the last push reads that far back).
+__host__ __device__ inline int64_t chunk_carry_start(int64_t total, int64_t frames, int hop, int pad) {
+  int64_t s = frames * hop - pad;
+  if (pad > 0 && s > total - (pad + 1)) s = total - (pad + 1);
+  if (s < 0) s = 0;
+  return s < total ? s : total;
+}
+
+// Frames a pool lane has returned after its push (the library has checked the lane on the host).
+__host__ __device__ inline int64_t lane_frames_after(const nnab_stream_lane& ln, int K, int hop, int pad,
+                                                     int pad_mode) {
+  const int64_t total = ln.received + ln.n;
+  return ln.end ? chunk_end_frames(total, K, hop, pad) : chunk_ready_frames(total, K, hop, pad, pad_mode);
+}
 
 struct FramedProblem {
   const void* x;       // (B, L) rows, pitch x_pitch samples of type x_dtype
@@ -215,6 +253,11 @@ int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_p
                    void* planes, cudaStream_t stream);
 // store raw samples [from, total) of the chunk into the carry ring (cs.received = raw index of chunk[0])
 int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream);
+// pools (cs.lanes): the carry of every one of the n_lanes lanes, each its own [from, total) (at most
+// `longest` samples), and the zeroing of output frames t >= the count of row i of out (A, rows, T, cols)
+int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream);
+int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int64_t T, int cols,
+                 cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
                   int64_t keep_hi, cudaStream_t stream);
 int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,

@@ -152,22 +152,39 @@ static void set_wave(FramedProblem& p, const Wave& w) {
 
 // ---- chunked streams (DESIGN §3.10) ------------------------------------------------------------
 // Host counters of a stream: `received` raw samples so far, the last `n_carry` of them in the carry ring,
-// `frames` frames returned.  Frame t is returned by the first push after which every raw sample it reads
-// has arrived: t * hop + K - pad samples (reflect padding: and at least pad + 1, the left mirror of frame
-// 0), or all remaining frames on the last push.
-static int64_t chunk_ready_frames(int64_t total, int K, int hop, int pad, int pad_mode) {
-  if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && total < pad + 1) return 0;
-  const int64_t need = (int64_t)K - pad;
-  return total < need ? 0 : (total - need) / hop + 1;
-}
+// `frames` frames returned (chunk_ready_frames / chunk_carry_start in common.cuh).
+struct StreamStep {
+  int64_t total;      // raw samples after the push
+  int64_t t_end;      // frames returned after the push
+  int64_t T;          // frames this push returns
+  int64_t from;       // raw samples [from, total) go into the ring after the push
+};
 
-// First raw sample the push after `frames` frames still reads: the first frame's start, and with centre
-// padding no later than total - (pad + 1) (the right mirror of the last push reads that far back).
-static int64_t chunk_carry_start(int64_t total, int64_t frames, int hop, int pad) {
-  int64_t s = frames * hop - pad;
-  if (pad > 0 && s > total - (pad + 1)) s = total - (pad + 1);
-  if (s < 0) s = 0;
-  return s < total ? s : total;
+// One push of one stream: n new samples, the last push iff `end`.  NNAB_EINVAL for counters no stream can
+// have (they must be those of a stream that returned every ready frame) and for an end the stream is too
+// short for (reflect padding needs pad < total; at least one frame).  Both the streams of *_chunk_forward
+// and every lane of a pool are checked here.
+static int stream_step(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int end, int K, int hop,
+                       int pad, int pad_mode, StreamStep* o) {
+  if (received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
+  if (frames != chunk_ready_frames(received, K, hop, pad, pad_mode) ||
+      n_carry != received - chunk_carry_start(received, frames, hop, pad))
+    return NNAB_EINVAL;
+  const int64_t total = received + n;
+  int64_t t_end;
+  if (end) {
+    if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad >= total) return NNAB_EINVAL;
+    t_end = chunk_end_frames(total, K, hop, pad);
+    if (t_end <= 0) return NNAB_EINVAL;
+  } else {
+    t_end = chunk_ready_frames(total, K, hop, pad, pad_mode);
+  }
+  o->total = total;
+  o->t_end = t_end;
+  o->T = t_end - frames;
+  const int64_t keep = chunk_carry_start(total, t_end, hop, pad);
+  o->from = keep > received ? keep : received;
+  return NNAB_OK;
 }
 
 struct ChunkPlan {
@@ -180,38 +197,105 @@ static int chunk_plan(const void* state, int64_t received, int64_t n_carry, int6
                       int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush, int K, int hop,
                       int pad, int pad_mode, ChunkPlan* o) {
   if (state == nullptr || !dtype_ok(chunk_dtype) || B < 0 || B > 65535 || n < 0 || (n > 0 && chunk == nullptr) ||
-      chunk_pitch < n || K < 2 || hop <= 0 || received < 0 || frames < 0)
+      chunk_pitch < n || K < 2 || hop <= 0)
     return NNAB_EINVAL;
   if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
-  // the counters must be those of a stream that returned every ready frame
-  if (frames != chunk_ready_frames(received, K, hop, pad, pad_mode) ||
-      n_carry != received - chunk_carry_start(received, frames, hop, pad))
-    return NNAB_EINVAL;
-  const int64_t total = received + n;
-  int64_t t_end;
-  if (flush) {
-    if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad >= total) return NNAB_EINVAL;
-    t_end = frames_of(total, K, hop, pad);
-    if (t_end <= 0) return NNAB_EINVAL;
-  } else {
-    t_end = chunk_ready_frames(total, K, hop, pad, pad_mode);
-  }
+  StreamStep st;
+  const int rc = stream_step(received, n_carry, frames, n, flush, K, hop, pad, pad_mode, &st);
+  if (rc) return rc;
   ChunkSource& c = o->cs;
+  c = ChunkSource{};
   c.ring = static_cast<const float*>(state);
   c.ring_pitch = K;
   c.ring_len = K;
   c.chunk = chunk;
   c.chunk_pitch = chunk_pitch;
   c.received = received;
-  c.total = total;
+  c.total = st.total;
   c.origin = frames * hop - pad;
-  c.length = t_end > frames ? (t_end - frames - 1) * hop + K : 0;
+  c.length = st.T > 0 ? (st.T - 1) * hop + K : 0;
   c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
   c.at_end = flush ? 1 : 0;
-  o->T = t_end - frames;
-  const int64_t keep = chunk_carry_start(total, t_end, hop, pad);
-  o->from = keep > received ? keep : received;
+  o->T = st.T;
+  o->from = st.from;
   return NNAB_OK;
+}
+
+// ---- stream pools (DESIGN §3.10 "Pools") ---------------------------------------------------------------
+struct PoolPlan {
+  ChunkSource cs;     // lanes = the device table; length = the clip of T_max frames
+  int64_t A, T_max;
+  int64_t longest;    // the most samples one lane stores into the ring
+};
+
+// Checks the whole push (every lane by stream_step, the table's order and totals) before anything runs.
+static int pool_plan(const void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                     int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots, int64_t n,
+                     int64_t chunk_pitch, int K, int hop, int pad, int pad_mode, int64_t T_max, PoolPlan* o) {
+  if (state == nullptr || !dtype_ok(chunk_dtype) || slots < 1 || slots > 65535 || n < 0 ||
+      (n > 0 && chunk == nullptr) || chunk_pitch < n || K < 2 || hop <= 0 || n_lanes < 0 || n_lanes > slots ||
+      A < 0 || A > n_lanes || T_max < 0 || (n_lanes > 0 && (lanes == nullptr || d_lanes == nullptr)))
+    return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  std::vector<uint8_t> seen((size_t)slots, 0);
+  int64_t t_max = 0, longest = 0;
+  for (int64_t i = 0; i < n_lanes; ++i) {
+    const nnab_stream_lane& ln = lanes[i];
+    if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
+    if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
+    seen[(size_t)ln.slot] = 1;
+    if (ln.n > n || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
+    StreamStep st;
+    const int rc = stream_step(ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, K, hop, pad, pad_mode, &st);
+    if (rc) return rc;
+    if ((i < A) != (st.T > 0)) return NNAB_EINVAL;           // the A lanes with frames come first
+    if (st.T == 0 && ln.n == 0 && !ln.end) return NNAB_EINVAL;  // a lane with nothing to do
+    if (st.T > t_max) t_max = st.T;
+    if (st.total - st.from > longest) longest = st.total - st.from;
+  }
+  if (t_max != T_max) return NNAB_EINVAL;
+  ChunkSource& c = o->cs;
+  c = ChunkSource{};
+  c.ring = static_cast<const float*>(state);
+  c.ring_pitch = K;
+  c.ring_len = K;
+  c.chunk = chunk;
+  c.chunk_pitch = chunk_pitch;
+  c.length = T_max > 0 ? (T_max - 1) * hop + K : 0;
+  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
+  c.lanes = d_lanes;
+  c.K = K; c.hop = hop; c.pad = pad;
+  o->A = A;
+  o->T_max = T_max;
+  o->longest = longest;
+  return NNAB_OK;
+}
+
+// Floats per (row, frame) of an output format (nnab.h): complex pairs and unit phasors take two.
+static int format_cols(int out_format) {
+  return out_format == NNAB_FMT_COMPLEX || out_format == NNAB_FMT_PHASE_UNIT ? 2 : 1;
+}
+
+// Clip length of a pool push's batch (0: no lane returns a frame); host only, no validation.
+static int64_t pool_clip_length(int64_t A, int64_t T_max, int K, int hop) {
+  return A > 0 && T_max > 0 ? (T_max - 1) * (int64_t)hop + K : 0;
+}
+
+// The offline plan on the A rows' clips, the zeroing of every row's frames past its count, then each lane's
+// carry.  As chunk_forward, a plan that cannot read the clips returns NNAB_EUNSUPPORTED before anything is
+// enqueued (when A > 0).
+template <typename Run>
+static int pool_forward(const PoolPlan& pp, int chunk_dtype, int64_t n_lanes, float* out, int64_t rows, int cols,
+                        Run&& run, void* stream) {
+  int rc = check_arch();
+  if (rc) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (pp.A > 0) {
+    const Wave w{nullptr, chunk_dtype, pp.A, pp.cs.length, pp.cs.length, 0, pp.cs.pad_mode, &pp.cs};
+    if ((rc = run(w, s))) return rc;
+    if ((rc = tc_pool_mask(pp.cs, pp.A, out, rows, pp.T_max, cols, s))) return rc;
+  }
+  return tc_pool_carry(pp.cs, chunk_dtype, n_lanes, pp.longest, s);
 }
 
 static Wave chunk_wave(const ChunkPlan& cp, int chunk_dtype, int64_t B) {
@@ -2091,6 +2175,106 @@ int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry,
   return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
                          out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+// ------------------------------------------------------------ stream pools ----
+size_t nnab_stft_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int path) {
+  const int64_t Lv = pool_clip_length(A, T_max, n_fft, hop);
+  return Lv > 0 ? nnab_stft_workspace_bytes(A, Lv, n_fft, F, hop, 0, path) : 0;
+}
+
+int nnab_stft_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                           int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots, int64_t n,
+                           int64_t chunk_pitch, const float* wcos, const float* wsin, const void* packed, int n_fft,
+                           int F, int hop, int center, int pad_mode, int out_format, float sqrt_eps, float* out,
+                           int64_t T_max, void* workspace, size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = pool_plan(state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots, n, chunk_pitch, n_fft, hop,
+                     center ? n_fft / 2 : 0, pad_mode, T_max, &pp);
+  if (rc) return rc;
+  if (F <= 0 || (A > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
+  return pool_forward(pp, chunk_dtype, n_lanes, out, F, format_cols(out_format),
+                      [&](const Wave& w, cudaStream_t s) {
+    return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T_max, workspace, ws_bytes,
+                    path, s);
+  }, stream);
+}
+
+size_t nnab_filterbank_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_fb,
+                                            int path, int has_table) {
+  const int64_t Lv = pool_clip_length(A, T_max, n_fft, hop);
+  return Lv > 0 ? filterbank_ws_bytes(A, Lv, n_fft, F, hop, 0, n_fb, path, has_table) : 0;
+}
+
+int nnab_stft_filterbank_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                      int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                      int64_t n, int64_t chunk_pitch, const float* wcos, const float* wsin,
+                                      const void* packed, int n_fft, int F, int hop, int center, int pad_mode,
+                                      float sqrt_eps, float power, const float* fb, int n_fb, const void* fb_table,
+                                      float* out, int64_t T_max, void* workspace, size_t ws_bytes, int path,
+                                      void* stream) {
+  PoolPlan pp;
+  int rc = pool_plan(state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots, n, chunk_pitch, n_fft, hop,
+                     center ? n_fft / 2 : 0, pad_mode, T_max, &pp);
+  if (rc) return rc;
+  if (F <= 0 || (A > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
+  return pool_forward(pp, chunk_dtype, n_lanes, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
+    return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T_max,
+                          workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+size_t nnab_mfcc_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_mels, int path,
+                                      int has_table) {
+  (void)has_table;
+  const int64_t Lv = pool_clip_length(A, T_max, n_fft, hop);
+  return Lv > 0 ? mfcc_ws_bytes(A, Lv, n_fft, F, hop, 0, n_mels, path) : 0;
+}
+
+int nnab_mfcc_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                           int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots, int64_t n,
+                           int64_t chunk_pitch, const float* wcos, const float* wsin, const void* packed, int n_fft,
+                           int F, int hop, int center, int pad_mode, float sqrt_eps, float power,
+                           const float* mel_basis, int n_mels, const void* fb_table, float amin, float ref,
+                           float top_db, const float* dct, int n_mfcc, float* out, int64_t T_max, void* workspace,
+                           size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = pool_plan(state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots, n, chunk_pitch, n_fft, hop,
+                     center ? n_fft / 2 : 0, pad_mode, T_max, &pp);
+  if (rc) return rc;
+  // the top_db floor is a maximum over the whole clip: a stream cannot apply it frame by frame
+  if (F <= 0 || (A > 0 && out == nullptr) || top_db >= 0.f ||
+      mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin))
+    return NNAB_EINVAL;
+  return pool_forward(pp, chunk_dtype, n_lanes, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
+    return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
+                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+size_t nnab_cqt1992v2_pool_workspace_bytes(int64_t A, int64_t T_max, int width, int n_bins, int hop, int path) {
+  const int64_t Lv = pool_clip_length(A, T_max, width, hop);
+  return Lv > 0 ? nnab_cqt1992v2_workspace_bytes(A, Lv, width, n_bins, hop, 0, path) : 0;
+}
+
+int nnab_cqt1992v2_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                int64_t n, int64_t chunk_pitch, const float* k_real, const float* k_imag,
+                                const void* packed, const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins,
+                                int width, int hop, int center, int pad_mode, const float* scale, float scale_all,
+                                int out_format, float sqrt_eps, float* out, int64_t T_max, void* workspace,
+                                size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = pool_plan(state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots, n, chunk_pitch, width, hop,
+                     center ? width / 2 : 0, pad_mode, T_max, &pp);
+  if (rc) return rc;
+  if (n_bins <= 0 || (A > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
+    return NNAB_EINVAL;
+  return pool_forward(pp, chunk_dtype, n_lanes, out, n_bins, format_cols(out_format),
+                      [&](const Wave& w, cudaStream_t s) {
+    return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
+                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s);
   }, stream);
 }
 

@@ -25,6 +25,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdlib.h>
+#include <type_traits>
 
 #include "common.cuh"
 #include "epilogue.cuh"
@@ -192,16 +193,27 @@ __global__ void __launch_bounds__(256) pad_split_kernel(
 
 // pad_split_kernel on a push's virtual clip (ChunkSource): each sample is taken from the fp32 carry ring or
 // the chunk, with the reflect / constant centre padding of the whole stream at its two ends.  The planes of
-// frame t0 + j are then those the whole-clip pre-pass writes for frame t0 + j.
-template <typename Tx>
+// frame t0 + j are then those the whole-clip pre-pass writes for frame t0 + j.  LANES (stream pools): row b
+// builds the clip of lane b of c.lanes, from its own ring / chunk row, counters and end; its samples past
+// what its own frames read are zeros.
+template <typename Tx, bool LANES>
 __global__ void __launch_bounds__(256) chunk_split_kernel(
     ChunkSource c, const Tx* __restrict__ chunk, int shift, int64_t clip_pitch, int64_t plane_stride,
     int poly_hop, __nv_bfloat16* __restrict__ planes) {
   const int64_t b = blockIdx.y;
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i0 >= clip_pitch) return;
-  const float* __restrict__ ring = c.ring + b * c.ring_pitch;
-  const Tx* __restrict__ xb = chunk + b * c.chunk_pitch;
+  int64_t row = b;
+  if constexpr (LANES) {
+    const nnab_stream_lane& ln = c.lanes[b];
+    row = ln.slot;
+    c.received = ln.received;
+    c.total = ln.received + ln.n;
+    c.origin = ln.frames * c.hop - c.pad;
+    c.at_end = (int)ln.end;
+  }
+  const float* __restrict__ ring = c.ring + row * c.ring_pitch;
+  const Tx* __restrict__ xb = chunk + row * c.chunk_pitch;
   const bool reflect = c.pad_mode == NNAB_PAD_REFLECT;
   const int64_t s0 = split_src(i0, poly_hop) + shift;
   const int step = poly_hop ? 4 : 1;  // the 8 positions of a thread: consecutive samples, or one phase
@@ -217,7 +229,8 @@ __global__ void __launch_bounds__(256) chunk_split_kernel(
       if (r < 0) {
         if (reflect) r = -r; else live = false;
       } else if (r >= c.total) {
-        if (c.at_end && reflect) r = 2 * (c.total - 1) - r; else live = false;
+        // a pool row's clip runs past its own right padding (the longest row sets the length): zeros there
+        if (c.at_end && reflect && (!LANES || r - c.total < c.pad)) r = 2 * (c.total - 1) - r; else live = false;
       }
       if (live) v = r < c.received ? __ldg(ring + r % c.ring_len) : sample_f32(__ldg(xb + (r - c.received)));
     }
@@ -230,15 +243,41 @@ __global__ void __launch_bounds__(256) chunk_split_kernel(
 
 // Raw samples [from, total) of the chunk into the carry ring.  Runs after every kernel of the push that reads
 // the ring (same stream), and never overwrites a sample the next push reads: the ring holds ring_len >= the
-// longest carry.
-template <typename Tx>
+// longest carry.  LANES: row b is lane b of c.lanes, which keeps its own [from, total) by the same rule as
+// the host (chunk_carry_start after the lane's frames, and never before its first new sample).
+template <typename Tx, bool LANES>
 __global__ void __launch_bounds__(256) chunk_carry_kernel(ChunkSource c, const Tx* __restrict__ chunk,
                                                           int64_t from) {
-  const int64_t b = blockIdx.y;
+  int64_t row = blockIdx.y;
+  if constexpr (LANES) {
+    const nnab_stream_lane ln = c.lanes[blockIdx.y];
+    row = ln.slot;
+    c.received = ln.received;
+    c.total = ln.received + ln.n;
+    const int64_t keep =
+        chunk_carry_start(c.total, lane_frames_after(ln, c.K, c.hop, c.pad, c.pad_mode), c.hop, c.pad);
+    from = keep > c.received ? keep : c.received;
+  }
   const int64_t r = from + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= c.total) return;
-  const_cast<float*>(c.ring)[b * c.ring_pitch + r % c.ring_len] =
-      sample_f32(__ldg(chunk + b * c.chunk_pitch + (r - c.received)));
+  const_cast<float*>(c.ring)[row * c.ring_pitch + r % c.ring_len] =
+      sample_f32(__ldg(chunk + row * c.chunk_pitch + (r - c.received)));
+}
+
+// Stream pools: frames t >= count of row i of out (A, rows, T, cols) are exact zeros (the row's clip is the
+// batch's longest, so the transform also computed frames its stream has not completed).
+__global__ void __launch_bounds__(256) pool_mask_kernel(ChunkSource c, float* __restrict__ out, int64_t rows,
+                                                        int64_t T, int cols) {
+  const nnab_stream_lane ln = c.lanes[blockIdx.y];
+  const int64_t count = lane_frames_after(ln, c.K, c.hop, c.pad, c.pad_mode) - ln.frames;
+  if (count >= T) return;
+  const int64_t row_len = (T - count) * cols;  // the tail of each of the `rows` rows
+  float* __restrict__ o = out + (int64_t)blockIdx.y * rows * T * cols;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < rows * row_len;
+       k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = k / row_len;
+    o[r * T * cols + count * cols + (k - r * row_len)] = 0.f;
+  }
 }
 
 // The one sample-type dispatch (NNAB_DTYPE_*): f(samples) launches one kernel on x as fp32, bf16 or fp16
@@ -1340,7 +1379,13 @@ size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K) {
 static int launch_chunk_split(const ChunkSource& cs, int x_dtype, dim3 grid, int shift, int64_t clip_pitch,
                               int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream) {
   return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
-    chunk_split_kernel<<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop, planes);
+    using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    if (cs.lanes != nullptr)
+      chunk_split_kernel<Tx, true><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
+                                                             planes);
+    else
+      chunk_split_kernel<Tx, false><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
+                                                              planes);
   });
 }
 
@@ -1358,8 +1403,30 @@ int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, 
   if (B > 65535) return NNAB_EUNSUPPORTED;
   const dim3 grid((unsigned)ceil_div64(cs.total - from, 256), (unsigned)B);
   return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
-    chunk_carry_kernel<<<grid, 256, 0, stream>>>(cs, xs, from);
+    using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    chunk_carry_kernel<Tx, false><<<grid, 256, 0, stream>>>(cs, xs, from);
   });
+}
+
+int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream) {
+  if (longest <= 0 || n_lanes <= 0) return NNAB_OK;
+  if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(longest, 256), (unsigned)n_lanes);
+  return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    chunk_carry_kernel<Tx, true><<<grid, 256, 0, stream>>>(cs, xs, 0);
+  });
+}
+
+int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int64_t T, int cols,
+                 cudaStream_t stream) {
+  if (A <= 0 || T <= 0) return NNAB_OK;
+  if (A > 65535) return NNAB_EUNSUPPORTED;
+  const int64_t per_row = rows * T * cols;
+  const dim3 grid((unsigned)(ceil_div64(per_row, 256) < 64 ? ceil_div64(per_row, 256) : 64), (unsigned)A);
+  pool_mask_kernel<<<grid, 256, 0, stream>>>(cs, out, rows, T, cols);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
 }
 
 // ---------------------------------------------------------------------------

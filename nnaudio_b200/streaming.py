@@ -13,6 +13,11 @@ bf16 planes from the carried fp32 samples and the new chunk.  Plans that read th
 upcast chunk, padded and concatenated with torch, through the module's offline call with ``center=False``.
 A push never reads the device back or synchronises.
 
+``StreamPool(module, slots)`` serves independent streams that advance by their own amounts: each
+``push(chunk, lengths, end)`` appends ``chunk[s, :lengths[s]]`` to slot ``s``'s stream, ends the streams
+flagged in ``end``, and returns the new frames of the slots that have some; ``reset(slots)`` starts new streams
+in some slots while the others carry on.  Each stream's frames are those of ``StreamingTransform``.
+
 ``StreamingPyramid(module, batch)`` streams through the ÷2 resampling pyramid of ``CQT2010v2``, ``VQT`` and
 ``CQT2010`` on the whole-clip call's tensor-core plan: each push returns the frames final in every octave.
 
@@ -21,6 +26,9 @@ output samples no later frame can change, ``flush(length=None)`` the rest.
 """
 from __future__ import annotations
 
+from typing import NamedTuple
+
+import numpy as np
 import torch
 
 from . import _C
@@ -32,7 +40,7 @@ from .features.mel import MFCC, MelSpectrogram
 from .features.stft import STFT, _inverse_args, iSTFT
 from .features.vqt import VQT
 
-__all__ = ["StreamingTransform", "StreamingPyramid", "StreamingInverse"]
+__all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "StreamingInverse"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
 _PYRAMIDS = (CQT2010v2, VQT, CQT2010)
@@ -196,6 +204,176 @@ class StreamingTransform:
         n_bins = kw["k_real"].shape[0]
         return torch.empty((self.batch, n_bins, 0) if kw["out_format"] == _C.FMT_MAGNITUDE
                            else (self.batch, n_bins, 0, 2), device=dev)
+
+
+class PoolOutput(NamedTuple):
+    """One ``StreamPool.push``: row i of ``frames`` (offline layout, batch = A, T_max frames) holds the new
+    frames of slot ``slots[i]``, ``counts[i]`` of them; frames t >= counts[i] are exact zeros.  ``slots``
+    (ascending) and ``counts`` are int64 CPU tensors."""
+    frames: torch.Tensor
+    slots: torch.Tensor
+    counts: torch.Tensor
+
+
+class StreamPool:
+    """Serve up to ``slots`` independent streams through ``module``, each advancing by its own amount.
+
+    ``push(chunk, lengths, end=None)``: ``chunk`` is a (slots, n) CUDA float32 / bfloat16 / float16 tensor and
+    slot s takes ``chunk[s, :lengths[s]]`` (``lengths``: CPU integers, 0 <= lengths[s] <= n).  ``end[s]`` (CPU
+    bools) makes this push the last of slot s's stream: it gets its remaining frames with the module's right
+    padding, as ``StreamingTransform.flush`` would give them, and takes no more samples until ``reset([s])``.
+    Returns a ``PoolOutput`` with a row for each slot that has new frames.  Concatenated along time, a slot's
+    rows up to their counts equal ``module(x)`` on its whole stream, bit for bit on the tensor-core routes (the
+    rules and the one CQT1992v2 exception of ``StreamingTransform``).  Every argument is checked before anything
+    is enqueued, and a push never reads the device back or synchronises.  ``module`` and ``forward_kwargs``:
+    those of ``StreamingTransform``; the pool's sample type is fixed by its first push.
+
+    A push is one C call (``_C.*_pool_forward``): the offline plan on the A slots with new frames, each row's
+    virtual clip built by the pre-pass from its own carry ring row and chunk row, the batch's clips all as long
+    as the longest; then the zeroing of each row's frames past its count and the carry of every slot that
+    received samples.  Idle slots cost nothing.  Plans that read the waveform as fp32 directly (the SIMT
+    kernels) take the concat route, as in ``StreamingTransform``.
+    """
+
+    def __init__(self, module, slots, _strict=False, **forward_kwargs):
+        slots = int(slots)
+        if slots < 1 or slots > _C.MAX_BATCH:
+            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        # module checks, the offline call's arguments and the (slots, K) fp32 carry ring: StreamingTransform's
+        self._st = st = StreamingTransform(module, slots, _strict=_strict, **forward_kwargs)
+        self.module, self.slots, self._strict = module, slots, bool(_strict)
+        self.K, self.hop, self.pad, self._reflect = st.K, st.hop, st.pad, st._reflect
+        self.ring = st.ring
+        self.received = np.zeros(slots, np.int64)  # host counters of every slot's stream
+        self.frames = np.zeros(slots, np.int64)
+        self.ended = np.zeros(slots, bool)
+        self.dtype = None
+
+    def reset(self, slots=None):
+        """Start new streams in ``slots`` (all slots by default; then the sample type is free again)."""
+        if slots is None:
+            idx = np.arange(self.slots)
+            self.dtype = None
+        else:
+            idx = np.asarray(slots.cpu() if isinstance(slots, torch.Tensor) else slots, dtype=np.int64).reshape(-1)
+            if ((idx < 0) | (idx >= self.slots)).any():
+                raise ValueError(f"slots must be in [0, {self.slots}), got {idx.tolist()}")
+        self.received[idx] = 0
+        self.frames[idx] = 0
+        self.ended[idx] = False
+
+    def _per_slot(self, v, what, integer):
+        if isinstance(v, torch.Tensor):
+            if v.device.type != "cpu":
+                raise TypeError(f"{what} must be on the CPU: reading it from {v.device} would synchronise")
+            v = v.numpy()
+        a = np.asarray(v)
+        if a.shape != (self.slots,):
+            raise ValueError(f"{what} must hold one value per slot ({self.slots}), got shape {a.shape}")
+        if integer and a.dtype != bool and np.issubdtype(a.dtype, np.integer):
+            return a.astype(np.int64)
+        if not integer and (a.dtype == bool or (np.issubdtype(a.dtype, np.integer) and np.isin(a, (0, 1)).all())):
+            return a.astype(bool)
+        raise TypeError(f"{what} must be {'integers' if integer else 'bools'}, got {a.dtype}")
+
+    # ------------------------------------------------------------------------------------------------ #
+    def push(self, chunk: torch.Tensor, lengths, end=None) -> PoolOutput:
+        """Append ``chunk[s, :lengths[s]]`` to every slot s, end the slots flagged in ``end``; returns the new
+        frames of the slots that have some."""
+        if not isinstance(chunk, torch.Tensor):
+            raise TypeError("chunk must be a torch.Tensor")
+        if chunk.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+        if chunk.dim() != 2 or chunk.shape[0] != self.slots:
+            raise ValueError(f"chunk must be ({self.slots}, n), got {tuple(chunk.shape)}")
+        if chunk.dtype not in _C._WAVE_DTYPES:
+            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
+        if self.dtype is not None and chunk.dtype != self.dtype:
+            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within the pool")
+        n = chunk.shape[1]
+        lengths = self._per_slot(lengths, "lengths", True)
+        end = np.zeros(self.slots, bool) if end is None else self._per_slot(end, "end", False)
+        bad = np.flatnonzero((lengths < 0) | (lengths > n))
+        if len(bad):
+            raise ValueError(f"lengths must be in [0, {n}] (the chunk width): slot {bad[0]} has {lengths[bad[0]]}")
+        bad = np.flatnonzero(self.ended & ((lengths > 0) | end))
+        if len(bad):
+            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
+        # every lane's counters and frame count, by the rules of StreamingTransform (push / flush)
+        active = np.flatnonzero((lengths > 0) | end)
+        K, hop, pad = self.K, self.hop, self.pad
+        count = np.zeros(len(active), np.int64)
+        n_carry = np.zeros(len(active), np.int64)
+        for j, s in enumerate(active.tolist()):
+            R, F0 = int(self.received[s]), int(self.frames[s])
+            total = R + int(lengths[s])
+            if end[s]:
+                try:
+                    self._st._check_length(total)  # the exception module(x) raises for a stream this short
+                except Exception as e:
+                    raise type(e)(f"slot {s}: {e}") from None
+                count[j] = (total + 2 * pad - K) // hop + 1 - F0
+            else:
+                count[j] = _ready_frames(total, K, hop, pad, self._reflect) - F0
+            n_carry[j] = R - _carry_start(R, F0, hop, pad)
+        if self.dtype is None:
+            self.dtype = chunk.dtype
+        order = np.lexsort((active, count == 0))  # the lanes with frames first, slots ascending in each group
+        active, count, n_carry = active[order], count[order], n_carry[order]
+        A = int((count > 0).sum())
+        T_max = int(count.max()) if A else 0
+        lanes = np.stack([active, self.received[active], n_carry, self.frames[active], lengths[active],
+                          end[active].astype(np.int64)], 1).astype(np.int64)
+        out = self._advance(chunk, lanes, A, T_max, count)
+        self.received[active] += lengths[active]
+        self.frames[active] += count
+        self.ended[active] |= end[active]
+        return PoolOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
+
+    # ------------------------------------------------------------------------------------------------ #
+    def _advance(self, chunk, lanes, A, T_max, count):
+        name, kw = self._st._args()
+        out = getattr(_C, name.replace("_forward", "_pool_forward"))(self, lanes, chunk, A, T_max, **kw)
+        if out is None:
+            if self._strict:
+                raise RuntimeError(f"{name}: no fused pool route for this configuration (NNAB_EUNSUPPORTED)")
+            out = self._concat_route(chunk, lanes, A, T_max, count, name, kw)
+        return out
+
+    def _concat_route(self, chunk, lanes, A, T_max, count, name, kw):
+        """The push on the module's offline call: every row's virtual clip gathered with torch from its ring
+        row and chunk row (one index gather), framed with center=False, the frames past each row's count
+        zeroed; then the carry ring update."""
+        K, hop, pad, dev = self.K, self.hop, self.pad, self.ring.device
+        x = chunk.float() if chunk.shape[1] > 0 else self.ring[:, :0]
+        out = self._st._empty(name, kw)[:0]
+        if A > 0:
+            lt = torch.as_tensor(lanes[:A]).to(dev)
+            slot, R, frm, end = lt[:, 0:1], lt[:, 1:2], lt[:, 3:4], lt[:, 5:6] > 0
+            total = R + lt[:, 4:5]
+            Lv = (T_max - 1) * hop + K
+            r = frm * hop - pad + torch.arange(Lv, device=dev)[None]
+            if self._reflect:
+                r = torch.where(r < 0, -r, r)
+                r = torch.where(end & (r >= total) & (r < total + pad), 2 * (total - 1) - r, r)
+            live = (r >= 0) & (r < total)
+            src = torch.cat([self.ring[slot[:, 0]], x[slot[:, 0]]], 1)  # (A, K + n): ring row, then chunk row
+            idx = torch.where(r < R, r.remainder(K), K + r - R).clamp(0, src.shape[1] - 1)
+            v = torch.where(live, torch.gather(src, 1, idx), torch.zeros((), device=dev))
+            out = getattr(_C, name)(v, **dict(kw, center=False))
+            keep = torch.arange(T_max, device=dev)[None] < torch.as_tensor(count[:A]).to(dev)[:, None]
+            keep = keep[:, None, :, None] if out.dim() == 4 else keep[:, None, :]
+            out = out.masked_fill(~keep, 0.0)
+        rows, raw, pos = [np.zeros(0, np.int64)], [np.zeros(0, np.int64)], [np.zeros(0, np.int64)]
+        for (s, R, _, F0, m, _), T in zip(lanes.tolist(), count.tolist()):
+            r = np.arange(max(_carry_start(R + m, F0 + T, hop, pad), R), R + m)  # what the slot's ring keeps
+            rows.append(np.full(len(r), s))
+            raw.append(r)
+            pos.append(r - R)
+        rows, raw, pos = (torch.as_tensor(np.concatenate(a)).to(dev) for a in (rows, raw, pos))
+        if rows.numel():
+            self.ring[rows, raw.remainder(K)] = x[rows, pos]
+        return out
 
 
 def _check_chunk(st, chunk):
