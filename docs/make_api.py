@@ -46,6 +46,10 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   a `PoolOutput(frames, slots, counts)` with a row for each slot that has new frames; `reset(slots)` starts new
   streams in some slots while the others carry on.  Each slot's rows equal `module(x)` on its own stream, with the
   rules of `StreamingTransform`.
+  `InversePool(istft_module, slots, onesided=None)` does the same for the inverse STFT: `push(X, slots, counts,
+  end=None, length=None)` appends `X[r, :, :counts[r]]` to slot `slots[r]`, ends the flagged slots with the
+  `StreamingInverse.flush` rules and returns an `InverseOutput(samples, slots, counts)`; a `PoolOutput` of
+  `StreamPool` feeds it as is.  Each slot's samples equal `StreamingInverse` on its own frames, to fp32 rounding.
   `StreamingPyramid(module, batch)` streams the CQT pyramid of `CQT2010v2` / `VQT` / `CQT2010` bit for bit on the
   whole-clip call's tensor-core plan (DESIGN.md §3.10).
 

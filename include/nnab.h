@@ -523,6 +523,39 @@ int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const
                              int flush, int64_t length, float* out, int64_t out_len, void* workspace,
                              size_t ws_bytes, void* stream);
 
+/* Inverse STFT pools: `slots` independent streamed inverse STFTs that advance by their own frame counts
+ * (DESIGN.md §3.10 "Inverse pools").  nnab_istft_chunk_forward's arguments with the counters, flush and length
+ * moved into a lane table:
+ *   state     DEVICE fp32, nnab_chunk_state_bytes(slots, n_fft) bytes; row s holds slot s's open partial sums
+ *   lanes, d_lanes   the same n_lanes lanes, a HOST copy the library checks and a DEVICE copy the kernels read
+ *             (the caller keeps both alive until the call's work has run).  One lane per slot that receives
+ *             frames or ends in this push: its counters before the push (frames, emitted: as for
+ *             *_chunk_forward), `row` = its row of X (-1: no new frames), T its new frames X[row, :, :T], end = 1
+ *             on its last push and `length` (< 0: None; read only where end is set).  The A lanes that return
+ *             samples come first, then the others; slots ascend within each group and appear once.
+ *   X         (R, f_in, t, 2) fp32 frames, rows distinct between lanes; frames past a lane's T are never read
+ *   A, n_max, T_max   lanes that return samples, the most samples one of them returns, the most frames one
+ *             lane brings
+ * out is (A, n_max): row i holds lane i's new samples, those nnab_istft_chunk_forward returns for the same
+ * counters and frames, then exact zeros.  NNAB_EINVAL for counters no stream has (by the rules of
+ * nnab_istft_chunk_forward, flush without any frame and a length shorter than the samples already returned
+ * included), a slot out of range / repeated / out of order, a row out of range / repeated / not -1 exactly
+ * when T = 0, T > t, an A, n_max or T_max that disagrees with the lanes, or a lane with nothing to do; all
+ * checks run before anything is enqueued.  A push is one seed launch (the carried sums of every lane), the
+ * FMT_OLA pre-pass and GEMM once over n_lanes x T_max frames, and one finalize launch (samples, zeros, carry);
+ * idle slots cost nothing.  After the call the caller advances each lane's counters as for
+ * *_chunk_forward.  The workspace query is 0 when n_lanes is 0, else
+ * nnab_istft_workspace_bytes(n_lanes, f_in, max(T_max, 1), n_fft, hop) plus the overlap-add rows' lead of n_fft
+ * positions: n_lanes rows of n_fft floats, each rounded up to 8 floats, the total to 256 bytes. */
+typedef struct nnab_istft_lane {
+  int64_t slot, row, frames, emitted, T, end, length;
+} nnab_istft_lane;
+size_t nnab_istft_pool_workspace_bytes(int64_t n_lanes, int f_in, int64_t T_max, int n_fft, int hop);
+int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nnab_istft_lane* d_lanes,
+                            int64_t n_lanes, int64_t A, int64_t slots, const float* X, int64_t R, int f_in, int64_t t,
+                            const void* packed, const float* window, int n_fft, int hop, int center, float* out,
+                            int64_t n_max, int64_t T_max, void* workspace, size_t ws_bytes, void* stream);
+
 /* Kernel launches issued by this library since load (process wide; used by
  * bench.py for its `gpu_launches` claim). */
 uint64_t nnab_launch_count(void);

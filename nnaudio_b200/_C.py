@@ -150,6 +150,10 @@ SIGNATURES["nnab_istft_chunk_workspace_bytes"] = SIGNATURES["nnab_istft_workspac
 SIGNATURES["nnab_istft_chunk_forward"] = (
     c_int, [_P, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, c_int, c_int64, _P,
             c_int64, _P, c_size_t, _P])
+SIGNATURES["nnab_istft_pool_workspace_bytes"] = SIGNATURES["nnab_istft_workspace_bytes"]
+SIGNATURES["nnab_istft_pool_forward"] = (
+    c_int, [_P, _P, _P, c_int64, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, _P,
+            c_int64, c_int64, _P, c_size_t, _P])
 
 _lib = None
 
@@ -683,10 +687,14 @@ LANE_FIELDS = ("slot", "received", "n_carry", "frames", "n", "end")
 def _pool_lanes(pool, lanes):
     """Host and device copies of a lane table: the host copy in pinned memory, the device copy made from it
     without blocking (torch's host allocator keeps the pinned block until the copy has run)."""
+    return _lane_copies(lanes, pool.ring.device)
+
+
+def _lane_copies(lanes, device):
     if len(lanes) == 0:
         return None, None
     host = torch.as_tensor(lanes, dtype=torch.int64).contiguous().pin_memory()
-    return host, host.to(pool.ring.device, non_blocking=True)
+    return host, host.to(device, non_blocking=True)
 
 
 def stft_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format,
@@ -826,6 +834,33 @@ def istft_chunk_forward(st, X, flush, length, n_out, packed, window, n_fft, hop,
                                         -1 if length is None else int(length), _ptr(out), n_out, _ptr(ws), wsb,
                                         _stream(dev))
     _check(rc, "nnab_istft_chunk_forward")
+    return out
+
+
+ISTFT_LANE_FIELDS = ("slot", "row", "frames", "emitted", "T", "end", "length")
+
+
+def istft_pool_forward(pool, lanes, X, A, n_max, T_max, packed, window, n_fft, hop, center):
+    """One push of an inverse STFT pool (nnaudio_b200.streaming.InversePool): ``lanes`` is the push's (n_lanes, 7)
+    int64 table of nnab_istft_lane rows (the A lanes with samples first), X the (R, f_in, t, 2) fp32 CUDA frames.
+    ``pool`` carries the device state ``pool.state`` (one row per slot) and ``pool.slots``.  Returns the (A, n_max)
+    samples, zeros past each row's count."""
+    L = lib()
+    dev = pool.state.device
+    out = torch.empty((A, n_max), dtype=torch.float32, device=dev)
+    if len(lanes) == 0:
+        return out
+    X = _dev_f32(X, "X")
+    X = X if X.is_contiguous() else X.contiguous()
+    R, f_in, t, _ = X.shape
+    with torch.cuda.device(dev):
+        hl, dl = _lane_copies(lanes, dev)
+        ws, wsb = _workspace(L.nnab_istft_pool_workspace_bytes(len(lanes), f_in, T_max, n_fft, hop), dev)
+        rc = L.nnab_istft_pool_forward(
+            _ptr(pool.state), _ptr(hl), _ptr(dl), len(lanes), A, pool.slots, _ptr(X) if X.numel() else None, R,
+            f_in, t, _ptr(packed), _ptr(window), n_fft, hop, int(center), _ptr(out) if out.numel() else None, n_max,
+            T_max, _ptr(ws), wsb, _stream(dev))
+    _check(rc, "nnab_istft_pool_forward")
     return out
 
 

@@ -180,6 +180,67 @@ __host__ __device__ inline int64_t lane_frames_after(const nnab_stream_lane& ln,
   return ln.end ? chunk_end_frames(total, K, hop, pad) : chunk_ready_frames(total, K, hop, pad, pad_mode);
 }
 
+// ---- the counters of one streamed inverse STFT (DESIGN §3.10), shared by the host checks and the pool kernels
+// Overlap-add positions s (pad-cropped output sample s - offset).  After n frames, positions below n * hop are
+// final; the output can still end as early as istft_end_min(n) (length None).
+__host__ __device__ inline int64_t istft_end_min(int64_t n, int n_fft, int hop, int center) {
+  const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
+  return center ? ola_len - n_fft / 2 : ola_len;
+}
+
+struct IstftChunkPlan {
+  int64_t origin;      // first position the push's overlap-add buffer holds (= first carried position)
+  int64_t carried;     // positions carried in: [origin, origin + carried)
+  int64_t buf_len;     // positions the push's buffer holds
+  int64_t emit_begin, emit_end;
+  int64_t carry_begin, carry_len;  // carried out
+};
+
+// Host counters: `frames` frames pushed so far, `emitted` output samples returned.  EINVAL for counters no
+// stream has, or a `length` shorter than what was returned.
+__host__ __device__ inline int istft_chunk_plan(int64_t frames, int64_t emitted, int64_t T, int n_fft, int hop,
+                                                int center, int flush, int64_t length, IstftChunkPlan* o) {
+  if (frames < 0 || emitted < 0 || T < 0 || n_fft <= 0 || hop <= 0 || hop > n_fft) return NNAB_EINVAL;
+  const int64_t offset = center ? n_fft / 2 : 0;
+  auto emitted_end = [&](int64_t n) {  // end of the positions returned by the pushes of n frames
+    if (n <= 0) return offset;
+    const int64_t e = n * hop < istft_end_min(n, n_fft, hop, center) ? n * hop : istft_end_min(n, n_fft, hop, center);
+    return e > offset ? e : offset;
+  };
+  const int64_t E = emitted_end(frames);
+  if (offset + emitted != E) return NNAB_EINVAL;
+  const int64_t n = frames + T;
+  if (flush && n <= 0) return NNAB_EINVAL;
+  o->origin = frames > 0 ? (E < frames * hop ? E : frames * hop) : 0;
+  o->carried = frames > 0 ? (frames - 1) * (int64_t)hop + n_fft - o->origin : 0;
+  o->buf_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - o->origin : 0;
+  o->emit_begin = E;
+  if (flush) {
+    const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
+    int64_t want = length >= 0 ? length : (center ? ola_len - 2 * offset : ola_len);
+    if (offset + want > ola_len) want = ola_len - offset;  // slicing past the end just truncates
+    if (want < 0) want = 0;
+    if (offset + want < E) return NNAB_EINVAL;  // shorter than the samples already returned
+    o->emit_end = offset + want;
+    o->carry_begin = o->carry_len = 0;
+  } else {
+    o->emit_end = emitted_end(n);
+    const int64_t c = n > 0 ? (o->emit_end < n * hop ? o->emit_end : n * hop) : 0;
+    o->carry_begin = c;
+    o->carry_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - c : 0;
+  }
+  if (o->carried > n_fft || o->carry_len > n_fft) return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+// A lane's plan on the device (the library has checked the lane on the host with the same function).
+__host__ __device__ inline IstftChunkPlan istft_lane_plan(const nnab_istft_lane& ln, int n_fft, int hop,
+                                                          int center) {
+  IstftChunkPlan pl{};
+  istft_chunk_plan(ln.frames, ln.emitted, ln.T, n_fft, hop, center, (int)ln.end, ln.end ? ln.length : -1, &pl);
+  return pl;
+}
+
 struct FramedProblem {
   const void* x;       // (B, L) rows, pitch x_pitch samples of type x_dtype
   int x_dtype;         // NNAB_DTYPE_*: only the pad / split pre-pass reads 16-bit samples, the SIMT kernel fp32
@@ -286,6 +347,18 @@ int tc_istft_finalize(const float* ola, int64_t ola_pitch, int64_t B, const floa
 int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window, int n_fft,
                             int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
                             int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream);
+// inverse STFT pools (DEVICE lane table `lanes`): row i of the (n_lanes, ola_pitch) overlap-add buffer holds
+// lane i's positions from frames_i * hop - lead.  Seed: every row's carried sums from its state row, zeros
+// elsewhere.  Prep: plane row i * T_max + t from X[row_i, :, t] of the (R, f_in, x_T, 2) frames for t < T_i, zeros
+// past T_i and for row_i = -1.  Finalize: rows i < A of out (A, n_max) get lane i's final samples then zeros;
+// every lane's open tail goes to its state row.
+int tc_istft_pool_seed(const nnab_istft_lane* lanes, int64_t n_lanes, const float* state, int n_fft, int hop,
+                       int center, int64_t lead, float* ola, int64_t ola_pitch, cudaStream_t stream);
+int tc_istft_pool_prep(const float* X, const nnab_istft_lane* lanes, int64_t n_lanes, int f_in, int64_t T_max,
+                       int64_t x_T, void* planes, cudaStream_t stream);
+int tc_istft_pool_finalize(const nnab_istft_lane* lanes, int64_t n_lanes, int64_t A, const float* ola,
+                           int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop, int center,
+                           float* out, int64_t n_max, float* state, cudaStream_t stream);
 size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K);
 // block-partial kernel (tcb_kernels.cu): default N-tile geometry of an (n_fft, hop) transform (nb packed
 // columns per tile, nb - 2 new bins each, `phases` families per tile: 1, or 4 when hop % 128 == 0) -- the column

@@ -321,58 +321,7 @@ static int chunk_forward(const ChunkPlan& cp, int chunk_dtype, int64_t B, Run&& 
   return tc_chunk_carry(cp.cs, chunk_dtype, B, cp.from, (cudaStream_t)stream);
 }
 
-// ---- streamed inverse STFT -----------------------------------------------------------------------
-// Overlap-add positions s (pad-cropped output sample s - offset).  After n frames, positions below n * hop are
-// final; the output can still end as early as istft_end_min(n) (length None).
-static int64_t istft_end_min(int64_t n, int n_fft, int hop, int center) {
-  const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
-  return center ? ola_len - n_fft / 2 : ola_len;
-}
-
-struct IstftChunkPlan {
-  int64_t origin;      // first position the push's overlap-add buffer holds (= first carried position)
-  int64_t carried;     // positions carried in: [origin, origin + carried)
-  int64_t buf_len;     // positions the push's buffer holds
-  int64_t emit_begin, emit_end;
-  int64_t carry_begin, carry_len;  // carried out
-};
-
-// Host counters: `frames` frames pushed so far, `emitted` output samples returned.  EINVAL for counters no
-// stream has, or a `length` shorter than what was returned.
-static int istft_chunk_plan(int64_t frames, int64_t emitted, int64_t T, int n_fft, int hop, int center, int flush,
-                            int64_t length, IstftChunkPlan* o) {
-  if (frames < 0 || emitted < 0 || T < 0 || n_fft <= 0 || hop <= 0 || hop > n_fft) return NNAB_EINVAL;
-  const int64_t offset = center ? n_fft / 2 : 0;
-  auto emitted_end = [&](int64_t n) {  // end of the positions returned by the pushes of n frames
-    if (n <= 0) return offset;
-    const int64_t e = n * hop < istft_end_min(n, n_fft, hop, center) ? n * hop : istft_end_min(n, n_fft, hop, center);
-    return e > offset ? e : offset;
-  };
-  const int64_t E = emitted_end(frames);
-  if (offset + emitted != E) return NNAB_EINVAL;
-  const int64_t n = frames + T;
-  if (flush && n <= 0) return NNAB_EINVAL;
-  o->origin = frames > 0 ? (E < frames * hop ? E : frames * hop) : 0;
-  o->carried = frames > 0 ? (frames - 1) * (int64_t)hop + n_fft - o->origin : 0;
-  o->buf_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - o->origin : 0;
-  o->emit_begin = E;
-  if (flush) {
-    const int64_t ola_len = n_fft + (int64_t)hop * (n - 1);
-    int64_t want = length >= 0 ? length : (center ? ola_len - 2 * offset : ola_len);
-    if (offset + want > ola_len) want = ola_len - offset;  // slicing past the end just truncates
-    if (want < 0) want = 0;
-    if (offset + want < E) return NNAB_EINVAL;  // shorter than the samples already returned
-    o->emit_end = offset + want;
-    o->carry_begin = o->carry_len = 0;
-  } else {
-    o->emit_end = emitted_end(n);
-    const int64_t c = n > 0 ? (o->emit_end < n * hop ? o->emit_end : n * hop) : 0;
-    o->carry_begin = c;
-    o->carry_len = n > 0 ? (n - 1) * (int64_t)hop + n_fft - c : 0;
-  }
-  if (o->carried > n_fft || o->carry_len > n_fft) return NNAB_EINVAL;
-  return NNAB_OK;
-}
+// ---- streamed inverse STFT: istft_chunk_plan (common.cuh) ------------------------------------------
 
 }  // namespace nnab
 
@@ -1973,6 +1922,94 @@ int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const
   // 3. final samples / window sum-square at their global positions, the open tail into the carry
   return tc_istft_chunk_finalize(ola, ola_pitch, B, window, n_fft, hop, frames + T, pl.origin, pl.emit_begin, out,
                                  n_out, pl.carry_begin, pl.carry_len, carry, s);
+}
+
+// ---- inverse STFT pools (DESIGN §3.10 "Inverse pools") ---------------------------------------------------
+// Row i of a push's overlap-add buffer starts `lead` = n_fft positions before lane i's first new frame, so the
+// carried sums (at most n_fft / 2 before it) fit and the new frames of every lane start at column `lead`.
+static int64_t istft_pool_ola_pitch(int64_t T_max, int n_fft, int hop) {
+  const int64_t T = T_max > 0 ? T_max : 1;
+  return (int64_t)align_up((size_t)(2 * (int64_t)n_fft + (int64_t)hop * (T - 1)), 8);
+}
+
+size_t nnab_istft_pool_workspace_bytes(int64_t n_lanes, int f_in, int64_t T_max, int n_fft, int hop) {
+  if (n_lanes <= 0) return 0;
+  return nnab_istft_workspace_bytes(n_lanes, f_in, T_max > 0 ? T_max : 1, n_fft, hop) +
+         align_up((size_t)n_lanes * align_up((size_t)n_fft, 8) * sizeof(float), 256);
+}
+
+int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nnab_istft_lane* d_lanes,
+                            int64_t n_lanes, int64_t A, int64_t slots, const float* X, int64_t R, int f_in, int64_t t,
+                            const void* packed, const float* window, int n_fft, int hop, int center, float* out,
+                            int64_t n_max, int64_t T_max, void* workspace, size_t ws_bytes, void* stream) {
+  if (state == nullptr || packed == nullptr || window == nullptr || slots < 1 || slots > 65535 || n_lanes < 0 ||
+      n_lanes > slots || A < 0 || A > n_lanes || R < 0 || t < 0 || f_in <= 0 || n_max < 0 || T_max < 0 ||
+      (n_lanes > 0 && (lanes == nullptr || d_lanes == nullptr)))
+    return NNAB_EINVAL;
+  // every lane by istft_chunk_plan, then the table's order, rows and totals, before anything runs
+  std::vector<uint8_t> seen((size_t)slots, 0), used((size_t)R, 0);
+  int64_t n_most = 0, t_most = 0;
+  for (int64_t i = 0; i < n_lanes; ++i) {
+    const nnab_istft_lane& ln = lanes[i];
+    if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
+    if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
+    seen[(size_t)ln.slot] = 1;
+    if (ln.T < 0 || ln.T > t || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
+    if ((ln.row < 0) != (ln.T == 0)) return NNAB_EINVAL;  // a row exactly for the lanes with frames
+    if (ln.row >= 0) {
+      if (ln.row >= R || used[(size_t)ln.row]) return NNAB_EINVAL;
+      used[(size_t)ln.row] = 1;
+    }
+    if (ln.T == 0 && !ln.end) return NNAB_EINVAL;  // a lane with nothing to do
+    IstftChunkPlan pl;
+    const int rc = istft_chunk_plan(ln.frames, ln.emitted, ln.T, n_fft, hop, center, (int)ln.end,
+                                    ln.end ? ln.length : -1, &pl);
+    if (rc) return rc;
+    const int64_t n_out = pl.emit_end - pl.emit_begin;
+    if ((i < A) != (n_out > 0)) return NNAB_EINVAL;  // the A lanes with samples come first
+    if (n_out > n_most) n_most = n_out;
+    if (ln.T > t_most) t_most = ln.T;
+  }
+  if (n_most != n_max || t_most != T_max) return NNAB_EINVAL;
+  if ((t_most > 0 && X == nullptr) || (A > 0 && out == nullptr)) return NNAB_EINVAL;
+  int rc = check_arch();
+  if (rc) return rc;
+  const size_t need = nnab_istft_pool_workspace_bytes(n_lanes, f_in, T_max, n_fft, hop);
+  if (n_lanes > 0 && (workspace == nullptr || ws_bytes < need)) return NNAB_EWORKSPACE;
+  if (n_lanes == 0) return NNAB_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  float* carry = static_cast<float*>(state);
+
+  // nnab_istft_forward's layout for n_lanes x max(T_max, 1) frames, each row `lead` positions longer
+  const int64_t lead = n_fft;
+  const int64_t ola_pitch = istft_pool_ola_pitch(T_max, n_fft, hop);
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  void* planes = ws;
+  const size_t planes_b = align_up(tc_istft_planes_bytes(n_lanes, T_max > 0 ? T_max : 1, f_in), 256);
+  const size_t ola_b = align_up((size_t)n_lanes * ola_pitch * sizeof(float), 256);
+  float* ola = (float*)(ws + planes_b);
+  float* scale = (float*)(ws + planes_b + ola_b);
+
+  // 1. every row: its carried sums where they lie, zeros elsewhere
+  if ((rc = tc_istft_pool_seed(d_lanes, n_lanes, carry, n_fft, hop, center, lead, ola, ola_pitch, s))) return rc;
+  // 2. the new frames of every lane, overlap-added from column `lead` (one FMT_OLA GEMM over n_lanes x T_max)
+  if (T_max > 0) {
+    if ((rc = tc_istft_pool_prep(X, d_lanes, n_lanes, f_in, T_max, t, planes, s))) return rc;
+    istft_scale_kernel<<<(n_fft + 255) / 256, 256, 0, s>>>(window, 1.0f / (float)n_fft, n_fft, scale);
+    NNAB_LAUNCH_CHECK();
+    const int kpad = tc_istft_k(f_in);
+    FramedProblem p{};
+    p.x = nullptr; p.B = n_lanes; p.L = T_max * (int64_t)kpad; p.x_pitch = 0;
+    p.F = n_fft; p.K = kpad; p.hop = kpad; p.pad = 0; p.pad_mode = NNAB_PAD_CONSTANT;
+    p.scale = scale; p.scale_all = 1.f; p.fmt = FMT_OLA; p.eps = 0.f; p.power = 1.f;
+    p.out = ola + lead; p.T = T_max; p.out_bins = n_fft; p.bin_offset = 0;
+    p.presplit = planes;
+    p.ola_pitch = ola_pitch; p.ola_hop = hop;
+    if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
+  }
+  // 3. every lane's final samples / window sum-square (rows i < A of out, zeros up to n_max), its tail carried
+  return tc_istft_pool_finalize(d_lanes, n_lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center, out, n_max,
+                                carry, s);
 }
 
 // ------------------------------------------------------------- input gradient ----

@@ -608,20 +608,32 @@ size_t tc_istft_planes_bytes(int64_t B, int64_t T, int f_in) {
 }
 
 // X (B, F, T, 2) fp32 -> A planes: row g = b*T + t, column part*F + f (K-major), bf16 hi/lo.
+// LANES (inverse STFT pools): plane row b*T + t comes from X[lanes[b].row, :, t] of (R, F, x_T, 2) frames for
+// t < lanes[b].T, and is zeros past it and for row -1 (frames past a lane's count are never read: NaN * 0 is NaN).
+template <bool LANES>
 __global__ void __launch_bounds__(256) istft_prep_kernel(const float* __restrict__ X, int f_in,
                                                          int64_t T, int kpad, int64_t plane_stride,
-                                                         __nv_bfloat16* __restrict__ planes) {
+                                                         __nv_bfloat16* __restrict__ planes,
+                                                         const nnab_istft_lane* __restrict__ lanes, int64_t x_T) {
   __shared__ float tile[2][32][33];
   const int64_t b = blockIdx.z;
   const int64_t t0 = (int64_t)blockIdx.x * 32;
   const int f0 = blockIdx.y * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8
   const float* __restrict__ Xb = X + b * (int64_t)f_in * T * 2;
+  int64_t t_read = T;  // frames of this row that X holds
+  if constexpr (LANES) {
+    const int64_t row = lanes[b].row;
+    t_read = row >= 0 ? lanes[b].T : 0;
+    Xb = X + (row >= 0 ? row : 0) * (int64_t)f_in * x_T * 2;
+  } else {
+    x_T = T;
+  }
   for (int r = ty; r < 32; r += 8) {
     const int f = f0 + r;
     const int64_t t = t0 + tx;
     float2 v = make_float2(0.f, 0.f);
-    if (f < f_in && t < T) v = *reinterpret_cast<const float2*>(Xb + ((int64_t)f * T + t) * 2);
+    if (f < f_in && t < t_read) v = *reinterpret_cast<const float2*>(Xb + ((int64_t)f * x_T + t) * 2);
     tile[0][r][tx] = v.x;
     tile[1][r][tx] = v.y;
   }
@@ -642,8 +654,9 @@ __global__ void __launch_bounds__(256) istft_prep_kernel(const float* __restrict
   }
 }
 
-int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes_v,
-                  cudaStream_t stream) {
+// The A planes of B x T frames: zeroed where istft_prep_kernel writes nothing, then that kernel's launch.
+static int launch_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes_v,
+                             const nnab_istft_lane* lanes, int64_t x_T, cudaStream_t stream) {
   if (B > 65535) return NNAB_EUNSUPPORTED;
   const int kpad = tc_istft_k(f_in);
   const SplitGeom g = split_geom(B, T * kpad, kpad, kpad, 0);
@@ -656,9 +669,22 @@ int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes_v
     if (rc) return rc;
   }
   dim3 grid((unsigned)ceil_div64(T, 32), (unsigned)((f_in + 31) / 32), (unsigned)B);
-  istft_prep_kernel<<<grid, 256, 0, stream>>>(X, f_in, T, kpad, g.plane_stride, planes);
+  if (lanes != nullptr)
+    istft_prep_kernel<true><<<grid, 256, 0, stream>>>(X, f_in, T, kpad, g.plane_stride, planes, lanes, x_T);
+  else
+    istft_prep_kernel<false><<<grid, 256, 0, stream>>>(X, f_in, T, kpad, g.plane_stride, planes, nullptr, T);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
+}
+
+int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes_v,
+                  cudaStream_t stream) {
+  return launch_istft_prep(X, B, f_in, T, planes_v, nullptr, T, stream);
+}
+
+int tc_istft_pool_prep(const float* X, const nnab_istft_lane* lanes, int64_t n_lanes, int f_in, int64_t T_max,
+                       int64_t x_T, void* planes, cudaStream_t stream) {
+  return launch_istft_prep(X, n_lanes, f_in, T_max, planes, lanes, x_T, stream);
 }
 
 // ---------------------------------------------------------------------------
@@ -789,6 +815,22 @@ int tc_unpad_adjoint(const float* gp, int64_t gp_pitch, int64_t gp_len, int64_t 
   return NNAB_OK;
 }
 
+// Window sum-square of overlap-add position s over T frames (utils.py:43-49), summed from the last frame that
+// covers s down: the one order every inverse-STFT finalize uses.
+__device__ __forceinline__ float istft_wss(const float* __restrict__ window, int n_fft, int hop, int64_t T,
+                                           int64_t s) {
+  int64_t t_hi = s / hop;
+  if (t_hi > T - 1) t_hi = T - 1;
+  float wss = 0.f;
+  for (int64_t t = t_hi; t >= 0; --t) {
+    const int64_t n = s - t * hop;
+    if (n >= n_fft) break;
+    const float w = __ldg(window + n);
+    wss = fmaf(w, w, wss);
+  }
+  return wss;
+}
+
 // Divide the overlap-added frames by the window sum-square (utils.py:43-49; only where it
 // exceeds 1e-10) and strip the centre padding: out[b, i] = ola[b, i + offset] / wss(i + offset).
 __global__ void __launch_bounds__(256) istft_finalize_kernel(const float* __restrict__ ola,
@@ -801,15 +843,7 @@ __global__ void __launch_bounds__(256) istft_finalize_kernel(const float* __rest
   const int64_t b = blockIdx.y;
   if (i >= out_len) return;
   const int64_t s = i + offset;
-  int64_t t_hi = s / hop;
-  if (t_hi > T - 1) t_hi = T - 1;
-  float wss = 0.f;
-  for (int64_t t = t_hi; t >= 0; --t) {
-    const int64_t n = s - t * hop;
-    if (n >= n_fft) break;
-    const float w = __ldg(window + n);
-    wss = fmaf(w, w, wss);
-  }
+  const float wss = istft_wss(window, n_fft, hop, T, s);
   float v = ola[b * ola_pitch + s];
   if (wss > 1e-10f) v = v / wss;
   out[b * out_len + i] = v;
@@ -841,15 +875,7 @@ __global__ void __launch_bounds__(256) istft_chunk_finalize_kernel(
   const float* __restrict__ row = ola + b * ola_pitch;
   if (i < out_len) {
     const int64_t s = emit_begin + i;
-    int64_t t_hi = s / hop;
-    if (t_hi > T - 1) t_hi = T - 1;
-    float wss = 0.f;
-    for (int64_t t = t_hi; t >= 0; --t) {
-      const int64_t n = s - t * hop;
-      if (n >= n_fft) break;
-      const float w = __ldg(window + n);
-      wss = fmaf(w, w, wss);
-    }
+    const float wss = istft_wss(window, n_fft, hop, T, s);
     float v = row[s - origin];
     if (wss > 1e-10f) v = v / wss;
     out[b * out_len + i] = v;
@@ -866,6 +892,76 @@ int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, cons
   dim3 grid((unsigned)ceil_div64(n, 256), (unsigned)B);
   istft_chunk_finalize_kernel<<<grid, 256, 0, stream>>>(ola, ola_pitch, window, n_fft, hop, T, origin, emit_begin,
                                                         out, out_len, carry_begin, carry_len, carry);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+// Inverse STFT pools.  Row i of the overlap-add buffer holds lane i's global positions from
+// frames_i * hop - lead on (lead = n_fft): its carried sums start at most hop - n_fft / 2 positions before
+// frames_i * hop (istft_chunk_plan's origin), so every lane's new frames start at column `lead` and one FMT_OLA
+// GEMM with out = ola + lead serves all rows.  The seed writes each row whole: the lane's carried sums from
+// state row slot_i where they lie, zeros elsewhere (the memset and 2-D copy of the one-stream push).
+__global__ void __launch_bounds__(256) istft_pool_seed_kernel(const nnab_istft_lane* __restrict__ lanes,
+                                                              const float* __restrict__ state, int n_fft,
+                                                              int hop, int center, int64_t lead,
+                                                              float* __restrict__ ola, int64_t ola_pitch) {
+  const nnab_istft_lane ln = lanes[blockIdx.y];
+  const IstftChunkPlan pl = istft_lane_plan(ln, n_fft, hop, center);
+  const int64_t base = ln.frames * hop - lead - pl.origin;  // column c holds carried position c + base
+  const float* __restrict__ src = state + ln.slot * n_fft;
+  float* __restrict__ row = ola + (int64_t)blockIdx.y * ola_pitch;
+  for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < ola_pitch;
+       c += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = c + base;
+    row[c] = k >= 0 && k < pl.carried ? __ldg(src + k) : 0.f;
+  }
+}
+
+// istft_chunk_finalize_kernel on every lane: rows i < A of out (A, n_max) take lane i's final samples, each
+// divided by the window sum-square of its global position over the lane's frames_i + T_i frames (istft_wss),
+// then exact zeros up to n_max; every lane's open tail goes un-normalised to its state row.
+__global__ void __launch_bounds__(256) istft_pool_finalize_kernel(
+    const nnab_istft_lane* __restrict__ lanes, int64_t A, const float* __restrict__ ola, int64_t ola_pitch,
+    int64_t lead, const float* __restrict__ window, int n_fft, int hop, int center, float* __restrict__ out,
+    int64_t n_max, float* __restrict__ state) {
+  const int64_t i = blockIdx.y;
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const nnab_istft_lane ln = lanes[i];
+  const IstftChunkPlan pl = istft_lane_plan(ln, n_fft, hop, center);
+  const float* __restrict__ row = ola + i * ola_pitch;
+  const int64_t base = ln.frames * hop - lead;  // global position of column 0
+  if (i < A && j < n_max) {
+    float v = 0.f;
+    if (j < pl.emit_end - pl.emit_begin) {
+      const int64_t s = pl.emit_begin + j;
+      const float wss = istft_wss(window, n_fft, hop, ln.frames + ln.T, s);
+      v = row[s - base];
+      if (wss > 1e-10f) v = v / wss;
+    }
+    out[i * n_max + j] = v;
+  }
+  if (j < pl.carry_len) state[ln.slot * n_fft + j] = row[pl.carry_begin - base + j];
+}
+
+int tc_istft_pool_seed(const nnab_istft_lane* lanes, int64_t n_lanes, const float* state, int n_fft, int hop,
+                       int center, int64_t lead, float* ola, int64_t ola_pitch, cudaStream_t stream) {
+  if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
+  if (n_lanes <= 0) return NNAB_OK;
+  const dim3 grid((unsigned)ceil_div64(ola_pitch, 256), (unsigned)n_lanes);
+  istft_pool_seed_kernel<<<grid, 256, 0, stream>>>(lanes, state, n_fft, hop, center, lead, ola, ola_pitch);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_istft_pool_finalize(const nnab_istft_lane* lanes, int64_t n_lanes, int64_t A, const float* ola,
+                           int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop, int center,
+                           float* out, int64_t n_max, float* state, cudaStream_t stream) {
+  if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
+  if (n_lanes <= 0) return NNAB_OK;
+  const int64_t n = n_max > n_fft ? n_max : n_fft;  // a carried tail holds at most n_fft positions
+  const dim3 grid((unsigned)ceil_div64(n, 256), (unsigned)n_lanes);
+  istft_pool_finalize_kernel<<<grid, 256, 0, stream>>>(lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center,
+                                                       out, n_max, state);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }

@@ -23,6 +23,10 @@ in some slots while the others carry on.  Each stream's frames are those of ``St
 
 ``StreamingInverse(module, batch)`` streams complex frames through the inverse STFT: each push returns the
 output samples no later frame can change, ``flush(length=None)`` the rest.
+
+``InversePool(module, slots)`` is ``StreamPool``'s counterpart for the inverse STFT: each
+``push(X, slots, counts, end, length)`` appends ``X[r, :, :counts[r]]`` to slot ``slots[r]``'s stream and ends the
+flagged slots; a ``PoolOutput`` of ``StreamPool`` feeds it as is.
 """
 from __future__ import annotations
 
@@ -40,7 +44,8 @@ from .features.mel import MFCC, MelSpectrogram
 from .features.stft import STFT, _inverse_args, iSTFT
 from .features.vqt import VQT
 
-__all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "StreamingInverse"]
+__all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "StreamingInverse", "InversePool",
+           "InverseOutput"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
 _PYRAMIDS = (CQT2010v2, VQT, CQT2010)
@@ -596,3 +601,150 @@ class StreamingInverse:
         self.frames += X.shape[2]
         self.emitted += n_out
         return out
+
+
+class InverseOutput(NamedTuple):
+    """One ``InversePool.push``: row i of ``samples`` (A, n_max) holds the new output samples of slot
+    ``slots[i]``, ``counts[i]`` of them, then exact zeros.  ``slots`` (ascending) and ``counts`` are int64 CPU
+    tensors."""
+    samples: torch.Tensor
+    slots: torch.Tensor
+    counts: torch.Tensor
+
+
+def _cpu_ints(v, what, n=None, kind="integers"):
+    """A CPU array of ints (or bools, kind="bools") of shape (n,); device tensors are refused, since reading
+    them would synchronise."""
+    if isinstance(v, torch.Tensor):
+        if v.device.type != "cpu":
+            raise TypeError(f"{what} must be on the CPU: reading it from {v.device} would synchronise")
+        v = v.numpy()
+    a = np.asarray(v)
+    if n is not None and a.shape != (n,):
+        raise ValueError(f"{what} must hold {n} values, got shape {a.shape}")
+    if a.ndim != 1:
+        raise ValueError(f"{what} must be one-dimensional, got shape {a.shape}")
+    if kind == "integers" and a.dtype != bool and (np.issubdtype(a.dtype, np.integer) or a.size == 0):
+        return a.astype(np.int64)
+    if kind == "bools" and (a.dtype == bool or (np.issubdtype(a.dtype, np.integer) and np.isin(a, (0, 1)).all())):
+        return a.astype(bool)
+    raise TypeError(f"{what} must be {kind}, got {a.dtype}")
+
+
+class InversePool:
+    """Serve up to ``slots`` independent streamed inverse STFTs, each advancing by its own frame count.
+
+    ``module`` and ``onesided``: those of ``StreamingInverse``.  ``push(X, slots, counts, end=None,
+    length=None)``: ``X`` is (R, bins, t, 2) float32 CUDA frames and row r appends ``X[r, :, :counts[r]]`` to
+    slot ``slots[r]`` (``slots``, ``counts``: R CPU integers; slots distinct, ``0 <= counts[r] <= t``; frames past
+    a count are never read).  ``end`` (``slots`` CPU bools) ends the flagged slots: they get the rest of their
+    samples under the ``StreamingInverse.flush`` rules, with ``length[s]`` (``slots`` CPU integers, -1: None; read
+    only where ``end`` is set), and take no more frames until ``reset([s])``.  A ``PoolOutput`` of
+    ``StreamPool`` and the ``end`` given to it can be passed on as they are.  Returns an ``InverseOutput`` with a
+    row for each slot that has new samples.  Concatenated, a slot's rows up to their counts equal
+    ``StreamingInverse`` on the same packets and ``module(X_s)`` / ``module.inverse(X_s)`` on all its frames, to
+    fp32 rounding (every overlap-add uses fp32 atomics).  Every argument is checked before anything is enqueued,
+    and a push never reads the device back or synchronises.
+
+    A push is one C call (``_C.istft_pool_forward``): a seed launch (every lane's carried sums), the offline
+    pre-pass and FMT_OLA GEMM once over all lanes' frames, and one finalize launch; idle slots cost nothing.
+    """
+
+    def __init__(self, module, slots, onesided=None):
+        slots = int(slots)
+        if slots < 1 or slots > _C.MAX_BATCH:
+            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        # module checks, the inverse arguments and the (slots, n_fft) fp32 state: StreamingInverse's
+        self._si = si = StreamingInverse(module, slots, onesided=onesided)
+        self.module, self.slots, self.onesided = module, slots, si.onesided
+        self.n_fft, self.hop, self.center, self.f_in, self.offset = si.n_fft, si.hop, si.center, si.f_in, si.offset
+        self.state = si.state  # row s: slot s's open overlap-add sums
+        self.frames = np.zeros(slots, np.int64)  # host counters of every slot's stream
+        self.emitted = np.zeros(slots, np.int64)
+        self.ended = np.zeros(slots, bool)
+
+    def reset(self, slots=None):
+        """Start new streams in ``slots`` (all slots by default)."""
+        idx = np.arange(self.slots) if slots is None else _cpu_ints(
+            np.reshape(slots.cpu() if isinstance(slots, torch.Tensor) else slots, -1), "slots")
+        if ((idx < 0) | (idx >= self.slots)).any():
+            raise ValueError(f"slots must be in [0, {self.slots}), got {idx.tolist()}")
+        self.frames[idx] = 0
+        self.emitted[idx] = 0
+        self.ended[idx] = False
+
+    def _emit_end(self, n):
+        """``StreamingInverse._emit_end`` over an array of frame counts."""
+        end_min = self.n_fft + self.hop * (n - 1) - self.offset
+        return np.where(n <= 0, self.offset, np.maximum(self.offset, np.minimum(n * self.hop, end_min)))
+
+    def _flush_end(self, n, length):
+        """End position of the output after n frames under ``StreamingInverse.flush(length)`` (length < 0:
+        None), over arrays."""
+        ola_len = self.n_fft + self.hop * (n - 1)
+        want = np.where(length >= 0, length, ola_len - 2 * self.offset)
+        return self.offset + np.clip(want, 0, np.maximum(ola_len - self.offset, 0))
+
+    # ------------------------------------------------------------------------------------------------ #
+    def push(self, X: torch.Tensor, slots, counts, end=None, length=None) -> InverseOutput:
+        """Append ``X[r, :, :counts[r]]`` to slot ``slots[r]`` for every row r, end the slots flagged in ``end``;
+        returns the new samples of the slots that have some."""
+        if not isinstance(X, torch.Tensor):
+            raise TypeError("X must be a torch.Tensor")
+        if X.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the frames require grad")
+        if X.dim() != 4 or X.shape[1] != self.f_in or X.shape[3] != 2:
+            raise ValueError(f"frames must be (rows, {self.f_in}, t, 2), got {tuple(X.shape)}")
+        if X.dtype != torch.float32:
+            raise ValueError(f"frames must be float32, got {X.dtype}")
+        R, t = X.shape[0], X.shape[2]
+        rows_slot = _cpu_ints(slots, "slots", R)
+        rows_count = _cpu_ints(counts, "counts", R)
+        end = np.zeros(self.slots, bool) if end is None else _cpu_ints(end, "end", self.slots, "bools")
+        length = np.full(self.slots, -1, np.int64) if length is None else _cpu_ints(length, "length", self.slots)
+        bad = np.flatnonzero((rows_slot < 0) | (rows_slot >= self.slots))
+        if len(bad):
+            raise ValueError(f"slots must be in [0, {self.slots}): row {bad[0]} has slot {rows_slot[bad[0]]}")
+        uniq, first = np.unique(rows_slot, return_counts=True)
+        if (first > 1).any():
+            raise ValueError(f"slot {uniq[first > 1][0]} appears in more than one row")
+        bad = np.flatnonzero((rows_count < 0) | (rows_count > t))
+        if len(bad):
+            raise ValueError(f"counts must be in [0, {t}] (the frames of X): slot {rows_slot[bad[0]]} has "
+                             f"{rows_count[bad[0]]}")
+        T = np.zeros(self.slots, np.int64)  # new frames and their row of X, per slot
+        row = np.full(self.slots, -1, np.int64)
+        T[rows_slot] = rows_count
+        row[rows_slot] = np.arange(R)
+        row[T == 0] = -1
+        bad = np.flatnonzero(self.ended & ((T > 0) | end))
+        if len(bad):
+            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
+        n = self.frames + T
+        bad = np.flatnonzero(end & (n == 0))
+        if len(bad):
+            raise RuntimeError(f"slot {bad[0]}: ending a stream without frames; the inverse STFT needs at least one")
+        # every slot's output end after the push, by the rules of StreamingInverse (push / flush)
+        emit_end = np.where(end, self._flush_end(n, length), self._emit_end(n))
+        count = emit_end - (self.offset + self.emitted)
+        bad = np.flatnonzero(end & (count < 0))
+        if len(bad):
+            s = bad[0]
+            raise ValueError(f"slot {s}: length {length[s]} is shorter than the {self.emitted[s]} samples already "
+                             "returned")
+        active = np.flatnonzero((T > 0) | end)
+        order = np.lexsort((active, count[active] == 0))  # lanes with samples first, slots ascending in each group
+        active = active[order]
+        count = count[active]
+        A = int((count > 0).sum())
+        n_max = int(count.max()) if A else 0
+        T_max = int(T[active].max()) if len(active) else 0
+        lanes = np.stack([active, row[active], self.frames[active], self.emitted[active], T[active],
+                          end[active].astype(np.int64), np.where(end[active], length[active], -1)], 1)
+        _, _, packed, win = self._si._args()
+        out = _C.istft_pool_forward(self, lanes.astype(np.int64), X, A, n_max, T_max, packed, win, self.n_fft,
+                                    self.hop, self.center)
+        self.frames[active] += T[active]
+        self.emitted[active] += count
+        self.ended[active] |= end[active]
+        return InverseOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
