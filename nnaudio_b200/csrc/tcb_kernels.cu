@@ -13,7 +13,9 @@
 //
 // (tools/block_dft_emulation.py is the executable spec; exact in exact arithmetic.)  R times fewer
 // MMA flops than the dense form, the A operand is a plain (blocks x hop) matrix, and the epilogue
-// does the 3-tap bin filter in registers and the R-block frame sum with warp shuffles.
+// does the R-block frame sum with warp shuffles and the 3-tap bin filter in registers, in that order:
+//   S_t[k] = sum_{j<R} c_k^j Z_{t+j}[k],   X_t[k] = 1/2 S_t[k] - 1/4 (S_t[k-1] + S_t[k+1])
+// (the same sum, since c_k w = c_{k-1}; tools/block_epilogue_emulation.py).
 //
 // GEMM view: M = block rows g of the whole batch (the split-signal planes of tc_kernels.cu viewed
 // as a (rows x hop) matrix), K = hop, N = 2 * (F + 2) columns (re | im of bins -1 .. F: the two
@@ -91,12 +93,13 @@ struct TcbSmem {
   __host__ __device__ static uint32_t stage_bytes(int nb, int passes) {
     return a_planes(passes) * A_BYTES + 4 * part_bytes(nb);
   }
-  static int stages(int nb, int passes) {
-    const int s = (int)((LIMIT - 1024 - BAR_BYTES - acc_bytes(nb)) / stage_bytes(nb, passes));
+  // `extra`: bytes a kernel keeps behind the barriers (framed_tcb_ws_kernel's fused-filterbank action slices)
+  static int stages(int nb, int passes, uint32_t extra = 0) {
+    const int s = (int)((LIMIT - 1024 - BAR_BYTES - extra - acc_bytes(nb)) / stage_bytes(nb, passes));
     return s < TCB_MAX_STAGES ? s : TCB_MAX_STAGES;
   }
-  static uint32_t total(int nb, int passes) {
-    return 1024 + acc_bytes(nb) + stages(nb, passes) * stage_bytes(nb, passes) + BAR_BYTES;
+  static uint32_t total(int nb, int passes, uint32_t extra = 0) {
+    return 1024 + acc_bytes(nb) + stages(nb, passes, extra) * stage_bytes(nb, passes) + BAR_BYTES + extra;
   }
 };
 
@@ -215,14 +218,25 @@ int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
 
 // ---------------------------------------------------------------------------
 // epilogue: one warp = one 32-row quarter of the accumulator tile (32 consecutive block rows) x a range
-// of 8-column chunks.  The body of a chunk is straight-line code (no branches between the load and the
-// stores), so the 8 bins' dependency chains (3-tap filter -> shuffles -> twiddles -> magnitude)
-// interleave: with one or two warps per scheduler the epilogue is latency-bound, not issue-bound.
+// of 8-column chunks.  The arithmetic of a chunk is straight-line code, so the 8 columns' dependency chains
+// (shuffles and twiddles -> 3-tap filter -> magnitude) interleave: with one or two warps per scheduler the
+// epilogue is latency-bound, not issue-bound.
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ float sqrt_approx(float x) {
   float r;
   asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(x));  // <= 1 ulp-ish: far below the 1e-4 bar
   return r;
+}
+
+// FMT 5 fast path: static action list and the default power 2 without eps; anything else (other powers,
+// trainable eps, no action list) takes the rolled MelRun path
+__device__ __forceinline__ bool fb_fast_path(const EpiParams& e) {
+  return e.fb_steps != nullptr && e.power == 2.0f && e.eps == 0.f;
+}
+
+// |X|^2 from 2X: (2X)^2 times the exact 1/4, the same float as rounding |X|^2 itself (outside subnormals)
+__device__ __forceinline__ float power_of_2x(float yr, float yi) {
+  return __fmul_rn(0.25f, __fadd_rn(__fmul_rn(yr, yr), __fmul_rn(yi, yi)));
 }
 
 // fire-and-forget fp32 add, predicated (no branch: the chunk body stays one basic block)
@@ -243,10 +257,15 @@ __device__ __forceinline__ void red_add_if(float* addr, float v, bool on) {
 // sums of the filters open at the cut.  Part 1 keeps the first flush of each slot, which belongs to the filter
 // part 0 ends with, and passes it through shared memory (`handover`, named barrier 2 + quarter); part 0 adds it
 // to its own final sum before its one atomic add.  So a filter gets one partial sum per (family, tile).
-template <int FMT, int R, int PH>
+//
+// Fused filterbank actions: without STAGED they are read from fb_steps with __ldg, a chunk ahead of its
+// arithmetic; with STAGED, `acts` is the warp's copy in shared memory of fb_steps entries k_tile0 + 8 c_begin - 3
+// .. k_tile0 + 8 c_end - 3 (tcb_stage_actions), read where they are used.
+template <int FMT, int R, int PH, bool STAGED = false>
 __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t trow, int64_t g, int lane,
                                                     int k_tile0, int klo, int khi, int64_t col0, int c_begin,
-                                                    int c_end, int part, int quarter, uint32_t handover) {
+                                                    int c_end, int part, int quarter, uint32_t handover,
+                                                    const int4* acts) {
   const int nb = p.nb;
   const int64_t b = g / p.t_slots;
   const int64_t t = g - b * p.t_slots;  // frame index inside the clip = index of its first block
@@ -257,9 +276,7 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
   if constexpr (FMT == 5) mel = p.epi.out + ((int64_t)b * p.epi.n_fb) * p.epi.T + t;
   else if constexpr (FMT != 9) dst = p.epi.out + (((int64_t)b * p.epi.out_bins + p.epi.bin_offset) * p.epi.T + t) * CH;
   MelRun run;
-  // FMT 5 fast path: static action list and the default power 2 without eps; anything else (other
-  // powers, trainable eps, no action list) takes the rolled MelRun path below
-  const bool fast_fb = (FMT == 5) && p.epi.fb_steps != nullptr && p.epi.power == 2.0f && p.epi.eps == 0.f;
+  const bool fast_fb = (FMT == 5) && fb_fast_path(p.epi);
   float ma = 0.f, mb = 0.f;  // FMT 5, static action list: the two running filter sums
   int mca = -1, mcb = -1;    //   and the filters they currently belong to
   constexpr bool HANDOVER = FMT == 5 && PH == 4;
@@ -268,18 +285,18 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
   if constexpr (HANDOVER) {
     const int kq = k_tile0 + 8 * c_begin - 3;  // the bin before this part's first
     if (fast_fb && part == 1 && kq >= 0) {
-      const int w = __ldg(reinterpret_cast<const int4*>(p.epi.fb_steps) + kq).w;
+      const int w = STAGED ? acts[0].w : __ldg(reinterpret_cast<const int4*>(p.epi.fb_steps) + kq).w;
       first_a = (short)(w & 0xffff) >= 0;
       first_b = (short)((unsigned)w >> 16) >= 0;
     }
   }
 
-  // twiddles c_k^j of the 4 residues the unrolled loop meets: output o = 8c - 2 + e is bin
-  // k = k_tile0 + o, so k mod 4 = (k_tile0 + 2 + e) mod 4 (8c drops out).
+  // twiddles c_k of the 4 residues the unrolled loop meets: packed column 8c + e is bin
+  // k = k_tile0 + 8c + e - 1, so k mod 4 = (k_tile0 + 3 + e) mod 4 (8c drops out).
   float cr[4], ci[4], c2[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const int m = (k_tile0 + 2 + i) & 3;
+    const int m = (k_tile0 + 3 + i) & 3;
     if constexpr (R == 4) {  // c = (-i)^k
       cr[i] = (m == 0) ? 1.f : ((m == 2) ? -1.f : 0.f);
       ci[i] = (m == 3) ? 1.f : ((m == 1) ? -1.f : 0.f);
@@ -288,22 +305,36 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
     }
     c2[i] = (m & 1) ? -1.f : 1.f;  // R = 4: c^2 = (-1)^k;  R = 2: c = (-1)^k
   }
+  // S_t = sum_{j<R} c^j Z_{t+j} of one packed column, row t = lane (the rows past 32 - R read garbage that no
+  // valid lane uses).  R = 4 as pair sums: Q_t = Z_t + c Z_{t+1}, S_t = Q_t + c^2 Q_{t+2}.
+  auto frame_sum = [&](float zr, float zi, int i, float& s_r, float& s_i) {
+    const float z1r = __shfl_down_sync(0xffffffffu, zr, 1), z1i = __shfl_down_sync(0xffffffffu, zi, 1);
+    if constexpr (R == 4) {
+      const float qr = fmaf(cr[i], z1r, fmaf(-ci[i], z1i, zr)), qi = fmaf(cr[i], z1i, fmaf(ci[i], z1r, zi));
+      const float q2r = __shfl_down_sync(0xffffffffu, qr, 2), q2i = __shfl_down_sync(0xffffffffu, qi, 2);
+      s_r = fmaf(c2[i], q2r, qr);
+      s_i = fmaf(c2[i], q2i, qi);
+    } else {
+      s_r = fmaf(c2[i], z1r, zr);
+      s_i = fmaf(c2[i], z1i, zi);
+    }
+  };
 
-  float wr[10], wi[10];  // packed columns 8c-2 .. 8c+7 of this row (re, im)
+  float wr[10], wi[10];  // S of packed columns 8c-2 .. 8c+7 of this row (re, im)
   wr[8] = wr[9] = wi[8] = wi[9] = 0.f;
   if (c_begin > 0) {  // a column range that starts inside the tile: seed the two carried columns
     uint32_t re[8], im[8];
     acc_ld8(trow + (uint32_t)(8 * (c_begin - 1)), re);
     acc_ld8(trow + (uint32_t)(nb + 8 * (c_begin - 1)), im);
-    wr[8] = __uint_as_float(re[6]); wr[9] = __uint_as_float(re[7]);
-    wi[8] = __uint_as_float(im[6]); wi[9] = __uint_as_float(im[7]);
+    frame_sum(__uint_as_float(re[6]), __uint_as_float(im[6]), 2, wr[8], wi[8]);
+    frame_sum(__uint_as_float(re[7]), __uint_as_float(im[7]), 3, wr[9], wi[9]);
   }
 #pragma unroll 1
   for (int c = c_begin; c < c_end; ++c) {
     wr[0] = wr[8]; wr[1] = wr[9]; wi[0] = wi[8]; wi[1] = wi[9];
-    int4 st[8];  // FMT 5: this chunk's filterbank actions, requested before the accumulator loads
+    int4 st[8];  // FMT 5 from fb_steps: this chunk's filterbank actions, requested before the accumulator loads
     if constexpr (FMT == 5) {
-      if (fast_fb) {
+      if (!STAGED && fast_fb) {
         const int kq = k_tile0 + 8 * c - 2;
 #pragma unroll
         for (int e = 0; e < 8; ++e)
@@ -315,36 +346,15 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
       acc_ld8(trow + (uint32_t)(8 * c), re);
       acc_ld8(trow + (uint32_t)(nb + 8 * c), im);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) { wr[e + 2] = __uint_as_float(re[e]); wi[e + 2] = __uint_as_float(im[e]); }
+      for (int e = 0; e < 8; ++e) frame_sum(__uint_as_float(re[e]), __uint_as_float(im[e]), e & 3, wr[e + 2], wi[e + 2]);
     }
+    // the Hann window on the frame sums: X[k] = 1/2 S[k] - 1/4 (S[k-1] + S[k+1]).  xr / xi hold 2 X; the exact
+    // factor 1/2 is applied by the format tails (1/4 on the power, power_of_2x).
     float xr[8], xi[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
-      const float zmr = wr[e], zmi = wi[e], z0r = wr[e + 1], z0i = wi[e + 1], zpr = wr[e + 2],
-                  zpi = wi[e + 2];
-      const float sr = zmr + zpr, si = zmi + zpi;
-      const float ar = 0.5f * z0r, ai = 0.5f * z0i;
-      if constexpr (R == 4) {
-        const float dr = zmr - zpr, di = zmi - zpi;
-        const float v0r = fmaf(-0.25f, sr, ar), v0i = fmaf(-0.25f, si, ai);
-        float v2r = fmaf(0.25f, sr, ar), v2i = fmaf(0.25f, si, ai);
-        float v1r = fmaf(0.25f, di, ar), v1i = fmaf(-0.25f, dr, ai);   // a - (i/4) D
-        float v3r = fmaf(-0.25f, di, ar), v3i = fmaf(0.25f, dr, ai);   // a + (i/4) D
-        v1r = __shfl_down_sync(0xffffffffu, v1r, 1); v1i = __shfl_down_sync(0xffffffffu, v1i, 1);
-        v2r = __shfl_down_sync(0xffffffffu, v2r, 2); v2i = __shfl_down_sync(0xffffffffu, v2i, 2);
-        v3r = __shfl_down_sync(0xffffffffu, v3r, 3); v3i = __shfl_down_sync(0xffffffffu, v3i, 3);
-        const float qr = cr[e & 3], qi = ci[e & 3], q2 = c2[e & 3];
-        // X = V0 + c V1 + c^2 V2 + conj(c) V3
-        xr[e] = v0r + (qr * v1r - qi * v1i) + q2 * v2r + (qr * v3r + qi * v3i);
-        xi[e] = v0i + (qr * v1i + qi * v1r) + q2 * v2i + (qr * v3i - qi * v3r);
-      } else {
-        const float v0r = fmaf(-0.25f, sr, ar), v0i = fmaf(-0.25f, si, ai);
-        float v1r = fmaf(0.25f, sr, ar), v1i = fmaf(0.25f, si, ai);
-        v1r = __shfl_down_sync(0xffffffffu, v1r, 1); v1i = __shfl_down_sync(0xffffffffu, v1i, 1);
-        const float q2 = c2[e & 3];
-        xr[e] = fmaf(q2, v1r, v0r);
-        xi[e] = fmaf(q2, v1i, v0i);
-      }
+      xr[e] = fmaf(-0.5f, wr[e] + wr[e + 2], wr[e + 1]);
+      xi[e] = fmaf(-0.5f, wi[e] + wi[e + 2], wi[e + 1]);
     }
     const int k0 = k_tile0 + 8 * c - 2;          // bin of e = 0 (outputs -2, -1 of chunk 0 do not exist)
     const int e_lo = (c == 0) ? 2 : 0;
@@ -356,9 +366,9 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
       for (int e = 0; e < 8; ++e) {
         const bool ok = valid && own(e);
         if constexpr (FMT == NNAB_FMT_COMPLEX) {
-          if (ok) *reinterpret_cast<float2*>(q) = make_float2(xr[e], xi[e]);
+          if (ok) *reinterpret_cast<float2*>(q) = make_float2(0.5f * xr[e], 0.5f * xi[e]);
         } else {
-          float pw = __fadd_rn(__fmul_rn(xr[e], xr[e]), __fmul_rn(xi[e], xi[e]));
+          float pw = power_of_2x(xr[e], xi[e]);
           if (p.epi.eps != 0.f) pw = __fadd_rn(pw, p.epi.eps);
           float v;
           if constexpr (FMT == NNAB_FMT_MAGNITUDE) {
@@ -381,7 +391,7 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
       __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
-        float pw = __fadd_rn(__fmul_rn(xr[e], xr[e]), __fmul_rn(xi[e], xi[e]));
+        float pw = power_of_2x(xr[e], xi[e]);
         if (p.epi.eps != 0.f) pw = __fadd_rn(pw, p.epi.eps);
         float v = (p.epi.power == 2.0f) ? pw
                   : ((p.epi.power == 1.0f) ? sqrt_approx(pw) : powf(sqrt_approx(pw), p.epi.power));
@@ -396,18 +406,18 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
       }
     } else if constexpr (FMT == 5) {
       if (fast_fb) {
-        // banded filterbank, static action list: branch-free, two running sums per row.
-        // Bins this quarter does not own (the two columns of chunk 0 that belong to the previous tile,
-        // another family's bins, bins past F) contribute with power 0.
+        // banded filterbank, static action list: two running sums per row.  Bins this quarter does not own
+        // (the two columns of chunk 0 that belong to the previous tile, another family's bins, bins past F)
+        // contribute with power 0.  power == 2 (the default, mel.py:186: |X| ** 2): the power spectrum itself.
+        const int4* a = acts + 8 * (c - c_begin) + 1;  // (STAGED) the chunk's 8 actions
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-          const int4 raw = st[e];
-          // power == 2 (the default, mel.py:186: |X| ** 2): the power spectrum itself, to 1 ulp
-          const float pw = own(e) ? __fadd_rn(__fmul_rn(xr[e], xr[e]), __fmul_rn(xi[e], xi[e])) : 0.f;
+          const float pw = own(e) ? power_of_2x(xr[e], xi[e]) : 0.f;
+          const int z = STAGED ? a[e].z : st[e].z;
           // a filter ends at ~1 bin in 6 (and at the same bins for every row): one warp-uniform test
           // on the packed flush word keeps the address / predicate / RED code off the common path
-          if (__any_sync(0xffffffffu, raw.z != -1)) {
-            const int fa = (int)(short)(raw.z & 0xffff), fb = (int)(short)((unsigned)raw.z >> 16);
+          if (__any_sync(0xffffffffu, z != -1)) {
+            const int fa = (int)(short)(z & 0xffff), fb = (int)(short)((unsigned)z >> 16);
             bool keep_a = false, keep_b = false;
             if constexpr (HANDOVER) {
               keep_a = first_a && fa >= 0;
@@ -422,11 +432,12 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
             ma = fa >= 0 ? 0.f : ma;
             mb = fb >= 0 ? 0.f : mb;
           }
-          ma = fmaf(__int_as_float(raw.x), pw, ma);
-          mb = fmaf(__int_as_float(raw.y), pw, mb);
+          ma = fmaf(__int_as_float(STAGED ? a[e].x : st[e].x), pw, ma);
+          mb = fmaf(__int_as_float(STAGED ? a[e].y : st[e].y), pw, mb);
         }
-        mca = (int)(short)(st[7].w & 0xffff);  // filters the two sums belong to after this chunk
-        mcb = (int)(short)((unsigned)st[7].w >> 16);
+        const int cur = STAGED ? a[7].w : st[7].w;  // filters the two sums belong to after this chunk
+        mca = (int)(short)(cur & 0xffff);
+        mcb = (int)(short)((unsigned)cur >> 16);
       } else {
 #pragma unroll 1
         for (int e = e_lo; e < 8; ++e) {
@@ -436,7 +447,7 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
           float re = xr[0], im = xi[0];
 #pragma unroll
           for (int j = 1; j < 8; ++j) { re = (e == j) ? xr[j] : re; im = (e == j) ? xi[j] : im; }
-          run.add(p.epi, mel, valid, k, epi_power(p.epi, re, im));
+          run.add(p.epi, mel, valid, k, epi_power(p.epi, 0.5f * re, 0.5f * im));
         }
       }
     } else {
@@ -450,7 +461,7 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
         float re = xr[0], im = xi[0];
 #pragma unroll
         for (int j = 1; j < 8; ++j) { re = (e == j) ? xr[j] : re; im = (e == j) ? xi[j] : im; }
-        if (valid) epi_store_fmt<FMT>(p.epi, dst, k, re, im);
+        if (valid) epi_store_fmt<FMT>(p.epi, dst, k, 0.5f * re, 0.5f * im);
       }
     }
   }
@@ -632,9 +643,10 @@ __device__ __forceinline__ void tcb_butterfly(const TcbParams& p, uint32_t tile,
 
 // One warp's share of a tile's epilogue: 32-row quarter `quarter` (four phases: family `quarter`) and column
 // part `part` of the accumulator tile.
-template <int FMT, int R, int PH>
+template <int FMT, int R, int PH, bool STAGED = false>
 __device__ __forceinline__ void tcb_epilogue(const TcbParams& p, uint32_t tile_addr, int m_tile, int n_tile,
-                                             int quarter, int part, int lane, uint32_t handover) {
+                                             int quarter, int part, int lane, uint32_t handover,
+                                             const int4* acts = nullptr) {
   constexpr int FW = 33 - R;  // frames per warp quarter
   constexpr int TILE_ROWS = PH == 4 ? FW : 4 * FW;  // block rows an M tile advances
   const int nb = p.nb;
@@ -644,8 +656,24 @@ __device__ __forceinline__ void tcb_epilogue(const TcbParams& p, uint32_t tile_a
   block_family_span(n_tile, PH == 4 ? quarter : 0, nb, PH == 4 ? p.fam_M : 0, p.epi.F, &k_tile0, &klo, &khi);
   if (klo < k_tile0) klo = k_tile0;
   const int64_t col0 = (int64_t)nb * (PH * n_tile + (PH == 4 ? quarter : 0));
-  epilogue_tile_block<FMT, R, PH>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, k_tile0, klo, khi,
-                                  col0, c_begin, c_end, part, quarter, handover);
+  epilogue_tile_block<FMT, R, PH, STAGED>(p, tile_addr + acc_row((uint32_t)quarter * 32u), g, lane, k_tile0, klo,
+                                          khi, col0, c_begin, c_end, part, quarter, handover, acts);
+}
+
+// Four phases, fused filterbank: copy the fb_steps entries warp (quarter, part) of tile n_tile reads into its
+// shared-memory slice `acts` (epilogue_tile_block, STAGED).  They do not depend on the accumulators, so the
+// warp-specialised kernel loads them before it waits for the tile.  Negative bins read entry 0.
+__device__ __forceinline__ void tcb_stage_actions(const TcbParams& p, int n_tile, int quarter, int part, int lane,
+                                                  int4* acts) {
+  if (!fb_fast_path(p.epi)) return;
+  const int c_begin = part == 0 ? 0 : p.c_split, c_end = part == 0 ? p.c_split : p.nb / 8;
+  int k_tile0, klo, khi;
+  block_family_span(n_tile, quarter, p.nb, p.fam_M, p.epi.F, &k_tile0, &klo, &khi);
+  const int base = k_tile0 + 8 * c_begin - 3;
+  const int4* __restrict__ steps = reinterpret_cast<const int4*>(p.epi.fb_steps);
+  __syncwarp();  // every lane is done with the previous tile's slice
+  for (int i = lane; i <= 8 * (c_end - c_begin); i += 32) acts[i] = __ldg(steps + (base + i < 0 ? 0 : base + i));
+  __syncwarp();
 }
 
 template <int FMT, int R, int PASSES, int PH>
@@ -741,9 +769,15 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 // the 88 accumulators of MMA width 2 TCB_WS_NB_MAX (ptxas needs >= 114 for that wgmma).  A separate producer warp
 // (17 warps) would cut every thread to 96, and ptxas does not raise the allocation inside setmaxnreg regions.
 // There is one accumulator tile: two do not fit beside a stage at nb = 88 (2 x 96 KB + 38 KB > 227 KB), so a tile
-// still takes store + butterfly + epilogue; the MMAs are what is hidden.
+// still takes store + butterfly + epilogue; the MMAs are what is hidden.  With the fused filterbank the epilogue
+// warps' fb_steps slices (TCB_WS_ACT_BYTES) sit behind the barriers: at nb = 88 the ring keeps its 3 stages, at
+// nb = 80 (three passes) it has 3 instead of 4.
 constexpr int TCB_WS_THREADS = 512;
 constexpr int TCB_WS_NB_MAX = 88;
+// fused filterbank: each epilogue warp's slice of fb_steps (tcb_stage_actions), 8 entries per chunk of its larger
+// column part plus the one before, behind the barriers
+constexpr int TCB_WS_ACTS = 8 * (TCB_WS_NB_MAX / 8 - TCB_WS_NB_MAX / 8 / TCB_PARTS) + 1;
+constexpr uint32_t TCB_WS_ACT_BYTES = 8 * TCB_WS_ACTS * sizeof(int4);
 
 template <int FMT, int R, int PASSES>
 __global__ void __launch_bounds__(TCB_WS_THREADS, 1)
@@ -829,13 +863,17 @@ framed_tcb_ws_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
 
   // ===================== epilogue warps =====================
   const int ew = warp - 8;
+  int4* acts = reinterpret_cast<int4*>(nnab_dyn_smem + (ring.bars + S::BAR_BYTES - smem_u32(nnab_dyn_smem))) +
+               ew * TCB_WS_ACTS;
   uint32_t full_phase = 0;
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int m_tile = tile / p.num_n_tiles;
     const int n_tile = tile - m_tile * p.num_n_tiles;
+    if constexpr (FMT == 5) tcb_stage_actions(p, n_tile, ew & 3, ew >> 2, lane, acts);
     mbar_wait(acc_full, full_phase);
     full_phase ^= 1u;
-    tcb_epilogue<FMT, R, 4>(p, tile_addr, m_tile, n_tile, ew & 3, ew >> 2, lane, ring.bars + S::HANDOVER_OFF);
+    tcb_epilogue<FMT, R, 4, FMT == 5>(p, tile_addr, m_tile, n_tile, ew & 3, ew >> 2, lane,
+                                      ring.bars + S::HANDOVER_OFF, acts);
     mbar_arrive(acc_empty);
   }
 }
@@ -852,13 +890,19 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   // keep framed_tcb_kernel: their epilogue is shorter than the MMA warps' share of a tile, and with separate roles
   // Magnitude STFT-2048 measured 7 % slower, where the Mel, MFCC and Gammatone workloads run 3-5 % faster.
   constexpr bool WS = PH == 4 && (FMT == 5 || FMT == 9);
-  const size_t smem = S::total(prm.nb, PASSES);
-  if (!WS || prm.nb > TCB_WS_NB_MAX)
-    return launch_persistent<framed_tcb_kernel<FMT, R, PASSES, PH>>(grid, TC_KERNEL_THREADS, smem, S::LIMIT, stream,
-                                                                    ma, mb, prm);
-  if constexpr (WS)
-    return launch_persistent<framed_tcb_ws_kernel<FMT, R, PASSES>>(grid, TCB_WS_THREADS, smem, S::LIMIT, stream,
-                                                                   ma, mb, prm);
+  TcbParams q = prm;
+  if (!WS || prm.nb > TCB_WS_NB_MAX) {
+    q.stages = S::stages(prm.nb, PASSES);
+    return launch_persistent<framed_tcb_kernel<FMT, R, PASSES, PH>>(grid, TC_KERNEL_THREADS, S::total(prm.nb, PASSES),
+                                                                    S::LIMIT, stream, ma, mb, q);
+  }
+  if constexpr (WS) {
+    const uint32_t extra = FMT == 5 ? TCB_WS_ACT_BYTES : 0;
+    q.stages = S::stages(prm.nb, PASSES, extra);
+    return launch_persistent<framed_tcb_ws_kernel<FMT, R, PASSES>>(grid, TCB_WS_THREADS,
+                                                                   S::total(prm.nb, PASSES, extra), S::LIMIT, stream,
+                                                                   ma, mb, q);
+  }
   return NNAB_EINVAL;  // (not reached)
 }
 
@@ -964,7 +1008,6 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   prm.num_n_tiles = n_tiles;
   prm.nb = nb;
   prm.kb_n = Kb / TCB_BK;
-  prm.stages = TcbSmem::stages(nb, passes);
   prm.c_split = c_split;
   prm.fam_M = poly ? q.K / 4 : 0;
   prm.twiddle = poly ? reinterpret_cast<const float2*>((const char*)packed + block_twiddle_offset(q.K, q.hop))
