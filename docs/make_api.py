@@ -52,6 +52,9 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   `StreamPool` feeds it as is.  Each slot's samples equal `StreamingInverse` on its own frames, to fp32 rounding.
   `StreamingPyramid(module, batch)` streams the CQT pyramid of `CQT2010v2` / `VQT` / `CQT2010` bit for bit on the
   whole-clip call's tensor-core plan (DESIGN.md §3.10).
+  `PyramidPool(module, slots)` serves independent pyramid streams with `StreamPool`'s `push(chunk, lengths, end)` /
+  `reset(slots)` surface: each slot's rows equal `module(x)` on its own stream bit for bit, and a one-stream
+  `StreamingPyramid` fed the same packets.
 
 Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
 schedule of the CQT1992v2 kernel).

@@ -505,6 +505,33 @@ int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t fra
                                   int n_octaves, const int32_t* widths, int hop, int early_factor, int pad_mode,
                                   int64_t* out);
 
+/* Pool of streamed CQT pyramids: the stream pools' (state, lanes, d_lanes, n_lanes, A, chunk, chunk_dtype, slots,
+ * n, chunk_pitch) in front of nnab_cqt_pyramid_chunk_forward's pyramid arguments, then (out, T_max).  The state is
+ * nnab_cqt_pyramid_chunk_state_bytes(slots, ...): row s of every signal's ring belongs to slot s.  A lane's n_carry
+ * is the raw-ring carry of nnab_cqt_pyramid_chunk_forward and its `end` that call's flush; each lane is checked
+ * by that call's rules (counters, frame bound, ring capacity, the octaves' frame counts at an end), the table by the
+ * pools' (order, repeated slots, A, T_max, n above the chunk width), and every launch against the kernels' limits,
+ * all before anything is enqueued.  Row i of out (A, n_bins, T_max[, 2]) holds lane i's frames, bit for bit those
+ * of the whole-clip call on its stream, then exact zeros.  The launches are the chunk call's over the same stages
+ * on (n_lanes, ...) rows (the octaves on the A rows), one plan launch and one mask launch.  The workspace query is
+ * host-only and takes the host lane table. */
+size_t nnab_cqt_pyramid_pool_workspace_bytes(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
+                                             int64_t T_max, int n_octaves, const int32_t* widths, int hop,
+                                             int early_factor, int pad_mode);
+int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                  int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                  int64_t n, int64_t chunk_pitch, int n_octaves, const float* const* h_k_real,
+                                  const float* const* h_k_imag, const void* const* h_packed,
+                                  const int32_t* h_widths, int n_filters, const float* lowpass,
+                                  const void* lowpass_packed, const float* early_filter, const void* early_packed,
+                                  int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
+                                  float scale_all, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                  void* workspace, size_t ws_bytes, int path, void* stream);
+/* Host-only plan of one pool push for tests: for lane i, out[i (8 n_signals + 1) ..] in the layout of
+ * nnab_debug_pyramid_chunk_plan, from the lane's (signal, lane) descriptors. */
+int nnab_debug_pyramid_pool_plan(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A, int n_octaves,
+                                 const int32_t* widths, int hop, int early_factor, int pad_mode, int64_t* out);
+
 /* Streamed inverse STFT: nnab_istft_forward's arguments, with the frames of ONE push as X (B, f_in, T, 2)
  * (T may be 0) and in front of them
  *   state     DEVICE fp32, nnab_chunk_state_bytes(B, n_fft) bytes: the overlap-add partial sums later frames

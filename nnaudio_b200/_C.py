@@ -11,6 +11,7 @@ import ctypes
 import os
 from ctypes import c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
+import numpy as np
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -146,6 +147,12 @@ SIGNATURES["nnab_cqt_pyramid_chunk_forward"] = (
     c_int, _CHUNK_HEAD + SIGNATURES["nnab_cqt_pyramid_forward"][1][4:])
 SIGNATURES["nnab_debug_pyramid_chunk_plan"] = (
     c_int, [c_int64, c_int64, c_int64, c_int64, c_int, c_int, _P, c_int, c_int, c_int, _P])
+# pyramid pools: the pool head in front of the chunk call's pyramid arguments; the workspace query and the debug
+# plan take the host lane table
+SIGNATURES["nnab_cqt_pyramid_pool_forward"] = (c_int, _POOL_HEAD + SIGNATURES["nnab_cqt_pyramid_forward"][1][4:])
+SIGNATURES["nnab_cqt_pyramid_pool_workspace_bytes"] = (
+    c_size_t, [_P, c_int64, c_int64, c_int64, c_int, _P, c_int, c_int, c_int])
+SIGNATURES["nnab_debug_pyramid_pool_plan"] = (c_int, [_P, c_int64, c_int64, c_int, _P, c_int, c_int, c_int, _P])
 SIGNATURES["nnab_istft_chunk_workspace_bytes"] = SIGNATURES["nnab_istft_workspace_bytes"]
 SIGNATURES["nnab_istft_chunk_forward"] = (
     c_int, [_P, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, c_int, c_int64, _P,
@@ -816,6 +823,65 @@ def cqt_pyramid_chunk_forward(st, x, flush, T, banks_real, banks_imag, packed, l
             _ptr(early_filter), _ptr(early_packed), early_factor, hop, pad_mode, n_bins, _ptr(scale), scale_all,
             out_format, sqrt_eps, _ptr(out) if T > 0 else None, T, _ptr(ws), wsb, path, _stream(dev))
     return _chunk_result(rc, out, "nnab_cqt_pyramid_chunk_forward")
+
+
+def _lane_table(lanes):
+    """A C copy of an (n_lanes, 6) int64 lane table (host-only calls)."""
+    a = np.ascontiguousarray(np.asarray(lanes, dtype=np.int64).reshape(-1, 6))
+    return a, (a.ctypes.data_as(c_void_p) if len(a) else None)
+
+
+def cqt_pyramid_pool_plan(lanes, A, widths, hop, pad_mode, early_factor=1):
+    """Host-only plan of one pool push (``nnab_debug_pyramid_pool_plan``): for each lane, the levels and frame
+    bound of ``cqt_pyramid_chunk_plan``.  Raises on a lane table the library refuses."""
+    n_sig = len(widths) + (1 if early_factor > 1 else 0)
+    a, ptr = _lane_table(lanes)
+    w = (c_int32 * len(widths))(*[int(v) for v in widths])
+    buf = (c_int64 * max(1, len(a) * (8 * n_sig + 1)))()
+    _check(lib().nnab_debug_pyramid_pool_plan(ptr, len(a), int(A), len(widths), w, int(hop), int(early_factor),
+                                              int(pad_mode), buf), "nnab_debug_pyramid_pool_plan")
+    out = []
+    for i in range(len(a)):
+        o = buf[i * (8 * n_sig + 1):(i + 1) * (8 * n_sig + 1)]
+        out.append(([tuple(o[8 * s:8 * s + 8]) for s in range(n_sig)], int(o[8 * n_sig])))
+    return out
+
+
+def cqt_pyramid_pool_workspace_bytes(lanes, A, T_max, widths, hop, early_factor, pad_mode) -> int:
+    a, ptr = _lane_table(lanes)
+    w = (c_int32 * len(widths))(*[int(v) for v in widths])
+    return int(lib().nnab_cqt_pyramid_pool_workspace_bytes(ptr, len(a), int(A), int(T_max), len(widths), w,
+                                                            int(hop), int(early_factor), int(pad_mode)))
+
+
+def cqt_pyramid_pool_forward(pool, lanes, x, A, T_max, banks_real, banks_imag, packed, lowpass, lowpass_packed,
+                             early_filter, early_packed, early_factor, hop, pad_mode, n_bins, scale, scale_all,
+                             out_format, sqrt_eps, path=None):
+    """One push of ``nnaudio_b200.streaming.PyramidPool``: ``lanes`` its (n_lanes, 6) lane table (the A lanes with
+    frames first), ``x`` the (slots, n) chunk or None; ``pool`` carries the rings (``pool.ring``), ``pool.slots``
+    and ``pool.dtype``.  The remaining arguments are ``cqt_pyramid_forward``'s.  Returns the (A, n_bins, T_max[, 2])
+    frames, or None when the configuration has no streamed plan (NNAB_EUNSUPPORTED, nothing enqueued)."""
+    L = lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    dev = pool.ring.device
+    out = torch.empty((A, n_bins, T_max) if out_format == FMT_MAGNITUDE else (A, n_bins, T_max, 2),
+                      dtype=torch.float32, device=dev)
+    n_oct = len(banks_real)
+    re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
+    im_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_imag])
+    pk_arr = (c_void_p * n_oct)(*[(t.data_ptr() if t is not None else None) for t in packed])
+    widths = [int(t.shape[1]) for t in banks_real]
+    path = resolve_path(path)
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(cqt_pyramid_pool_workspace_bytes(lanes, A, T_max, widths, hop, early_factor, pad_mode),
+                             dev)
+        hl, dl = _pool_lanes(pool, lanes)
+        rc = L.nnab_cqt_pyramid_pool_forward(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, n_oct, re_arr,
+            im_arr, pk_arr, (c_int32 * n_oct)(*widths), banks_real[0].shape[0], _ptr(lowpass), _ptr(lowpass_packed),
+            _ptr(early_filter), _ptr(early_packed), early_factor, hop, pad_mode, n_bins, _ptr(scale), scale_all,
+            out_format, sqrt_eps, _ptr(out) if out.numel() else None, T_max, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, "nnab_cqt_pyramid_pool_forward")
 
 
 def istft_chunk_forward(st, X, flush, length, n_out, packed, window, n_fft, hop, center):

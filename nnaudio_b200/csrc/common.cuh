@@ -135,6 +135,7 @@ __host__ __device__ inline int poly4_range(int k, int M, int nb) {
 // table names its ring row and chunk row (`slot`), its counters and its end; origin = frames * hop - pad and
 // received / total / at_end come from the lane, and the fields of the same name above are unused.  The clip
 // length is the batch's longest; a row's samples past its own stream read as zeros.
+struct PyrLaneSig;
 struct ChunkSource {
   const float* ring;
   int64_t ring_pitch;
@@ -146,6 +147,12 @@ struct ChunkSource {
   int at_end;
   const nnab_stream_lane* lanes;  // pools only, else nullptr
   int K, hop, pad;                // pools only: the framing that places each lane's clip
+  // pyramid pools (rows != nullptr, lanes == nullptr): row b of the launch takes everything from the DEVICE
+  // descriptor rows[b] (PyrLaneSig below): its ring row, its source row and base, its counts, and -- rows_oct = 1,
+  // an octave clip (pad: the octave's) -- the octave's frame origin, padding and end, or -- rows_oct = 0, a FIR
+  // stage source -- the stage's source origin, with zeros past the row's samples.
+  const PyrLaneSig* rows;
+  int rows_oct;
 };
 
 // ---- the counters of one stream (DESIGN §3.10), shared by the host checks and the pool kernels ----------
@@ -178,6 +185,116 @@ __host__ __device__ inline int64_t lane_frames_after(const nnab_stream_lane& ln,
                                                      int pad_mode) {
   const int64_t total = ln.received + ln.n;
   return ln.end ? chunk_end_frames(total, K, hop, pad) : chunk_ready_frames(total, K, hop, pad, pad_mode);
+}
+
+// ---- the streamed CQT pyramid (DESIGN §3.10 "Pyramid streams"), shared by the host checks and the pool kernels
+// Level lengths follow conv1d(stride=n, padding=127, kernel=256): (len - 2)/n + 1.
+__host__ __device__ inline int64_t decimated_len(int64_t len, int factor) {
+  return len < 2 ? 0 : (len - 2) / factor + 1;
+}
+
+// Signals of a stream: the raw samples when an early stage feeds level 0, then one per octave (octave i on
+// signal i + e).  Stage s turns signal s into s + 1 (factor d[s]): y[n] = sum_m fir[m] x[d n + m - 127].
+// Every per-signal number is a function of the raw count alone: before the end, sample n of signal s + 1 is
+// final once d n + c of signal s have arrived -- c = 129 (its last tap reads d n + 128), 130 on the gen-2 plan,
+// whose edge fix recomputes the last 64 outputs of the whole clip on the CUDA cores: with one sample more, n is
+// never one of them.  Signal s keeps an fp32 ring (stream b at ring[b * len + r % len]) of what later pushes read.
+struct PyrStream {
+  int n_sig, e, n_oct, c;
+  bool gen2;
+  int d[33];
+  int width[32], hop[32], pad[32];
+  int64_t ring_len[33];
+  size_t ring_off[33];  // floats
+  size_t state_floats;  // per stream
+};
+
+// Samples of every signal after `raw` raw samples: final ones before the end, all of them on flush.
+__host__ __device__ inline void pyr_counts(const PyrStream& p, int64_t raw, int flush, int64_t* R) {
+  R[0] = raw;
+  for (int s = 0; s + 1 < p.n_sig; ++s) {
+    if (flush) R[s + 1] = decimated_len(R[s], p.d[s]);
+    else R[s + 1] = R[s] >= p.c ? (R[s] - p.c) / p.d[s] + 1 : 0;
+  }
+}
+
+// Frames final in every octave (before the end).
+__host__ __device__ inline int64_t pyr_ready_frames(const PyrStream& p, const int64_t* R, int pad_mode) {
+  int64_t t = INT64_MAX;
+  for (int i = 0; i < p.n_oct; ++i) {
+    const int64_t f = chunk_ready_frames(R[i + p.e], p.width[i], p.hop[i], p.pad[i], pad_mode);
+    t = f < t ? f : t;
+  }
+  return t;
+}
+
+// First sample of signal s a later push reads, after `frames` frames with the counts R.
+__host__ __device__ inline int64_t pyr_keep(const PyrStream& p, int s, const int64_t* R, int64_t frames) {
+  int64_t k = R[s];
+  const int l = s - p.e;
+  if (l >= 0) k = chunk_carry_start(R[s], frames, p.hop[l], p.pad[l]);
+  if (s + 1 < p.n_sig) {
+    int64_t f = 128 * (int64_t)p.d[s] * (R[s + 1] / 128) - 128;
+    f = f < 0 ? 0 : f;
+    k = f < k ? f : k;
+  }
+  return k;
+}
+
+// One pool lane's plan for signal s of a push: what the one-stream push (nnab_cqt_pyramid_chunk_forward) of the
+// lane's counters does with that signal.  The plan kernel writes it per (signal, lane) into the workspace and
+// every lane-aware kernel reads it; the host checks the lanes with the same functions first.
+struct PyrLaneSig {
+  int64_t slot;            // ring row
+  int64_t R0, R1;          // final samples of the signal before and after the push
+  int64_t keep;            // the ring keeps [keep, R1) after the push (R1 at an end: nothing)
+  int64_t src_row, base;   // the new samples: source row (chunk row / new-sample row), sample R0 at `base`
+  int64_t t0;              // first 128-output row of the FIR stage s -> s + 1 (-1: the lane has no new output)
+  int64_t fir_origin;      // its source origin 128 d t0 - 128
+  int64_t fir_len_src, fir_len_out;  // source samples / outputs from that row on (R1 - 128 d t0, R1' - 128 t0)
+  int64_t oct_origin;      // the octave's first unreturned frame: frames * hop_l - pad_l
+  int64_t count;           // frames the push returns (the lane's, the same on every signal)
+  int32_t mode;            // the octave's padding (reflect falls back to constant on a short level at the end)
+  int32_t end;
+  int32_t head, tail;      // the FIR stage's CUDA-core edge fix: the stream's first / last 64 outputs
+};
+
+__host__ __device__ inline PyrLaneSig pyr_lane_signal(const PyrStream& p, const nnab_stream_lane& ln, int64_t lane,
+                                                      int s, int pad_mode) {
+  int64_t R0[33], R1[33];
+  pyr_counts(p, ln.received, 0, R0);
+  pyr_counts(p, ln.received + ln.n, (int)ln.end, R1);
+  const int64_t t_end = ln.end ? chunk_end_frames(R1[p.e], p.width[0], p.hop[0], p.pad[0])
+                               : pyr_ready_frames(p, R1, pad_mode);
+  PyrLaneSig o{};
+  o.slot = ln.slot;
+  o.R0 = R0[s];
+  o.R1 = R1[s];
+  const int64_t k = ln.end ? R1[s] : pyr_keep(p, s, R1, t_end);
+  o.keep = k > R0[s] ? k : R0[s];
+  // the raw signal comes from the lane's chunk row; a decimated one from row `lane` of its new-sample buffer,
+  // which holds the stage's outputs from its first row, 128 floor(R0 / 128), on
+  o.src_row = s == 0 ? ln.slot : lane;
+  o.base = s == 0 ? 0 : R0[s] % 128;
+  o.t0 = -1;
+  if (s + 1 < p.n_sig && R1[s + 1] > R0[s + 1]) {
+    const int64_t t0 = R0[s + 1] / 128, d = p.d[s];
+    o.t0 = t0;
+    o.fir_origin = 128 * d * t0 - 128;
+    o.fir_len_src = R1[s] - 128 * d * t0;
+    o.fir_len_out = R1[s + 1] - 128 * t0;
+    o.head = p.gen2 && t0 == 0;
+    o.tail = p.gen2 && ln.end;
+  }
+  const int l = s - p.e;
+  o.mode = pad_mode;
+  if (l >= 0) {
+    o.oct_origin = ln.frames * p.hop[l] - p.pad[l];
+    if (ln.end && pad_mode == NNAB_PAD_REFLECT && p.pad[l] >= R1[s]) o.mode = NNAB_PAD_CONSTANT;
+  }
+  o.count = t_end - ln.frames;
+  o.end = (int32_t)ln.end;
+  return o;
 }
 
 // ---- the counters of one streamed inverse STFT (DESIGN §3.10), shared by the host checks and the pool kernels
@@ -318,6 +435,14 @@ int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, 
 // `longest` samples), and the zeroing of output frames t >= the count of row i of out (A, rows, T, cols)
 int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream);
 int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int64_t T, int cols,
+                 cudaStream_t stream);
+// pyramid pools: the (signal, lane) descriptor table of a push (table[s * n_lanes + i] = pyr_lane_signal of lane i
+// of the DEVICE lane table), every row's carry [keep, R1) of one signal (cs.rows; at most `longest` samples), and
+// the zeroing of frames t >= rows[i].count of row i of out (A, n_rows, T, cols)
+int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int pad_mode,
+                     PyrLaneSig* table, cudaStream_t stream);
+int tc_rows_carry(const ChunkSource& cs, int x_dtype, int64_t n_rows, int64_t longest, cudaStream_t stream);
+int tc_rows_mask(const PyrLaneSig* rows, int64_t A, float* out, int64_t n_rows, int64_t T, int cols,
                  cudaStream_t stream);
 int tc_zero_slots(void* planes, int64_t B, int64_t clip_pitch, int64_t plane_stride, int64_t keep_lo,
                   int64_t keep_hi, cudaStream_t stream);

@@ -844,11 +844,7 @@ int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, 
 }
 
 // ------------------------------------------------ CQT2010v2 / VQT pyramid ----
-// Level lengths follow conv1d(stride=n, padding=127, kernel=256): (len - 2)/n + 1.
-static inline int64_t decimated_len(int64_t len, int factor) {
-  return len < 2 ? 0 : (len - 2) / factor + 1;
-}
-
+// (level lengths: decimated_len, common.cuh)
 static size_t pyramid_level_bytes(int64_t B, int64_t L, int early_factor) {
   // [early (B, L0)] + ping/pong level buffers (B, <= L0/2 + 1)
   const int64_t L0 = early_factor > 1 ? decimated_len(L, early_factor) : L;
@@ -1421,22 +1417,7 @@ int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L
 }
 
 // ------------------------------------------------------------ streamed pyramid ----
-// Signals of a stream: the raw samples when an early stage feeds level 0, then one per octave (octave i on
-// signal i + e).  Stage s turns signal s into s + 1 (factor d[s]): y[n] = sum_m fir[m] x[d n + m - 127].
-// Every per-signal number is a function of the raw count alone: before the end, sample n of signal s + 1 is
-// final once d n + c of signal s have arrived -- c = 129 (its last tap reads d n + 128), 130 on the gen-2 plan,
-// whose edge fix recomputes the last 64 outputs of the whole clip on the CUDA cores: with one sample more, n is
-// never one of them.  Signal s keeps an fp32 ring (stream b at ring[b * len + r % len]) of what later pushes read.
-struct PyrStream {
-  int n_sig, e, n_oct, c;
-  bool gen2;
-  int d[33];
-  int width[32], hop[32], pad[32];
-  int64_t ring_len[33];
-  size_t ring_off[33];  // floats
-  size_t state_floats;  // per stream
-};
-
+// (a stream's signals and counters: PyrStream, pyr_counts, pyr_ready_frames and pyr_keep in common.cuh)
 static bool pyr_stream_init(int n_octaves, const int32_t* widths, int hop, int early_factor, bool gen2,
                             PyrStream* ps) {
   if (n_octaves <= 0 || n_octaves > 32 || widths == nullptr || hop <= 0 || early_factor < 1) return false;
@@ -1477,38 +1458,6 @@ static bool pyr_stream_init(int n_octaves, const int32_t* widths, int hop, int e
   }
   p.state_floats = off;
   return true;
-}
-
-// Samples of every signal after `raw` raw samples: final ones before the end, all of them on flush.
-static void pyr_counts(const PyrStream& p, int64_t raw, int flush, int64_t* R) {
-  R[0] = raw;
-  for (int s = 0; s + 1 < p.n_sig; ++s) {
-    if (flush) R[s + 1] = decimated_len(R[s], p.d[s]);
-    else R[s + 1] = R[s] >= p.c ? (R[s] - p.c) / p.d[s] + 1 : 0;
-  }
-}
-
-// Frames final in every octave (before the end).
-static int64_t pyr_ready_frames(const PyrStream& p, const int64_t* R, int pad_mode) {
-  int64_t t = INT64_MAX;
-  for (int i = 0; i < p.n_oct; ++i) {
-    const int64_t f = chunk_ready_frames(R[i + p.e], p.width[i], p.hop[i], p.pad[i], pad_mode);
-    t = f < t ? f : t;
-  }
-  return t;
-}
-
-// First sample of signal s a later push reads, after `frames` frames with the counts R.
-static int64_t pyr_keep(const PyrStream& p, int s, const int64_t* R, int64_t frames) {
-  int64_t k = R[s];
-  const int l = s - p.e;
-  if (l >= 0) k = chunk_carry_start(R[s], frames, p.hop[l], p.pad[l]);
-  if (s + 1 < p.n_sig) {
-    int64_t f = 128 * (int64_t)p.d[s] * (R[s + 1] / 128) - 128;
-    f = f < 0 ? 0 : f;
-    k = f < k ? f : k;
-  }
-  return k;
 }
 
 // One push: the counts before (R0) and after (R1) it, the frames it returns and the workspace layout.
@@ -1788,6 +1737,263 @@ int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t fra
     r[7] = (stage && p.gen2 && flush) ? (pp.R1[s + 1] - 64 > pp.R0[s + 1] ? pp.R1[s + 1] - 64 : pp.R0[s + 1]) : -1;
   }
   out[8 * p.n_sig] = pp.t_end;
+  return NNAB_OK;
+}
+
+// ------------------------------------------------------------ pyramid pools ----
+// One push of a pool of pyramid streams (DESIGN §3.10 "Pyramid pools"): every lane checked by the one-stream rules
+// (pyr_push_plan), the table as a whole, and the batch-wide geometry of each launch.
+struct PyrPoolPlan {
+  int64_t T_max;
+  int64_t len_out[33];  // stage s: the most outputs one lane's FIR rows hold from their first row (0: no lane advances)
+  int64_t np[33];       // new-sample row pitch of signal s >= 1 (floats)
+  int64_t longest[33];  // the most samples one lane keeps of signal s
+  size_t table, nbuf[33], scratch, scratch_bytes, total;
+};
+
+static int pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
+                         int64_t slots, int64_t n, int pad_mode, PyrPoolPlan* o) {
+  if (n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes || (n_lanes > 0 && lanes == nullptr)) return NNAB_EINVAL;
+  std::vector<uint8_t> seen((size_t)slots, 0);
+  o->T_max = 0;
+  for (int s = 0; s < p.n_sig; ++s) o->len_out[s] = o->longest[s] = 0;
+  for (int64_t i = 0; i < n_lanes; ++i) {
+    const nnab_stream_lane& ln = lanes[i];
+    if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
+    if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
+    seen[(size_t)ln.slot] = 1;
+    if (ln.n > n || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
+    PyrPush pp;
+    const int rc = pyr_push_plan(p, 1, ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, pad_mode, &pp);
+    if (rc) return rc;
+    const int64_t T = pp.t_end - ln.frames;
+    if ((i < A) != (T > 0)) return NNAB_EINVAL;               // the A lanes with frames come first
+    if (T == 0 && ln.n == 0 && !ln.end) return NNAB_EINVAL;   // a lane with nothing to do
+    if (T > o->T_max) o->T_max = T;
+    for (int s = 0; s < p.n_sig; ++s) {
+      const PyrLaneSig d = pyr_lane_signal(p, ln, i, s, pad_mode);
+      if (d.R0 != pp.R0[s] || d.R1 != pp.R1[s] || d.count != T) return NNAB_EINVAL;  // one set of rules
+      if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
+      if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
+    }
+  }
+  // workspace: the descriptor table, the new samples of every computed signal (row i: lane i's stage outputs from
+  // its first row), then one scratch reused by the launches in order
+  size_t off = 0;
+  o->table = off;
+  off += align_up((size_t)(n_lanes > 0 ? n_lanes : 1) * p.n_sig * sizeof(PyrLaneSig), 256);
+  for (int s = 1; s < p.n_sig; ++s) {
+    o->np[s] = (int64_t)align_up((size_t)(o->len_out[s - 1] > 0 ? o->len_out[s - 1] : 1), 8);
+    o->nbuf[s] = off;
+    off += align_up((size_t)(n_lanes > 0 ? n_lanes : 1) * o->np[s] * sizeof(float), 256);
+  }
+  size_t sc = 0;
+  for (int s = 0; s < p.n_sig; ++s) {
+    const int l = s - p.e;
+    if (l >= 0 && A > 0 && o->T_max > 0) {
+      const int64_t len = (o->T_max - 1) * p.hop[l] + p.width[l];
+      size_t need = tc_workspace_bytes(A, len, p.width[l], p.hop[l], 0);
+      if (p.gen2 && p.hop[l] % 8 == 0) {
+        int64_t pitch, plane;
+        pyr_oct_geom(p, l, A, len, &pitch, &plane);
+        need = (size_t)plane * 4 + 256;
+      }
+      sc = need > sc ? need : sc;
+    }
+    if (s + 1 < p.n_sig && o->len_out[s] > 0) {
+      const int64_t FT = (o->len_out[s] + 127) / 128;
+      const int kf = tc_fir_k(FIR_TAPS, p.d[s]);
+      const size_t need = p.gen2 ? (size_t)((n_lanes * (FT + 1) + 2) * 256) * 4 + 256
+                                 : tc_workspace_bytes(n_lanes, (FT - 1) * 128 * (int64_t)p.d[s] + kf, kf,
+                                                      128 * p.d[s], 0);
+      sc = need > sc ? need : sc;
+    }
+  }
+  o->scratch = off;
+  o->scratch_bytes = sc;
+  o->total = off + sc + 512;
+  return NNAB_OK;
+}
+
+size_t nnab_cqt_pyramid_pool_workspace_bytes(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
+                                             int64_t T_max, int n_octaves, const int32_t* widths, int hop,
+                                             int early_factor, int pad_mode) {
+  PyrStream p;
+  PyrPoolPlan pl;
+  if (widths == nullptr || n_lanes <= 0 ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return 0;
+  if (pyr_pool_plan(p, lanes, n_lanes, A, 65535, INT64_MAX, pad_mode, &pl) || pl.T_max != T_max) return 0;
+  return pl.total;
+}
+
+int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
+                                  int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
+                                  int64_t n, int64_t chunk_pitch, int n_octaves, const float* const* h_k_real,
+                                  const float* const* h_k_imag, const void* const* h_packed,
+                                  const int32_t* h_widths, int n_filters, const float* lowpass,
+                                  const void* lowpass_packed, const float* early_filter, const void* early_packed,
+                                  int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
+                                  float scale_all, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                  void* workspace, size_t ws_bytes, int path, void* stream) {
+  if (state == nullptr || !dtype_ok(chunk_dtype) || slots < 1 || slots > 65535 || n < 0 ||
+      (n > 0 && chunk == nullptr) || chunk_pitch < n || n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes ||
+      T_max < 0 || (A > 0 && T_max > 0 && out == nullptr) || (n_lanes > 0 && (lanes == nullptr || d_lanes == nullptr)) ||
+      h_k_real == nullptr || h_k_imag == nullptr || h_widths == nullptr || lowpass == nullptr || n_octaves <= 0 ||
+      n_octaves > 32 || n_filters <= 0 || hop <= 0 || n_bins <= 0 || early_factor < 1 ||
+      (early_factor > 1 && early_filter == nullptr))
+    return NNAB_EINVAL;
+  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX && out_format != NNAB_FMT_PHASE_UNIT)
+    return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  const bool gen2 = pyr_gen2(n_octaves, h_widths, early_factor);
+  PyrStream p;
+  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, gen2, &p)) return NNAB_EUNSUPPORTED;
+  PyrPoolPlan pl;
+  int rc = pyr_pool_plan(p, lanes, n_lanes, A, slots, n, pad_mode, &pl);
+  if (rc) return rc;
+  if (pl.T_max != T_max) return NNAB_EINVAL;
+  bool packed_ok = path != NNAB_PATH_SIMT && h_packed != nullptr && lowpass_packed != nullptr &&
+                   (early_factor <= 1 || early_packed != nullptr);
+  for (int i = 0; packed_ok && i < n_octaves; ++i) packed_ok = h_packed[i] != nullptr;
+  if (!packed_ok) return NNAB_EUNSUPPORTED;
+  if ((rc = check_arch())) return rc;
+  if (n_lanes == 0) return NNAB_OK;
+  if (workspace == nullptr || ws_bytes < pl.total) return NNAB_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* scratch = ws + pl.scratch;
+  PyrLaneSig* table = (PyrLaneSig*)(ws + pl.table);
+  // the octaves run on the A lanes with frames (rows 0 .. A - 1), T_max frames each
+  const PyramidCall c{nullptr, NNAB_DTYPE_F32, A, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
+                      n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
+                      scale_all, out_format, sqrt_eps, out, T_max, ws, ws_bytes, s};
+  float* ring = static_cast<float*>(state);
+
+  // pass 0 checks every launch against the kernels' limits, as the chunk call does; pass 1 runs them
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass == 1 && (rc = tc_pyr_pool_plan(p, d_lanes, n_lanes, pad_mode, table, s))) return rc;
+    for (int sg = 0; sg < p.n_sig; ++sg) {
+      ChunkSource cs{};
+      cs.ring = ring + (size_t)slots * p.ring_off[sg];
+      cs.ring_pitch = cs.ring_len = p.ring_len[sg];
+      cs.chunk = sg == 0 ? chunk : (const void*)(ws + pl.nbuf[sg]);
+      cs.chunk_pitch = sg == 0 ? chunk_pitch : pl.np[sg];
+      cs.pad_mode = NNAB_PAD_CONSTANT;
+      cs.rows = table + (size_t)sg * n_lanes;
+      const int dt = sg == 0 ? chunk_dtype : NNAB_DTYPE_F32;
+      const int l = sg - p.e;
+      if (l >= 0 && A > 0 && T_max > 0) {
+        // octave l: each row from its lane's first unreturned frame, T_max frames, on the whole-clip plan's kernel
+        ChunkSource co = cs;
+        co.rows_oct = 1;
+        co.pad = p.pad[l];
+        co.length = (T_max - 1) * p.hop[l] + p.width[l];
+        FramedProblem q = octave_problem(c, l, co.length, p.hop[l], pad_mode);
+        q.pad = 0; q.x_dtype = dt; q.chunk = &co;
+        if (gen2 && p.hop[l] % 8 == 0) {
+          int64_t pitch, plane;
+          pyr_oct_geom(p, l, A, co.length, &pitch, &plane);
+          FramedProblem qp = q;
+          qp.chunk = nullptr;
+          qp.presplit = scratch; qp.presplit_t_slots = pitch / p.hop[l]; qp.presplit_plane_stride = plane;
+          const bool oct = octave_tc_ok(qp);
+          if (pass == 0) {
+            if (!oct && !tc_supported(qp)) return NNAB_EUNSUPPORTED;
+          } else {
+            if ((rc = tc_chunk_split(co, dt, A, pitch, plane, scratch, s))) return rc;
+            if (oct) {
+              std::pair<cudaEvent_t, cudaEvent_t> pr;
+              const bool timed = prof_begin(s, &pr);
+              rc = launch_octave_tc(qp, c.packed[l], s);
+              if (timed) prof_end(s, pr);
+            } else {
+              rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
+            }
+            if (rc) return rc;
+          }
+        } else if (pass == 0) {
+          if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+        } else if ((rc = run_framed(q, c.packed[l], scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+          return rc;
+        }
+      }
+      if (sg + 1 < p.n_sig && pl.len_out[sg] > 0) {
+        // stage sg -> sg + 1 on every lane, each row from its lane's first 128-output row (the whole clip's
+        // accumulation order); row i of the new-sample buffer holds lane i's outputs from that row on
+        const int d = p.d[sg];
+        const int64_t FT = (pl.len_out[sg] + 127) / 128;
+        ChunkSource cf = cs;
+        cf.rows_oct = 0;
+        DecimParams dec{};
+        dec.len_out = pl.len_out[sg];
+        dec.lo = 0;
+        dec.y32 = (float*)(ws + pl.nbuf[sg + 1]);
+        dec.y32_pitch = pl.np[sg + 1];
+        dec.skip_edges = 3;
+        const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
+        if (gen2) {
+          if (pass == 1) {
+            const int64_t pitch = 256 * (FT + 1), plane = (n_lanes * (FT + 1) + 2) * 256;
+            cf.length = pitch;
+            if ((rc = tc_chunk_split(cf, dt, n_lanes, pitch, plane, scratch, s))) return rc;
+            if ((rc = launch_fir_stage_tc(scratch, n_lanes, 0, pitch, plane, FIR_OFF, fir_packed, c.lowpass,
+                                          FIR_TAPS, dec, s, cf.rows)))
+              return rc;
+          }
+        } else {
+          FramedProblem q{};
+          q.B = n_lanes; q.x_dtype = dt; q.F = 64; q.K = tc_fir_k(FIR_TAPS, d); q.hop = 128 * d;
+          q.L = (FT - 1) * q.hop + q.K; q.pad = 0; q.pad_mode = NNAB_PAD_CONSTANT; q.scale_all = 1.f;
+          q.fmt = FMT_DECIM; q.power = 1.f; q.T = FT; q.out_bins = 64;
+          q.dec = dec;
+          cf.length = q.L;
+          q.chunk = &cf;
+          if (pass == 0) {
+            if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+          } else if ((rc = run_framed(q, fir_packed, scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+            return rc;
+          }
+        }
+      }
+      // after this signal's readers: what later pushes read of it, into each lane's slot row of its ring
+      if (pass == 1 && (rc = tc_rows_carry(cs, dt, n_lanes, pl.longest[sg], s))) return rc;
+    }
+  }
+  // frames t >= a row's count were computed from the zeros past its stream: exact zeros
+  return tc_rows_mask(table, A, out, n_bins, T_max, format_cols(out_format), s);
+}
+
+int nnab_debug_pyramid_pool_plan(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A, int n_octaves,
+                                 const int32_t* widths, int hop, int early_factor, int pad_mode, int64_t* out) {
+  if (out == nullptr) return NNAB_EINVAL;
+  PyrStream p;
+  PyrPoolPlan pl;
+  if (widths == nullptr ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  const int rc = pyr_pool_plan(p, lanes, n_lanes, A, 65535, INT64_MAX, pad_mode, &pl);
+  if (rc) return rc;
+  // per lane, the layout of nnab_debug_pyramid_chunk_plan, from the lane's descriptors
+  const int64_t stride = 8 * p.n_sig + 1;
+  for (int64_t i = 0; i < n_lanes; ++i) {
+    int64_t* o = out + i * stride;
+    const int64_t t_end = lanes[i].frames + pyr_lane_signal(p, lanes[i], i, 0, pad_mode).count;
+    int64_t R1[33];
+    pyr_counts(p, lanes[i].received + lanes[i].n, (int)lanes[i].end, R1);
+    for (int s = 0; s < p.n_sig; ++s) {
+      const PyrLaneSig d = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
+      const PyrLaneSig dn = s + 1 < p.n_sig ? pyr_lane_signal(p, lanes[i], i, s + 1, pad_mode) : d;
+      int64_t* r = o + 8 * s;
+      r[0] = d.R0; r[1] = d.R1; r[2] = p.ring_len[s];
+      r[3] = d.end ? d.R1 : pyr_keep(p, s, R1, t_end);
+      r[4] = d.t0 >= 0 ? d.fir_origin : 0;
+      r[5] = d.t0;
+      r[6] = d.head ? (dn.R1 < 64 ? dn.R1 : 64) : 0;
+      r[7] = d.tail ? (dn.R1 - 64 > dn.R0 ? dn.R1 - 64 : dn.R0) : -1;
+    }
+    o[8 * p.n_sig] = t_end;
+  }
   return NNAB_OK;
 }
 

@@ -77,10 +77,12 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
 int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* workspace, size_t ws_bytes,
                           cudaStream_t stream);
 
-// FIR decimator stage with banded taps (tct_kernels.cu); NNAB_EUNSUPPORTED = geometry not eligible
+// FIR decimator stage with banded taps (tct_kernels.cu); NNAB_EUNSUPPORTED = geometry not eligible.  lane_rows
+// (pyramid pools): clip b's edge fix follows lane_rows[b] (its own lengths, head and tail) instead of src_len / dec.
 int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int64_t src_pitch,
                         int64_t src_plane_stride, int src_pad, const void* fir_packed,
-                        const float* fir, int taps, const DecimParams& dec, cudaStream_t stream);
+                        const float* fir, int taps, const DecimParams& dec, cudaStream_t stream,
+                        const PyrLaneSig* lane_rows = nullptr);
 
 // octave CQT on shared level planes: resident bank, tall A blocks, frame phases (tct_kernels.cu)
 bool octave_tc_ok(const FramedProblem& q);

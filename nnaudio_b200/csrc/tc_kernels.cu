@@ -280,6 +280,84 @@ __global__ void __launch_bounds__(256) pool_mask_kernel(ChunkSource c, float* __
   }
 }
 
+// ---- pyramid pools (DESIGN §3.10 "Pyramid pools"): the kernels that know where each row's samples come from --
+// The (signal, lane) descriptor table of a push: one thread per entry, pyr_lane_signal of the lane's counters.
+__global__ void __launch_bounds__(128) pyr_pool_plan_kernel(const PyrStream p,
+                                                            const nnab_stream_lane* __restrict__ lanes,
+                                                            int64_t n_lanes, int pad_mode,
+                                                            PyrLaneSig* __restrict__ table) {
+  const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_lanes * p.n_sig) return;
+  const int s = (int)(k / n_lanes);
+  const int64_t i = k - s * n_lanes;
+  table[k] = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
+}
+
+// chunk_split_kernel in the per-row descriptor mode (ChunkSource::rows): row b builds its own clip -- a FIR
+// stage source from the lane's first 128-output row, or an octave clip from its first unreturned frame -- from its
+// slot's ring row and its own source row, with its own counts, padding and end; past its samples, zeros.
+template <typename Tx>
+__global__ void __launch_bounds__(256) chunk_split_rows_kernel(
+    ChunkSource c, const Tx* __restrict__ chunk, int shift, int64_t clip_pitch, int64_t plane_stride,
+    int poly_hop, __nv_bfloat16* __restrict__ planes) {
+  const int64_t b = blockIdx.y;
+  const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if (i0 >= clip_pitch) return;
+  const PyrLaneSig& d = c.rows[b];
+  const int64_t origin = c.rows_oct ? d.oct_origin : d.fir_origin;
+  const bool reflect = c.rows_oct && d.mode == NNAB_PAD_REFLECT;
+  const bool at_end = !c.rows_oct || d.end;
+  const float* __restrict__ ring = c.ring + d.slot * c.ring_pitch;
+  const Tx* __restrict__ xb = chunk + d.src_row * c.chunk_pitch + d.base;
+  const int64_t s0 = split_src(i0, poly_hop) + shift;
+  const int step = poly_hop ? 4 : 1;
+  __align__(16) __nv_bfloat16 hi[8];
+  __align__(16) __nv_bfloat16 lo[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const int64_t i = s0 + step * e;
+    float v = 0.f;
+    if (i < c.length) {
+      int64_t r = origin + i;
+      bool live = true;
+      if (r < 0) {
+        if (reflect) r = -r; else live = false;
+      } else if (r >= d.R1) {
+        if (at_end && reflect && r - d.R1 < c.pad) r = 2 * (d.R1 - 1) - r; else live = false;
+      }
+      if (live) v = r < d.R0 ? __ldg(ring + r % c.ring_len) : sample_f32(__ldg(xb + (r - d.R0)));
+    }
+    split_bf16(v, hi[e], lo[e]);
+  }
+  const int64_t o = b * clip_pitch + i0;
+  *reinterpret_cast<uint4*>(planes + o) = *reinterpret_cast<const uint4*>(hi);
+  *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
+}
+
+// chunk_carry_kernel in the descriptor mode: row b keeps [keep, R1) of its signal in its slot's ring row.
+template <typename Tx>
+__global__ void __launch_bounds__(256) chunk_carry_rows_kernel(ChunkSource c, const Tx* __restrict__ chunk) {
+  const PyrLaneSig& d = c.rows[blockIdx.y];
+  const int64_t r = d.keep + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= d.R1) return;
+  const_cast<float*>(c.ring)[d.slot * c.ring_pitch + r % c.ring_len] =
+      sample_f32(__ldg(chunk + d.src_row * c.chunk_pitch + d.base + (r - d.R0)));
+}
+
+// pool_mask_kernel with the count of each row from its descriptor.
+__global__ void __launch_bounds__(256) rows_mask_kernel(const PyrLaneSig* __restrict__ desc,
+                                                        float* __restrict__ out, int64_t rows, int64_t T, int cols) {
+  const int64_t count = desc[blockIdx.y].count;
+  if (count >= T) return;
+  const int64_t row_len = (T - count) * cols;
+  float* __restrict__ o = out + (int64_t)blockIdx.y * rows * T * cols;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < rows * row_len;
+       k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = k / row_len;
+    o[r * T * cols + count * cols + (k - r * row_len)] = 0.f;
+  }
+}
+
 // The one sample-type dispatch (NNAB_DTYPE_*): f(samples) launches one kernel on x as fp32, bf16 or fp16
 // samples, and the launch is checked.  (The deduced return type instantiates each call's kernels where the call
 // stands, which keeps the module's kernel order.)
@@ -1476,7 +1554,10 @@ static int launch_chunk_split(const ChunkSource& cs, int x_dtype, dim3 grid, int
                               int64_t plane_stride, int poly_hop, __nv_bfloat16* planes, cudaStream_t stream) {
   return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
     using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
-    if (cs.lanes != nullptr)
+    if (cs.rows != nullptr)
+      chunk_split_rows_kernel<Tx><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
+                                                            planes);
+    else if (cs.lanes != nullptr)
       chunk_split_kernel<Tx, true><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
                                                              planes);
     else
@@ -1521,6 +1602,36 @@ int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int
   const int64_t per_row = rows * T * cols;
   const dim3 grid((unsigned)(ceil_div64(per_row, 256) < 64 ? ceil_div64(per_row, 256) : 64), (unsigned)A);
   pool_mask_kernel<<<grid, 256, 0, stream>>>(cs, out, rows, T, cols);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int pad_mode,
+                     PyrLaneSig* table, cudaStream_t stream) {
+  if (n_lanes <= 0) return NNAB_OK;
+  const int64_t n = n_lanes * p.n_sig;
+  pyr_pool_plan_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, stream>>>(p, lanes, n_lanes, pad_mode, table);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_rows_carry(const ChunkSource& cs, int x_dtype, int64_t n_rows, int64_t longest, cudaStream_t stream) {
+  if (longest <= 0 || n_rows <= 0) return NNAB_OK;
+  if (n_rows > 65535) return NNAB_EUNSUPPORTED;
+  const dim3 grid((unsigned)ceil_div64(longest, 256), (unsigned)n_rows);
+  return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
+    using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
+    chunk_carry_rows_kernel<Tx><<<grid, 256, 0, stream>>>(cs, xs);
+  });
+}
+
+int tc_rows_mask(const PyrLaneSig* rows, int64_t A, float* out, int64_t n_rows, int64_t T, int cols,
+                 cudaStream_t stream) {
+  if (A <= 0 || T <= 0) return NNAB_OK;
+  if (A > 65535) return NNAB_EUNSUPPORTED;
+  const int64_t per_row = n_rows * T * cols;
+  const dim3 grid((unsigned)(ceil_div64(per_row, 256) < 64 ? ceil_div64(per_row, 256) : 64), (unsigned)A);
+  rows_mask_kernel<<<grid, 256, 0, stream>>>(rows, out, n_rows, T, cols);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }

@@ -763,12 +763,49 @@ __global__ void __launch_bounds__(128) fir_edge_fix_kernel(
   if (d.y32 != nullptr) d.y32[b * d.y32_pitch + (n - d.lo)] = acc;
 }
 
+// fir_edge_fix_kernel of a pyramid pool's stage (rows: the stage's source descriptors, DecimParams::lo = 0, the
+// fp32 copy only): row b recomputes the stream's first 64 outputs where its first row is the stream's (head) and
+// its last 64 where its stream ends (tail), with its own source and output lengths from that row -- the sums of
+// fir_edge_fix_kernel, term for term.
+__global__ void __launch_bounds__(128) fir_edge_fix_rows_kernel(
+    const __nv_bfloat16* __restrict__ src, int64_t src_pitch, int64_t src_plane, int src_off,
+    const float* __restrict__ fir, int taps, DecimParams d, const PyrLaneSig* __restrict__ rows) {
+  const int64_t b = blockIdx.y;
+  const int lane = threadIdx.x & 31;
+  const int i = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const PyrLaneSig& r = rows[b];
+  if (r.t0 < 0) return;  // the lane has no new output in this stage
+  const bool head = r.head != 0;
+  if (i < 64 ? !head : !r.tail) return;
+  const int64_t len_out = r.fir_len_out, len_src = r.fir_len_src;
+  const int64_t n = (i < 64) ? i : len_out - 128 + i;
+  if (i >= 64 && head && n < 64) return;
+  if (n < 0 || n >= len_out) return;
+  const __nv_bfloat16* sb = src + b * src_pitch + src_off;
+  const int64_t j_lo = head ? 0 : -(int64_t)src_off;
+  float acc = 0.f;
+#pragma unroll 8
+  for (int m = lane; m < taps; m += 32) {
+    const int64_t j = 2 * n + m - (taps - 1) / 2;
+    const bool in = j >= j_lo && j < len_src;
+    const float hi = in ? __bfloat162float(sb[j]) : 0.f;
+    const float lo = in ? __bfloat162float(sb[src_plane + j]) : 0.f;
+    acc = fmaf(__ldg(fir + m), hi + lo, acc);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane != 0) return;
+  d.y32[b * d.y32_pitch + n] = acc;
+}
+
 // One FIR stage: source level planes (single set, samples at offset src_pad, clip pitch a multiple of
 // 256) -> destination level through `dec` (pc planes with their own pad, optional fp32 copy).
 int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int64_t src_pitch,
                         int64_t src_plane_stride, int src_pad, const void* fir_packed,
-                        const float* fir, int taps, const DecimParams& dec, cudaStream_t stream) {
+                        const float* fir, int taps, const DecimParams& dec, cudaStream_t stream,
+                        const PyrLaneSig* lane_rows) {
   if (taps != 256 || src_pad != 128) return NNAB_EUNSUPPORTED;  // frame origin = row origin
+  if (lane_rows != nullptr && (dec.y32 == nullptr || dec.pc != nullptr || dec.lo != 0)) return NNAB_EUNSUPPORTED;
   if (src_pitch % 256 != 0 || B > 65535 || dec.pf != nullptr) return NNAB_EUNSUPPORTED;
   const int64_t FT = (dec.len_out + 127) / 128;
   const int64_t t_slots = src_pitch / 256;
@@ -798,6 +835,13 @@ int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int6
     return rc;
   add_exec_flops(3.0 * 2.0 * (double)prm.num_m_tiles * TC_BM * 640.0 * 64.0);  // banded: 640 columns x 64
   // clip edges
+  if (lane_rows != nullptr) {
+    fir_edge_fix_rows_kernel<<<dim3(32, (unsigned)B), 128, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(src_planes), src_pitch, src_plane_stride, src_pad, fir, taps, dec,
+        lane_rows);
+    NNAB_LAUNCH_CHECK();
+    return NNAB_OK;
+  }
   fir_edge_fix_kernel<<<dim3(32, (unsigned)B), 128, 0, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(src_planes), src_pitch, src_plane_stride, src_pad, src_len,
       fir, taps, dec);

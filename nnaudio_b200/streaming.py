@@ -21,6 +21,9 @@ in some slots while the others carry on.  Each stream's frames are those of ``St
 ``StreamingPyramid(module, batch)`` streams through the ÷2 resampling pyramid of ``CQT2010v2``, ``VQT`` and
 ``CQT2010`` on the whole-clip call's tensor-core plan: each push returns the frames final in every octave.
 
+``PyramidPool(module, slots)`` is ``StreamPool`` for the pyramids: independent streams with ragged pushes, each
+slot's frames those of a one-stream ``StreamingPyramid``.
+
 ``StreamingInverse(module, batch)`` streams complex frames through the inverse STFT: each push returns the
 output samples no later frame can change, ``flush(length=None)`` the rest.
 
@@ -30,6 +33,7 @@ flagged slots; a ``PoolOutput`` of ``StreamPool`` feeds it as is.
 """
 from __future__ import annotations
 
+from types import SimpleNamespace
 from typing import NamedTuple
 
 import numpy as np
@@ -44,8 +48,8 @@ from .features.mel import MFCC, MelSpectrogram
 from .features.stft import STFT, _inverse_args, iSTFT
 from .features.vqt import VQT
 
-__all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "StreamingInverse", "InversePool",
-           "InverseOutput"]
+__all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "PyramidPool", "StreamingInverse",
+           "InversePool", "InverseOutput"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
 _PYRAMIDS = (CQT2010v2, VQT, CQT2010)
@@ -518,6 +522,136 @@ class StreamingPyramid:
         self.received, self.frames = total, self.frames + T
         self.n_carry = self._n_carry(total, self.frames)
         return out
+
+
+class PyramidPool:
+    """Serve up to ``slots`` independent streams through the CQT pyramid of ``CQT2010v2``, ``VQT`` or ``CQT2010``,
+    each advancing by its own amount.
+
+    ``push(chunk, lengths, end=None)`` and ``reset(slots=None)`` are ``StreamPool``'s, and a push returns a
+    ``PoolOutput``.  Each slot's frames follow ``StreamingPyramid``'s rules for its own stream: before its end the
+    frames final in every octave, on its end the rest with the stream's right padding, raising (the slot named) and
+    warning as ``module(x)`` does for the stream's total length.  Concatenated along time, a slot's rows up to their
+    counts equal ``module(x)`` on its whole stream bit for bit (a 16-bit stream: ``module(x.float())``), and a
+    one-stream ``StreamingPyramid`` fed the same packets.  Every argument is checked before anything is enqueued,
+    and a push never reads the device back or synchronises.  ``module`` and ``forward_kwargs``: those of
+    ``StreamingPyramid`` (``hop_length`` a multiple of ``2 ** (n_octaves - 1)``).
+
+    A push is one C call (``_C.cqt_pyramid_pool_forward``): the whole-clip call's tensor-core plan, each stage and
+    octave once over the lanes, every row aligned on its own stream (DESIGN.md §3.10 "Pyramid pools").  Idle
+    slots cost nothing.  There is no concat route: a plan that cannot read the chunk (``NNAUDIO_B200_PATH=simt``,
+    a missing packed operand) raises ``RuntimeError`` with the pool unchanged.
+    """
+
+    def __init__(self, module, slots, **forward_kwargs):
+        slots = int(slots)
+        if slots < 1 or slots > _C.MAX_BATCH:
+            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        # module checks, the pyramid arguments, the plan and one ring row per slot per signal: StreamingPyramid's
+        self._sp = sp = StreamingPyramid(module, slots, **forward_kwargs)
+        self.module, self.slots = module, slots
+        self.widths, self.hop, self.early, self.generation = sp.widths, sp.hop, sp.early, sp.generation
+        self._reflect = sp._reflect
+        self.ring = sp.ring
+        self.received = np.zeros(slots, np.int64)  # host counters of every slot's stream
+        self.frames = np.zeros(slots, np.int64)
+        self.ended = np.zeros(slots, bool)
+        self.dtype = None
+
+    reset = StreamPool.reset
+    _per_slot = StreamPool._per_slot
+
+    # ---- StreamingPyramid's counters over arrays of lanes ------------------------------------------------- #
+    def _counts(self, raw, end):
+        """Samples of every signal after ``raw`` raw samples: the final ones, or (``end``) all of them."""
+        c = 130 if self.generation == 2 else 129
+        R = [raw]
+        for s in range(len(self.widths) + (self.early > 1) - 1):
+            d = self.early if (self.early > 1 and s == 0) else 2
+            r = R[-1]
+            R.append(np.where(end, np.where(r < 2, 0, (r - 2) // d + 1), np.where(r >= c, (r - c) // d + 1, 0)))
+        return R
+
+    def _ready(self, raw):
+        """Frames final in every octave after ``raw`` samples (``StreamingPyramid._ready``)."""
+        R = self._counts(raw, False)[1 if self.early > 1 else 0:]
+        t = None
+        for i, w in enumerate(self.widths):
+            pad, need = w // 2, w - w // 2
+            f = np.where(R[i] < need, 0, (R[i] - need) // (self.hop >> i) + 1)
+            if self._reflect:
+                f = np.where(R[i] < pad + 1, 0, f)
+            t = f if t is None else np.minimum(t, f)
+        return t
+
+    def _n_carry(self, raw, frames):
+        """Raw samples the raw ring carries (``StreamingPyramid._n_carry``)."""
+        keep = raw
+        if self.early == 1:
+            pad = self.widths[0] // 2
+            s = frames * self.hop - pad
+            if pad > 0:
+                s = np.minimum(s, raw - (pad + 1))
+            keep = np.minimum(np.maximum(s, 0), raw)
+        R = self._counts(raw, False)
+        if len(R) > 1:
+            d = self.early if self.early > 1 else 2
+            keep = np.minimum(keep, np.maximum(0, 128 * d * (R[1] // 128) - 128))
+        return raw - keep
+
+    # ------------------------------------------------------------------------------------------------ #
+    def push(self, chunk: torch.Tensor, lengths, end=None) -> PoolOutput:
+        """Append ``chunk[s, :lengths[s]]`` to every slot s, end the slots flagged in ``end``; returns the new
+        frames of the slots that have some."""
+        if not isinstance(chunk, torch.Tensor):
+            raise TypeError("chunk must be a torch.Tensor")
+        if chunk.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+        if chunk.dim() != 2 or chunk.shape[0] != self.slots:
+            raise ValueError(f"chunk must be ({self.slots}, n), got {tuple(chunk.shape)}")
+        if chunk.dtype not in _C._WAVE_DTYPES:
+            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
+        if self.dtype is not None and chunk.dtype != self.dtype:
+            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within the pool")
+        n = chunk.shape[1]
+        lengths = self._per_slot(lengths, "lengths", True)
+        end = np.zeros(self.slots, bool) if end is None else self._per_slot(end, "end", False)
+        bad = np.flatnonzero((lengths < 0) | (lengths > n))
+        if len(bad):
+            raise ValueError(f"lengths must be in [0, {n}] (the chunk width): slot {bad[0]} has {lengths[bad[0]]}")
+        bad = np.flatnonzero(self.ended & ((lengths > 0) | end))
+        if len(bad):
+            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
+        # every lane's counts, by the rules of StreamingPyramid (push / flush); per lane only the length plan of an end
+        active = np.flatnonzero((lengths > 0) | end)
+        R, F0, m, e = self.received[active], self.frames[active], lengths[active], end[active]
+        total = R + m
+        count = self._ready(total) - F0
+        for j in np.flatnonzero(e).tolist():
+            s = int(active[j])
+            try:
+                T_total, _ = _pyramid_length_plan(self.module, 1, int(total[j]))
+            except Exception as ex:
+                raise type(ex)(f"slot {s}: {ex}") from None
+            count[j] = T_total - F0[j]
+        n_carry = self._n_carry(R, F0)
+        order = np.lexsort((active, count == 0))  # the lanes with frames first, slots ascending in each group
+        active, count = active[order], count[order]
+        A = int((count > 0).sum())
+        T_max = int(count.max()) if A else 0
+        lanes = np.stack([active, self.received[active], n_carry[order], self.frames[active], lengths[active],
+                          end[active].astype(np.int64)], 1).astype(np.int64)
+        dtype = self.dtype if self.dtype is not None else chunk.dtype
+        view = SimpleNamespace(ring=self.ring, slots=self.slots, dtype=dtype)  # the pool as the C call reads it
+        out = _C.cqt_pyramid_pool_forward(view, lanes, chunk, A, T_max, **self._sp._args())
+        if out is None:
+            raise RuntimeError(f"{type(self.module).__name__}: no streamed tensor-core pyramid plan for this call "
+                               "(NNAB_EUNSUPPORTED, e.g. NNAUDIO_B200_PATH=simt); the pool is unchanged")
+        self.dtype = dtype
+        self.received[active] += lengths[active]
+        self.frames[active] += count
+        self.ended[active] |= end[active]
+        return PoolOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
 
 
 class StreamingInverse:
