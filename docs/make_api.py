@@ -50,6 +50,12 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   end=None, length=None)` appends `X[r, :, :counts[r]]` to slot `slots[r]`, ends the flagged slots with the
   `StreamingInverse.flush` rules and returns an `InverseOutput(samples, slots, counts)`; a `PoolOutput` of
   `StreamPool` feeds it as is.  Each slot's samples equal `StreamingInverse` on its own frames, to fp32 rounding.
+  `DeviceStreamPool(module, slots, chunk, dtype=torch.float32)` and `DeviceInversePool(istft_module, slots, frames,
+  onesided=None)` are `StreamPool` and `InversePool` with their counters, lengths and end flags on the GPU: `push(x,
+  lengths, end)` / `push(X, counts, end, length)` take device tensors, overwrite the pool-owned `frames` / `samples`
+  and `counts` (row s = slot s, `T_cap` / `n_cap` wide) and read nothing on the host, so a tick can be captured in a
+  CUDA graph; `reset(restart=None)` takes a device mask, and `check()` raises what the host pool would have raised
+  for a dropped slot (DESIGN.md §3.10 "Device pools").
   `StreamingPyramid(module, batch)` streams the CQT pyramid of `CQT2010v2` / `VQT` / `CQT2010` bit for bit on the
   whole-clip call's tensor-core plan (DESIGN.md §3.10).
   `PyramidPool(module, slots)` serves independent pyramid streams with `StreamPool`'s `push(chunk, lengths, end)` /

@@ -583,6 +583,90 @@ int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nna
                             const void* packed, const float* window, int n_fft, int hop, int center, float* out,
                             int64_t n_max, int64_t T_max, void* workspace, size_t ws_bytes, void* stream);
 
+/* Device-planned pools (DESIGN.md §3.10 "Device pools"): the stream pools and the inverse STFT pool with every
+ * per-push number on the DEVICE, so that a push reads nothing on the host, has one fixed geometry and can be
+ * captured in a CUDA graph.  All slots are computed on every push: row s of every output is slot s.
+ *   counters  DEVICE int64 (3, slots): forward pools received, frames, ended; the inverse pool frames, emitted,
+ *             ended.  Zero for fresh streams; the push advances them, nnab_pool_device_reset zeroes masked slots.
+ *   errors, error_info   DEVICE int32 (slots) and int64 (slots, 2): a slot whose push the host pool would refuse is
+ *             dropped whole (counters, ring / state untouched, zero frames) and errors[s] records the first such
+ *             NNAB_LANE_* code, error_info[s] its values, until the slot's reset.  The other slots proceed.
+ *   counts    DEVICE int32 (slots): frames (samples) row s holds after the push; the rest of the row is zeros.
+ *   d_lanes   DEVICE scratch of `slots` lanes that the plan launch writes and the pool kernels read.
+ * One plan launch (one thread per slot, the host checks' own functions) writes the lanes, counts, codes and the
+ * advanced counters; an idle, ended or dropped slot gets an all-zero lane, which returns nothing and carries
+ * nothing.  Then the body of the matching *_pool_forward runs with n_lanes = A = slots. */
+enum {
+  NNAB_LANE_OK = 0,
+  NNAB_LANE_ELENGTH = 1,   /* lengths[s] (counts[s]) outside [0, chunk width (frames of X)]; info: the value */
+  NNAB_LANE_EENDED = 2,    /* samples / frames or an end for an ended stream                               */
+  NNAB_LANE_ESHORT = 3,    /* an end on a stream too short for the module; info: its length                 */
+  NNAB_LANE_ENOFRAMES = 4, /* inverse: an end on a stream without frames                                     */
+  NNAB_LANE_ELENGTH_SHORT = 5 /* inverse: length shorter than the samples returned; info: length, emitted   */
+};
+/* T_cap: the most frames one push of at most `chunk` samples can return (an end included), for framing (K, hop,
+ * pad, pad_mode).  n_cap: the most samples one inverse push of at most `frames` frames can return (a flush with
+ * any length included).  Host only; 0 for arguments no pool takes. */
+int64_t nnab_pool_frame_cap(int64_t chunk, int K, int hop, int pad, int pad_mode);
+int64_t nnab_istft_pool_sample_cap(int64_t frames, int n_fft, int hop, int center);
+/* Forward: the *_pool_forward arguments with (lanes, d_lanes, n_lanes, A) replaced by (counters, lengths, end,
+ * errors, error_info, counts, d_lanes): lengths DEVICE int32 (slots), end DEVICE uint8 (slots).  n is the fixed
+ * chunk width, T_max must be nnab_pool_frame_cap(n, ...) and out is (slots, ..., T_max).  The workspace is
+ * *_pool_workspace_bytes(slots, T_max, ...).  Only host-side arguments are checked (NNAB_EINVAL).  The SIMT plans
+ * return NNAB_EUNSUPPORTED with only the plan launch enqueued: a push with every length 0 and no end then changes
+ * nothing, which is how a caller can probe the route. */
+int nnab_stft_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                  int32_t* errors, int64_t* error_info, int32_t* counts, nnab_stream_lane* d_lanes,
+                                  const void* chunk, int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                  const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                                  int center, int pad_mode, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                  void* workspace, size_t ws_bytes, int path, void* stream);
+int nnab_stft_filterbank_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths,
+                                             const uint8_t* end, int32_t* errors, int64_t* error_info,
+                                             int32_t* counts, nnab_stream_lane* d_lanes, const void* chunk,
+                                             int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                             const float* wcos, const float* wsin, const void* packed, int n_fft,
+                                             int F, int hop, int center, int pad_mode, float sqrt_eps, float power,
+                                             const float* fb, int n_fb, const void* fb_table, float* out,
+                                             int64_t T_max, void* workspace, size_t ws_bytes, int path, void* stream);
+int nnab_mfcc_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                  int32_t* errors, int64_t* error_info, int32_t* counts, nnab_stream_lane* d_lanes,
+                                  const void* chunk, int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                  const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                                  int center, int pad_mode, float sqrt_eps, float power, const float* mel_basis,
+                                  int n_mels, const void* fb_table, float amin, float ref, float top_db,
+                                  const float* dct, int n_mfcc, float* out, int64_t T_max, void* workspace,
+                                  size_t ws_bytes, int path, void* stream);
+int nnab_cqt1992v2_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                       int32_t* errors, int64_t* error_info, int32_t* counts,
+                                       nnab_stream_lane* d_lanes, const void* chunk, int chunk_dtype, int64_t slots,
+                                       int64_t n, int64_t chunk_pitch, const float* k_real, const float* k_imag,
+                                       const void* packed, const int32_t* h_k_begin, const int32_t* h_k_end,
+                                       int n_bins, int width, int hop, int center, int pad_mode, const float* scale,
+                                       float scale_all, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                       void* workspace, size_t ws_bytes, int path, void* stream);
+/* Inverse: X (slots, f_in, t, 2) fp32, row s slot s's frames; frame_counts DEVICE int32 (slots) its new frames
+ * X[s, :, :frame_counts[s]]; end DEVICE uint8 and length DEVICE int64 (slots; < 0: None).  out is (slots, n_max)
+ * with n_max = nnab_istft_pool_sample_cap(t, ...); the workspace nnab_istft_pool_workspace_bytes(slots, f_in, t,
+ * n_fft, hop). */
+int nnab_istft_pool_device_forward(void* state, int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                                   const int64_t* length, int32_t* errors, int64_t* error_info, int32_t* counts,
+                                   nnab_istft_lane* d_lanes, int64_t slots, const float* X, int f_in, int64_t t,
+                                   const void* packed, const float* window, int n_fft, int hop, int center,
+                                   float* out, int64_t n_max, void* workspace, size_t ws_bytes, void* stream);
+/* New streams in the slots where mask[s] != 0 (mask NULL: every slot): their counters, errors and error_info
+ * become zero.  One launch; the ring / state needs no clearing (a fresh lane reads none of it). */
+int nnab_pool_device_reset(int64_t* counters, int32_t* errors, int64_t* error_info, const uint8_t* mask,
+                           int64_t slots, void* stream);
+/* Host-only runs of the plan launches for tests, on HOST arrays of the layouts above (counters advanced in
+ * place; lanes written as int64 rows of 6 / 7). */
+int nnab_debug_device_pool_plan(int64_t* counters, const int32_t* lengths, const uint8_t* end, int32_t* errors,
+                                int64_t* error_info, int32_t* counts, nnab_stream_lane* lanes, int64_t slots,
+                                int64_t n, int K, int hop, int pad, int pad_mode);
+int nnab_debug_device_istft_plan(int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                                 const int64_t* length, int32_t* errors, int64_t* error_info, int32_t* counts,
+                                 nnab_istft_lane* lanes, int64_t slots, int64_t t, int n_fft, int hop, int center);
+
 /* Kernel launches issued by this library since load (process wide; used by
  * bench.py for its `gpu_launches` claim). */
 uint64_t nnab_launch_count(void);

@@ -128,6 +128,7 @@ for _name in ("nnab_stft_forward", "nnab_stft_filterbank_forward", "nnab_mfcc_fo
 _CHUNK_HEAD = [_P, c_int64, c_int64, c_int64, _P, c_int, c_int64, c_int64, c_int64, c_int]
 _CHUNK_WS_HEAD = [c_int64, c_int64, c_int64, c_int64, c_int]
 _POOL_HEAD = [_P, _P, _P, c_int64, c_int64, _P, c_int, c_int64, c_int64, c_int64]
+_DEVICE_HEAD = [_P] * 9 + [c_int, c_int64, c_int64, c_int64]
 SIGNATURES["nnab_chunk_state_bytes"] = (c_size_t, [c_int64, c_int])
 for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_forward", "nnab_filterbank"),
                    ("nnab_mfcc_forward", "nnab_mfcc"), ("nnab_cqt1992v2_forward", "nnab_cqt1992v2")):
@@ -140,6 +141,16 @@ for _name, _ws in (("nnab_stft_forward", "nnab_stft"), ("nnab_stft_filterbank_fo
     # and no `center`
     SIGNATURES[_name.replace("_forward", "_pool_forward")] = (_res, _POOL_HEAD + _args[4:])
     SIGNATURES[_ws + "_pool_workspace_bytes"] = (_wres, [c_int64, c_int64] + _wargs[2:5] + _wargs[6:])
+    # the *_pool_device_forward entry points: (state, counters, lengths, end, errors, error_info, counts,
+    # d_lanes, chunk, chunk_dtype, slots, n, chunk_pitch) in place of (x, B, L, x_pitch)
+    SIGNATURES[_name.replace("_forward", "_pool_device_forward")] = (_res, _DEVICE_HEAD + _args[4:])
+SIGNATURES["nnab_pool_frame_cap"] = (c_int64, [c_int64, c_int, c_int, c_int, c_int])
+SIGNATURES["nnab_istft_pool_sample_cap"] = (c_int64, [c_int64, c_int, c_int, c_int])
+SIGNATURES["nnab_istft_pool_device_forward"] = (
+    c_int, [_P] * 9 + [c_int64, _P, c_int, c_int64, _P, _P, c_int, c_int, c_int, _P, c_int64, _P, c_size_t, _P])
+SIGNATURES["nnab_pool_device_reset"] = (c_int, [_P, _P, _P, _P, c_int64, _P])
+SIGNATURES["nnab_debug_device_pool_plan"] = (c_int, [_P] * 7 + [c_int64, c_int64, c_int, c_int, c_int, c_int])
+SIGNATURES["nnab_debug_device_istft_plan"] = (c_int, [_P] * 8 + [c_int64, c_int64, c_int, c_int, c_int])
 SIGNATURES["nnab_cqt_pyramid_chunk_state_bytes"] = (c_size_t, [c_int64, c_int, _P, c_int, c_int])
 SIGNATURES["nnab_cqt_pyramid_chunk_workspace_bytes"] = (
     c_size_t, [c_int64, c_int64, c_int64, c_int64, c_int64, c_int, c_int, _P, c_int, c_int, c_int])
@@ -928,6 +939,134 @@ def istft_pool_forward(pool, lanes, X, A, n_max, T_max, packed, window, n_fft, h
             T_max, _ptr(ws), wsb, _stream(dev))
     _check(rc, "nnab_istft_pool_forward")
     return out
+
+
+# --------------------------------------------------------------------------- #
+# device pools (nnaudio_b200.streaming.DeviceStreamPool / DeviceInversePool): every per-push number on the device.
+# The arguments that do not change from push to push (module buffers, outputs, workspace) are bound once.
+# --------------------------------------------------------------------------- #
+LANE_OK, LANE_ELENGTH, LANE_EENDED, LANE_ESHORT, LANE_ENOFRAMES, LANE_ELENGTH_SHORT = range(6)
+
+
+def pool_frame_cap(chunk: int, K: int, hop: int, pad: int, pad_mode: int) -> int:
+    """The most frames one push of at most ``chunk`` samples can return, an end included."""
+    return int(lib().nnab_pool_frame_cap(int(chunk), int(K), int(hop), int(pad), int(pad_mode)))
+
+
+def istft_pool_sample_cap(frames: int, n_fft: int, hop: int, center: bool) -> int:
+    """The most samples one inverse push of at most ``frames`` frames can return, a flush included."""
+    return int(lib().nnab_istft_pool_sample_cap(int(frames), int(n_fft), int(hop), int(center)))
+
+
+def pool_device_bind(name, kw, slots, T_cap, device, path=None):
+    """The fixed part of a device pool's pushes on the offline call ``name`` with arguments ``kw``: returns
+    (C function, output (slots, ..., T_cap), workspace, argument tail after the chunk pitch, stream excluded)."""
+    L = lib()
+    path = resolve_path(path)
+    hop = kw["hop"]
+    if name in ("stft_forward", "stft_filterbank_forward", "mfcc_forward"):
+        n_fft, F = kw["n_fft"], kw["wcos"].shape[0]
+        head = (_ptr(kw["wcos"]), _ptr(kw["wsin"]), _ptr(kw["packed"]), n_fft, F, hop, int(kw["center"]),
+                kw["pad_mode"])
+        has_table = int(kw.get("fb_table") is not None)
+        if name == "stft_forward":
+            fmt = kw["out_format"]
+            shape = (slots, F, T_cap, 2) if fmt == FMT_COMPLEX else (slots, F, T_cap)
+            nbytes = L.nnab_stft_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, path)
+            mid = head + (fmt, kw["sqrt_eps"])
+        elif name == "stft_filterbank_forward":
+            n_fb = kw["fb"].shape[0]
+            shape = (slots, n_fb, T_cap)
+            nbytes = L.nnab_filterbank_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, n_fb, path, has_table)
+            mid = head + (kw["sqrt_eps"], kw["power"], _ptr(kw["fb"]), n_fb, _ptr(kw.get("fb_table")))
+        else:
+            n_mels, n_mfcc = kw["mel_basis"].shape[0], kw["dct"].shape[0]
+            shape = (slots, n_mfcc, T_cap)
+            nbytes = L.nnab_mfcc_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, n_mels, path, has_table)
+            top_db = kw["top_db"]
+            mid = head + (kw["sqrt_eps"], kw["power"], _ptr(kw["mel_basis"]), n_mels, _ptr(kw.get("fb_table")),
+                          kw["amin"], kw["ref"], -1.0 if top_db is None else float(top_db), _ptr(kw["dct"]), n_mfcc)
+    elif name == "cqt1992v2_forward":
+        (n_bins, width), fmt = kw["k_real"].shape, kw["out_format"]
+        shape = (slots, n_bins, T_cap) if fmt == FMT_MAGNITUDE else (slots, n_bins, T_cap, 2)
+        nbytes = L.nnab_cqt1992v2_pool_workspace_bytes(slots, T_cap, width, n_bins, hop, path)
+        kb, ke = kw["k_begin"], kw["k_end"]
+        mid = (_ptr(kw["k_real"]), _ptr(kw["k_imag"]), _ptr(kw["packed"]),
+               kb.ctypes.data_as(c_void_p) if kb is not None else None,
+               ke.ctypes.data_as(c_void_p) if ke is not None else None, n_bins, width, hop, int(kw["center"]),
+               kw["pad_mode"], _ptr(kw["scale"]), kw["scale_all"], fmt, kw["sqrt_eps"])
+    else:
+        raise ValueError(f"no device pool for {name}")
+    out = torch.zeros(shape, dtype=torch.float32, device=device)
+    ws, wsb = _workspace(nbytes, device)
+    fn = getattr(L, "nnab_" + name.replace("_forward", "_pool_device_forward"))
+    return fn, out, ws, mid + (_ptr(out), T_cap, _ptr(ws), wsb, path)
+
+
+def pool_device_forward(pool, x, lengths, end):
+    """One push of a DeviceStreamPool (``pool``: its device buffers and bound call); every argument checked by the
+    caller.  False when the plan cannot read the chunk (NNAB_EUNSUPPORTED)."""
+    dev = pool.ring.device
+    with torch.cuda.device(dev):
+        rc = pool._fn(_ptr(pool.ring), _ptr(pool.counters), _ptr(lengths), _ptr(end), _ptr(pool.errors),
+                      _ptr(pool.error_info), _ptr(pool.counts), _ptr(pool._lanes), _ptr(x), _WAVE_DTYPES[x.dtype],
+                      pool.slots, x.shape[1], x.stride(0) if x.shape[0] > 1 else x.shape[1], *pool._tail,
+                      _stream(dev))
+    if rc == EUNSUPPORTED:
+        return False
+    _check(rc, pool._fn.__name__)
+    return True
+
+
+def istft_pool_device_forward(pool, X, counts, end, length):
+    """One push of a DeviceInversePool; every argument checked by the caller."""
+    dev = pool.state.device
+    with torch.cuda.device(dev):
+        rc = lib().nnab_istft_pool_device_forward(
+            _ptr(pool.state), _ptr(pool.counters), _ptr(counts), _ptr(end), _ptr(length), _ptr(pool.errors),
+            _ptr(pool.error_info), _ptr(pool.counts), _ptr(pool._lanes), pool.slots, _ptr(X), pool.f_in,
+            pool.frames_cap, _ptr(pool._packed), _ptr(pool._window), pool.n_fft, pool.hop, int(pool.center),
+            _ptr(pool.samples), pool.n_cap, _ptr(pool._ws), pool._ws.numel(), _stream(dev))
+    _check(rc, "nnab_istft_pool_device_forward")
+
+
+def pool_device_reset(pool, mask):
+    """Zero the counters, errors and error values of the slots where ``mask`` (uint8 CUDA, or None: all) is set."""
+    dev = pool.counters.device
+    with torch.cuda.device(dev):
+        _check(lib().nnab_pool_device_reset(_ptr(pool.counters), _ptr(pool.errors), _ptr(pool.error_info), _ptr(mask),
+                                            pool.slots, _stream(dev)), "nnab_pool_device_reset")
+
+
+def debug_device_pool_plan(counters, lengths, end, errors, error_info, n, K, hop, pad, pad_mode):
+    """Host-only run of a device pool's plan launch (``nnab_debug_device_pool_plan``) on numpy arrays: counters
+    (3, slots) int64, errors (slots,) int32 and error_info (slots, 2) int64 are updated in place; returns (lanes
+    (slots, 6) int64, counts (slots,) int32)."""
+    slots = len(lengths)
+    lengths = np.ascontiguousarray(lengths, np.int32)
+    end = np.ascontiguousarray(end, np.uint8)
+    lanes = np.zeros((slots, 6), np.int64)
+    counts = np.zeros(slots, np.int32)
+    p = lambda a: a.ctypes.data_as(c_void_p)
+    _check(lib().nnab_debug_device_pool_plan(p(counters), p(lengths), p(end), p(errors), p(error_info), p(counts),
+                                             p(lanes), slots, int(n), int(K), int(hop), int(pad), int(pad_mode)),
+           "nnab_debug_device_pool_plan")
+    return lanes, counts
+
+
+def debug_device_istft_plan(counters, frame_counts, end, length, errors, error_info, t, n_fft, hop, center):
+    """``debug_device_pool_plan`` for a device inverse pool: returns (lanes (slots, 7) int64, counts (slots,))."""
+    slots = len(frame_counts)
+    frame_counts = np.ascontiguousarray(frame_counts, np.int32)
+    end = np.ascontiguousarray(end, np.uint8)
+    length = np.ascontiguousarray(length, np.int64)
+    lanes = np.zeros((slots, 7), np.int64)
+    counts = np.zeros(slots, np.int32)
+    p = lambda a: a.ctypes.data_as(c_void_p)
+    _check(lib().nnab_debug_device_istft_plan(p(counters), p(frame_counts), p(end), p(length), p(errors),
+                                              p(error_info), p(counts), p(lanes), slots, int(t), int(n_fft), int(hop),
+                                              int(center)), "nnab_debug_device_istft_plan")
+    return lanes, counts
 
 
 def pack_istft_basis(kernel_cos: torch.Tensor, kernel_sin: torch.Tensor, f_in: int, onesided: bool):

@@ -180,6 +180,42 @@ __host__ __device__ inline int64_t chunk_carry_start(int64_t total, int64_t fram
   return s < total ? s : total;
 }
 
+// Host counters of a stream: `received` raw samples so far, the last `n_carry` of them in the carry ring,
+// `frames` frames returned.
+struct StreamStep {
+  int64_t total;      // raw samples after the push
+  int64_t t_end;      // frames returned after the push
+  int64_t T;          // frames this push returns
+  int64_t from;       // raw samples [from, total) go into the ring after the push
+};
+
+// One push of one stream: n new samples, the last push iff `end`.  NNAB_EINVAL for counters no stream can
+// have (they must be those of a stream that returned every ready frame) and for an end the stream is too
+// short for (reflect padding needs pad < total; at least one frame).  The streams of *_chunk_forward, every
+// lane of a pool and every slot of a device pool's plan launch are checked here.
+__host__ __device__ inline int stream_step(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int end,
+                                           int K, int hop, int pad, int pad_mode, StreamStep* o) {
+  if (received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
+  if (frames != chunk_ready_frames(received, K, hop, pad, pad_mode) ||
+      n_carry != received - chunk_carry_start(received, frames, hop, pad))
+    return NNAB_EINVAL;
+  const int64_t total = received + n;
+  int64_t t_end;
+  if (end) {
+    if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad >= total) return NNAB_EINVAL;
+    t_end = chunk_end_frames(total, K, hop, pad);
+    if (t_end <= 0) return NNAB_EINVAL;
+  } else {
+    t_end = chunk_ready_frames(total, K, hop, pad, pad_mode);
+  }
+  o->total = total;
+  o->t_end = t_end;
+  o->T = t_end - frames;
+  const int64_t keep = chunk_carry_start(total, t_end, hop, pad);
+  o->from = keep > received ? keep : received;
+  return NNAB_OK;
+}
+
 // Frames a pool lane has returned after its push (the library has checked the lane on the host).
 __host__ __device__ inline int64_t lane_frames_after(const nnab_stream_lane& ln, int K, int hop, int pad,
                                                      int pad_mode) {
@@ -358,6 +394,91 @@ __host__ __device__ inline IstftChunkPlan istft_lane_plan(const nnab_istft_lane&
   return pl;
 }
 
+// ---- device pools (DESIGN §3.10 "Device pools"): one slot's share of the plan launch, shared by the kernel and
+// the host-only debug entry point.  counters is (3, slots); a dropped push leaves them as they are, writes an
+// all-zero lane (no frame, no sample, no carry: the lane-aware kernels map it to nothing) and keeps the slot's
+// first error code until its reset.
+__host__ __device__ inline void device_lane_error(int64_t s, int code, int64_t a, int64_t b, int32_t* errors,
+                                                  int64_t* info) {
+  if (errors[s] != NNAB_LANE_OK) return;
+  errors[s] = code;
+  info[2 * s] = a;
+  info[2 * s + 1] = b;
+}
+
+__host__ __device__ inline void device_pool_slot(int64_t s, int64_t slots, int64_t* counters, const int32_t* lengths,
+                                                 const uint8_t* end_in, int32_t* errors, int64_t* info,
+                                                 int32_t* counts, nnab_stream_lane* lanes, int64_t chunk, int K,
+                                                 int hop, int pad, int pad_mode) {
+  const int64_t received = counters[s], frames = counters[slots + s];
+  const bool ended = counters[2 * slots + s] != 0;
+  const int64_t n = lengths[s];
+  const int end = end_in[s] != 0;
+  nnab_stream_lane ln{};
+  ln.slot = s;
+  int64_t T = 0;
+  int code = NNAB_LANE_OK;
+  StreamStep st{};
+  if (n < 0 || n > chunk) {
+    code = NNAB_LANE_ELENGTH;
+  } else if (ended && (n > 0 || end)) {
+    code = NNAB_LANE_EENDED;
+  } else if (n > 0 || end) {
+    const int64_t n_carry = received - chunk_carry_start(received, frames, hop, pad);
+    if (stream_step(received, n_carry, frames, n, end, K, hop, pad, pad_mode, &st) != NNAB_OK) {
+      code = NNAB_LANE_ESHORT;  // the counters are the plan's own: only the end can be refused
+    } else {
+      ln.received = received; ln.n_carry = n_carry; ln.frames = frames; ln.n = n; ln.end = end;
+      T = st.T;
+      counters[s] = st.total;
+      counters[slots + s] = st.t_end;
+      counters[2 * slots + s] = ended || end;
+    }
+  }
+  if (code != NNAB_LANE_OK)
+    device_lane_error(s, code, code == NNAB_LANE_ESHORT ? received + n : n, 0, errors, info);
+  lanes[s] = ln;
+  counts[s] = (int32_t)T;
+}
+
+__host__ __device__ inline void device_istft_slot(int64_t s, int64_t slots, int64_t* counters,
+                                                  const int32_t* frame_counts, const uint8_t* end_in,
+                                                  const int64_t* length_in, int32_t* errors, int64_t* info,
+                                                  int32_t* counts, nnab_istft_lane* lanes, int64_t t, int n_fft,
+                                                  int hop, int center) {
+  const int64_t frames = counters[s], emitted = counters[slots + s];
+  const bool ended = counters[2 * slots + s] != 0;
+  const int64_t T = frame_counts[s];
+  const int end = end_in[s] != 0;
+  const int64_t length = end ? (length_in[s] < 0 ? -1 : length_in[s]) : -1;
+  nnab_istft_lane ln{};
+  ln.slot = s; ln.row = -1; ln.length = -1;
+  int64_t n_out = 0;
+  int code = NNAB_LANE_OK;
+  IstftChunkPlan pl{};
+  if (T < 0 || T > t) {
+    code = NNAB_LANE_ELENGTH;
+  } else if (ended && (T > 0 || end)) {
+    code = NNAB_LANE_EENDED;
+  } else if (end && frames + T == 0) {
+    code = NNAB_LANE_ENOFRAMES;
+  } else if (T > 0 || end) {
+    if (istft_chunk_plan(frames, emitted, T, n_fft, hop, center, end, length, &pl) != NNAB_OK) {
+      code = NNAB_LANE_ELENGTH_SHORT;  // the counters are the plan's own: only the length can be refused
+    } else {
+      ln.row = T > 0 ? s : -1; ln.frames = frames; ln.emitted = emitted; ln.T = T; ln.end = end; ln.length = length;
+      n_out = pl.emit_end - pl.emit_begin;
+      counters[s] = frames + T;
+      counters[slots + s] = emitted + n_out;
+      counters[2 * slots + s] = ended || end;
+    }
+  }
+  if (code != NNAB_LANE_OK)
+    device_lane_error(s, code, code == NNAB_LANE_ELENGTH_SHORT ? length : T, emitted, errors, info);
+  lanes[s] = ln;
+  counts[s] = (int32_t)n_out;
+}
+
 struct FramedProblem {
   const void* x;       // (B, L) rows, pitch x_pitch samples of type x_dtype
   int x_dtype;         // NNAB_DTYPE_*: only the pad / split pre-pass reads 16-bit samples, the SIMT kernel fp32
@@ -436,6 +557,15 @@ int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, 
 int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream);
 int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int64_t T, int cols,
                  cudaStream_t stream);
+// device pools: the plan launches (device_pool_slot / device_istft_slot per slot) and the masked reset
+int tc_device_pool_plan(int64_t slots, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                        int32_t* errors, int64_t* info, int32_t* counts, nnab_stream_lane* lanes, int64_t chunk,
+                        int K, int hop, int pad, int pad_mode, cudaStream_t stream);
+int tc_device_istft_plan(int64_t slots, int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                         const int64_t* length, int32_t* errors, int64_t* info, int32_t* counts,
+                         nnab_istft_lane* lanes, int64_t t, int n_fft, int hop, int center, cudaStream_t stream);
+int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int64_t* info, const uint8_t* mask,
+                         cudaStream_t stream);
 // pyramid pools: the (signal, lane) descriptor table of a push (table[s * n_lanes + i] = pyr_lane_signal of lane i
 // of the DEVICE lane table), every row's carry [keep, R1) of one signal (cs.rows; at most `longest` samples), and
 // the zeroing of frames t >= rows[i].count of row i of out (A, n_rows, T, cols)

@@ -151,42 +151,7 @@ static void set_wave(FramedProblem& p, const Wave& w) {
 }
 
 // ---- chunked streams (DESIGN §3.10) ------------------------------------------------------------
-// Host counters of a stream: `received` raw samples so far, the last `n_carry` of them in the carry ring,
-// `frames` frames returned (chunk_ready_frames / chunk_carry_start in common.cuh).
-struct StreamStep {
-  int64_t total;      // raw samples after the push
-  int64_t t_end;      // frames returned after the push
-  int64_t T;          // frames this push returns
-  int64_t from;       // raw samples [from, total) go into the ring after the push
-};
-
-// One push of one stream: n new samples, the last push iff `end`.  NNAB_EINVAL for counters no stream can
-// have (they must be those of a stream that returned every ready frame) and for an end the stream is too
-// short for (reflect padding needs pad < total; at least one frame).  Both the streams of *_chunk_forward
-// and every lane of a pool are checked here.
-static int stream_step(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int end, int K, int hop,
-                       int pad, int pad_mode, StreamStep* o) {
-  if (received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
-  if (frames != chunk_ready_frames(received, K, hop, pad, pad_mode) ||
-      n_carry != received - chunk_carry_start(received, frames, hop, pad))
-    return NNAB_EINVAL;
-  const int64_t total = received + n;
-  int64_t t_end;
-  if (end) {
-    if (pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad >= total) return NNAB_EINVAL;
-    t_end = chunk_end_frames(total, K, hop, pad);
-    if (t_end <= 0) return NNAB_EINVAL;
-  } else {
-    t_end = chunk_ready_frames(total, K, hop, pad, pad_mode);
-  }
-  o->total = total;
-  o->t_end = t_end;
-  o->T = t_end - frames;
-  const int64_t keep = chunk_carry_start(total, t_end, hop, pad);
-  o->from = keep > received ? keep : received;
-  return NNAB_OK;
-}
-
+// The counters of a stream and one push's step on them: StreamStep / stream_step in common.cuh.
 struct ChunkPlan {
   ChunkSource cs;
   int64_t T;          // frames this push returns
@@ -296,6 +261,50 @@ static int pool_forward(const PoolPlan& pp, int chunk_dtype, int64_t n_lanes, fl
     if ((rc = tc_pool_mask(pp.cs, pp.A, out, rows, pp.T_max, cols, s))) return rc;
   }
   return tc_pool_carry(pp.cs, chunk_dtype, n_lanes, pp.longest, s);
+}
+
+// The host-side checks of a device-planned push and its fixed geometry: every slot is a lane (A = slots), each
+// clip T_max = T_cap frames long, and a lane stores at most the chunk width into its ring.
+static int device_pool_plan(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                            int32_t* errors, int64_t* info, int32_t* counts, nnab_stream_lane* d_lanes,
+                            const void* chunk, int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch, int K,
+                            int hop, int pad, int pad_mode, int64_t T_max, float* out, PoolPlan* o) {
+  if (state == nullptr || counters == nullptr || lengths == nullptr || end == nullptr || errors == nullptr ||
+      info == nullptr || counts == nullptr || d_lanes == nullptr || chunk == nullptr || out == nullptr ||
+      !dtype_ok(chunk_dtype) || slots < 1 || slots > 65535 || n < 1 || chunk_pitch < n || K < 2 || hop <= 0)
+    return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  if (T_max != nnab_pool_frame_cap(n, K, hop, pad, pad_mode)) return NNAB_EINVAL;
+  ChunkSource& c = o->cs;
+  c = ChunkSource{};
+  c.ring = static_cast<const float*>(state);
+  c.ring_pitch = K;
+  c.ring_len = K;
+  c.chunk = chunk;
+  c.chunk_pitch = chunk_pitch;
+  c.length = (T_max - 1) * hop + K;
+  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
+  c.lanes = d_lanes;
+  c.K = K; c.hop = hop; c.pad = pad;
+  o->A = slots;
+  o->T_max = T_max;
+  o->longest = n;
+  return NNAB_OK;
+}
+
+// The plan launch, then the stream pools' body on every slot.
+template <typename Run>
+static int device_pool_forward(const PoolPlan& pp, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                               int32_t* errors, int64_t* info, int32_t* counts, int chunk_dtype, int64_t n, float* out,
+                               int64_t rows, int cols, Run&& run, void* stream) {
+  int rc = check_arch();
+  if (rc) return rc;
+  const int pad_mode = pp.cs.pad_mode;
+  if ((rc = tc_device_pool_plan(pp.A, counters, lengths, end, errors, info, counts,
+                                const_cast<nnab_stream_lane*>(pp.cs.lanes), n, pp.cs.K, pp.cs.hop, pp.cs.pad, pad_mode,
+                                (cudaStream_t)stream)))
+    return rc;
+  return pool_forward(pp, chunk_dtype, pp.A, out, rows, cols, run, stream);
 }
 
 static Wave chunk_wave(const ChunkPlan& cp, int chunk_dtype, int64_t B) {
@@ -2138,6 +2147,10 @@ static int64_t istft_pool_ola_pitch(int64_t T_max, int n_fft, int hop) {
   return (int64_t)align_up((size_t)(2 * (int64_t)n_fft + (int64_t)hop * (T - 1)), 8);
 }
 
+static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t n_lanes, int64_t A, const float* X,
+                          int f_in, int64_t t, const void* packed, const float* window, int n_fft, int hop,
+                          int center, float* out, int64_t n_max, int64_t T_max, void* workspace, cudaStream_t s);
+
 size_t nnab_istft_pool_workspace_bytes(int64_t n_lanes, int f_in, int64_t T_max, int n_fft, int hop) {
   if (n_lanes <= 0) return 0;
   return nnab_istft_workspace_bytes(n_lanes, f_in, T_max > 0 ? T_max : 1, n_fft, hop) +
@@ -2183,9 +2196,15 @@ int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nna
   const size_t need = nnab_istft_pool_workspace_bytes(n_lanes, f_in, T_max, n_fft, hop);
   if (n_lanes > 0 && (workspace == nullptr || ws_bytes < need)) return NNAB_EWORKSPACE;
   if (n_lanes == 0) return NNAB_OK;
-  cudaStream_t s = (cudaStream_t)stream;
-  float* carry = static_cast<float*>(state);
+  return istft_pool_run(static_cast<float*>(state), d_lanes, n_lanes, A, X, f_in, t, packed, window, n_fft, hop,
+                        center, out, n_max, T_max, workspace, (cudaStream_t)stream);
+}
 
+// The launches of an inverse pool push on a checked lane table (seed, pre-pass and GEMM, finalize).
+static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t n_lanes, int64_t A, const float* X,
+                          int f_in, int64_t t, const void* packed, const float* window, int n_fft, int hop,
+                          int center, float* out, int64_t n_max, int64_t T_max, void* workspace, cudaStream_t s) {
+  int rc;
   // nnab_istft_forward's layout for n_lanes x max(T_max, 1) frames, each row `lead` positions longer
   const int64_t lead = n_fft;
   const int64_t ola_pitch = istft_pool_ola_pitch(T_max, n_fft, hop);
@@ -2216,6 +2235,73 @@ int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nna
   // 3. every lane's final samples / window sum-square (rows i < A of out, zeros up to n_max), its tail carried
   return tc_istft_pool_finalize(d_lanes, n_lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center, out, n_max,
                                 carry, s);
+}
+
+// ---- device pools (DESIGN §3.10 "Device pools") -----------------------------------------------------------
+// n_cap: a push of `frames` frames returns the most samples on a flush with the longest length, after enough
+// frames that neither the centre crop nor the earliest possible end hold any back: the whole overlap-add span of
+// the new frames past the first returned position, hop * frames + max(n_fft - hop, offset).  Pushes before the
+// end return at most hop * frames.
+int64_t nnab_istft_pool_sample_cap(int64_t frames, int n_fft, int hop, int center) {
+  if (frames < 1 || n_fft <= 0 || hop <= 0 || hop > n_fft) return 0;
+  const int64_t offset = center ? n_fft / 2 : 0;
+  return (int64_t)hop * frames + (n_fft - hop > offset ? n_fft - hop : offset);
+}
+
+int nnab_istft_pool_device_forward(void* state, int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                                   const int64_t* length, int32_t* errors, int64_t* error_info, int32_t* counts,
+                                   nnab_istft_lane* d_lanes, int64_t slots, const float* X, int f_in, int64_t t,
+                                   const void* packed, const float* window, int n_fft, int hop, int center,
+                                   float* out, int64_t n_max, void* workspace, size_t ws_bytes, void* stream) {
+  if (state == nullptr || counters == nullptr || frame_counts == nullptr || end == nullptr || length == nullptr ||
+      errors == nullptr || error_info == nullptr || counts == nullptr || d_lanes == nullptr || X == nullptr ||
+      packed == nullptr || window == nullptr || out == nullptr || slots < 1 || slots > 65535 || f_in <= 0 || t < 1 ||
+      n_max != nnab_istft_pool_sample_cap(t, n_fft, hop, center))
+    return NNAB_EINVAL;
+  int rc = check_arch();
+  if (rc) return rc;
+  if (workspace == nullptr || ws_bytes < nnab_istft_pool_workspace_bytes(slots, f_in, t, n_fft, hop))
+    return NNAB_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = tc_device_istft_plan(slots, counters, frame_counts, end, length, errors, error_info, counts, d_lanes, t,
+                                 n_fft, hop, center, s)))
+    return rc;
+  return istft_pool_run(static_cast<float*>(state), d_lanes, slots, slots, X, f_in, t, packed, window, n_fft, hop,
+                        center, out, n_max, t, workspace, s);
+}
+
+int nnab_pool_device_reset(int64_t* counters, int32_t* errors, int64_t* error_info, const uint8_t* mask,
+                           int64_t slots, void* stream) {
+  if (counters == nullptr || errors == nullptr || error_info == nullptr || slots < 1 || slots > 65535)
+    return NNAB_EINVAL;
+  const int rc = check_arch();
+  if (rc) return rc;
+  return tc_device_pool_reset(slots, counters, errors, error_info, mask, (cudaStream_t)stream);
+}
+
+int nnab_debug_device_pool_plan(int64_t* counters, const int32_t* lengths, const uint8_t* end, int32_t* errors,
+                                int64_t* error_info, int32_t* counts, nnab_stream_lane* lanes, int64_t slots,
+                                int64_t n, int K, int hop, int pad, int pad_mode) {
+  if (counters == nullptr || lengths == nullptr || end == nullptr || errors == nullptr || error_info == nullptr ||
+      counts == nullptr || lanes == nullptr || slots < 1 || n < 1 || K < 2 || hop <= 0 || pad < 0 || 2 * pad > K ||
+      (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT))
+    return NNAB_EINVAL;
+  for (int64_t s = 0; s < slots; ++s)
+    device_pool_slot(s, slots, counters, lengths, end, errors, error_info, counts, lanes, n, K, hop, pad, pad_mode);
+  return NNAB_OK;
+}
+
+int nnab_debug_device_istft_plan(int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                                 const int64_t* length, int32_t* errors, int64_t* error_info, int32_t* counts,
+                                 nnab_istft_lane* lanes, int64_t slots, int64_t t, int n_fft, int hop, int center) {
+  if (counters == nullptr || frame_counts == nullptr || end == nullptr || length == nullptr || errors == nullptr ||
+      error_info == nullptr || counts == nullptr || lanes == nullptr || slots < 1 || t < 1 || n_fft <= 0 ||
+      hop <= 0 || hop > n_fft)
+    return NNAB_EINVAL;
+  for (int64_t s = 0; s < slots; ++s)
+    device_istft_slot(s, slots, counters, frame_counts, end, length, errors, error_info, counts, lanes, t, n_fft,
+                      hop, center);
+  return NNAB_OK;
 }
 
 // ------------------------------------------------------------- input gradient ----
@@ -2516,6 +2602,97 @@ int nnab_cqt1992v2_pool_forward(void* state, const nnab_stream_lane* lanes, cons
     return NNAB_EINVAL;
   return pool_forward(pp, chunk_dtype, n_lanes, out, n_bins, format_cols(out_format),
                       [&](const Wave& w, cudaStream_t s) {
+    return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
+                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+// ------------------------------------------------------------ device pools ----
+// T_cap: frame t is ready once thr(t) samples have arrived, so a stream one sample short of its first frame
+// (thr - 1 samples: K - pad, and with reflect padding at least pad + 1) that takes `chunk` more and ends returns
+// the most frames, ((thr - 1) + chunk + 2 pad - K) / hop + 1.  Later positions return at most
+// ceil((chunk + pad) / hop), never more.
+int64_t nnab_pool_frame_cap(int64_t chunk, int K, int hop, int pad, int pad_mode) {
+  if (chunk < 1 || K < 2 || hop <= 0 || pad < 0 || 2 * pad > K) return 0;
+  const int64_t need = (int64_t)K - pad;
+  const int64_t thr = pad > 0 && pad_mode == NNAB_PAD_REFLECT && pad + 1 > need ? pad + 1 : need;
+  return (thr - 1 + chunk + 2 * (int64_t)pad - K) / hop + 1;
+}
+
+int nnab_stft_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                  int32_t* errors, int64_t* error_info, int32_t* counts, nnab_stream_lane* d_lanes,
+                                  const void* chunk, int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                  const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                                  int center, int pad_mode, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                  void* workspace, size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = device_pool_plan(state, counters, lengths, end, errors, error_info, counts, d_lanes, chunk, chunk_dtype,
+                            slots, n, chunk_pitch, n_fft, hop, center ? n_fft / 2 : 0, pad_mode, T_max, out, &pp);
+  if (rc) return rc;
+  if (F <= 0 || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
+  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, F,
+                             format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
+    return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T_max, workspace, ws_bytes,
+                    path, s);
+  }, stream);
+}
+
+int nnab_stft_filterbank_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths,
+                                             const uint8_t* end, int32_t* errors, int64_t* error_info,
+                                             int32_t* counts, nnab_stream_lane* d_lanes, const void* chunk,
+                                             int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                             const float* wcos, const float* wsin, const void* packed, int n_fft,
+                                             int F, int hop, int center, int pad_mode, float sqrt_eps, float power,
+                                             const float* fb, int n_fb, const void* fb_table, float* out,
+                                             int64_t T_max, void* workspace, size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = device_pool_plan(state, counters, lengths, end, errors, error_info, counts, d_lanes, chunk, chunk_dtype,
+                            slots, n, chunk_pitch, n_fft, hop, center ? n_fft / 2 : 0, pad_mode, T_max, out, &pp);
+  if (rc) return rc;
+  if (F <= 0 || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
+  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_fb, 1,
+                             [&](const Wave& w, cudaStream_t s) {
+    return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T_max,
+                          workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+int nnab_mfcc_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                  int32_t* errors, int64_t* error_info, int32_t* counts, nnab_stream_lane* d_lanes,
+                                  const void* chunk, int chunk_dtype, int64_t slots, int64_t n, int64_t chunk_pitch,
+                                  const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
+                                  int center, int pad_mode, float sqrt_eps, float power, const float* mel_basis,
+                                  int n_mels, const void* fb_table, float amin, float ref, float top_db,
+                                  const float* dct, int n_mfcc, float* out, int64_t T_max, void* workspace,
+                                  size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = device_pool_plan(state, counters, lengths, end, errors, error_info, counts, d_lanes, chunk, chunk_dtype,
+                            slots, n, chunk_pitch, n_fft, hop, center ? n_fft / 2 : 0, pad_mode, T_max, out, &pp);
+  if (rc) return rc;
+  // the top_db floor is a maximum over the whole clip: a stream cannot apply it frame by frame
+  if (F <= 0 || top_db >= 0.f || mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin)) return NNAB_EINVAL;
+  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_mfcc, 1,
+                             [&](const Wave& w, cudaStream_t s) {
+    return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
+                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s);
+  }, stream);
+}
+
+int nnab_cqt1992v2_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                       int32_t* errors, int64_t* error_info, int32_t* counts,
+                                       nnab_stream_lane* d_lanes, const void* chunk, int chunk_dtype, int64_t slots,
+                                       int64_t n, int64_t chunk_pitch, const float* k_real, const float* k_imag,
+                                       const void* packed, const int32_t* h_k_begin, const int32_t* h_k_end,
+                                       int n_bins, int width, int hop, int center, int pad_mode, const float* scale,
+                                       float scale_all, int out_format, float sqrt_eps, float* out, int64_t T_max,
+                                       void* workspace, size_t ws_bytes, int path, void* stream) {
+  PoolPlan pp;
+  int rc = device_pool_plan(state, counters, lengths, end, errors, error_info, counts, d_lanes, chunk, chunk_dtype,
+                            slots, n, chunk_pitch, width, hop, center ? width / 2 : 0, pad_mode, T_max, out, &pp);
+  if (rc) return rc;
+  if (n_bins <= 0 || cqt1992v2_args_ok(k_real, k_imag, out_format)) return NNAB_EINVAL;
+  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_bins,
+                             format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
                          out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s);
   }, stream);

@@ -228,6 +228,8 @@ __global__ void __launch_bounds__(256) chunk_split_kernel(
       bool live = true;
       if (r < 0) {
         if (reflect) r = -r; else live = false;
+        // a device pool's row without frames may mirror past its own samples: nothing to read there
+        if constexpr (LANES) if (r >= c.total) live = false;
       } else if (r >= c.total) {
         // a pool row's clip runs past its own right padding (the longest row sets the length): zeros there
         if (c.at_end && reflect && (!LANES || r - c.total < c.pad)) r = 2 * (c.total - 1) - r; else live = false;
@@ -278,6 +280,65 @@ __global__ void __launch_bounds__(256) pool_mask_kernel(ChunkSource c, float* __
     const int64_t r = k / row_len;
     o[r * T * cols + count * cols + (k - r * row_len)] = 0.f;
   }
+}
+
+// ---- device pools (DESIGN §3.10 "Device pools"): one thread per slot --------------------------------------
+__global__ void __launch_bounds__(128) device_pool_plan_kernel(
+    int64_t slots, int64_t* __restrict__ counters, const int32_t* __restrict__ lengths,
+    const uint8_t* __restrict__ end, int32_t* __restrict__ errors, int64_t* __restrict__ info,
+    int32_t* __restrict__ counts, nnab_stream_lane* __restrict__ lanes, int64_t chunk, int K, int hop, int pad,
+    int pad_mode) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= slots) return;
+  device_pool_slot(s, slots, counters, lengths, end, errors, info, counts, lanes, chunk, K, hop, pad, pad_mode);
+}
+
+__global__ void __launch_bounds__(128) device_istft_plan_kernel(
+    int64_t slots, int64_t* __restrict__ counters, const int32_t* __restrict__ frame_counts,
+    const uint8_t* __restrict__ end, const int64_t* __restrict__ length, int32_t* __restrict__ errors,
+    int64_t* __restrict__ info, int32_t* __restrict__ counts, nnab_istft_lane* __restrict__ lanes, int64_t t,
+    int n_fft, int hop, int center) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= slots) return;
+  device_istft_slot(s, slots, counters, frame_counts, end, length, errors, info, counts, lanes, t, n_fft, hop,
+                    center);
+}
+
+__global__ void __launch_bounds__(128) device_pool_reset_kernel(int64_t slots, int64_t* __restrict__ counters,
+                                                                int32_t* __restrict__ errors,
+                                                                int64_t* __restrict__ info,
+                                                                const uint8_t* __restrict__ mask) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= slots || (mask != nullptr && mask[s] == 0)) return;
+  counters[s] = counters[slots + s] = counters[2 * slots + s] = 0;
+  errors[s] = NNAB_LANE_OK;
+  info[2 * s] = info[2 * s + 1] = 0;
+}
+
+int tc_device_pool_plan(int64_t slots, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                        int32_t* errors, int64_t* info, int32_t* counts, nnab_stream_lane* lanes, int64_t chunk,
+                        int K, int hop, int pad, int pad_mode, cudaStream_t stream) {
+  device_pool_plan_kernel<<<(unsigned)ceil_div64(slots, 128), 128, 0, stream>>>(
+      slots, counters, lengths, end, errors, info, counts, lanes, chunk, K, hop, pad, pad_mode);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_device_istft_plan(int64_t slots, int64_t* counters, const int32_t* frame_counts, const uint8_t* end,
+                         const int64_t* length, int32_t* errors, int64_t* info, int32_t* counts,
+                         nnab_istft_lane* lanes, int64_t t, int n_fft, int hop, int center, cudaStream_t stream) {
+  device_istft_plan_kernel<<<(unsigned)ceil_div64(slots, 128), 128, 0, stream>>>(
+      slots, counters, frame_counts, end, length, errors, info, counts, lanes, t, n_fft, hop, center);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int64_t* info, const uint8_t* mask,
+                         cudaStream_t stream) {
+  device_pool_reset_kernel<<<(unsigned)ceil_div64(slots, 128), 128, 0, stream>>>(slots, counters, errors, info,
+                                                                                   mask);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
 }
 
 // ---- pyramid pools (DESIGN §3.10 "Pyramid pools"): the kernels that know where each row's samples come from --

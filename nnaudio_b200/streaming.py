@@ -30,6 +30,9 @@ output samples no later frame can change, ``flush(length=None)`` the rest.
 ``InversePool(module, slots)`` is ``StreamPool``'s counterpart for the inverse STFT: each
 ``push(X, slots, counts, end, length)`` appends ``X[r, :, :counts[r]]`` to slot ``slots[r]``'s stream and ends the
 flagged slots; a ``PoolOutput`` of ``StreamPool`` feeds it as is.
+
+``DeviceStreamPool`` and ``DeviceInversePool`` are ``StreamPool`` and ``InversePool`` with their counters, lengths
+and end flags on the GPU and one fixed geometry per push, so a serving tick can be captured in a CUDA graph.
 """
 from __future__ import annotations
 
@@ -49,7 +52,7 @@ from .features.stft import STFT, _inverse_args, iSTFT
 from .features.vqt import VQT
 
 __all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "PyramidPool", "StreamingInverse",
-           "InversePool", "InverseOutput"]
+           "InversePool", "InverseOutput", "DeviceStreamPool", "DeviceInversePool"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
 _PYRAMIDS = (CQT2010v2, VQT, CQT2010)
@@ -882,3 +885,218 @@ class InversePool:
         self.emitted[active] += count
         self.ended[active] |= end[active]
         return InverseOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
+
+
+# ---- device pools (DESIGN.md §3.10 "Device pools") ------------------------------------------------------------- #
+def _device_vector(v, what, slots, dtype, device):
+    """``v`` as a device pool's push reads it: a contiguous (slots,) tensor of ``dtype`` on ``device``."""
+    if not isinstance(v, torch.Tensor):
+        raise TypeError(f"{what} must be a torch.Tensor on {device}, filled in place each push")
+    if v.device != device:
+        raise TypeError(f"{what} must be on {device}: the push reads it there, got {v.device}")
+    if v.dtype != dtype:
+        raise TypeError(f"{what} must be {dtype}, got {v.dtype}")
+    if tuple(v.shape) != (slots,) or not v.is_contiguous():
+        raise ValueError(f"{what} must hold one value per slot ({slots}), contiguous, got shape {tuple(v.shape)}")
+    return v
+
+
+def _first_error(pool):
+    """(slot, code, info a, info b) of the lowest slot with an error code, or None; synchronises."""
+    errors = pool.errors.cpu()
+    bad = torch.nonzero(errors).flatten()
+    if len(bad) == 0:
+        return None
+    s = int(bad[0])
+    a, b = pool.error_info[s].tolist()
+    return s, int(errors[s]), a, b
+
+
+def _ended_error(s):
+    return RuntimeError(f"slot {s}: its stream has ended; call reset([{s}]) to start a new one")
+
+
+class DeviceStreamPool:
+    """``StreamPool`` with every per-push number on the GPU: a push reads nothing on the host and has one fixed
+    geometry, so it can be captured in a CUDA graph (``torch.cuda.graph``) and replayed.
+
+    ``DeviceStreamPool(module, slots, chunk, dtype=torch.float32, **forward_kwargs)``: ``module`` and
+    ``forward_kwargs`` are ``StreamPool``'s; ``chunk`` is the fixed chunk width and ``dtype`` the fixed sample type
+    (float32, bfloat16 or float16).  ``push(x, lengths, end=None)``: ``x`` is a (slots, chunk) CUDA tensor of that
+    type, ``lengths`` an int32 and ``end`` a bool (slots,) tensor on the same device; slot s appends
+    ``x[s, :lengths[s]]`` and ends where ``end[s]``.  The push overwrites the pool-owned ``frames`` (slots, ...,
+    T_cap) float32 and ``counts`` (slots,) int32: row s holds slot s's new frames, ``counts[s]`` of them, then exact
+    zeros.  Concatenated up to its counts, a slot's rows equal ``StreamPool`` on the same packets (the same
+    bit-for-bit rules and CQT1992v2 exception).  ``reset(restart=None)`` starts new streams where the bool device
+    mask ``restart`` is set (None: every slot); it too is one launch and can be captured.
+
+    ``T_cap`` is the most frames one push of at most ``chunk`` samples can return, an end included, derived from
+    the framing.  Every slot is computed on every push at ``T_cap`` frames, so an idle slot costs its share of the
+    launch (``StreamPool`` computes only the slots with new frames, at their longest count, but reads its
+    bookkeeping on the host).  A push cannot raise for its values: a slot whose push ``StreamPool`` would refuse (a
+    length outside [0, chunk], samples or an end on an ended stream, an end on a stream too short for the module)
+    is dropped whole -- counters, ring and row untouched, count 0 -- and ``errors[s]`` (int32, device) keeps the
+    first such code until the slot's reset, while the other slots proceed.  ``check()`` synchronises and raises
+    what ``StreamPool`` would have raised, naming the slot.  There is no concat route: a plan without a fused pool
+    route (``NNAUDIO_B200_PATH=simt``) raises at construction.  The constructor builds every cache a push uses and
+    allocates the state, counters (``counters``: received, frames, ended per slot), outputs and workspace, so a
+    captured push allocates nothing.
+    """
+
+    def __init__(self, module, slots, chunk, dtype=torch.float32, **forward_kwargs):
+        slots, chunk = int(slots), int(chunk)
+        if slots < 1 or slots > _C.MAX_BATCH:
+            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        if chunk < 1:
+            raise ValueError(f"chunk must be at least 1 sample, got {chunk}")
+        if dtype not in _C._WAVE_DTYPES:
+            raise ValueError(f"dtype must be float32, bfloat16 or float16, got {dtype}")
+        # module checks, the offline call's arguments and the (slots, K) fp32 carry ring: StreamingTransform's
+        self._st = st = StreamingTransform(module, slots, _strict=True, **forward_kwargs)
+        self.module, self.slots, self.chunk, self.dtype = module, slots, chunk, dtype
+        self.K, self.hop, self.pad = st.K, st.hop, st.pad
+        self.ring = st.ring
+        dev = self.ring.device
+        name, self._kw = st._args()  # packed basis, filterbank table (synchronises once), scales: built here
+        self.T_cap = _C.pool_frame_cap(chunk, self.K, self.hop, self.pad, self._kw["pad_mode"])
+        self.counters = torch.zeros((3, slots), dtype=torch.int64, device=dev)
+        self.errors = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self.error_info = torch.zeros((slots, 2), dtype=torch.int64, device=dev)
+        self.counts = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self._lanes = torch.zeros((slots, len(_C.LANE_FIELDS)), dtype=torch.int64, device=dev)
+        self._fn, self.frames, self._ws, self._tail = _C.pool_device_bind(name, self._kw, slots, self.T_cap, dev)
+        self._no_end = torch.zeros(slots, dtype=torch.bool, device=dev)
+        # an idle push changes nothing; it runs the route once and finds a plan that cannot read the chunk
+        idle = torch.zeros(slots, dtype=torch.int32, device=dev)
+        if not _C.pool_device_forward(self, torch.zeros((slots, chunk), dtype=dtype, device=dev), idle, self._no_end):
+            raise RuntimeError(f"{name}: no fused pool route for this configuration (NNAB_EUNSUPPORTED, e.g. "
+                               "NNAUDIO_B200_PATH=simt); DeviceStreamPool has no concat route")
+
+    def reset(self, restart=None):
+        """Start new streams where the bool device mask ``restart`` is set (None: every slot)."""
+        mask = None if restart is None else _device_vector(restart, "restart", self.slots, torch.bool,
+                                                           self.counters.device)
+        _C.pool_device_reset(self, mask)
+
+    def push(self, x: torch.Tensor, lengths: torch.Tensor, end: torch.Tensor = None):
+        """Append ``x[s, :lengths[s]]`` to every slot s and end the slots flagged in ``end``; the new frames go
+        to ``frames`` / ``counts``."""
+        if not isinstance(x, torch.Tensor):
+            raise TypeError("chunk must be a torch.Tensor")
+        if x.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+        if x.dim() != 2 or tuple(x.shape) != (self.slots, self.chunk):
+            raise ValueError(f"chunk must be ({self.slots}, {self.chunk}), got {tuple(x.shape)}")
+        if x.dtype != self.dtype:
+            raise ValueError(f"chunk must be {self.dtype} (the pool's sample type), got {x.dtype}")
+        if x.device != self.ring.device:
+            raise RuntimeError(f"chunk is on {x.device}: the pool runs on {self.ring.device}")
+        if x.stride(-1) != 1 or (self.slots > 1 and x.stride(0) < self.chunk):
+            x = x.contiguous()
+        dev = self.ring.device
+        lengths = _device_vector(lengths, "lengths", self.slots, torch.int32, dev)
+        end = self._no_end if end is None else _device_vector(end, "end", self.slots, torch.bool, dev)
+        if not _C.pool_device_forward(self, x, lengths, end):
+            raise RuntimeError("no fused pool route for this configuration (NNAB_EUNSUPPORTED)")
+
+    def check(self):
+        """Synchronise and raise what ``StreamPool`` would have raised for the lowest slot with an error code."""
+        err = _first_error(self)
+        if err is None:
+            return
+        s, code, a, _ = err
+        if code == _C.LANE_ELENGTH:
+            raise ValueError(f"lengths must be in [0, {self.chunk}] (the chunk width): slot {s} has {a}")
+        if code == _C.LANE_EENDED:
+            raise _ended_error(s)
+        if code == _C.LANE_ESHORT:
+            try:
+                self._st._check_length(a)  # the exception module(x) raises for a stream this short
+            except Exception as e:
+                raise type(e)(f"slot {s}: {e}") from None
+        raise RuntimeError(f"slot {s}: push dropped with error code {code}")
+
+
+class DeviceInversePool:
+    """``InversePool`` with every per-push number on the GPU, capturable in a CUDA graph like ``DeviceStreamPool``.
+
+    ``DeviceInversePool(module, slots, frames, onesided=None)``: ``module`` and ``onesided`` are ``InversePool``'s,
+    ``frames`` the fixed frame capacity of a push.  ``push(X, counts, end=None, length=None)``: ``X`` is (slots,
+    bins, frames, 2) float32 CUDA (row s: slot s's frames; a ``DeviceStreamPool``'s ``frames`` in the Complex format
+    with ``frames=pool.T_cap`` fits), ``counts`` int32, ``end`` bool and ``length`` int64 (-1: None; read where
+    ``end`` is set) (slots,) tensors on the same device; slot s appends ``X[s, :, :counts[s]]``, and ends under
+    ``StreamingInverse.flush``'s rules.  The push overwrites the pool-owned ``samples`` (slots, n_cap) and
+    ``counts`` (slots,) int32: row s holds slot s's new samples, then exact zeros.  ``n_cap`` is the most samples
+    one push of at most ``frames`` frames can return, a flush included.  Concatenated, a slot's rows equal
+    ``InversePool`` on the same packets to fp32 rounding (both overlap-add with fp32 atomics).  Errors, ``check()``,
+    ``reset(restart=None)`` and the cost of idle slots are ``DeviceStreamPool``'s; the refused pushes are
+    ``InversePool``'s (counts outside [0, frames], frames or an end on an ended stream, an end without any frame,
+    a length shorter than the samples already returned).
+    """
+
+    def __init__(self, module, slots, frames, onesided=None):
+        slots, frames = int(slots), int(frames)
+        if slots < 1 or slots > _C.MAX_BATCH:
+            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        if frames < 1:
+            raise ValueError(f"frames must be at least 1, got {frames}")
+        # module checks, the inverse arguments and the (slots, n_fft) fp32 state: StreamingInverse's
+        self._si = si = StreamingInverse(module, slots, onesided=onesided)
+        self.module, self.slots, self.onesided, self.frames_cap = module, slots, si.onesided, frames
+        self.n_fft, self.hop, self.center, self.f_in = si.n_fft, si.hop, si.center, si.f_in
+        self.state = si.state
+        dev = self.state.device
+        _, _, self._packed, self._window = si._args()
+        self.n_cap = _C.istft_pool_sample_cap(frames, self.n_fft, self.hop, self.center)
+        self.counters = torch.zeros((3, slots), dtype=torch.int64, device=dev)  # frames, emitted, ended
+        self.errors = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self.error_info = torch.zeros((slots, 2), dtype=torch.int64, device=dev)
+        self.counts = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self.samples = torch.zeros((slots, self.n_cap), dtype=torch.float32, device=dev)
+        self._lanes = torch.zeros((slots, len(_C.ISTFT_LANE_FIELDS)), dtype=torch.int64, device=dev)
+        self._ws = torch.empty(_C.lib().nnab_istft_pool_workspace_bytes(slots, self.f_in, frames, self.n_fft,
+                                                                         self.hop), dtype=torch.uint8, device=dev)
+        self._no_end = torch.zeros(slots, dtype=torch.bool, device=dev)
+        self._no_length = torch.full((slots,), -1, dtype=torch.int64, device=dev)
+        idle = torch.zeros(slots, dtype=torch.int32, device=dev)  # an idle push changes nothing
+        _C.istft_pool_device_forward(self, torch.zeros((slots, self.f_in, frames, 2), device=dev), idle,
+                                     self._no_end, self._no_length)
+
+    reset = DeviceStreamPool.reset
+
+    def push(self, X: torch.Tensor, counts: torch.Tensor, end: torch.Tensor = None, length: torch.Tensor = None):
+        """Append ``X[s, :, :counts[s]]`` to every slot s and end the slots flagged in ``end``; the new samples go
+        to ``samples`` / ``counts``."""
+        if not isinstance(X, torch.Tensor):
+            raise TypeError("X must be a torch.Tensor")
+        if X.requires_grad:
+            raise NotImplementedError("the streaming API is forward-only: the frames require grad")
+        want = (self.slots, self.f_in, self.frames_cap, 2)
+        if tuple(X.shape) != want:
+            raise ValueError(f"frames must be {want}, got {tuple(X.shape)}")
+        if X.dtype != torch.float32:
+            raise ValueError(f"frames must be float32, got {X.dtype}")
+        dev = self.state.device
+        if X.device != dev:
+            raise RuntimeError(f"X is on {X.device}: the pool runs on {dev}")
+        X = X if X.is_contiguous() else X.contiguous()
+        counts = _device_vector(counts, "counts", self.slots, torch.int32, dev)
+        end = self._no_end if end is None else _device_vector(end, "end", self.slots, torch.bool, dev)
+        length = self._no_length if length is None else _device_vector(length, "length", self.slots, torch.int64, dev)
+        _C.istft_pool_device_forward(self, X, counts, end, length)
+
+    def check(self):
+        """Synchronise and raise what ``InversePool`` would have raised for the lowest slot with an error code."""
+        err = _first_error(self)
+        if err is None:
+            return
+        s, code, a, b = err
+        if code == _C.LANE_ELENGTH:
+            raise ValueError(f"counts must be in [0, {self.frames_cap}] (the frames of X): slot {s} has {a}")
+        if code == _C.LANE_EENDED:
+            raise _ended_error(s)
+        if code == _C.LANE_ENOFRAMES:
+            raise RuntimeError(f"slot {s}: ending a stream without frames; the inverse STFT needs at least one")
+        if code == _C.LANE_ELENGTH_SHORT:
+            raise ValueError(f"slot {s}: length {a} is shorter than the {b} samples already returned")
+        raise RuntimeError(f"slot {s}: push dropped with error code {code}")
