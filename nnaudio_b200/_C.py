@@ -461,104 +461,133 @@ def build_filterbank_table(fb: torch.Tensor):
 
 
 # --------------------------------------------------------------------------- #
-# forward calls
+# the framed transforms (STFT, filterbank, MFCC, CQT1992v2): one argument spec each, read by every call mode.
+# A forward call is (waveform head, transform tail, out, T, workspace, workspace bytes, path, stream); the heads
+# differ by mode (SIGNATURES), the tail is the same in all four.  The workspace queries take (K, F, hop) after
+# their own head, then `center` (offline, chunk), the pad mode (chunk) and the transform's query tail.
 # --------------------------------------------------------------------------- #
+def _kb(k):
+    return k.ctypes.data_as(c_void_p) if k is not None else None
+
+
+class _Spec:
+    """The C names and argument rules of one framed transform; ``kw`` holds its offline call's arguments."""
+
+    def __init__(self, stem, ws, shape, geometry, tail, ws_tail):
+        self.shape = shape        # (rows, T, kw) -> output shape
+        self.geometry = geometry  # kw -> (K, F, hop) of the workspace queries
+        self.tail = tail          # kw -> the arguments between the waveform head and `out`
+        self.ws_tail = ws_tail    # (kw, path) -> the workspace query's arguments after its geometry
+        self.forward, self.ws = f"nnab_{stem}_forward_ex", f"nnab_{ws}_workspace_bytes"
+        self.chunk, self.chunk_ws = f"nnab_{stem}_chunk_forward", f"nnab_{ws}_chunk_workspace_bytes"
+        self.pool, self.pool_ws = f"nnab_{stem}_pool_forward", f"nnab_{ws}_pool_workspace_bytes"
+        self.device = f"nnab_{stem}_pool_device_forward"
+
+
+def _stft_geometry(kw):
+    return kw["n_fft"], kw["wcos"].shape[0], kw["hop"]
+
+
+def _stft_head(kw):
+    return (_ptr(kw["wcos"]), _ptr(kw["wsin"]), _ptr(kw["packed"]), kw["n_fft"], kw["wcos"].shape[0], kw["hop"],
+            int(kw["center"]), kw["pad_mode"])
+
+
+def _has_table(kw):
+    return int(kw.get("fb_table") is not None)
+
+
+def _complex_shape(rows, bins, T, complex_out):
+    return (rows, bins, T, 2) if complex_out else (rows, bins, T)
+
+
+_SPECS = {
+    "stft_forward": _Spec(
+        "stft", "stft",
+        lambda B, T, kw: _complex_shape(B, kw["wcos"].shape[0], T, kw["out_format"] == FMT_COMPLEX),
+        _stft_geometry,
+        lambda kw: _stft_head(kw) + (kw["out_format"], kw["sqrt_eps"]),
+        lambda kw, path: (path,)),
+    "stft_filterbank_forward": _Spec(
+        "stft_filterbank", "filterbank",
+        lambda B, T, kw: (B, kw["fb"].shape[0], T),
+        _stft_geometry,
+        lambda kw: _stft_head(kw) + (kw["sqrt_eps"], kw["power"], _ptr(kw["fb"]), kw["fb"].shape[0],
+                                     _ptr(kw.get("fb_table"))),
+        lambda kw, path: (kw["fb"].shape[0], path, _has_table(kw))),
+    "mfcc_forward": _Spec(
+        "mfcc", "mfcc",
+        lambda B, T, kw: (B, kw["dct"].shape[0], T),
+        _stft_geometry,
+        lambda kw: _stft_head(kw) + (kw["sqrt_eps"], kw["power"], _ptr(kw["mel_basis"]), kw["mel_basis"].shape[0],
+                                     _ptr(kw.get("fb_table")), kw["amin"], kw["ref"],
+                                     -1.0 if kw["top_db"] is None else float(kw["top_db"]), _ptr(kw["dct"]),
+                                     kw["dct"].shape[0]),
+        lambda kw, path: (kw["mel_basis"].shape[0], path, _has_table(kw))),
+    "cqt1992v2_forward": _Spec(
+        "cqt1992v2", "cqt1992v2",
+        lambda B, T, kw: _complex_shape(B, kw["k_real"].shape[0], T, kw["out_format"] != FMT_MAGNITUDE),
+        lambda kw: (kw["k_real"].shape[1], kw["k_real"].shape[0], kw["hop"]),
+        lambda kw: (_ptr(kw["k_real"]), _ptr(kw["k_imag"]), _ptr(kw["packed"]), _kb(kw["k_begin"]),
+                    _kb(kw["k_end"]), kw["k_real"].shape[0], kw["k_real"].shape[1], kw["hop"], int(kw["center"]),
+                    kw["pad_mode"], _ptr(kw["scale"]), kw["scale_all"], kw["out_format"], kw["sqrt_eps"]),
+        lambda kw, path: (path,)),
+}
+
+
+def _offline(name, x, kw):
+    spec, L = _SPECS[name], lib()
+    x, B, Ln, pitch, dt = _wave_rows(x)
+    K, F, hop = spec.geometry(kw)
+    pad = K // 2 if kw["center"] else 0
+    T = (Ln + 2 * pad - K) // hop + 1
+    out = _new_out(spec.shape(B, T, kw), x.device)
+    path = resolve_path(kw["path"])
+    tail = spec.tail(kw)
+    fn = getattr(L, spec.forward)
+    with torch.cuda.device(x.device):
+        ws, wsb = _workspace(getattr(L, spec.ws)(B, Ln, K, F, hop, int(kw["center"]), *spec.ws_tail(kw, path)),
+                             x.device)
+        rc = _call_wave(lambda xs, p, d: fn(_ptr(xs), d, B, Ln, p, *tail, _ptr(out), T, _ptr(ws), wsb, path,
+                                            _stream(x.device)), x, pitch, dt, kw["strict_dtype"])
+    _check(rc, spec.forward)
+    return out
+
+
 # x of the forward calls: a float32, bfloat16 or float16 (B, L) CUDA tensor; the output is float32.
 @_batch_chunked
 def stft_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format, sqrt_eps,
                  path=None, strict_dtype=False):
-    L = lib()
-    x, B, Ln, pitch, dt = _wave_rows(x)
-    F = wcos.shape[0]
-    pad = n_fft // 2 if center else 0
-    T = (Ln + 2 * pad - n_fft) // hop + 1
-    shape = (B, F, T, 2) if out_format == FMT_COMPLEX else (B, F, T)
-    out = _new_out(shape, x.device)
-    path = resolve_path(path)
-    with torch.cuda.device(x.device):
-        ws, wsb = _workspace(L.nnab_stft_workspace_bytes(B, Ln, n_fft, F, hop, int(center), path),
-                             x.device)
-        rc = _call_wave(lambda xs, p, d: L.nnab_stft_forward_ex(
-            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center),
-            pad_mode, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)),
-            x, pitch, dt, strict_dtype)
-    _check(rc, "nnab_stft_forward_ex")
-    return out
+    return _offline("stft_forward", x, locals())
 
 
 @_batch_chunked
 def stft_filterbank_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
                             fb, fb_table=None, path=None, strict_dtype=False):
-    L = lib()
-    x, B, Ln, pitch, dt = _wave_rows(x)
-    F = wcos.shape[0]
-    n_fb = fb.shape[0]
-    pad = n_fft // 2 if center else 0
-    T = (Ln + 2 * pad - n_fft) // hop + 1
-    out = _new_out((B, n_fb, T), x.device)
-    path = resolve_path(path)
-    with torch.cuda.device(x.device):
-        ws, wsb = _workspace(
-            L.nnab_filterbank_workspace_bytes(B, Ln, n_fft, F, hop, int(center), n_fb, path,
-                                              int(fb_table is not None)),
-            x.device)
-        rc = _call_wave(lambda xs, p, d: L.nnab_stft_filterbank_forward_ex(
-            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
-            int(center), pad_mode, sqrt_eps, power, _ptr(fb), n_fb, _ptr(fb_table), _ptr(out), T,
-            _ptr(ws), wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
-    _check(rc, "nnab_stft_filterbank_forward_ex")
-    return out
+    return _offline("stft_filterbank_forward", x, locals())
 
 
 @_batch_chunked
 def mfcc_forward(x, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power, mel_basis,
                  amin, ref, top_db, dct, fb_table=None, path=None, strict_dtype=False):
-    L = lib()
-    x, B, Ln, pitch, dt = _wave_rows(x)
-    F = wcos.shape[0]
-    n_mels = mel_basis.shape[0]
-    n_mfcc = dct.shape[0]
-    pad = n_fft // 2 if center else 0
-    T = (Ln + 2 * pad - n_fft) // hop + 1
-    out = _new_out((B, n_mfcc, T), x.device)
-    path = resolve_path(path)
-    with torch.cuda.device(x.device):
-        ws, wsb = _workspace(
-            L.nnab_mfcc_workspace_bytes(B, Ln, n_fft, F, hop, int(center), n_mels, path,
-                                        int(fb_table is not None)), x.device)
-        rc = _call_wave(lambda xs, p, d: L.nnab_mfcc_forward_ex(
-            _ptr(xs), d, B, Ln, p, _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop,
-            int(center), pad_mode, sqrt_eps, power, _ptr(mel_basis), n_mels, _ptr(fb_table), amin, ref,
-            -1.0 if top_db is None else float(top_db), _ptr(dct), n_mfcc, _ptr(out), T, _ptr(ws),
-            wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
-    _check(rc, "nnab_mfcc_forward_ex")
-    return out
+    return _offline("mfcc_forward", x, locals())
 
 
 @_batch_chunked
 def cqt1992v2_forward(x, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode, scale,
                       scale_all, out_format, sqrt_eps, path=None, strict_dtype=False):
     """k_begin / k_end: host int32 numpy arrays (per-bin support) or None."""
-    L = lib()
-    x, B, Ln, pitch, dt = _wave_rows(x)
-    n_bins, width = k_real.shape
-    pad = width // 2 if center else 0
-    T = (Ln + 2 * pad - width) // hop + 1
-    shape = (B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2)
-    out = _new_out(shape, x.device)
-    path = resolve_path(path)
-    kb = k_begin.ctypes.data_as(c_void_p) if k_begin is not None else None
-    ke = k_end.ctypes.data_as(c_void_p) if k_end is not None else None
-    with torch.cuda.device(x.device):
-        ws, wsb = _workspace(
-            L.nnab_cqt1992v2_workspace_bytes(B, Ln, width, n_bins, hop, int(center), path),
-            x.device)
-        rc = _call_wave(lambda xs, p, d: L.nnab_cqt1992v2_forward_ex(
-            _ptr(xs), d, B, Ln, p, _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins,
-            width, hop, int(center), pad_mode, _ptr(scale), scale_all, out_format, sqrt_eps,
-            _ptr(out), T, _ptr(ws), wsb, path, _stream(x.device)), x, pitch, dt, strict_dtype)
-    _check(rc, "nnab_cqt1992v2_forward_ex")
-    return out
+    return _offline("cqt1992v2_forward", x, locals())
+
+
+def _bank_arrays(banks_real, banks_imag, packed):
+    """The pyramid's per-octave C arrays: bank pointers (real, imaginary), packed bases (NULL where absent) and
+    bank widths."""
+    n = len(banks_real)
+    return ((c_void_p * n)(*[t.data_ptr() for t in banks_real]),
+            (c_void_p * n)(*[t.data_ptr() for t in banks_imag]),
+            (c_void_p * n)(*[(t.data_ptr() if t is not None else None) for t in packed]),
+            (c_int32 * n)(*[int(t.shape[1]) for t in banks_real]))
 
 
 @_batch_chunked
@@ -571,13 +600,9 @@ def cqt_pyramid_forward(x, banks_real, banks_imag, packed, lowpass, lowpass_pack
     x, B, Ln, pitch, dt = _wave_rows(x)
     n_oct = len(banks_real)
     n_filters = banks_real[0].shape[0]
-    re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
-    im_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_imag])
-    pk_arr = (c_void_p * n_oct)(*[(t.data_ptr() if t is not None else None) for t in packed])
-    widths = (c_int32 * n_oct)(*[int(t.shape[1]) for t in banks_real])
-    max_width = max(int(t.shape[1]) for t in banks_real)
-    shape = (B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2)
-    out = _new_out(shape, x.device)
+    re_arr, im_arr, pk_arr, widths = _bank_arrays(banks_real, banks_imag, packed)
+    max_width = max(widths)
+    out = _new_out(_complex_shape(B, n_bins, T, out_format != FMT_MAGNITUDE), x.device)
     path = resolve_path(path)
     with torch.cuda.device(x.device):
         ws, wsb = _workspace(
@@ -605,8 +630,12 @@ def chunk_state_bytes(B: int, K: int) -> int:
 
 
 def _chunk_args(st, x):
-    if x is None or x.shape[-1] == 0:
+    """(chunk, n, pitch, NNAB sample type) of a push: the chunk's type, or the stream's when there is no chunk
+    (a flush)."""
+    if x is None:
         return None, 0, 0, _WAVE_DTYPES[st.dtype]
+    if x.shape[-1] == 0:
+        return None, 0, 0, _WAVE_DTYPES[x.dtype]
     x, _, n, pitch, dt = _wave_rows(x)
     return x, n, pitch, dt
 
@@ -618,176 +647,93 @@ def _chunk_result(rc, out, what):
     return out
 
 
+def _chunk(name, st, x, flush, T, kw):
+    spec, L = _SPECS[name], lib()
+    xs, n, pitch, dt = _chunk_args(st, x)
+    B, dev = st.batch, st.ring.device
+    out = torch.empty(spec.shape(B, T, kw), dtype=torch.float32, device=dev)
+    path = resolve_path(kw["path"])
+    with torch.cuda.device(dev):
+        ws, wsb = _workspace(getattr(L, spec.chunk_ws)(B, st.received, st.frames, n, int(flush), *spec.geometry(kw),
+                                                       int(kw["center"]), kw["pad_mode"], *spec.ws_tail(kw, path)), dev)
+        rc = getattr(L, spec.chunk)(
+            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush), *spec.tail(kw),
+            _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, spec.chunk)
+
+
 def stft_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format, sqrt_eps,
                        path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(st, x)
-    B, F, dev = st.batch, wcos.shape[0], st.ring.device
-    out = torch.empty((B, F, T, 2) if out_format == FMT_COMPLEX else (B, F, T), dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        ws, wsb = _workspace(L.nnab_stft_chunk_workspace_bytes(B, st.received, st.frames, n, int(flush), n_fft, F,
-                                                               hop, int(center), pad_mode, path), dev)
-        rc = L.nnab_stft_chunk_forward(
-            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
-            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, out_format, sqrt_eps,
-            _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_stft_chunk_forward")
+    return _chunk("stft_forward", st, x, flush, T, locals())
 
 
 def stft_filterbank_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps,
                                   power, fb, fb_table=None, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(st, x)
-    B, F, n_fb, dev = st.batch, wcos.shape[0], fb.shape[0], st.ring.device
-    out = torch.empty((B, n_fb, T), dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        ws, wsb = _workspace(L.nnab_filterbank_chunk_workspace_bytes(
-            B, st.received, st.frames, n, int(flush), n_fft, F, hop, int(center), pad_mode, n_fb, path,
-            int(fb_table is not None)), dev)
-        rc = L.nnab_stft_filterbank_chunk_forward(
-            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
-            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(fb),
-            n_fb, _ptr(fb_table), _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_stft_filterbank_chunk_forward")
+    return _chunk("stft_filterbank_forward", st, x, flush, T, locals())
 
 
 def mfcc_chunk_forward(st, x, flush, T, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
                        mel_basis, amin, ref, top_db, dct, fb_table=None, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(st, x)
-    B, F, n_mels, n_mfcc, dev = st.batch, wcos.shape[0], mel_basis.shape[0], dct.shape[0], st.ring.device
-    out = torch.empty((B, n_mfcc, T), dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        ws, wsb = _workspace(L.nnab_mfcc_chunk_workspace_bytes(
-            B, st.received, st.frames, n, int(flush), n_fft, F, hop, int(center), pad_mode, n_mels, path,
-            int(fb_table is not None)), dev)
-        rc = L.nnab_mfcc_chunk_forward(
-            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
-            _ptr(wcos), _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power,
-            _ptr(mel_basis), n_mels, _ptr(fb_table), amin, ref, -1.0 if top_db is None else float(top_db),
-            _ptr(dct), n_mfcc, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_mfcc_chunk_forward")
+    return _chunk("mfcc_forward", st, x, flush, T, locals())
 
 
 def cqt1992v2_chunk_forward(st, x, flush, T, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode, scale,
                             scale_all, out_format, sqrt_eps, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(st, x)
-    (n_bins, width), B, dev = k_real.shape, st.batch, st.ring.device
-    out = torch.empty((B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2), dtype=torch.float32,
-                      device=dev)
-    path = resolve_path(path)
-    kb = k_begin.ctypes.data_as(c_void_p) if k_begin is not None else None
-    ke = k_end.ctypes.data_as(c_void_p) if k_end is not None else None
-    with torch.cuda.device(dev):
-        ws, wsb = _workspace(L.nnab_cqt1992v2_chunk_workspace_bytes(
-            B, st.received, st.frames, n, int(flush), width, n_bins, hop, int(center), pad_mode, path), dev)
-        rc = L.nnab_cqt1992v2_chunk_forward(
-            _ptr(st.ring), st.received, st.n_carry, st.frames, _ptr(xs), dt, B, n, pitch, int(flush),
-            _ptr(k_real), _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode,
-            _ptr(scale), scale_all, out_format, sqrt_eps, _ptr(out), T, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_cqt1992v2_chunk_forward")
+    return _chunk("cqt1992v2_forward", st, x, flush, T, locals())
 
 
 # --------------------------------------------------------------------------- #
 # pool calls (nnaudio_b200.streaming.StreamPool): one push of a stream pool.  `pool` carries the device carry
-# ring (pool.ring, one row per slot), pool.slots and pool.dtype; `lanes` is the push's (n_lanes, 6) int64 lane
-# table (nnab_stream_lane rows, the A lanes with frames first); `x` the (slots, n) chunk or None.  The remaining
-# arguments are those of the offline call.  Returns the (A, ..., T_max) frames, or None when the plan cannot
-# read a chunk (NNAB_EUNSUPPORTED, nothing enqueued).
+# ring (pool.ring, one row per slot) and pool.slots; `lanes` is the push's (n_lanes, 6) int64 lane table
+# (nnab_stream_lane rows, the A lanes with frames first); `x` the (slots, n) chunk.  The remaining arguments are
+# those of the offline call.  Returns the (A, ..., T_max) frames, or None when the plan cannot read a chunk
+# (NNAB_EUNSUPPORTED, nothing enqueued).
 # --------------------------------------------------------------------------- #
 LANE_FIELDS = ("slot", "received", "n_carry", "frames", "n", "end")
 
 
-def _pool_lanes(pool, lanes):
+def _lane_copies(lanes, device):
     """Host and device copies of a lane table: the host copy in pinned memory, the device copy made from it
     without blocking (torch's host allocator keeps the pinned block until the copy has run)."""
-    return _lane_copies(lanes, pool.ring.device)
-
-
-def _lane_copies(lanes, device):
     if len(lanes) == 0:
         return None, None
     host = torch.as_tensor(lanes, dtype=torch.int64).contiguous().pin_memory()
     return host, host.to(device, non_blocking=True)
 
 
+def _pool(name, pool, lanes, x, A, T_max, kw):
+    spec, L = _SPECS[name], lib()
+    xs, n, pitch, dt = _chunk_args(pool, x)
+    dev = pool.ring.device
+    out = torch.empty(spec.shape(A, T_max, kw), dtype=torch.float32, device=dev)
+    path = resolve_path(kw["path"])
+    with torch.cuda.device(dev):
+        hl, dl = _lane_copies(lanes, dev)
+        ws, wsb = _workspace(getattr(L, spec.pool_ws)(A, T_max, *spec.geometry(kw), *spec.ws_tail(kw, path)), dev)
+        rc = getattr(L, spec.pool)(
+            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, *spec.tail(kw),
+            _ptr(out), T_max, _ptr(ws), wsb, path, _stream(dev))
+    return _chunk_result(rc, out, spec.pool)
+
+
 def stft_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode, out_format,
                       sqrt_eps, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(pool, x)
-    F, dev = wcos.shape[0], pool.ring.device
-    out = torch.empty((A, F, T_max, 2) if out_format == FMT_COMPLEX else (A, F, T_max), dtype=torch.float32,
-                      device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        hl, dl = _pool_lanes(pool, lanes)
-        ws, wsb = _workspace(L.nnab_stft_pool_workspace_bytes(A, T_max, n_fft, F, hop, path), dev)
-        rc = L.nnab_stft_pool_forward(
-            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
-            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, out_format, sqrt_eps, _ptr(out), T_max,
-            _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_stft_pool_forward")
+    return _pool("stft_forward", pool, lanes, x, A, T_max, locals())
 
 
 def stft_filterbank_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode,
                                  sqrt_eps, power, fb, fb_table=None, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(pool, x)
-    F, n_fb, dev = wcos.shape[0], fb.shape[0], pool.ring.device
-    out = torch.empty((A, n_fb, T_max), dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        hl, dl = _pool_lanes(pool, lanes)
-        ws, wsb = _workspace(L.nnab_filterbank_pool_workspace_bytes(A, T_max, n_fft, F, hop, n_fb, path,
-                                                                    int(fb_table is not None)), dev)
-        rc = L.nnab_stft_filterbank_pool_forward(
-            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
-            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(fb), n_fb,
-            _ptr(fb_table), _ptr(out), T_max, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_stft_filterbank_pool_forward")
+    return _pool("stft_filterbank_forward", pool, lanes, x, A, T_max, locals())
 
 
 def mfcc_pool_forward(pool, lanes, x, A, T_max, wcos, wsin, packed, n_fft, hop, center, pad_mode, sqrt_eps, power,
                       mel_basis, amin, ref, top_db, dct, fb_table=None, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(pool, x)
-    F, n_mels, n_mfcc, dev = wcos.shape[0], mel_basis.shape[0], dct.shape[0], pool.ring.device
-    out = torch.empty((A, n_mfcc, T_max), dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    with torch.cuda.device(dev):
-        hl, dl = _pool_lanes(pool, lanes)
-        ws, wsb = _workspace(L.nnab_mfcc_pool_workspace_bytes(A, T_max, n_fft, F, hop, n_mels, path,
-                                                              int(fb_table is not None)), dev)
-        rc = L.nnab_mfcc_pool_forward(
-            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(wcos),
-            _ptr(wsin), _ptr(packed), n_fft, F, hop, int(center), pad_mode, sqrt_eps, power, _ptr(mel_basis), n_mels,
-            _ptr(fb_table), amin, ref, -1.0 if top_db is None else float(top_db), _ptr(dct), n_mfcc, _ptr(out),
-            T_max, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_mfcc_pool_forward")
+    return _pool("mfcc_forward", pool, lanes, x, A, T_max, locals())
 
 
 def cqt1992v2_pool_forward(pool, lanes, x, A, T_max, k_real, k_imag, packed, k_begin, k_end, hop, center, pad_mode,
                            scale, scale_all, out_format, sqrt_eps, path=None):
-    L = lib()
-    xs, n, pitch, dt = _chunk_args(pool, x)
-    (n_bins, width), dev = k_real.shape, pool.ring.device
-    out = torch.empty((A, n_bins, T_max) if out_format == FMT_MAGNITUDE else (A, n_bins, T_max, 2),
-                      dtype=torch.float32, device=dev)
-    path = resolve_path(path)
-    kb = k_begin.ctypes.data_as(c_void_p) if k_begin is not None else None
-    ke = k_end.ctypes.data_as(c_void_p) if k_end is not None else None
-    with torch.cuda.device(dev):
-        hl, dl = _pool_lanes(pool, lanes)
-        ws, wsb = _workspace(L.nnab_cqt1992v2_pool_workspace_bytes(A, T_max, width, n_bins, hop, path), dev)
-        rc = L.nnab_cqt1992v2_pool_forward(
-            _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, _ptr(k_real),
-            _ptr(k_imag), _ptr(packed), kb, ke, n_bins, width, hop, int(center), pad_mode, _ptr(scale), scale_all,
-            out_format, sqrt_eps, _ptr(out), T_max, _ptr(ws), wsb, path, _stream(dev))
-    return _chunk_result(rc, out, "nnab_cqt1992v2_pool_forward")
+    return _pool("cqt1992v2_forward", pool, lanes, x, A, T_max, locals())
 
 
 def cqt_pyramid_chunk_state_bytes(B: int, widths, hop: int, early_factor: int) -> int:
@@ -818,12 +764,8 @@ def cqt_pyramid_chunk_forward(st, x, flush, T, banks_real, banks_imag, packed, l
     xs, n, pitch, dt = _chunk_args(st, x)
     B, dev = st.batch, st.ring.device
     n_oct = len(banks_real)
-    re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
-    im_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_imag])
-    pk_arr = (c_void_p * n_oct)(*[(t.data_ptr() if t is not None else None) for t in packed])
-    widths = (c_int32 * n_oct)(*[int(t.shape[1]) for t in banks_real])
-    out = torch.empty((B, n_bins, T) if out_format == FMT_MAGNITUDE else (B, n_bins, T, 2), dtype=torch.float32,
-                      device=dev)
+    re_arr, im_arr, pk_arr, widths = _bank_arrays(banks_real, banks_imag, packed)
+    out = torch.empty(_complex_shape(B, n_bins, T, out_format != FMT_MAGNITUDE), dtype=torch.float32, device=dev)
     path = resolve_path(path)
     with torch.cuda.device(dev):
         ws, wsb = _workspace(L.nnab_cqt_pyramid_chunk_workspace_bytes(
@@ -869,27 +811,22 @@ def cqt_pyramid_pool_forward(pool, lanes, x, A, T_max, banks_real, banks_imag, p
                              early_filter, early_packed, early_factor, hop, pad_mode, n_bins, scale, scale_all,
                              out_format, sqrt_eps, path=None):
     """One push of ``nnaudio_b200.streaming.PyramidPool``: ``lanes`` its (n_lanes, 6) lane table (the A lanes with
-    frames first), ``x`` the (slots, n) chunk or None; ``pool`` carries the rings (``pool.ring``), ``pool.slots``
-    and ``pool.dtype``.  The remaining arguments are ``cqt_pyramid_forward``'s.  Returns the (A, n_bins, T_max[, 2])
-    frames, or None when the configuration has no streamed plan (NNAB_EUNSUPPORTED, nothing enqueued)."""
+    frames first), ``x`` the (slots, n) chunk; ``pool`` carries the rings (``pool.ring``) and ``pool.slots``.  The
+    remaining arguments are ``cqt_pyramid_forward``'s.  Returns the (A, n_bins, T_max[, 2]) frames, or None when the configuration has no streamed plan (NNAB_EUNSUPPORTED, nothing enqueued)."""
     L = lib()
     xs, n, pitch, dt = _chunk_args(pool, x)
     dev = pool.ring.device
-    out = torch.empty((A, n_bins, T_max) if out_format == FMT_MAGNITUDE else (A, n_bins, T_max, 2),
-                      dtype=torch.float32, device=dev)
+    out = torch.empty(_complex_shape(A, n_bins, T_max, out_format != FMT_MAGNITUDE), dtype=torch.float32, device=dev)
     n_oct = len(banks_real)
-    re_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_real])
-    im_arr = (c_void_p * n_oct)(*[t.data_ptr() for t in banks_imag])
-    pk_arr = (c_void_p * n_oct)(*[(t.data_ptr() if t is not None else None) for t in packed])
-    widths = [int(t.shape[1]) for t in banks_real]
+    re_arr, im_arr, pk_arr, widths = _bank_arrays(banks_real, banks_imag, packed)
     path = resolve_path(path)
     with torch.cuda.device(dev):
         ws, wsb = _workspace(cqt_pyramid_pool_workspace_bytes(lanes, A, T_max, widths, hop, early_factor, pad_mode),
                              dev)
-        hl, dl = _pool_lanes(pool, lanes)
+        hl, dl = _lane_copies(lanes, dev)
         rc = L.nnab_cqt_pyramid_pool_forward(
             _ptr(pool.ring), _ptr(hl), _ptr(dl), len(lanes), A, _ptr(xs), dt, pool.slots, n, pitch, n_oct, re_arr,
-            im_arr, pk_arr, (c_int32 * n_oct)(*widths), banks_real[0].shape[0], _ptr(lowpass), _ptr(lowpass_packed),
+            im_arr, pk_arr, widths, banks_real[0].shape[0], _ptr(lowpass), _ptr(lowpass_packed),
             _ptr(early_filter), _ptr(early_packed), early_factor, hop, pad_mode, n_bins, _ptr(scale), scale_all,
             out_format, sqrt_eps, _ptr(out) if out.numel() else None, T_max, _ptr(ws), wsb, path, _stream(dev))
     return _chunk_result(rc, out, "nnab_cqt_pyramid_pool_forward")
@@ -961,46 +898,13 @@ def istft_pool_sample_cap(frames: int, n_fft: int, hop: int, center: bool) -> in
 def pool_device_bind(name, kw, slots, T_cap, device, path=None):
     """The fixed part of a device pool's pushes on the offline call ``name`` with arguments ``kw``: returns
     (C function, output (slots, ..., T_cap), workspace, argument tail after the chunk pitch, stream excluded)."""
-    L = lib()
-    path = resolve_path(path)
-    hop = kw["hop"]
-    if name in ("stft_forward", "stft_filterbank_forward", "mfcc_forward"):
-        n_fft, F = kw["n_fft"], kw["wcos"].shape[0]
-        head = (_ptr(kw["wcos"]), _ptr(kw["wsin"]), _ptr(kw["packed"]), n_fft, F, hop, int(kw["center"]),
-                kw["pad_mode"])
-        has_table = int(kw.get("fb_table") is not None)
-        if name == "stft_forward":
-            fmt = kw["out_format"]
-            shape = (slots, F, T_cap, 2) if fmt == FMT_COMPLEX else (slots, F, T_cap)
-            nbytes = L.nnab_stft_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, path)
-            mid = head + (fmt, kw["sqrt_eps"])
-        elif name == "stft_filterbank_forward":
-            n_fb = kw["fb"].shape[0]
-            shape = (slots, n_fb, T_cap)
-            nbytes = L.nnab_filterbank_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, n_fb, path, has_table)
-            mid = head + (kw["sqrt_eps"], kw["power"], _ptr(kw["fb"]), n_fb, _ptr(kw.get("fb_table")))
-        else:
-            n_mels, n_mfcc = kw["mel_basis"].shape[0], kw["dct"].shape[0]
-            shape = (slots, n_mfcc, T_cap)
-            nbytes = L.nnab_mfcc_pool_workspace_bytes(slots, T_cap, n_fft, F, hop, n_mels, path, has_table)
-            top_db = kw["top_db"]
-            mid = head + (kw["sqrt_eps"], kw["power"], _ptr(kw["mel_basis"]), n_mels, _ptr(kw.get("fb_table")),
-                          kw["amin"], kw["ref"], -1.0 if top_db is None else float(top_db), _ptr(kw["dct"]), n_mfcc)
-    elif name == "cqt1992v2_forward":
-        (n_bins, width), fmt = kw["k_real"].shape, kw["out_format"]
-        shape = (slots, n_bins, T_cap) if fmt == FMT_MAGNITUDE else (slots, n_bins, T_cap, 2)
-        nbytes = L.nnab_cqt1992v2_pool_workspace_bytes(slots, T_cap, width, n_bins, hop, path)
-        kb, ke = kw["k_begin"], kw["k_end"]
-        mid = (_ptr(kw["k_real"]), _ptr(kw["k_imag"]), _ptr(kw["packed"]),
-               kb.ctypes.data_as(c_void_p) if kb is not None else None,
-               ke.ctypes.data_as(c_void_p) if ke is not None else None, n_bins, width, hop, int(kw["center"]),
-               kw["pad_mode"], _ptr(kw["scale"]), kw["scale_all"], fmt, kw["sqrt_eps"])
-    else:
+    if name not in _SPECS:
         raise ValueError(f"no device pool for {name}")
-    out = torch.zeros(shape, dtype=torch.float32, device=device)
-    ws, wsb = _workspace(nbytes, device)
-    fn = getattr(L, "nnab_" + name.replace("_forward", "_pool_device_forward"))
-    return fn, out, ws, mid + (_ptr(out), T_cap, _ptr(ws), wsb, path)
+    spec, L = _SPECS[name], lib()
+    path = resolve_path(path)
+    out = torch.zeros(spec.shape(slots, T_cap, kw), dtype=torch.float32, device=device)
+    ws, wsb = _workspace(getattr(L, spec.pool_ws)(slots, T_cap, *spec.geometry(kw), *spec.ws_tail(kw, path)), device)
+    return getattr(L, spec.device), out, ws, spec.tail(kw) + (_ptr(out), T_cap, _ptr(ws), wsb, path)
 
 
 def pool_device_forward(pool, x, lengths, end):

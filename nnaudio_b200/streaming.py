@@ -36,7 +36,6 @@ and end flags on the GPU and one fixed geometry per push, so a serving tick can 
 """
 from __future__ import annotations
 
-from types import SimpleNamespace
 from typing import NamedTuple
 
 import numpy as np
@@ -75,6 +74,65 @@ def _carry_start(total, frames, hop, pad):
     return min(max(s, 0), total)
 
 
+def _streams(v, what):
+    """``batch`` / ``slots`` of a constructor: how many streams one C call may carry."""
+    v = int(v)
+    if v < 1 or v > _C.MAX_BATCH:
+        raise ValueError(f"{what} must be in [1, {_C.MAX_BATCH}], got {v}")
+    return v
+
+
+def _check_chunk(chunk, rows, dtype, where="within a stream", width=None):
+    """The checks of a push's chunk: a (rows, n) tensor without grad in a sample type the forward calls read, the
+    same as ``dtype`` (the stream's or the pool's, ``where``) once that is set.  A device pool fixes the width and
+    the sample type (``width``, ``dtype``)."""
+    if not isinstance(chunk, torch.Tensor):
+        raise TypeError("chunk must be a torch.Tensor")
+    if chunk.requires_grad:
+        raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
+    if chunk.dim() != 2 or chunk.shape[0] != rows or (width is not None and chunk.shape[1] != width):
+        raise ValueError(f"chunk must be ({rows}, {'n' if width is None else width}), got {tuple(chunk.shape)}")
+    if width is not None:
+        if chunk.dtype != dtype:
+            raise ValueError(f"chunk must be {dtype} (the pool's sample type), got {chunk.dtype}")
+        return
+    if chunk.dtype not in _C._WAVE_DTYPES:
+        raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
+    if dtype is not None and chunk.dtype != dtype:
+        raise ValueError(f"chunk dtype changed from {dtype} to {chunk.dtype} {where}")
+
+
+def _for_slot(s, check, *args):
+    """``check(*args)``, re-raising what it raises with slot ``s`` named."""
+    try:
+        return check(*args)
+    except Exception as e:
+        raise type(e)(f"slot {s}: {e}") from None
+
+
+def _cpu_ints(v, what, n=None, kind="integers"):
+    """A CPU array of ints (or bools, kind="bools") of shape (n,); device tensors are refused, since reading
+    them would synchronise."""
+    if isinstance(v, torch.Tensor):
+        if v.device.type != "cpu":
+            raise TypeError(f"{what} must be on the CPU: reading it from {v.device} would synchronise")
+        v = v.numpy()
+    a = np.asarray(v)
+    if n is not None and a.shape != (n,):
+        raise ValueError(f"{what} must hold {n} values, got shape {a.shape}")
+    if a.ndim != 1:
+        raise ValueError(f"{what} must be one-dimensional, got shape {a.shape}")
+    if kind == "integers" and a.dtype != bool and (np.issubdtype(a.dtype, np.integer) or a.size == 0):
+        return a.astype(np.int64)
+    if kind == "bools" and (a.dtype == bool or (np.issubdtype(a.dtype, np.integer) and np.isin(a, (0, 1)).all())):
+        return a.astype(bool)
+    raise TypeError(f"{what} must be {kind}, got {a.dtype}")
+
+
+def _ended_error(s):
+    return RuntimeError(f"slot {s}: its stream has ended; call reset([{s}]) to start a new one")
+
+
 class StreamingTransform:
     """Stream ``batch`` signals chunk by chunk through ``module``.
 
@@ -95,9 +153,7 @@ class StreamingTransform:
                 "MFCC with top_db set cannot be streamed: its floor is a maximum over the whole clip. "
                 "Build the module with top_db=None."
             )
-        batch = int(batch)
-        if batch < 1 or batch > _C.MAX_BATCH:
-            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        batch = _streams(batch, "batch")
         self.module, self.batch, self._strict = module, batch, bool(_strict)
         if isinstance(module, (CQT1992v2, CQT1992)):
             fmt = forward_kwargs.get("output_format") or module.output_format
@@ -134,18 +190,8 @@ class StreamingTransform:
         """Feed ``chunk`` (batch, n), any n >= 0; returns the frames completed by it."""
         if self._flushed:
             raise RuntimeError("push() after flush(): call reset() to start new streams")
-        if not isinstance(chunk, torch.Tensor):
-            raise TypeError("chunk must be a torch.Tensor")
-        if chunk.requires_grad:
-            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
-        if chunk.dim() != 2 or chunk.shape[0] != self.batch:
-            raise ValueError(f"chunk must be ({self.batch}, n), got {tuple(chunk.shape)}")
-        if chunk.dtype not in _C._WAVE_DTYPES:
-            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
-        if self.dtype is None:
-            self.dtype = chunk.dtype
-        elif chunk.dtype != self.dtype:
-            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within a stream")
+        _check_chunk(chunk, self.batch, self.dtype)
+        self.dtype = chunk.dtype
         n = chunk.shape[1]
         T = _ready_frames(self.received + n, self.K, self.hop, self.pad, self._reflect) - self.frames
         return self._advance(chunk, n, False, T)
@@ -204,18 +250,7 @@ class StreamingTransform:
 
     def _empty(self, name, kw):
         """The offline call's output layout with no frame."""
-        dev = self.ring.device
-        if name == "stft_forward":
-            F = kw["wcos"].shape[0]
-            return torch.empty((self.batch, F, 0, 2) if kw["out_format"] == _C.FMT_COMPLEX else (self.batch, F, 0),
-                               device=dev)
-        if name == "stft_filterbank_forward":
-            return torch.empty((self.batch, kw["fb"].shape[0], 0), device=dev)
-        if name == "mfcc_forward":
-            return torch.empty((self.batch, kw["dct"].shape[0], 0), device=dev)
-        n_bins = kw["k_real"].shape[0]
-        return torch.empty((self.batch, n_bins, 0) if kw["out_format"] == _C.FMT_MAGNITUDE
-                           else (self.batch, n_bins, 0, 2), device=dev)
+        return torch.empty(_C._SPECS[name].shape(self.batch, 0, kw), device=self.ring.device)
 
 
 class PoolOutput(NamedTuple):
@@ -227,7 +262,70 @@ class PoolOutput(NamedTuple):
     counts: torch.Tensor
 
 
-class StreamPool:
+class _HostPool:
+    """What the host-planned pools share: the per-slot counters (``_COUNTERS``) and ended flags, kept on the host,
+    and their reset."""
+    _COUNTERS = ("received", "frames")
+
+    def _init_slots(self, slots):
+        self.slots = slots
+        for name in self._COUNTERS:
+            setattr(self, name, np.zeros(slots, np.int64))  # host counters of every slot's stream
+        self.ended = np.zeros(slots, bool)
+
+    def reset(self, slots=None):
+        """Start new streams in ``slots`` (all slots by default; then a chunk pool's sample type is free again)."""
+        if slots is None:
+            idx = np.arange(self.slots)
+            if hasattr(self, "dtype"):
+                self.dtype = None
+        else:
+            idx = _cpu_ints(np.reshape(slots.cpu() if isinstance(slots, torch.Tensor) else slots, -1), "slots")
+            if ((idx < 0) | (idx >= self.slots)).any():
+                raise ValueError(f"slots must be in [0, {self.slots}), got {idx.tolist()}")
+        for name in self._COUNTERS:
+            getattr(self, name)[idx] = 0
+        self.ended[idx] = False
+
+    def _refuse_ended(self, new, end):
+        bad = np.flatnonzero(self.ended & (new | end))
+        if len(bad):
+            raise _ended_error(bad[0])
+
+
+class _ChunkPool(_HostPool):
+    """The push of the waveform pools (``StreamPool``, ``PyramidPool``): argument checks, the lane table, the
+    counter commit.  A pool supplies ``_lane_counts`` (its counting rules) and ``_advance`` (the C call)."""
+
+    def push(self, chunk: torch.Tensor, lengths, end=None) -> PoolOutput:
+        """Append ``chunk[s, :lengths[s]]`` to every slot s, end the slots flagged in ``end``; returns the new
+        frames of the slots that have some."""
+        _check_chunk(chunk, self.slots, self.dtype, "within the pool")
+        n = chunk.shape[1]
+        lengths = _cpu_ints(lengths, "lengths", self.slots)
+        end = np.zeros(self.slots, bool) if end is None else _cpu_ints(end, "end", self.slots, "bools")
+        bad = np.flatnonzero((lengths < 0) | (lengths > n))
+        if len(bad):
+            raise ValueError(f"lengths must be in [0, {n}] (the chunk width): slot {bad[0]} has {lengths[bad[0]]}")
+        self._refuse_ended(lengths > 0, end)
+        active = np.flatnonzero((lengths > 0) | end)
+        count, n_carry = self._lane_counts(active, lengths, end)
+        order = np.lexsort((active, count == 0))  # the lanes with frames first, slots ascending in each group
+        active, count, n_carry = active[order], count[order], n_carry[order]
+        A = int((count > 0).sum())
+        T_max = int(count.max()) if A else 0
+        lanes = np.stack([active, self.received[active], n_carry, self.frames[active], lengths[active],
+                          end[active].astype(np.int64)], 1).astype(np.int64)
+        out = self._advance(chunk, lanes, A, T_max, count)
+        # committed once the push has run: a refused push leaves the pool as it was
+        self.dtype = chunk.dtype
+        self.received[active] += lengths[active]
+        self.frames[active] += count
+        self.ended[active] |= end[active]
+        return PoolOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
+
+
+class StreamPool(_ChunkPool):
     """Serve up to ``slots`` independent streams through ``module``, each advancing by its own amount.
 
     ``push(chunk, lengths, end=None)``: ``chunk`` is a (slots, n) CUDA float32 / bfloat16 / float16 tensor and
@@ -248,71 +346,17 @@ class StreamPool:
     """
 
     def __init__(self, module, slots, _strict=False, **forward_kwargs):
-        slots = int(slots)
-        if slots < 1 or slots > _C.MAX_BATCH:
-            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        slots = _streams(slots, "slots")
         # module checks, the offline call's arguments and the (slots, K) fp32 carry ring: StreamingTransform's
         self._st = st = StreamingTransform(module, slots, _strict=_strict, **forward_kwargs)
-        self.module, self.slots, self._strict = module, slots, bool(_strict)
+        self.module, self._strict = module, bool(_strict)
         self.K, self.hop, self.pad, self._reflect = st.K, st.hop, st.pad, st._reflect
         self.ring = st.ring
-        self.received = np.zeros(slots, np.int64)  # host counters of every slot's stream
-        self.frames = np.zeros(slots, np.int64)
-        self.ended = np.zeros(slots, bool)
+        self._init_slots(slots)
         self.dtype = None
 
-    def reset(self, slots=None):
-        """Start new streams in ``slots`` (all slots by default; then the sample type is free again)."""
-        if slots is None:
-            idx = np.arange(self.slots)
-            self.dtype = None
-        else:
-            idx = np.asarray(slots.cpu() if isinstance(slots, torch.Tensor) else slots, dtype=np.int64).reshape(-1)
-            if ((idx < 0) | (idx >= self.slots)).any():
-                raise ValueError(f"slots must be in [0, {self.slots}), got {idx.tolist()}")
-        self.received[idx] = 0
-        self.frames[idx] = 0
-        self.ended[idx] = False
-
-    def _per_slot(self, v, what, integer):
-        if isinstance(v, torch.Tensor):
-            if v.device.type != "cpu":
-                raise TypeError(f"{what} must be on the CPU: reading it from {v.device} would synchronise")
-            v = v.numpy()
-        a = np.asarray(v)
-        if a.shape != (self.slots,):
-            raise ValueError(f"{what} must hold one value per slot ({self.slots}), got shape {a.shape}")
-        if integer and a.dtype != bool and np.issubdtype(a.dtype, np.integer):
-            return a.astype(np.int64)
-        if not integer and (a.dtype == bool or (np.issubdtype(a.dtype, np.integer) and np.isin(a, (0, 1)).all())):
-            return a.astype(bool)
-        raise TypeError(f"{what} must be {'integers' if integer else 'bools'}, got {a.dtype}")
-
-    # ------------------------------------------------------------------------------------------------ #
-    def push(self, chunk: torch.Tensor, lengths, end=None) -> PoolOutput:
-        """Append ``chunk[s, :lengths[s]]`` to every slot s, end the slots flagged in ``end``; returns the new
-        frames of the slots that have some."""
-        if not isinstance(chunk, torch.Tensor):
-            raise TypeError("chunk must be a torch.Tensor")
-        if chunk.requires_grad:
-            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
-        if chunk.dim() != 2 or chunk.shape[0] != self.slots:
-            raise ValueError(f"chunk must be ({self.slots}, n), got {tuple(chunk.shape)}")
-        if chunk.dtype not in _C._WAVE_DTYPES:
-            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
-        if self.dtype is not None and chunk.dtype != self.dtype:
-            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within the pool")
-        n = chunk.shape[1]
-        lengths = self._per_slot(lengths, "lengths", True)
-        end = np.zeros(self.slots, bool) if end is None else self._per_slot(end, "end", False)
-        bad = np.flatnonzero((lengths < 0) | (lengths > n))
-        if len(bad):
-            raise ValueError(f"lengths must be in [0, {n}] (the chunk width): slot {bad[0]} has {lengths[bad[0]]}")
-        bad = np.flatnonzero(self.ended & ((lengths > 0) | end))
-        if len(bad):
-            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
-        # every lane's counters and frame count, by the rules of StreamingTransform (push / flush)
-        active = np.flatnonzero((lengths > 0) | end)
+    def _lane_counts(self, active, lengths, end):
+        """Every lane's frame count and carried samples, by the rules of StreamingTransform (push / flush)."""
         K, hop, pad = self.K, self.hop, self.pad
         count = np.zeros(len(active), np.int64)
         n_carry = np.zeros(len(active), np.int64)
@@ -320,27 +364,12 @@ class StreamPool:
             R, F0 = int(self.received[s]), int(self.frames[s])
             total = R + int(lengths[s])
             if end[s]:
-                try:
-                    self._st._check_length(total)  # the exception module(x) raises for a stream this short
-                except Exception as e:
-                    raise type(e)(f"slot {s}: {e}") from None
+                _for_slot(s, self._st._check_length, total)  # the exception module(x) raises for a stream this short
                 count[j] = (total + 2 * pad - K) // hop + 1 - F0
             else:
                 count[j] = _ready_frames(total, K, hop, pad, self._reflect) - F0
             n_carry[j] = R - _carry_start(R, F0, hop, pad)
-        if self.dtype is None:
-            self.dtype = chunk.dtype
-        order = np.lexsort((active, count == 0))  # the lanes with frames first, slots ascending in each group
-        active, count, n_carry = active[order], count[order], n_carry[order]
-        A = int((count > 0).sum())
-        T_max = int(count.max()) if A else 0
-        lanes = np.stack([active, self.received[active], n_carry, self.frames[active], lengths[active],
-                          end[active].astype(np.int64)], 1).astype(np.int64)
-        out = self._advance(chunk, lanes, A, T_max, count)
-        self.received[active] += lengths[active]
-        self.frames[active] += count
-        self.ended[active] |= end[active]
-        return PoolOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
+        return count, n_carry
 
     # ------------------------------------------------------------------------------------------------ #
     def _advance(self, chunk, lanes, A, T_max, count):
@@ -388,22 +417,6 @@ class StreamPool:
         return out
 
 
-def _check_chunk(st, chunk):
-    """The checks every push makes (shape, dtype, grad, one dtype per stream), as StreamingTransform.push."""
-    if st._flushed:
-        raise RuntimeError("push() after flush(): call reset() to start new streams")
-    if not isinstance(chunk, torch.Tensor):
-        raise TypeError("chunk must be a torch.Tensor")
-    if chunk.requires_grad:
-        raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
-    if chunk.dim() != 2 or chunk.shape[0] != st.batch:
-        raise ValueError(f"chunk must be ({st.batch}, n), got {tuple(chunk.shape)}")
-    if chunk.dtype not in _C._WAVE_DTYPES:
-        raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
-    if st.dtype is not None and chunk.dtype != st.dtype:
-        raise ValueError(f"chunk dtype changed from {st.dtype} to {chunk.dtype} within a stream")
-
-
 class StreamingPyramid:
     """Stream ``batch`` signals chunk by chunk through the CQT pyramid of ``CQT2010v2``, ``VQT`` or ``CQT2010``.
 
@@ -421,9 +434,7 @@ class StreamingPyramid:
     def __init__(self, module, batch, **forward_kwargs):
         if not isinstance(module, _PYRAMIDS):
             raise TypeError(f"StreamingPyramid supports CQT2010v2, VQT and CQT2010, not {type(module).__name__}")
-        batch = int(batch)
-        if batch < 1 or batch > _C.MAX_BATCH:
-            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        batch = _streams(batch, "batch")
         fmt = forward_kwargs.get("output_format") or module.output_format
         norm = forward_kwargs.get("normalization_type", "librosa")
         _check_format_and_norm(fmt, norm)
@@ -498,9 +509,10 @@ class StreamingPyramid:
 
     def push(self, chunk: torch.Tensor) -> torch.Tensor:
         """Feed ``chunk`` (batch, n), any n >= 0; returns the frames final in every octave."""
-        _check_chunk(self, chunk)
-        if self.dtype is None:
-            self.dtype = chunk.dtype
+        if self._flushed:
+            raise RuntimeError("push() after flush(): call reset() to start new streams")
+        _check_chunk(chunk, self.batch, self.dtype)
+        self.dtype = chunk.dtype
         n = chunk.shape[1]
         T = self._ready(self.received + n) - self.frames
         return self._advance(chunk, n, False, T)
@@ -527,7 +539,7 @@ class StreamingPyramid:
         return out
 
 
-class PyramidPool:
+class PyramidPool(_ChunkPool):
     """Serve up to ``slots`` independent streams through the CQT pyramid of ``CQT2010v2``, ``VQT`` or ``CQT2010``,
     each advancing by its own amount.
 
@@ -547,22 +559,15 @@ class PyramidPool:
     """
 
     def __init__(self, module, slots, **forward_kwargs):
-        slots = int(slots)
-        if slots < 1 or slots > _C.MAX_BATCH:
-            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        slots = _streams(slots, "slots")
         # module checks, the pyramid arguments, the plan and one ring row per slot per signal: StreamingPyramid's
         self._sp = sp = StreamingPyramid(module, slots, **forward_kwargs)
-        self.module, self.slots = module, slots
+        self.module = module
         self.widths, self.hop, self.early, self.generation = sp.widths, sp.hop, sp.early, sp.generation
         self._reflect = sp._reflect
         self.ring = sp.ring
-        self.received = np.zeros(slots, np.int64)  # host counters of every slot's stream
-        self.frames = np.zeros(slots, np.int64)
-        self.ended = np.zeros(slots, bool)
+        self._init_slots(slots)
         self.dtype = None
-
-    reset = StreamPool.reset
-    _per_slot = StreamPool._per_slot
 
     # ---- StreamingPyramid's counters over arrays of lanes ------------------------------------------------- #
     def _counts(self, raw, end):
@@ -603,58 +608,23 @@ class PyramidPool:
         return raw - keep
 
     # ------------------------------------------------------------------------------------------------ #
-    def push(self, chunk: torch.Tensor, lengths, end=None) -> PoolOutput:
-        """Append ``chunk[s, :lengths[s]]`` to every slot s, end the slots flagged in ``end``; returns the new
-        frames of the slots that have some."""
-        if not isinstance(chunk, torch.Tensor):
-            raise TypeError("chunk must be a torch.Tensor")
-        if chunk.requires_grad:
-            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
-        if chunk.dim() != 2 or chunk.shape[0] != self.slots:
-            raise ValueError(f"chunk must be ({self.slots}, n), got {tuple(chunk.shape)}")
-        if chunk.dtype not in _C._WAVE_DTYPES:
-            raise ValueError(f"chunk must be float32, bfloat16 or float16, got {chunk.dtype}")
-        if self.dtype is not None and chunk.dtype != self.dtype:
-            raise ValueError(f"chunk dtype changed from {self.dtype} to {chunk.dtype} within the pool")
-        n = chunk.shape[1]
-        lengths = self._per_slot(lengths, "lengths", True)
-        end = np.zeros(self.slots, bool) if end is None else self._per_slot(end, "end", False)
-        bad = np.flatnonzero((lengths < 0) | (lengths > n))
-        if len(bad):
-            raise ValueError(f"lengths must be in [0, {n}] (the chunk width): slot {bad[0]} has {lengths[bad[0]]}")
-        bad = np.flatnonzero(self.ended & ((lengths > 0) | end))
-        if len(bad):
-            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
-        # every lane's counts, by the rules of StreamingPyramid (push / flush); per lane only the length plan of an end
-        active = np.flatnonzero((lengths > 0) | end)
-        R, F0, m, e = self.received[active], self.frames[active], lengths[active], end[active]
-        total = R + m
+    def _lane_counts(self, active, lengths, end):
+        """Every lane's frame count and carried raw samples, by the rules of StreamingPyramid (push / flush); per
+        lane only the length plan of an end."""
+        R, F0, e = self.received[active], self.frames[active], end[active]
+        total = R + lengths[active]
         count = self._ready(total) - F0
         for j in np.flatnonzero(e).tolist():
-            s = int(active[j])
-            try:
-                T_total, _ = _pyramid_length_plan(self.module, 1, int(total[j]))
-            except Exception as ex:
-                raise type(ex)(f"slot {s}: {ex}") from None
+            T_total, _ = _for_slot(int(active[j]), _pyramid_length_plan, self.module, 1, int(total[j]))
             count[j] = T_total - F0[j]
-        n_carry = self._n_carry(R, F0)
-        order = np.lexsort((active, count == 0))  # the lanes with frames first, slots ascending in each group
-        active, count = active[order], count[order]
-        A = int((count > 0).sum())
-        T_max = int(count.max()) if A else 0
-        lanes = np.stack([active, self.received[active], n_carry[order], self.frames[active], lengths[active],
-                          end[active].astype(np.int64)], 1).astype(np.int64)
-        dtype = self.dtype if self.dtype is not None else chunk.dtype
-        view = SimpleNamespace(ring=self.ring, slots=self.slots, dtype=dtype)  # the pool as the C call reads it
-        out = _C.cqt_pyramid_pool_forward(view, lanes, chunk, A, T_max, **self._sp._args())
+        return count, self._n_carry(R, F0)
+
+    def _advance(self, chunk, lanes, A, T_max, count):
+        out = _C.cqt_pyramid_pool_forward(self, lanes, chunk, A, T_max, **self._sp._args())
         if out is None:
             raise RuntimeError(f"{type(self.module).__name__}: no streamed tensor-core pyramid plan for this call "
                                "(NNAB_EUNSUPPORTED, e.g. NNAUDIO_B200_PATH=simt); the pool is unchanged")
-        self.dtype = dtype
-        self.received[active] += lengths[active]
-        self.frames[active] += count
-        self.ended[active] |= end[active]
-        return PoolOutput(out, torch.from_numpy(active[:A].copy()), torch.from_numpy(count[:A].copy()))
+        return out
 
 
 class StreamingInverse:
@@ -678,9 +648,7 @@ class StreamingInverse:
         else:
             raise TypeError(f"StreamingInverse takes an iSTFT or an STFT built with iSTFT=True, not "
                             f"{type(module).__name__}{'' if not isinstance(module, STFT) else ' without iSTFT=True'}")
-        batch = int(batch)
-        if batch < 1 or batch > _C.MAX_BATCH:
-            raise ValueError(f"batch must be in [1, {_C.MAX_BATCH}], got {batch}")
+        batch = _streams(batch, "batch")
         self.module, self.batch, self.onesided = module, batch, onesided
         self.n_fft, self.hop, self.center = module.n_fft, module.stride, bool(module.center)
         if self.hop > self.n_fft:
@@ -749,26 +717,7 @@ class InverseOutput(NamedTuple):
     counts: torch.Tensor
 
 
-def _cpu_ints(v, what, n=None, kind="integers"):
-    """A CPU array of ints (or bools, kind="bools") of shape (n,); device tensors are refused, since reading
-    them would synchronise."""
-    if isinstance(v, torch.Tensor):
-        if v.device.type != "cpu":
-            raise TypeError(f"{what} must be on the CPU: reading it from {v.device} would synchronise")
-        v = v.numpy()
-    a = np.asarray(v)
-    if n is not None and a.shape != (n,):
-        raise ValueError(f"{what} must hold {n} values, got shape {a.shape}")
-    if a.ndim != 1:
-        raise ValueError(f"{what} must be one-dimensional, got shape {a.shape}")
-    if kind == "integers" and a.dtype != bool and (np.issubdtype(a.dtype, np.integer) or a.size == 0):
-        return a.astype(np.int64)
-    if kind == "bools" and (a.dtype == bool or (np.issubdtype(a.dtype, np.integer) and np.isin(a, (0, 1)).all())):
-        return a.astype(bool)
-    raise TypeError(f"{what} must be {kind}, got {a.dtype}")
-
-
-class InversePool:
+class InversePool(_HostPool):
     """Serve up to ``slots`` independent streamed inverse STFTs, each advancing by its own frame count.
 
     ``module`` and ``onesided``: those of ``StreamingInverse``.  ``push(X, slots, counts, end=None,
@@ -787,28 +736,16 @@ class InversePool:
     pre-pass and FMT_OLA GEMM once over all lanes' frames, and one finalize launch; idle slots cost nothing.
     """
 
+    _COUNTERS = ("frames", "emitted")
+
     def __init__(self, module, slots, onesided=None):
-        slots = int(slots)
-        if slots < 1 or slots > _C.MAX_BATCH:
-            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        slots = _streams(slots, "slots")
         # module checks, the inverse arguments and the (slots, n_fft) fp32 state: StreamingInverse's
         self._si = si = StreamingInverse(module, slots, onesided=onesided)
-        self.module, self.slots, self.onesided = module, slots, si.onesided
+        self.module, self.onesided = module, si.onesided
         self.n_fft, self.hop, self.center, self.f_in, self.offset = si.n_fft, si.hop, si.center, si.f_in, si.offset
         self.state = si.state  # row s: slot s's open overlap-add sums
-        self.frames = np.zeros(slots, np.int64)  # host counters of every slot's stream
-        self.emitted = np.zeros(slots, np.int64)
-        self.ended = np.zeros(slots, bool)
-
-    def reset(self, slots=None):
-        """Start new streams in ``slots`` (all slots by default)."""
-        idx = np.arange(self.slots) if slots is None else _cpu_ints(
-            np.reshape(slots.cpu() if isinstance(slots, torch.Tensor) else slots, -1), "slots")
-        if ((idx < 0) | (idx >= self.slots)).any():
-            raise ValueError(f"slots must be in [0, {self.slots}), got {idx.tolist()}")
-        self.frames[idx] = 0
-        self.emitted[idx] = 0
-        self.ended[idx] = False
+        self._init_slots(slots)
 
     def _emit_end(self, n):
         """``StreamingInverse._emit_end`` over an array of frame counts."""
@@ -854,9 +791,7 @@ class InversePool:
         T[rows_slot] = rows_count
         row[rows_slot] = np.arange(R)
         row[T == 0] = -1
-        bad = np.flatnonzero(self.ended & ((T > 0) | end))
-        if len(bad):
-            raise RuntimeError(f"slot {bad[0]}: its stream has ended; call reset([{bad[0]}]) to start a new one")
+        self._refuse_ended(T > 0, end)
         n = self.frames + T
         bad = np.flatnonzero(end & (n == 0))
         if len(bad):
@@ -901,22 +836,37 @@ def _device_vector(v, what, slots, dtype, device):
     return v
 
 
-def _first_error(pool):
-    """(slot, code, info a, info b) of the lowest slot with an error code, or None; synchronises."""
-    errors = pool.errors.cpu()
-    bad = torch.nonzero(errors).flatten()
-    if len(bad) == 0:
-        return None
-    s = int(bad[0])
-    a, b = pool.error_info[s].tolist()
-    return s, int(errors[s]), a, b
+class _DevicePool:
+    """What the device pools share: the per-slot counters, error codes and values, counts and lane table on the
+    device, the reset and the lookup of the first error."""
+
+    def _init_device(self, slots, lane_fields, dev):
+        self.slots = slots
+        self.counters = torch.zeros((3, slots), dtype=torch.int64, device=dev)
+        self.errors = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self.error_info = torch.zeros((slots, 2), dtype=torch.int64, device=dev)
+        self.counts = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self._lanes = torch.zeros((slots, len(lane_fields)), dtype=torch.int64, device=dev)
+        self._no_end = torch.zeros(slots, dtype=torch.bool, device=dev)
+
+    def reset(self, restart=None):
+        """Start new streams where the bool device mask ``restart`` is set (None: every slot)."""
+        mask = None if restart is None else _device_vector(restart, "restart", self.slots, torch.bool,
+                                                           self.counters.device)
+        _C.pool_device_reset(self, mask)
+
+    def _first_error(self):
+        """(slot, code, info a, info b) of the lowest slot with an error code, or None; synchronises."""
+        errors = self.errors.cpu()
+        bad = torch.nonzero(errors).flatten()
+        if len(bad) == 0:
+            return None
+        s = int(bad[0])
+        a, b = self.error_info[s].tolist()
+        return s, int(errors[s]), a, b
 
 
-def _ended_error(s):
-    return RuntimeError(f"slot {s}: its stream has ended; call reset([{s}]) to start a new one")
-
-
-class DeviceStreamPool:
+class DeviceStreamPool(_DevicePool):
     """``StreamPool`` with every per-push number on the GPU: a push reads nothing on the host and has one fixed
     geometry, so it can be captured in a CUDA graph (``torch.cuda.graph``) and replayed.
 
@@ -944,51 +894,31 @@ class DeviceStreamPool:
     """
 
     def __init__(self, module, slots, chunk, dtype=torch.float32, **forward_kwargs):
-        slots, chunk = int(slots), int(chunk)
-        if slots < 1 or slots > _C.MAX_BATCH:
-            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        slots, chunk = _streams(slots, "slots"), int(chunk)
         if chunk < 1:
             raise ValueError(f"chunk must be at least 1 sample, got {chunk}")
         if dtype not in _C._WAVE_DTYPES:
             raise ValueError(f"dtype must be float32, bfloat16 or float16, got {dtype}")
         # module checks, the offline call's arguments and the (slots, K) fp32 carry ring: StreamingTransform's
         self._st = st = StreamingTransform(module, slots, _strict=True, **forward_kwargs)
-        self.module, self.slots, self.chunk, self.dtype = module, slots, chunk, dtype
+        self.module, self.chunk, self.dtype = module, chunk, dtype
         self.K, self.hop, self.pad = st.K, st.hop, st.pad
         self.ring = st.ring
         dev = self.ring.device
         name, self._kw = st._args()  # packed basis, filterbank table (synchronises once), scales: built here
         self.T_cap = _C.pool_frame_cap(chunk, self.K, self.hop, self.pad, self._kw["pad_mode"])
-        self.counters = torch.zeros((3, slots), dtype=torch.int64, device=dev)
-        self.errors = torch.zeros(slots, dtype=torch.int32, device=dev)
-        self.error_info = torch.zeros((slots, 2), dtype=torch.int64, device=dev)
-        self.counts = torch.zeros(slots, dtype=torch.int32, device=dev)
-        self._lanes = torch.zeros((slots, len(_C.LANE_FIELDS)), dtype=torch.int64, device=dev)
+        self._init_device(slots, _C.LANE_FIELDS, dev)
         self._fn, self.frames, self._ws, self._tail = _C.pool_device_bind(name, self._kw, slots, self.T_cap, dev)
-        self._no_end = torch.zeros(slots, dtype=torch.bool, device=dev)
         # an idle push changes nothing; it runs the route once and finds a plan that cannot read the chunk
         idle = torch.zeros(slots, dtype=torch.int32, device=dev)
         if not _C.pool_device_forward(self, torch.zeros((slots, chunk), dtype=dtype, device=dev), idle, self._no_end):
             raise RuntimeError(f"{name}: no fused pool route for this configuration (NNAB_EUNSUPPORTED, e.g. "
                                "NNAUDIO_B200_PATH=simt); DeviceStreamPool has no concat route")
 
-    def reset(self, restart=None):
-        """Start new streams where the bool device mask ``restart`` is set (None: every slot)."""
-        mask = None if restart is None else _device_vector(restart, "restart", self.slots, torch.bool,
-                                                           self.counters.device)
-        _C.pool_device_reset(self, mask)
-
     def push(self, x: torch.Tensor, lengths: torch.Tensor, end: torch.Tensor = None):
         """Append ``x[s, :lengths[s]]`` to every slot s and end the slots flagged in ``end``; the new frames go
         to ``frames`` / ``counts``."""
-        if not isinstance(x, torch.Tensor):
-            raise TypeError("chunk must be a torch.Tensor")
-        if x.requires_grad:
-            raise NotImplementedError("the streaming API is forward-only: the chunk requires grad")
-        if x.dim() != 2 or tuple(x.shape) != (self.slots, self.chunk):
-            raise ValueError(f"chunk must be ({self.slots}, {self.chunk}), got {tuple(x.shape)}")
-        if x.dtype != self.dtype:
-            raise ValueError(f"chunk must be {self.dtype} (the pool's sample type), got {x.dtype}")
+        _check_chunk(x, self.slots, self.dtype, width=self.chunk)
         if x.device != self.ring.device:
             raise RuntimeError(f"chunk is on {x.device}: the pool runs on {self.ring.device}")
         if x.stride(-1) != 1 or (self.slots > 1 and x.stride(0) < self.chunk):
@@ -1001,7 +931,7 @@ class DeviceStreamPool:
 
     def check(self):
         """Synchronise and raise what ``StreamPool`` would have raised for the lowest slot with an error code."""
-        err = _first_error(self)
+        err = self._first_error()
         if err is None:
             return
         s, code, a, _ = err
@@ -1010,14 +940,11 @@ class DeviceStreamPool:
         if code == _C.LANE_EENDED:
             raise _ended_error(s)
         if code == _C.LANE_ESHORT:
-            try:
-                self._st._check_length(a)  # the exception module(x) raises for a stream this short
-            except Exception as e:
-                raise type(e)(f"slot {s}: {e}") from None
+            _for_slot(s, self._st._check_length, a)  # the exception module(x) raises for a stream this short
         raise RuntimeError(f"slot {s}: push dropped with error code {code}")
 
 
-class DeviceInversePool:
+class DeviceInversePool(_DevicePool):
     """``InversePool`` with every per-push number on the GPU, capturable in a CUDA graph like ``DeviceStreamPool``.
 
     ``DeviceInversePool(module, slots, frames, onesided=None)``: ``module`` and ``onesided`` are ``InversePool``'s,
@@ -1035,34 +962,25 @@ class DeviceInversePool:
     """
 
     def __init__(self, module, slots, frames, onesided=None):
-        slots, frames = int(slots), int(frames)
-        if slots < 1 or slots > _C.MAX_BATCH:
-            raise ValueError(f"slots must be in [1, {_C.MAX_BATCH}], got {slots}")
+        slots, frames = _streams(slots, "slots"), int(frames)
         if frames < 1:
             raise ValueError(f"frames must be at least 1, got {frames}")
         # module checks, the inverse arguments and the (slots, n_fft) fp32 state: StreamingInverse's
         self._si = si = StreamingInverse(module, slots, onesided=onesided)
-        self.module, self.slots, self.onesided, self.frames_cap = module, slots, si.onesided, frames
+        self.module, self.onesided, self.frames_cap = module, si.onesided, frames
         self.n_fft, self.hop, self.center, self.f_in = si.n_fft, si.hop, si.center, si.f_in
         self.state = si.state
         dev = self.state.device
         _, _, self._packed, self._window = si._args()
         self.n_cap = _C.istft_pool_sample_cap(frames, self.n_fft, self.hop, self.center)
-        self.counters = torch.zeros((3, slots), dtype=torch.int64, device=dev)  # frames, emitted, ended
-        self.errors = torch.zeros(slots, dtype=torch.int32, device=dev)
-        self.error_info = torch.zeros((slots, 2), dtype=torch.int64, device=dev)
-        self.counts = torch.zeros(slots, dtype=torch.int32, device=dev)
+        self._init_device(slots, _C.ISTFT_LANE_FIELDS, dev)  # counters: frames, emitted, ended
         self.samples = torch.zeros((slots, self.n_cap), dtype=torch.float32, device=dev)
-        self._lanes = torch.zeros((slots, len(_C.ISTFT_LANE_FIELDS)), dtype=torch.int64, device=dev)
         self._ws = torch.empty(_C.lib().nnab_istft_pool_workspace_bytes(slots, self.f_in, frames, self.n_fft,
                                                                          self.hop), dtype=torch.uint8, device=dev)
-        self._no_end = torch.zeros(slots, dtype=torch.bool, device=dev)
         self._no_length = torch.full((slots,), -1, dtype=torch.int64, device=dev)
         idle = torch.zeros(slots, dtype=torch.int32, device=dev)  # an idle push changes nothing
         _C.istft_pool_device_forward(self, torch.zeros((slots, self.f_in, frames, 2), device=dev), idle,
                                      self._no_end, self._no_length)
-
-    reset = DeviceStreamPool.reset
 
     def push(self, X: torch.Tensor, counts: torch.Tensor, end: torch.Tensor = None, length: torch.Tensor = None):
         """Append ``X[s, :, :counts[s]]`` to every slot s and end the slots flagged in ``end``; the new samples go
@@ -1087,7 +1005,7 @@ class DeviceInversePool:
 
     def check(self):
         """Synchronise and raise what ``InversePool`` would have raised for the lowest slot with an error code."""
-        err = _first_error(self)
+        err = self._first_error()
         if err is None:
             return
         s, code, a, b = err

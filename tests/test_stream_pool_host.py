@@ -219,6 +219,9 @@ def test_rules_and_errors_change_nothing(monkeypatch):
         pool.push(torch.randn(4, 0), [0, 0, 0, 0], [True, False, False, False])  # ... and no second end
     out = pool.push(torch.randn(4, 0), [0, 0, 0, 0])  # an empty push
     assert out.frames.shape[0] == 0 and out.slots.numel() == 0
+    with pytest.raises(TypeError):
+        pool.reset(np.array([0.0]))  # slots are integers, as in InversePool.reset
+    assert pool.ended[0]
     pool.reset([0])
     assert pool.received[0] == 0 and not pool.ended[0] and pool.received[1] == 10
     assert pool.push(torch.randn(4, 100), [100, 0, 0, 0]).counts.tolist() == [_ready_frames(100, 64, 16, 32, True)]
@@ -232,6 +235,10 @@ def test_strict_pool_refuses_the_concat_route(monkeypatch):
     pool = StreamPool(make(), 2, _strict=True)
     with pytest.raises(RuntimeError, match="no fused pool route"):
         pool.push(torch.randn(2, 200), [200, 100])
+    # nothing ran, so nothing is committed: not the counters, not the sample type
+    assert pool.dtype is None and not pool.received.any() and not pool.frames.any()
+    with pytest.raises(RuntimeError, match="no fused pool route"):
+        pool.push(torch.randn(2, 200, dtype=torch.bfloat16), [200, 100])
 
 
 # ------------------------------------------------------------------------------------------- C host checks
