@@ -61,6 +61,11 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   `PyramidPool(module, slots)` serves independent pyramid streams with `StreamPool`'s `push(chunk, lengths, end)` /
   `reset(slots)` surface: each slot's rows equal `module(x)` on its own stream bit for bit, and a one-stream
   `StreamingPyramid` fed the same packets.
+  `DevicePyramidPool(module, slots, chunk, dtype=torch.float32)` is `PyramidPool` with `DeviceStreamPool`'s surface:
+  device `lengths` / `end`, the pool-owned `frames` (slots, n_bins, `T_cap`[, 2]) and `counts`, `reset(restart=None)`
+  and `check()`, so a pyramid tick can be captured in a CUDA graph.  A push never sees the lengths on the host, so it
+  cannot issue `module(x)`'s reflect-fallback `UserWarning` for a short stream (DESIGN.md §3.10 "Device pyramid
+  pools").
 
 Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
 schedule of the CQT1992v2 kernel).

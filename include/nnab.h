@@ -667,6 +667,41 @@ int nnab_debug_device_istft_plan(int64_t* counters, const int32_t* frame_counts,
                                  const int64_t* length, int32_t* errors, int64_t* error_info, int32_t* counts,
                                  nnab_istft_lane* lanes, int64_t slots, int64_t t, int n_fft, int hop, int center);
 
+/* Device-planned pool of streamed CQT pyramids (DESIGN.md §3.10 "Device pyramid pools"): nnab_cqt_pyramid_pool_forward
+ * with (lanes, d_lanes, n_lanes, A) replaced by the device pools' (counters, lengths, end, errors, error_info, counts,
+ * d_lanes); counters are received, frames, ended per slot, a lane's n_carry is derived from them.  n is the fixed
+ * chunk width; T_max must be caps[0] of nnab_cqt_pyramid_pool_device_caps(n, ...) and out is (slots, n_bins,
+ * T_max[, 2]).  A slot whose push PyramidPool would refuse is dropped (NNAB_LANE_ELENGTH, NNAB_LANE_EENDED, or
+ * NNAB_LANE_ESHORT for an end the stream is too short for; info: its length).  Every stage and octave launches on
+ * every push over all slots at the caps, so the launch list does not depend on the traffic.  Only host-side
+ * arguments are checked; the SIMT path, a missing packed operand or a launch outside the kernels' limits returns
+ * NNAB_EUNSUPPORTED before anything is enqueued.
+ * The caps query (host only) fills caps[0] = T_cap, the most frames one push of at most `chunk` samples returns
+ * (an end included), caps[1 + s] = the most FIR outputs stage s -> s + 1 computes for one lane from its first
+ * 128-output row (0 for the last signal), caps[1 + n_signals + s] = the most samples one push stores into signal
+ * s's ring; n_signals = n_octaves (+ 1 with early_factor > 1).  It is NNAB_EINVAL if a push without an end could be
+ * refused, which the ring bounds exclude.  The workspace query is host-only (0 for arguments no pool takes). */
+int nnab_cqt_pyramid_pool_device_caps(int64_t chunk, int n_octaves, const int32_t* widths, int hop,
+                                      int early_factor, int pad_mode, int64_t* caps);
+size_t nnab_cqt_pyramid_pool_device_workspace_bytes(int64_t slots, int64_t chunk, int n_octaves,
+                                                    const int32_t* widths, int hop, int early_factor, int pad_mode);
+int nnab_cqt_pyramid_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                         int32_t* errors, int64_t* error_info, int32_t* counts,
+                                         nnab_stream_lane* d_lanes, const void* chunk, int chunk_dtype, int64_t slots,
+                                         int64_t n, int64_t chunk_pitch, int n_octaves, const float* const* h_k_real,
+                                         const float* const* h_k_imag, const void* const* h_packed,
+                                         const int32_t* h_widths, int n_filters, const float* lowpass,
+                                         const void* lowpass_packed, const float* early_filter,
+                                         const void* early_packed, int early_factor, int hop, int pad_mode,
+                                         int n_bins, const float* scale, float scale_all, int out_format,
+                                         float sqrt_eps, float* out, int64_t T_max, void* workspace, size_t ws_bytes,
+                                         int path, void* stream);
+/* Host-only run of its plan launch for tests (nnab_debug_device_pool_plan's layout). */
+int nnab_debug_device_pyramid_plan(int64_t* counters, const int32_t* lengths, const uint8_t* end, int32_t* errors,
+                                   int64_t* error_info, int32_t* counts, nnab_stream_lane* lanes, int64_t slots,
+                                   int64_t n, int n_octaves, const int32_t* widths, int hop, int early_factor,
+                                   int pad_mode);
+
 /* Kernel launches issued by this library since load (process wide; used by
  * bench.py for its `gpu_launches` claim). */
 uint64_t nnab_launch_count(void);

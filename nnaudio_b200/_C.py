@@ -164,6 +164,14 @@ SIGNATURES["nnab_cqt_pyramid_pool_forward"] = (c_int, _POOL_HEAD + SIGNATURES["n
 SIGNATURES["nnab_cqt_pyramid_pool_workspace_bytes"] = (
     c_size_t, [_P, c_int64, c_int64, c_int64, c_int, _P, c_int, c_int, c_int])
 SIGNATURES["nnab_debug_pyramid_pool_plan"] = (c_int, [_P, c_int64, c_int64, c_int, _P, c_int, c_int, c_int, _P])
+# device pyramid pools: the device head in front of the pyramid arguments; the caps, workspace and debug plan queries
+# take the geometry (chunk, n_octaves, widths, hop, early_factor, pad_mode)
+_PYR_GEOMETRY = [c_int, _P, c_int, c_int, c_int]
+SIGNATURES["nnab_cqt_pyramid_pool_device_forward"] = (
+    c_int, _DEVICE_HEAD + SIGNATURES["nnab_cqt_pyramid_forward"][1][4:])
+SIGNATURES["nnab_cqt_pyramid_pool_device_caps"] = (c_int, [c_int64] + _PYR_GEOMETRY + [_P])
+SIGNATURES["nnab_cqt_pyramid_pool_device_workspace_bytes"] = (c_size_t, [c_int64, c_int64] + _PYR_GEOMETRY)
+SIGNATURES["nnab_debug_device_pyramid_plan"] = (c_int, [_P] * 7 + [c_int64, c_int64] + _PYR_GEOMETRY)
 SIGNATURES["nnab_istft_chunk_workspace_bytes"] = SIGNATURES["nnab_istft_workspace_bytes"]
 SIGNATURES["nnab_istft_chunk_forward"] = (
     c_int, [_P, c_int64, c_int64, _P, c_int64, c_int, c_int64, _P, _P, c_int, c_int, c_int, c_int, c_int64, _P,
@@ -970,6 +978,56 @@ def debug_device_istft_plan(counters, frame_counts, end, length, errors, error_i
     _check(lib().nnab_debug_device_istft_plan(p(counters), p(frame_counts), p(end), p(length), p(errors),
                                               p(error_info), p(counts), p(lanes), slots, int(t), int(n_fft), int(hop),
                                               int(center)), "nnab_debug_device_istft_plan")
+    return lanes, counts
+
+
+def _widths(widths):
+    return (c_int32 * len(widths))(*[int(v) for v in widths])
+
+
+def cqt_pyramid_pool_device_caps(chunk, widths, hop, early_factor, pad_mode):
+    """The fixed geometry of a device pyramid pool (``nnab_cqt_pyramid_pool_device_caps``, host only): (T_cap, the
+    most FIR outputs per lane of each stage (0 for the last signal), the most samples one push stores into each
+    signal's ring).  Raises if a push without an end could be refused."""
+    n_sig = len(widths) + (1 if early_factor > 1 else 0)
+    buf = (c_int64 * (1 + 2 * n_sig))()
+    _check(lib().nnab_cqt_pyramid_pool_device_caps(int(chunk), len(widths), _widths(widths), int(hop),
+                                                   int(early_factor), int(pad_mode), buf),
+           "nnab_cqt_pyramid_pool_device_caps")
+    return int(buf[0]), list(buf[1:1 + n_sig]), list(buf[1 + n_sig:1 + 2 * n_sig])
+
+
+def pyramid_pool_device_bind(kw, slots, chunk, T_cap, device, path=None):
+    """``pool_device_bind`` for a device pyramid pool on the pyramid arguments ``kw`` (``cqt_pyramid_forward``'s):
+    (C function, output (slots, n_bins, T_cap[, 2]), workspace, argument tail after the chunk pitch).  The tail holds
+    the ctypes bank arrays; the caller keeps the tensors of ``kw`` alive."""
+    L = lib()
+    path = resolve_path(path)
+    re_arr, im_arr, pk_arr, widths = _bank_arrays(kw["banks_real"], kw["banks_imag"], kw["packed"])
+    n_oct = len(kw["banks_real"])
+    out = torch.zeros(_complex_shape(slots, kw["n_bins"], T_cap, kw["out_format"] != FMT_MAGNITUDE),
+                      dtype=torch.float32, device=device)
+    ws, wsb = _workspace(L.nnab_cqt_pyramid_pool_device_workspace_bytes(
+        slots, chunk, n_oct, widths, kw["hop"], kw["early_factor"], kw["pad_mode"]), device)
+    tail = (n_oct, re_arr, im_arr, pk_arr, widths, kw["banks_real"][0].shape[0], _ptr(kw["lowpass"]),
+            _ptr(kw["lowpass_packed"]), _ptr(kw["early_filter"]), _ptr(kw["early_packed"]), kw["early_factor"],
+            kw["hop"], kw["pad_mode"], kw["n_bins"], _ptr(kw["scale"]), kw["scale_all"], kw["out_format"],
+            kw["sqrt_eps"], _ptr(out), T_cap, _ptr(ws), wsb, path)
+    return L.nnab_cqt_pyramid_pool_device_forward, out, ws, tail
+
+
+def debug_device_pyramid_plan(counters, lengths, end, errors, error_info, n, widths, hop, early_factor, pad_mode):
+    """``debug_device_pool_plan`` for a device pyramid pool (``nnab_debug_device_pyramid_plan``): returns (lanes
+    (slots, 6) int64, counts (slots,) int32)."""
+    slots = len(lengths)
+    lengths = np.ascontiguousarray(lengths, np.int32)
+    end = np.ascontiguousarray(end, np.uint8)
+    lanes = np.zeros((slots, 6), np.int64)
+    counts = np.zeros(slots, np.int32)
+    p = lambda a: a.ctypes.data_as(c_void_p)
+    _check(lib().nnab_debug_device_pyramid_plan(p(counters), p(lengths), p(end), p(errors), p(error_info), p(counts),
+                                                p(lanes), slots, int(n), len(widths), _widths(widths), int(hop),
+                                                int(early_factor), int(pad_mode)), "nnab_debug_device_pyramid_plan")
     return lanes, counts
 
 

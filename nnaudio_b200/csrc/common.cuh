@@ -277,6 +277,48 @@ __host__ __device__ inline int64_t pyr_keep(const PyrStream& p, int s, const int
   return k;
 }
 
+// The per-stream rules of one push (n new samples, the last push iff `end`): the counts before (R0) and after (R1)
+// it, the frame bound after it and each octave's padding (reflect falls back to constant on a level the end leaves
+// no longer than its pad).  NNAB_EINVAL for counters no stream can have (they must be those of a stream that
+// returned every ready frame and carries what pyr_keep keeps), for an end the stream is too short for (a level
+// left empty, an octave without frames, octave frame counts that differ, fewer frames than already returned) and
+// for a push that would overrun a ring.  The one-stream push, every lane of a pool and every slot of a device
+// pool's plan launch are checked here.
+struct PyrStep {
+  int64_t R0[33], R1[33];
+  int64_t t_end;
+  int mode[32];
+};
+
+__host__ __device__ inline int pyr_step(const PyrStream& p, int64_t received, int64_t n_carry, int64_t frames,
+                                        int64_t n, int end, int pad_mode, PyrStep* o) {
+  if (received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
+  pyr_counts(p, received, 0, o->R0);
+  if (frames != pyr_ready_frames(p, o->R0, pad_mode) || n_carry != received - pyr_keep(p, 0, o->R0, frames))
+    return NNAB_EINVAL;
+  pyr_counts(p, received + n, end, o->R1);
+  for (int i = 0; i < p.n_oct; ++i) {
+    const int64_t len = o->R1[i + p.e];
+    o->mode[i] = (end && pad_mode == NNAB_PAD_REFLECT && p.pad[i] >= len) ? NNAB_PAD_CONSTANT : pad_mode;
+  }
+  if (end) {
+    o->t_end = -1;
+    for (int i = 0; i < p.n_oct; ++i) {
+      const int64_t len = o->R1[i + p.e];
+      if (len <= 0) return NNAB_EINVAL;
+      const int64_t f = chunk_end_frames(len, p.width[i], p.hop[i], p.pad[i]);
+      if (f <= 0 || (o->t_end >= 0 && f != o->t_end)) return NNAB_EINVAL;
+      o->t_end = f;
+    }
+    if (o->t_end < frames) return NNAB_EINVAL;
+  } else {
+    o->t_end = pyr_ready_frames(p, o->R1, pad_mode);
+    for (int s = 0; s < p.n_sig; ++s)
+      if (o->R1[s] - pyr_keep(p, s, o->R1, o->t_end) > p.ring_len[s]) return NNAB_EINVAL;
+  }
+  return NNAB_OK;
+}
+
 // One pool lane's plan for signal s of a push: what the one-stream push (nnab_cqt_pyramid_chunk_forward) of the
 // lane's counters does with that signal.  The plan kernel writes it per (signal, lane) into the workspace and
 // every lane-aware kernel reads it; the host checks the lanes with the same functions first.
@@ -441,6 +483,45 @@ __host__ __device__ inline void device_pool_slot(int64_t s, int64_t slots, int64
   counts[s] = (int32_t)T;
 }
 
+// device_pool_slot for a pool of pyramid streams: the counters' n_carry is the raw ring's (pyr_keep of signal 0),
+// the rules pyr_step's.  The counters are the plan's own, so only an end can be refused (NNAB_LANE_ESHORT, info:
+// the stream's length): pyr_stream_init's ring bounds hold every push that does not end.
+__host__ __device__ inline void device_pyramid_slot(int64_t s, int64_t slots, int64_t* counters,
+                                                    const int32_t* lengths, const uint8_t* end_in, int32_t* errors,
+                                                    int64_t* info, int32_t* counts, nnab_stream_lane* lanes,
+                                                    int64_t chunk, const PyrStream& p, int pad_mode) {
+  const int64_t received = counters[s], frames = counters[slots + s];
+  const bool ended = counters[2 * slots + s] != 0;
+  const int64_t n = lengths[s];
+  const int end = end_in[s] != 0;
+  nnab_stream_lane ln{};
+  ln.slot = s;
+  int64_t T = 0;
+  int code = NNAB_LANE_OK;
+  if (n < 0 || n > chunk) {
+    code = NNAB_LANE_ELENGTH;
+  } else if (ended && (n > 0 || end)) {
+    code = NNAB_LANE_EENDED;
+  } else if (n > 0 || end) {
+    PyrStep st;
+    pyr_counts(p, received, 0, st.R0);
+    const int64_t n_carry = received - pyr_keep(p, 0, st.R0, frames);
+    if (pyr_step(p, received, n_carry, frames, n, end, pad_mode, &st) != NNAB_OK) {
+      code = NNAB_LANE_ESHORT;
+    } else {
+      ln.received = received; ln.n_carry = n_carry; ln.frames = frames; ln.n = n; ln.end = end;
+      T = st.t_end - frames;
+      counters[s] = received + n;
+      counters[slots + s] = st.t_end;
+      counters[2 * slots + s] = ended || end;
+    }
+  }
+  if (code != NNAB_LANE_OK)
+    device_lane_error(s, code, code == NNAB_LANE_ESHORT ? received + n : n, 0, errors, info);
+  lanes[s] = ln;
+  counts[s] = (int32_t)T;
+}
+
 __host__ __device__ inline void device_istft_slot(int64_t s, int64_t slots, int64_t* counters,
                                                   const int32_t* frame_counts, const uint8_t* end_in,
                                                   const int64_t* length_in, int32_t* errors, int64_t* info,
@@ -571,6 +652,10 @@ int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int6
 // the zeroing of frames t >= rows[i].count of row i of out (A, n_rows, T, cols)
 int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int pad_mode,
                      PyrLaneSig* table, cudaStream_t stream);
+// device pyramid pools: the plan launch (device_pyramid_slot per slot)
+int tc_device_pyramid_plan(const PyrStream& p, int64_t slots, int64_t* counters, const int32_t* lengths,
+                           const uint8_t* end, int32_t* errors, int64_t* info, int32_t* counts,
+                           nnab_stream_lane* lanes, int64_t chunk, int pad_mode, cudaStream_t stream);
 int tc_rows_carry(const ChunkSource& cs, int x_dtype, int64_t n_rows, int64_t longest, cudaStream_t stream);
 int tc_rows_mask(const PyrLaneSig* rows, int64_t A, float* out, int64_t n_rows, int64_t T, int cols,
                  cudaStream_t stream);

@@ -1469,11 +1469,9 @@ static bool pyr_stream_init(int n_octaves, const int32_t* widths, int hop, int e
   return true;
 }
 
-// One push: the counts before (R0) and after (R1) it, the frames it returns and the workspace layout.
-struct PyrPush {
-  int64_t R0[33], R1[33];
-  int64_t t_end;
-  int mode[32];               // each octave's padding (reflect falls back to constant on short levels at flush)
+// One push: the stream's step (PyrStep: the counts before and after it, the frames it returns, each octave's
+// padding) and the workspace layout.
+struct PyrPush : PyrStep {
   int64_t np[33];             // new-sample buffer pitch of signal s >= 1 (floats)
   size_t nbuf[33], scratch, scratch_bytes, total;
 };
@@ -1491,32 +1489,10 @@ static void pyr_oct_geom(const PyrStream& p, int l, int64_t B, int64_t len, int6
 
 static int pyr_push_plan(const PyrStream& p, int64_t B, int64_t received, int64_t n_carry, int64_t frames,
                          int64_t n, int flush, int pad_mode, PyrPush* o) {
-  if (B < 0 || B > 65535 || received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
+  if (B < 0 || B > 65535) return NNAB_EINVAL;
   if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
-  pyr_counts(p, received, 0, o->R0);
-  if (frames != pyr_ready_frames(p, o->R0, pad_mode) || n_carry != received - pyr_keep(p, 0, o->R0, frames))
-    return NNAB_EINVAL;
-  const int64_t total = received + n;
-  pyr_counts(p, total, flush, o->R1);
-  for (int i = 0; i < p.n_oct; ++i) {
-    const int64_t len = o->R1[i + p.e];
-    o->mode[i] = (flush && pad_mode == NNAB_PAD_REFLECT && p.pad[i] >= len) ? NNAB_PAD_CONSTANT : pad_mode;
-  }
-  if (flush) {
-    o->t_end = -1;
-    for (int i = 0; i < p.n_oct; ++i) {
-      const int64_t len = o->R1[i + p.e];
-      if (len <= 0) return NNAB_EINVAL;
-      const int64_t f = frames_of(len, p.width[i], p.hop[i], p.pad[i]);
-      if (f <= 0 || (o->t_end >= 0 && f != o->t_end)) return NNAB_EINVAL;
-      o->t_end = f;
-    }
-    if (o->t_end < frames) return NNAB_EINVAL;
-  } else {
-    o->t_end = pyr_ready_frames(p, o->R1, pad_mode);
-    for (int s = 0; s < p.n_sig; ++s)
-      if (o->R1[s] - pyr_keep(p, s, o->R1, o->t_end) > p.ring_len[s]) return NNAB_EINVAL;
-  }
+  const int rc = pyr_step(p, received, n_carry, frames, n, flush, pad_mode, o);
+  if (rc) return rc;
   // workspace: the new samples of every computed signal, then one scratch reused by the launches in order
   size_t off = 0;
   for (int s = 1; s < p.n_sig; ++s) {
@@ -1751,7 +1727,8 @@ int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t fra
 
 // ------------------------------------------------------------ pyramid pools ----
 // One push of a pool of pyramid streams (DESIGN §3.10 "Pyramid pools"): every lane checked by the one-stream rules
-// (pyr_push_plan), the table as a whole, and the batch-wide geometry of each launch.
+// (pyr_step), the table as a whole, and the batch-wide geometry of each launch.  A device pool's plan has the same
+// form with its fixed geometry (pyr_device_plan).
 struct PyrPoolPlan {
   int64_t T_max;
   int64_t len_out[33];  // stage s: the most outputs one lane's FIR rows hold from their first row (0: no lane advances)
@@ -1760,34 +1737,10 @@ struct PyrPoolPlan {
   size_t table, nbuf[33], scratch, scratch_bytes, total;
 };
 
-static int pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
-                         int64_t slots, int64_t n, int pad_mode, PyrPoolPlan* o) {
-  if (n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes || (n_lanes > 0 && lanes == nullptr)) return NNAB_EINVAL;
-  std::vector<uint8_t> seen((size_t)slots, 0);
-  o->T_max = 0;
-  for (int s = 0; s < p.n_sig; ++s) o->len_out[s] = o->longest[s] = 0;
-  for (int64_t i = 0; i < n_lanes; ++i) {
-    const nnab_stream_lane& ln = lanes[i];
-    if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
-    if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
-    seen[(size_t)ln.slot] = 1;
-    if (ln.n > n || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
-    PyrPush pp;
-    const int rc = pyr_push_plan(p, 1, ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, pad_mode, &pp);
-    if (rc) return rc;
-    const int64_t T = pp.t_end - ln.frames;
-    if ((i < A) != (T > 0)) return NNAB_EINVAL;               // the A lanes with frames come first
-    if (T == 0 && ln.n == 0 && !ln.end) return NNAB_EINVAL;   // a lane with nothing to do
-    if (T > o->T_max) o->T_max = T;
-    for (int s = 0; s < p.n_sig; ++s) {
-      const PyrLaneSig d = pyr_lane_signal(p, ln, i, s, pad_mode);
-      if (d.R0 != pp.R0[s] || d.R1 != pp.R1[s] || d.count != T) return NNAB_EINVAL;  // one set of rules
-      if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
-      if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
-    }
-  }
-  // workspace: the descriptor table, the new samples of every computed signal (row i: lane i's stage outputs from
-  // its first row), then one scratch reused by the launches in order
+// The workspace of a push of n_lanes lanes, the A first of which return frames, from the plan's T_max, len_out:
+// the descriptor table, the new samples of every computed signal (row i: lane i's stage outputs from its first
+// row), then one scratch reused by the launches in order.
+static void pyr_pool_layout(const PyrStream& p, int64_t n_lanes, int64_t A, PyrPoolPlan* o) {
   size_t off = 0;
   o->table = off;
   off += align_up((size_t)(n_lanes > 0 ? n_lanes : 1) * p.n_sig * sizeof(PyrLaneSig), 256);
@@ -1821,6 +1774,35 @@ static int pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int6
   o->scratch = off;
   o->scratch_bytes = sc;
   o->total = off + sc + 512;
+}
+
+static int pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
+                         int64_t slots, int64_t n, int pad_mode, PyrPoolPlan* o) {
+  if (n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes || (n_lanes > 0 && lanes == nullptr)) return NNAB_EINVAL;
+  std::vector<uint8_t> seen((size_t)slots, 0);
+  o->T_max = 0;
+  for (int s = 0; s < p.n_sig; ++s) o->len_out[s] = o->longest[s] = 0;
+  for (int64_t i = 0; i < n_lanes; ++i) {
+    const nnab_stream_lane& ln = lanes[i];
+    if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
+    if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
+    seen[(size_t)ln.slot] = 1;
+    if (ln.n > n || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
+    PyrPush pp;
+    const int rc = pyr_push_plan(p, 1, ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, pad_mode, &pp);
+    if (rc) return rc;
+    const int64_t T = pp.t_end - ln.frames;
+    if ((i < A) != (T > 0)) return NNAB_EINVAL;               // the A lanes with frames come first
+    if (T == 0 && ln.n == 0 && !ln.end) return NNAB_EINVAL;   // a lane with nothing to do
+    if (T > o->T_max) o->T_max = T;
+    for (int s = 0; s < p.n_sig; ++s) {
+      const PyrLaneSig d = pyr_lane_signal(p, ln, i, s, pad_mode);
+      if (d.R0 != pp.R0[s] || d.R1 != pp.R1[s] || d.count != T) return NNAB_EINVAL;  // one set of rules
+      if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
+      if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
+    }
+  }
+  pyr_pool_layout(p, n_lanes, A, o);
   return NNAB_OK;
 }
 
@@ -1836,6 +1818,131 @@ size_t nnab_cqt_pyramid_pool_workspace_bytes(const nnab_stream_lane* lanes, int6
   return pl.total;
 }
 
+// The pyramid arguments both pool entry points share, checked on the host.
+static int pyr_pool_args_ok(int n_octaves, const float* const* h_k_real, const float* const* h_k_imag,
+                            const int32_t* h_widths, int n_filters, const float* lowpass, const float* early_filter,
+                            int early_factor, int hop, int pad_mode, int n_bins, int out_format) {
+  if (h_k_real == nullptr || h_k_imag == nullptr || h_widths == nullptr || lowpass == nullptr || n_octaves <= 0 ||
+      n_octaves > 32 || n_filters <= 0 || hop <= 0 || n_bins <= 0 || early_factor < 1 ||
+      (early_factor > 1 && early_filter == nullptr))
+    return NNAB_EINVAL;
+  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX && out_format != NNAB_FMT_PHASE_UNIT)
+    return NNAB_EINVAL;
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  return NNAB_OK;
+}
+
+// The whole-clip call's all-tensor-core plans need every packed operand and the tensor-core path.
+static bool pyr_packed_ok(int n_octaves, const void* const* h_packed, const void* lowpass_packed,
+                          const void* early_packed, int early_factor, int path) {
+  bool ok = path != NNAB_PATH_SIMT && h_packed != nullptr && lowpass_packed != nullptr &&
+            (early_factor <= 1 || early_packed != nullptr);
+  for (int i = 0; ok && i < n_octaves; ++i) ok = h_packed[i] != nullptr;
+  return ok;
+}
+
+// The body of a pool push on the plan `pl`: every signal's octave (on the A rows, T_max frames each), its FIR stage
+// (on the n_lanes rows) and its carry, then the mask.  `table` holds the (signal, lane) descriptors, which the plan
+// launch(es) have written before pass 1.  Pass 0 checks every launch against the kernels' limits on the host (as
+// the chunk call does) and enqueues nothing; pass 1 runs them.
+static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const PyramidCall& c, float* ring,
+                        const void* chunk, int chunk_dtype, int64_t slots, int64_t chunk_pitch, int64_t n_lanes,
+                        PyrLaneSig* table, char* ws, int pass) {
+  const int64_t A = c.B, T_max = c.T;
+  const cudaStream_t s = c.s;
+  char* scratch = ws + pl.scratch;
+  int rc;
+  for (int sg = 0; sg < p.n_sig; ++sg) {
+    ChunkSource cs{};
+    cs.ring = ring + (size_t)slots * p.ring_off[sg];
+    cs.ring_pitch = cs.ring_len = p.ring_len[sg];
+    cs.chunk = sg == 0 ? chunk : (const void*)(ws + pl.nbuf[sg]);
+    cs.chunk_pitch = sg == 0 ? chunk_pitch : pl.np[sg];
+    cs.pad_mode = NNAB_PAD_CONSTANT;
+    cs.rows = table + (size_t)sg * n_lanes;
+    const int dt = sg == 0 ? chunk_dtype : NNAB_DTYPE_F32;
+    const int l = sg - p.e;
+    if (l >= 0 && A > 0 && T_max > 0) {
+      // octave l: each row from its lane's first unreturned frame, T_max frames, on the whole-clip plan's kernel
+      ChunkSource co = cs;
+      co.rows_oct = 1;
+      co.pad = p.pad[l];
+      co.length = (T_max - 1) * p.hop[l] + p.width[l];
+      FramedProblem q = octave_problem(c, l, co.length, p.hop[l], c.pad_mode);
+      q.pad = 0; q.x_dtype = dt; q.chunk = &co;
+      if (p.gen2 && p.hop[l] % 8 == 0) {
+        int64_t pitch, plane;
+        pyr_oct_geom(p, l, A, co.length, &pitch, &plane);
+        FramedProblem qp = q;
+        qp.chunk = nullptr;
+        qp.presplit = scratch; qp.presplit_t_slots = pitch / p.hop[l]; qp.presplit_plane_stride = plane;
+        const bool oct = octave_tc_ok(qp);
+        if (pass == 0) {
+          if (!oct && !tc_supported(qp)) return NNAB_EUNSUPPORTED;
+        } else {
+          if ((rc = tc_chunk_split(co, dt, A, pitch, plane, scratch, s))) return rc;
+          if (oct) {
+            std::pair<cudaEvent_t, cudaEvent_t> pr;
+            const bool timed = prof_begin(s, &pr);
+            rc = launch_octave_tc(qp, c.packed[l], s);
+            if (timed) prof_end(s, pr);
+          } else {
+            rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
+          }
+          if (rc) return rc;
+        }
+      } else if (pass == 0) {
+        if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+      } else if ((rc = run_framed(q, c.packed[l], scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+        return rc;
+      }
+    }
+    if (sg + 1 < p.n_sig && pl.len_out[sg] > 0) {
+      // stage sg -> sg + 1 on every lane, each row from its lane's first 128-output row (the whole clip's
+      // accumulation order); row i of the new-sample buffer holds lane i's outputs from that row on
+      const int d = p.d[sg];
+      const int64_t FT = (pl.len_out[sg] + 127) / 128;
+      ChunkSource cf = cs;
+      cf.rows_oct = 0;
+      DecimParams dec{};
+      dec.len_out = pl.len_out[sg];
+      dec.lo = 0;
+      dec.y32 = (float*)(ws + pl.nbuf[sg + 1]);
+      dec.y32_pitch = pl.np[sg + 1];
+      dec.skip_edges = 3;
+      const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
+      if (p.gen2) {
+        if (pass == 1) {
+          const int64_t pitch = 256 * (FT + 1), plane = (n_lanes * (FT + 1) + 2) * 256;
+          cf.length = pitch;
+          if ((rc = tc_chunk_split(cf, dt, n_lanes, pitch, plane, scratch, s))) return rc;
+          if ((rc = launch_fir_stage_tc(scratch, n_lanes, 0, pitch, plane, FIR_OFF, fir_packed, c.lowpass,
+                                        FIR_TAPS, dec, s, cf.rows)))
+            return rc;
+        }
+      } else {
+        FramedProblem q{};
+        q.B = n_lanes; q.x_dtype = dt; q.F = 64; q.K = tc_fir_k(FIR_TAPS, d); q.hop = 128 * d;
+        q.L = (FT - 1) * q.hop + q.K; q.pad = 0; q.pad_mode = NNAB_PAD_CONSTANT; q.scale_all = 1.f;
+        q.fmt = FMT_DECIM; q.power = 1.f; q.T = FT; q.out_bins = 64;
+        q.dec = dec;
+        cf.length = q.L;
+        q.chunk = &cf;
+        if (pass == 0) {
+          if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
+        } else if ((rc = run_framed(q, fir_packed, scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
+          return rc;
+        }
+      }
+    }
+    // after this signal's readers: what later pushes read of it, into each lane's slot row of its ring
+    if (pass == 1 && (rc = tc_rows_carry(cs, dt, n_lanes, pl.longest[sg], s))) return rc;
+  }
+  if (pass == 0) return NNAB_OK;
+  // frames t >= a row's count were computed from the zeros past its stream: exact zeros
+  return tc_rows_mask(table, A, c.out, c.n_bins, T_max, format_cols(c.out_format), s);
+}
+
 int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
                                   int64_t n_lanes, int64_t A, const void* chunk, int chunk_dtype, int64_t slots,
                                   int64_t n, int64_t chunk_pitch, int n_octaves, const float* const* h_k_real,
@@ -1847,130 +1954,208 @@ int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, co
                                   void* workspace, size_t ws_bytes, int path, void* stream) {
   if (state == nullptr || !dtype_ok(chunk_dtype) || slots < 1 || slots > 65535 || n < 0 ||
       (n > 0 && chunk == nullptr) || chunk_pitch < n || n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes ||
-      T_max < 0 || (A > 0 && T_max > 0 && out == nullptr) || (n_lanes > 0 && (lanes == nullptr || d_lanes == nullptr)) ||
-      h_k_real == nullptr || h_k_imag == nullptr || h_widths == nullptr || lowpass == nullptr || n_octaves <= 0 ||
-      n_octaves > 32 || n_filters <= 0 || hop <= 0 || n_bins <= 0 || early_factor < 1 ||
-      (early_factor > 1 && early_filter == nullptr))
+      T_max < 0 || (A > 0 && T_max > 0 && out == nullptr) || (n_lanes > 0 && (lanes == nullptr || d_lanes == nullptr)))
     return NNAB_EINVAL;
-  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX && out_format != NNAB_FMT_PHASE_UNIT)
-    return NNAB_EINVAL;
-  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
-  const bool gen2 = pyr_gen2(n_octaves, h_widths, early_factor);
-  PyrStream p;
-  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, gen2, &p)) return NNAB_EUNSUPPORTED;
-  PyrPoolPlan pl;
-  int rc = pyr_pool_plan(p, lanes, n_lanes, A, slots, n, pad_mode, &pl);
+  int rc = pyr_pool_args_ok(n_octaves, h_k_real, h_k_imag, h_widths, n_filters, lowpass, early_filter, early_factor,
+                            hop, pad_mode, n_bins, out_format);
   if (rc) return rc;
+  PyrStream p;
+  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, pyr_gen2(n_octaves, h_widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  PyrPoolPlan pl;
+  if ((rc = pyr_pool_plan(p, lanes, n_lanes, A, slots, n, pad_mode, &pl))) return rc;
   if (pl.T_max != T_max) return NNAB_EINVAL;
-  bool packed_ok = path != NNAB_PATH_SIMT && h_packed != nullptr && lowpass_packed != nullptr &&
-                   (early_factor <= 1 || early_packed != nullptr);
-  for (int i = 0; packed_ok && i < n_octaves; ++i) packed_ok = h_packed[i] != nullptr;
-  if (!packed_ok) return NNAB_EUNSUPPORTED;
+  if (!pyr_packed_ok(n_octaves, h_packed, lowpass_packed, early_packed, early_factor, path)) return NNAB_EUNSUPPORTED;
   if ((rc = check_arch())) return rc;
   if (n_lanes == 0) return NNAB_OK;
   if (workspace == nullptr || ws_bytes < pl.total) return NNAB_EWORKSPACE;
   cudaStream_t s = (cudaStream_t)stream;
   char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  char* scratch = ws + pl.scratch;
   PyrLaneSig* table = (PyrLaneSig*)(ws + pl.table);
   // the octaves run on the A lanes with frames (rows 0 .. A - 1), T_max frames each
   const PyramidCall c{nullptr, NNAB_DTYPE_F32, A, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
                       n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
                       scale_all, out_format, sqrt_eps, out, T_max, ws, ws_bytes, s};
   float* ring = static_cast<float*>(state);
+  if ((rc = pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, n_lanes, table, ws, 0))) return rc;
+  if ((rc = tc_pyr_pool_plan(p, d_lanes, n_lanes, pad_mode, table, s))) return rc;
+  return pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, n_lanes, table, ws, 1);
+}
 
-  // pass 0 checks every launch against the kernels' limits, as the chunk call does; pass 1 runs them
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass == 1 && (rc = tc_pyr_pool_plan(p, d_lanes, n_lanes, pad_mode, table, s))) return rc;
-    for (int sg = 0; sg < p.n_sig; ++sg) {
-      ChunkSource cs{};
-      cs.ring = ring + (size_t)slots * p.ring_off[sg];
-      cs.ring_pitch = cs.ring_len = p.ring_len[sg];
-      cs.chunk = sg == 0 ? chunk : (const void*)(ws + pl.nbuf[sg]);
-      cs.chunk_pitch = sg == 0 ? chunk_pitch : pl.np[sg];
-      cs.pad_mode = NNAB_PAD_CONSTANT;
-      cs.rows = table + (size_t)sg * n_lanes;
-      const int dt = sg == 0 ? chunk_dtype : NNAB_DTYPE_F32;
-      const int l = sg - p.e;
-      if (l >= 0 && A > 0 && T_max > 0) {
-        // octave l: each row from its lane's first unreturned frame, T_max frames, on the whole-clip plan's kernel
-        ChunkSource co = cs;
-        co.rows_oct = 1;
-        co.pad = p.pad[l];
-        co.length = (T_max - 1) * p.hop[l] + p.width[l];
-        FramedProblem q = octave_problem(c, l, co.length, p.hop[l], pad_mode);
-        q.pad = 0; q.x_dtype = dt; q.chunk = &co;
-        if (gen2 && p.hop[l] % 8 == 0) {
-          int64_t pitch, plane;
-          pyr_oct_geom(p, l, A, co.length, &pitch, &plane);
-          FramedProblem qp = q;
-          qp.chunk = nullptr;
-          qp.presplit = scratch; qp.presplit_t_slots = pitch / p.hop[l]; qp.presplit_plane_stride = plane;
-          const bool oct = octave_tc_ok(qp);
-          if (pass == 0) {
-            if (!oct && !tc_supported(qp)) return NNAB_EUNSUPPORTED;
-          } else {
-            if ((rc = tc_chunk_split(co, dt, A, pitch, plane, scratch, s))) return rc;
-            if (oct) {
-              std::pair<cudaEvent_t, cudaEvent_t> pr;
-              const bool timed = prof_begin(s, &pr);
-              rc = launch_octave_tc(qp, c.packed[l], s);
-              if (timed) prof_end(s, pr);
-            } else {
-              rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
-            }
-            if (rc) return rc;
-          }
-        } else if (pass == 0) {
-          if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
-        } else if ((rc = run_framed(q, c.packed[l], scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
-          return rc;
-        }
+// ------------------------------------------------------------ device pyramid pools ----
+// The fixed geometry of a device pool's push (DESIGN §3.10 "Device pyramid pools"): over every slot's possible
+// push of at most `chunk` samples, an end included, the most frames (T_cap), FIR outputs of each stage from the
+// lane's first 128-output row (len_out) and samples one signal's carry stores (longest).  For a given total
+// t = received + n every one is nonincreasing in `received` (frames, R0 and R0's 128-row all grow with it, and the
+// frame bound, R1 and the ring's first kept sample depend on t alone), so the largest comes from the push that
+// reaches t with the most samples: n = chunk from received = t - chunk, or n = t from received = 0.  And every one
+// is periodic in t once start-up is past: shifting t by P shifts every count of signal s by P / (d_0 ... d_{s-1})
+// and the frames by P / (E hop) (E: the early factor, or 1), so with P = lcm(E hop, 128 d_0 ... d_{n-2}) the
+// frames, counts and 128-row alignments of every stage all repeat (ready(raw + f E hop) = ready(raw) + f).
+// Start-up is past once no clamp of the rules is active: every level holds at least M = 2 max width + 256 + c
+// samples (frames past every pad, rows past 128, the FIR read-back past 0), which raw >= (M + c) d_0 ... d_{n-2}
+// ensures.  So the sweep runs pyr_step and pyr_lane_signal themselves, with and without an end, on n = chunk over
+// received in [0, start-up + P) and on every n <= chunk from received = 0.  A refused end gets the zero lane and
+// contributes nothing; a refused push without an end never happens (pyr_stream_init's ring bounds), and the sweep
+// returns NNAB_EINVAL if it did.
+struct PyrCaps {
+  int64_t T_cap, len_out[33], longest[33];
+};
+
+static int pyr_caps_sweep(const PyrStream& p, int64_t chunk, int pad_mode, PyrCaps* o) {
+  int64_t D = 1;
+  for (int s = 0; s + 1 < p.n_sig; ++s) D *= p.d[s];
+  int max_w = 0;
+  for (int i = 0; i < p.n_oct; ++i) max_w = p.width[i] > max_w ? p.width[i] : max_w;
+  const int64_t M = 2 * (int64_t)max_w + 256 + p.c;
+  const int64_t E = p.e ? p.d[0] : 1;
+  const int64_t a = E * p.hop[0], b = 128 * D;
+  const int64_t period = a / gcd64(a, b) * b;
+  const int64_t sweep = (M + p.c) * D + period;
+  o->T_cap = 0;
+  for (int s = 0; s < 33; ++s) o->len_out[s] = o->longest[s] = 0;
+  for (int64_t k = -chunk; k < sweep; ++k) {  // k < 0: received 0, n = chunk + k
+    const int64_t rec = k < 0 ? 0 : k;
+    nnab_stream_lane ln{};
+    PyrStep st;
+    pyr_counts(p, rec, 0, st.R0);
+    ln.received = rec;
+    ln.frames = pyr_ready_frames(p, st.R0, pad_mode);
+    ln.n_carry = rec - pyr_keep(p, 0, st.R0, ln.frames);
+    ln.n = k < 0 ? chunk + k : chunk;
+    for (int end = 0; end < 2; ++end) {
+      ln.end = end;
+      if (pyr_step(p, ln.received, ln.n_carry, ln.frames, ln.n, end, pad_mode, &st) != NNAB_OK) {
+        if (!end) return NNAB_EINVAL;
+        continue;
       }
-      if (sg + 1 < p.n_sig && pl.len_out[sg] > 0) {
-        // stage sg -> sg + 1 on every lane, each row from its lane's first 128-output row (the whole clip's
-        // accumulation order); row i of the new-sample buffer holds lane i's outputs from that row on
-        const int d = p.d[sg];
-        const int64_t FT = (pl.len_out[sg] + 127) / 128;
-        ChunkSource cf = cs;
-        cf.rows_oct = 0;
-        DecimParams dec{};
-        dec.len_out = pl.len_out[sg];
-        dec.lo = 0;
-        dec.y32 = (float*)(ws + pl.nbuf[sg + 1]);
-        dec.y32_pitch = pl.np[sg + 1];
-        dec.skip_edges = 3;
-        const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
-        if (gen2) {
-          if (pass == 1) {
-            const int64_t pitch = 256 * (FT + 1), plane = (n_lanes * (FT + 1) + 2) * 256;
-            cf.length = pitch;
-            if ((rc = tc_chunk_split(cf, dt, n_lanes, pitch, plane, scratch, s))) return rc;
-            if ((rc = launch_fir_stage_tc(scratch, n_lanes, 0, pitch, plane, FIR_OFF, fir_packed, c.lowpass,
-                                          FIR_TAPS, dec, s, cf.rows)))
-              return rc;
-          }
-        } else {
-          FramedProblem q{};
-          q.B = n_lanes; q.x_dtype = dt; q.F = 64; q.K = tc_fir_k(FIR_TAPS, d); q.hop = 128 * d;
-          q.L = (FT - 1) * q.hop + q.K; q.pad = 0; q.pad_mode = NNAB_PAD_CONSTANT; q.scale_all = 1.f;
-          q.fmt = FMT_DECIM; q.power = 1.f; q.T = FT; q.out_bins = 64;
-          q.dec = dec;
-          cf.length = q.L;
-          q.chunk = &cf;
-          if (pass == 0) {
-            if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
-          } else if ((rc = run_framed(q, fir_packed, scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
-            return rc;
-          }
-        }
+      for (int s = 0; s < p.n_sig; ++s) {
+        const PyrLaneSig d = pyr_lane_signal(p, ln, 0, s, pad_mode);
+        if (d.count > o->T_cap) o->T_cap = d.count;
+        if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
+        if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
       }
-      // after this signal's readers: what later pushes read of it, into each lane's slot row of its ring
-      if (pass == 1 && (rc = tc_rows_carry(cs, dt, n_lanes, pl.longest[sg], s))) return rc;
     }
   }
-  // frames t >= a row's count were computed from the zeros past its stream: exact zeros
-  return tc_rows_mask(table, A, out, n_bins, T_max, format_cols(out_format), s);
+  return NNAB_OK;
+}
+
+// pyr_caps_sweep, computed once per geometry for the life of the process (the push checks its T_max against it).
+static int pyr_caps(const PyrStream& p, int64_t chunk, int pad_mode, PyrCaps* o) {
+  static std::mutex mu;
+  static std::vector<std::pair<std::vector<int64_t>, PyrCaps>> memo;
+  std::vector<int64_t> key{chunk, pad_mode, p.n_oct, p.e, p.d[0], p.c, p.hop[0]};
+  for (int i = 0; i < p.n_oct; ++i) key.push_back(p.width[i]);
+  {
+    std::lock_guard<std::mutex> g(mu);
+    for (const auto& m : memo)
+      if (m.first == key) { *o = m.second; return NNAB_OK; }
+  }
+  const int rc = pyr_caps_sweep(p, chunk, pad_mode, o);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(mu);
+  memo.emplace_back(key, *o);
+  return NNAB_OK;
+}
+
+// A device pool's plan: its caps, every slot a lane (n_lanes = A = slots), and the workspace layout.
+static int pyr_device_plan(int64_t slots, int64_t chunk, int n_octaves, const int32_t* widths, int hop,
+                           int early_factor, int pad_mode, PyrStream* p, PyrPoolPlan* o) {
+  if (slots < 1 || slots > 65535 || chunk < 1 || widths == nullptr ||
+      (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT))
+    return NNAB_EINVAL;
+  if (!pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), p))
+    return NNAB_EUNSUPPORTED;
+  PyrCaps caps;
+  const int rc = pyr_caps(*p, chunk, pad_mode, &caps);
+  if (rc) return rc;
+  o->T_max = caps.T_cap;
+  for (int s = 0; s < 33; ++s) {
+    o->len_out[s] = caps.len_out[s];
+    o->longest[s] = caps.longest[s];
+  }
+  pyr_pool_layout(*p, slots, slots, o);
+  return NNAB_OK;
+}
+
+int nnab_cqt_pyramid_pool_device_caps(int64_t chunk, int n_octaves, const int32_t* widths, int hop,
+                                      int early_factor, int pad_mode, int64_t* caps) {
+  if (caps == nullptr) return NNAB_EINVAL;
+  PyrStream p;
+  PyrPoolPlan pl;
+  const int rc = pyr_device_plan(1, chunk, n_octaves, widths, hop, early_factor, pad_mode, &p, &pl);
+  if (rc) return rc;
+  caps[0] = pl.T_max;
+  for (int s = 0; s < p.n_sig; ++s) {
+    caps[1 + s] = s + 1 < p.n_sig ? pl.len_out[s] : 0;
+    caps[1 + p.n_sig + s] = pl.longest[s];
+  }
+  return NNAB_OK;
+}
+
+size_t nnab_cqt_pyramid_pool_device_workspace_bytes(int64_t slots, int64_t chunk, int n_octaves,
+                                                    const int32_t* widths, int hop, int early_factor, int pad_mode) {
+  PyrStream p;
+  PyrPoolPlan pl;
+  if (pyr_device_plan(slots, chunk, n_octaves, widths, hop, early_factor, pad_mode, &p, &pl)) return 0;
+  return pl.total;
+}
+
+int nnab_cqt_pyramid_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
+                                         int32_t* errors, int64_t* error_info, int32_t* counts,
+                                         nnab_stream_lane* d_lanes, const void* chunk, int chunk_dtype, int64_t slots,
+                                         int64_t n, int64_t chunk_pitch, int n_octaves, const float* const* h_k_real,
+                                         const float* const* h_k_imag, const void* const* h_packed,
+                                         const int32_t* h_widths, int n_filters, const float* lowpass,
+                                         const void* lowpass_packed, const float* early_filter,
+                                         const void* early_packed, int early_factor, int hop, int pad_mode,
+                                         int n_bins, const float* scale, float scale_all, int out_format,
+                                         float sqrt_eps, float* out, int64_t T_max, void* workspace, size_t ws_bytes,
+                                         int path, void* stream) {
+  if (state == nullptr || counters == nullptr || lengths == nullptr || end == nullptr || errors == nullptr ||
+      error_info == nullptr || counts == nullptr || d_lanes == nullptr || chunk == nullptr || out == nullptr ||
+      !dtype_ok(chunk_dtype) || slots < 1 || slots > 65535 || n < 1 || chunk_pitch < n)
+    return NNAB_EINVAL;
+  int rc = pyr_pool_args_ok(n_octaves, h_k_real, h_k_imag, h_widths, n_filters, lowpass, early_filter, early_factor,
+                            hop, pad_mode, n_bins, out_format);
+  if (rc) return rc;
+  PyrStream p;
+  PyrPoolPlan pl;
+  if ((rc = pyr_device_plan(slots, n, n_octaves, h_widths, hop, early_factor, pad_mode, &p, &pl))) return rc;
+  if (T_max != pl.T_max) return NNAB_EINVAL;
+  if (!pyr_packed_ok(n_octaves, h_packed, lowpass_packed, early_packed, early_factor, path)) return NNAB_EUNSUPPORTED;
+  if ((rc = check_arch())) return rc;
+  if (workspace == nullptr || ws_bytes < pl.total) return NNAB_EWORKSPACE;
+  cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  PyrLaneSig* table = (PyrLaneSig*)(ws + pl.table);
+  // every slot is a lane and an octave row: row s of out is slot s, T_cap frames
+  const PyramidCall c{nullptr, NNAB_DTYPE_F32, slots, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
+                      n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
+                      scale_all, out_format, sqrt_eps, out, T_max, ws, ws_bytes, s};
+  float* ring = static_cast<float*>(state);
+  if ((rc = pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, slots, table, ws, 0))) return rc;
+  if ((rc = tc_device_pyramid_plan(p, slots, counters, lengths, end, errors, error_info, counts, d_lanes, n, pad_mode,
+                                   s)))
+    return rc;
+  if ((rc = tc_pyr_pool_plan(p, d_lanes, slots, pad_mode, table, s))) return rc;
+  return pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, slots, table, ws, 1);
+}
+
+int nnab_debug_device_pyramid_plan(int64_t* counters, const int32_t* lengths, const uint8_t* end, int32_t* errors,
+                                   int64_t* error_info, int32_t* counts, nnab_stream_lane* lanes, int64_t slots,
+                                   int64_t n, int n_octaves, const int32_t* widths, int hop, int early_factor,
+                                   int pad_mode) {
+  if (counters == nullptr || lengths == nullptr || end == nullptr || errors == nullptr || error_info == nullptr ||
+      counts == nullptr || lanes == nullptr || widths == nullptr || slots < 1 || n < 1 ||
+      (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT))
+    return NNAB_EINVAL;
+  PyrStream p;
+  if (!pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  for (int64_t s = 0; s < slots; ++s)
+    device_pyramid_slot(s, slots, counters, lengths, end, errors, error_info, counts, lanes, n, p, pad_mode);
+  return NNAB_OK;
 }
 
 int nnab_debug_pyramid_pool_plan(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A, int n_octaves,

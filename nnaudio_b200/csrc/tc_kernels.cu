@@ -354,6 +354,16 @@ __global__ void __launch_bounds__(128) pyr_pool_plan_kernel(const PyrStream p,
   table[k] = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
 }
 
+// A device pyramid pool's plan launch: one thread per slot.
+__global__ void __launch_bounds__(128) device_pyramid_plan_kernel(
+    const PyrStream p, int64_t slots, int64_t* __restrict__ counters, const int32_t* __restrict__ lengths,
+    const uint8_t* __restrict__ end, int32_t* __restrict__ errors, int64_t* __restrict__ info,
+    int32_t* __restrict__ counts, nnab_stream_lane* __restrict__ lanes, int64_t chunk, int pad_mode) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= slots) return;
+  device_pyramid_slot(s, slots, counters, lengths, end, errors, info, counts, lanes, chunk, p, pad_mode);
+}
+
 // chunk_split_kernel in the per-row descriptor mode (ChunkSource::rows): row b builds its own clip -- a FIR
 // stage source from the lane's first 128-output row, or an octave clip from its first unreturned frame -- from its
 // slot's ring row and its own source row, with its own counts, padding and end; past its samples, zeros.
@@ -383,6 +393,9 @@ __global__ void __launch_bounds__(256) chunk_split_rows_kernel(
       bool live = true;
       if (r < 0) {
         if (reflect) r = -r; else live = false;
+        // a row without frames yet (or the zero lane of an idle device-pool slot) may mirror past its own
+        // samples: those frames are masked, and nothing past R1 is there to read
+        if (r >= d.R1) live = false;
       } else if (r >= d.R1) {
         if (at_end && reflect && r - d.R1 < c.pad) r = 2 * (d.R1 - 1) - r; else live = false;
       }
@@ -1672,6 +1685,15 @@ int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t 
   if (n_lanes <= 0) return NNAB_OK;
   const int64_t n = n_lanes * p.n_sig;
   pyr_pool_plan_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, stream>>>(p, lanes, n_lanes, pad_mode, table);
+  NNAB_LAUNCH_CHECK();
+  return NNAB_OK;
+}
+
+int tc_device_pyramid_plan(const PyrStream& p, int64_t slots, int64_t* counters, const int32_t* lengths,
+                           const uint8_t* end, int32_t* errors, int64_t* info, int32_t* counts,
+                           nnab_stream_lane* lanes, int64_t chunk, int pad_mode, cudaStream_t stream) {
+  device_pyramid_plan_kernel<<<(unsigned)ceil_div64(slots, 128), 128, 0, stream>>>(
+      p, slots, counters, lengths, end, errors, info, counts, lanes, chunk, pad_mode);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }

@@ -31,8 +31,9 @@ output samples no later frame can change, ``flush(length=None)`` the rest.
 ``push(X, slots, counts, end, length)`` appends ``X[r, :, :counts[r]]`` to slot ``slots[r]``'s stream and ends the
 flagged slots; a ``PoolOutput`` of ``StreamPool`` feeds it as is.
 
-``DeviceStreamPool`` and ``DeviceInversePool`` are ``StreamPool`` and ``InversePool`` with their counters, lengths
-and end flags on the GPU and one fixed geometry per push, so a serving tick can be captured in a CUDA graph.
+``DeviceStreamPool``, ``DevicePyramidPool`` and ``DeviceInversePool`` are ``StreamPool``, ``PyramidPool`` and
+``InversePool`` with their counters, lengths and end flags on the GPU and one fixed geometry per push, so a serving
+tick can be captured in a CUDA graph.
 """
 from __future__ import annotations
 
@@ -51,7 +52,7 @@ from .features.stft import STFT, _inverse_args, iSTFT
 from .features.vqt import VQT
 
 __all__ = ["StreamingTransform", "StreamPool", "PoolOutput", "StreamingPyramid", "PyramidPool", "StreamingInverse",
-           "InversePool", "InverseOutput", "DeviceStreamPool", "DeviceInversePool"]
+           "InversePool", "InverseOutput", "DeviceStreamPool", "DevicePyramidPool", "DeviceInversePool"]
 
 _SUPPORTED = (STFT, MelSpectrogram, Gammatonegram, MFCC, CQT1992v2, CQT1992)
 _PYRAMIDS = (CQT2010v2, VQT, CQT2010)
@@ -941,6 +942,82 @@ class DeviceStreamPool(_DevicePool):
             raise _ended_error(s)
         if code == _C.LANE_ESHORT:
             _for_slot(s, self._st._check_length, a)  # the exception module(x) raises for a stream this short
+        raise RuntimeError(f"slot {s}: push dropped with error code {code}")
+
+
+class DevicePyramidPool(_DevicePool):
+    """``PyramidPool`` with every per-push number on the GPU, capturable in a CUDA graph like ``DeviceStreamPool``.
+
+    ``DevicePyramidPool(module, slots, chunk, dtype=torch.float32, **forward_kwargs)``: ``module`` and
+    ``forward_kwargs`` are ``PyramidPool``'s (``CQT2010v2``, ``VQT`` or ``CQT2010``; ``hop_length`` a multiple of
+    ``2 ** (n_octaves - 1)``), ``chunk`` the fixed chunk width and ``dtype`` the fixed sample type.  ``push(x,
+    lengths, end=None)``, ``reset(restart=None)``, ``errors``, ``error_info``, ``counters`` and ``check()`` are
+    ``DeviceStreamPool``'s; a push overwrites the pool-owned ``frames`` (slots, n_bins, T_cap[, 2]) float32 and
+    ``counts`` (slots,) int32.  Concatenated up to its counts, a slot's rows equal ``PyramidPool`` on the same packets
+    and ``module(x)`` on its whole stream, bit for bit (a 16-bit stream: ``module(x.float())``).  A push never sees
+    the lengths on the host, so it cannot issue the reflect-fallback ``UserWarning`` that ``module(x)`` and
+    ``PyramidPool`` give for a short stream; the frames are those of the fallback all the same.  A slot whose push
+    ``PyramidPool`` would refuse (a length outside [0, chunk], samples or an end on an ended stream, an end on a
+    stream too short for the module) is dropped whole and flagged in ``errors``.
+
+    ``T_cap``, the FIR outputs each stage computes per slot and the samples each ring takes per push are the most
+    one push of at most ``chunk`` samples can need, an end included (``_C.cqt_pyramid_pool_device_caps``).  Every
+    stage and octave runs on every slot at those caps on every push: an ending stream returns its whole pending
+    tail (the pyramid's look-ahead), so ``T_cap`` is that tail in frames plus the chunk's own, and an idle or
+    steady slot costs its share of that.  There is no concat route: a plan without a streamed tensor-core route
+    (``NNAUDIO_B200_PATH=simt``, a missing packed operand) raises ``RuntimeError`` at construction.  The constructor
+    builds every cache a push uses and allocates the rings, counters, outputs and workspace, so a captured push
+    allocates nothing.
+    """
+
+    def __init__(self, module, slots, chunk, dtype=torch.float32, **forward_kwargs):
+        slots, chunk = _streams(slots, "slots"), int(chunk)
+        if chunk < 1:
+            raise ValueError(f"chunk must be at least 1 sample, got {chunk}")
+        if dtype not in _C._WAVE_DTYPES:
+            raise ValueError(f"dtype must be float32, bfloat16 or float16, got {dtype}")
+        # module checks, the pyramid arguments, the plan and one ring row per slot per signal: StreamingPyramid's
+        self._sp = sp = StreamingPyramid(module, slots, **forward_kwargs)
+        self.module, self.chunk, self.dtype = module, chunk, dtype
+        self.widths, self.hop, self.early, self.generation = sp.widths, sp.hop, sp.early, sp.generation
+        self.ring = sp.ring
+        dev = self.ring.device
+        self._kw = kw = sp._args()  # banks, packed operands, filters, scale: built here and kept alive
+        self.T_cap = _C.cqt_pyramid_pool_device_caps(chunk, self.widths, self.hop, self.early, kw["pad_mode"])[0]
+        self._init_device(slots, _C.LANE_FIELDS, dev)
+        self._fn, self.frames, self._ws, self._tail = _C.pyramid_pool_device_bind(kw, slots, chunk, self.T_cap, dev)
+        # an idle push changes nothing; it finds a plan that cannot read the chunk before anything is enqueued
+        idle = torch.zeros(slots, dtype=torch.int32, device=dev)
+        if not _C.pool_device_forward(self, torch.zeros((slots, chunk), dtype=dtype, device=dev), idle, self._no_end):
+            raise RuntimeError(f"{type(module).__name__}: no streamed tensor-core pyramid plan for this call "
+                               "(NNAB_EUNSUPPORTED, e.g. NNAUDIO_B200_PATH=simt); DevicePyramidPool has no concat route")
+
+    def push(self, x: torch.Tensor, lengths: torch.Tensor, end: torch.Tensor = None):
+        """Append ``x[s, :lengths[s]]`` to every slot s and end the slots flagged in ``end``; the new frames go
+        to ``frames`` / ``counts``."""
+        _check_chunk(x, self.slots, self.dtype, width=self.chunk)
+        if x.device != self.ring.device:
+            raise RuntimeError(f"chunk is on {x.device}: the pool runs on {self.ring.device}")
+        if x.stride(-1) != 1 or (self.slots > 1 and x.stride(0) < self.chunk):
+            x = x.contiguous()
+        dev = self.ring.device
+        lengths = _device_vector(lengths, "lengths", self.slots, torch.int32, dev)
+        end = self._no_end if end is None else _device_vector(end, "end", self.slots, torch.bool, dev)
+        if not _C.pool_device_forward(self, x, lengths, end):
+            raise RuntimeError("no streamed tensor-core pyramid plan for this call (NNAB_EUNSUPPORTED)")
+
+    def check(self):
+        """Synchronise and raise what ``PyramidPool`` would have raised for the lowest slot with an error code."""
+        err = self._first_error()
+        if err is None:
+            return
+        s, code, a, _ = err
+        if code == _C.LANE_ELENGTH:
+            raise ValueError(f"lengths must be in [0, {self.chunk}] (the chunk width): slot {s} has {a}")
+        if code == _C.LANE_EENDED:
+            raise _ended_error(s)
+        if code == _C.LANE_ESHORT:
+            _for_slot(s, _pyramid_length_plan, self.module, 1, a)  # the exception module(x) raises for this length
         raise RuntimeError(f"slot {s}: push dropped with error code {code}")
 
 
