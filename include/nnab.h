@@ -725,6 +725,27 @@ int nnab_profile_read_exec_flops(double* exec_flops);
  * CTAs, framed_tct_kernel<., true>) since load -- lets a test tell which schedule it exercised. */
 uint64_t nnab_balanced_launch_count(void);
 
+/* Routes of nnab_cqt_pyramid_forward(_ex), counted since load so that a test can tell which one a call took.
+ * Each counter grows by one per successful enqueue of its stage, inside that entry point only: the plan once
+ * per call, an octave route once per octave, a FIR route once per decimation stage (the early stage included).
+ * The chunk, pool and device-pool entry points run the same kernels but count nothing. */
+enum {
+  NNAB_PYR_PLAN_GEN2 = 0,         /* one plane set per level, banded FIR stages                         */
+  NNAB_PYR_PLAN_GEN1 = 1,         /* early downsampling and any bank width, dense FIR stages             */
+  NNAB_PYR_PLAN_PER_OCTAVE = 2,   /* octave by octave on fp32 levels, CUDA-core FIR stages               */
+  NNAB_PYR_OCT_KERNEL = 3,        /* the octave kernel (resident bank, frame phases) on the level planes */
+  NNAB_PYR_OCT_DENSE_PLANES = 4,  /* the dense tensor-core kernel on the level planes (hop % 8 == 0)     */
+  NNAB_PYR_OCT_DENSE_FP32 = 5,    /* the dense tensor-core kernel on the fp32 level, split per frame phase */
+  NNAB_PYR_OCT_TC_LOOP = 6,       /* per-octave plan: the dense tensor-core kernel                       */
+  NNAB_PYR_OCT_SIMT = 7,          /* per-octave plan: the SIMT kernel                                    */
+  NNAB_PYR_FIR_BANDED = 8,        /* gen-2: banded tensor-core FIR stage with its clip-edge fix          */
+  NNAB_PYR_FIR_DENSE = 9,         /* gen-1: FIR stage on the dense tensor-core kernel                    */
+  NNAB_PYR_FIR_SIMT = 10,         /* per-octave plan: CUDA-core FIR stage                                */
+  NNAB_PYR_ROUTES = 11
+};
+/* The counter of `route` (an NNAB_PYR_* value); 0 for any other value. */
+uint64_t nnab_pyramid_route_count(int route);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

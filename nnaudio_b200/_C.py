@@ -41,6 +41,7 @@ SIGNATURES = {
     "nnab_profile_read": (c_int, [_P, _P]),
     "nnab_profile_read_exec_flops": (c_int, [_P]),
     "nnab_balanced_launch_count": (c_uint64, []),
+    "nnab_pyramid_route_count": (c_uint64, [c_int]),
     "nnab_pack_tile_n": (c_int, [c_int]),
     "nnab_packed_basis_bytes": (c_size_t, [c_int, c_int]),
     "nnab_pack_basis": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -225,6 +226,18 @@ def launch_count() -> int:
 def balanced_launch_count() -> int:
     """Tall-A CQT launches that ran the balanced (shared-tile) schedule since load."""
     return int(lib().nnab_balanced_launch_count())
+
+
+# routes of nnab_cqt_pyramid_forward (NNAB_PYR_*): the plan, each octave's kernel, each FIR stage's kernel
+(PYR_PLAN_GEN2, PYR_PLAN_GEN1, PYR_PLAN_PER_OCTAVE, PYR_OCT_KERNEL, PYR_OCT_DENSE_PLANES, PYR_OCT_DENSE_FP32,
+ PYR_OCT_TC_LOOP, PYR_OCT_SIMT, PYR_FIR_BANDED, PYR_FIR_DENSE, PYR_FIR_SIMT) = range(11)
+PYR_ROUTES = 11
+
+
+def pyramid_route_count(route: int) -> int:
+    """Stages of the offline CQT pyramid call that took ``route`` (a PYR_* constant) since load; the streaming
+    and pool calls count nothing."""
+    return int(lib().nnab_pyramid_route_count(int(route)))
 
 
 def set_sm_reserve(n_sms: int) -> int:

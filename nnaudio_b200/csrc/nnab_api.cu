@@ -25,6 +25,8 @@ void set_cuda_error(const char* where, cudaError_t e) {
 void set_error_text(const char* text) { snprintf(g_err, sizeof(g_err), "%s", text); }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 void count_balanced_launch() { g_balanced_launches.fetch_add(1, std::memory_order_relaxed); }
+static std::atomic<uint64_t> g_pyr_routes[NNAB_PYR_ROUTES];
+static void count_route(int route) { g_pyr_routes[route].fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<int> g_sm_reserve{0};
 int sm_reserve() { return g_sm_reserve.load(std::memory_order_relaxed); }
 
@@ -358,6 +360,10 @@ const char* nnab_last_cuda_error(void) { return g_err; }
 uint64_t nnab_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 uint64_t nnab_balanced_launch_count(void) { return g_balanced_launches.load(std::memory_order_relaxed); }
+uint64_t nnab_pyramid_route_count(int route) {
+  if (route < 0 || route >= NNAB_PYR_ROUTES) return 0;
+  return g_pyr_routes[route].load(std::memory_order_relaxed);
+}
 
 int nnab_set_sm_reserve(int n_sms) {
   if (n_sms < 0) n_sms = 0;
@@ -1150,18 +1156,23 @@ static int pyramid_fused2(const PyramidCall& c, const Lvl2* lv, size_t scratch_o
   for (int i = 0; i < c.n_octaves; ++i) {
     const Lvl2& l = lv[i];
     const FramedProblem p = octave2_problem(c, l, i);
+    int route;
     if (octave_tc_ok(p)) {
       // resident bank + tall A blocks + frame phases: one fetch per sample and tile
       std::pair<cudaEvent_t, cudaEvent_t> pr;
       const bool timed = prof_begin(s, &pr);
       rc = launch_octave_tc(p, c.packed[i], s);
       if (timed) prof_end(s, pr);
+      route = NNAB_PYR_OCT_KERNEL;
     } else if (l.presplit) {
       rc = run_framed(p, c.packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s);
+      route = NNAB_PYR_OCT_DENSE_PLANES;
     } else {
       rc = run_framed(p, c.packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s);
+      route = NNAB_PYR_OCT_DENSE_FP32;
     }
     if (rc) return rc;
+    count_route(route);
     if (i == c.n_octaves - 1) break;
     // ---- FIR stage: level i -> level i + 1
     const Lvl2& d = lv[i + 1];
@@ -1180,7 +1191,9 @@ static int pyramid_fused2(const PyramidCall& c, const Lvl2* lv, size_t scratch_o
     rc = launch_fir_stage_tc(ws + l.pc, B, l.len, l.pitch, l.plane, l.pad, c.lowpass_packed, c.lowpass,
                              FIR_TAPS, dec, s);
     if (rc) return rc;
+    count_route(NNAB_PYR_FIR_BANDED);
   }
+  count_route(NNAB_PYR_PLAN_GEN2);
   return NNAB_OK;
 }
 
@@ -1261,7 +1274,9 @@ static int pyramid_fused(const PyramidCall& c, const PyrLevel* lv, size_t pf_ear
       rc = tc_zero_slots(ws + dst.pf, B, dst.pf_pitch, dst.pf_plane, FIR_OFF, FIR_OFF + dst.len, s);
       if (rc) return rc;
     }
-    return run_framed(fir1_problem(c, src, src_len, dec, dst), fir_packed, nullptr, 0, NNAB_PATH_TCGEN05, s);
+    rc = run_framed(fir1_problem(c, src, src_len, dec, dst), fir_packed, nullptr, 0, NNAB_PATH_TCGEN05, s);
+    if (rc == NNAB_OK) count_route(NNAB_PYR_FIR_DENSE);
+    return rc;
   };
 
   // ---- level 0 ------------------------------------------------------------------------
@@ -1295,9 +1310,11 @@ static int pyramid_fused(const PyramidCall& c, const PyrLevel* lv, size_t pf_ear
     if (l.presplit) rc = run_framed(p, c.packed[i], nullptr, 0, NNAB_PATH_TCGEN05, s);
     else rc = run_framed(p, c.packed[i], scratch, scratch_bytes, NNAB_PATH_TCGEN05, s);
     if (rc) return rc;
+    count_route(l.presplit ? NNAB_PYR_OCT_DENSE_PLANES : NNAB_PYR_OCT_DENSE_FP32);
     if (i < c.n_octaves - 1)
       if ((rc = fir_stage(ws + l.pf, l.len, 2, c.lowpass_packed, lv[i + 1]))) return rc;
   }
+  count_route(NNAB_PYR_PLAN_GEN1);
   return NNAB_OK;
 }
 
@@ -1386,6 +1403,7 @@ int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L
     if ((rc = launch_fir_decimate(cur, B, L, x_pitch, early_filter, 256, early_factor, e, L0,
                                   pitch0, s)))
       return rc;
+    count_route(NNAB_PYR_FIR_SIMT);
     cur = e; cur_len = L0; cur_pitch = pitch0;
   }
   const int64_t half_pitch = (int64_t)align_up((size_t)(cur_len / 2 + 1), 4);
@@ -1401,6 +1419,7 @@ int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L
       if ((rc = launch_fir_decimate(cur, B, cur_len, cur_pitch, lowpass, 256, 2, dst, nl,
                                     half_pitch, s)))
         return rc;
+      count_route(NNAB_PYR_FIR_SIMT);
       cur = dst; cur_len = nl; cur_pitch = half_pitch;
       cur_hop /= 2;
     }
@@ -1417,11 +1436,14 @@ int nnab_cqt_pyramid_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L
     if (pk != nullptr && path != NNAB_PATH_SIMT && tc_supported(p) &&
         tc_ws_bytes >= tc_workspace_bytes(B, cur_len, width, cur_hop, pad)) {
       if ((rc = run_framed(p, pk, tc_ws, tc_ws_bytes, NNAB_PATH_TCGEN05, s))) return rc;
+      count_route(NNAB_PYR_OCT_TC_LOOP);
     } else {
       if (path == NNAB_PATH_TCGEN05) return NNAB_EALIGN;
       if ((rc = run_framed(p, nullptr, nullptr, 0, NNAB_PATH_SIMT, s))) return rc;
+      count_route(NNAB_PYR_OCT_SIMT);
     }
   }
+  count_route(NNAB_PYR_PLAN_PER_OCTAVE);
   return NNAB_OK;
 }
 

@@ -205,19 +205,30 @@ class CQT(CQT1992v2):
     pass
 
 
+def _decimated_len(n, factor):
+    """Samples conv1d(stride=factor, padding=127) leaves of ``n`` under the 256-tap FIR (utils.py:73-100)."""
+    return (n - 2) // factor + 1 if n >= 2 else 0
+
+
+def _octave_levels(L, hop, n_octaves):
+    """(signal lengths, hops) of the octaves of the ÷2 pyramid on a level-0 signal of ``L`` samples."""
+    lens, hops = [], []
+    cur, h = L, hop
+    for i in range(n_octaves):
+        if i > 0:
+            cur = _decimated_len(cur, 2)
+            h = h // 2
+        lens.append(cur)
+        hops.append(h)
+    return lens, hops
+
+
 def _octave_plan(L, hop, widths, pad_mode):
     """Per-octave signal lengths of the ÷2 pyramid and whether the reference's
     reflect padding would fall back to zero padding (utils.py:505-517).
     Returns (T, fallback_flags) or raises like torch.cat would."""
-    lens, hops, flags = [], [], []
-    cur, h = L, hop
-    for i, w in enumerate(widths):
-        if i > 0:
-            cur = (cur - 2) // 2 + 1 if cur >= 2 else 0
-            h = h // 2
-        lens.append(cur)
-        hops.append(h)
-        flags.append(pad_mode == "reflect" and w // 2 >= cur)
+    lens, hops = _octave_levels(L, hop, len(widths))
+    flags = [pad_mode == "reflect" and w // 2 >= cur for w, cur in zip(widths, lens)]
     if min(hops) <= 0 or min(lens) <= 0:
         raise RuntimeError(
             "CQT pyramid: hop_length or signal too small for the number of octaves "
@@ -386,7 +397,7 @@ def _pyramid_length_plan(mod, B, L):
     """(T, per-octave reflect fallbacks) of ``B`` clips of ``L`` samples through ``mod``'s pyramid, with the
     reference's errors and warnings (also the end of a stream)."""
     factor = int(mod.downsample_factor) if mod.earlydownsample else 1
-    L0 = (L - 2) // factor + 1 if factor > 1 else L
+    L0 = _decimated_len(L, factor) if factor > 1 else L
     if factor > 1 and L < 2:
         raise RuntimeError("Kernel size can't be greater than actual input size")
     widths = [int(b.shape[1]) for b in mod._banks()[0]]
