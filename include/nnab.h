@@ -746,6 +746,22 @@ enum {
 /* The counter of `route` (an NNAB_PYR_* value); 0 for any other value. */
 uint64_t nnab_pyramid_route_count(int route);
 
+/* Kernel routes of nnab_cqt1992v2_forward(_ex), counted since load so that a test can tell which one a call took.
+ * Each successful call adds one to the counter of the route it enqueued (a dense call once, however many frame
+ * phases it launches).  The chunk, pool and device-pool entry points run the same kernels but count nothing. */
+enum {
+  NNAB_CQ1992_TALL = 0,           /* tall-A kernel (8-bin-group bank), static schedule                  */
+  NNAB_CQ1992_TALL_BALANCED = 1,  /* tall-A kernel, balanced schedule (nnab_balanced_launch_count)      */
+  NNAB_CQ1992_VARN = 2,           /* per-K-block-width kernel (8-bin-group bank the tall kernel refuses) */
+  NNAB_CQ1992_VARN_SPLITK = 3,    /* the same, K cut into chunks, then the split-K finalize             */
+  NNAB_CQ1992_DENSE = 4,          /* dense tensor-core kernel, one launch per frame phase               */
+  NNAB_CQ1992_DENSE_SPLITK = 5,   /* the same with K cut into chunks, then the split-K finalize         */
+  NNAB_CQ1992_SIMT = 6,           /* CUDA-core kernel                                                   */
+  NNAB_CQ1992_ROUTES = 7
+};
+/* The counter of `route` (an NNAB_CQ1992_* value); 0 for any other value. */
+uint64_t nnab_cqt1992v2_route_count(int route);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -42,6 +42,7 @@ SIGNATURES = {
     "nnab_profile_read_exec_flops": (c_int, [_P]),
     "nnab_balanced_launch_count": (c_uint64, []),
     "nnab_pyramid_route_count": (c_uint64, [c_int]),
+    "nnab_cqt1992v2_route_count": (c_uint64, [c_int]),
     "nnab_pack_tile_n": (c_int, [c_int]),
     "nnab_packed_basis_bytes": (c_size_t, [c_int, c_int]),
     "nnab_pack_basis": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -238,6 +239,18 @@ def pyramid_route_count(route: int) -> int:
     """Stages of the offline CQT pyramid call that took ``route`` (a PYR_* constant) since load; the streaming
     and pool calls count nothing."""
     return int(lib().nnab_pyramid_route_count(int(route)))
+
+
+# kernel routes of nnab_cqt1992v2_forward (NNAB_CQ1992_*)
+(CQ1992_TALL, CQ1992_TALL_BALANCED, CQ1992_VARN, CQ1992_VARN_SPLITK, CQ1992_DENSE, CQ1992_DENSE_SPLITK,
+ CQ1992_SIMT) = range(7)
+CQ1992_ROUTES = 7
+
+
+def cqt1992v2_route_count(route: int) -> int:
+    """Offline CQT1992v2 calls that took kernel route ``route`` (a CQ1992_* constant) since load; the streaming
+    and pool calls count nothing."""
+    return int(lib().nnab_cqt1992v2_route_count(int(route)))
 
 
 def set_sm_reserve(n_sms: int) -> int:

@@ -27,6 +27,7 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 void count_balanced_launch() { g_balanced_launches.fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<uint64_t> g_pyr_routes[NNAB_PYR_ROUTES];
 static void count_route(int route) { g_pyr_routes[route].fetch_add(1, std::memory_order_relaxed); }
+static std::atomic<uint64_t> g_cq1992_routes[NNAB_CQ1992_ROUTES];
 static std::atomic<int> g_sm_reserve{0};
 int sm_reserve() { return g_sm_reserve.load(std::memory_order_relaxed); }
 
@@ -119,7 +120,9 @@ static int run_framed_inner(const FramedProblem& p, const void* packed, void* ws
     return NNAB_EINVAL;
   }
   if (use_tc) return launch_framed_tc(p, packed, ws, ws_bytes, stream);
-  return launch_framed_simt(p, stream);
+  const int rc = launch_framed_simt(p, stream);
+  if (rc == NNAB_OK && p.route != nullptr) *p.route = NNAB_CQ1992_SIMT;
+  return rc;
 }
 
 // The split-K scratch (long kernels only) sits behind the split-signal planes in the workspace.
@@ -363,6 +366,10 @@ uint64_t nnab_balanced_launch_count(void) { return g_balanced_launches.load(std:
 uint64_t nnab_pyramid_route_count(int route) {
   if (route < 0 || route >= NNAB_PYR_ROUTES) return 0;
   return g_pyr_routes[route].load(std::memory_order_relaxed);
+}
+uint64_t nnab_cqt1992v2_route_count(int route) {
+  if (route < 0 || route >= NNAB_CQ1992_ROUTES) return 0;
+  return g_cq1992_routes[route].load(std::memory_order_relaxed);
 }
 
 int nnab_set_sm_reserve(int n_sms) {
@@ -817,7 +824,8 @@ static int cqt1992v2_args_ok(const float* k_real, const float* k_imag, int out_f
 static int cqt1992v2_run(const Wave& w, const float* k_real, const float* k_imag, const void* packed,
                          const int32_t* h_k_begin, const int32_t* h_k_end, int n_bins, int width, int hop,
                          const float* scale, float scale_all, int out_format, float sqrt_eps, float* out,
-                         int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream) {
+                         int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream,
+                         int* route = nullptr) {
   FramedProblem p{};
   set_wave(p, w);
   p.w_re = k_real; p.w_im = k_imag; p.F = n_bins; p.K = width; p.hop = hop;
@@ -825,6 +833,7 @@ static int cqt1992v2_run(const Wave& w, const float* k_real, const float* k_imag
   p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
   p.out_bins = n_bins; p.bin_offset = 0;
   p.h_k_begin = h_k_begin; p.h_k_end = h_k_end;
+  p.route = route;
   attach_splitk_scratch(p, workspace, ws_bytes);
   return run_framed(p, packed, workspace, ws_bytes, path, stream);
 }
@@ -853,9 +862,12 @@ int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, 
   if (rc) return rc;
   if (out == nullptr || cqt1992v2_args_ok(k_real, k_imag, out_format)) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  return cqt1992v2_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, k_real, k_imag, packed, h_k_begin,
-                       h_k_end, n_bins, width, hop, scale, scale_all, out_format, sqrt_eps, out, T, workspace,
-                       ws_bytes, path, (cudaStream_t)stream);
+  int route = -1;  // stays -1 when nothing was enqueued
+  rc = cqt1992v2_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, k_real, k_imag, packed, h_k_begin,
+                     h_k_end, n_bins, width, hop, scale, scale_all, out_format, sqrt_eps, out, T, workspace,
+                     ws_bytes, path, (cudaStream_t)stream, &route);
+  if (rc == NNAB_OK && route >= 0) g_cq1992_routes[route].fetch_add(1, std::memory_order_relaxed);
+  return rc;
 }
 
 // ------------------------------------------------ CQT2010v2 / VQT pyramid ----

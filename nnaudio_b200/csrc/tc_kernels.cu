@@ -2100,7 +2100,9 @@ static int launch_framed_tc_varn(const FramedProblem& q, const void* packed, voi
     default: rc = NNAB_EINVAL;
   }
   if (rc) return rc;
-  return split ? launch_splitk_finalize(final_epi, q.B, stream) : NNAB_OK;
+  if (split && (rc = launch_splitk_finalize(final_epi, q.B, stream))) return rc;
+  if (q.route != nullptr) *q.route = split ? NNAB_CQ1992_VARN_SPLITK : NNAB_CQ1992_VARN;
+  return NNAB_OK;
 }
 
 int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace, size_t ws_bytes,
@@ -2212,7 +2214,9 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
     rc = launch_tc_kernel(s.ma, mb, prm, grid, stream);
     if (rc) return rc;
   }
-  return split ? launch_splitk_finalize(final_epi, q.B, stream) : NNAB_OK;
+  if (split && (rc = launch_splitk_finalize(final_epi, q.B, stream))) return rc;
+  if (q.route != nullptr) *q.route = split ? NNAB_CQ1992_DENSE_SPLITK : NNAB_CQ1992_DENSE;
+  return NNAB_OK;
 }
 
 }  // namespace nnab

@@ -545,9 +545,12 @@ int launch_framed_tc_tall(const FramedProblem& q, const void* packed, void* work
   }
   if (balanced) {
     count_balanced_launch();
-    return launch_tct<true>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
+    rc = launch_tct<true>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
+  } else {
+    rc = launch_tct<false>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
   }
-  return launch_tct<false>(q.fmt, ma, mb8, mb32, prm, plan, grid, stream);
+  if (rc == NNAB_OK && q.route != nullptr) *q.route = balanced ? NNAB_CQ1992_TALL_BALANCED : NNAB_CQ1992_TALL;
+  return rc;
 }
 
 // ===========================================================================
