@@ -479,7 +479,10 @@ int nnab_cqt1992v2_pool_forward(void* state, const nnab_stream_lane* lanes, cons
  * (d = 2, or early_factor for the early stage; c = 130 on the plan without early downsampling whose FIR-source
  * banks are 256 wide ("generation 2"), else 129), and T counts the frames final in every octave; on flush
  * every level gets its full length and T is the rest (octave frame counts that differ: NNAB_EINVAL).  The
- * pushes run the whole-clip call's tensor-core plan and kernels, so their frames equal it bit for bit.  hop
+ * pushes run the whole-clip call's tensor-core plan and kernels, so their frames equal it bit for bit.  A push is
+ * the pool push (nnab_cqt_pyramid_pool_forward) of B lanes that share these counters, lane b in slot b: one plan
+ * launch that writes the lanes' descriptors, then per signal its octave launches on the B rows (when T > 0), its
+ * FIR stage launches and its carry launch, then one mask launch.  hop
  * must be a multiple of 2^(n_octaves - 1).  The SIMT path, a missing packed operand, or a launch outside the
  * kernels' limits returns NNAB_EUNSUPPORTED before anything is enqueued.  Both size queries are host-only. */
 size_t nnab_cqt_pyramid_chunk_state_bytes(int64_t B, int n_octaves, const int32_t* widths, int hop,
@@ -512,9 +515,9 @@ int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t fra
  * by that call's rules (counters, frame bound, ring capacity, the octaves' frame counts at an end), the table by the
  * pools' (order, repeated slots, A, T_max, n above the chunk width), and every launch against the kernels' limits,
  * all before anything is enqueued.  Row i of out (A, n_bins, T_max[, 2]) holds lane i's frames, bit for bit those
- * of the whole-clip call on its stream, then exact zeros.  The launches are the chunk call's over the same stages
- * on (n_lanes, ...) rows (the octaves on the A rows), one plan launch and one mask launch.  The workspace query is
- * host-only and takes the host lane table. */
+ * of the whole-clip call on its stream, then exact zeros.  The launches are the chunk call's, the plan and mask
+ * launches included, over the same stages on (n_lanes, ...) rows (the octaves on the A rows).  The workspace query
+ * is host-only and takes the host lane table. */
 size_t nnab_cqt_pyramid_pool_workspace_bytes(const nnab_stream_lane* lanes, int64_t n_lanes, int64_t A,
                                              int64_t T_max, int n_octaves, const int32_t* widths, int hop,
                                              int early_factor, int pad_mode);

@@ -64,11 +64,6 @@ struct DecimParams {
   void* pf; int64_t pf_plane, pf_pitch;
   float* y32; int64_t y32_pitch;
   int64_t len_out;  // valid samples per clip of the next level
-  // streamed pushes (DESIGN §3.10): outputs below `lo` are not stored and y32 holds output n at n - lo;
-  // skip_edges bit 0 / 1: fir_edge_fix_kernel leaves the head / tail alone (the launch does not start at the
-  // stream's first output / the stream has not ended).  Zero for the whole-clip call.
-  int64_t lo;
-  int skip_edges;
 };
 
 // Banded filterbank table: the (at most two) non-zero weights of every FFT bin.
@@ -650,10 +645,11 @@ int tc_device_istft_plan(int64_t slots, int64_t* counters, const int32_t* frame_
 int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int64_t* info, const uint8_t* mask,
                          cudaStream_t stream);
 // pyramid pools: the (signal, lane) descriptor table of a push (table[s * n_lanes + i] = pyr_lane_signal of lane i
-// of the DEVICE lane table), every row's carry [keep, R1) of one signal (cs.rows; at most `longest` samples), and
-// the zeroing of frames t >= rows[i].count of row i of out (A, n_rows, T, cols)
-int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int pad_mode,
-                     PyrLaneSig* table, cudaStream_t stream);
+// of the DEVICE lane table, or with lanes == nullptr of `shared` in slot i), every row's carry [keep, R1) of one
+// signal (cs.rows; at most `longest` samples), and the zeroing of frames t >= rows[i].count of row i of out
+// (A, n_rows, T, cols)
+int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, const nnab_stream_lane& shared,
+                     int64_t n_lanes, int pad_mode, PyrLaneSig* table, cudaStream_t stream);
 // device pyramid pools: the plan launch (device_pyramid_slot per slot)
 int tc_device_pyramid_plan(const PyrStream& p, int64_t slots, int64_t* counters, const int32_t* lengths,
                            const uint8_t* end, int32_t* errors, int64_t* info, int32_t* counts,

@@ -1503,13 +1503,6 @@ static bool pyr_stream_init(int n_octaves, const int32_t* widths, int hop, int e
   return true;
 }
 
-// One push: the stream's step (PyrStep: the counts before and after it, the frames it returns, each octave's
-// padding) and the workspace layout.
-struct PyrPush : PyrStep {
-  int64_t np[33];             // new-sample buffer pitch of signal s >= 1 (floats)
-  size_t nbuf[33], scratch, scratch_bytes, total;
-};
-
 // Plane geometry of octave l's push clip of `len` samples for the octave kernel (gen-2 single-phase levels):
 // (clip pitch, plane stride); the pitch is a multiple of lcm(hop, 64), as the kernel's row blocks need.
 static void pyr_oct_geom(const PyrStream& p, int l, int64_t B, int64_t len, int64_t* pitch, int64_t* plane) {
@@ -1519,47 +1512,6 @@ static void pyr_oct_geom(const PyrStream& p, int l, int64_t B, int64_t len, int6
   const int64_t kpad = (p.width[l] + 63) / 64 * 64;
   const int64_t rows = B * (*pitch / h) + (kpad + h - 1) / h + 1;
   *plane = (rows * h + 255) / 256 * 256;
-}
-
-static int pyr_push_plan(const PyrStream& p, int64_t B, int64_t received, int64_t n_carry, int64_t frames,
-                         int64_t n, int flush, int pad_mode, PyrPush* o) {
-  if (B < 0 || B > 65535) return NNAB_EINVAL;
-  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
-  const int rc = pyr_step(p, received, n_carry, frames, n, flush, pad_mode, o);
-  if (rc) return rc;
-  // workspace: the new samples of every computed signal, then one scratch reused by the launches in order
-  size_t off = 0;
-  for (int s = 1; s < p.n_sig; ++s) {
-    o->np[s] = (int64_t)align_up((size_t)(o->R1[s] - o->R0[s] > 0 ? o->R1[s] - o->R0[s] : 1), 8);
-    o->nbuf[s] = off;
-    off += align_up((size_t)B * o->np[s] * sizeof(float), 256);
-  }
-  size_t sc = 0;
-  const int64_t T = o->t_end - frames;
-  for (int s = 0; s < p.n_sig; ++s) {
-    const int l = s - p.e;
-    if (l >= 0 && T > 0) {
-      const int64_t len = (T - 1) * p.hop[l] + p.width[l];
-      size_t need = tc_workspace_bytes(B, len, p.width[l], p.hop[l], 0);
-      if (p.gen2 && p.hop[l] % 8 == 0) {
-        int64_t pitch, plane;
-        pyr_oct_geom(p, l, B, len, &pitch, &plane);
-        need = (size_t)plane * 4 + 256;
-      }
-      sc = need > sc ? need : sc;
-    }
-    if (s + 1 < p.n_sig && o->R1[s + 1] > o->R0[s + 1]) {
-      const int64_t FT = (o->R1[s + 1] + 127) / 128 - o->R0[s + 1] / 128;
-      const int kf = tc_fir_k(FIR_TAPS, p.d[s]);
-      const size_t need = p.gen2 ? (size_t)((B * (FT + 1) + 2) * 256) * 4 + 256
-                                 : tc_workspace_bytes(B, (FT - 1) * 128 * (int64_t)p.d[s] + kf, kf, 128 * p.d[s], 0);
-      sc = need > sc ? need : sc;
-    }
-  }
-  o->scratch = off;
-  o->scratch_bytes = sc;
-  o->total = off + sc + 512;
-  return NNAB_OK;
 }
 
 // The whole-clip call's plan for these shapes: gen-2 without early downsampling when every FIR-source bank is
@@ -1578,191 +1530,10 @@ size_t nnab_cqt_pyramid_chunk_state_bytes(int64_t B, int n_octaves, const int32_
   return (size_t)B * p.state_floats * sizeof(float);
 }
 
-size_t nnab_cqt_pyramid_chunk_workspace_bytes(int64_t B, int64_t received, int64_t n_carry, int64_t frames,
-                                              int64_t n, int flush, int n_octaves, const int32_t* widths,
-                                              int hop, int early_factor, int pad_mode) {
-  PyrStream p;
-  PyrPush pp;
-  if (widths == nullptr ||
-      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
-    return 0;
-  if (pyr_push_plan(p, B, received, n_carry, frames, n, flush, pad_mode, &pp)) return 0;
-  return pp.total;
-}
-
-int nnab_cqt_pyramid_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
-                                   const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
-                                   int flush, int n_octaves, const float* const* h_k_real,
-                                   const float* const* h_k_imag, const void* const* h_packed,
-                                   const int32_t* h_widths, int n_filters, const float* lowpass,
-                                   const void* lowpass_packed, const float* early_filter, const void* early_packed,
-                                   int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
-                                   float scale_all, int out_format, float sqrt_eps, float* out, int64_t T,
-                                   void* workspace, size_t ws_bytes, int path, void* stream) {
-  if (state == nullptr || !dtype_ok(chunk_dtype) || (n > 0 && chunk == nullptr) || chunk_pitch < n ||
-      (T > 0 && out == nullptr) || h_k_real == nullptr || h_k_imag == nullptr || h_widths == nullptr ||
-      lowpass == nullptr || n_octaves <= 0 || n_octaves > 32 || n_filters <= 0 || hop <= 0 || n_bins <= 0 ||
-      early_factor < 1 || (early_factor > 1 && early_filter == nullptr) || T < 0)
-    return NNAB_EINVAL;
-  if (out_format != NNAB_FMT_MAGNITUDE && out_format != NNAB_FMT_COMPLEX && out_format != NNAB_FMT_PHASE_UNIT)
-    return NNAB_EINVAL;
-  const bool gen2 = pyr_gen2(n_octaves, h_widths, early_factor);
-  PyrStream p;
-  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, gen2, &p)) return NNAB_EUNSUPPORTED;
-  PyrPush pp;
-  int rc = pyr_push_plan(p, B, received, n_carry, frames, n, flush, pad_mode, &pp);
-  if (rc) return rc;
-  if (T != pp.t_end - frames) return NNAB_EINVAL;
-  // the whole-clip call's all-tensor-core plans need every packed operand and the tensor-core path
-  bool packed_ok = path != NNAB_PATH_SIMT && h_packed != nullptr && lowpass_packed != nullptr &&
-                   (early_factor <= 1 || early_packed != nullptr);
-  for (int i = 0; packed_ok && i < n_octaves; ++i) packed_ok = h_packed[i] != nullptr;
-  if (!packed_ok) return NNAB_EUNSUPPORTED;
-  if ((rc = check_arch())) return rc;
-  if (workspace == nullptr || ws_bytes < pp.total) return NNAB_EWORKSPACE;
-  if (B == 0) return NNAB_OK;
-  cudaStream_t s = (cudaStream_t)stream;
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  char* scratch = ws + pp.scratch;
-  const PyramidCall c{nullptr, NNAB_DTYPE_F32, B, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
-                      n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
-                      scale_all, out_format, sqrt_eps, out, T, ws, ws_bytes, s};
-  float* ring = static_cast<float*>(state);
-
-  // pass 0 checks every launch against the kernels' limits (as the whole-clip plan selection does) so that a
-  // push that cannot run returns before anything is enqueued; pass 1 runs them
-  for (int pass = 0; pass < 2; ++pass) {
-    for (int sg = 0; sg < p.n_sig; ++sg) {
-      // signal sg of this push: ring [keep, R0) then the new samples [R0, R1) (the chunk for the raw signal)
-      ChunkSource cs{};
-      cs.ring = ring + (size_t)B * p.ring_off[sg];
-      cs.ring_pitch = cs.ring_len = p.ring_len[sg];
-      cs.chunk = sg == 0 ? chunk : (const void*)(ws + pp.nbuf[sg]);
-      cs.chunk_pitch = sg == 0 ? chunk_pitch : pp.np[sg];
-      cs.received = pp.R0[sg];
-      cs.total = pp.R1[sg];
-      const int dt = sg == 0 ? chunk_dtype : NNAB_DTYPE_F32;
-      const int l = sg - p.e;
-      if (l >= 0 && T > 0) {
-        // octave l: frames [frames, t_end) from its first unreturned frame, on the whole-clip plan's kernel
-        ChunkSource co = cs;
-        co.origin = frames * p.hop[l] - p.pad[l];
-        co.length = (T - 1) * p.hop[l] + p.width[l];
-        co.pad_mode = pp.mode[l];
-        co.at_end = flush ? 1 : 0;
-        FramedProblem q = octave_problem(c, l, co.length, p.hop[l], pp.mode[l]);
-        q.pad = 0; q.x_dtype = dt; q.chunk = &co;
-        if (gen2 && p.hop[l] % 8 == 0) {
-          // gen-2 single-phase level: caller planes, the octave kernel when it takes the problem
-          int64_t pitch, plane;
-          pyr_oct_geom(p, l, B, co.length, &pitch, &plane);
-          FramedProblem qp = q;
-          qp.chunk = nullptr;
-          qp.presplit = scratch; qp.presplit_t_slots = pitch / p.hop[l]; qp.presplit_plane_stride = plane;
-          const bool oct = octave_tc_ok(qp);
-          if (pass == 0) {
-            if (!oct && !tc_supported(qp)) return NNAB_EUNSUPPORTED;
-          } else {
-            if ((rc = tc_chunk_split(co, dt, B, pitch, plane, scratch, s))) return rc;
-            if (oct) {
-              std::pair<cudaEvent_t, cudaEvent_t> pr;
-              const bool timed = prof_begin(s, &pr);
-              rc = launch_octave_tc(qp, c.packed[l], s);
-              if (timed) prof_end(s, pr);
-            } else {
-              rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
-            }
-            if (rc) return rc;
-          }
-        } else if (pass == 0) {
-          if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
-        } else if ((rc = run_framed(q, c.packed[l], scratch, pp.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
-          return rc;
-        }
-      }
-      if (sg + 1 < p.n_sig && pp.R1[sg + 1] > pp.R0[sg + 1]) {
-        // stage sg -> sg + 1 from the row holding its first new output: the rows' accumulation order is the
-        // whole clip's; only the new outputs are stored, and the edge fix runs only at the stream's true ends
-        const int d = p.d[sg];
-        const int64_t t0 = pp.R0[sg + 1] / 128;
-        const int64_t FT = (pp.R1[sg + 1] + 127) / 128 - t0;
-        ChunkSource cf = cs;
-        cf.origin = 128 * d * t0 - 128;
-        cf.pad_mode = NNAB_PAD_CONSTANT;
-        cf.at_end = 1;
-        DecimParams dec{};
-        dec.len_out = pp.R1[sg + 1] - 128 * t0;
-        dec.lo = pp.R0[sg + 1] - 128 * t0;
-        dec.y32 = (float*)(ws + pp.nbuf[sg + 1]);
-        dec.y32_pitch = pp.np[sg + 1];
-        dec.skip_edges = (t0 > 0 ? 1 : 0) | (flush ? 0 : 2);
-        const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
-        if (gen2) {
-          if (pass == 1) {
-            const int64_t pitch = 256 * (FT + 1), plane = (B * (FT + 1) + 2) * 256;
-            cf.length = pitch;
-            if ((rc = tc_chunk_split(cf, dt, B, pitch, plane, scratch, s))) return rc;
-            if ((rc = launch_fir_stage_tc(scratch, B, pp.R1[sg] - 256 * t0, pitch, plane, FIR_OFF, fir_packed,
-                                          c.lowpass, FIR_TAPS, dec, s)))
-              return rc;
-          }
-        } else {
-          FramedProblem q{};
-          q.B = B; q.x_dtype = dt; q.F = 64; q.K = tc_fir_k(FIR_TAPS, d); q.hop = 128 * d;
-          q.L = (FT - 1) * q.hop + q.K; q.pad = 0; q.pad_mode = NNAB_PAD_CONSTANT; q.scale_all = 1.f;
-          q.fmt = FMT_DECIM; q.power = 1.f; q.T = FT; q.out_bins = 64;
-          q.dec = dec;
-          cf.length = q.L;
-          q.chunk = &cf;
-          if (pass == 0) {
-            if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
-          } else if ((rc = run_framed(q, fir_packed, scratch, pp.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
-            return rc;
-          }
-        }
-      }
-      if (pass == 1 && !flush) {  // after this signal's readers: what later pushes read of it into its ring
-        const int64_t keep = pyr_keep(p, sg, pp.R1, pp.t_end);
-        if ((rc = tc_chunk_carry(cs, dt, B, keep > pp.R0[sg] ? keep : pp.R0[sg], s))) return rc;
-      }
-    }
-  }
-  return NNAB_OK;
-}
-
-int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int flush,
-                                  int n_octaves, const int32_t* widths, int hop, int early_factor, int pad_mode,
-                                  int64_t* out) {
-  if (out == nullptr) return NNAB_EINVAL;
-  PyrStream p;
-  PyrPush pp;
-  if (widths == nullptr ||
-      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
-    return NNAB_EUNSUPPORTED;
-  const int rc = pyr_push_plan(p, 1, received, n_carry, frames, n, flush, pad_mode, &pp);
-  if (rc) return rc;
-  // per signal: R before, R after, ring length, keep after (flush: R after), FIR source origin, first row
-  // (-1: no stage), then the stage's edge-fix windows of next-level outputs: head [R0', head_end) and tail
-  // [tail_begin, R1') (empty: head_end = 0, tail_begin = -1); then the frame bound
-  for (int s = 0; s < p.n_sig; ++s) {
-    int64_t* r = out + 8 * s;
-    r[0] = pp.R0[s]; r[1] = pp.R1[s]; r[2] = p.ring_len[s];
-    r[3] = flush ? pp.R1[s] : pyr_keep(p, s, pp.R1, pp.t_end);
-    const bool stage = s + 1 < p.n_sig && pp.R1[s + 1] > pp.R0[s + 1];
-    const int64_t t0 = stage ? pp.R0[s + 1] / 128 : 0;
-    r[4] = stage ? 128 * (int64_t)p.d[s] * t0 - 128 : 0;
-    r[5] = stage ? t0 : -1;
-    r[6] = (stage && p.gen2 && t0 == 0) ? (pp.R1[s + 1] < 64 ? pp.R1[s + 1] : 64) : 0;
-    r[7] = (stage && p.gen2 && flush) ? (pp.R1[s + 1] - 64 > pp.R0[s + 1] ? pp.R1[s + 1] - 64 : pp.R0[s + 1]) : -1;
-  }
-  out[8 * p.n_sig] = pp.t_end;
-  return NNAB_OK;
-}
-
 // ------------------------------------------------------------ pyramid pools ----
-// One push of a pool of pyramid streams (DESIGN §3.10 "Pyramid pools"): every lane checked by the one-stream rules
-// (pyr_step), the table as a whole, and the batch-wide geometry of each launch.  A device pool's plan has the same
-// form with its fixed geometry (pyr_device_plan).
+// One push of pyramid streams (DESIGN §3.10 "Pyramid pools"): every lane checked by the one-stream rules (pyr_step)
+// and the batch-wide geometry of each launch.  A pool's plan comes from its lane table (pyr_pool_plan), a device
+// pool's from its fixed geometry (pyr_device_plan), a lock-step push's from its one set of counters (pyr_chunk_plan).
 struct PyrPoolPlan {
   int64_t T_max;
   int64_t len_out[33];  // stage s: the most outputs one lane's FIR rows hold from their first row (0: no lane advances)
@@ -1770,6 +1541,25 @@ struct PyrPoolPlan {
   int64_t longest[33];  // the most samples one lane keeps of signal s
   size_t table, nbuf[33], scratch, scratch_bytes, total;
 };
+
+// Lane `ln` (row `lane`) of a push: its step by the one-stream rules, its descriptors held to them, and the plan's
+// T_max, len_out and longest widened to take it.  *T: the frames the lane returns.
+static int pyr_plan_lane(const PyrStream& p, const nnab_stream_lane& ln, int64_t lane, int pad_mode, PyrPoolPlan* o,
+                         int64_t* T) {
+  if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
+  PyrStep st;
+  const int rc = pyr_step(p, ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, pad_mode, &st);
+  if (rc) return rc;
+  *T = st.t_end - ln.frames;
+  if (*T > o->T_max) o->T_max = *T;
+  for (int s = 0; s < p.n_sig; ++s) {
+    const PyrLaneSig d = pyr_lane_signal(p, ln, lane, s, pad_mode);
+    if (d.R0 != st.R0[s] || d.R1 != st.R1[s] || d.count != *T) return NNAB_EINVAL;  // one set of rules
+    if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
+    if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
+  }
+  return NNAB_OK;
+}
 
 // The workspace of a push of n_lanes lanes, the A first of which return frames, from the plan's T_max, len_out:
 // the descriptor table, the new samples of every computed signal (row i: lane i's stage outputs from its first
@@ -1814,27 +1604,18 @@ static int pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int6
                          int64_t slots, int64_t n, int pad_mode, PyrPoolPlan* o) {
   if (n_lanes < 0 || n_lanes > slots || A < 0 || A > n_lanes || (n_lanes > 0 && lanes == nullptr)) return NNAB_EINVAL;
   std::vector<uint8_t> seen((size_t)slots, 0);
-  o->T_max = 0;
-  for (int s = 0; s < p.n_sig; ++s) o->len_out[s] = o->longest[s] = 0;
+  *o = PyrPoolPlan{};
   for (int64_t i = 0; i < n_lanes; ++i) {
     const nnab_stream_lane& ln = lanes[i];
     if (ln.slot < 0 || ln.slot >= slots || seen[(size_t)ln.slot]) return NNAB_EINVAL;
     if (i > 0 && i != A && ln.slot <= lanes[i - 1].slot) return NNAB_EINVAL;  // ascending within each group
     seen[(size_t)ln.slot] = 1;
     if (ln.n > n || (ln.end != 0 && ln.end != 1)) return NNAB_EINVAL;
-    PyrPush pp;
-    const int rc = pyr_push_plan(p, 1, ln.received, ln.n_carry, ln.frames, ln.n, (int)ln.end, pad_mode, &pp);
+    int64_t T;
+    const int rc = pyr_plan_lane(p, ln, i, pad_mode, o, &T);
     if (rc) return rc;
-    const int64_t T = pp.t_end - ln.frames;
     if ((i < A) != (T > 0)) return NNAB_EINVAL;               // the A lanes with frames come first
     if (T == 0 && ln.n == 0 && !ln.end) return NNAB_EINVAL;   // a lane with nothing to do
-    if (T > o->T_max) o->T_max = T;
-    for (int s = 0; s < p.n_sig; ++s) {
-      const PyrLaneSig d = pyr_lane_signal(p, ln, i, s, pad_mode);
-      if (d.R0 != pp.R0[s] || d.R1 != pp.R1[s] || d.count != T) return NNAB_EINVAL;  // one set of rules
-      if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
-      if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
-    }
   }
   pyr_pool_layout(p, n_lanes, A, o);
   return NNAB_OK;
@@ -1875,10 +1656,11 @@ static bool pyr_packed_ok(int n_octaves, const void* const* h_packed, const void
   return ok;
 }
 
-// The body of a pool push on the plan `pl`: every signal's octave (on the A rows, T_max frames each), its FIR stage
-// (on the n_lanes rows) and its carry, then the mask.  `table` holds the (signal, lane) descriptors, which the plan
-// launch(es) have written before pass 1.  Pass 0 checks every launch against the kernels' limits on the host (as
-// the chunk call does) and enqueues nothing; pass 1 runs them.
+// The body of every pyramid push (pool, device pool and lock-step) on the plan `pl`: every signal's octave (on the A
+// rows, T_max frames each), its FIR stage (on the n_lanes rows) and its carry, then the mask.  `table` holds the
+// (signal, lane) descriptors, which the plan launch(es) have written before pass 1.  Pass 0 checks every launch
+// against the kernels' limits on the host (as the whole-clip plan selection does) and enqueues nothing, so a push
+// that cannot run returns before anything is enqueued; pass 1 runs them.
 static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const PyramidCall& c, float* ring,
                         const void* chunk, int chunk_dtype, int64_t slots, int64_t chunk_pitch, int64_t n_lanes,
                         PyrLaneSig* table, char* ws, int pass) {
@@ -1940,10 +1722,8 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
       cf.rows_oct = 0;
       DecimParams dec{};
       dec.len_out = pl.len_out[sg];
-      dec.lo = 0;
       dec.y32 = (float*)(ws + pl.nbuf[sg + 1]);
       dec.y32_pitch = pl.np[sg + 1];
-      dec.skip_edges = 3;
       const void* fir_packed = (p.e && sg == 0) ? c.early_packed : c.lowpass_packed;
       if (p.gen2) {
         if (pass == 1) {
@@ -2012,8 +1792,109 @@ int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, co
                       scale_all, out_format, sqrt_eps, out, T_max, ws, ws_bytes, s};
   float* ring = static_cast<float*>(state);
   if ((rc = pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, n_lanes, table, ws, 0))) return rc;
-  if ((rc = tc_pyr_pool_plan(p, d_lanes, n_lanes, pad_mode, table, s))) return rc;
+  if ((rc = tc_pyr_pool_plan(p, d_lanes, nnab_stream_lane{}, n_lanes, pad_mode, table, s))) return rc;
   return pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, n_lanes, table, ws, 1);
+}
+
+// One lane's plan in the layout of nnab_debug_pyramid_chunk_plan, from its descriptors.
+static void pyr_debug_lane(const PyrStream& p, const nnab_stream_lane& ln, int pad_mode, int64_t* o) {
+  const int64_t t_end = ln.frames + pyr_lane_signal(p, ln, 0, 0, pad_mode).count;
+  int64_t R1[33];
+  pyr_counts(p, ln.received + ln.n, (int)ln.end, R1);
+  for (int s = 0; s < p.n_sig; ++s) {
+    const PyrLaneSig d = pyr_lane_signal(p, ln, 0, s, pad_mode);
+    const PyrLaneSig dn = s + 1 < p.n_sig ? pyr_lane_signal(p, ln, 0, s + 1, pad_mode) : d;
+    int64_t* r = o + 8 * s;
+    r[0] = d.R0; r[1] = d.R1; r[2] = p.ring_len[s];
+    r[3] = d.end ? d.R1 : pyr_keep(p, s, R1, t_end);
+    r[4] = d.t0 >= 0 ? d.fir_origin : 0;
+    r[5] = d.t0;
+    r[6] = d.head ? (dn.R1 < 64 ? dn.R1 : 64) : 0;
+    r[7] = d.tail ? (dn.R1 - 64 > dn.R0 ? dn.R1 - 64 : dn.R0) : -1;
+  }
+  o[8 * p.n_sig] = t_end;
+}
+
+// ------------------------------------------------------------ lock-step pyramid streams ----
+// A push of StreamingPyramid is a pool push of B lanes that share one set of counters, lane b in slot b (row b of
+// the chunk and of every ring): its plan is that one lane's, over B rows.
+static int pyr_chunk_plan(const PyrStream& p, int64_t B, const nnab_stream_lane& ln, int pad_mode, PyrPoolPlan* o) {
+  if (B < 0 || B > 65535) return NNAB_EINVAL;
+  *o = PyrPoolPlan{};
+  int64_t T;
+  const int rc = pyr_plan_lane(p, ln, 0, pad_mode, o, &T);
+  if (rc) return rc;
+  pyr_pool_layout(p, B, T > 0 ? B : 0, o);
+  return NNAB_OK;
+}
+
+size_t nnab_cqt_pyramid_chunk_workspace_bytes(int64_t B, int64_t received, int64_t n_carry, int64_t frames,
+                                              int64_t n, int flush, int n_octaves, const int32_t* widths,
+                                              int hop, int early_factor, int pad_mode) {
+  PyrStream p;
+  PyrPoolPlan pl;
+  if (widths == nullptr ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return 0;
+  const nnab_stream_lane ln{0, received, n_carry, frames, n, flush ? 1 : 0};
+  if (pyr_chunk_plan(p, B, ln, pad_mode, &pl)) return 0;
+  return pl.total;
+}
+
+int nnab_cqt_pyramid_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
+                                   const void* chunk, int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch,
+                                   int flush, int n_octaves, const float* const* h_k_real,
+                                   const float* const* h_k_imag, const void* const* h_packed,
+                                   const int32_t* h_widths, int n_filters, const float* lowpass,
+                                   const void* lowpass_packed, const float* early_filter, const void* early_packed,
+                                   int early_factor, int hop, int pad_mode, int n_bins, const float* scale,
+                                   float scale_all, int out_format, float sqrt_eps, float* out, int64_t T,
+                                   void* workspace, size_t ws_bytes, int path, void* stream) {
+  if (state == nullptr || !dtype_ok(chunk_dtype) || (n > 0 && chunk == nullptr) || chunk_pitch < n ||
+      (T > 0 && out == nullptr) || T < 0)
+    return NNAB_EINVAL;
+  int rc = pyr_pool_args_ok(n_octaves, h_k_real, h_k_imag, h_widths, n_filters, lowpass, early_filter, early_factor,
+                            hop, pad_mode, n_bins, out_format);
+  if (rc) return rc;
+  PyrStream p;
+  if (!pyr_stream_init(n_octaves, h_widths, hop, early_factor, pyr_gen2(n_octaves, h_widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  const nnab_stream_lane ln{0, received, n_carry, frames, n, flush ? 1 : 0};
+  PyrPoolPlan pl;
+  if ((rc = pyr_chunk_plan(p, B, ln, pad_mode, &pl))) return rc;
+  if (T != pl.T_max) return NNAB_EINVAL;
+  if (!pyr_packed_ok(n_octaves, h_packed, lowpass_packed, early_packed, early_factor, path)) return NNAB_EUNSUPPORTED;
+  if ((rc = check_arch())) return rc;
+  if (workspace == nullptr || ws_bytes < pl.total) return NNAB_EWORKSPACE;
+  if (B == 0) return NNAB_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  PyrLaneSig* table = (PyrLaneSig*)(ws + pl.table);
+  // the octaves run on every row when the push returns frames
+  const int64_t A = T > 0 ? B : 0;
+  const PyramidCall c{nullptr, NNAB_DTYPE_F32, A, 0, 0, n_octaves, h_k_real, h_k_imag, h_packed, h_widths,
+                      n_filters, lowpass, lowpass_packed, early_packed, early_factor, hop, pad_mode, n_bins, scale,
+                      scale_all, out_format, sqrt_eps, out, T, ws, ws_bytes, s};
+  float* ring = static_cast<float*>(state);
+  if ((rc = pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, B, chunk_pitch, B, table, ws, 0))) return rc;
+  if ((rc = tc_pyr_pool_plan(p, nullptr, ln, B, pad_mode, table, s))) return rc;
+  return pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, B, chunk_pitch, B, table, ws, 1);
+}
+
+int nnab_debug_pyramid_chunk_plan(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int flush,
+                                  int n_octaves, const int32_t* widths, int hop, int early_factor, int pad_mode,
+                                  int64_t* out) {
+  if (out == nullptr) return NNAB_EINVAL;
+  PyrStream p;
+  PyrPoolPlan pl;
+  if (widths == nullptr ||
+      !pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), &p))
+    return NNAB_EUNSUPPORTED;
+  const nnab_stream_lane ln{0, received, n_carry, frames, n, flush ? 1 : 0};
+  const int rc = pyr_chunk_plan(p, 1, ln, pad_mode, &pl);
+  if (rc) return rc;
+  pyr_debug_lane(p, ln, pad_mode, out);
+  return NNAB_OK;
 }
 
 // ------------------------------------------------------------ device pyramid pools ----
@@ -2031,12 +1912,8 @@ int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, co
 // ensures.  So the sweep runs pyr_step and pyr_lane_signal themselves, with and without an end, on n = chunk over
 // received in [0, start-up + P) and on every n <= chunk from received = 0.  A refused end gets the zero lane and
 // contributes nothing; a refused push without an end never happens (pyr_stream_init's ring bounds), and the sweep
-// returns NNAB_EINVAL if it did.
-struct PyrCaps {
-  int64_t T_cap, len_out[33], longest[33];
-};
-
-static int pyr_caps_sweep(const PyrStream& p, int64_t chunk, int pad_mode, PyrCaps* o) {
+// returns NNAB_EINVAL if it did.  The caps are a PyrPoolPlan's T_max, len_out and longest.
+static int pyr_caps_sweep(const PyrStream& p, int64_t chunk, int pad_mode, PyrPoolPlan* o) {
   int64_t D = 1;
   for (int s = 0; s + 1 < p.n_sig; ++s) D *= p.d[s];
   int max_w = 0;
@@ -2046,38 +1923,28 @@ static int pyr_caps_sweep(const PyrStream& p, int64_t chunk, int pad_mode, PyrCa
   const int64_t a = E * p.hop[0], b = 128 * D;
   const int64_t period = a / gcd64(a, b) * b;
   const int64_t sweep = (M + p.c) * D + period;
-  o->T_cap = 0;
-  for (int s = 0; s < 33; ++s) o->len_out[s] = o->longest[s] = 0;
+  *o = PyrPoolPlan{};
   for (int64_t k = -chunk; k < sweep; ++k) {  // k < 0: received 0, n = chunk + k
     const int64_t rec = k < 0 ? 0 : k;
     nnab_stream_lane ln{};
-    PyrStep st;
-    pyr_counts(p, rec, 0, st.R0);
+    int64_t R0[33], T;
+    pyr_counts(p, rec, 0, R0);
     ln.received = rec;
-    ln.frames = pyr_ready_frames(p, st.R0, pad_mode);
-    ln.n_carry = rec - pyr_keep(p, 0, st.R0, ln.frames);
+    ln.frames = pyr_ready_frames(p, R0, pad_mode);
+    ln.n_carry = rec - pyr_keep(p, 0, R0, ln.frames);
     ln.n = k < 0 ? chunk + k : chunk;
     for (int end = 0; end < 2; ++end) {
       ln.end = end;
-      if (pyr_step(p, ln.received, ln.n_carry, ln.frames, ln.n, end, pad_mode, &st) != NNAB_OK) {
-        if (!end) return NNAB_EINVAL;
-        continue;
-      }
-      for (int s = 0; s < p.n_sig; ++s) {
-        const PyrLaneSig d = pyr_lane_signal(p, ln, 0, s, pad_mode);
-        if (d.count > o->T_cap) o->T_cap = d.count;
-        if (d.t0 >= 0 && d.fir_len_out > o->len_out[s]) o->len_out[s] = d.fir_len_out;
-        if (d.R1 - d.keep > o->longest[s]) o->longest[s] = d.R1 - d.keep;
-      }
+      if (pyr_plan_lane(p, ln, 0, pad_mode, o, &T) != NNAB_OK && !end) return NNAB_EINVAL;
     }
   }
   return NNAB_OK;
 }
 
 // pyr_caps_sweep, computed once per geometry for the life of the process (the push checks its T_max against it).
-static int pyr_caps(const PyrStream& p, int64_t chunk, int pad_mode, PyrCaps* o) {
+static int pyr_caps(const PyrStream& p, int64_t chunk, int pad_mode, PyrPoolPlan* o) {
   static std::mutex mu;
-  static std::vector<std::pair<std::vector<int64_t>, PyrCaps>> memo;
+  static std::vector<std::pair<std::vector<int64_t>, PyrPoolPlan>> memo;
   std::vector<int64_t> key{chunk, pad_mode, p.n_oct, p.e, p.d[0], p.c, p.hop[0]};
   for (int i = 0; i < p.n_oct; ++i) key.push_back(p.width[i]);
   {
@@ -2100,14 +1967,8 @@ static int pyr_device_plan(int64_t slots, int64_t chunk, int n_octaves, const in
     return NNAB_EINVAL;
   if (!pyr_stream_init(n_octaves, widths, hop, early_factor, pyr_gen2(n_octaves, widths, early_factor), p))
     return NNAB_EUNSUPPORTED;
-  PyrCaps caps;
-  const int rc = pyr_caps(*p, chunk, pad_mode, &caps);
+  const int rc = pyr_caps(*p, chunk, pad_mode, o);
   if (rc) return rc;
-  o->T_max = caps.T_cap;
-  for (int s = 0; s < 33; ++s) {
-    o->len_out[s] = caps.len_out[s];
-    o->longest[s] = caps.longest[s];
-  }
   pyr_pool_layout(*p, slots, slots, o);
   return NNAB_OK;
 }
@@ -2172,7 +2033,7 @@ int nnab_cqt_pyramid_pool_device_forward(void* state, int64_t* counters, const i
   if ((rc = tc_device_pyramid_plan(p, slots, counters, lengths, end, errors, error_info, counts, d_lanes, n, pad_mode,
                                    s)))
     return rc;
-  if ((rc = tc_pyr_pool_plan(p, d_lanes, slots, pad_mode, table, s))) return rc;
+  if ((rc = tc_pyr_pool_plan(p, d_lanes, nnab_stream_lane{}, slots, pad_mode, table, s))) return rc;
   return pyr_pool_run(p, pl, c, ring, chunk, chunk_dtype, slots, chunk_pitch, slots, table, ws, 1);
 }
 
@@ -2202,26 +2063,7 @@ int nnab_debug_pyramid_pool_plan(const nnab_stream_lane* lanes, int64_t n_lanes,
     return NNAB_EUNSUPPORTED;
   const int rc = pyr_pool_plan(p, lanes, n_lanes, A, 65535, INT64_MAX, pad_mode, &pl);
   if (rc) return rc;
-  // per lane, the layout of nnab_debug_pyramid_chunk_plan, from the lane's descriptors
-  const int64_t stride = 8 * p.n_sig + 1;
-  for (int64_t i = 0; i < n_lanes; ++i) {
-    int64_t* o = out + i * stride;
-    const int64_t t_end = lanes[i].frames + pyr_lane_signal(p, lanes[i], i, 0, pad_mode).count;
-    int64_t R1[33];
-    pyr_counts(p, lanes[i].received + lanes[i].n, (int)lanes[i].end, R1);
-    for (int s = 0; s < p.n_sig; ++s) {
-      const PyrLaneSig d = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
-      const PyrLaneSig dn = s + 1 < p.n_sig ? pyr_lane_signal(p, lanes[i], i, s + 1, pad_mode) : d;
-      int64_t* r = o + 8 * s;
-      r[0] = d.R0; r[1] = d.R1; r[2] = p.ring_len[s];
-      r[3] = d.end ? d.R1 : pyr_keep(p, s, R1, t_end);
-      r[4] = d.t0 >= 0 ? d.fir_origin : 0;
-      r[5] = d.t0;
-      r[6] = d.head ? (dn.R1 < 64 ? dn.R1 : 64) : 0;
-      r[7] = d.tail ? (dn.R1 - 64 > dn.R0 ? dn.R1 - 64 : dn.R0) : -1;
-    }
-    o[8 * p.n_sig] = t_end;
-  }
+  for (int64_t i = 0; i < n_lanes; ++i) pyr_debug_lane(p, lanes[i], pad_mode, out + i * (8 * p.n_sig + 1));
   return NNAB_OK;
 }
 

@@ -31,7 +31,7 @@ __device__ __forceinline__ void epilogue_decim(const DecimParams& d, uint32_t tr
           uint32_t v[8];
           acc_ld8(trow + (uint32_t)c0, v);  // re half = outputs 0..half-1, im half = the rest
           const int64_t n = n0 + c0;
-          if (valid && n < d.len_out && n + 8 > d.lo) {
+          if (valid && n < d.len_out) {
             __align__(16) __nv_bfloat16 hi[8];
             __align__(16) __nv_bfloat16 lo[8];
 #pragma unroll
@@ -70,9 +70,8 @@ __device__ __forceinline__ void epilogue_decim(const DecimParams& d, uint32_t tr
               }
             }
             if (d.y32 != nullptr) {
-              float* q = d.y32 + b * d.y32_pitch + (n - d.lo);
-              for (int e = 0; e < 8 && n + e < d.len_out; ++e)
-                if (n + e >= d.lo) q[e] = __uint_as_float(v[e]);
+              float* q = d.y32 + b * d.y32_pitch + n;
+              for (int e = 0; e < 8 && n + e < d.len_out; ++e) q[e] = __uint_as_float(v[e]);
             }
           }
         }

@@ -343,15 +343,22 @@ int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int6
 
 // ---- pyramid pools (DESIGN §3.10 "Pyramid pools"): the kernels that know where each row's samples come from --
 // The (signal, lane) descriptor table of a push: one thread per entry, pyr_lane_signal of the lane's counters.
+// Without a lane table (a lock-step push) lane i is `shared` in slot i.
 __global__ void __launch_bounds__(128) pyr_pool_plan_kernel(const PyrStream p,
                                                             const nnab_stream_lane* __restrict__ lanes,
-                                                            int64_t n_lanes, int pad_mode,
-                                                            PyrLaneSig* __restrict__ table) {
+                                                            const nnab_stream_lane shared, int64_t n_lanes,
+                                                            int pad_mode, PyrLaneSig* __restrict__ table) {
   const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_lanes * p.n_sig) return;
   const int s = (int)(k / n_lanes);
   const int64_t i = k - s * n_lanes;
-  table[k] = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
+  if (lanes != nullptr) {  // two calls: one call on a selected lane copy spills a register
+    table[k] = pyr_lane_signal(p, lanes[i], i, s, pad_mode);
+    return;
+  }
+  nnab_stream_lane ln = shared;
+  ln.slot = i;
+  table[k] = pyr_lane_signal(p, ln, i, s, pad_mode);
 }
 
 // A device pyramid pool's plan launch: one thread per slot.
@@ -1680,11 +1687,12 @@ int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int
   return NNAB_OK;
 }
 
-int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, int64_t n_lanes, int pad_mode,
-                     PyrLaneSig* table, cudaStream_t stream) {
+int tc_pyr_pool_plan(const PyrStream& p, const nnab_stream_lane* lanes, const nnab_stream_lane& shared,
+                     int64_t n_lanes, int pad_mode, PyrLaneSig* table, cudaStream_t stream) {
   if (n_lanes <= 0) return NNAB_OK;
   const int64_t n = n_lanes * p.n_sig;
-  pyr_pool_plan_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, stream>>>(p, lanes, n_lanes, pad_mode, table);
+  pyr_pool_plan_kernel<<<(unsigned)ceil_div64(n, 128), 128, 0, stream>>>(p, lanes, shared, n_lanes, pad_mode,
+                                                                         table);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }

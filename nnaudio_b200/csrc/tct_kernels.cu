@@ -729,20 +729,15 @@ __global__ void __launch_bounds__(128) fir_edge_fix_kernel(
   const int64_t b = blockIdx.y;
   const int lane = threadIdx.x & 31;
   const int i = blockIdx.x * 4 + (threadIdx.x >> 5);  // 0..63: head outputs, 64..127: tail outputs
-  const bool head = !(d.skip_edges & 1);
-  if (i < 64 ? !head : (d.skip_edges & 2) != 0) return;
   const int64_t n = (i < 64) ? i : d.len_out - 128 + i;
-  if (i >= 64 && head && n < 64) return;  // short clip: the head half already covers it
-  if (n < d.lo || n >= d.len_out) return;
+  if (i >= 64 && n < 64) return;  // short clip: the head half already covers it
+  if (n < 0 || n >= d.len_out) return;
   const __nv_bfloat16* sb = src + b * src_pitch + src_off;
-  // below the launch's first sample lies the stream's zero padding, or (a push past the stream's first row)
-  // the src_off carried samples in front of it
-  const int64_t j_lo = head ? 0 : -(int64_t)src_off;
   float acc = 0.f;
 #pragma unroll 8
   for (int m = lane; m < taps; m += 32) {  // taps / 32 independent loads in flight per lane
     const int64_t j = 2 * n + m - (taps - 1) / 2;
-    const bool in = j >= j_lo && j < len_src;
+    const bool in = j >= 0 && j < len_src;
     const float hi = in ? __bfloat162float(sb[j]) : 0.f;
     const float lo = in ? __bfloat162float(sb[src_plane + j]) : 0.f;
     acc = fmaf(__ldg(fir + m), hi + lo, acc);
@@ -763,13 +758,13 @@ __global__ void __launch_bounds__(128) fir_edge_fix_kernel(
       }
     }
   }
-  if (d.y32 != nullptr) d.y32[b * d.y32_pitch + (n - d.lo)] = acc;
+  if (d.y32 != nullptr) d.y32[b * d.y32_pitch + n] = acc;
 }
 
-// fir_edge_fix_kernel of a pyramid pool's stage (rows: the stage's source descriptors, DecimParams::lo = 0, the
-// fp32 copy only): row b recomputes the stream's first 64 outputs where its first row is the stream's (head) and
-// its last 64 where its stream ends (tail), with its own source and output lengths from that row -- the sums of
-// fir_edge_fix_kernel, term for term.
+// fir_edge_fix_kernel of a streamed pyramid push's stage (rows: the stage's source descriptors, the fp32 copy only):
+// row b recomputes the stream's first 64 outputs where its first row is the stream's (head) and its last 64 where its
+// stream ends (tail), with its own source and output lengths from that row -- the sums of fir_edge_fix_kernel, term
+// for term.
 __global__ void __launch_bounds__(128) fir_edge_fix_rows_kernel(
     const __nv_bfloat16* __restrict__ src, int64_t src_pitch, int64_t src_plane, int src_off,
     const float* __restrict__ fir, int taps, DecimParams d, const PyrLaneSig* __restrict__ rows) {
@@ -808,7 +803,7 @@ int launch_fir_stage_tc(const void* src_planes, int64_t B, int64_t src_len, int6
                         const float* fir, int taps, const DecimParams& dec, cudaStream_t stream,
                         const PyrLaneSig* lane_rows) {
   if (taps != 256 || src_pad != 128) return NNAB_EUNSUPPORTED;  // frame origin = row origin
-  if (lane_rows != nullptr && (dec.y32 == nullptr || dec.pc != nullptr || dec.lo != 0)) return NNAB_EUNSUPPORTED;
+  if (lane_rows != nullptr && (dec.y32 == nullptr || dec.pc != nullptr)) return NNAB_EUNSUPPORTED;
   if (src_pitch % 256 != 0 || B > 65535 || dec.pf != nullptr) return NNAB_EUNSUPPORTED;
   const int64_t FT = (dec.len_out + 127) / 128;
   const int64_t t_slots = src_pitch / 256;

@@ -233,3 +233,28 @@ def test_pool_plan_equals_one_stream_plan(name, monkeypatch):
             checked += 1
         pool.reset(np.flatnonzero(end))
     assert checked > 40
+
+
+@pytest.mark.parametrize("name", sorted(REPLAY))
+def test_lock_step_workspace_equals_pool_of_its_lanes(name, monkeypatch):
+    """A StreamingPyramid push of B streams is a pool push of B lanes with its counters in slots 0 .. B-1: over
+    seeded push sequences ending in a flush, the chunk call's workspace query equals the pool's for that table."""
+    _install(monkeypatch)
+    st = StreamingPyramid(REPLAY[name](), 1)
+    widths, hop, early, pm = st.widths, st.hop, st.early, _C.PAD_REFLECT
+    w = (ctypes.c_int32 * len(widths))(*widths)
+    rng = np.random.default_rng(9)
+    for B in (1, 3):
+        received = n_carry = frames = 0
+        for step in range(30):
+            n, flush = int(rng.integers(1, 3000)), int(step == 29)
+            _, t_end = _C.cqt_pyramid_chunk_plan(received, n_carry, frames, n, flush, widths, hop, pm, early)
+            T = t_end - frames
+            lanes = [[b, received, n_carry, frames, n, flush] for b in range(B)]
+            want = _C.cqt_pyramid_pool_workspace_bytes(lanes, B if T > 0 else 0, T, widths, hop, early, pm)
+            got = _C.lib().nnab_cqt_pyramid_chunk_workspace_bytes(B, received, n_carry, frames, n, flush,
+                                                                   len(widths), w, hop, early, pm)
+            assert want > 0 and got == want, (name, B, step)
+            received += n
+            frames = t_end
+            n_carry = st._n_carry(received, frames)
