@@ -354,6 +354,18 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
                                 int pad_mode, float* dw, void* workspace, size_t ws_bytes,
                                 void* stream);
 
+/* The inverse STFT and both gradients above run one overlap-add GEMM of M_rows rows x F_out output samples
+ * over K_gemm (rounded up to 64):
+ *   nnab_framed_backward_input   M_rows = B*T, F_out = K,     K_gemm = 2F
+ *   nnab_istft_forward           M_rows = B*T, F_out = n_fft, K_gemm = 2 f_in
+ *   nnab_framed_backward_weight  M_rows = 2F,  F_out = K,     K_gemm = B*T rounded up to 64
+ * K is cut into chunks of at most 4096 products per fp32 accumulator, at most k_splits_hint of them (64 for the
+ * three calls): min(ceil(K_gemm / 4096), 64); the overlap-add atomics sum the chunks.  F_out is limited to 32768
+ * (128 N tiles of 256 samples); above it the three calls return NNAB_EUNSUPPORTED before anything is enqueued.
+ * Host only (tests): out[0..4] = supported (0 / 1), N tile width, N tiles, K chunks the launch uses, MMA flops it
+ * executes (bf16 split terms and tile padding included). */
+int nnab_debug_ola_plan(int F_out, int K_gemm, int64_t M_rows, int k_splits_hint, double* out);
+
 /* ------------------------------------------------------------------------- *
  * Chunked streams: B streams that advance together, one push per chunk (DESIGN.md §3.10).
  * Each *_chunk_forward takes the arguments of the matching *_forward_ex with (x, L, x_pitch) replaced by

@@ -106,6 +106,7 @@ SIGNATURES = {
     "nnab_packed_block_bytes": (c_size_t, [c_int, c_int]),
     "nnab_pack_basis_block": (c_int, [c_int, c_int, _P, _P]),
     "nnab_debug_varn_plan": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    "nnab_debug_ola_plan": (c_int, [c_int, c_int, c_int64, c_int, _P]),
     "nnab_fir_decimate": (c_int, [_P, c_int64, c_int64, c_int64, _P, c_int, c_int, _P, c_int64, _P]),
     "nnab_fir_decimate_adjoint": (
         c_int, [_P, c_int64, c_int64, c_int64, _P, c_int, c_int, _P, c_int64, _P]),
@@ -1057,6 +1058,29 @@ def debug_device_pyramid_plan(counters, lengths, end, errors, error_info, n, wid
     return lanes, counts
 
 
+# The overlap-add GEMM of the inverse STFT and of both gradients takes frames of at most this many output samples
+# (n_fft of the inverse, kernel width of the gradients): 128 N tiles of 256.
+OLA_MAX_WIDTH = 32768
+
+
+def ola_plan(F_out: int, K_gemm: int, M_rows: int, k_splits_hint: int = 0) -> dict:
+    """Host-only launch shape of the overlap-add GEMM (``nnab_debug_ola_plan``; the operands of each caller are
+    listed in include/nnab.h)."""
+    out = (ctypes.c_double * 5)()
+    _check(lib().nnab_debug_ola_plan(int(F_out), int(K_gemm), int(M_rows), int(k_splits_hint), out),
+           "nnab_debug_ola_plan")
+    return dict(supported=bool(out[0]), bn=int(out[1]), n_tiles=int(out[2]), k_splits=int(out[3]),
+                exec_flops=float(out[4]))
+
+
+def _check_ola(rc: int, what: str, width: int, name: str):
+    """``_check`` for the overlap-add GEMM's callers: a frame wider than the GEMM takes is named as such."""
+    if rc == EUNSUPPORTED and width > OLA_MAX_WIDTH:
+        raise RuntimeError(f"{what} failed: {name} {width} is above the overlap-add GEMM's limit of "
+                           f"{OLA_MAX_WIDTH} samples (status {rc})")
+    _check(rc, what)
+
+
 def pack_istft_basis(kernel_cos: torch.Tensor, kernel_sin: torch.Tensor, f_in: int, onesided: bool):
     """Tensor-core packing of the (n_fft, n_fft) inverse kernels; the mirroring of a
     one-sided spectrum (utils.py:63-70) is folded into the packed rows."""
@@ -1088,7 +1112,7 @@ def istft_forward(X, packed, window, n_fft, hop, center, length):
         rc = L.nnab_istft_forward(_ptr(X), B, f_in, T, _ptr(packed), _ptr(window), n_fft, hop,
                                   int(center), -1 if length is None else int(length), _ptr(out),
                                   want, _ptr(ws), wsb, _stream(X.device))
-    _check(rc, "nnab_istft_forward")
+    _check_ola(rc, "nnab_istft_forward", n_fft, "n_fft")
     return out
 
 
@@ -1144,7 +1168,7 @@ def framed_backward_input(g, packed_adj, K, hop, center, pad_mode, L_in):
         rc = L.nnab_framed_backward_input(_ptr(g), B, F, T, _ptr(packed_adj), K, hop, int(center),
                                           pad_mode, _ptr(dx), L_in, _ptr(ws), wsb,
                                           _stream(g.device))
-    _check(rc, "nnab_framed_backward_input")
+    _check_ola(rc, "nnab_framed_backward_input", K, "kernel width")
     return dx
 
 
@@ -1162,5 +1186,5 @@ def framed_backward_weight(g, x, K, hop, center, pad_mode):
         rc = L.nnab_framed_backward_weight(_ptr(g), _ptr(x), B, Ln, pitch, F, T, K, hop,
                                            int(center), pad_mode, _ptr(dw), _ptr(ws), wsb,
                                            _stream(g.device))
-    _check(rc, "nnab_framed_backward_weight")
+    _check_ola(rc, "nnab_framed_backward_weight", K, "kernel width")
     return dw[:F], -dw[F:]

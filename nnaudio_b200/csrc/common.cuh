@@ -665,6 +665,15 @@ int tc_pad_split2(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pi
 // inverse STFT pieces (tc_kernels.cu)
 int tc_istft_k(int f_in);
 int tc_istft_bn(int n_fft);
+// Launch shape of the FMT_OLA GEMM (the inverse STFT and both gradients): M_rows frames (rows) x F_out output
+// samples in n_tiles tiles of bn, K_gemm rounded up to 64 and cut into k_splits chunks of at most 64 k-blocks (at
+// most k_splits_hint of them), exec_flops the MMA flops of the launch.  tc_supported and launch_framed_tc both read it.
+struct OlaPlan {
+  int supported, bn, n_tiles, k_splits;
+  double exec_flops;
+};
+OlaPlan tc_ola_plan(int F_out, int K_gemm, int64_t M_rows, int k_splits_hint);
+constexpr int TC_OLA_MAX_SPLITS = 64;  // the K chunks the offline callers allow
 size_t tc_packed_istft_bytes(int n_fft, int f_in);
 int tc_pack_istft(const float* kc, const float* ks, int n_fft, int f_in, int onesided, void* packed,
                   cudaStream_t stream, int transposed = 0);

@@ -1038,6 +1038,17 @@ int nnab_debug_varn_plan(const int32_t* h_k_begin, const int32_t* h_k_end, int n
                              chunk_begin, n_blocks, n_chunks);
 }
 
+int nnab_debug_ola_plan(int F_out, int K_gemm, int64_t M_rows, int k_splits_hint, double* out) {
+  if (out == nullptr || F_out <= 0 || K_gemm <= 0 || M_rows < 0) return NNAB_EINVAL;
+  const OlaPlan o = tc_ola_plan(F_out, K_gemm, M_rows, k_splits_hint);
+  out[0] = o.supported;
+  out[1] = o.bn;
+  out[2] = o.n_tiles;
+  out[3] = o.k_splits;
+  out[4] = o.exec_flops;
+  return NNAB_OK;
+}
+
 int nnab_fir_decimate(const float* x, int64_t B, int64_t L, int64_t x_pitch, const float* fir,
                       int taps, int factor, float* y, int64_t Ly, void* stream) {
   if (x == nullptr || fir == nullptr || y == nullptr || B < 0 || L <= 0 || x_pitch < L || taps <= 0 ||
@@ -2103,6 +2114,7 @@ int nnab_istft_forward(const float* X, int64_t B, int f_in, int64_t T, const voi
   if (X == nullptr || packed == nullptr || window == nullptr || out == nullptr || B < 0 ||
       f_in <= 0 || T <= 0 || n_fft <= 0 || hop <= 0)
     return NNAB_EINVAL;
+  if (!tc_ola_plan(n_fft, tc_istft_k(f_in), B * T, TC_OLA_MAX_SPLITS).supported) return NNAB_EUNSUPPORTED;
   int rc = check_arch();
   if (rc) return rc;
   const size_t need = nnab_istft_workspace_bytes(B, f_in, T, n_fft, hop);
@@ -2138,6 +2150,7 @@ int nnab_istft_forward(const float* X, int64_t B, int f_in, int64_t T, const voi
   p.out = ola; p.T = T; p.out_bins = n_fft; p.bin_offset = 0;
   p.presplit = planes;
   p.ola_pitch = ola_pitch; p.ola_hop = hop;
+  p.k_splits_hint = TC_OLA_MAX_SPLITS;
   if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
   return tc_istft_finalize(ola, ola_pitch, B, window, n_fft, hop, T, offset, out, want, s);
 }
@@ -2391,6 +2404,7 @@ int nnab_framed_backward_input(const float* g, int64_t B, int F, int64_t T, cons
     return NNAB_EINVAL;
   const int pad = center ? K / 2 : 0;
   if (T != frames_of(L, K, hop, pad) || T <= 0) return NNAB_EINVAL;
+  if (!tc_ola_plan(K, tc_istft_k(F), B * T, TC_OLA_MAX_SPLITS).supported) return NNAB_EUNSUPPORTED;
   int rc = check_arch();
   if (rc) return rc;
   const size_t need = nnab_framed_backward_input_workspace_bytes(B, L, K, F, hop, center);
@@ -2414,6 +2428,7 @@ int nnab_framed_backward_input(const float* g, int64_t B, int F, int64_t T, cons
   p.out = gp; p.T = T; p.out_bins = K; p.bin_offset = 0;
   p.presplit = planes;
   p.ola_pitch = pitch; p.ola_hop = hop;
+  p.k_splits_hint = TC_OLA_MAX_SPLITS;
   if ((rc = run_framed(p, packed_adj, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
   return tc_unpad_adjoint(gp, pitch, gp_len, B, pad, pad_mode, L, dx, s);
 }
@@ -2435,6 +2450,9 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
     return NNAB_EINVAL;
   const int pad = center ? K / 2 : 0;
   if (T != frames_of(L, K, hop, pad) || T <= 0) return NNAB_EINVAL;
+  const int64_t gpad = tc_dw_gpad(B, T);
+  if (gpad >= (1ll << 31)) return NNAB_EUNSUPPORTED;
+  if (!tc_ola_plan(K, (int)gpad, 2 * (int64_t)F, TC_OLA_MAX_SPLITS).supported) return NNAB_EUNSUPPORTED;
   int rc = check_arch();
   if (rc) return rc;
   const size_t need = nnab_framed_backward_weight_workspace_bytes(B, L, K, F, hop, center);
@@ -2443,8 +2461,6 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
   char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   void* gplanes = ws;
   void* frames = ws + align_up(tc_dw_grad_planes_bytes(B, T, F), 256);
-  const int64_t gpad = tc_dw_gpad(B, T);
-  if (gpad >= (1ll << 31)) return NNAB_EUNSUPPORTED;
 
   if ((rc = tc_dw_prep_grad(g, B, F, T, gplanes, s))) return rc;
   if ((rc = tc_dw_prep_frames(x, B, L, x_pitch, K, hop, pad, pad_mode, T, frames, s))) return rc;
@@ -2457,8 +2473,7 @@ int nnab_framed_backward_weight(const float* g, const float* x, int64_t B, int64
   p.out = dw; p.T = 2 * F; p.out_bins = K; p.bin_offset = 0;
   p.presplit = gplanes;
   p.ola_pitch = 0; p.ola_hop = K;        // row m of dW starts at m * K
-  p.k_splits_hint = (int)((gpad / 64 + 63) / 64);  // <= 64 k-blocks per accumulator chunk
-  if (p.k_splits_hint > 64) p.k_splits_hint = 64;
+  p.k_splits_hint = TC_OLA_MAX_SPLITS;  // <= 64 k-blocks per accumulator chunk
   return run_framed(p, frames, nullptr, 0, NNAB_PATH_TCGEN05, s);
 }
 

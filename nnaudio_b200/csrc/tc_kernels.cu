@@ -87,12 +87,34 @@ size_t tc_workspace_bytes(int64_t B, int64_t L, int K, int hop, int pad) {
   return (size_t)(2 * g.plane_stride) * sizeof(__nv_bfloat16) + 256;
 }
 
+int tc_istft_bn(int n_fft) { return n_fft >= 256 ? 256 : (round_up_i(n_fft, 16) < 32 ? 32 : round_up_i(n_fft, 16)); }
+
+// The FMT_OLA GEMM's N axis is the frame's F_out output samples in tc_istft_bn(F_out)-wide tiles, each with
+// its own kb_begin / kb_end entry (so F_out <= TC_MAX_N_TILES x 256 = 32768).  Its callers pass no per-bin tap
+// support, so every tile runs all round_up(K_gemm, 64) / 64 k-blocks.  Those are cut into chunks of at most 64
+// k-blocks (4096 products per fp32 accumulator, as the dense kernel's split-K does), at most k_splits_hint of them;
+// the overlap-add atomics sum the chunks.  A 24576-sample frame summed in one accumulator is 1e-4 off.
+OlaPlan tc_ola_plan(int F_out, int K_gemm, int64_t M_rows, int k_splits_hint) {
+  OlaPlan o{};
+  if (F_out <= 0 || K_gemm <= 0 || M_rows < 0) return o;
+  o.bn = tc_istft_bn(F_out);
+  o.n_tiles = (F_out + o.bn - 1) / o.bn;
+  o.supported = o.n_tiles <= TC_MAX_N_TILES;
+  const int kpad = round_up_i(K_gemm, 64);
+  const int nkb = kpad / 64;
+  const int ks = (nkb + 63) / 64;  // <= nkb
+  o.k_splits = ks < k_splits_hint ? ks : (k_splits_hint > 1 ? k_splits_hint : 1);
+  o.exec_flops = 3.0 * 2.0 * (double)ceil_div64(M_rows, TC_BM) * TC_BM * ((double)o.n_tiles * o.bn) * kpad;
+  return o;
+}
+
 bool tc_supported(const FramedProblem& p, const void* packed) {
   if (p.hop <= 0 || p.K < 16) return false;
   // (pre-split planes are laid out by the caller, which guarantees >= 1 valid frame)
   if (p.presplit == nullptr && p.L + 2 * (int64_t)p.pad < p.K) return false;
   const SplitGeom g = split_geom(p.B > 0 ? p.B : 1, p.L, p.K, p.hop, p.pad);
   if (g.rows >= (1ll << 31) || g.plane_stride >= (1ll << 38)) return false;
+  if (p.fmt == FMT_OLA) return tc_ola_plan(p.F, p.K, g.nv, p.k_splits_hint).supported;
   // a block-partial basis runs on framed_tcb_kernel, whose nb-wide N tiles tc_block_shape_ok bounds (35 at
   // n_fft = 32768); the dense kernel's N-tile limit below would send n_fft = 24576 and 32768 to the SIMT kernel
   if (packed != nullptr && packed_kind(packed) == PACK_BLOCK) return tc_block_shape_ok(p.K, p.hop);
@@ -707,7 +729,6 @@ int tc_zero_slots(void* planes_v, int64_t B, int64_t clip_pitch, int64_t plane_s
 // row-major matrix.  The FMT_OLA epilogue windows the frame and overlap-adds it.
 // ---------------------------------------------------------------------------
 int tc_istft_k(int f_in) { return round_up_i(2 * f_in, 64); }
-int tc_istft_bn(int n_fft) { return n_fft >= 256 ? 256 : (round_up_i(n_fft, 16) < 32 ? 32 : round_up_i(n_fft, 16)); }
 size_t tc_packed_istft_bytes(int n_fft, int f_in) {
   const int bn = tc_istft_bn(n_fft);
   const size_t rows = (size_t)((n_fft + bn - 1) / bn) * bn;
@@ -2128,8 +2149,13 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   const int n_ph = s.n_ph;
   const int kpad = round_up_i(q.K, 64);
   // FMT_OLA: the N axis is the frame's n_fft output samples (q.F), not (re | im) bin pairs
-  const int bn = (q.fmt == FMT_OLA) ? tc_istft_bn(q.F) : choose_bn(q.F);
-  const int n_tiles = (q.fmt == FMT_OLA) ? (q.F + bn - 1) / bn : (2 * q.F + bn - 1) / bn;
+  OlaPlan ola{};
+  if (q.fmt == FMT_OLA) {
+    ola = tc_ola_plan(q.F, q.K, s.g.nv, q.k_splits_hint);
+    if (!ola.supported || q.h_k_begin != nullptr) return NNAB_EINVAL;
+  }
+  const int bn = (q.fmt == FMT_OLA) ? ola.bn : choose_bn(q.F);
+  const int n_tiles = (q.fmt == FMT_OLA) ? ola.n_tiles : (2 * q.F + bn - 1) / bn;
   const int rows_w = n_tiles * bn;
   CUtensorMap mb;
   rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)kpad, (uint64_t)rows_w, 2,
@@ -2174,15 +2200,7 @@ int launch_framed_tc(const FramedProblem& q, const void* packed, void* workspace
   if (q.fmt == FMT_FBANK && (q.fb_table == nullptr || q.n_fb <= 0)) return NNAB_EINVAL;
   if (q.fmt == FMT_DECIM && (bn != 128 || n_tiles != 1)) return NNAB_EINVAL;
 
-  if (q.fmt == FMT_OLA && q.k_splits_hint > 1) {  // the OLA atomics accumulate K chunks as is
-    int min_range = nkb;
-    for (int tl = 0; tl < n_tiles; ++tl) {
-      const int r = prm.kb_end[tl] - prm.kb_begin[tl];
-      min_range = r < min_range ? r : min_range;
-    }
-    prm.k_splits = q.k_splits_hint < min_range ? q.k_splits_hint : min_range;
-    if (prm.k_splits < 1) prm.k_splits = 1;
-  }
+  if (q.fmt == FMT_OLA) prm.k_splits = ola.k_splits;  // the OLA atomics accumulate K chunks as is
 
   // ---- split-K (long kernels, caller supplied the raw scratch) ---------------------------
   EpiParams final_epi = prm.epi;
