@@ -382,6 +382,10 @@ int nnab_debug_ola_plan(int F_out, int K_gemm, int64_t M_rows, int k_splits_hint
  * those the offline call gives for the whole stream, bit for bit on the tensor-core plans.  After the call
  * the caller advances its counters: received += n, frames += T,
  * n_carry = received - max(0, min(frames*hop - pad, pad > 0 ? received - pad - 1 : received)).
+ * A push is the pool push (*_pool_forward below) of B lanes that share these counters, lane b in slot b: the
+ * launches of the offline call on (B, (T - 1) * hop + K samples) when T > 0, then one carry launch (every row
+ * returns T frames, so there is no mask launch).  The workspace queries equal *_pool_workspace_bytes(T > 0 ? B : 0,
+ * T, ...) for the T this push returns.
  * Plans that read x as fp32 directly (SIMT) return NNAB_EUNSUPPORTED before anything is enqueued.
  * The MFCC call takes top_db < 0 (None) only: the floor is a maximum over the whole clip.
  * ------------------------------------------------------------------------- */
@@ -558,7 +562,10 @@ int nnab_debug_pyramid_pool_plan(const nnab_stream_lane* lanes, int64_t n_lanes,
  * with the offline length / centre rules.  out_len must be that count; NNAB_EINVAL for counters no stream has
  * or a length shorter than the samples already returned.  Each sample is divided by the window sum-square of
  * its global position.  The concatenation equals nnab_istft_forward on all frames to fp32 rounding (both
- * overlap-add with fp32 atomics). */
+ * overlap-add with fp32 atomics).  A push is the pool push (nnab_istft_pool_forward below) of B lanes that share
+ * these counters, lane b in slot b with X row b: one seed launch, the FMT_OLA pre-pass and GEMM over B x T frames
+ * (when T > 0) and one finalize launch.  The workspace query equals nnab_istft_pool_workspace_bytes(B, f_in, T,
+ * n_fft, hop), so it includes the overlap-add rows' lead of n_fft positions. */
 size_t nnab_istft_chunk_workspace_bytes(int64_t B, int f_in, int64_t T, int n_fft, int hop);
 int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const float* X, int64_t B, int f_in,
                              int64_t T, const void* packed, const float* window, int n_fft, int hop, int center,

@@ -121,15 +121,15 @@ __host__ __device__ inline int poly4_range(int k, int M, int nb) {
   return f * 4096 + kq / (nb - 2);
 }
 
-// The signal of one push of a chunked stream (DESIGN §3.10): the "virtual clip" of `length` samples whose
-// sample i is raw stream sample r = origin + i.  Raw samples [.., received) come from the fp32 carry ring
-// (raw r of stream b at ring[b * ring_pitch + r % ring_len]), [received, total) from the chunk (samples of
-// type FramedProblem::x_dtype, rows of chunk_pitch).  r < 0 is the left centre padding; on the last push
-// (at_end) r >= total is the right one.
-// A stream pool's push (lanes != nullptr) gives every batch row b its own stream: lane b of the DEVICE lane
-// table names its ring row and chunk row (`slot`), its counters and its end; origin = frames * hop - pad and
-// received / total / at_end come from the lane, and the fields of the same name above are unused.  The clip
-// length is the batch's longest; a row's samples past its own stream read as zeros.
+// The signals of one push of chunked streams (DESIGN §3.10): batch row b is the "virtual clip" of `length`
+// samples of one stream, lane b of the push.  The lane names the stream's ring row and chunk row (`slot`), its
+// counters and its end; the clip's sample i is the stream's raw sample r = frames * hop - pad + i.  Raw samples
+// [.., received) come from the fp32 carry ring (raw r of slot s at ring[s * ring_pitch + r % ring_len]),
+// [received, received + n) from the chunk (samples of type FramedProblem::x_dtype, rows of chunk_pitch).
+// r < 0 is the left centre padding; on the stream's last push (end) r >= received + n is the right one.  The
+// clip length is the batch's longest; a row's samples past its own stream read as zeros.
+// Lane b is lanes[b] of the DEVICE lane table (stream pools), or without one (a lock-step push of B streams
+// that share one set of counters) `shared` in slot b.
 struct PyrLaneSig;
 struct ChunkSource {
   const float* ring;
@@ -137,11 +137,11 @@ struct ChunkSource {
   int64_t ring_len;
   const void* chunk;
   int64_t chunk_pitch;
-  int64_t received, total, origin, length;
+  int64_t length;
   int pad_mode;
-  int at_end;
-  const nnab_stream_lane* lanes;  // pools only, else nullptr
-  int K, hop, pad;                // pools only: the framing that places each lane's clip
+  const nnab_stream_lane* lanes;
+  nnab_stream_lane shared;        // lane b when lanes == nullptr (slot = b)
+  int K, hop, pad;                // the framing that places each lane's clip
   // pyramid pools (rows != nullptr, lanes == nullptr): row b of the launch takes everything from the DEVICE
   // descriptor rows[b] (PyrLaneSig below): its ring row, its source row and base, its counts, and -- rows_oct = 1,
   // an octave clip (pad: the octave's) -- the octave's frame origin, padding and end, or -- rows_oct = 0, a FIR
@@ -186,8 +186,9 @@ struct StreamStep {
 
 // One push of one stream: n new samples, the last push iff `end`.  NNAB_EINVAL for counters no stream can
 // have (they must be those of a stream that returned every ready frame) and for an end the stream is too
-// short for (reflect padding needs pad < total; at least one frame).  The streams of *_chunk_forward, every
-// lane of a pool and every slot of a device pool's plan launch are checked here.
+// short for (reflect padding needs pad < total; at least one frame).  Every lane of a push is checked here: the
+// one lane the B streams of *_chunk_forward share, each lane of a pool's table and every slot of a device pool's
+// plan launch.
 __host__ __device__ inline int stream_step(int64_t received, int64_t n_carry, int64_t frames, int64_t n, int end,
                                            int K, int hop, int pad, int pad_mode, StreamStep* o) {
   if (received < 0 || frames < 0 || n < 0) return NNAB_EINVAL;
@@ -625,13 +626,13 @@ int tc_pad_split_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_
 constexpr int TC_SPLIT_PLAIN = 0;
 constexpr int TC_SPLIT_POLY4 = 1;
 int tc_problem_split(const FramedProblem& q, void* planes, cudaStream_t stream, int layout);
-// planes of the virtual clip cs (clip_pitch samples per clip from its first sample) in a caller geometry
+// planes of the B virtual clips of cs, row b that of lane b (clip_pitch samples per clip from its first sample),
+// in a caller geometry
 int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_pitch, int64_t plane_stride,
                    void* planes, cudaStream_t stream);
-// store raw samples [from, total) of the chunk into the carry ring (cs.received = raw index of chunk[0])
-int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream);
-// pools (cs.lanes): the carry of every one of the n_lanes lanes, each its own [from, total) (at most
-// `longest` samples), and the zeroing of output frames t >= the count of row i of out (A, rows, T, cols)
+// the carry of every one of the n_lanes lanes of cs (lanes[i], or `shared` in slot i): each stores its own raw
+// samples [from, received + n) of the chunk into its ring row (at most `longest` samples); and for a lane table,
+// the zeroing of output frames t >= the count of row i of out (A, rows, T, cols)
 int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream);
 int tc_pool_mask(const ChunkSource& cs, int64_t A, float* out, int64_t rows, int64_t T, int cols,
                  cudaStream_t stream);
@@ -691,21 +692,20 @@ int tc_istft_prep(const float* X, int64_t B, int f_in, int64_t T, void* planes, 
 int tc_istft_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window,
                       int n_fft, int hop, int64_t T, int64_t offset, float* out, int64_t out_len,
                       cudaStream_t stream);
-int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window, int n_fft,
-                            int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
-                            int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream);
-// inverse STFT pools (DEVICE lane table `lanes`): row i of the (n_lanes, ola_pitch) overlap-add buffer holds
-// lane i's positions from frames_i * hop - lead.  Seed: every row's carried sums from its state row, zeros
-// elsewhere.  Prep: plane row i * T_max + t from X[row_i, :, t] of the (R, f_in, x_T, 2) frames for t < T_i, zeros
-// past T_i and for row_i = -1.  Finalize: rows i < A of out (A, n_max) get lane i's final samples then zeros;
-// every lane's open tail goes to its state row.
-int tc_istft_pool_seed(const nnab_istft_lane* lanes, int64_t n_lanes, const float* state, int n_fft, int hop,
-                       int center, int64_t lead, float* ola, int64_t ola_pitch, cudaStream_t stream);
+// inverse STFT pools: lane i is lanes[i] of the DEVICE lane table or, without one (a lock-step push), `shared` in
+// slot i.  Row i of the (n_lanes, ola_pitch) overlap-add buffer holds lane i's positions from frames_i * hop - lead.
+// Seed: every row's carried sums from its state row, zeros elsewhere.  Prep: plane row i * T_max + t from
+// X[row_i, :, t] of the (R, f_in, x_T, 2) frames for t < T_i, zeros past T_i and for row_i = -1 (without a lane
+// table, X is (n_lanes, f_in, T_max, 2)).  Finalize: rows i < A of out (A, n_max) get lane i's final samples then
+// zeros; every lane's open tail goes to its state row.
+int tc_istft_pool_seed(const nnab_istft_lane* lanes, const nnab_istft_lane& shared, int64_t n_lanes,
+                       const float* state, int n_fft, int hop, int center, int64_t lead, float* ola, int64_t ola_pitch,
+                       cudaStream_t stream);
 int tc_istft_pool_prep(const float* X, const nnab_istft_lane* lanes, int64_t n_lanes, int f_in, int64_t T_max,
                        int64_t x_T, void* planes, cudaStream_t stream);
-int tc_istft_pool_finalize(const nnab_istft_lane* lanes, int64_t n_lanes, int64_t A, const float* ola,
-                           int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop, int center,
-                           float* out, int64_t n_max, float* state, cudaStream_t stream);
+int tc_istft_pool_finalize(const nnab_istft_lane* lanes, const nnab_istft_lane& shared, int64_t n_lanes, int64_t A,
+                           const float* ola, int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop,
+                           int center, float* out, int64_t n_max, float* state, cudaStream_t stream);
 size_t tc_splitk_scratch_bytes(int64_t B, int F, int64_t T, int K);
 // block-partial kernel (tcb_kernels.cu): default N-tile geometry of an (n_fft, hop) transform (nb packed
 // columns per tile, nb - 2 new bins each, `phases` families per tile: 1, or 4 when hop % 128 == 0) -- the column

@@ -155,17 +155,37 @@ static void set_wave(FramedProblem& p, const Wave& w) {
   p.pad = w.pad; p.pad_mode = w.pad_mode; p.chunk = w.chunk;
 }
 
-// ---- chunked streams (DESIGN §3.10) ------------------------------------------------------------
-// The counters of a stream and one push's step on them: StreamStep / stream_step in common.cuh.
-struct ChunkPlan {
-  ChunkSource cs;
-  int64_t T;          // frames this push returns
-  int64_t from;       // raw samples [from, total) go into the ring after the push
+// ---- chunked streams and stream pools (DESIGN §3.10) ----------------------------------------------------
+// A push of lanes, each one stream (counters: StreamStep / stream_step in common.cuh).  A pool's lanes come from
+// its device lane table; a lock-step push of B streams is the push of B lanes that share one set of counters.
+struct PoolPlan {
+  ChunkSource cs;     // lanes = the device table, or nullptr and `shared`; length = the clip of T_max frames
+  int64_t A, T_max;
+  int64_t longest;    // the most samples one lane stores into the ring
 };
 
-static int chunk_plan(const void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
-                      int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush, int K, int hop,
-                      int pad, int pad_mode, ChunkPlan* o) {
+// The source of a push's clips of `length` samples: ring rows of K floats, chunk rows of chunk_pitch samples.
+static ChunkSource chunk_source(const void* state, const void* chunk, int64_t chunk_pitch, int K, int hop, int pad,
+                                int pad_mode, int64_t length, const nnab_stream_lane* lanes,
+                                const nnab_stream_lane& shared) {
+  ChunkSource c{};
+  c.ring = static_cast<const float*>(state);
+  c.ring_pitch = K;
+  c.ring_len = K;
+  c.chunk = chunk;
+  c.chunk_pitch = chunk_pitch;
+  c.length = length;
+  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
+  c.lanes = lanes;
+  c.shared = shared;
+  c.K = K; c.hop = hop; c.pad = pad;
+  return c;
+}
+
+// A lock-step push: B streams with these counters, lane b in slot b; T_max is the frames it returns.
+static int lock_step_plan(const void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
+                          int chunk_dtype, int64_t B, int64_t n, int64_t chunk_pitch, int flush, int K, int hop,
+                          int pad, int pad_mode, PoolPlan* o) {
   if (state == nullptr || !dtype_ok(chunk_dtype) || B < 0 || B > 65535 || n < 0 || (n > 0 && chunk == nullptr) ||
       chunk_pitch < n || K < 2 || hop <= 0)
     return NNAB_EINVAL;
@@ -173,30 +193,14 @@ static int chunk_plan(const void* state, int64_t received, int64_t n_carry, int6
   StreamStep st;
   const int rc = stream_step(received, n_carry, frames, n, flush, K, hop, pad, pad_mode, &st);
   if (rc) return rc;
-  ChunkSource& c = o->cs;
-  c = ChunkSource{};
-  c.ring = static_cast<const float*>(state);
-  c.ring_pitch = K;
-  c.ring_len = K;
-  c.chunk = chunk;
-  c.chunk_pitch = chunk_pitch;
-  c.received = received;
-  c.total = st.total;
-  c.origin = frames * hop - pad;
-  c.length = st.T > 0 ? (st.T - 1) * hop + K : 0;
-  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
-  c.at_end = flush ? 1 : 0;
-  o->T = st.T;
-  o->from = st.from;
+  const nnab_stream_lane ln{0, received, n_carry, frames, n, flush ? 1 : 0};
+  o->cs = chunk_source(state, chunk, chunk_pitch, K, hop, pad, pad_mode, st.T > 0 ? (st.T - 1) * hop + K : 0,
+                       nullptr, ln);
+  o->A = st.T > 0 ? B : 0;
+  o->T_max = st.T;
+  o->longest = st.total - st.from;
   return NNAB_OK;
 }
-
-// ---- stream pools (DESIGN §3.10 "Pools") ---------------------------------------------------------------
-struct PoolPlan {
-  ChunkSource cs;     // lanes = the device table; length = the clip of T_max frames
-  int64_t A, T_max;
-  int64_t longest;    // the most samples one lane stores into the ring
-};
 
 // Checks the whole push (every lane by stream_step, the table's order and totals) before anything runs.
 static int pool_plan(const void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
@@ -224,17 +228,8 @@ static int pool_plan(const void* state, const nnab_stream_lane* lanes, const nna
     if (st.total - st.from > longest) longest = st.total - st.from;
   }
   if (t_max != T_max) return NNAB_EINVAL;
-  ChunkSource& c = o->cs;
-  c = ChunkSource{};
-  c.ring = static_cast<const float*>(state);
-  c.ring_pitch = K;
-  c.ring_len = K;
-  c.chunk = chunk;
-  c.chunk_pitch = chunk_pitch;
-  c.length = T_max > 0 ? (T_max - 1) * hop + K : 0;
-  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
-  c.lanes = d_lanes;
-  c.K = K; c.hop = hop; c.pad = pad;
+  o->cs = chunk_source(state, chunk, chunk_pitch, K, hop, pad, pad_mode, T_max > 0 ? (T_max - 1) * hop + K : 0,
+                       d_lanes, nnab_stream_lane{});
   o->A = A;
   o->T_max = T_max;
   o->longest = longest;
@@ -252,8 +247,9 @@ static int64_t pool_clip_length(int64_t A, int64_t T_max, int K, int hop) {
 }
 
 // The offline plan on the A rows' clips, the zeroing of every row's frames past its count, then each lane's
-// carry.  As chunk_forward, a plan that cannot read the clips returns NNAB_EUNSUPPORTED before anything is
-// enqueued (when A > 0).
+// carry.  A plan that cannot read the clips (the SIMT kernels) returns NNAB_EUNSUPPORTED before anything is
+// enqueued, the ring included (when A > 0).  Lanes that share their counters all return T_max frames: nothing
+// to zero.
 template <typename Run>
 static int pool_forward(const PoolPlan& pp, int chunk_dtype, int64_t n_lanes, float* out, int64_t rows, int cols,
                         Run&& run, void* stream) {
@@ -263,7 +259,7 @@ static int pool_forward(const PoolPlan& pp, int chunk_dtype, int64_t n_lanes, fl
   if (pp.A > 0) {
     const Wave w{nullptr, chunk_dtype, pp.A, pp.cs.length, pp.cs.length, 0, pp.cs.pad_mode, &pp.cs};
     if ((rc = run(w, s))) return rc;
-    if ((rc = tc_pool_mask(pp.cs, pp.A, out, rows, pp.T_max, cols, s))) return rc;
+    if (pp.cs.lanes != nullptr && (rc = tc_pool_mask(pp.cs, pp.A, out, rows, pp.T_max, cols, s))) return rc;
   }
   return tc_pool_carry(pp.cs, chunk_dtype, n_lanes, pp.longest, s);
 }
@@ -280,17 +276,8 @@ static int device_pool_plan(void* state, int64_t* counters, const int32_t* lengt
     return NNAB_EINVAL;
   if (pad_mode != NNAB_PAD_REFLECT && pad_mode != NNAB_PAD_CONSTANT) return NNAB_EINVAL;
   if (T_max != nnab_pool_frame_cap(n, K, hop, pad, pad_mode)) return NNAB_EINVAL;
-  ChunkSource& c = o->cs;
-  c = ChunkSource{};
-  c.ring = static_cast<const float*>(state);
-  c.ring_pitch = K;
-  c.ring_len = K;
-  c.chunk = chunk;
-  c.chunk_pitch = chunk_pitch;
-  c.length = (T_max - 1) * hop + K;
-  c.pad_mode = pad > 0 ? pad_mode : NNAB_PAD_CONSTANT;
-  c.lanes = d_lanes;
-  c.K = K; c.hop = hop; c.pad = pad;
+  o->cs = chunk_source(state, chunk, chunk_pitch, K, hop, pad, pad_mode, (T_max - 1) * hop + K, d_lanes,
+                       nnab_stream_lane{});
   o->A = slots;
   o->T_max = T_max;
   o->longest = n;
@@ -312,27 +299,12 @@ static int device_pool_forward(const PoolPlan& pp, int64_t* counters, const int3
   return pool_forward(pp, chunk_dtype, pp.A, out, rows, cols, run, stream);
 }
 
-static Wave chunk_wave(const ChunkPlan& cp, int chunk_dtype, int64_t B) {
-  return Wave{nullptr, chunk_dtype, B, cp.cs.length, cp.cs.length, 0, cp.cs.pad_mode, &cp.cs};
-}
-
-// Length of a push's virtual clip (0: the push returns no frame); host only, no validation.
-static int64_t chunk_clip_length(int64_t received, int64_t frames, int64_t n, int flush, int K, int hop,
-                                 int pad, int pad_mode) {
+// Frames a lock-step push returns (0: none); host only, no validation.
+static int64_t chunk_frames(int64_t received, int64_t frames, int64_t n, int flush, int K, int hop, int pad,
+                            int pad_mode) {
   const int64_t total = received + n;
   const int64_t t_end = flush ? frames_of(total, K, hop, pad) : chunk_ready_frames(total, K, hop, pad, pad_mode);
-  return t_end > frames ? (t_end - frames - 1) * (int64_t)hop + K : 0;
-}
-
-// The frames of a push on the offline plan (stft_run & co. with the virtual clip as their signal), then the
-// samples the next push needs into the carry ring.  A plan that cannot read the clip (the SIMT kernels)
-// returns NNAB_EUNSUPPORTED before anything is enqueued, the ring included.
-template <typename Run>
-static int chunk_forward(const ChunkPlan& cp, int chunk_dtype, int64_t B, Run&& run, void* stream) {
-  int rc = check_arch();
-  if (rc) return rc;
-  if (cp.T > 0 && B > 0 && (rc = run(chunk_wave(cp, chunk_dtype, B), (cudaStream_t)stream))) return rc;
-  return tc_chunk_carry(cp.cs, chunk_dtype, B, cp.from, (cudaStream_t)stream);
+  return t_end > frames ? t_end - frames : 0;
 }
 
 // ---- streamed inverse STFT: istft_chunk_plan (common.cuh) ------------------------------------------
@@ -2155,11 +2127,30 @@ int nnab_istft_forward(const float* X, int64_t B, int f_in, int64_t T, const voi
   return tc_istft_finalize(ola, ola_pitch, B, window, n_fft, hop, T, offset, out, want, s);
 }
 
-size_t nnab_istft_chunk_workspace_bytes(int64_t B, int f_in, int64_t T, int n_fft, int hop) {
-  // the push's buffer holds at most T * hop + n_fft positions: that of T + 1 frames
-  return nnab_istft_workspace_bytes(B, f_in, (T > 0 ? T : 1) + 1, n_fft, hop);
+// ---- streamed inverse STFT and inverse STFT pools (DESIGN §3.10 "Inverse pools") ---------------------------
+// Row i of a push's overlap-add buffer starts `lead` = n_fft positions before lane i's first new frame, so the
+// carried sums (at most n_fft / 2 before it) fit and the new frames of every lane start at column `lead`.
+static int64_t istft_pool_ola_pitch(int64_t T_max, int n_fft, int hop) {
+  const int64_t T = T_max > 0 ? T_max : 1;
+  return (int64_t)align_up((size_t)(2 * (int64_t)n_fft + (int64_t)hop * (T - 1)), 8);
 }
 
+static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, const nnab_istft_lane& shared,
+                          int64_t n_lanes, int64_t A, const float* X, int f_in, int64_t t, const void* packed,
+                          const float* window, int n_fft, int hop, int center, float* out, int64_t n_max,
+                          int64_t T_max, void* workspace, cudaStream_t s);
+
+size_t nnab_istft_pool_workspace_bytes(int64_t n_lanes, int f_in, int64_t T_max, int n_fft, int hop) {
+  if (n_lanes <= 0) return 0;
+  return nnab_istft_workspace_bytes(n_lanes, f_in, T_max > 0 ? T_max : 1, n_fft, hop) +
+         align_up((size_t)n_lanes * align_up((size_t)n_fft, 8) * sizeof(float), 256);
+}
+
+size_t nnab_istft_chunk_workspace_bytes(int64_t B, int f_in, int64_t T, int n_fft, int hop) {
+  return nnab_istft_pool_workspace_bytes(B, f_in, T, n_fft, hop);
+}
+
+// A lock-step push: the pool push of B lanes that share these counters, lane b in slot b and X row b.
 int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const float* X, int64_t B, int f_in,
                              int64_t T, const void* packed, const float* window, int n_fft, int hop, int center,
                              int flush, int64_t length, float* out, int64_t out_len, void* workspace,
@@ -2176,59 +2167,9 @@ int nnab_istft_chunk_forward(void* state, int64_t frames, int64_t emitted, const
   const size_t need = nnab_istft_chunk_workspace_bytes(B, f_in, T, n_fft, hop);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
   if (B == 0 || (T == 0 && n_out == 0)) return NNAB_OK;  // nothing new: the carry stays as it is
-  cudaStream_t s = (cudaStream_t)stream;
-  float* carry = static_cast<float*>(state);
-
-  // same layout as nnab_istft_forward, with room for T + 1 frames of overlap-add positions
-  char* ws = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  void* planes = ws;
-  int64_t ola_pitch = 0;
-  const size_t planes_b = align_up(tc_istft_planes_bytes(B, T > 0 ? T : 1, f_in), 256);
-  const size_t ola_b = istft_ola_bytes(B, (T > 0 ? T : 1) + 1, n_fft, hop, &ola_pitch);
-  float* ola = (float*)(ws + planes_b);
-  float* scale = (float*)(ws + planes_b + ola_b);
-
-  // 1. the buffer: carried partial sums, then zeros
-  NNAB_CUDA_TRY(cudaMemsetAsync(ola, 0, (size_t)B * ola_pitch * sizeof(float), s));
-  if (pl.carried > 0)
-    NNAB_CUDA_TRY(cudaMemcpy2DAsync(ola, (size_t)ola_pitch * sizeof(float), carry, (size_t)n_fft * sizeof(float),
-                                    (size_t)pl.carried * sizeof(float), (size_t)B, cudaMemcpyDeviceToDevice, s));
-  // 2. the new frames, overlap-added at their global positions (the FMT_OLA GEMM of nnab_istft_forward)
-  if (T > 0) {
-    if ((rc = tc_istft_prep(X, B, f_in, T, planes, s))) return rc;
-    istft_scale_kernel<<<(n_fft + 255) / 256, 256, 0, s>>>(window, 1.0f / (float)n_fft, n_fft, scale);
-    NNAB_LAUNCH_CHECK();
-    const int kpad = tc_istft_k(f_in);
-    FramedProblem p{};
-    p.x = nullptr; p.B = B; p.L = T * (int64_t)kpad; p.x_pitch = 0;
-    p.F = n_fft; p.K = kpad; p.hop = kpad; p.pad = 0; p.pad_mode = NNAB_PAD_CONSTANT;
-    p.scale = scale; p.scale_all = 1.f; p.fmt = FMT_OLA; p.eps = 0.f; p.power = 1.f;
-    p.out = ola + (frames * (int64_t)hop - pl.origin); p.T = T; p.out_bins = n_fft; p.bin_offset = 0;
-    p.presplit = planes;
-    p.ola_pitch = ola_pitch; p.ola_hop = hop;
-    if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
-  }
-  // 3. final samples / window sum-square at their global positions, the open tail into the carry
-  return tc_istft_chunk_finalize(ola, ola_pitch, B, window, n_fft, hop, frames + T, pl.origin, pl.emit_begin, out,
-                                 n_out, pl.carry_begin, pl.carry_len, carry, s);
-}
-
-// ---- inverse STFT pools (DESIGN §3.10 "Inverse pools") ---------------------------------------------------
-// Row i of a push's overlap-add buffer starts `lead` = n_fft positions before lane i's first new frame, so the
-// carried sums (at most n_fft / 2 before it) fit and the new frames of every lane start at column `lead`.
-static int64_t istft_pool_ola_pitch(int64_t T_max, int n_fft, int hop) {
-  const int64_t T = T_max > 0 ? T_max : 1;
-  return (int64_t)align_up((size_t)(2 * (int64_t)n_fft + (int64_t)hop * (T - 1)), 8);
-}
-
-static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t n_lanes, int64_t A, const float* X,
-                          int f_in, int64_t t, const void* packed, const float* window, int n_fft, int hop,
-                          int center, float* out, int64_t n_max, int64_t T_max, void* workspace, cudaStream_t s);
-
-size_t nnab_istft_pool_workspace_bytes(int64_t n_lanes, int f_in, int64_t T_max, int n_fft, int hop) {
-  if (n_lanes <= 0) return 0;
-  return nnab_istft_workspace_bytes(n_lanes, f_in, T_max > 0 ? T_max : 1, n_fft, hop) +
-         align_up((size_t)n_lanes * align_up((size_t)n_fft, 8) * sizeof(float), 256);
+  const nnab_istft_lane ln{0, 0, frames, emitted, T, flush ? 1 : 0, length};
+  return istft_pool_run(static_cast<float*>(state), nullptr, ln, B, n_out > 0 ? B : 0, X, f_in, T, packed, window,
+                        n_fft, hop, center, out, n_out, T, workspace, (cudaStream_t)stream);
 }
 
 int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nnab_istft_lane* d_lanes,
@@ -2270,14 +2211,16 @@ int nnab_istft_pool_forward(void* state, const nnab_istft_lane* lanes, const nna
   const size_t need = nnab_istft_pool_workspace_bytes(n_lanes, f_in, T_max, n_fft, hop);
   if (n_lanes > 0 && (workspace == nullptr || ws_bytes < need)) return NNAB_EWORKSPACE;
   if (n_lanes == 0) return NNAB_OK;
-  return istft_pool_run(static_cast<float*>(state), d_lanes, n_lanes, A, X, f_in, t, packed, window, n_fft, hop,
-                        center, out, n_max, T_max, workspace, (cudaStream_t)stream);
+  return istft_pool_run(static_cast<float*>(state), d_lanes, nnab_istft_lane{}, n_lanes, A, X, f_in, t, packed,
+                        window, n_fft, hop, center, out, n_max, T_max, workspace, (cudaStream_t)stream);
 }
 
-// The launches of an inverse pool push on a checked lane table (seed, pre-pass and GEMM, finalize).
-static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t n_lanes, int64_t A, const float* X,
-                          int f_in, int64_t t, const void* packed, const float* window, int n_fft, int hop,
-                          int center, float* out, int64_t n_max, int64_t T_max, void* workspace, cudaStream_t s) {
+// The launches of an inverse push on checked lanes (seed, pre-pass and GEMM, finalize): the DEVICE lane table
+// d_lanes, or without one `shared` in slot i with X row i.
+static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, const nnab_istft_lane& shared,
+                          int64_t n_lanes, int64_t A, const float* X, int f_in, int64_t t, const void* packed,
+                          const float* window, int n_fft, int hop, int center, float* out, int64_t n_max,
+                          int64_t T_max, void* workspace, cudaStream_t s) {
   int rc;
   // nnab_istft_forward's layout for n_lanes x max(T_max, 1) frames, each row `lead` positions longer
   const int64_t lead = n_fft;
@@ -2290,7 +2233,8 @@ static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t 
   float* scale = (float*)(ws + planes_b + ola_b);
 
   // 1. every row: its carried sums where they lie, zeros elsewhere
-  if ((rc = tc_istft_pool_seed(d_lanes, n_lanes, carry, n_fft, hop, center, lead, ola, ola_pitch, s))) return rc;
+  if ((rc = tc_istft_pool_seed(d_lanes, shared, n_lanes, carry, n_fft, hop, center, lead, ola, ola_pitch, s)))
+    return rc;
   // 2. the new frames of every lane, overlap-added from column `lead` (one FMT_OLA GEMM over n_lanes x T_max)
   if (T_max > 0) {
     if ((rc = tc_istft_pool_prep(X, d_lanes, n_lanes, f_in, T_max, t, planes, s))) return rc;
@@ -2307,8 +2251,8 @@ static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, int64_t 
     if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
   }
   // 3. every lane's final samples / window sum-square (rows i < A of out, zeros up to n_max), its tail carried
-  return tc_istft_pool_finalize(d_lanes, n_lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center, out, n_max,
-                                carry, s);
+  return tc_istft_pool_finalize(d_lanes, shared, n_lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center, out,
+                                n_max, carry, s);
 }
 
 // ---- device pools (DESIGN §3.10 "Device pools") -----------------------------------------------------------
@@ -2340,8 +2284,8 @@ int nnab_istft_pool_device_forward(void* state, int64_t* counters, const int32_t
   if ((rc = tc_device_istft_plan(slots, counters, frame_counts, end, length, errors, error_info, counts, d_lanes, t,
                                  n_fft, hop, center, s)))
     return rc;
-  return istft_pool_run(static_cast<float*>(state), d_lanes, slots, slots, X, f_in, t, packed, window, n_fft, hop,
-                        center, out, n_max, t, workspace, s);
+  return istft_pool_run(static_cast<float*>(state), d_lanes, nnab_istft_lane{}, slots, slots, X, f_in, t, packed,
+                        window, n_fft, hop, center, out, n_max, t, workspace, s);
 }
 
 int nnab_pool_device_reset(int64_t* counters, int32_t* errors, int64_t* error_info, const uint8_t* mask,
@@ -2484,8 +2428,8 @@ size_t nnab_chunk_state_bytes(int64_t B, int K) {
 
 size_t nnab_stft_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
                                        int n_fft, int F, int hop, int center, int pad_mode, int path) {
-  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
-  return Lv > 0 ? nnab_stft_workspace_bytes(B, Lv, n_fft, F, hop, 0, path) : 0;
+  const int64_t T = chunk_frames(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return nnab_stft_pool_workspace_bytes(T > 0 ? B : 0, T, n_fft, F, hop, path);
 }
 
 int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
@@ -2493,12 +2437,13 @@ int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
                             const float* wcos, const float* wsin, const void* packed, int n_fft, int F, int hop,
                             int center, int pad_mode, int out_format, float sqrt_eps, float* out, int64_t T,
                             void* workspace, size_t ws_bytes, int path, void* stream) {
-  ChunkPlan cp;
-  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
-                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  PoolPlan pp;
+  int rc = lock_step_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                          center ? n_fft / 2 : 0, pad_mode, &pp);
   if (rc) return rc;
-  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
-  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+  if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format))
+    return NNAB_EINVAL;
+  return pool_forward(pp, chunk_dtype, B, out, F, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
   }, stream);
 }
@@ -2506,8 +2451,8 @@ int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
 size_t nnab_filterbank_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
                                              int n_fft, int F, int hop, int center, int pad_mode, int n_fb,
                                              int path, int has_table) {
-  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
-  return Lv > 0 ? filterbank_ws_bytes(B, Lv, n_fft, F, hop, 0, n_fb, path, has_table) : 0;
+  const int64_t T = chunk_frames(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return nnab_filterbank_pool_workspace_bytes(T > 0 ? B : 0, T, n_fft, F, hop, n_fb, path, has_table);
 }
 
 int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
@@ -2517,13 +2462,13 @@ int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_
                                        float sqrt_eps, float power, const float* fb, int n_fb,
                                        const void* fb_table, float* out, int64_t T, void* workspace,
                                        size_t ws_bytes, int path, void* stream) {
-  ChunkPlan cp;
-  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
-                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  PoolPlan pp;
+  int rc = lock_step_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                          center ? n_fft / 2 : 0, pad_mode, &pp);
   if (rc) return rc;
-  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb))
+  if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb))
     return NNAB_EINVAL;
-  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+  return pool_forward(pp, chunk_dtype, B, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
     return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T,
                           workspace, ws_bytes, path, s);
   }, stream);
@@ -2532,9 +2477,8 @@ int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_
 size_t nnab_mfcc_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
                                        int n_fft, int F, int hop, int center, int pad_mode, int n_mels, int path,
                                        int has_table) {
-  (void)has_table;
-  const int64_t Lv = chunk_clip_length(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
-  return Lv > 0 ? mfcc_ws_bytes(B, Lv, n_fft, F, hop, 0, n_mels, path) : 0;
+  const int64_t T = chunk_frames(received, frames, n, flush, n_fft, hop, center ? n_fft / 2 : 0, pad_mode);
+  return nnab_mfcc_pool_workspace_bytes(T > 0 ? B : 0, T, n_fft, F, hop, n_mels, path, has_table);
 }
 
 int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames, const void* chunk,
@@ -2544,15 +2488,15 @@ int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
                             int n_mels, const void* fb_table, float amin, float ref, float top_db,
                             const float* dct, int n_mfcc, float* out, int64_t T, void* workspace,
                             size_t ws_bytes, int path, void* stream) {
-  ChunkPlan cp;
-  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
-                      center ? n_fft / 2 : 0, pad_mode, &cp);
+  PoolPlan pp;
+  int rc = lock_step_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, n_fft, hop,
+                          center ? n_fft / 2 : 0, pad_mode, &pp);
   if (rc) return rc;
   // the top_db floor is a maximum over the whole clip: a stream cannot apply it frame by frame
-  if (T != cp.T || F <= 0 || (T > 0 && out == nullptr) || top_db >= 0.f ||
+  if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || top_db >= 0.f ||
       mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin))
     return NNAB_EINVAL;
-  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+  return pool_forward(pp, chunk_dtype, B, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
     return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
                     ref, top_db, dct, n_mfcc, out, T, workspace, ws_bytes, path, s);
   }, stream);
@@ -2560,8 +2504,8 @@ int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
 
 size_t nnab_cqt1992v2_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
                                             int width, int n_bins, int hop, int center, int pad_mode, int path) {
-  const int64_t Lv = chunk_clip_length(received, frames, n, flush, width, hop, center ? width / 2 : 0, pad_mode);
-  return Lv > 0 ? nnab_cqt1992v2_workspace_bytes(B, Lv, width, n_bins, hop, 0, path) : 0;
+  const int64_t T = chunk_frames(received, frames, n, flush, width, hop, center ? width / 2 : 0, pad_mode);
+  return nnab_cqt1992v2_pool_workspace_bytes(T > 0 ? B : 0, T, width, n_bins, hop, path);
 }
 
 int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry, int64_t frames,
@@ -2571,13 +2515,13 @@ int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry,
                                  int hop, int center, int pad_mode, const float* scale, float scale_all,
                                  int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
                                  size_t ws_bytes, int path, void* stream) {
-  ChunkPlan cp;
-  int rc = chunk_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, width, hop,
-                      center ? width / 2 : 0, pad_mode, &cp);
+  PoolPlan pp;
+  int rc = lock_step_plan(state, received, n_carry, frames, chunk, chunk_dtype, B, n, chunk_pitch, flush, width, hop,
+                          center ? width / 2 : 0, pad_mode, &pp);
   if (rc) return rc;
-  if (T != cp.T || n_bins <= 0 || (T > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
+  if (T != pp.T_max || n_bins <= 0 || (T > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
     return NNAB_EINVAL;
-  return chunk_forward(cp, chunk_dtype, B, [&](const Wave& w, cudaStream_t s) {
+  return pool_forward(pp, chunk_dtype, B, out, n_bins, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
                          out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
   }, stream);

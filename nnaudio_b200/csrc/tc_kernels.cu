@@ -213,29 +213,25 @@ __global__ void __launch_bounds__(256) pad_split_kernel(
   *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
-// pad_split_kernel on a push's virtual clip (ChunkSource): each sample is taken from the fp32 carry ring or
-// the chunk, with the reflect / constant centre padding of the whole stream at its two ends.  The planes of
-// frame t0 + j are then those the whole-clip pre-pass writes for frame t0 + j.  LANES (stream pools): row b
-// builds the clip of lane b of c.lanes, from its own ring / chunk row, counters and end; its samples past
-// what its own frames read are zeros.
-template <typename Tx, bool LANES>
+// pad_split_kernel on a push's virtual clips (ChunkSource): row b builds the clip of lane b, each sample taken
+// from its fp32 carry ring row or its chunk row, with the reflect / constant centre padding of its whole stream
+// at the two ends.  The planes of frame t0 + j are then those the whole-clip pre-pass writes for the lane's frame
+// frames + t0 + j; the row's samples past what its own frames read are zeros.  A row with frames never mirrors
+// past its samples on the left, nor further than pad on the right; a device pool's row without frames may, and
+// reads nothing there.
+template <typename Tx>
 __global__ void __launch_bounds__(256) chunk_split_kernel(
     ChunkSource c, const Tx* __restrict__ chunk, int shift, int64_t clip_pitch, int64_t plane_stride,
     int poly_hop, __nv_bfloat16* __restrict__ planes) {
   const int64_t b = blockIdx.y;
   const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i0 >= clip_pitch) return;
-  int64_t row = b;
-  if constexpr (LANES) {
-    const nnab_stream_lane& ln = c.lanes[b];
-    row = ln.slot;
-    c.received = ln.received;
-    c.total = ln.received + ln.n;
-    c.origin = ln.frames * c.hop - c.pad;
-    c.at_end = (int)ln.end;
-  }
-  const float* __restrict__ ring = c.ring + row * c.ring_pitch;
-  const Tx* __restrict__ xb = chunk + row * c.chunk_pitch;
+  nnab_stream_lane ln = c.shared;
+  ln.slot = b;
+  if (c.lanes != nullptr) ln = c.lanes[b];
+  const int64_t received = ln.received, total = ln.received + ln.n, origin = ln.frames * c.hop - c.pad;
+  const float* __restrict__ ring = c.ring + ln.slot * c.ring_pitch;
+  const Tx* __restrict__ xb = chunk + ln.slot * c.chunk_pitch;
   const bool reflect = c.pad_mode == NNAB_PAD_REFLECT;
   const int64_t s0 = split_src(i0, poly_hop) + shift;
   const int step = poly_hop ? 4 : 1;  // the 8 positions of a thread: consecutive samples, or one phase
@@ -246,17 +242,16 @@ __global__ void __launch_bounds__(256) chunk_split_kernel(
     const int64_t i = s0 + step * e;
     float v = 0.f;
     if (i < c.length) {
-      int64_t r = c.origin + i;
+      int64_t r = origin + i;
       bool live = true;
       if (r < 0) {
         if (reflect) r = -r; else live = false;
-        // a device pool's row without frames may mirror past its own samples: nothing to read there
-        if constexpr (LANES) if (r >= c.total) live = false;
-      } else if (r >= c.total) {
-        // a pool row's clip runs past its own right padding (the longest row sets the length): zeros there
-        if (c.at_end && reflect && (!LANES || r - c.total < c.pad)) r = 2 * (c.total - 1) - r; else live = false;
+        if (r >= total) live = false;
+      } else if (r >= total) {
+        // the clip runs past the row's own right padding (the longest row sets the length): zeros there
+        if (ln.end && reflect && r - total < c.pad) r = 2 * (total - 1) - r; else live = false;
       }
-      if (live) v = r < c.received ? __ldg(ring + r % c.ring_len) : sample_f32(__ldg(xb + (r - c.received)));
+      if (live) v = r < received ? __ldg(ring + r % c.ring_len) : sample_f32(__ldg(xb + (r - received)));
     }
     split_bf16(v, hi[e], lo[e]);
   }
@@ -265,27 +260,22 @@ __global__ void __launch_bounds__(256) chunk_split_kernel(
   *reinterpret_cast<uint4*>(planes + plane_stride + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
-// Raw samples [from, total) of the chunk into the carry ring.  Runs after every kernel of the push that reads
-// the ring (same stream), and never overwrites a sample the next push reads: the ring holds ring_len >= the
-// longest carry.  LANES: row b is lane b of c.lanes, which keeps its own [from, total) by the same rule as
-// the host (chunk_carry_start after the lane's frames, and never before its first new sample).
-template <typename Tx, bool LANES>
-__global__ void __launch_bounds__(256) chunk_carry_kernel(ChunkSource c, const Tx* __restrict__ chunk,
-                                                          int64_t from) {
-  int64_t row = blockIdx.y;
-  if constexpr (LANES) {
-    const nnab_stream_lane ln = c.lanes[blockIdx.y];
-    row = ln.slot;
-    c.received = ln.received;
-    c.total = ln.received + ln.n;
-    const int64_t keep =
-        chunk_carry_start(c.total, lane_frames_after(ln, c.K, c.hop, c.pad, c.pad_mode), c.hop, c.pad);
-    from = keep > c.received ? keep : c.received;
-  }
+// Raw samples [from, received + n) of lane b's chunk row into its carry ring row, from = chunk_carry_start after
+// the lane's frames and never before its first new sample (the host's rule, stream_step).  Runs after every
+// kernel of the push that reads the ring (same stream), and never overwrites a sample the next push reads: the
+// ring holds ring_len >= the longest carry.
+template <typename Tx>
+__global__ void __launch_bounds__(256) chunk_carry_kernel(ChunkSource c, const Tx* __restrict__ chunk) {
+  nnab_stream_lane ln = c.shared;
+  ln.slot = blockIdx.y;
+  if (c.lanes != nullptr) ln = c.lanes[blockIdx.y];
+  const int64_t total = ln.received + ln.n;
+  const int64_t keep = chunk_carry_start(total, lane_frames_after(ln, c.K, c.hop, c.pad, c.pad_mode), c.hop, c.pad);
+  const int64_t from = keep > ln.received ? keep : ln.received;
   const int64_t r = from + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= c.total) return;
-  const_cast<float*>(c.ring)[row * c.ring_pitch + r % c.ring_len] =
-      sample_f32(__ldg(chunk + row * c.chunk_pitch + (r - c.received)));
+  if (r >= total) return;
+  const_cast<float*>(c.ring)[ln.slot * c.ring_pitch + r % c.ring_len] =
+      sample_f32(__ldg(chunk + ln.slot * c.chunk_pitch + (r - ln.received)));
 }
 
 // Stream pools: frames t >= count of row i of out (A, rows, T, cols) are exact zeros (the row's clip is the
@@ -1041,51 +1031,20 @@ int tc_istft_finalize(const float* ola, int64_t ola_pitch, int64_t B, const floa
   return NNAB_OK;
 }
 
-// One push of a streamed inverse STFT.  `ola` holds overlap-add positions [origin, ...) of the stream (the
-// carried partial sums, then this push's frames).  Samples [emit_begin, emit_begin + out_len) are final: divided
-// by the window sum-square of their GLOBAL position over the T frames received so far (the same sum, in the same
-// order, as istft_finalize_kernel) and written to out.  Positions [carry_begin, carry_begin + carry_len), still
-// open to later frames, go un-normalised into the carry state (rows of n_fft floats).
-__global__ void __launch_bounds__(256) istft_chunk_finalize_kernel(
-    const float* __restrict__ ola, int64_t ola_pitch, const float* __restrict__ window, int n_fft, int hop,
-    int64_t T, int64_t origin, int64_t emit_begin, float* __restrict__ out, int64_t out_len, int64_t carry_begin,
-    int64_t carry_len, float* __restrict__ carry) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t b = blockIdx.y;
-  const float* __restrict__ row = ola + b * ola_pitch;
-  if (i < out_len) {
-    const int64_t s = emit_begin + i;
-    const float wss = istft_wss(window, n_fft, hop, T, s);
-    float v = row[s - origin];
-    if (wss > 1e-10f) v = v / wss;
-    out[b * out_len + i] = v;
-  }
-  if (i < carry_len) carry[b * n_fft + i] = row[carry_begin - origin + i];
-}
-
-int tc_istft_chunk_finalize(const float* ola, int64_t ola_pitch, int64_t B, const float* window, int n_fft,
-                            int hop, int64_t T, int64_t origin, int64_t emit_begin, float* out, int64_t out_len,
-                            int64_t carry_begin, int64_t carry_len, float* carry, cudaStream_t stream) {
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  const int64_t n = out_len > carry_len ? out_len : carry_len;
-  if (n <= 0 || B <= 0) return NNAB_OK;
-  dim3 grid((unsigned)ceil_div64(n, 256), (unsigned)B);
-  istft_chunk_finalize_kernel<<<grid, 256, 0, stream>>>(ola, ola_pitch, window, n_fft, hop, T, origin, emit_begin,
-                                                        out, out_len, carry_begin, carry_len, carry);
-  NNAB_LAUNCH_CHECK();
-  return NNAB_OK;
-}
-
-// Inverse STFT pools.  Row i of the overlap-add buffer holds lane i's global positions from
-// frames_i * hop - lead on (lead = n_fft): its carried sums start at most hop - n_fft / 2 positions before
-// frames_i * hop (istft_chunk_plan's origin), so every lane's new frames start at column `lead` and one FMT_OLA
-// GEMM with out = ola + lead serves all rows.  The seed writes each row whole: the lane's carried sums from
-// state row slot_i where they lie, zeros elsewhere (the memset and 2-D copy of the one-stream push).
+// Streamed inverse STFT pushes.  Lane i is lanes[i] of the DEVICE lane table or, without one (a lock-step push
+// of B streams that share their counters), `shared` in slot i.  Row i of the overlap-add buffer holds lane i's
+// global positions from frames_i * hop - lead on (lead = n_fft): its carried sums start at most hop - n_fft / 2
+// positions before frames_i * hop (istft_chunk_plan's origin), so every lane's new frames start at column `lead`
+// and one FMT_OLA GEMM with out = ola + lead serves all rows.  The seed writes each row whole: the lane's carried
+// sums from state row slot_i where they lie, zeros elsewhere.
 __global__ void __launch_bounds__(256) istft_pool_seed_kernel(const nnab_istft_lane* __restrict__ lanes,
+                                                              const nnab_istft_lane shared,
                                                               const float* __restrict__ state, int n_fft,
                                                               int hop, int center, int64_t lead,
                                                               float* __restrict__ ola, int64_t ola_pitch) {
-  const nnab_istft_lane ln = lanes[blockIdx.y];
+  nnab_istft_lane ln = shared;
+  ln.slot = blockIdx.y;
+  if (lanes != nullptr) ln = lanes[blockIdx.y];
   const IstftChunkPlan pl = istft_lane_plan(ln, n_fft, hop, center);
   const int64_t base = ln.frames * hop - lead - pl.origin;  // column c holds carried position c + base
   const float* __restrict__ src = state + ln.slot * n_fft;
@@ -1097,16 +1056,18 @@ __global__ void __launch_bounds__(256) istft_pool_seed_kernel(const nnab_istft_l
   }
 }
 
-// istft_chunk_finalize_kernel on every lane: rows i < A of out (A, n_max) take lane i's final samples, each
-// divided by the window sum-square of its global position over the lane's frames_i + T_i frames (istft_wss),
-// then exact zeros up to n_max; every lane's open tail goes un-normalised to its state row.
+// Rows i < A of out (A, n_max) take lane i's final samples, each divided by the window sum-square of its global
+// position over the lane's frames_i + T_i frames (istft_wss: the same sum, in the same order, as
+// istft_finalize_kernel), then exact zeros up to n_max; every lane's open tail goes un-normalised to its state row.
 __global__ void __launch_bounds__(256) istft_pool_finalize_kernel(
-    const nnab_istft_lane* __restrict__ lanes, int64_t A, const float* __restrict__ ola, int64_t ola_pitch,
-    int64_t lead, const float* __restrict__ window, int n_fft, int hop, int center, float* __restrict__ out,
-    int64_t n_max, float* __restrict__ state) {
+    const nnab_istft_lane* __restrict__ lanes, const nnab_istft_lane shared, int64_t A,
+    const float* __restrict__ ola, int64_t ola_pitch, int64_t lead, const float* __restrict__ window, int n_fft,
+    int hop, int center, float* __restrict__ out, int64_t n_max, float* __restrict__ state) {
   const int64_t i = blockIdx.y;
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const nnab_istft_lane ln = lanes[i];
+  nnab_istft_lane ln = shared;
+  ln.slot = i;
+  if (lanes != nullptr) ln = lanes[i];
   const IstftChunkPlan pl = istft_lane_plan(ln, n_fft, hop, center);
   const float* __restrict__ row = ola + i * ola_pitch;
   const int64_t base = ln.frames * hop - lead;  // global position of column 0
@@ -1123,25 +1084,26 @@ __global__ void __launch_bounds__(256) istft_pool_finalize_kernel(
   if (j < pl.carry_len) state[ln.slot * n_fft + j] = row[pl.carry_begin - base + j];
 }
 
-int tc_istft_pool_seed(const nnab_istft_lane* lanes, int64_t n_lanes, const float* state, int n_fft, int hop,
-                       int center, int64_t lead, float* ola, int64_t ola_pitch, cudaStream_t stream) {
+int tc_istft_pool_seed(const nnab_istft_lane* lanes, const nnab_istft_lane& shared, int64_t n_lanes,
+                       const float* state, int n_fft, int hop, int center, int64_t lead, float* ola, int64_t ola_pitch,
+                       cudaStream_t stream) {
   if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
   if (n_lanes <= 0) return NNAB_OK;
   const dim3 grid((unsigned)ceil_div64(ola_pitch, 256), (unsigned)n_lanes);
-  istft_pool_seed_kernel<<<grid, 256, 0, stream>>>(lanes, state, n_fft, hop, center, lead, ola, ola_pitch);
+  istft_pool_seed_kernel<<<grid, 256, 0, stream>>>(lanes, shared, state, n_fft, hop, center, lead, ola, ola_pitch);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
 
-int tc_istft_pool_finalize(const nnab_istft_lane* lanes, int64_t n_lanes, int64_t A, const float* ola,
-                           int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop, int center,
-                           float* out, int64_t n_max, float* state, cudaStream_t stream) {
+int tc_istft_pool_finalize(const nnab_istft_lane* lanes, const nnab_istft_lane& shared, int64_t n_lanes, int64_t A,
+                           const float* ola, int64_t ola_pitch, int64_t lead, const float* window, int n_fft, int hop,
+                           int center, float* out, int64_t n_max, float* state, cudaStream_t stream) {
   if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
   if (n_lanes <= 0) return NNAB_OK;
   const int64_t n = n_max > n_fft ? n_max : n_fft;  // a carried tail holds at most n_fft positions
   const dim3 grid((unsigned)ceil_div64(n, 256), (unsigned)n_lanes);
-  istft_pool_finalize_kernel<<<grid, 256, 0, stream>>>(lanes, A, ola, ola_pitch, lead, window, n_fft, hop, center,
-                                                       out, n_max, state);
+  istft_pool_finalize_kernel<<<grid, 256, 0, stream>>>(lanes, shared, A, ola, ola_pitch, lead, window, n_fft, hop,
+                                                       center, out, n_max, state);
   NNAB_LAUNCH_CHECK();
   return NNAB_OK;
 }
@@ -1659,12 +1621,8 @@ static int launch_chunk_split(const ChunkSource& cs, int x_dtype, dim3 grid, int
     if (cs.rows != nullptr)
       chunk_split_rows_kernel<Tx><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
                                                             planes);
-    else if (cs.lanes != nullptr)
-      chunk_split_kernel<Tx, true><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
-                                                             planes);
     else
-      chunk_split_kernel<Tx, false><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop,
-                                                              planes);
+      chunk_split_kernel<Tx><<<grid, 256, 0, stream>>>(cs, xs, shift, clip_pitch, plane_stride, poly_hop, planes);
   });
 }
 
@@ -1677,23 +1635,13 @@ int tc_chunk_split(const ChunkSource& cs, int x_dtype, int64_t B, int64_t clip_p
                             stream);
 }
 
-int tc_chunk_carry(const ChunkSource& cs, int x_dtype, int64_t B, int64_t from, cudaStream_t stream) {
-  if (from >= cs.total || B <= 0) return NNAB_OK;
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  const dim3 grid((unsigned)ceil_div64(cs.total - from, 256), (unsigned)B);
-  return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
-    using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
-    chunk_carry_kernel<Tx, false><<<grid, 256, 0, stream>>>(cs, xs, from);
-  });
-}
-
 int tc_pool_carry(const ChunkSource& cs, int x_dtype, int64_t n_lanes, int64_t longest, cudaStream_t stream) {
   if (longest <= 0 || n_lanes <= 0) return NNAB_OK;
   if (n_lanes > 65535) return NNAB_EUNSUPPORTED;
   const dim3 grid((unsigned)ceil_div64(longest, 256), (unsigned)n_lanes);
   return with_sample_type(x_dtype, cs.chunk, [&](auto* xs) {
     using Tx = std::remove_const_t<std::remove_pointer_t<decltype(xs)>>;
-    chunk_carry_kernel<Tx, true><<<grid, 256, 0, stream>>>(cs, xs, 0);
+    chunk_carry_kernel<Tx><<<grid, 256, 0, stream>>>(cs, xs);
   });
 }
 

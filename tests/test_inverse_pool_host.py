@@ -324,3 +324,17 @@ def test_istft_pool_workspace_query_obeys_its_rule():
         lead = up(n_lanes * up(n_fft, 8) * 4, 256)  # n_lanes rows of n_fft floats, rows rounded up to 8 floats
         assert lib.nnab_istft_pool_workspace_bytes(n_lanes, f_in, T_max, n_fft, hop) == \
             lib.nnab_istft_workspace_bytes(n_lanes, f_in, max(T_max, 1), n_fft, hop) + lead
+
+
+def test_istft_chunk_workspace_equals_pool_of_its_lanes():
+    """A lock-step inverse push of B streams is a pool push of B lanes that share its counters, lane b in slot b
+    and X row b: its workspace query equals the pool's for n_lanes = B and T_max = T, over seeded cases."""
+    lib = _C.lib()
+    rng = np.random.default_rng(5)
+    for _ in range(200):
+        n_fft = int(rng.choice([16, 64, 200, 512, 2048]))
+        hop = int(rng.integers(1, n_fft + 1))
+        f_in = int(rng.choice([n_fft // 2 + 1, n_fft]))
+        T, B = int(rng.integers(0, 40)), int(rng.choice([1, 2, 7, 256, 65535]))
+        assert lib.nnab_istft_chunk_workspace_bytes(B, f_in, T, n_fft, hop) == \
+            lib.nnab_istft_pool_workspace_bytes(B, f_in, T, n_fft, hop), (B, f_in, T, n_fft, hop)

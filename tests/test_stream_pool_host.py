@@ -313,3 +313,36 @@ def test_pool_workspace_queries_equal_the_offline_queries():
                 lib.nnab_cqt1992v2_workspace_bytes(A, L, 64, 24, 16, 0, path)
     assert lib.nnab_stft_pool_workspace_bytes(0, 5, 64, 33, 16, 0) == 0
     assert lib.nnab_stft_pool_workspace_bytes(3, 0, 64, 33, 16, 0) == 0
+
+
+@pytest.mark.parametrize("K, hop, center, pm", [(64, 16, 1, _C.PAD_REFLECT), (64, 16, 1, _C.PAD_CONSTANT),
+                                                (400, 160, 0, _C.PAD_REFLECT), (512, 128, 1, _C.PAD_REFLECT)])
+def test_lock_step_workspace_equals_pool_of_its_lanes(K, hop, center, pm):
+    """A lock-step push of B streams is a pool push of B lanes that share its counters: over seeded push sequences
+    ending in a flush, each chunk call's workspace query equals its pool query for A = B (0 when the push returns no
+    frame) and T_max = the push's frames."""
+    lib = _C.lib()
+    pad, F = K // 2 if center else 0, K // 2 + 1
+    rng = np.random.default_rng(K + hop + pm)
+    for path in (_C.PATH_AUTO, _C.PATH_SIMT):
+        for B in (1, 3, 256):
+            received = frames = 0
+            for step in range(25):
+                n, flush = int(rng.choice([0, 1, hop, int(rng.integers(0, 3 * K))])), int(step == 24)
+                total = received + n
+                t_end = ((total + 2 * pad - K) // hop + 1 if flush
+                         else _ready_frames(total, K, hop, pad, pm == _C.PAD_REFLECT))
+                T = t_end - frames
+                A, head = (B if T > 0 else 0), (B, received, frames, n, flush)
+                assert lib.nnab_stft_chunk_workspace_bytes(*head, K, F, hop, center, pm, path) == \
+                    lib.nnab_stft_pool_workspace_bytes(A, T, K, F, hop, path), (B, step)
+                for has_table in (0, 1):
+                    assert lib.nnab_filterbank_chunk_workspace_bytes(*head, K, F, hop, center, pm, 12, path,
+                                                                     has_table) == \
+                        lib.nnab_filterbank_pool_workspace_bytes(A, T, K, F, hop, 12, path, has_table), (B, step)
+                    assert lib.nnab_mfcc_chunk_workspace_bytes(*head, K, F, hop, center, pm, 12, path, has_table) == \
+                        lib.nnab_mfcc_pool_workspace_bytes(A, T, K, F, hop, 12, path, has_table), (B, step)
+                assert lib.nnab_cqt1992v2_chunk_workspace_bytes(*head, K, 24, hop, center, pm, path) == \
+                    lib.nnab_cqt1992v2_pool_workspace_bytes(A, T, K, 24, hop, path), (B, step)
+                received, frames = total, t_end
+            assert frames > 0

@@ -313,7 +313,7 @@ def test_inverse_rules(monkeypatch):
         st.push(torch.zeros(2, 33, 1, 2))
 
 
-def test_istft_chunk_entry_point_rejects_bad_counters_on_the_host():
+def test_istft_chunk_entry_point_rejects_bad_counters_and_sizes_a_pool_workspace():
     lib = _C.lib()
     P = ctypes.c_void_p
     p = P(256)
@@ -330,4 +330,6 @@ def test_istft_chunk_entry_point_rejects_bad_counters_on_the_host():
     assert call(frames=4, emitted=32, T=0, flush=1, length=10, out_len=0) == EINVAL, "length < returned"
     assert call(hop=65) == EINVAL, "frames that do not overlap"
     assert call(frames=0, T=0, flush=1, out_len=0) == EINVAL, "flush without frames"
-    assert lib.nnab_istft_chunk_workspace_bytes(2, 33, 4, 64, 16) == lib.nnab_istft_workspace_bytes(2, 33, 5, 64, 16)
+    # the push is the pool push of its B lanes: the pool layout, a lead of n_fft positions per overlap-add row
+    assert lib.nnab_istft_chunk_workspace_bytes(2, 33, 4, 64, 16) == \
+        lib.nnab_istft_pool_workspace_bytes(2, 33, 4, 64, 16)
