@@ -161,6 +161,13 @@ int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64
 size_t nnab_filterbank_table_bytes(int F);
 int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table,
                                 int* h_max_nnz, void* stream);
+/* 1 when a forward call given this table (built above), this packed basis and n_fft sums the bank in the
+ * contraction's epilogue, 0 when it runs the un-fused filterbank: pass the result as `has_table` to the workspace
+ * queries.  The epilogue adds one fp32 atomic partial sum per N tile a filter's bins meet; on a dense basis the
+ * table is used only when that is at most two for every filter, so that the sum does not depend on the order they
+ * land in, and only for n_fft < 8192: a longer basis needs the split-K accumulation only the un-fused power
+ * spectrogram has. */
+int nnab_filterbank_table_fuses(const void* table, const void* packed, int n_fft);
 
 /* ------------------------------------------------------------------------- *
  * MelSpectrogram.forward / Gammatonegram.forward — features/mel.py:171-189,
@@ -783,6 +790,24 @@ enum {
 };
 /* The counter of `route` (an NNAB_CQ1992_* value); 0 for any other value. */
 uint64_t nnab_cqt1992v2_route_count(int route);
+
+/* Routes of nnab_stft_forward(_ex), nnab_stft_filterbank_forward(_ex) and nnab_mfcc_forward(_ex), counted since
+ * load so that a test can tell which one a call took.  Each successful call adds one to the counter of the
+ * contraction route it enqueued (a dense call once, however many frame phases it launches); a filterbank or MFCC
+ * call also adds one to the counter of its filterbank route.  The chunk, pool and device-pool entry points run the
+ * same kernels but count nothing. */
+enum {
+  NNAB_STFT_BLOCK = 0,         /* block-partial kernel (periodic-Hann DFT basis)                         */
+  NNAB_STFT_DENSE = 1,         /* dense tensor-core kernel, one launch per frame phase                   */
+  NNAB_STFT_DENSE_SPLITK = 2,  /* the same with K cut into chunks, then the split-K finalize             */
+  NNAB_STFT_SIMT = 3,          /* CUDA-core kernel                                                       */
+  NNAB_STFT_FB_FUSED = 4,      /* filterbank summed in the contraction's epilogue (banded table)         */
+  NNAB_STFT_FB_PLANES = 5,     /* |X| ** power as bf16 operand planes, then a tensor-core GEMM with the bank */
+  NNAB_STFT_FB_GEMM = 6,       /* fp32 (B, F, T) power spectrogram, then the CUDA-core filterbank GEMM   */
+  NNAB_STFT_ROUTES = 7
+};
+/* The counter of `route` (an NNAB_STFT_* value); 0 for any other value. */
+uint64_t nnab_stft_route_count(int route);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

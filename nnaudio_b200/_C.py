@@ -43,6 +43,7 @@ SIGNATURES = {
     "nnab_balanced_launch_count": (c_uint64, []),
     "nnab_pyramid_route_count": (c_uint64, [c_int]),
     "nnab_cqt1992v2_route_count": (c_uint64, [c_int]),
+    "nnab_stft_route_count": (c_uint64, [c_int]),
     "nnab_pack_tile_n": (c_int, [c_int]),
     "nnab_packed_basis_bytes": (c_size_t, [c_int, c_int]),
     "nnab_pack_basis": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -54,6 +55,7 @@ SIGNATURES = {
     ),
     "nnab_filterbank_table_bytes": (c_size_t, [c_int]),
     "nnab_build_filterbank_table": (c_int, [_P, c_int, c_int, _P, _P, _P]),
+    "nnab_filterbank_table_fuses": (c_int, [_P, _P, c_int]),
     "nnab_filterbank_workspace_bytes": (
         c_size_t, [c_int64, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
     "nnab_stft_filterbank_forward": (
@@ -252,6 +254,18 @@ def cqt1992v2_route_count(route: int) -> int:
     """Offline CQT1992v2 calls that took kernel route ``route`` (a CQ1992_* constant) since load; the streaming
     and pool calls count nothing."""
     return int(lib().nnab_cqt1992v2_route_count(int(route)))
+
+
+# routes of nnab_stft_forward / nnab_stft_filterbank_forward / nnab_mfcc_forward (NNAB_STFT_*): the contraction's
+# kernel, then (filterbank and MFCC calls) how the bank was applied
+(STFT_BLOCK, STFT_DENSE, STFT_DENSE_SPLITK, STFT_SIMT, STFT_FB_FUSED, STFT_FB_PLANES, STFT_FB_GEMM) = range(7)
+STFT_ROUTES = 7
+
+
+def stft_route_count(route: int) -> int:
+    """Offline STFT / filterbank / MFCC calls that took route ``route`` (a STFT_* constant) since load; the
+    streaming and pool calls count nothing."""
+    return int(lib().nnab_stft_route_count(int(route)))
 
 
 def set_sm_reserve(n_sms: int) -> int:
@@ -529,7 +543,9 @@ def _stft_head(kw):
 
 
 def _has_table(kw):
-    return int(kw.get("fb_table") is not None)
+    """The workspace queries' ``has_table``: the call sums the bank in the contraction's epilogue."""
+    t = kw.get("fb_table")
+    return int(t is not None and lib().nnab_filterbank_table_fuses(_ptr(t), _ptr(kw["packed"]), kw["n_fft"]) != 0)
 
 
 def _complex_shape(rows, bins, T, complex_out):

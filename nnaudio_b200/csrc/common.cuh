@@ -594,9 +594,11 @@ struct FramedProblem {
   // non-null: the tensor-core pre-pass builds the planes from this push's virtual clip instead of x
   // (then L = chunk->length, pad = 0); the SIMT kernel returns NNAB_EUNSUPPORTED
   const ChunkSource* chunk;
-  // host, or nullptr: receives the NNAB_CQ1992_* kernel route a successful launch enqueued
+  // host, or nullptr: receives the NNAB_CQ1992_* kernel route a successful launch enqueued (ROUTE_BLOCK for the
+  // block-partial kernel, which only the STFT family runs)
   int* route;
 };
+constexpr int ROUTE_BLOCK = NNAB_CQ1992_ROUTES;
 
 int launch_framed_simt(const FramedProblem& p, cudaStream_t stream);
 

@@ -2,6 +2,7 @@
 // and the reference file:line each call replaces.
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 #include <stdlib.h>
@@ -28,6 +29,20 @@ void count_balanced_launch() { g_balanced_launches.fetch_add(1, std::memory_orde
 static std::atomic<uint64_t> g_pyr_routes[NNAB_PYR_ROUTES];
 static void count_route(int route) { g_pyr_routes[route].fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<uint64_t> g_cq1992_routes[NNAB_CQ1992_ROUTES];
+static std::atomic<uint64_t> g_stft_routes[NNAB_STFT_ROUTES];
+// routes[0]: the contraction's kernel route (NNAB_CQ1992_* / ROUTE_BLOCK, as the launchers write it); routes[1]:
+// the filterbank route (NNAB_STFT_FB_*), or -1
+static void count_stft_routes(const int (&routes)[2]) {
+  int r = -1;
+  switch (routes[0]) {
+    case ROUTE_BLOCK: r = NNAB_STFT_BLOCK; break;
+    case NNAB_CQ1992_DENSE: r = NNAB_STFT_DENSE; break;
+    case NNAB_CQ1992_DENSE_SPLITK: r = NNAB_STFT_DENSE_SPLITK; break;
+    case NNAB_CQ1992_SIMT: r = NNAB_STFT_SIMT; break;
+  }
+  if (r >= 0) g_stft_routes[r].fetch_add(1, std::memory_order_relaxed);
+  if (routes[1] >= 0) g_stft_routes[routes[1]].fetch_add(1, std::memory_order_relaxed);
+}
 static std::atomic<int> g_sm_reserve{0};
 int sm_reserve() { return g_sm_reserve.load(std::memory_order_relaxed); }
 
@@ -343,6 +358,10 @@ uint64_t nnab_cqt1992v2_route_count(int route) {
   if (route < 0 || route >= NNAB_CQ1992_ROUTES) return 0;
   return g_cq1992_routes[route].load(std::memory_order_relaxed);
 }
+uint64_t nnab_stft_route_count(int route) {
+  if (route < 0 || route >= NNAB_STFT_ROUTES) return 0;
+  return g_stft_routes[route].load(std::memory_order_relaxed);
+}
 
 int nnab_set_sm_reserve(int n_sms) {
   if (n_sms < 0) n_sms = 0;
@@ -455,13 +474,14 @@ static int stft_args_ok(const float* wcos, const float* wsin, int out_format) {
 
 static int stft_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft, int F,
                     int hop, int out_format, float sqrt_eps, float* out, int64_t T, void* workspace,
-                    size_t ws_bytes, int path, cudaStream_t stream) {
+                    size_t ws_bytes, int path, cudaStream_t stream, int* route = nullptr) {
   FramedProblem p{};
   set_wave(p, w);
   p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
   p.scale = nullptr; p.scale_all = 1.f;
   p.fmt = out_format; p.eps = sqrt_eps; p.power = 1.f; p.out = out; p.T = T;
   p.out_bins = F; p.bin_offset = 0;
+  p.route = route;
   attach_splitk_scratch(p, workspace, ws_bytes);
   return run_framed(p, packed, workspace, ws_bytes, path, stream);
 }
@@ -475,8 +495,11 @@ int nnab_stft_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64
   if (rc) return rc;
   if (out == nullptr || (rc = stft_args_ok(wcos, wsin, out_format))) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  return stft_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
-                  out_format, sqrt_eps, out, T, workspace, ws_bytes, path, (cudaStream_t)stream);
+  int routes[2] = {-1, -1};  // stays -1 when nothing was enqueued
+  rc = stft_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
+                out_format, sqrt_eps, out, T, workspace, ws_bytes, path, (cudaStream_t)stream, &routes[0]);
+  if (rc == NNAB_OK) count_stft_routes(routes);
+  return rc;
 }
 
 // ------------------------------------------------- Mel / Gammatone / MFCC ----
@@ -493,14 +516,44 @@ size_t nnab_filterbank_table_bytes(int F) {
 }
 
 // deterministic tile widths per table buffer (host copy of the device meta words; read at launch time):
-// the one-phase kernel's nb mask and the four-phase kernel's (nb | split << 8)
-struct FbWidth { int nb_mask, poly_tile; };
+// the one-phase kernel's nb mask and the four-phase kernel's (nb | split << 8); dense_ok: the dense kernel's
+// epilogue gives every filter at most two partial sums
+struct FbWidth { int nb_mask, poly_tile; bool dense_ok; };
 static std::mutex g_fbw_mu;
 static std::unordered_map<const void*, FbWidth> g_fb_width;
 static FbWidth fb_width_of(const void* table) {
   std::lock_guard<std::mutex> lk(g_fbw_mu);
   auto it = g_fb_width.find(table);
-  return it == g_fb_width.end() ? FbWidth{0, 0} : it->second;
+  return it == g_fb_width.end() ? FbWidth{0, 0, false} : it->second;
+}
+
+// Replay of the dense kernel's fused-filterbank epilogue (tc_kernels.cu, FMT_FBANK) over the bin axis: each
+// tc_tile_n(F) / 2 bins of an N tile run two running filter sums, and every flush is one fp32 atomic partial sum
+// of that filter.  Two partial sums land on the zeroed output in either order with the same result; three do not.
+static bool dense_fbank_ok(const std::vector<FbEntry>& tab, int n_fb, int F) {
+  const int half = tc_tile_n(F) / 2;
+  std::vector<int> sums(n_fb, 0);
+  for (int f0 = 0; f0 < F; f0 += half) {
+    int c0 = -1, c1 = -1;
+    for (int f = f0; f < F && f < f0 + half; ++f) {
+      const FbEntry& e = tab[f];
+      if (e.j0 != c0) {
+        if (e.j0 == c1) {
+          std::swap(c0, c1);
+        } else {
+          if (c0 >= 0) ++sums[c0];
+          c0 = e.j0;
+        }
+      }
+      if (e.j1 != c1) {
+        if (c1 >= 0) ++sums[c1];
+        c1 = e.j1;
+      }
+    }
+    if (c0 >= 0) ++sums[c0];
+    if (c1 >= 0) ++sums[c1];
+  }
+  return std::all_of(sums.begin(), sums.end(), [](int n) { return n <= 2; });
 }
 
 int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table, int* h_max_nnz,
@@ -517,14 +570,24 @@ int nnab_build_filterbank_table(const float* fb, int n_fb, int F, void* table, i
                             reinterpret_cast<FbStep*>(base + fb_steps_offset(F)), d_meta + 1, s)))
     return rc;
   int h_meta[4] = {0, 0, 0, 0};
+  std::vector<FbEntry> h_table(F);
   NNAB_CUDA_TRY(cudaMemcpyAsync(h_meta, d_meta, sizeof(h_meta), cudaMemcpyDeviceToHost, s));
+  NNAB_CUDA_TRY(cudaMemcpyAsync(h_table.data(), table, (size_t)F * sizeof(FbEntry), cudaMemcpyDeviceToHost, s));
   NNAB_CUDA_TRY(cudaStreamSynchronize(s));
   *h_max_nnz = h_meta[0];
+  const bool dense_ok = dense_fbank_ok(h_table, n_fb, F);
   {
     std::lock_guard<std::mutex> lk(g_fbw_mu);
-    g_fb_width[table] = (n_fb < 32768) ? FbWidth{h_meta[2], h_meta[3]} : FbWidth{0, 0};
+    g_fb_width[table] = (n_fb < 32768) ? FbWidth{h_meta[2], h_meta[3], dense_ok} : FbWidth{0, 0, dense_ok};
   }
   return NNAB_OK;
+}
+
+int nnab_filterbank_table_fuses(const void* table, const void* packed, int n_fft) {
+  if (table == nullptr || packed == nullptr) return 0;
+  if (packed_kind(packed) == PACK_BLOCK) return 1;
+  // the dense kernel's fused epilogue cannot split K: a long basis takes the power spectrogram, which can
+  return (fb_width_of(table).dense_ok && tc_splitk_scratch_bytes(1, 1, 1, n_fft) == 0) ? 1 : 0;
 }
 
 // ---- dense filterbank (Gammatonegram, dense mel banks) on the tensor cores -------------------------
@@ -571,8 +634,12 @@ static size_t filterbank_ws_bytes(int64_t B, int64_t L, int n_fft, int F, int ho
   const int64_t T = frames_of(L, n_fft, hop, pad);
   const bool tc = wants_tc(path, n_fft, hop);
   size_t n = 0;
-  if (!(has_table && tc)) n += power_bytes(B, F, T);  // un-fused: (B,F,T) power spectrogram
-  if (tc) n += tc_workspace_bytes(B, L, n_fft, hop, pad);
+  if (has_table && tc) {
+    n += tc_workspace_bytes(B, L, n_fft, hop, pad);
+  } else {  // un-fused: (B,F,T) power spectrogram, then the contraction's planes and a long basis's split-K scratch
+    n += power_bytes(B, F, T);
+    if (tc) n += align_up(tc_workspace_bytes(B, L, n_fft, hop, pad), 256) + tc_splitk_scratch_bytes(B, F, T, n_fft);
+  }
   if (!has_table && tc) {  // dense bank on the tensor cores: operand planes instead of the fp32 spectrogram
     FbPlanes fp;
     if (fb_planes_layout(B, L, n_fft, F, hop, pad, T, n_fb, &fp) && fp.total > n) n = fp.total;
@@ -588,13 +655,15 @@ size_t nnab_filterbank_workspace_bytes(int64_t B, int64_t L, int n_fft, int F, i
 static int power_spectrogram(const Wave& w, const float* wcos, const float* wsin, const void* packed,
                              int n_fft, int F, int hop, float sqrt_eps,
                              float power, float* P, int64_t T, void* tc_ws, size_t tc_ws_bytes,
-                             int path, cudaStream_t stream) {
+                             int path, cudaStream_t stream, int* route) {
   FramedProblem p{};
   set_wave(p, w);
   p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
   p.scale = nullptr; p.scale_all = 1.f;
   p.fmt = FMT_POWER; p.eps = sqrt_eps; p.power = power; p.out = P; p.T = T;
   p.out_bins = F; p.bin_offset = 0;
+  p.route = route;
+  attach_splitk_scratch(p, tc_ws, tc_ws_bytes);
   return run_framed(p, packed, tc_ws, tc_ws_bytes, path, stream);
 }
 
@@ -616,12 +685,14 @@ static int filterbank_args_ok(const float* wcos, const float* wsin, const float*
 static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft,
                           int F, int hop, float sqrt_eps, float power, const float* fb, int n_fb,
                           const void* fb_table, float* out, int64_t T, void* workspace, size_t ws_bytes, int path,
-                          cudaStream_t s) {
+                          cudaStream_t s, int (*routes)[2] = nullptr) {
   const int64_t B = w.B, L = w.L;
   const int pad = w.pad;
   int rc;
-  bool fused = fused_fbank(path, packed, fb_table, n_fft, hop);
-  if (fused) {
+  int scratch[2];
+  int (&r)[2] = routes != nullptr ? *routes : scratch;
+  // the fused epilogue on a dense basis only when its atomics stay order-independent (nnab_filterbank_table_fuses)
+  if (fused_fbank(path, packed, fb_table, n_fft, hop) && nnab_filterbank_table_fuses(fb_table, packed, n_fft)) {
     FramedProblem p{};
     set_wave(p, w);
     p.w_re = wcos; p.w_im = wsin; p.F = F; p.K = n_fft; p.hop = hop;
@@ -633,14 +704,16 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     const FbWidth fw = fb_width_of(fb_table);
     p.fb_nb_mask = fw.nb_mask;
     p.fb_poly_tile = fw.poly_tile;
+    p.route = &r[0];
     if (tc_supported(p, packed)) {
       const size_t need = tc_workspace_bytes(B, L, n_fft, hop, pad);
       if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
       // the epilogue accumulates filter sums with fp32 atomics: start from zero
       NNAB_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)B * n_fb * T * sizeof(float), s));
-      return run_framed(p, packed, workspace, ws_bytes, NNAB_PATH_TCGEN05, s);
+      if ((rc = run_framed(p, packed, workspace, ws_bytes, NNAB_PATH_TCGEN05, s))) return rc;
+      r[1] = NNAB_STFT_FB_FUSED;
+      return NNAB_OK;
     }
-    fused = false;
   }
   const size_t need = filterbank_ws_bytes(B, L, n_fft, F, hop, pad, n_fb, path, 0);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
@@ -662,6 +735,7 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
     p.fmt = FMT_PLANES; p.eps = sqrt_eps; p.power = power; p.out = reinterpret_cast<float*>(planes); p.T = T;
     p.out_bins = F; p.bin_offset = 0;
     p.planes_stride = plane_stride; p.planes_pitch = fp.kp;
+    p.route = &r[0];
     // 2. rows x bank on the dense kernel: every frame is one "hop" of kp samples
     FramedProblem g{};
     g.x = nullptr; g.B = B; g.L = T * fp.kp; g.x_pitch = T * fp.kp;
@@ -682,15 +756,18 @@ static int filterbank_run(const Wave& w, const float* wcos, const float* wsin, c
         NNAB_CUDA_TRY(cudaMemset2DAsync(planes + written, (size_t)fp.kp * 2, 0, (size_t)(fp.kp - written) * 2,
                                         (size_t)(2 * fp.rows), s));
       if ((rc = run_framed(p, packed, ws, fp.off_planes, NNAB_PATH_TCGEN05, s))) return rc;
-      return run_framed(g, bank, nullptr, 0, NNAB_PATH_TCGEN05, s);
+      if ((rc = run_framed(g, bank, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
+      r[1] = NNAB_STFT_FB_PLANES;
+      return NNAB_OK;
     }
   }
   float* P = (float*)workspace;
   const size_t pb = power_bytes(B, F, T);
   rc = power_spectrogram(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, P, T, (char*)workspace + pb,
-                         ws_bytes - pb, path, s);
-  if (rc) return rc;
-  return launch_filterbank(P, fb, B, F, T, n_fb, out, s);
+                         ws_bytes - pb, path, s, &r[0]);
+  if (rc || (rc = launch_filterbank(P, fb, B, F, T, n_fb, out, s))) return rc;
+  r[1] = NNAB_STFT_FB_GEMM;
+  return NNAB_OK;
 }
 
 int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64_t x_pitch,
@@ -704,9 +781,12 @@ int nnab_stft_filterbank_forward_ex(const void* x, int x_dtype, int64_t B, int64
   if (rc) return rc;
   if (out == nullptr || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  return filterbank_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F,
-                        hop, sqrt_eps, power, fb, n_fb, fb_table, out, T, workspace, ws_bytes, path,
-                        (cudaStream_t)stream);
+  int routes[2] = {-1, -1};
+  rc = filterbank_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
+                      sqrt_eps, power, fb, n_fb, fb_table, out, T, workspace, ws_bytes, path, (cudaStream_t)stream,
+                      &routes);
+  if (rc == NNAB_OK) count_stft_routes(routes);
+  return rc;
 }
 
 static size_t mel_bytes(int64_t B, int n_mels, int64_t T) {
@@ -748,14 +828,15 @@ static int mfcc_args_ok(const float* wcos, const float* wsin, const float* mel_b
 static int mfcc_run(const Wave& w, const float* wcos, const float* wsin, const void* packed, int n_fft, int F,
                     int hop, float sqrt_eps, float power, const float* mel_basis, int n_mels,
                     const void* fb_table, float amin, float ref, float top_db, const float* dct, int n_mfcc,
-                    float* out, int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream) {
+                    float* out, int64_t T, void* workspace, size_t ws_bytes, int path, cudaStream_t stream,
+                    int (*routes)[2] = nullptr) {
   const size_t need = mfcc_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
   const size_t fbw = align_up(filterbank_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path, 0), 256);
   float* mel = (float*)((char*)workspace + fbw);
   unsigned int* scratch = (unsigned int*)((char*)workspace + fbw + mel_bytes(w.B, n_mels, T));
   int rc = filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table,
-                          mel, T, workspace, fbw, path, stream);
+                          mel, T, workspace, fbw, path, stream, routes);
   if (rc) return rc;
   return launch_mfcc_tail(mel, w.B, n_mels, T, amin, ref, top_db, dct, n_mfcc, out, scratch, stream);
 }
@@ -771,9 +852,12 @@ int nnab_mfcc_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, int64
   if (rc) return rc;
   if (out == nullptr || mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin)) return NNAB_EINVAL;
   if ((rc = check_arch())) return rc;
-  return mfcc_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
-                  sqrt_eps, power, mel_basis, n_mels, fb_table, amin, ref, top_db, dct, n_mfcc, out, T, workspace,
-                  ws_bytes, path, (cudaStream_t)stream);
+  int routes[2] = {-1, -1};
+  rc = mfcc_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, wcos, wsin, packed, n_fft, F, hop,
+                sqrt_eps, power, mel_basis, n_mels, fb_table, amin, ref, top_db, dct, n_mfcc, out, T, workspace,
+                ws_bytes, path, (cudaStream_t)stream, &routes);
+  if (rc == NNAB_OK) count_stft_routes(routes);
+  return rc;
 }
 
 // ------------------------------------------------------------- CQT1992v2 ----

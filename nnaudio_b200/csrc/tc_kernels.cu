@@ -38,14 +38,16 @@ namespace nnab {
 constexpr int TC_MAX_N_TILES = 128;
 
 
-// N tile (columns = re + im rows of bn/2 bins): minimise padded columns.
+// N tile (columns = re + im rows of bn/2 bins): minimise padded columns among the widths that need at most
+// TC_MAX_N_TILES tiles (256 when none does: tc_supported then refuses the basis).
 static int choose_bn(int F) {
   const int cols = 2 * F;
   if (cols <= 256) return round_up_i(cols, 16) < 32 ? 32 : round_up_i(cols, 16);
   int best = 256, best_total = round_up_i(cols, 256);
   for (int bn = 240; bn >= 128; bn -= 16) {
-    const int total = (cols + bn - 1) / bn * bn;
-    if (total < best_total) { best_total = total; best = bn; }
+    const int tiles = (cols + bn - 1) / bn;
+    if (tiles > TC_MAX_N_TILES) break;  // narrower widths need more tiles still
+    if (tiles * bn < best_total) { best_total = tiles * bn; best = bn; }
   }
   return best;
 }

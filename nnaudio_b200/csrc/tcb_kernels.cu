@@ -1021,8 +1021,10 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   const int64_t tiles = (int64_t)prm.num_m_tiles * n_tiles;
   const int grid = (int)(tiles < sms ? tiles : sms);
   add_exec_flops(passes * 2.0 * (double)tiles * TC_BM * (2 * nb) * Kb);
-  return poly ? launch_tcb_ph<4>(R, passes, q.fmt, ma, mb, prm, grid, stream)
-              : launch_tcb_ph<1>(R, passes, q.fmt, ma, mb, prm, grid, stream);
+  rc = poly ? launch_tcb_ph<4>(R, passes, q.fmt, ma, mb, prm, grid, stream)
+            : launch_tcb_ph<1>(R, passes, q.fmt, ma, mb, prm, grid, stream);
+  if (rc == NNAB_OK && q.route != nullptr) *q.route = ROUTE_BLOCK;
+  return rc;
 }
 
 }  // namespace nnab

@@ -99,12 +99,15 @@ def fbank_nb(fb, n_fft, hop):
 
 
 def choose_bn(F):
-    """choose_bn (tc_kernels.cu): the dense kernel's N tile for F complex rows."""
+    """choose_bn (tc_kernels.cu): the dense kernel's N tile for F complex rows, the least padded width among those
+    that need at most 128 tiles (TC_MAX_N_TILES; 256 when none does)."""
     cols = 2 * F
     if cols <= 256:
         return max(32, -(-cols // 16) * 16)
     best, best_total = 256, -(-cols // 256) * 256
     for bn in range(240, 127, -16):
+        if -(-cols // bn) > 128:
+            break
         total = -(-cols // bn) * bn
         if total < best_total:
             best, best_total = bn, total

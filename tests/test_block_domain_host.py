@@ -7,6 +7,7 @@ import pytest
 import block_domain as bd
 from block_domain import bp
 from helpers import build, oracle, rel_errors
+from nnaudio_b200 import _C
 from nnaudio_b200.design import gammatone_filterbank, mel_filterbank
 
 # (n_fft, hop, L, center, pad_mode)
@@ -123,10 +124,11 @@ def test_planes_gemm_model():
     assert bd.choose_bn(32) == 64
 
 
-@pytest.mark.parametrize("n_fft,hop", [(24576, 6144), (32768, 8192)])
+@pytest.mark.parametrize("n_fft,hop", [(32768, 16384), (32768, 8192)])
 def test_block_shapes_past_the_dense_kernels_n_tile_limit(n_fft, hop):
-    """The dense kernel takes at most 128 N tiles (TC_MAX_N_TILES); these block shapes need more, so the dispatch
-    must not hold a block-partial basis to that limit (it would run the SIMT kernel instead)."""
+    """The dense kernel takes at most 128 N tiles (TC_MAX_N_TILES); these block shapes need more at any width, so
+    the dispatch must not hold a block-partial basis to that limit (it would run the SIMT kernel instead)."""
+    assert _C.block_layout_ok(n_fft, hop)
     F = n_fft // 2 + 1
     assert -(-(2 * F) // bd.choose_bn(F)) > 128
     assert bp.n_tiles_of(bd.basis_bins(n_fft, hop), bp.choose_nb(bd.basis_bins(n_fft, hop))) <= 35

@@ -1,7 +1,10 @@
 """Run-to-run repeatability of the CUDA path (-m gpu): the reference is deterministic, so every
 forward transform must return bit-identical results when called twice (VERDICT r1 item 5).
 Split-K partial sums are combined by ordered read-modify-writes of one thread, the fused filterbank
-gets at most two partial sums per filter (commutative), nothing else accumulates through atomics."""
+gets at most two partial sums per filter (commutative), nothing else accumulates through atomics.
+The dense kernel fuses a bank only when its tile cut allows that bound (else the un-fused GEMM runs).
+The block-partial kernel's fused Mel keeps it at power 2 with a width the table builder found; a bank
+with no such width, or power != 2, is outside this claim (test_zz_gpu_block_domain.py)."""
 import numpy as np
 import pytest
 import torch
