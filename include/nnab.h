@@ -757,7 +757,7 @@ uint64_t nnab_balanced_launch_count(void);
 /* Routes of nnab_cqt_pyramid_forward(_ex), counted since load so that a test can tell which one a call took.
  * Each counter grows by one per successful enqueue of its stage, inside that entry point only: the plan once
  * per call, an octave route once per octave, a FIR route once per decimation stage (the early stage included).
- * The chunk, pool and device-pool entry points run the same kernels but count nothing. */
+ * The chunk, pool and device-pool entry points run the same kernels and count in nnab_stream_route_count. */
 enum {
   NNAB_PYR_PLAN_GEN2 = 0,         /* one plane set per level, banded FIR stages                         */
   NNAB_PYR_PLAN_GEN1 = 1,         /* early downsampling and any bank width, dense FIR stages             */
@@ -777,7 +777,7 @@ uint64_t nnab_pyramid_route_count(int route);
 
 /* Kernel routes of nnab_cqt1992v2_forward(_ex), counted since load so that a test can tell which one a call took.
  * Each successful call adds one to the counter of the route it enqueued (a dense call once, however many frame
- * phases it launches).  The chunk, pool and device-pool entry points run the same kernels but count nothing. */
+ * phases it launches).  The chunk, pool and device-pool entry points count in nnab_stream_route_count. */
 enum {
   NNAB_CQ1992_TALL = 0,           /* tall-A kernel (8-bin-group bank), static schedule                  */
   NNAB_CQ1992_TALL_BALANCED = 1,  /* tall-A kernel, balanced schedule (nnab_balanced_launch_count)      */
@@ -794,8 +794,8 @@ uint64_t nnab_cqt1992v2_route_count(int route);
 /* Routes of nnab_stft_forward(_ex), nnab_stft_filterbank_forward(_ex) and nnab_mfcc_forward(_ex), counted since
  * load so that a test can tell which one a call took.  Each successful call adds one to the counter of the
  * contraction route it enqueued (a dense call once, however many frame phases it launches); a filterbank or MFCC
- * call also adds one to the counter of its filterbank route.  The chunk, pool and device-pool entry points run the
- * same kernels but count nothing. */
+ * call also adds one to the counter of its filterbank route.  The chunk, pool and device-pool entry points count
+ * in nnab_stream_route_count. */
 enum {
   NNAB_STFT_BLOCK = 0,         /* block-partial kernel (periodic-Hann DFT basis)                         */
   NNAB_STFT_DENSE = 1,         /* dense tensor-core kernel, one launch per frame phase                   */
@@ -808,6 +808,17 @@ enum {
 };
 /* The counter of `route` (an NNAB_STFT_* value); 0 for any other value. */
 uint64_t nnab_stft_route_count(int route);
+
+/* Routes of the streamed calls, counted apart from the offline counters above so that a test can tell which kernels
+ * a push took.  The chunk, pool and device-pool entry points of STFT, filterbank, MFCC and CQT1992v2 count as their
+ * offline calls do (family NNAB_ROUTES_STFT or NNAB_ROUTES_CQ1992, the same route values); the three pyramid stream
+ * calls count the plan once per push, an octave route per octave and a FIR route per decimation stage they launch
+ * (family NNAB_ROUTES_PYR).  A push counts after it succeeds, and only when it returns frames: a push of no frames, or
+ * one refused with NNAB_EUNSUPPORTED, counts nothing, and no push moves an offline counter.  A device-pool push counts
+ * when it is enqueued; replaying a captured CUDA graph of it counts nothing. */
+enum { NNAB_ROUTES_STFT = 0, NNAB_ROUTES_CQ1992 = 1, NNAB_ROUTES_PYR = 2 };
+/* The stream counter of `route` in `family` (an NNAB_ROUTES_* value); 0 for any other pair. */
+uint64_t nnab_stream_route_count(int family, int route);
 
 #if defined(__GNUC__)
 #pragma GCC visibility pop

@@ -44,6 +44,7 @@ SIGNATURES = {
     "nnab_pyramid_route_count": (c_uint64, [c_int]),
     "nnab_cqt1992v2_route_count": (c_uint64, [c_int]),
     "nnab_stft_route_count": (c_uint64, [c_int]),
+    "nnab_stream_route_count": (c_uint64, [c_int, c_int]),
     "nnab_pack_tile_n": (c_int, [c_int]),
     "nnab_packed_basis_bytes": (c_size_t, [c_int, c_int]),
     "nnab_pack_basis": (c_int, [_P, _P, c_int, c_int, _P, _P]),
@@ -240,7 +241,7 @@ PYR_ROUTES = 11
 
 def pyramid_route_count(route: int) -> int:
     """Stages of the offline CQT pyramid call that took ``route`` (a PYR_* constant) since load; the streaming
-    and pool calls count nothing."""
+    and pool calls count in stream_route_count."""
     return int(lib().nnab_pyramid_route_count(int(route)))
 
 
@@ -252,7 +253,7 @@ CQ1992_ROUTES = 7
 
 def cqt1992v2_route_count(route: int) -> int:
     """Offline CQT1992v2 calls that took kernel route ``route`` (a CQ1992_* constant) since load; the streaming
-    and pool calls count nothing."""
+    and pool calls count in stream_route_count."""
     return int(lib().nnab_cqt1992v2_route_count(int(route)))
 
 
@@ -264,8 +265,19 @@ STFT_ROUTES = 7
 
 def stft_route_count(route: int) -> int:
     """Offline STFT / filterbank / MFCC calls that took route ``route`` (a STFT_* constant) since load; the
-    streaming and pool calls count nothing."""
+    streaming and pool calls count in stream_route_count."""
     return int(lib().nnab_stft_route_count(int(route)))
+
+
+# counter families of nnab_stream_route_count: each takes its offline counterpart's route values
+ROUTES_STFT, ROUTES_CQ1992, ROUTES_PYR = 0, 1, 2
+
+
+def stream_route_count(family: int, route: int) -> int:
+    """Pushes of the chunk, pool and device-pool calls that took ``route`` since load, in ``family`` (ROUTES_STFT
+    with a STFT_* route, ROUTES_CQ1992 with a CQ1992_* route, ROUTES_PYR with a PYR_* route).  Only a successful push
+    that returns frames counts; a replayed CUDA graph counts nothing."""
+    return int(lib().nnab_stream_route_count(int(family), int(route)))
 
 
 def set_sm_reserve(n_sms: int) -> int:

@@ -30,9 +30,13 @@ static std::atomic<uint64_t> g_pyr_routes[NNAB_PYR_ROUTES];
 static void count_route(int route) { g_pyr_routes[route].fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<uint64_t> g_cq1992_routes[NNAB_CQ1992_ROUTES];
 static std::atomic<uint64_t> g_stft_routes[NNAB_STFT_ROUTES];
+// the same routes, counted by the chunk, pool and device-pool entry points (nnab_stream_route_count)
+static std::atomic<uint64_t> g_stream_stft[NNAB_STFT_ROUTES];
+static std::atomic<uint64_t> g_stream_cq1992[NNAB_CQ1992_ROUTES];
+static std::atomic<uint64_t> g_stream_pyr[NNAB_PYR_ROUTES];
 // routes[0]: the contraction's kernel route (NNAB_CQ1992_* / ROUTE_BLOCK, as the launchers write it); routes[1]:
 // the filterbank route (NNAB_STFT_FB_*), or -1
-static void count_stft_routes(const int (&routes)[2]) {
+static void count_stft_routes(const int (&routes)[2], std::atomic<uint64_t>* counters = g_stft_routes) {
   int r = -1;
   switch (routes[0]) {
     case ROUTE_BLOCK: r = NNAB_STFT_BLOCK; break;
@@ -40,8 +44,11 @@ static void count_stft_routes(const int (&routes)[2]) {
     case NNAB_CQ1992_DENSE_SPLITK: r = NNAB_STFT_DENSE_SPLITK; break;
     case NNAB_CQ1992_SIMT: r = NNAB_STFT_SIMT; break;
   }
-  if (r >= 0) g_stft_routes[r].fetch_add(1, std::memory_order_relaxed);
-  if (routes[1] >= 0) g_stft_routes[routes[1]].fetch_add(1, std::memory_order_relaxed);
+  if (r >= 0) counters[r].fetch_add(1, std::memory_order_relaxed);
+  if (routes[1] >= 0) counters[routes[1]].fetch_add(1, std::memory_order_relaxed);
+}
+static void count_cq1992_route(int route, std::atomic<uint64_t>* counters) {
+  if (route >= 0) counters[route].fetch_add(1, std::memory_order_relaxed);
 }
 static std::atomic<int> g_sm_reserve{0};
 int sm_reserve() { return g_sm_reserve.load(std::memory_order_relaxed); }
@@ -361,6 +368,17 @@ uint64_t nnab_cqt1992v2_route_count(int route) {
 uint64_t nnab_stft_route_count(int route) {
   if (route < 0 || route >= NNAB_STFT_ROUTES) return 0;
   return g_stft_routes[route].load(std::memory_order_relaxed);
+}
+uint64_t nnab_stream_route_count(int family, int route) {
+  switch (family) {
+    case NNAB_ROUTES_STFT:
+      return route < 0 || route >= NNAB_STFT_ROUTES ? 0 : g_stream_stft[route].load(std::memory_order_relaxed);
+    case NNAB_ROUTES_CQ1992:
+      return route < 0 || route >= NNAB_CQ1992_ROUTES ? 0 : g_stream_cq1992[route].load(std::memory_order_relaxed);
+    case NNAB_ROUTES_PYR:
+      return route < 0 || route >= NNAB_PYR_ROUTES ? 0 : g_stream_pyr[route].load(std::memory_order_relaxed);
+  }
+  return 0;
 }
 
 int nnab_set_sm_reserve(int n_sms) {
@@ -922,7 +940,7 @@ int nnab_cqt1992v2_forward_ex(const void* x, int x_dtype, int64_t B, int64_t L, 
   rc = cqt1992v2_run(Wave{x, x_dtype, B, L, x_pitch, pad, pad_mode, nullptr}, k_real, k_imag, packed, h_k_begin,
                      h_k_end, n_bins, width, hop, scale, scale_all, out_format, sqrt_eps, out, T, workspace,
                      ws_bytes, path, (cudaStream_t)stream, &route);
-  if (rc == NNAB_OK && route >= 0) g_cq1992_routes[route].fetch_add(1, std::memory_order_relaxed);
+  if (rc == NNAB_OK) count_cq1992_route(route, g_cq1992_routes);
   return rc;
 }
 
@@ -1727,7 +1745,8 @@ static bool pyr_packed_ok(int n_octaves, const void* const* h_packed, const void
 // rows, T_max frames each), its FIR stage (on the n_lanes rows) and its carry, then the mask.  `table` holds the
 // (signal, lane) descriptors, which the plan launch(es) have written before pass 1.  Pass 0 checks every launch
 // against the kernels' limits on the host (as the whole-clip plan selection does) and enqueues nothing, so a push
-// that cannot run returns before anything is enqueued; pass 1 runs them.
+// that cannot run returns before anything is enqueued; pass 1 runs them, and a push that returns frames then counts
+// its routes as pyramid_fused2 / pyramid_fused count the whole clip's (nnab_stream_route_count).
 static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const PyramidCall& c, float* ring,
                         const void* chunk, int chunk_dtype, int64_t slots, int64_t chunk_pitch, int64_t n_lanes,
                         PyrLaneSig* table, char* ws, int pass) {
@@ -1735,6 +1754,8 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
   const cudaStream_t s = c.s;
   char* scratch = ws + pl.scratch;
   int rc;
+  int routes[NNAB_PYR_ROUTES] = {};
+  routes[p.gen2 ? NNAB_PYR_PLAN_GEN2 : NNAB_PYR_PLAN_GEN1] = 1;
   for (int sg = 0; sg < p.n_sig; ++sg) {
     ChunkSource cs{};
     cs.ring = ring + (size_t)slots * p.ring_off[sg];
@@ -1773,11 +1794,14 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
             rc = run_framed(qp, c.packed[l], nullptr, 0, NNAB_PATH_TCGEN05, s);
           }
           if (rc) return rc;
+          ++routes[oct ? NNAB_PYR_OCT_KERNEL : NNAB_PYR_OCT_DENSE_PLANES];
         }
       } else if (pass == 0) {
         if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
       } else if ((rc = run_framed(q, c.packed[l], scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
         return rc;
+      } else {
+        ++routes[NNAB_PYR_OCT_DENSE_FP32];
       }
     }
     if (sg + 1 < p.n_sig && pl.len_out[sg] > 0) {
@@ -1800,6 +1824,7 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
           if ((rc = launch_fir_stage_tc(scratch, n_lanes, 0, pitch, plane, FIR_OFF, fir_packed, c.lowpass,
                                         FIR_TAPS, dec, s, cf.rows)))
             return rc;
+          ++routes[NNAB_PYR_FIR_BANDED];
         }
       } else {
         FramedProblem q{};
@@ -1813,6 +1838,8 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
           if (!tc_supported(q)) return NNAB_EUNSUPPORTED;
         } else if ((rc = run_framed(q, fir_packed, scratch, pl.scratch_bytes, NNAB_PATH_TCGEN05, s))) {
           return rc;
+        } else {
+          ++routes[NNAB_PYR_FIR_DENSE];
         }
       }
     }
@@ -1821,7 +1848,11 @@ static int pyr_pool_run(const PyrStream& p, const PyrPoolPlan& pl, const Pyramid
   }
   if (pass == 0) return NNAB_OK;
   // frames t >= a row's count were computed from the zeros past its stream: exact zeros
-  return tc_rows_mask(table, A, c.out, c.n_bins, T_max, format_cols(c.out_format), s);
+  if ((rc = tc_rows_mask(table, A, c.out, c.n_bins, T_max, format_cols(c.out_format), s))) return rc;
+  if (A > 0 && T_max > 0)
+    for (int r = 0; r < NNAB_PYR_ROUTES; ++r)
+      if (routes[r]) g_stream_pyr[r].fetch_add(routes[r], std::memory_order_relaxed);
+  return NNAB_OK;
 }
 
 int nnab_cqt_pyramid_pool_forward(void* state, const nnab_stream_lane* lanes, const nnab_stream_lane* d_lanes,
@@ -2332,6 +2363,7 @@ static int istft_pool_run(float* carry, const nnab_istft_lane* d_lanes, const nn
     p.out = ola + lead; p.T = T_max; p.out_bins = n_fft; p.bin_offset = 0;
     p.presplit = planes;
     p.ola_pitch = ola_pitch; p.ola_hop = hop;
+    p.k_splits_hint = TC_OLA_MAX_SPLITS;  // K chunks of nnab_istft_forward: <= 4096 products per fp32 accumulator
     if ((rc = run_framed(p, packed, nullptr, 0, NNAB_PATH_TCGEN05, s))) return rc;
   }
   // 3. every lane's final samples / window sum-square (rows i < A of out, zeros up to n_max), its tail carried
@@ -2527,9 +2559,13 @@ int nnab_stft_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
   if (rc) return rc;
   if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, B, out, F, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
-    return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
+  int routes[2] = {-1, -1};  // stays -1 when nothing was enqueued
+  rc = pool_forward(pp, chunk_dtype, B, out, F, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
+    return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T, workspace,
+                    ws_bytes, path, s, &routes[0]);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_filterbank_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
@@ -2552,10 +2588,13 @@ int nnab_stft_filterbank_chunk_forward(void* state, int64_t received, int64_t n_
   if (rc) return rc;
   if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, B, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = pool_forward(pp, chunk_dtype, B, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
     return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T,
-                          workspace, ws_bytes, path, s);
+                          workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_mfcc_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
@@ -2580,10 +2619,13 @@ int nnab_mfcc_chunk_forward(void* state, int64_t received, int64_t n_carry, int6
   if (T != pp.T_max || F <= 0 || (T > 0 && out == nullptr) || top_db >= 0.f ||
       mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, B, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = pool_forward(pp, chunk_dtype, B, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
     return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
-                    ref, top_db, dct, n_mfcc, out, T, workspace, ws_bytes, path, s);
+                    ref, top_db, dct, n_mfcc, out, T, workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_cqt1992v2_chunk_workspace_bytes(int64_t B, int64_t received, int64_t frames, int64_t n, int flush,
@@ -2605,10 +2647,13 @@ int nnab_cqt1992v2_chunk_forward(void* state, int64_t received, int64_t n_carry,
   if (rc) return rc;
   if (T != pp.T_max || n_bins <= 0 || (T > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, B, out, n_bins, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
+  int route = -1;
+  rc = pool_forward(pp, chunk_dtype, B, out, n_bins, format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
-                         out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s);
+                         out_format, sqrt_eps, out, T, workspace, ws_bytes, path, s, &route);
   }, stream);
+  if (rc == NNAB_OK) count_cq1992_route(route, g_stream_cq1992);
+  return rc;
 }
 
 // ------------------------------------------------------------ stream pools ----
@@ -2627,11 +2672,14 @@ int nnab_stft_pool_forward(void* state, const nnab_stream_lane* lanes, const nna
                      center ? n_fft / 2 : 0, pad_mode, T_max, &pp);
   if (rc) return rc;
   if (F <= 0 || (A > 0 && out == nullptr) || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, n_lanes, out, F, format_cols(out_format),
+  int routes[2] = {-1, -1};  // stays -1 when nothing was enqueued
+  rc = pool_forward(pp, chunk_dtype, n_lanes, out, F, format_cols(out_format),
                       [&](const Wave& w, cudaStream_t s) {
     return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T_max, workspace, ws_bytes,
-                    path, s);
+                    path, s, &routes[0]);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_filterbank_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_fb,
@@ -2652,10 +2700,13 @@ int nnab_stft_filterbank_pool_forward(void* state, const nnab_stream_lane* lanes
                      center ? n_fft / 2 : 0, pad_mode, T_max, &pp);
   if (rc) return rc;
   if (F <= 0 || (A > 0 && out == nullptr) || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, n_lanes, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = pool_forward(pp, chunk_dtype, n_lanes, out, n_fb, 1, [&](const Wave& w, cudaStream_t s) {
     return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T_max,
-                          workspace, ws_bytes, path, s);
+                          workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_mfcc_pool_workspace_bytes(int64_t A, int64_t T_max, int n_fft, int F, int hop, int n_mels, int path,
@@ -2680,10 +2731,13 @@ int nnab_mfcc_pool_forward(void* state, const nnab_stream_lane* lanes, const nna
   if (F <= 0 || (A > 0 && out == nullptr) || top_db >= 0.f ||
       mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, n_lanes, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = pool_forward(pp, chunk_dtype, n_lanes, out, n_mfcc, 1, [&](const Wave& w, cudaStream_t s) {
     return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
-                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s);
+                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 size_t nnab_cqt1992v2_pool_workspace_bytes(int64_t A, int64_t T_max, int width, int n_bins, int hop, int path) {
@@ -2704,11 +2758,14 @@ int nnab_cqt1992v2_pool_forward(void* state, const nnab_stream_lane* lanes, cons
   if (rc) return rc;
   if (n_bins <= 0 || (A > 0 && out == nullptr) || cqt1992v2_args_ok(k_real, k_imag, out_format))
     return NNAB_EINVAL;
-  return pool_forward(pp, chunk_dtype, n_lanes, out, n_bins, format_cols(out_format),
+  int route = -1;
+  rc = pool_forward(pp, chunk_dtype, n_lanes, out, n_bins, format_cols(out_format),
                       [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
-                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s);
+                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s, &route);
   }, stream);
+  if (rc == NNAB_OK) count_cq1992_route(route, g_stream_cq1992);
+  return rc;
 }
 
 // ------------------------------------------------------------ device pools ----
@@ -2734,11 +2791,14 @@ int nnab_stft_pool_device_forward(void* state, int64_t* counters, const int32_t*
                             slots, n, chunk_pitch, n_fft, hop, center ? n_fft / 2 : 0, pad_mode, T_max, out, &pp);
   if (rc) return rc;
   if (F <= 0 || stft_args_ok(wcos, wsin, out_format)) return NNAB_EINVAL;
-  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, F,
-                             format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};  // stays -1 when nothing was enqueued
+  rc = device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, F,
+                           format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return stft_run(w, wcos, wsin, packed, n_fft, F, hop, out_format, sqrt_eps, out, T_max, workspace, ws_bytes,
-                    path, s);
+                    path, s, &routes[0]);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 int nnab_stft_filterbank_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths,
@@ -2754,11 +2814,14 @@ int nnab_stft_filterbank_pool_device_forward(void* state, int64_t* counters, con
                             slots, n, chunk_pitch, n_fft, hop, center ? n_fft / 2 : 0, pad_mode, T_max, out, &pp);
   if (rc) return rc;
   if (F <= 0 || filterbank_args_ok(wcos, wsin, fb, n_fb)) return NNAB_EINVAL;
-  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_fb, 1,
-                             [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_fb, 1,
+                           [&](const Wave& w, cudaStream_t s) {
     return filterbank_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, fb, n_fb, fb_table, out, T_max,
-                          workspace, ws_bytes, path, s);
+                          workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 int nnab_mfcc_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
@@ -2775,11 +2838,14 @@ int nnab_mfcc_pool_device_forward(void* state, int64_t* counters, const int32_t*
   if (rc) return rc;
   // the top_db floor is a maximum over the whole clip: a stream cannot apply it frame by frame
   if (F <= 0 || top_db >= 0.f || mfcc_args_ok(wcos, wsin, mel_basis, n_mels, dct, n_mfcc, amin)) return NNAB_EINVAL;
-  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_mfcc, 1,
-                             [&](const Wave& w, cudaStream_t s) {
+  int routes[2] = {-1, -1};
+  rc = device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_mfcc, 1,
+                           [&](const Wave& w, cudaStream_t s) {
     return mfcc_run(w, wcos, wsin, packed, n_fft, F, hop, sqrt_eps, power, mel_basis, n_mels, fb_table, amin,
-                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s);
+                    ref, top_db, dct, n_mfcc, out, T_max, workspace, ws_bytes, path, s, &routes);
   }, stream);
+  if (rc == NNAB_OK) count_stft_routes(routes, g_stream_stft);
+  return rc;
 }
 
 int nnab_cqt1992v2_pool_device_forward(void* state, int64_t* counters, const int32_t* lengths, const uint8_t* end,
@@ -2795,11 +2861,14 @@ int nnab_cqt1992v2_pool_device_forward(void* state, int64_t* counters, const int
                             slots, n, chunk_pitch, width, hop, center ? width / 2 : 0, pad_mode, T_max, out, &pp);
   if (rc) return rc;
   if (n_bins <= 0 || cqt1992v2_args_ok(k_real, k_imag, out_format)) return NNAB_EINVAL;
-  return device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_bins,
-                             format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
+  int route = -1;
+  rc = device_pool_forward(pp, counters, lengths, end, errors, error_info, counts, chunk_dtype, n, out, n_bins,
+                           format_cols(out_format), [&](const Wave& w, cudaStream_t s) {
     return cqt1992v2_run(w, k_real, k_imag, packed, h_k_begin, h_k_end, n_bins, width, hop, scale, scale_all,
-                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s);
+                         out_format, sqrt_eps, out, T_max, workspace, ws_bytes, path, s, &route);
   }, stream);
+  if (rc == NNAB_OK) count_cq1992_route(route, g_stream_cq1992);
+  return rc;
 }
 
 }  // extern "C"

@@ -309,9 +309,10 @@ def row_options(name):
     return dict(DEFAULT_OPTS, **ROWS[name][4])
 
 
-def row_geometry(name):
-    """(K, F, hop, center, pad_mode, block, trainable) of a row, from its constructor alone (no basis built)."""
-    cls, ctor = ROWS[name][:2]
+def row_geometry(name, row=None):
+    """(K, F, hop, center, pad_mode, block, trainable) of a row (``row``: a row of this layout kept elsewhere), from
+    its constructor alone (no basis built)."""
+    cls, ctor = (row or ROWS[name])[:2]
     K, hop = ctor["n_fft"], ctor["hop_length"]
     F = ctor.get("freq_bins") or K // 2 + 1
     trainable = bool(ctor.get("trainable", False))
