@@ -160,7 +160,10 @@ class _CFPBase(nn.Module):
 
     # ---- the three contractions ---------------------------------------------------------------
     def _stft_magnitude(self, x: torch.Tensor) -> torch.Tensor:
-        """``|STFT| / |h|`` for bins 0 .. N/2 -> (B, N//2 + 1, T), T = L // hop + 1 (cfp.py:138-150)."""
+        """``|STFT| / |h|`` for bins 0 .. N/2 -> (B, N//2 + 1, T) (cfp.py:138-150), with torch.stft's frame count
+        ``T = (L + 2 (N // 2) - N) // hop + 1``: ``L // hop + 1`` for even N, ``(L - 1) // hop + 1`` for odd N.  The
+        kernel's even ``K``-tap bank frames ``L // hop + 1`` times, so for odd N and ``L % hop == 0`` its last frame
+        (one the reference does not have) is dropped."""
         h = self.h.detach()
         _C._dev_f32(h, "h")
         N, W, H = self.N, int(self.window_size), self._half()
@@ -180,8 +183,9 @@ class _CFPBase(nn.Module):
 
         key = (h.data_ptr(), h._version, N, W)
         w_re, w_im, packed = self._stft_bank.lookup(h.device, key, build, keep=(h,))
-        return _C.cqt1992v2_forward(x, w_re, w_im, packed, None, None, int(self.hop_length), True,
-                                    _C.PAD_CONSTANT, None, 1.0, _C.FMT_MAGNITUDE, 0.0)
+        y = _C.cqt1992v2_forward(x, w_re, w_im, packed, None, None, int(self.hop_length), True,
+                                 _C.PAD_CONSTANT, None, 1.0, _C.FMT_MAGNITUDE, 0.0)
+        return y[:, :, :(x.shape[-1] + 2 * (N // 2) - N) // int(self.hop_length) + 1]
 
     def _cos_matrix(self, device) -> torch.Tensor:
         N, H = self.N, self._half()

@@ -560,7 +560,7 @@ def cfp(x, h, freq2logfreq, quef2logfreq, N, hop, g, tc_idx, fc_idx, high_freq, 
     win = np.zeros(N, dtype=dtype)
     left = (N - W) // 2
     win[left:left + W] = h
-    T = 1 + L // hop
+    T = 1 + (L + 2 * (N // 2) - N) // hop  # torch.stft's count: one fewer than L // hop + 1 for odd N, L % hop == 0
     idx = np.arange(T)[:, None] * hop + np.arange(N)[None, :]
     spec_c = np.fft.fft(xp[:, idx] * win, axis=-1)                   # (B, T, N)
     tfr0 = (np.abs(spec_c) / np.linalg.norm(h)).astype(dtype)
