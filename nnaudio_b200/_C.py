@@ -408,6 +408,12 @@ def _batch_chunked(fn):
     return wrapper
 
 
+def _batch_starts(B: int):
+    """First clip of each C call of a ``B``-clip batch (the training and inverse wrappers split like
+    ``_batch_chunked``)."""
+    return range(0, B, MAX_BATCH)
+
+
 def _as_rows(x: torch.Tensor):
     if x.dim() != 2:
         raise ValueError("internal: expected (B, L)")
@@ -1125,6 +1131,9 @@ def pack_istft_basis(kernel_cos: torch.Tensor, kernel_sin: torch.Tensor, f_in: i
 
 def istft_forward(X, packed, window, n_fft, hop, center, length):
     """X (B, f_in, T, 2) fp32 CUDA -> waveform (B, out_len)."""
+    if X.dim() == 4 and X.shape[0] > MAX_BATCH:
+        return torch.cat([istft_forward(X[i:i + MAX_BATCH], packed, window, n_fft, hop, center, length)
+                          for i in _batch_starts(X.shape[0])], 0)
     L = lib()
     X = _dev_f32(X, "X")
     X = X if X.is_contiguous() else X.contiguous()
@@ -1146,6 +1155,8 @@ def istft_forward(X, packed, window, n_fft, hop, center, length):
 
 def fir_decimate(x, fir, factor):
     """EXPERIMENTAL: y = conv1d(x, fir, stride=factor, padding=(taps-1)//2) for (B, L) rows."""
+    if x.dim() == 2 and x.shape[0] > MAX_BATCH:
+        return torch.cat([fir_decimate(x[i:i + MAX_BATCH], fir, factor) for i in _batch_starts(x.shape[0])], 0)
     L = lib()
     x, B, Ln, pitch = _rows(x)
     fir = _dev_f32(fir, "fir").reshape(-1).contiguous()
@@ -1161,6 +1172,9 @@ def fir_decimate(x, fir, factor):
 
 def fir_decimate_adjoint(g, fir, factor, L_in):
     """EXPERIMENTAL: gradient of fir_decimate w.r.t. its input, (B, Ly) -> (B, L_in)."""
+    if g.dim() == 2 and g.shape[0] > MAX_BATCH:
+        return torch.cat([fir_decimate_adjoint(g[i:i + MAX_BATCH], fir, factor, L_in)
+                          for i in _batch_starts(g.shape[0])], 0)
     L = lib()
     g, B, Ly, pitch = _rows(g)
     fir = _dev_f32(fir, "fir").reshape(-1).contiguous()
@@ -1185,6 +1199,9 @@ def pack_adjoint_basis(w_re: torch.Tensor, w_im: torch.Tensor):
 
 def framed_backward_input(g, packed_adj, K, hop, center, pad_mode, L_in):
     """g (B, F, T, 2) -> dx (B, L_in)."""
+    if g.dim() == 4 and g.shape[0] > MAX_BATCH:
+        return torch.cat([framed_backward_input(g[i:i + MAX_BATCH], packed_adj, K, hop, center, pad_mode, L_in)
+                          for i in _batch_starts(g.shape[0])], 0)
     L = lib()
     g = _dev_f32(g, "grad")
     g = g if g.is_contiguous() else g.contiguous()
@@ -1201,7 +1218,14 @@ def framed_backward_input(g, packed_adj, K, hop, center, pad_mode, L_in):
 
 
 def framed_backward_weight(g, x, K, hop, center, pad_mode):
-    """g (B, F, T, 2), x (B, L) -> (d w_re, d w_im), each (F, K)."""
+    """g (B, F, T, 2), x (B, L) -> (d w_re, d w_im), each (F, K).  The clips are the GEMM's K, so a batch of
+    more than ``MAX_BATCH`` clips is the sum of its chunks' gradients, added in chunk order."""
+    if g.dim() == 4 and g.shape[0] > MAX_BATCH:
+        d_re = d_im = None
+        for i in _batch_starts(g.shape[0]):
+            r, m = framed_backward_weight(g[i:i + MAX_BATCH], x[i:i + MAX_BATCH], K, hop, center, pad_mode)
+            d_re, d_im = (r, m) if d_re is None else (d_re + r, d_im + m)
+        return d_re, d_im
     L = lib()
     g = _dev_f32(g, "grad")
     g = g if g.is_contiguous() else g.contiguous()
