@@ -753,6 +753,10 @@ int nnab_profile_read_exec_flops(double* exec_flops);
 /* Launches of the tall-A CQT kernel that ran the balanced schedule (tiles shared between two
  * CTAs, framed_tct_kernel<., true>) since load -- lets a test tell which schedule it exercised. */
 uint64_t nnab_balanced_launch_count(void);
+/* Launches of the block-partial STFT kernel that ran with separate MMA and epilogue warps
+ * (framed_tcb_ws_kernel: four phases, fused filterbank or operand planes, nb <= 88) since load.  The
+ * plain four-phase kernel executes the same MMA flops at the same width; this tells the two apart. */
+uint64_t nnab_block_ws_launch_count(void);
 
 /* Routes of nnab_cqt_pyramid_forward(_ex), counted since load so that a test can tell which one a call took.
  * Each counter grows by one per successful enqueue of its stage, inside that entry point only: the plan once

@@ -41,6 +41,7 @@ SIGNATURES = {
     "nnab_profile_read": (c_int, [_P, _P]),
     "nnab_profile_read_exec_flops": (c_int, [_P]),
     "nnab_balanced_launch_count": (c_uint64, []),
+    "nnab_block_ws_launch_count": (c_uint64, []),
     "nnab_pyramid_route_count": (c_uint64, [c_int]),
     "nnab_cqt1992v2_route_count": (c_uint64, [c_int]),
     "nnab_stft_route_count": (c_uint64, [c_int]),
@@ -231,6 +232,12 @@ def launch_count() -> int:
 def balanced_launch_count() -> int:
     """Tall-A CQT launches that ran the balanced (shared-tile) schedule since load."""
     return int(lib().nnab_balanced_launch_count())
+
+
+def block_ws_launch_count() -> int:
+    """Block-partial STFT launches that ran the warp-specialised kernel (separate MMA and epilogue warps) since
+    load."""
+    return int(lib().nnab_block_ws_launch_count())
 
 
 # routes of nnab_cqt_pyramid_forward (NNAB_PYR_*): the plan, each octave's kernel, each FIR stage's kernel

@@ -14,6 +14,7 @@ void set_cuda_error(const char* where, cudaError_t e);
 void set_error_text(const char* text);
 void count_launch();
 void count_balanced_launch();
+void count_block_ws_launch();
 int sm_reserve();
 // tensor-pipe accounting for bench.py: MMA flops a tensor-core launch EXECUTES (all split terms,
 // tile padding and structural zeros included); summed while nnab_profile_enable(1)
@@ -730,6 +731,8 @@ int launch_filterbank(const float* P, const float* fb, int64_t B, int F, int64_t
                       float* out, cudaStream_t stream);
 int launch_fb_tile_bank(const float* fb, int n_fb, int F, int nb, int n_tiles, int phases, int kp, int fh, float* w_re,
                         float* w_im, cudaStream_t stream);
+// clip_max_kernel puts one clip on each blockIdx.y
+constexpr int64_t MFCC_MAX_CLIPS = 65535;
 int launch_mfcc_tail(const float* mel, int64_t B, int n_mels, int64_t T, float amin, float ref,
                      float top_db, const float* dct, int n_mfcc, float* out,
                      unsigned int* scratch /* B words */, cudaStream_t stream);

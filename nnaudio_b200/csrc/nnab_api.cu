@@ -19,6 +19,7 @@ namespace nnab {
 static thread_local char g_err[512] = "";
 static std::atomic<uint64_t> g_launches{0};
 static std::atomic<uint64_t> g_balanced_launches{0};
+static std::atomic<uint64_t> g_block_ws_launches{0};
 
 void set_cuda_error(const char* where, cudaError_t e) {
   snprintf(g_err, sizeof(g_err), "%s: %s (%s)", where, cudaGetErrorName(e), cudaGetErrorString(e));
@@ -26,6 +27,7 @@ void set_cuda_error(const char* where, cudaError_t e) {
 void set_error_text(const char* text) { snprintf(g_err, sizeof(g_err), "%s", text); }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 void count_balanced_launch() { g_balanced_launches.fetch_add(1, std::memory_order_relaxed); }
+void count_block_ws_launch() { g_block_ws_launches.fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<uint64_t> g_pyr_routes[NNAB_PYR_ROUTES];
 static void count_route(int route) { g_pyr_routes[route].fetch_add(1, std::memory_order_relaxed); }
 static std::atomic<uint64_t> g_cq1992_routes[NNAB_CQ1992_ROUTES];
@@ -357,6 +359,7 @@ const char* nnab_last_cuda_error(void) { return g_err; }
 uint64_t nnab_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 uint64_t nnab_balanced_launch_count(void) { return g_balanced_launches.load(std::memory_order_relaxed); }
+uint64_t nnab_block_ws_launch_count(void) { return g_block_ws_launches.load(std::memory_order_relaxed); }
 uint64_t nnab_pyramid_route_count(int route) {
   if (route < 0 || route >= NNAB_PYR_ROUTES) return 0;
   return g_pyr_routes[route].load(std::memory_order_relaxed);
@@ -850,6 +853,7 @@ static int mfcc_run(const Wave& w, const float* wcos, const float* wsin, const v
                     int (*routes)[2] = nullptr) {
   const size_t need = mfcc_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path);
   if (workspace == nullptr || ws_bytes < need) return NNAB_EWORKSPACE;
+  if (w.B > MFCC_MAX_CLIPS) return NNAB_EUNSUPPORTED;  // refused before the mel stage is enqueued
   const size_t fbw = align_up(filterbank_ws_bytes(w.B, w.L, n_fft, F, hop, w.pad, n_mels, path, 0), 256);
   float* mel = (float*)((char*)workspace + fbw);
   unsigned int* scratch = (unsigned int*)((char*)workspace + fbw + mel_bytes(w.B, n_mels, T));

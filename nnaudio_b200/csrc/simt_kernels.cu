@@ -459,66 +459,78 @@ __global__ void __launch_bounds__(256) clip_max_kernel(const float* __restrict__
 }
 
 constexpr int MFCC_CHUNK = 32;
+// mel rows of DCT coefficients staged in shared memory at a time: 384 x 32 fp32 = 48 KB, the default dynamic
+// shared-memory limit, so any n_mels runs without an opt-in and without a size to refuse
+constexpr int MFCC_MEL_SLICE = 384;
 
 // One thread per (clip, frame), flattened over the batch so every block is full (T = 157 at cfg5
 // would leave 38 % of a per-clip grid idle).  dB through MUFU.LG2 (10 log10 x = 3.0103 log2 x; abs
 // error ~1e-6 dB on a +-100 dB range), DCT rows transposed in shared memory ([mel][coef], float4
-// broadcast reads: 1 LDS.128 per 4 FMAs).  HBM-bound target: read (B, n_mels, T) once, coalesced in t.
+// broadcast reads: 1 LDS.128 per 4 FMAs), one MFCC_MEL_SLICE of mel rows at a time.  Every accumulator
+// still sums the mel rows in order 0 .. n_mels - 1, so the slicing does not change a bit of the result.
+// HBM-bound target: read (B, n_mels, T) once, coalesced in t.
 __global__ void __launch_bounds__(128) mfcc_tail_kernel(const float* __restrict__ S, int n_mels,
                                                         int64_t T, int64_t BT, float amin, float ref_db,
                                                         float top_db,
                                                         const unsigned int* __restrict__ clip_max,
                                                         const float* __restrict__ dct, int n_mfcc,
                                                         int c0, float* __restrict__ out) {
-  extern __shared__ __align__(16) float dsm[];  // [n_mels][MFCC_CHUNK]
+  extern __shared__ __align__(16) float dsm[];  // [min(n_mels, MFCC_MEL_SLICE)][MFCC_CHUNK]
   const int nc = min(MFCC_CHUNK, n_mfcc - c0);
-  for (int i = threadIdx.x; i < n_mels * MFCC_CHUNK; i += blockDim.x) {
-    const int m = i / MFCC_CHUNK, c = i % MFCC_CHUNK;
-    dsm[i] = (c < nc) ? __ldg(dct + (int64_t)(c0 + c) * n_mels + m) : 0.f;
-  }
-  __syncthreads();
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= BT) return;
-  const int64_t b = g / T, t = g - b * T;
+  // threads past the last frame stay to the end: they share in staging every slice and its barriers
+  const bool live = g < BT;
+  const int64_t b = live ? g / T : 0, t = g - b * T;
   const float* __restrict__ Sb = S + b * (int64_t)n_mels * T + t;
   float floor_db = -INFINITY;
-  if (top_db >= 0.f) {
+  if (live && top_db >= 0.f) {
     const float peak = 3.0102999566f * __log2f(__uint_as_float(clip_max[b])) - ref_db;
     floor_db = peak - top_db;
   }
   float acc[MFCC_CHUNK];
 #pragma unroll
   for (int c = 0; c < MFCC_CHUNK; ++c) acc[c] = 0.f;
+  for (int m0 = 0; m0 < n_mels; m0 += MFCC_MEL_SLICE) {
+    const int ms = min(MFCC_MEL_SLICE, n_mels - m0);
+    if (m0 > 0) __syncthreads();  // every thread has finished reading the previous slice
+    for (int i = threadIdx.x; i < ms * MFCC_CHUNK; i += blockDim.x) {
+      const int m = i / MFCC_CHUNK, c = i % MFCC_CHUNK;
+      dsm[i] = (c < nc) ? __ldg(dct + (int64_t)(c0 + c) * n_mels + m0 + m) : 0.f;
+    }
+    __syncthreads();
+    if (!live) continue;
 #pragma unroll 4
-  for (int m = 0; m < n_mels; ++m) {
-    float v = 3.0102999566f * __log2f(fmaxf(__ldg(Sb + (int64_t)m * T), amin)) - ref_db;
-    v = fmaxf(v, floor_db);
-    const float4* w = reinterpret_cast<const float4*>(dsm + m * MFCC_CHUNK);
+    for (int m = 0; m < ms; ++m) {
+      float v = 3.0102999566f * __log2f(fmaxf(__ldg(Sb + (int64_t)(m0 + m) * T), amin)) - ref_db;
+      v = fmaxf(v, floor_db);
+      const float4* w = reinterpret_cast<const float4*>(dsm + m * MFCC_CHUNK);
 #pragma unroll
-    for (int c4 = 0; c4 < MFCC_CHUNK / 4; ++c4) {
-      if (4 * c4 < nc) {  // block-uniform
-        const float4 d = w[c4];
-        acc[4 * c4 + 0] = fmaf(d.x, v, acc[4 * c4 + 0]);
-        acc[4 * c4 + 1] = fmaf(d.y, v, acc[4 * c4 + 1]);
-        acc[4 * c4 + 2] = fmaf(d.z, v, acc[4 * c4 + 2]);
-        acc[4 * c4 + 3] = fmaf(d.w, v, acc[4 * c4 + 3]);
+      for (int c4 = 0; c4 < MFCC_CHUNK / 4; ++c4) {
+        if (4 * c4 < nc) {  // block-uniform
+          const float4 d = w[c4];
+          acc[4 * c4 + 0] = fmaf(d.x, v, acc[4 * c4 + 0]);
+          acc[4 * c4 + 1] = fmaf(d.y, v, acc[4 * c4 + 1]);
+          acc[4 * c4 + 2] = fmaf(d.z, v, acc[4 * c4 + 2]);
+          acc[4 * c4 + 3] = fmaf(d.w, v, acc[4 * c4 + 3]);
+        }
       }
     }
   }
+  if (!live) return;
   float* __restrict__ ob = out + ((int64_t)b * n_mfcc + c0) * T + t;
 #pragma unroll
   for (int c = 0; c < MFCC_CHUNK; ++c)
     if (c < nc) ob[(int64_t)c * T] = acc[c];
 }
 
-// `scratch` holds B uint32 (per-clip max bits), provided by the caller's workspace.
+// `scratch` holds B uint32 (per-clip max bits), provided by the caller's workspace.  B <= MFCC_MAX_CLIPS (the
+// caller checks it before enqueueing the mel stage).
 int launch_mfcc_tail(const float* mel, int64_t B, int n_mels, int64_t T, float amin,
                           float ref, float top_db, const float* dct, int n_mfcc, float* out,
                           unsigned int* scratch, cudaStream_t stream) {
   if (B <= 0 || T <= 0) return NNAB_OK;
-  if (B > 65535) return NNAB_EUNSUPPORTED;
-  const size_t smem = (size_t)MFCC_CHUNK * n_mels * sizeof(float);
-  if (smem > 200 * 1024) return NNAB_EUNSUPPORTED;
+  if (B > MFCC_MAX_CLIPS) return NNAB_EUNSUPPORTED;
+  const size_t smem = (size_t)MFCC_CHUNK * (n_mels < MFCC_MEL_SLICE ? n_mels : MFCC_MEL_SLICE) * sizeof(float);
   const float ref_db = 10.0f * log10f(fmaxf(amin, fabsf(ref)));
   if (top_db >= 0.f) {
     NNAB_CUDA_TRY(cudaMemsetAsync(scratch, 0, (size_t)B * sizeof(unsigned int), stream));
@@ -529,9 +541,6 @@ int launch_mfcc_tail(const float* mel, int64_t B, int n_mels, int64_t T, float a
     clip_max_kernel<<<dim3(gx, (unsigned)B), 256, 0, stream>>>(mel, per_clip, amin, scratch);
     NNAB_LAUNCH_CHECK();
   }
-  if (smem > 48 * 1024)
-    NNAB_CUDA_TRY(cudaFuncSetAttribute(mfcc_tail_kernel,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t BT = B * T;
   for (int c0 = 0; c0 < n_mfcc; c0 += MFCC_CHUNK) {
     mfcc_tail_kernel<<<(unsigned)ceil_div64(BT, 128), 128, smem, stream>>>(

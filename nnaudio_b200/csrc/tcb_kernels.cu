@@ -899,9 +899,11 @@ static int launch_tcb_fmt(const CUtensorMap& ma, const CUtensorMap& mb, const Tc
   if constexpr (WS) {
     const uint32_t extra = FMT == 5 ? TCB_WS_ACT_BYTES : 0;
     q.stages = S::stages(prm.nb, PASSES, extra);
-    return launch_persistent<framed_tcb_ws_kernel<FMT, R, PASSES>>(grid, TCB_WS_THREADS,
-                                                                   S::total(prm.nb, PASSES, extra), S::LIMIT, stream,
-                                                                   ma, mb, q);
+    const int rc = launch_persistent<framed_tcb_ws_kernel<FMT, R, PASSES>>(grid, TCB_WS_THREADS,
+                                                                           S::total(prm.nb, PASSES, extra), S::LIMIT,
+                                                                           stream, ma, mb, q);
+    if (rc == NNAB_OK) count_block_ws_launch();
+    return rc;
   }
   return NNAB_EINVAL;  // (not reached)
 }

@@ -41,6 +41,9 @@ def hann_dft_bases(n_fft):
     return (np.sin(ang) * win)[:, None, :], (np.cos(ang) * win)[:, None, :]
 
 
+WS_NB_MAX = 88  # TCB_WS_NB_MAX: the widest tile framed_tcb_ws_kernel takes
+
+
 def poly4(hop):
     """block_poly4: four polyphase rows per block whenever hop % 128 == 0."""
     return hop % 128 == 0

@@ -142,11 +142,15 @@ def dense_partial_sums(fb, F=None):
     return sums
 
 
-def plan(K, F, hop, B, L, center=True, block=False, path="auto", fb=None, passes=3):
+def plan(K, F, hop, B, L, center=True, block=False, path="auto", fb=None, passes=3, power=2.0, planes=True):
     """Routes and executed flops of one fp32 offline call: an STFT (``fb`` None) or a filterbank / MFCC
     (``fb``: the (n_fb, F) bank) with a K-tap basis of F bins, hop ``hop`` and (B, L) clips.  ``block``: the
-    module packed the block-partial layout; ``passes``: its MMA passes (2 for a bf16 waveform).  Returns a dict with ``routes`` ({STFT_* constant: 1}), ``flops`` and
-    the quantities they were decided on."""
+    module packed the block-partial layout; ``passes``: its MMA passes (2 for a bf16 waveform); ``power``: the
+    exponent of |X|; ``planes``: NNAB_FB_PLANES (a dense bank on a block basis takes the operand planes).
+    Returns a dict with ``routes`` ({STFT_* constant: 1}), ``flops`` and the quantities they were decided on,
+    and for the block-partial launch its tile width ``nb``, ``ws`` (1: it runs framed_tcb_ws_kernel, the
+    four-phase kernel with separate MMA and epilogue warps, else 0) and ``deterministic`` (two calls are bitwise
+    equal)."""
     pad = K // 2 if center else 0
     T = (L + 2 * pad - K) // hop + 1
     n_ph = num_phases(hop)
@@ -156,7 +160,8 @@ def plan(K, F, hop, B, L, center=True, block=False, path="auto", fb=None, passes
     tiles = _ceil(2 * F, bn)
     kpad = _ceil(K, 64) * 64
     p = dict(K=K, F=F, hop=hop, T=T, n_ph=n_ph, hop_eff=hop_eff, rows_mode=int(hop_eff % 64 == 0), bn=bn,
-             n_tiles=tiles, kpad=kpad, t_slots=t_slots, launched=min(n_ph, T), ks=1)
+             n_tiles=tiles, kpad=kpad, t_slots=t_slots, launched=min(n_ph, T), ks=1, nb=None, ws=0,
+             deterministic=True)
     simt = path == "simt"
     dense_tc = not simt and K >= 16 and L + 2 * pad >= K and tiles <= TC_MAX_N_TILES
     block = block and not simt
@@ -164,9 +169,14 @@ def plan(K, F, hop, B, L, center=True, block=False, path="auto", fb=None, passes
     def dense_flops():
         return 6.0 * p["launched"] * _ceil(B * t_slots, TC_BM) * TC_BM * tiles * kpad * bn
 
+    def block_launch(nb, ws_format):
+        """the block-partial launch at width nb; ws_format: a format framed_tcb_ws_kernel serves (FMT 5 / 9)"""
+        p.update(nb=nb, ws=int(ws_format and bd.poly4(hop) and nb <= bd.WS_NB_MAX))
+        return float(bd.block_exec_flops(K, hop, B, L, center, passes, nb=nb))
+
     def contraction(split_ok):
         if block:
-            return _C.STFT_BLOCK, float(bd.block_exec_flops(K, hop, B, L, center, passes))
+            return _C.STFT_BLOCK, block_launch(bd.bp.choose_nb(bd.basis_bins(K, hop)), False)
         if not dense_tc:
             return _C.STFT_SIMT, 0.0
         nkb = kpad // 64
@@ -186,13 +196,16 @@ def plan(K, F, hop, B, L, center=True, block=False, path="auto", fb=None, passes
     # split-K (nnab_filterbank_table_fuses)
     if has_table and not simt and (block or (dense_tc and max(sums) <= 2 and K < SPLITK_MIN_K)):
         r, flops = contraction(split_ok=False)
-        if block:  # the fused launch runs at the table's deterministic width
-            nb, _ = bd.fbank_nb(np.asarray(fb), K, hop)
-            flops = float(bd.block_exec_flops(K, hop, B, L, center, passes, nb=nb))
+        if block:  # the fused launch runs at the table's deterministic width, else at the default one
+            nb, det = bd.fbank_nb(np.asarray(fb), K, hop)
+            flops = block_launch(nb, True)
+            # the rolled MelRun epilogue (power != 2) flushes each warp part's sums on its own: the bound of two
+            # partial sums per filter, and with it run-to-run identical atomics, holds for the fast path only
+            p["deterministic"] = det and power == 2.0
         return dict(p, routes={r: 1, _C.STFT_FB_FUSED: 1}, flops=flops)
-    if block and F == K // 2 + 1:
-        flops = float(bd.block_exec_flops(K, hop, B, L, center, passes) + bd.planes_gemm_flops(K, hop, B, T, n_fb))
-        return dict(p, routes={_C.STFT_BLOCK: 1, _C.STFT_FB_PLANES: 1}, flops=flops)
+    if block and planes and F == K // 2 + 1:
+        flops = block_launch(bd.bp.choose_nb(bd.basis_bins(K, hop)), True) + bd.planes_gemm_flops(K, hop, B, T, n_fb)
+        return dict(p, routes={_C.STFT_BLOCK: 1, _C.STFT_FB_PLANES: 1}, flops=float(flops))
     r, flops = contraction(split_ok=True)  # the power spectrogram splits a long basis like the STFT
     return dict(p, routes={r: 1, _C.STFT_FB_GEMM: 1}, flops=flops)
 
