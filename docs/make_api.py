@@ -66,6 +66,13 @@ attributes as `nnAudio.features` v0.3.3 — checked against the unmodified refer
   and `check()`, so a pyramid tick can be captured in a CUDA graph.  A push never sees the lengths on the host, so it
   cannot issue `module(x)`'s reflect-fallback `UserWarning` for a short stream (DESIGN.md §3.10 "Device pyramid
   pools").
+  `nnaudio_b200.pcen.PCEN(n_channels=None, sr=22050, hop_length=512, time_constant=0.4, s=None, gain=0.98,
+  bias=2.0, power=0.5, eps=1e-6, trainable=False)` is per-channel energy normalisation of a `(B, C, T)` spectrogram:
+  one launch per call, a fused backward for the input and the (scalar or per-channel) parameters, which are buffers
+  or, with `trainable=True`, parameters.  `PCENStream(pcen, slots)` carries each stream's smoother across
+  `step(frames, counts=None, slots=None)` calls on the output of `StreamingTransform`, a `StreamPool` `PoolOutput` or
+  a `DeviceStreamPool`, bit for bit with the whole-clip call, with `reset(restart=None)` on a device mask
+  (DESIGN.md §3.11).
 
 Environment switches: `NNAUDIO_B200_PATH=auto|simt|tc` (kernel family), `NNAB_TALL_BALANCE=0|1` (balanced tile
 schedule of the CQT1992v2 kernel).

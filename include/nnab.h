@@ -731,6 +731,39 @@ int nnab_debug_device_pyramid_plan(int64_t* counters, const int32_t* lengths, co
                                    int64_t n, int n_octaves, const int32_t* widths, int hop, int early_factor,
                                    int pad_mode);
 
+/* Per-channel energy normalisation (PCEN; beyond the reference, DESIGN.md §3.11).  E is a non-negative (B, C, T)
+ * fp32 spectrogram; per row (b, c), with the parameters of channel c:
+ *   M[t] = (1 - s) M[t-1] + s E[t]          M[-1] = E[0]
+ *   P[t] = bias^power expm1(power log1p(E[t] (eps + M[t])^-gain / bias))
+ * The parameters s, gain, bias, power are DEVICE fp32 arrays: param_stride 1 reads element c (C of them),
+ * param_stride 0 element 0 (scalars).  Their values are not checked (0 < s <= 1, gain >= 0, bias > 0, power > 0
+ * are the caller's); eps must be > 0.  Each row is a sequential fp32 recurrence in frame order, so a row split
+ * into several streamed calls gives the same bits as one call.
+ *
+ * nnab_pcen_forward writes P (B, C, T).  Training: M (non-NULL) receives the (B, C, T) smoother output for
+ * nnab_pcen_backward; state must then be NULL.  Streaming: state (slots, C) fp32 and primed (slots, C) uint8
+ * carry each slot's last M; row b belongs to slot row_slot[b] (DEVICE int32, NULL: slot b, then B <= slots) and
+ * advances by counts[b] frames (DEVICE int32, clamped to [0, T]; NULL: T), its P zero past them.  A slot that is
+ * not primed starts from its first frame as the offline call does; a row with frames leaves its slot primed.
+ * Rows must map to distinct slots; a row mapped outside [0, slots) computes nothing.  counts and row_slot need
+ * state.  One launch; T == 0 or B == 0 enqueues nothing. */
+int nnab_pcen_forward(const float* E, int64_t B, int C, int64_t T, const float* s, const float* gain,
+                      const float* bias, const float* power, int param_stride, float eps, float* P, float* M,
+                      float* state, uint8_t* primed, int64_t slots, const int32_t* row_slot, const int32_t* counts,
+                      void* stream);
+/* Workspace of nnab_pcen_backward with grad_params: the per-row parameter partials (4 B C floats). */
+size_t nnab_pcen_workspace_bytes(int64_t B, int C);
+/* Adjoint of the offline call: grad_P (B, C, T) -> grad_E (B, C, T) (NULL: not written) and grad_params (4, n)
+ * with n = C (param_stride 1) or 1, rows in the order s, gain, bias, power (NULL: not computed; otherwise the
+ * workspace is required).  M is the training forward's output.  The parameter sums run in a fixed order (no
+ * atomics): two calls give the same bits.  One launch, plus one for grad_params. */
+int nnab_pcen_backward(const float* E, const float* M, const float* grad_P, int64_t B, int C, int64_t T,
+                       const float* s, const float* gain, const float* bias, const float* power, int param_stride,
+                       float eps, float* grad_E, float* grad_params, void* workspace, size_t ws_bytes, void* stream);
+/* Un-prime the stream slots where mask[s] != 0 (mask NULL: every slot) of a (slots, C) primed array.  One
+ * launch; reads nothing on the host, so it can be captured in a CUDA graph. */
+int nnab_pcen_reset(uint8_t* primed, const uint8_t* mask, int64_t slots, int C, void* stream);
+
 /* Kernel launches issued by this library since load (process wide; used by
  * bench.py for its `gpu_launches` claim). */
 uint64_t nnab_launch_count(void);

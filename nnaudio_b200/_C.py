@@ -1247,3 +1247,59 @@ def framed_backward_weight(g, x, K, hop, center, pad_mode):
                                            _stream(g.device))
     _check_ola(rc, "nnab_framed_backward_weight", K, "kernel width")
     return dw[:F], -dw[F:]
+
+
+# --------------------------------------------------------------------------- #
+# PCEN (nnaudio_b200.pcen): one (B, C, T) spectrogram per call; the parameters are (1,) or (C,) fp32 CUDA tensors
+# --------------------------------------------------------------------------- #
+SIGNATURES["nnab_pcen_forward"] = (
+    c_int, [_P, c_int64, c_int, c_int64, _P, _P, _P, _P, c_int, c_float, _P, _P, _P, _P, c_int64, _P, _P, _P])
+SIGNATURES["nnab_pcen_workspace_bytes"] = (c_size_t, [c_int64, c_int])
+SIGNATURES["nnab_pcen_backward"] = (
+    c_int, [_P, _P, _P, c_int64, c_int, c_int64, _P, _P, _P, _P, c_int, c_float, _P, _P, _P, c_size_t, _P])
+SIGNATURES["nnab_pcen_reset"] = (c_int, [_P, _P, c_int64, c_int, _P])
+
+
+def _pcen_params(params):
+    """(four pointers, parameter stride) of the (s, gain, bias, power) tensors: one value each, or one per channel."""
+    stride = 1 if params[0].numel() > 1 else 0
+    return [_ptr(p) for p in params], stride
+
+
+def pcen_forward(E, params, eps, M=None, stream_state=None, row_slot=None, counts=None):
+    """E (B, C, T) contiguous fp32 CUDA -> P (B, C, T).  ``M``: the training call's (B, C, T) smoother output.
+    ``stream_state``: (state (slots, C) fp32, primed (slots, C) uint8) of a streamed call, with the int32 device
+    ``row_slot`` (B,) / ``counts`` (B,) or None.  Every argument checked by the caller."""
+    B, C, T = E.shape
+    P = _new_out((B, C, T), E.device)
+    (s, gain, bias, power), stride = _pcen_params(params)
+    state, primed = stream_state if stream_state is not None else (None, None)
+    with torch.cuda.device(E.device):
+        rc = lib().nnab_pcen_forward(_ptr(E), B, C, T, s, gain, bias, power, stride, float(eps), _ptr(P), _ptr(M),
+                                     _ptr(state), _ptr(primed), 0 if state is None else state.shape[0],
+                                     _ptr(row_slot), _ptr(counts), _stream(E.device))
+    _check(rc, "nnab_pcen_forward")
+    return P
+
+
+def pcen_backward(E, M, gP, params, eps, want_E=True, want_params=True):
+    """(grad_E (B, C, T) or None, grad_params (4, n) or None) of the training call on E, its M and grad_P;
+    ``n`` is C for per-channel parameters, else 1 (rows s, gain, bias, power)."""
+    L = lib()
+    B, C, T = E.shape
+    (s, gain, bias, power), stride = _pcen_params(params)
+    dE = torch.empty((B, C, T), dtype=torch.float32, device=E.device) if want_E else None
+    dp = torch.empty((4, C if stride else 1), dtype=torch.float32, device=E.device) if want_params else None
+    with torch.cuda.device(E.device):
+        ws, wsb = _workspace(L.nnab_pcen_workspace_bytes(B, C) if want_params else 0, E.device)
+        rc = L.nnab_pcen_backward(_ptr(E), _ptr(M), _ptr(gP), B, C, T, s, gain, bias, power, stride, float(eps),
+                                  _ptr(dE), _ptr(dp), _ptr(ws), wsb, _stream(E.device))
+    _check(rc, "nnab_pcen_backward")
+    return dE, dp
+
+
+def pcen_reset(primed, mask):
+    """Un-prime the (slots, C) stream state where the uint8 device ``mask`` (slots,) is set (None: every slot)."""
+    with torch.cuda.device(primed.device):
+        _check(lib().nnab_pcen_reset(_ptr(primed), _ptr(mask), primed.shape[0], primed.shape[1],
+                                     _stream(primed.device)), "nnab_pcen_reset")

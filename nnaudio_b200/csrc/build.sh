@@ -12,7 +12,7 @@ mkdir -p "$root/build"
 "${PYTHON:-python3}" "$root/tools/gen_wgmma.py" "$root/build/wgmma_bf16.cuh"   # wgmma wrappers, one per MMA width
 objs=()
 pids=()
-for src in simt_kernels tc_kernels tcb_kernels tct_kernels tc_probe nnab_api; do
+for src in simt_kernels tc_kernels tcb_kernels tct_kernels tc_probe pcen_kernels nnab_api; do
   rm -f "$root/build/$src.o"   # a failed compile must not link yesterday's object
   "$NVCC" "${FLAGS[@]}" ${NNAB_PTXAS_V:+-Xptxas -v} -c "$here/$src.cu" -o "$root/build/$src.o" &
   pids+=($!)

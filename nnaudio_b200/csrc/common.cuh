@@ -648,6 +648,30 @@ int tc_device_istft_plan(int64_t slots, int64_t* counters, const int32_t* frame_
                          nnab_istft_lane* lanes, int64_t t, int n_fft, int hop, int center, cudaStream_t stream);
 int tc_device_pool_reset(int64_t slots, int64_t* counters, int32_t* errors, int64_t* info, const uint8_t* mask,
                          cudaStream_t stream);
+
+// ---- PCEN (pcen_kernels.cu) ---------------------------------------------------
+// per-channel (param_stride 1) or scalar (0) parameters, device pointers
+struct PcenArgs {
+  const float *s, *gain, *bias, *power;
+  int param_stride;
+  float eps;
+};
+// the streamed call's state: state / primed (slots, C); row b is slot row_slot[b] (NULL: slot b) and advances by
+// counts[b] frames (NULL: all of them); state == NULL for the offline and training calls
+struct PcenStream {
+  float* state;
+  uint8_t* primed;
+  int64_t slots;
+  const int32_t* row_slot;
+  const int32_t* counts;
+};
+int64_t pcen_blocks(int64_t rows);
+int pcen_forward(const float* E, int64_t B, int C, int64_t T, const PcenArgs& a, float* P, float* M_out,
+                 const PcenStream& st, cudaStream_t stream);
+// partial: 4 * B * C floats of workspace when grad_params != NULL
+int pcen_backward(const float* E, const float* M, const float* gP, int64_t B, int C, int64_t T, const PcenArgs& a,
+                  float* dE, float* grad_params, float* partial, cudaStream_t stream);
+int pcen_reset(uint8_t* primed, const uint8_t* mask, int64_t slots, int C, cudaStream_t stream);
 // pyramid pools: the (signal, lane) descriptor table of a push (table[s * n_lanes + i] = pyr_lane_signal of lane i
 // of the DEVICE lane table, or with lanes == nullptr of `shared` in slot i), every row's carry [keep, R1) of one
 // signal (cs.rows; at most `longest` samples), and the zeroing of frames t >= rows[i].count of row i of out

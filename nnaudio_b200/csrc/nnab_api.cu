@@ -2875,4 +2875,54 @@ int nnab_cqt1992v2_pool_device_forward(void* state, int64_t* counters, const int
   return rc;
 }
 
+// ---- PCEN (pcen_kernels.cu) ----
+static bool pcen_shape_ok(const float* s, const float* gain, const float* bias, const float* power,
+                          int param_stride, float eps, int64_t B, int C, int64_t T) {
+  return s != nullptr && gain != nullptr && bias != nullptr && power != nullptr &&
+         (param_stride == 0 || param_stride == 1) && eps > 0.f && eps < INFINITY && B >= 0 && C >= 1 && T >= 0 &&
+         pcen_blocks(B * (int64_t)C) < (int64_t)INT32_MAX;
+}
+
+size_t nnab_pcen_workspace_bytes(int64_t B, int C) {
+  return (B < 0 || C < 1) ? 0 : 4 * (size_t)B * (size_t)C * sizeof(float);
+}
+
+int nnab_pcen_forward(const float* E, int64_t B, int C, int64_t T, const float* s, const float* gain,
+                      const float* bias, const float* power, int param_stride, float eps, float* P, float* M,
+                      float* state, uint8_t* primed, int64_t slots, const int32_t* row_slot, const int32_t* counts,
+                      void* stream) {
+  if (E == nullptr || P == nullptr || !pcen_shape_ok(s, gain, bias, power, param_stride, eps, B, C, T))
+    return NNAB_EINVAL;
+  if ((state == nullptr) != (primed == nullptr)) return NNAB_EINVAL;
+  if (state == nullptr && (row_slot != nullptr || counts != nullptr)) return NNAB_EINVAL;  // stream-only arguments
+  if (state != nullptr && (M != nullptr || slots < 1 || (row_slot == nullptr && B > slots))) return NNAB_EINVAL;
+  const int rc = check_arch();
+  if (rc) return rc;
+  if (B == 0 || T == 0) return NNAB_OK;
+  return pcen_forward(E, B, C, T, PcenArgs{s, gain, bias, power, param_stride, eps}, P, M,
+                      PcenStream{state, primed, slots, row_slot, counts}, (cudaStream_t)stream);
+}
+
+int nnab_pcen_backward(const float* E, const float* M, const float* grad_P, int64_t B, int C, int64_t T,
+                       const float* s, const float* gain, const float* bias, const float* power, int param_stride,
+                       float eps, float* grad_E, float* grad_params, void* workspace, size_t ws_bytes, void* stream) {
+  if (E == nullptr || M == nullptr || grad_P == nullptr ||
+      !pcen_shape_ok(s, gain, bias, power, param_stride, eps, B, C, T))
+    return NNAB_EINVAL;
+  const int rc = check_arch();
+  if (rc) return rc;
+  if (grad_params != nullptr && (workspace == nullptr || ws_bytes < nnab_pcen_workspace_bytes(B, C)))
+    return NNAB_EWORKSPACE;
+  if (B == 0 || (grad_E == nullptr && grad_params == nullptr)) return NNAB_OK;
+  return pcen_backward(E, M, grad_P, B, C, T, PcenArgs{s, gain, bias, power, param_stride, eps}, grad_E, grad_params,
+                       static_cast<float*>(workspace), (cudaStream_t)stream);
+}
+
+int nnab_pcen_reset(uint8_t* primed, const uint8_t* mask, int64_t slots, int C, void* stream) {
+  if (primed == nullptr || slots < 1 || C < 1) return NNAB_EINVAL;
+  const int rc = check_arch();
+  if (rc) return rc;
+  return pcen_reset(primed, mask, slots, C, (cudaStream_t)stream);
+}
+
 }  // extern "C"
