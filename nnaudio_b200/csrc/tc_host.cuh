@@ -54,8 +54,9 @@ int num_phases(int hop);
 int encode_3d(CUtensorMap* map, void* base, uint64_t d0, uint64_t d1, uint64_t d2,
               uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t box0, uint32_t box1, int bk);
 
+// 4-D bf16 map {d0 (contiguous), d1, d2, d3}, box {box0, box1, box2, 1}, swizzle by bk as encode_3d
 int encode_4d(CUtensorMap* map, void* base, const uint64_t dims[4], const uint64_t strides[3],
-              const uint32_t box[3]);
+              const uint32_t box[3], int bk = 64);
 size_t tc_packed_bytes(int F, int K);
 int tc_pack_basis_varn(const float* w_re, const float* w_im, int F, int K, void* packed,
                        cudaStream_t stream);

@@ -1747,10 +1747,10 @@ int encode_3d(CUtensorMap* map, void* base, uint64_t d0, uint64_t d1, uint64_t d
   return NNAB_OK;
 }
 
-// 4-D bf16 map, SWIZZLE_128B, box {box0, box1, box2, 1}; strides in bytes for dims 1..3 (any order of
-// magnitude: a dimension may step by less than the extent of the one below it -- overlapping views)
+// 4-D bf16 map, box {box0, box1, box2, 1}, swizzle by bk as encode_3d; strides in bytes for dims 1..3 (any order
+// of magnitude: a dimension may step by less than the extent of the one below it -- overlapping views)
 int encode_4d(CUtensorMap* map, void* base, const uint64_t dims[4], const uint64_t strides[3],
-              const uint32_t box[3]) {
+              const uint32_t box[3], int bk) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) {
     set_error_text("cuTensorMapEncodeTiled entry point not available");
@@ -1761,7 +1761,8 @@ int encode_4d(CUtensorMap* map, void* base, const uint64_t dims[4], const uint64
   cuuint32_t bx[4] = {box[0], box[1], box[2], 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, gdim, gstr, bx, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        (bk == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char msg[240];

@@ -40,10 +40,13 @@
 //   Z[k'] = A0 + B0   Z[M + k'] = A1 - i B1   Z[M - k'] = conj(A1 + i B1)   Z[2M - k'] = conj(A0 - B0)
 //
 // (tools/block_poly_emulation.py is the executable spec.)  A quarter of the MMA work and of the operand bytes.
-// The 4 TMA boxes of an M tile are the 4 phases of the same 32 block rows (column origins q hop / 4); after
-// the MMAs a butterfly pass in the accumulator tile turns quarter q = phase q into quarter f = family f
-// (f1, f3 column-reversed so that every family runs over ascending bins, common.cuh block_family_span), and
-// the epilogue above runs on each quarter with its family's bin origin and bin range.  33 - R frames per tile.
+// The rows of an M tile's A operand are the 4 phases of the same 32 block rows, laid out so that one thread's
+// accumulators hold all four phases of one (block row, packed bin): each warpgroup runs both m64 slabs h = 0, 1
+// (slab row 16 w + 8 p + i = phase 2 h + p of block row 8 w + i) against its half of the N columns, and the packed
+// basis keeps each bin's re and im rows next to each other (tcb_poly_tile).  The butterfly then runs on the
+// registers, and its four families go into the accumulator tile as quarter f = family f (f1, f3 column-reversed
+// so that every family runs over ascending bins, common.cuh block_family_span); the epilogue above runs on each
+// quarter with its family's bin origin and bin range.  33 - R frames per tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -151,8 +154,10 @@ bool tc_block_shape_ok(int n_fft, int hop) {
 
 // packed[plane hi|lo][part re|im][p][n]: bin k = p - 1, sample n < hop:
 //   re row:  cos(2 pi k n / N)      im row: -sin(2 pi k n / N)     (so re + i im = e^{-i theta k n})
-// Four phases: the same rows of the M-point DFT over hop / 4 samples (n_fft = M, hop = hop / 4, F = F').
-__global__ void __launch_bounds__(256) pack_block_basis_kernel(int n_fft, int hop, int F, int p_rows,
+// Four phases: the same rows of the M-point DFT over hop / 4 samples (n_fft = M, hop = hop / 4, F = F'), stored
+// interleaved (`pairs`) as packed[plane][p][part re|im][n], so that a tile's re and im rows of bin p are MMA
+// columns 2 p and 2 p + 1 and either half of the tile's columns is one contiguous run of rows.  Same bytes.
+__global__ void __launch_bounds__(256) pack_block_basis_kernel(int n_fft, int hop, int F, int p_rows, bool pairs,
                                                                __nv_bfloat16* __restrict__ packed) {
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int k8 = hop / 8;
@@ -179,11 +184,12 @@ __global__ void __launch_bounds__(256) pack_block_basis_kernel(int n_fft, int ho
     il[e] = __float2bfloat16_rn(s - __bfloat162float(ih[e]));
   }
   const int64_t slab = (int64_t)p_rows * hop;
-  const int64_t o = (int64_t)p * hop + n0;
-  *reinterpret_cast<uint4*>(packed + 0 * slab + o) = *reinterpret_cast<const uint4*>(rh);
-  *reinterpret_cast<uint4*>(packed + 1 * slab + o) = *reinterpret_cast<const uint4*>(ih);
+  const int64_t o = (int64_t)(pairs ? 2 * p : p) * hop + n0;  // re row of bin p in the hi plane
+  const int64_t im = pairs ? hop : slab;                      // its im row
+  *reinterpret_cast<uint4*>(packed + o) = *reinterpret_cast<const uint4*>(rh);
+  *reinterpret_cast<uint4*>(packed + o + im) = *reinterpret_cast<const uint4*>(ih);
   *reinterpret_cast<uint4*>(packed + 2 * slab + o) = *reinterpret_cast<const uint4*>(rl);
-  *reinterpret_cast<uint4*>(packed + 3 * slab + o) = *reinterpret_cast<const uint4*>(il);
+  *reinterpret_cast<uint4*>(packed + 2 * slab + o + im) = *reinterpret_cast<const uint4*>(il);
 }
 
 // four phases: tw[q - 1][p] = e^{-2 pi i k q / N}, k = p - 1, q = 1 .. 3 (fp32, from float64)
@@ -205,7 +211,7 @@ int tc_pack_basis_block(int n_fft, int hop, void* packed, cudaStream_t stream) {
   const int p_rows = block_p_rows(F);
   const int64_t threads = (int64_t)p_rows * (K / 8);
   pack_block_basis_kernel<<<(unsigned)ceil_div64(threads, 256), 256, 0, stream>>>(
-      poly ? n_fft / 4 : n_fft, K, F, p_rows, (__nv_bfloat16*)packed);
+      poly ? n_fft / 4 : n_fft, K, F, p_rows, poly, (__nv_bfloat16*)packed);
   NNAB_LAUNCH_CHECK();
   if (poly) {
     pack_block_twiddle_kernel<<<(unsigned)ceil_div64(3 * p_rows, 256), 256, 0, stream>>>(
@@ -494,8 +500,8 @@ __device__ __forceinline__ void epilogue_tile_block(const TcbParams& p, uint32_t
 constexpr int TCB_PARTS = 2;
 static_assert(FB_EPI_PARTS == TCB_PARTS, "fused-filterbank column ranges follow the epilogue warps");
 
-// The stage ring.  A stage holds A (hi, lo planes, or hi only with two passes: four 32-row boxes each) and B
-// (four nb-row boxes: hi re, hi im, lo re, lo im); its empty barrier counts the 8 consumer warps.
+// The stage ring.  A stage holds A (hi, lo planes, or hi only with two passes; 128 rows each) and B (hi, lo
+// planes of 2 nb rows each); its empty barrier counts the 8 consumer warps.
 struct TcbRing {
   uint32_t base, stage_bytes, bars;
   int stages;
@@ -507,7 +513,7 @@ struct TcbRing {
 // One K block of tile (m_tile, n_tile) into ring stage `stage` (the stage's full barrier expects its bytes).
 template <int R, int PASSES, int PH>
 __device__ __forceinline__ void tcb_load_block(const CUtensorMap* tm_a, const CUtensorMap* tm_b, const TcbRing& ring,
-                                               int stage, int m_tile, int n_tile, int kb, int kb_n, int nb) {
+                                               int stage, int m_tile, int n_tile, int kb, int nb) {
   using S = TcbSmem;
   constexpr int BK = TCB_BK;
   constexpr int FW = 33 - R;  // frames per warp quarter
@@ -518,55 +524,76 @@ __device__ __forceinline__ void tcb_load_block(const CUtensorMap* tm_a, const CU
   const uint32_t full = ring.full(stage);
   mbar_expect_tx(full, ring.stage_bytes);
   const int k0 = kb * BK;
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    // one phase: 32-row boxes, row origins FW apart; four phases: phase q of the same 32 block rows
-    const int kc = PH == 4 ? q * kb_n * BK + k0 : k0;
-    const int row = PH == 4 ? m0 : m0 + q * FW;
-    tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, tm_a, full, kc, row, 0);
-    if constexpr (PASSES == 3)
-      tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, tm_a, full, kc, row, 1);
-  }
-  // B rows [0, nb) = re part, [nb, 2 nb) = im part of each plane: accumulator columns of the N = 2 nb MMA
   const uint32_t b = sb + S::a_planes(PASSES) * S::A_BYTES;
   const uint32_t part_bytes = S::part_bytes(nb);
+  if constexpr (PH == 4) {
+    // tm_a is (k, block row, phase, plane): a 16-row box is phases 2 h, 2 h + 1 of block rows m0 + 8 w .. + 7,
+    // slab h rows 16 w .. 16 w + 15 (tcb_poly_tile's row map)
 #pragma unroll
-  for (int j = 0; j < 4; ++j) tma_load_3d(b + (uint32_t)j * part_bytes, tm_b, full, k0, n0, j);
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {
+        const uint32_t dst = sb + (uint32_t)(64 * h + 16 * w) * BK * 2u;
+        tma_load_4d(dst, tm_a, full, k0, m0 + 8 * w, 2 * h, 0);
+        if constexpr (PASSES == 3) tma_load_4d(dst + S::A_BYTES, tm_a, full, k0, m0 + 8 * w, 2 * h, 1);
+      }
+    }
+    // B: one box of 2 nb rows per plane (bins n0 .. n0 + nb - 1, re and im rows interleaved)
+    tma_load_3d(b, tm_b, full, k0, 2 * n0, 0);
+    tma_load_3d(b + 2 * part_bytes, tm_b, full, k0, 2 * n0, 1);
+  } else {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {  // 32-row boxes, row origins FW apart
+      tma_load_3d(sb + (uint32_t)q * 32u * BK * 2u, tm_a, full, k0, m0 + q * FW, 0);
+      if constexpr (PASSES == 3)
+        tma_load_3d(sb + S::A_BYTES + (uint32_t)q * 32u * BK * 2u, tm_a, full, k0, m0 + q * FW, 1);
+    }
+    // B rows [0, nb) = re part, [nb, 2 nb) = im part of each plane: accumulator columns of the N = 2 nb MMA
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tma_load_3d(b + (uint32_t)j * part_bytes, tm_b, full, k0, n0, j);
+  }
 }
 
 struct TcbNoRefill {
-  __device__ void operator()() const {}
+  __device__ void operator()(int) const {}
 };
 
-// One tile's K loop at MMA width N = 2 nb.  Each K block is committed as one wgmma group; the stage of the
-// PREVIOUS block is released once that group has retired, so one group is always in flight.  A width fixed
-// at compile time keeps every in-flight wgmma off divergent paths (ptxas would serialise them).  `refill()`
-// runs after every release: the warp-specialised kernel refills the released stage from one MMA thread, a
-// divergent path, so there (IN_FLIGHT = 0) each block's group retires before its stage is released.
-template <int N, int PASSES, int IN_FLIGHT = 1, class Refill = TcbNoRefill>
+// One tile's K loop: SLABS m64 slabs of A (the first at byte a_off of a stage, the next 64 rows on) against N
+// columns of B (from byte b_off of each B plane), accumulators acc[h N / 2 ..] for slab h.  One phase: one slab,
+// this warpgroup's, at N = 2 nb; four phases: both slabs at N = nb (tcb_poly_tile).  Each K block is committed as
+// one wgmma group; the stage of the PREVIOUS block is released once that group has retired, so one group is
+// always in flight.  A width fixed at compile time keeps every in-flight wgmma off divergent paths (ptxas would
+// serialise them).  `refill(kb)` runs after K block kb's release: the warp-specialised kernel refills the released stage
+// from one MMA thread, a divergent path, so there (IN_FLIGHT = 0) each block's group retires before its stage is
+// released.
+template <int N, int PASSES, int SLABS, int IN_FLIGHT = 1, class Refill = TcbNoRefill>
 __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, int kb_n, uint32_t a_off,
-                                             uint32_t part_bytes, int lane, int& stage, uint32_t& phase,
-                                             Refill refill = Refill()) {
+                                             uint32_t b_off, uint32_t part_bytes, int lane, int& stage,
+                                             uint32_t& phase, Refill refill = Refill()) {
   static_assert(IN_FLIGHT == 0 || IN_FLIGHT == 1, "at most one wgmma group in flight");
   using S = TcbSmem;
   int prev = 0;
   for (int kb = 0; kb < kb_n; ++kb) {
     mbar_wait(ring.full(stage), phase);
     const uint32_t sb = ring.stage(stage);
-    const uint32_t b = sb + S::a_planes(PASSES) * S::A_BYTES;
+    const uint32_t b = sb + S::a_planes(PASSES) * S::A_BYTES + b_off;
     wgmma_fence();
-    if constexpr (PASSES == 3)
-      wg_kblock_split3_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(sb + S::A_BYTES + a_off),
-                                    wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes), kb != 0);
-    else
-      wg_kblock_split2_n<N, TCB_BK>(acc, wg_desc_lo(sb + a_off), wg_desc_lo(b), wg_desc_lo(b + 2 * part_bytes),
-                                    kb != 0);
+#pragma unroll
+    for (int h = 0; h < SLABS; ++h) {
+      const uint32_t a = sb + a_off + (uint32_t)h * 64u * (TCB_BK * 2);
+      if constexpr (PASSES == 3)
+        wg_kblock_split3_n<N, TCB_BK>(acc + h * (N / 2), wg_desc_lo(a), wg_desc_lo(a + S::A_BYTES), wg_desc_lo(b),
+                                      wg_desc_lo(b + 2 * part_bytes), kb != 0);
+      else
+        wg_kblock_split2_n<N, TCB_BK>(acc + h * (N / 2), wg_desc_lo(a), wg_desc_lo(b),
+                                      wg_desc_lo(b + 2 * part_bytes), kb != 0);
+    }
     wgmma_commit();
     wgmma_wait<IN_FLIGHT>();
     __syncwarp();
     if (IN_FLIGHT == 0 || kb > 0) {
       if (lane == 0) mbar_arrive(ring.empty(IN_FLIGHT == 0 ? stage : prev));
-      refill();
+      refill(IN_FLIGHT == 0 ? kb : kb - 1);
     }
     prev = stage;
     if (++stage == ring.stages) { stage = 0; phase ^= 1u; }
@@ -575,70 +602,90 @@ __device__ __forceinline__ void tcb_mainloop(float* acc, const TcbRing& ring, in
     wgmma_wait<0>();
     __syncwarp();
     if (lane == 0) mbar_arrive(ring.empty(prev));
-    refill();
+    refill(kb_n - 1);
   }
 }
 
-// Four phases: the radix-4 butterfly, in place in the accumulator tile.  Quarter q holds Y_q of the tile's
-// packed columns (column i <-> k' = n_tile (nb - 2) + i - 1) for 32 block rows; afterwards quarter f holds
-// family f, f1 and f3 at the mirrored column nb - 1 - i.  A thread owns row `lane` of all four quarters and a
-// 4-column group together with its mirror group, so every location it writes is one it alone reads.
-__device__ __forceinline__ void tcb_butterfly(const TcbParams& p, uint32_t tile, int n_tile, int warp, int lane) {
-  const int nb = p.nb;
-  const float2* __restrict__ tw = p.twiddle + n_tile * (nb - 2);
-#pragma unroll 1
-  for (int gi = warp; gi < nb / 8; gi += 8) {
-    int col[2];
-    col[0] = 4 * gi;
-    col[1] = nb - 4 - 4 * gi;  // the mirror group (never the same: nb is a multiple of 8)
-    float yr[4][8], yi[4][8];   // [phase][column: group 0, then group 1]
+// Four phases: one tile at MMA width N = nb.  Each warpgroup runs both m64 slabs of the A tile against its half of
+// the packed columns (bins wg nb / 2 .. + nb / 2 - 1, re and im interleaved), so with slab row 16 w + 8 p + i =
+// phase 2 h + p of block row 8 w + i, thread `lane` of warp w holds, for its block row r = 8 w + lane / 4 and bins
+// c = wg nb / 2 + 4 j + lane % 4:
+//   Y_0 = acc[4 j], acc[4 j + 1]   Y_1 = acc[4 j + 2], acc[4 j + 3]   (slab 0: rows 16 w + lane / 4, + 8)
+//   Y_2, Y_3 the same at acc[N / 2 + ..]                              (slab 1)
+// (re, im of each).  The radix-4 butterfly runs on those registers, in place, and once `wait()` has returned the
+// four families go into the accumulator tile: family f of bin c at row 32 f + r, column c (f0, f2) or nb - 1 - c
+// (f1, f3), re at that column, im nb columns on.  The four threads of a quad write 4 consecutive columns of one
+// row and a warp's eight quads 8 rows of distinct r & 7, so under acc_chunk_smem's row XOR every store is
+// conflict-free.  Column c's twiddles are Y_q's factors e^{-2 pi i k' q / N}, k' = n_tile (nb - 2) + c - 1.
+template <int N>
+__device__ __forceinline__ void tcb_butterfly_regs(const TcbParams& p, float* acc, int n_tile, int wg, int lane) {
+  const float2* __restrict__ tw = p.twiddle + n_tile * (N - 2) + wg * (N / 2) + (lane & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    float yr[4], yi[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t re[4], im[4];
-        acc_ld4(tile + (uint32_t)col[h], (uint32_t)(32 * q + lane), re);
-        acc_ld4(tile + (uint32_t)(nb + col[h]), (uint32_t)(32 * q + lane), im);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) { yr[q][4 * h + e] = __uint_as_float(re[e]); yi[q][4 * h + e] = __uint_as_float(im[e]); }
-      }
+      const int o = (q >> 1) * (N / 2) + 4 * j + 2 * (q & 1);
+      yr[q] = acc[o];
+      yi[q] = acc[o + 1];
     }
-    float fr[4][8], fi[4][8];  // [family][column]
+    float tr[4], ti[4];
+    tr[0] = yr[0]; ti[0] = yi[0];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int c = col[j >> 2] + (j & 3);
-      float tr[4], ti[4];
-      tr[0] = yr[0][j]; ti[0] = yi[0][j];
-#pragma unroll
-      for (int q = 1; q < 4; ++q) {
-        const float2 w = __ldg(tw + (q - 1) * p.tw_rows + c);
-        tr[q] = w.x * yr[q][j] - w.y * yi[q][j];
-        ti[q] = w.x * yi[q][j] + w.y * yr[q][j];
-      }
-      const float a0r = tr[0] + tr[2], a0i = ti[0] + ti[2], a1r = tr[0] - tr[2], a1i = ti[0] - ti[2];
-      const float b0r = tr[1] + tr[3], b0i = ti[1] + ti[3], b1r = tr[1] - tr[3], b1i = ti[1] - ti[3];
-      fr[0][j] = a0r + b0r;  fi[0][j] = a0i + b0i;     // Z[k']
-      fr[1][j] = a1r - b1i;  fi[1][j] = -(a1i + b1r);  // Z[M - k'] = conj(A1 + i B1)
-      fr[2][j] = a1r + b1i;  fi[2][j] = a1i - b1r;     // Z[M + k'] = A1 - i B1
-      fr[3][j] = a0r - b0r;  fi[3][j] = b0i - a0i;     // Z[2M - k'] = conj(A0 - B0)
+    for (int q = 1; q < 4; ++q) {
+      const float2 w = __ldg(tw + (q - 1) * p.tw_rows + 4 * j);
+      tr[q] = w.x * yr[q] - w.y * yi[q];
+      ti[q] = w.x * yi[q] + w.y * yr[q];
     }
+    const float a0r = tr[0] + tr[2], a0i = ti[0] + ti[2], a1r = tr[0] - tr[2], a1i = ti[0] - ti[2];
+    const float b0r = tr[1] + tr[3], b0i = ti[1] + ti[3], b1r = tr[1] - tr[3], b1i = ti[1] - ti[3];
+    float fr[4], fi[4];
+    fr[0] = a0r + b0r;  fi[0] = a0i + b0i;     // Z[k']
+    fr[1] = a1r - b1i;  fi[1] = -(a1i + b1r);  // Z[M - k'] = conj(A1 + i B1)
+    fr[2] = a1r + b1i;  fi[2] = a1i - b1r;     // Z[M + k'] = A1 - i B1
+    fr[3] = a0r - b0r;  fi[3] = b0i - a0i;     // Z[2M - k'] = conj(A0 - B0)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int j = 4 * h, m = 4 * (1 - h) + 3;  // group h in place; the other group's columns reversed
-#pragma unroll
-      for (int f = 0; f < 4; f += 2) {
-        const uint32_t r = (uint32_t)(32 * f + lane);
-        acc_st4(tile + (uint32_t)col[h], r, fr[f][j], fr[f][j + 1], fr[f][j + 2], fr[f][j + 3]);
-        acc_st4(tile + (uint32_t)(nb + col[h]), r, fi[f][j], fi[f][j + 1], fi[f][j + 2], fi[f][j + 3]);
-      }
-#pragma unroll
-      for (int f = 1; f < 4; f += 2) {
-        const uint32_t r = (uint32_t)(32 * f + lane);
-        acc_st4(tile + (uint32_t)col[h], r, fr[f][m], fr[f][m - 1], fr[f][m - 2], fr[f][m - 3]);
-        acc_st4(tile + (uint32_t)(nb + col[h]), r, fi[f][m], fi[f][m - 1], fi[f][m - 2], fi[f][m - 3]);
-      }
+    for (int f = 0; f < 4; ++f) {  // family f where phase f was
+      const int o = (f >> 1) * (N / 2) + 4 * j + 2 * (f & 1);
+      acc[o] = fr[f];
+      acc[o + 1] = fi[f];
     }
   }
+}
+
+// The accumulator tile is 2 N columns wide, so its row stride is a compile-time constant and the four families'
+// rows of one thread differ by immediates; acc_chunk_smem's row XOR is the same for all of them (32 f + r = r mod 8).
+template <int N>
+__device__ __forceinline__ void tcb_store_families(const float* acc, int wg, int warp, int lane) {
+  constexpr uint32_t STRIDE = (uint32_t)((2 * N + 31) / 32) * 128u;
+  const uint32_t r = (uint32_t)(8 * (warp & 3) + (lane >> 2));
+  const uint32_t row0 = acc_tile_base() + r * STRIDE;
+  const uint32_t swz = (r & 7u) << 4;  // acc_chunk_smem: 16-byte chunk c at position c ^ (row & 7)
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const uint32_t c = (uint32_t)(wg * (N / 2) + 4 * j + (lane & 3));
+#pragma unroll
+    for (int f = 0; f < 4; ++f) {
+      const int o = (f >> 1) * (N / 2) + 4 * j + 2 * (f & 1);
+      const uint32_t col = (f & 1) ? (uint32_t)(N - 1) - c : c;
+      const uint32_t at = row0 + 32u * f * STRIDE;
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(at + ((4u * col) ^ swz)), "f"(acc[o]) : "memory");
+      asm volatile("st.shared.f32 [%0], %1;" ::"r"(at + ((4u * (N + col)) ^ swz)), "f"(acc[o + 1]) : "memory");
+    }
+  }
+}
+
+template <int N, int PASSES, int IN_FLIGHT, class Wait, class Refill = TcbNoRefill>
+__device__ __forceinline__ void tcb_poly_tile(const TcbParams& p, float* acc, const TcbRing& ring, int n_tile,
+                                              int warp, int lane, int& stage, uint32_t& phase, Wait wait,
+                                              Refill refill = Refill()) {
+  const int wg = warp >> 2;
+  const uint32_t part_bytes = TcbSmem::part_bytes(N);
+  tcb_mainloop<N, PASSES, 2, IN_FLIGHT>(acc, ring, p.kb_n, 0u, (uint32_t)wg * part_bytes, part_bytes, lane, stage,
+                                        phase, refill);
+  tcb_butterfly_regs<N>(p, acc, n_tile, wg, lane);
+  wait();
+  tcb_store_families<N>(acc, wg, warp, lane);
 }
 
 // One warp's share of a tile's epilogue: 32-row quarter `quarter` (four phases: family `quarter`) and column
@@ -716,7 +763,7 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
         const int n_tile = tile - m_tile * p.num_n_tiles;
         for (int kb = 0; kb < p.kb_n; ++kb) {
           mbar_wait(ring.empty(stage), phase ^ 1u);
-          tcb_load_block<R, PASSES, PH>(&tm_a, &tm_b, ring, stage, m_tile, n_tile, kb, p.kb_n, nb);
+          tcb_load_block<R, PASSES, PH>(&tm_a, &tm_b, ring, stage, m_tile, n_tile, kb, nb);
           if (++stage == p.stages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -736,22 +783,32 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
     const int n_tile = tile - m_tile * p.num_n_tiles;
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    switch (2 * nb) {  // nb = 32 .. 128 in steps of 8
-#define NNAB_TCB_CASE(N) \
-  case N: tcb_mainloop<N, PASSES>(acc, ring, p.kb_n, a_off, part_bytes, lane, stage, phase); break;
-      NNAB_TCB_CASE(64) NNAB_TCB_CASE(80) NNAB_TCB_CASE(96) NNAB_TCB_CASE(112) NNAB_TCB_CASE(128)
-      NNAB_TCB_CASE(144) NNAB_TCB_CASE(160) NNAB_TCB_CASE(176) NNAB_TCB_CASE(192) NNAB_TCB_CASE(208)
-      NNAB_TCB_CASE(224) NNAB_TCB_CASE(240) NNAB_TCB_CASE(256)
-#undef NNAB_TCB_CASE
-      default: break;
-    }
-    consumer_sync();  // every warp is done reading the previous tile
-    acc_store<256>(tile_addr, acc, 2 * nb, wg * 64);
-    consumer_sync();
     if constexpr (PH == 4) {
-      tcb_butterfly(p, tile_addr, n_tile, warp, lane);
-      consumer_sync();
+      // the butterfly on the registers; the families are stored once every warp is done reading the previous tile
+      auto wait = [] { consumer_sync(); };
+      switch (nb) {  // nb = 32 .. 128 in steps of 8
+#define NNAB_TCB_CASE(N) \
+  case N: tcb_poly_tile<N, PASSES, 1>(p, acc, ring, n_tile, warp, lane, stage, phase, wait); break;
+        NNAB_TCB_CASE(32) NNAB_TCB_CASE(40) NNAB_TCB_CASE(48) NNAB_TCB_CASE(56) NNAB_TCB_CASE(64)
+        NNAB_TCB_CASE(72) NNAB_TCB_CASE(80) NNAB_TCB_CASE(88) NNAB_TCB_CASE(96) NNAB_TCB_CASE(104)
+        NNAB_TCB_CASE(112) NNAB_TCB_CASE(120) NNAB_TCB_CASE(128)
+#undef NNAB_TCB_CASE
+        default: break;
+      }
+    } else {
+      switch (2 * nb) {  // nb = 32 .. 128 in steps of 8
+#define NNAB_TCB_CASE(N) \
+  case N: tcb_mainloop<N, PASSES, 1>(acc, ring, p.kb_n, a_off, 0u, part_bytes, lane, stage, phase); break;
+        NNAB_TCB_CASE(64) NNAB_TCB_CASE(80) NNAB_TCB_CASE(96) NNAB_TCB_CASE(112) NNAB_TCB_CASE(128)
+        NNAB_TCB_CASE(144) NNAB_TCB_CASE(160) NNAB_TCB_CASE(176) NNAB_TCB_CASE(192) NNAB_TCB_CASE(208)
+        NNAB_TCB_CASE(224) NNAB_TCB_CASE(240) NNAB_TCB_CASE(256)
+#undef NNAB_TCB_CASE
+        default: break;
+      }
+      consumer_sync();  // every warp is done reading the previous tile
+      acc_store<256>(tile_addr, acc, 2 * nb, wg * 64);
     }
+    consumer_sync();
     // warp w: tile rows 32 (w & 3) .. + 31 (four phases: family w & 3), column part w >> 2
     tcb_epilogue<FMT, R, PH>(p, tile_addr, m_tile, n_tile, warp & 3, warp >> 2, lane, ring.bars + S::HANDOVER_OFF);
   }
@@ -759,17 +816,17 @@ framed_tcb_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constan
 
 // Four phases at nb <= TCB_WS_NB_MAX: the same tile schedule, ring, wgmma sequence and per-tile arithmetic as
 // framed_tcb_kernel, with separate warps for separate roles, so a tile's MMAs run while the previous tile drains:
-//   * warps 0-7 (two warpgroups): the K loop of tile i + 1 in registers while tile i is drained; then, once the
-//     epilogue warps have released the accumulator tile (acc_empty), acc_store, the butterfly, and acc_full.
+//   * warps 0-7 (two warpgroups): the K loop of tile i + 1 and the butterfly in registers while tile i is drained;
+//     then, once the epilogue warps have released the accumulator tile (acc_empty), the family stores and acc_full.
 //     Thread 0 also issues the TMA loads: after each release it waits until all 8 warps have released the stage
 //     and refills it with the block `stages` ahead (across tile ends, so the next tile's first blocks land while
 //     the MMA warps wait for acc_empty);
 //   * warps 8-15: the epilogue, warp 8 + w in the place of consumer warp w of framed_tcb_kernel.
 // 16 warps, because the register file is split over the four schedulers: 4 warps each get 128 registers, room for
-// the 88 accumulators of MMA width 2 TCB_WS_NB_MAX (ptxas needs >= 114 for that wgmma).  A separate producer warp
+// the 88 accumulators of two MMAs of width TCB_WS_NB_MAX (tcb_poly_tile).  A separate producer warp
 // (17 warps) would cut every thread to 96, and ptxas does not raise the allocation inside setmaxnreg regions.
 // There is one accumulator tile: two do not fit beside a stage at nb = 88 (2 x 96 KB + 38 KB > 227 KB), so a tile
-// still takes store + butterfly + epilogue; the MMAs are what is hidden.  With the fused filterbank the epilogue
+// still takes store + epilogue; the MMAs and the butterfly are what is hidden.  With the fused filterbank the epilogue
 // warps' fb_steps slices (TCB_WS_ACT_BYTES) sit behind the barriers: at nb = 88 the ring keeps its 3 stages, at
 // nb = 80 (three passes) it has 3 instead of 4.
 constexpr int TCB_WS_THREADS = 512;
@@ -790,7 +847,7 @@ framed_tcb_ws_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
   ring.stage_bytes = S::stage_bytes(nb, PASSES);
   ring.stages = p.stages;
   ring.bars = ring.base + (uint32_t)p.stages * ring.stage_bytes;
-  const uint32_t acc_full = ring.bars + S::ACC_BARS_OFF;  // the butterfly is done: the epilogue may read
+  const uint32_t acc_full = ring.bars + S::ACC_BARS_OFF;  // the families are stored: the epilogue may read
   const uint32_t acc_empty = acc_full + 8u;              // the epilogue is done: the MMA warps may store
 
   const int warp = threadIdx.x >> 5;
@@ -810,9 +867,6 @@ framed_tcb_ws_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
 
   if (warp < 8) {
     // ===================== MMA warps (thread 0: also the TMA loads) =====================
-    const int wg = warp >> 2;
-    const uint32_t a_off = (uint32_t)wg * 64u * (TCB_BK * 2);
-    const uint32_t part_bytes = S::part_bytes(nb);
     // this CTA's K blocks, in order: block b is K block b % kb_n of its tile b / kb_n, in ring stage b % stages
     const int my_tiles = blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const int total = my_tiles * p.kb_n;
@@ -820,12 +874,14 @@ framed_tcb_ws_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
       const int tile = (int)blockIdx.x + (b / p.kb_n) * (int)gridDim.x;
       const int m_tile = tile / p.num_n_tiles;
       tcb_load_block<R, PASSES, 4>(&tm_a, &tm_b, ring, b % p.stages, m_tile, tile - m_tile * p.num_n_tiles,
-                                   b % p.kb_n, p.kb_n, nb);
+                                   b % p.kb_n, nb);
     };
-    int released = 0;  // thread 0: blocks whose stage all 8 MMA warps have released
-    auto refill = [&]() {
+    // The tile loop keeps one counter, this CTA's tile index t: the tile, the refilled block and the acc_empty
+    // parity derive from it (each counter beside the 88 accumulators is a register the K loop may have to spill)
+    int t = 0;
+    auto refill = [&](int kb) {  // K block kb of tile t has been released by this warp
       if (threadIdx.x == 0) {
-        const int b = released++;
+        const int b = t * p.kb_n + kb;
         mbar_wait(ring.empty(b % p.stages), (uint32_t)(b / p.stages) & 1u);
         if (b + p.stages < total) load(b + p.stages);
       }
@@ -838,24 +894,24 @@ framed_tcb_ws_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_cons
     }
     float acc[TCB_WS_NB_MAX];
     int stage = 0;
-    uint32_t phase = 0, empty_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int n_tile = tile % p.num_n_tiles;
+    uint32_t phase = 0;
+    for (; t < my_tiles; ++t) {
+      const int n_tile = ((int)blockIdx.x + t * (int)gridDim.x) % p.num_n_tiles;
 #pragma unroll
       for (int i = 0; i < TCB_WS_NB_MAX; ++i) acc[i] = 0.f;
-      switch (2 * nb) {  // nb = 32 .. TCB_WS_NB_MAX in steps of 8
+      // the butterfly on the registers, then the families stored once the epilogue has read the previous tile
+      // (the first wait passes)
+      auto wait = [&] { mbar_wait(acc_empty, ((uint32_t)t & 1u) ^ 1u); };
+      switch (nb) {  // nb = 32 .. TCB_WS_NB_MAX in steps of 8
 #define NNAB_TCB_CASE(N) \
-  case N: tcb_mainloop<N, PASSES, 0>(acc, ring, p.kb_n, a_off, part_bytes, lane, stage, phase, refill); break;
-        NNAB_TCB_CASE(64) NNAB_TCB_CASE(80) NNAB_TCB_CASE(96) NNAB_TCB_CASE(112) NNAB_TCB_CASE(128)
-        NNAB_TCB_CASE(144) NNAB_TCB_CASE(160) NNAB_TCB_CASE(176)
+  case N:                                                                                                   \
+    tcb_poly_tile<N, PASSES, 0>(p, acc, ring, n_tile, warp, lane, stage, phase, wait, refill); \
+    break;
+        NNAB_TCB_CASE(32) NNAB_TCB_CASE(40) NNAB_TCB_CASE(48) NNAB_TCB_CASE(56) NNAB_TCB_CASE(64)
+        NNAB_TCB_CASE(72) NNAB_TCB_CASE(80) NNAB_TCB_CASE(88)
 #undef NNAB_TCB_CASE
         default: break;
       }
-      mbar_wait(acc_empty, empty_phase ^ 1u);  // the epilogue has read the previous tile (the first wait passes)
-      empty_phase ^= 1u;
-      acc_store<2 * TCB_WS_NB_MAX>(tile_addr, acc, 2 * nb, wg * 64);
-      consumer_sync();
-      tcb_butterfly(p, tile_addr, n_tile, warp, lane);
       mbar_arrive(acc_full);
     }
     return;
@@ -997,11 +1053,24 @@ int launch_framed_tc_block(const FramedProblem& q, const void* packed, void* wor
   const int n_tiles = block_n_tiles(Fb, nb);
   const int p_rows = block_p_rows(Fb);
   CUtensorMap ma, mb;
-  rc = encode_3d(&ma, planes, (uint64_t)q.hop, (uint64_t)g.rows, 2, (uint64_t)q.hop * 2,
-                 (uint64_t)g.plane_stride * 2, TCB_BK, 32, TCB_BK);
-  if (rc) return rc;
-  rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)Kb, (uint64_t)p_rows, 4,
-                 (uint64_t)Kb * 2, (uint64_t)p_rows * Kb * 2, TCB_BK, (uint32_t)nb, TCB_BK);
+  if (poly) {
+    // A as (k < hop / 4, block row, phase, plane): 16-row boxes of two phases x 8 block rows (tcb_load_block).
+    // The block-row dimension is the only one a box can leave, so the rows past the last block read as zeros.
+    const uint64_t dims[4] = {(uint64_t)Kb, (uint64_t)g.rows, 4, 2};
+    const uint64_t strides[3] = {(uint64_t)q.hop * 2, (uint64_t)Kb * 2, (uint64_t)g.plane_stride * 2};
+    const uint32_t box[3] = {TCB_BK, 8, 2};
+    rc = encode_4d(&ma, planes, dims, strides, box, TCB_BK);
+    if (rc) return rc;
+    // B: one box of 2 nb interleaved re / im rows per plane
+    rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)Kb, (uint64_t)(2 * p_rows), 2, (uint64_t)Kb * 2,
+                   (uint64_t)(2 * p_rows) * Kb * 2, TCB_BK, (uint32_t)(2 * nb), TCB_BK);
+  } else {
+    rc = encode_3d(&ma, planes, (uint64_t)q.hop, (uint64_t)g.rows, 2, (uint64_t)q.hop * 2,
+                   (uint64_t)g.plane_stride * 2, TCB_BK, 32, TCB_BK);
+    if (rc) return rc;
+    rc = encode_3d(&mb, const_cast<void*>(packed), (uint64_t)Kb, (uint64_t)p_rows, 4,
+                   (uint64_t)Kb * 2, (uint64_t)p_rows * Kb * 2, TCB_BK, (uint32_t)nb, TCB_BK);
+  }
   if (rc) return rc;
 
   TcbParams prm{};

@@ -87,10 +87,119 @@ def stft_poly(x, n_fft, hop):
     return X
 
 
+def tma_box(mem, elem_strides, dims, box, coords):
+    """A tiled TMA load: the box at `coords` of the map (dims, element strides; dimension 0 contiguous) over the
+    flat array `mem`, in shared-memory order (dimension 0 fastest), elements outside `dims` read as zero."""
+    out = np.zeros(int(np.prod(box)))
+    for n, idx in enumerate(np.ndindex(*box[::-1])):
+        c = [coords[d] + idx[::-1][d] for d in range(len(box))]
+        if all(0 <= c[d] < dims[d] for d in range(len(dims))):
+            out[n] = mem[sum(c[d] * elem_strides[d] for d in range(len(dims)))]
+    return out
+
+
+def a_map(hop, rows, plane_stride):
+    """launch_framed_tc_block's four-phase A map: (dims, element strides, box) of (k, block row, phase, plane)."""
+    return (hop // 4, rows, 4, 2), (1, hop, hop // 4, plane_stride), (32, 8, 2, 1)
+
+
+def b_map(kq, p_rows):
+    """launch_framed_tc_block's four-phase B map: (dims, element strides, box rows) of (k, row, plane), rows
+    2 p + part of the interleaved basis."""
+    return (kq, 2 * p_rows, 2), (1, kq, 2 * p_rows * kq)
+
+
+def load_a_stage(planes, hop, rows, plane_stride, m0, k0, plane):
+    """tcb_load_block's eight A boxes of one plane: the 128 x 32 shared-memory rows of K block k0 .. k0 + 31."""
+    dims, strides, box = a_map(hop, rows, plane_stride)
+    out = np.zeros((128, 32))
+    for h in range(2):
+        for w in range(4):
+            out[64 * h + 16 * w: 64 * h + 16 * w + 16] = tma_box(
+                planes, strides, dims, box, (k0, m0 + 8 * w, 2 * h, plane)).reshape(16, 32)
+    return out
+
+
+def load_b_stage(packed, kq, p_rows, nb, n0, k0, plane):
+    """tcb_load_block's B box of one plane: 2 nb shared-memory rows of K block k0 .. k0 + 31."""
+    dims, strides = b_map(kq, p_rows)
+    return tma_box(packed, strides, dims, (32, 2 * nb, 1), (k0, 2 * n0, plane)).reshape(2 * nb, 32)
+
+
+def pack_basis_pairs(basis_rows):
+    """pack_block_basis_kernel with four phases, as float64 (the hi plane exact, lo zero): packed[plane][2 p + part]."""
+    p_rows, kq = basis_rows.shape
+    packed = np.zeros((2, 2 * p_rows, kq))
+    packed[0, 0::2], packed[0, 1::2] = basis_rows.real, basis_rows.imag
+    return packed.ravel()
+
+
+def a_tile_rows(blocks):
+    """The A operand of one M tile in shared memory (tcb_load_block, four phases): slab h row 16 w + 8 p + i holds
+    phase 2 h + p of block row 8 w + i.  blocks: the tile's 32 block rows in polyphase order (hop columns)."""
+    kq = blocks.shape[1] // 4
+    rows = np.zeros((128, kq))
+    for h in range(2):
+        for w in range(4):
+            for p in range(2):
+                q = 2 * h + p
+                rows[64 * h + 16 * w + 8 * p: 64 * h + 16 * w + 8 * p + 8] = blocks[8 * w: 8 * w + 8, q * kq: (q + 1) * kq]
+    return rows
+
+
+def b_tile_rows(basis_rows):
+    """The B operand of one N tile (pack_block_basis_kernel with four phases): row 2 c + part = (re, im) of bin c."""
+    rows = np.zeros((2 * basis_rows.shape[0], basis_rows.shape[1]))
+    rows[0::2], rows[1::2] = basis_rows.real, basis_rows.imag
+    return rows
+
+
+def fragment(d, w, lane, n):
+    """wgmma m64nNk16 accumulator fragment of thread `lane` of warp w: register 4 j + 2 s + e holds row
+    16 w + lane / 4 + 8 s, column 8 j + 2 (lane % 4) + e of the warpgroup's 64 x N tile d."""
+    regs = np.zeros(n // 2)
+    for j in range(n // 8):
+        for s in range(2):
+            for e in range(2):
+                regs[4 * j + 2 * s + e] = d[16 * w + lane // 4 + 8 * s, 8 * j + 2 * (lane % 4) + e]
+    return regs
+
+
+def poly_tile(blocks, basis_rows, tw_rows):
+    """tcb_poly_tile on one (M tile, N tile): both warpgroups' two m64 x nb MMAs, the radix-4 butterfly on each
+    thread's registers and the family stores.  tw_rows[q][c]: the twiddle of tile column c.  Returns the
+    (128, 2 nb) accumulator tile the epilogue reads (quarter f = family f, f1 / f3 column-reversed; re columns, then
+    im) and how many times each of its locations was written."""
+    nb = basis_rows.shape[0]
+    a, b = a_tile_rows(blocks), b_tile_rows(basis_rows)
+    tile = np.zeros((128, 2 * nb))
+    written = np.zeros((128, 2 * nb), dtype=int)
+    for wg in range(2):
+        half = b[wg * nb: (wg + 1) * nb]                     # MMA N = nb: this warpgroup's bins, re / im interleaved
+        d = [a[64 * h: 64 * h + 64] @ half.T for h in range(2)]
+        for w in range(4):
+            for lane in range(32):
+                acc = [fragment(d[h], w, lane, nb) for h in range(2)]
+                r = 8 * w + lane // 4                        # block row
+                for j in range(nb // 8):
+                    c = wg * nb // 2 + 4 * j + lane % 4      # tile column (packed bin)
+                    y = [acc[q >> 1][4 * j + 2 * (q & 1)] + 1j * acc[q >> 1][4 * j + 2 * (q & 1) + 1] for q in range(4)]
+                    t = [y[q] * tw_rows[q][c] for q in range(4)]
+                    a0, a1, b0, b1 = t[0] + t[2], t[0] - t[2], t[1] + t[3], t[1] - t[3]
+                    fam = (a0 + b0, np.conj(a1 + 1j * b1), a1 - 1j * b1, np.conj(a0 - b0))
+                    for f in range(4):
+                        col = nb - 1 - c if f & 1 else c
+                        tile[32 * f + r, col], tile[32 * f + r, nb + col] = fam[f].real, fam[f].imag
+                        written[32 * f + r, col] += 1
+                        written[32 * f + r, nb + col] += 1
+    return tile, written
+
+
 def emulate(x, n_fft, hop, B=1, nb=None, split=None):
-    """framed_tcb_kernel<.., PH = 4> index by index: polyphase planes, one 32-row box per phase at column origin
-    q hop / 4, the butterfly into family quarters (f1, f3 column-reversed), the per-family epilogue windows.
-    Returns the (B, F, T) STFT and the number of times each (b, bin, frame) was written."""
+    """framed_tcb_kernel<.., PH = 4> index by index: polyphase planes, the A tile's phase-interleaved rows, the
+    butterfly on each thread's accumulator registers and its stores into family quarters (poly_tile), the
+    per-family epilogue windows.  Returns the (B, F, T) STFT and the number of times each (b, bin, frame) was
+    written."""
     assert hop % 128 == 0
     R = n_fft // hop
     FW = 33 - R
@@ -126,10 +235,9 @@ def emulate(x, n_fft, hop, B=1, nb=None, split=None):
         A = rows[m0: m0 + 32]
         for n_tile in range(n_tiles):
             n0 = n_tile * (nb - 2)
-            acc = [A[:, q * kq: (q + 1) * kq] @ basis[n0: n0 + nb].T for q in range(4)]   # quarter q = phase q
-            Tq = [tw[q, n0: n0 + nb][None, :] * acc[q] for q in range(4)]
-            A0, A1, B0, B1 = Tq[0] + Tq[2], Tq[0] - Tq[2], Tq[1] + Tq[3], Tq[1] - Tq[3]
-            fam = [A0 + B0, np.conj(A1 + 1j * B1)[:, ::-1], A1 - 1j * B1, np.conj(A0 - B0)[:, ::-1]]
+            tile, tile_written = poly_tile(A, basis[n0: n0 + nb], tw[:, n0: n0 + nb])
+            assert (tile_written == 1).all()
+            fam = [tile[32 * f: 32 * f + 32, :nb] + 1j * tile[32 * f: 32 * f + 32, nb:] for f in range(4)]
             for f in range(4):
                 k_tile0, lo, hi = family_span(n_tile, f, nb, M, F)
                 lo = max(lo, k_tile0)
