@@ -2891,7 +2891,9 @@ int nnab_pcen_forward(const float* E, int64_t B, int C, int64_t T, const float* 
                       const float* bias, const float* power, int param_stride, float eps, float* P, float* M,
                       float* state, uint8_t* primed, int64_t slots, const int32_t* row_slot, const int32_t* counts,
                       void* stream) {
-  if (E == nullptr || P == nullptr || !pcen_shape_ok(s, gain, bias, power, param_stride, eps, B, C, T))
+  // an empty spectrogram may come without storage: its pointers are only checked when there are frames
+  if (((E == nullptr || P == nullptr) && B * T > 0) ||
+      !pcen_shape_ok(s, gain, bias, power, param_stride, eps, B, C, T))
     return NNAB_EINVAL;
   if ((state == nullptr) != (primed == nullptr)) return NNAB_EINVAL;
   if (state == nullptr && (row_slot != nullptr || counts != nullptr)) return NNAB_EINVAL;  // stream-only arguments
@@ -2906,14 +2908,20 @@ int nnab_pcen_forward(const float* E, int64_t B, int C, int64_t T, const float* 
 int nnab_pcen_backward(const float* E, const float* M, const float* grad_P, int64_t B, int C, int64_t T,
                        const float* s, const float* gain, const float* bias, const float* power, int param_stride,
                        float eps, float* grad_E, float* grad_params, void* workspace, size_t ws_bytes, void* stream) {
-  if (E == nullptr || M == nullptr || grad_P == nullptr ||
+  if (((E == nullptr || M == nullptr || grad_P == nullptr) && B * T > 0) ||
       !pcen_shape_ok(s, gain, bias, power, param_stride, eps, B, C, T))
     return NNAB_EINVAL;
   const int rc = check_arch();
   if (rc) return rc;
-  if (grad_params != nullptr && (workspace == nullptr || ws_bytes < nnab_pcen_workspace_bytes(B, C)))
-    return NNAB_EWORKSPACE;
-  if (B == 0 || (grad_E == nullptr && grad_params == nullptr)) return NNAB_OK;
+  const size_t ws_need = grad_params != nullptr ? nnab_pcen_workspace_bytes(B, C) : 0;
+  if (ws_need > 0 && (workspace == nullptr || ws_bytes < ws_need)) return NNAB_EWORKSPACE;
+  if (B == 0 || T == 0) {  // no frames: grad_E is empty and every parameter gradient is zero
+    if (grad_params != nullptr)
+      NNAB_CUDA_TRY(cudaMemsetAsync(grad_params, 0, 4 * (size_t)(param_stride ? C : 1) * sizeof(float),
+                                    (cudaStream_t)stream));
+    return NNAB_OK;
+  }
+  if (grad_E == nullptr && grad_params == nullptr) return NNAB_OK;
   return pcen_backward(E, M, grad_P, B, C, T, PcenArgs{s, gain, bias, power, param_stride, eps}, grad_E, grad_params,
                        static_cast<float*>(workspace), (cudaStream_t)stream);
 }

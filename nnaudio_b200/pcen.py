@@ -133,10 +133,12 @@ class PCEN(nn.Module):
     def forward(self, E):
         E = self._checked(E)
         params = self._params(E.device)
-        if E.numel() == 0:
-            return torch.empty(E.shape, dtype=torch.float32, device=E.device)
+        # an empty E still goes through autograd: its backward gives an empty dE and zero parameter gradients, and
+        # neither direction launches a kernel
         if torch.is_grad_enabled() and (E.requires_grad or any(p.requires_grad for p in params)):
             return _PCENFn.apply(E, *params, self.eps)
+        if E.numel() == 0:
+            return torch.empty(E.shape, dtype=torch.float32, device=E.device)
         return _C.pcen_forward(E, [p.detach() for p in params], self.eps)
 
     def extra_repr(self) -> str:
