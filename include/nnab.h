@@ -770,8 +770,16 @@ uint64_t nnab_launch_count(void);
 
 /* Leave `n_sms` SMs out of the persistent tensor-core grids (process wide, default 0) so
  * that a concurrently running collective (the NCCL output gather of the multi-GPU path)
- * has SMs to run on; returns the previous value. */
+ * has SMs to run on; returns the previous value.  Any n_sms >= 0 is kept (a negative value
+ * becomes 0); a persistent grid never drops below one CTA, so a reserve of at least the
+ * device's SM count runs every persistent kernel on a single CTA. */
 int nnab_set_sm_reserve(int n_sms);
+
+/* Persistent-grid ledger: the persistent tensor-core launches enqueued since the last read (process
+ * wide), their summed CTAs, and the smallest and largest grid among them.  Writes each non-NULL
+ * pointer, then resets the ledger; with no launch since the last read all four are 0.  Counted on
+ * the host at launch, so replaying a captured CUDA graph counts nothing.  Returns NNAB_OK. */
+int nnab_persistent_grid_read(uint64_t* launches, uint64_t* ctas, int* min_grid, int* max_grid);
 
 /* Live timing of the dominant kernel (the framed contraction) for bench.py's
  * roofline: while enabled, every framed-contraction launch is bracketed by a

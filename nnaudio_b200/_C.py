@@ -37,6 +37,7 @@ SIGNATURES = {
     "nnab_last_cuda_error": (c_char_p, []),
     "nnab_launch_count": (c_uint64, []),
     "nnab_set_sm_reserve": (c_int, [c_int]),
+    "nnab_persistent_grid_read": (c_int, [_P, _P, _P, _P]),
     "nnab_profile_enable": (None, [c_int]),
     "nnab_profile_read": (c_int, [_P, _P]),
     "nnab_profile_read_exec_flops": (c_int, [_P]),
@@ -288,8 +289,20 @@ def stream_route_count(family: int, route: int) -> int:
 
 
 def set_sm_reserve(n_sms: int) -> int:
-    """Keep ``n_sms`` SMs out of the persistent kernels' grids (for a concurrent collective)."""
+    """Keep ``n_sms`` SMs out of the persistent kernels' grids (for a concurrent collective); returns the previous
+    reserve.  The grids never drop below one CTA."""
     return int(lib().nnab_set_sm_reserve(int(n_sms)))
+
+
+def persistent_grid_read():
+    """(launches, summed CTAs, min grid, max grid) of the persistent tensor-core launches enqueued since the last
+    read, then resets them; all zero when nothing launched.  Counted at launch: a replayed CUDA graph counts
+    nothing."""
+    n, c = c_uint64(0), c_uint64(0)
+    lo, hi = c_int(0), c_int(0)
+    _check(lib().nnab_persistent_grid_read(ctypes.byref(n), ctypes.byref(c), ctypes.byref(lo), ctypes.byref(hi)),
+           "nnab_persistent_grid_read")
+    return int(n.value), int(c.value), int(lo.value), int(hi.value)
 
 
 def profile_enable(on: bool):

@@ -16,6 +16,8 @@ void count_launch();
 void count_balanced_launch();
 void count_block_ws_launch();
 int sm_reserve();
+// the persistent-grid ledger (nnab_persistent_grid_read): one persistent launch of `grid` CTAs
+void count_persistent_grid(int grid);
 // tensor-pipe accounting for bench.py: MMA flops a tensor-core launch EXECUTES (all split terms,
 // tile padding and structural zeros included); summed while nnab_profile_enable(1)
 void add_exec_flops(double flops);

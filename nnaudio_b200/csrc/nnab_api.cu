@@ -4,6 +4,7 @@
 #include <cuda_bf16.h>
 #include <algorithm>
 #include <atomic>
+#include <climits>
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
@@ -54,6 +55,21 @@ static void count_cq1992_route(int route, std::atomic<uint64_t>* counters) {
 }
 static std::atomic<int> g_sm_reserve{0};
 int sm_reserve() { return g_sm_reserve.load(std::memory_order_relaxed); }
+// persistent-grid ledger (nnab_persistent_grid_read): launches, summed CTAs, min and max grid since the last read
+static std::atomic<uint64_t> g_pgrid_launches{0};
+static std::atomic<uint64_t> g_pgrid_ctas{0};
+static std::atomic<int> g_pgrid_min{INT_MAX};
+static std::atomic<int> g_pgrid_max{0};
+void count_persistent_grid(int grid) {
+  g_pgrid_launches.fetch_add(1, std::memory_order_relaxed);
+  g_pgrid_ctas.fetch_add((uint64_t)grid, std::memory_order_relaxed);
+  int lo = g_pgrid_min.load(std::memory_order_relaxed);
+  while (grid < lo && !g_pgrid_min.compare_exchange_weak(lo, grid, std::memory_order_relaxed)) {
+  }
+  int hi = g_pgrid_max.load(std::memory_order_relaxed);
+  while (grid > hi && !g_pgrid_max.compare_exchange_weak(hi, grid, std::memory_order_relaxed)) {
+  }
+}
 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -386,8 +402,19 @@ uint64_t nnab_stream_route_count(int family, int route) {
 
 int nnab_set_sm_reserve(int n_sms) {
   if (n_sms < 0) n_sms = 0;
-  if (n_sms > 64) n_sms = 64;
   return g_sm_reserve.exchange(n_sms);
+}
+
+int nnab_persistent_grid_read(uint64_t* launches, uint64_t* ctas, int* min_grid, int* max_grid) {
+  const uint64_t n = g_pgrid_launches.exchange(0, std::memory_order_relaxed);
+  const uint64_t c = g_pgrid_ctas.exchange(0, std::memory_order_relaxed);
+  const int lo = g_pgrid_min.exchange(INT_MAX, std::memory_order_relaxed);
+  const int hi = g_pgrid_max.exchange(0, std::memory_order_relaxed);
+  if (launches) *launches = n;
+  if (ctas) *ctas = c;
+  if (min_grid) *min_grid = n ? lo : 0;
+  if (max_grid) *max_grid = hi;
+  return NNAB_OK;
 }
 
 void nnab_profile_enable(int on) { g_prof_on.store(on ? 1 : 0); }

@@ -16,7 +16,8 @@ static inline int round_up_i(int v, int a) { return (v + a - 1) / a * a; }
 
 // Launches the persistent tensor-core kernel K.  Its dynamic shared-memory limit (smem_limit bytes) is set
 // first, once per device: the attribute is per device, and one process may drive several GPUs
-// (torch.nn.DataParallel).  Devices are tracked in a 64-bit mask indexed by device & 63.
+// (torch.nn.DataParallel).  Devices are tracked in a 64-bit mask indexed by device & 63.  Each successful
+// launch is entered in the persistent-grid ledger (nnab_persistent_grid_read).
 template <auto K, typename... Args>
 int launch_persistent(int grid, int threads, size_t smem, size_t smem_limit, cudaStream_t stream,
                       const Args&... args) {
@@ -29,6 +30,7 @@ int launch_persistent(int grid, int threads, size_t smem, size_t smem_limit, cud
   }
   K<<<grid, threads, smem, stream>>>(args...);
   NNAB_LAUNCH_CHECK();
+  count_persistent_grid(grid);
   return NNAB_OK;
 }
 

@@ -162,8 +162,12 @@ def test_fbank_domain(name):
         if p["ws"]:
             sms = torch.cuda.get_device_properties(0).multi_processor_count
             for grid in (1, 2):
+                _C.persistent_grid_read()
                 yg, _, fg, wg = _measured(lambda: call(x), reserve=sms - grid)
                 assert wg == 1 and fg == p["flops"], (case, grid, wg, fg)
+                # the ledger proves the leg's grid: no persistent launch ran more CTAs, and the block kernel's did
+                n, ctas, lo, hi = _C.persistent_grid_read()
+                assert n >= 1 and hi == grid and 1 <= lo and ctas <= n * grid, (case, grid, n, ctas, lo, hi)
                 assert torch.equal(y, yg), (case, grid)
         # a bf16 waveform: two MMA passes on the block-partial kernel, bit for bit with its fp32 upcast
         xh = x.to(torch.bfloat16)

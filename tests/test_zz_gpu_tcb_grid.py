@@ -29,7 +29,9 @@ CONFIGS = {
 
 
 def _forward(mod, x, reserve):
+    """(mod(x), persistent-grid ledger of the call) under an SM reserve of ``reserve``."""
     old = _C.set_sm_reserve(reserve)
+    _C.persistent_grid_read()
     try:
         with torch.no_grad(), warnings.catch_warnings():
             warnings.simplefilter("ignore")
@@ -37,7 +39,7 @@ def _forward(mod, x, reserve):
         torch.cuda.synchronize()
     finally:
         _C.set_sm_reserve(old)
-    return y
+    return y, _C.persistent_grid_read()
 
 
 @pytest.mark.parametrize("name", sorted(CONFIGS))
@@ -48,9 +50,13 @@ def test_full_grid_equals_single_cta_bitwise(name):
     x = torch.from_numpy(xn).cuda()
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     before = _C.launch_count()
-    full = _forward(mod, x, 0)
+    full, ledger_full = _forward(mod, x, 0)
     assert _C.launch_count() > before
-    single = _forward(mod, x, sms - 1)
+    single, ledger = _forward(mod, x, sms - 1)
+    # every persistent launch of the single-CTA leg ran one CTA; the full grid ran more
+    n = ledger[0]
+    assert n >= 1 and ledger == (n, n, 1, 1), (name, ledger)
+    assert ledger_full[0] == n and ledger_full[3] > 1, (name, ledger_full)
     assert full.shape == single.shape
     # (the fused Mel epilogue adds at most two partial sums per filter: its atomic adds commute)
     assert torch.equal(full, single)

@@ -43,7 +43,9 @@ def _length(n_fft, hop, m_tiles):
 
 
 def _run(mod, x, reserve):
+    """(mod(x), executed MMA flops, persistent-grid ledger) of one call under an SM reserve of ``reserve``."""
     old = _C.set_sm_reserve(reserve)
+    _C.persistent_grid_read()
     _C.profile_read_exec_flops()
     _C.profile_enable(True)
     try:
@@ -55,7 +57,7 @@ def _run(mod, x, reserve):
         _C.profile_enable(False)
         _C.profile_read()
         _C.set_sm_reserve(old)
-    return y, _C.profile_read_exec_flops()
+    return y, _C.profile_read_exec_flops(), _C.persistent_grid_read()
 
 
 @pytest.mark.parametrize("tiles_vs_sms", [-1, 0, 1])
@@ -78,7 +80,10 @@ def test_ws_kernel_grids_bitwise(name, tiles_vs_sms):
     want_flops = bd.block_exec_flops(n_fft, hop, 1, L, True, nb=nb)
     outs = []
     for grid in (sms, 1, 2, 3):
-        y, flops = _run(mod, x, sms - grid)
+        y, flops, ledger = _run(mod, x, sms - grid)
+        if grid < sms:  # each persistent launch (the block kernel, and the planes GEMM) ran at this grid
+            n = ledger[0]
+            assert n >= 1 and ledger == (n, n * grid, grid, grid), (name, grid, ledger)
         want = want_flops
         if route == "planes":
             want += bd.planes_gemm_flops(n_fft, hop, 1, y.shape[-1], mod.gammatone_basis.shape[0])
@@ -93,7 +98,7 @@ def test_ws_kernel_grids_bitwise(name, tiles_vs_sms):
         return
     for grid, y in outs[1:]:
         assert torch.equal(ref, y), (name, grid)
-    again, _ = _run(mod, x, 0)
+    again = _run(mod, x, 0)[0]
     assert torch.equal(ref, again), name
     emax, el2 = rel_errors(ref.cpu().numpy(), run_oracle(cls, mod, xn, {}))
     assert emax < 1e-4 and el2 < 1e-4, (name, emax, el2)
